@@ -88,6 +88,16 @@ class AdamSegment(C.Structure):
     ]
 
 
+class AdamDeviceSegment(C.Structure):
+    """Mirror of gab200_adam_device_segment."""
+    _fields_ = [
+        ("param", C.c_void_p), ("grad", C.c_void_p), ("exp_avg", C.c_void_p), ("exp_avg_sq", C.c_void_p),
+        ("n", C.c_int64), ("step", C.c_void_p), ("lr", C.c_double), ("has_schedule", C.c_int32),
+        ("reserved0", C.c_int32), ("lr_init", C.c_double), ("lr_final", C.c_double), ("lr_delay_mult", C.c_double),
+        ("lr_delay_steps", C.c_int64), ("max_steps", C.c_int64),
+    ]
+
+
 class DensifyArgs(C.Structure):
     """Mirror of gab200_densify_args."""
     _fields_ = [
@@ -134,7 +144,8 @@ EXPORTED_SYMBOLS = ("gab200_forward", "gab200_backward", "gab200_mark_visible", 
                     "gab200_stage_timing_enable", "gab200_stage_times", "gab200_face_frame_forward",
                     "gab200_face_frame_backward", "gab200_host_times", "gab200_l1_loss_u8", "gab200_l1_loss_u8_backward",
                     "gab200_photometric_loss", "gab200_adam_step", "gab200_tune", "gab200_counters_ok",
-                    "gab200_regularize_forward", "gab200_regularize_backward", "gab200_nvls_allreduce", "gab200_densify_scratch_bytes", "gab200_densify_plan", "gab200_densify_apply")
+                    "gab200_regularize_forward", "gab200_regularize_backward", "gab200_nvls_allreduce", "gab200_densify_scratch_bytes", "gab200_densify_plan", "gab200_densify_apply",
+                    "gab200_adam_step_device", "gab200_densify_stats")
 
 _lib = None
 _lock = threading.Lock()
@@ -201,6 +212,11 @@ def lib():
         L.gab200_adam_step.restype = C.c_int32
         L.gab200_adam_step.argtypes = [C.c_int32, C.POINTER(AdamSegment), C.c_int64, C.c_double, C.c_double,
                                        C.c_double, C.c_void_p]
+        L.gab200_adam_step_device.restype = C.c_int32
+        L.gab200_adam_step_device.argtypes = [C.c_int32, C.POINTER(AdamDeviceSegment), C.c_double, C.c_double,
+                                              C.c_double, C.c_void_p, C.c_void_p]
+        L.gab200_densify_stats.restype = C.c_int32
+        L.gab200_densify_stats.argtypes = [C.c_int32] + [C.c_void_p] * 7
         L.gab200_host_times.restype = None
         L.gab200_host_times.argtypes = [C.POINTER(C.c_double), C.c_int32]
         L.gab200_face_frame_forward.restype = C.c_int32

@@ -780,6 +780,28 @@ int32_t gab200_adam_step(int32_t num_segments, const gab200_adam_segment* segs, 
   return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
 }
 
+int32_t gab200_adam_step_device(int32_t num_segments, const gab200_adam_device_segment* segs, double beta1,
+                                double beta2, double eps, const int32_t* skip_flag, void* stream_) {
+  if (num_segments < 0 || (num_segments > 0 && segs == nullptr) || !(beta1 >= 0.0 && beta1 < 1.0) ||
+      !(beta2 >= 0.0 && beta2 < 1.0) || !(eps >= 0.0))
+    return GAB200_ERR_INVALID_ARGUMENT;
+  for (int i = 0; i < num_segments; i++) {
+    const gab200_adam_device_segment& s = segs[i];
+    if (s.n < 0 || !s.step || (s.n > 0 && (!s.param || !s.grad || !s.exp_avg || !s.exp_avg_sq)))
+      return GAB200_ERR_INVALID_ARGUMENT;
+    if (s.has_schedule) {
+      if (!(s.lr_init >= 0.0) || !(s.lr_final >= 0.0) || s.max_steps <= 0 || s.lr_delay_steps < 0 ||
+          !(s.lr_delay_mult >= 0.0))
+        return GAB200_ERR_INVALID_ARGUMENT;
+    } else if (!(s.lr >= 0.0)) {
+      return GAB200_ERR_INVALID_ARGUMENT;
+    }
+  }
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  launch_adam_device(num_segments, segs, beta1, beta2, eps, skip_flag, (cudaStream_t)stream_);
+  return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
 int32_t gab200_nvls_allreduce(float* mc_ptr, int64_t n, int32_t rank, int32_t world, void* stream_) {
   if (mc_ptr == nullptr || n < 0 || world < 1 || rank < 0 || rank >= world || ((uintptr_t)mc_ptr & 15) != 0)
     return GAB200_ERR_INVALID_ARGUMENT;
@@ -843,6 +865,16 @@ int32_t gab200_densify_apply(const gab200_densify_args* a, const gab200_densify_
   }
   if (check_arch() < 0) return GAB200_ERR_ARCH;
   GAB_CUDA(launch_densify_apply(*a, *o, stream));
+  return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
+int32_t gab200_densify_stats(int32_t P, const float* viewspace_grad, const int32_t* radii, float* xyz_gradient_accum,
+                             float* denom, float* max_radii2D, const int32_t* skip_flag, void* stream_) {
+  if (P < 0 || (P > 0 && (!viewspace_grad || !radii || !xyz_gradient_accum || !denom || !max_radii2D)))
+    return GAB200_ERR_INVALID_ARGUMENT;
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  launch_densify_stats(P, viewspace_grad, radii, xyz_gradient_accum, denom, max_radii2D, skip_flag,
+                       (cudaStream_t)stream_);
   return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
 }
 

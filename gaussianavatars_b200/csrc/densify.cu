@@ -285,4 +285,30 @@ cudaError_t launch_densify_apply(const gab200_densify_args& a, const gab200_dens
   return cudaSuccess;
 }
 
+// The statistics densify_and_prune consumes, accumulated once per rendered frame (train.py:197,
+// scene/gaussian_model.py:517-519) without the reference's two boolean-mask index passes (each a nonzero(): a host
+// wait).  Per splat: read the x, y of the view-space gradient (8 B), radii (4 B) and the three statistics (12 B);
+// write the statistics (12 B) where radii > 0.
+__global__ void __launch_bounds__(256) densify_stats_kernel(int P, const float* __restrict__ vgrad,
+                                                            const int32_t* __restrict__ radii, float* __restrict__ accum,
+                                                            float* __restrict__ denom, float* __restrict__ max_radii,
+                                                            const int32_t* __restrict__ skip) {
+  if (skip != nullptr && *skip != 0) return;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= P) return;
+  const int r = radii[i];
+  if (r <= 0) return;
+  max_radii[i] = fmaxf(max_radii[i], (float)r);
+  const float gx = vgrad[3 * (size_t)i], gy = vgrad[3 * (size_t)i + 1];
+  accum[i] += sqrtf(fmaf(gy, gy, gx * gx));  // torch.norm(grad[:, :2], dim=-1)
+  denom[i] += 1.f;
+}
+
+void launch_densify_stats(int P, const float* vgrad, const int32_t* radii, float* accum, float* denom, float* max_radii,
+                          const int32_t* skip, cudaStream_t stream) {
+  if (P <= 0) return;
+  densify_stats_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, vgrad, radii, accum, denom, max_radii, skip);
+  count_launch();
+}
+
 }  // namespace gab

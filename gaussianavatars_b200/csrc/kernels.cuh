@@ -175,6 +175,8 @@ void launch_photometric_loss(int C, int H, int W, const float* img, const void* 
 size_t densify_scratch_bytes(int P, int F);
 cudaError_t launch_densify_plan(const gab200_densify_args& a, cudaStream_t stream);
 cudaError_t launch_densify_apply(const gab200_densify_args& a, const gab200_densify_out& o, cudaStream_t stream);
+void launch_densify_stats(int P, const float* vgrad, const int32_t* radii, float* accum, float* denom, float* max_radii,
+                          const int32_t* skip, cudaStream_t stream);
 
 // regularize.cu
 cudaError_t launch_regularize_forward(const gab200_regularize_args& a, cudaStream_t stream);
@@ -186,5 +188,7 @@ void launch_nvls_allreduce(float* mc, int64_t n, int rank, int world, cudaStream
 // optim.cu
 void launch_adam(int num_segments, const gab200_adam_segment* segs, int64_t step, double beta1, double beta2, double eps,
                  cudaStream_t stream);
+void launch_adam_device(int num_segments, const gab200_adam_device_segment* segs, double beta1, double beta2,
+                        double eps, const int32_t* skip, cudaStream_t stream);
 
 }  // namespace gab

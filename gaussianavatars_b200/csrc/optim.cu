@@ -34,21 +34,16 @@ __device__ __forceinline__ void adam_one(float& p, float g, float& m, float& v, 
   p = p - step_size * (m / denom);
 }
 
-__global__ void __launch_bounds__(256) adam_kernel(AdamBatch b, float w1, float beta2, float w2, float inv_bc2_sqrt,
-                                                   float eps) {
-  const int s = blockIdx.y;
-  const int64_t n = b.n[s];
-  float* __restrict__ p = b.p[s];
-  const float* __restrict__ g = b.g[s];
-  float* __restrict__ m = b.m[s];
-  float* __restrict__ v = b.v[s];
-  const float step_size = b.step_size[s];
+// One segment's grid-stride update: the body of both launches below.
+__device__ __forceinline__ void adam_segment(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
+                                             float* __restrict__ v, int64_t n, int32_t vec4, float w1, float beta2,
+                                             float w2, float inv_bc2_sqrt, float eps, float step_size) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   const int64_t t0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   int64_t tail = 0;
-  if (b.vec4[s] & 1) {
+  if (vec4 & 1) {
     // the gradient is usually a view into the fused backward's flat buffer: its offset need not be 16-byte aligned
-    const bool g_vec = (b.vec4[s] & 2) != 0;
+    const bool g_vec = (vec4 & 2) != 0;
     const int64_t n4 = n >> 2;
     auto load_g = [&](int64_t i) {
       return g_vec ? reinterpret_cast<const float4*>(g)[i] : make_float4(g[4 * i], g[4 * i + 1], g[4 * i + 2], g[4 * i + 3]);
@@ -93,6 +88,12 @@ __global__ void __launch_bounds__(256) adam_kernel(AdamBatch b, float w1, float 
   }
 }
 
+__global__ void __launch_bounds__(256) adam_kernel(AdamBatch b, float w1, float beta2, float w2, float inv_bc2_sqrt,
+                                                   float eps) {
+  const int s = blockIdx.y;
+  adam_segment(b.p[s], b.g[s], b.m[s], b.v[s], b.n[s], b.vec4[s], w1, beta2, w2, inv_bc2_sqrt, eps, b.step_size[s]);
+}
+
 void launch_adam(int num_segments, const gab200_adam_segment* segs, int64_t step, double beta1, double beta2, double eps,
                  cudaStream_t stream) {
   const double bc1 = 1.0 - pow(beta1, (double)step);
@@ -128,6 +129,79 @@ void launch_adam(int num_segments, const gab200_adam_segment* segs, int64_t step
     if (blocks > GAB_NUM_SMS * 8 * 8) blocks = GAB_NUM_SMS * 8 * 8;
     adam_kernel<<<dim3((unsigned)blocks, (unsigned)cnt), 256, 0, stream>>>(
         b, (float)(1.0 - beta1), (float)beta2, (float)(1.0 - beta2), inv_bc2_sqrt, (float)eps);
+    count_launch();
+  }
+}
+
+// ---- capturable variant: every per-step scalar is formed on the device --------------------------------------------
+struct AdamDeviceBatch {
+  gab200_adam_device_segment seg[GAB_ADAM_MAX_SEGMENTS];
+  int32_t vec4[GAB_ADAM_MAX_SEGMENTS];
+};
+
+__device__ __forceinline__ bool skipped(const int32_t* skip) { return skip != nullptr && *skip != 0; }
+
+// get_expon_lr_func (utils/general_utils.py) in double, operation for operation: __dmul_rn / __dadd_rn keep the compiler
+// from contracting a * b + c into one fma, which numpy does not do either.
+__device__ double expon_lr(const gab200_adam_device_segment& s, double step) {
+  if (step < 0.0 || (s.lr_init == 0.0 && s.lr_final == 0.0)) return 0.0;
+  double delay_rate = 1.0;
+  if (s.lr_delay_steps > 0) {
+    const double x = fmin(fmax(step / (double)s.lr_delay_steps, 0.0), 1.0);
+    delay_rate = __dadd_rn(s.lr_delay_mult, __dmul_rn(1.0 - s.lr_delay_mult, sin(__dmul_rn(0.5 * M_PI, x))));
+  }
+  const double t = fmin(fmax(step / (double)s.max_steps, 0.0), 1.0);
+  const double log_lerp = exp(__dadd_rn(__dmul_rn(log(s.lr_init), 1.0 - t), __dmul_rn(log(s.lr_final), t)));
+  return __dmul_rn(delay_rate, log_lerp);
+}
+
+// A separate single-thread launch: if the Adam kernel incremented the counter itself, its other blocks could read
+// either the old or the new value.
+__global__ void adam_count_step_kernel(AdamDeviceBatch b, int cnt, const int32_t* __restrict__ skip) {
+  if (skipped(skip)) return;
+  for (int s = 0; s < cnt; s++) *b.seg[s].step += 1.0f;
+}
+
+__global__ void __launch_bounds__(256) adam_device_kernel(AdamDeviceBatch b, double beta1, double beta2, float w1,
+                                                          float beta2f, float w2, float eps,
+                                                          const int32_t* __restrict__ skip) {
+  if (skipped(skip)) return;
+  const int s = blockIdx.y;
+  const gab200_adam_device_segment& sg = b.seg[s];
+  __shared__ float scal[2];  // lr / bias_correction1, 1 / sqrt(bias_correction2): launch_adam's host arithmetic
+  if (threadIdx.x == 0) {
+    const double step = (double)*sg.step;
+    const double lr = sg.has_schedule ? expon_lr(sg, step) : sg.lr;
+    const double bc1 = 1.0 - pow(beta1, step);
+    const double bc2 = 1.0 - pow(beta2, step);
+    scal[0] = (float)(lr / bc1);
+    scal[1] = (float)(1.0 / sqrt(bc2));
+  }
+  __syncthreads();
+  adam_segment(sg.param, sg.grad, sg.exp_avg, sg.exp_avg_sq, sg.n, b.vec4[s], w1, beta2f, w2, scal[1], eps, scal[0]);
+}
+
+void launch_adam_device(int num_segments, const gab200_adam_device_segment* segs, double beta1, double beta2,
+                        double eps, const int32_t* skip, cudaStream_t stream) {
+  for (int first = 0; first < num_segments; first += GAB_ADAM_MAX_SEGMENTS) {
+    AdamDeviceBatch b;
+    memset(&b, 0, sizeof(b));
+    const int cnt = num_segments - first < GAB_ADAM_MAX_SEGMENTS ? num_segments - first : GAB_ADAM_MAX_SEGMENTS;
+    int64_t longest = 0;
+    for (int i = 0; i < cnt; i++) {
+      const gab200_adam_device_segment& s = segs[first + i];
+      b.seg[i] = s;
+      const uintptr_t bits = (uintptr_t)s.param | (uintptr_t)s.exp_avg | (uintptr_t)s.exp_avg_sq;
+      b.vec4[i] = (bits & 15) == 0 ? (((uintptr_t)s.grad & 15) == 0 ? 3 : 1) : 0;
+      longest = s.n > longest ? s.n : longest;
+    }
+    adam_count_step_kernel<<<1, 1, 0, stream>>>(b, cnt, skip);
+    count_launch();
+    int64_t blocks = (longest / 8 + 255) / 256;  // the grid of launch_adam
+    if (blocks < 1) blocks = 1;
+    if (blocks > GAB_NUM_SMS * 8 * 8) blocks = GAB_NUM_SMS * 8 * 8;
+    adam_device_kernel<<<dim3((unsigned)blocks, (unsigned)cnt), 256, 0, stream>>>(
+        b, beta1, beta2, (float)(1.0 - beta1), (float)beta2, (float)(1.0 - beta2), (float)eps, skip);
     count_launch();
   }
 }

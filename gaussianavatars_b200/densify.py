@@ -2,6 +2,8 @@
 moments instead of the reference's mask-index / torch.cat sequence (scene/gaussian_model.py:334-519).
 
     densify_arrays(...)       tensors in, tensors out (what the tests and other frameworks call)
+    add_densification_stats(model, viewspace_points, radii)
+                              train.py:197 + the reference's add_densification_stats in one launch, no host wait
     densify_and_prune(model)  the reference's method on an object with the reference's attribute names
                               (_xyz ... _rotation, optimizer with named groups, xyz_gradient_accum, denom,
                               max_radii2D, percent_dense, binding, binding_counter, face_scaling): parameters are
@@ -152,3 +154,44 @@ def densify_and_prune(model, max_grad, min_opacity, extent, max_screen_size, noi
         model.binding = b_out.to(binding.dtype)
         model.binding_counter = c_out.to(model.binding_counter.dtype)
     return info
+
+
+@torch.no_grad()
+def add_densification_stats(model, viewspace_points: torch.Tensor, radii: torch.Tensor,
+                            skip_flag: Optional[torch.Tensor] = None):
+    """What train.py:197 and GaussianModel.add_densification_stats (scene/gaussian_model.py:517-519) do after every
+    rendered frame, in place and in one launch: for every splat with radii > 0,
+    `max_radii2D = max(max_radii2D, radii)`, `xyz_gradient_accum += ||viewspace_points.grad[:, :2]||`, `denom += 1`.
+    The reference indexes with the boolean `visibility_filter` twice (a host wait each); this reads `radii` directly.
+    `model` carries the statistics densify_and_prune consumes: xyz_gradient_accum (P, 1), denom (P, 1),
+    max_radii2D (P,), float32 on the device.  `viewspace_points` is the render's `viewspace_points` after backward
+    (its `.grad` is read).  skip_flag: optional int32 device tensor; non-zero when the launch executes = no change
+    (graph.GraphedFrame passes its instance-overflow flag).  Capturable into a CUDA graph."""
+    g = viewspace_points.grad
+    if g is None:
+        raise ValueError("viewspace_points has no gradient: call it after backward")
+    device = g.device
+    if device.type != "cuda":
+        raise RuntimeError("gaussianavatars_b200 has no CPU path: tensors must be CUDA tensors")
+    P = radii.shape[0] if radii.dim() == 1 else -1
+    if P < 0 or radii.dtype != torch.int32 or radii.device != device:
+        raise TypeError(f"radii must be a (P,) int32 tensor on {device}")
+    if tuple(g.shape) != (P, 3) or g.dtype != torch.float32:
+        raise ValueError(f"viewspace_points.grad must be a float32 ({P}, 3) tensor, got {tuple(g.shape)} {g.dtype}")
+    stats = []
+    for name, shape in (("xyz_gradient_accum", (P, 1)), ("denom", (P, 1)), ("max_radii2D", (P,))):
+        t = getattr(model, name, None)
+        if t is None or tuple(t.shape) != shape or t.dtype != torch.float32 or t.device != device \
+                or not t.is_contiguous():
+            got = None if t is None else (tuple(t.shape), t.dtype, str(t.device))
+            raise ValueError(f"model.{name} must be a contiguous float32 {shape} tensor on {device} (P = {P} "
+                             f"splats rendered), got {got}")
+        stats.append(t)
+    if skip_flag is not None and (skip_flag.device != device or skip_flag.dtype != torch.int32):
+        raise TypeError(f"skip_flag must be an int32 tensor on {device}")
+    g = g if g.is_contiguous() else g.contiguous()
+    r = radii if radii.is_contiguous() else radii.contiguous()
+    with torch.cuda.device(device):
+        stream = torch.cuda.current_stream(device).cuda_stream
+        N.check(N.lib().gab200_densify_stats(P, g.data_ptr(), r.data_ptr(), *(t.data_ptr() for t in stats),
+                                             N.ptr(skip_flag), C.c_void_p(stream)), "gab200_densify_stats")

@@ -17,6 +17,13 @@ capacity renders from a truncated instance list -- memory-safe, wrong -- and rai
 `run(check=True)` waits for the replay, and on overflow grows the capacity, re-captures and replays: its results are
 then exactly those of an eager `render()`.  `run(check=False)` never touches the host; call `overflowed()` whenever
 convenient (bench.py does after its timed loop).
+
+With `optimizer=` (a capturable `Adam`) and `densify_stats=True` one replay is a whole training iteration of the
+reference (train.py:106-210): after backward the graph also accumulates the densification statistics
+(densify.add_densification_stats) and steps the optimizer, learning-rate schedule included (training.expon_lr_schedule).
+Both are skipped on the device when the replay overflowed its capacity: such a replay changes no parameter, moment,
+step or statistic.  densify_and_prune / reset_opacity / oneupSHdegree stay eager calls between replays; `run()` notices
+the tensors or sizes they replaced and re-captures.
 """
 from __future__ import annotations
 
@@ -27,7 +34,10 @@ import torch
 from . import rasterizer as R
 from .renderer import render
 from .rasterizer import l1_loss_u8
-from .training import binding_regularizers, photometric_loss
+from .densify import add_densification_stats
+from .training import Adam, binding_regularizers, photometric_loss
+
+_STATS = ("xyz_gradient_accum", "denom", "max_radii2D")
 
 
 class _Pipe:
@@ -62,6 +72,9 @@ def pair_with_deferred_reduce(frames, buffers, side_work_at: str = "start"):
     Call before capture()."""
     if len(frames) != 2 or len(buffers) != 2:
         raise ValueError("a deferred-reduction pair is two frames and two buffers")
+    if any(f.optimizer is not None for f in frames):
+        raise ValueError("a deferred-reduction pair reduces each step's gradients one replay late: a frame of the pair "
+                         "cannot step an optimizer inside its graph")
     for k, f in enumerate(frames):
         mine, other = buffers[k], buffers[1 - k]
 
@@ -88,7 +101,8 @@ class GraphedFrame:
     def __init__(self, pc, width: int, height: int, fovx: float, fovy: float, bg: torch.Tensor, loss: str = "l1_u8",
                  lambda_dssim: float = 0.2, host_inputs: bool = False, capacity: Optional[int] = None,
                  headroom: float = 1.25, after_backward=None, warm_cameras=None, regularizers: Optional[dict] = None,
-                 before_backward=None, side_work=None, side_work_at: str = "start"):
+                 before_backward=None, side_work=None, side_work_at: str = "start", optimizer: Optional[Adam] = None,
+                 densify_stats: bool = False):
         """loss: "l1_u8" (L1 vs a uint8 ground truth), "photometric" ((1-l) L1 + l (1-SSIM) vs a uint8 ground truth) or
         "dL_dimage" (the caller supplies dL/dimage in `self.dL_dimage`).
         host_inputs: the frame owns pinned STAGING tensors (`cam_stage` (35,) float32, `gt_stage` (3,H,W) uint8) that a
@@ -107,7 +121,17 @@ class GraphedFrame:
         (dist.SymmetricGradBuffer.reduce of the other frame of an alternating pair), which then costs no step time.
         warm_cameras: camera blocks (35,) rendered eagerly before the capture to size the instance capacity.
         regularizers: keyword arguments of `binding_regularizers` (threshold_xyz, lambda_scale, ...; {} = the
-        reference's defaults): the position / scale terms of train.py:134-146 are added to the loss inside the graph."""
+        reference's defaults): the position / scale terms of train.py:134-146 are added to the loss inside the graph.
+        densify_stats: after backward (and after_backward) the graph accumulates the densification statistics of the
+        frame into pc.xyz_gradient_accum / denom / max_radii2D (densify.add_densification_stats).
+        optimizer: a capturable `Adam` (capturable=True) over the model's parameters; the graph ends with its step(),
+        so one replay is one training iteration.  Capture leaves the parameters, moments, steps and statistics as
+        they are: the first run() is the first step.  The frame remembers what the capture baked in (P,
+        active_sh_degree, the addresses of every parameter, moment, step, statistic and binding, every group's
+        hyper-parameters) and run() re-captures (`captures` counts it) when any of it changed: after
+        densify_and_prune, reset_opacity or oneupSHdegree.  A learning rate written into a group on the host every
+        iteration therefore re-captures every iteration: give the group an `lr_schedule` instead.  Not combinable
+        with pair_with_deferred_reduce; a synchronous all-reduce in after_backward runs before the step."""
         if loss not in ("l1_u8", "photometric", "dL_dimage"):
             raise ValueError("loss must be 'l1_u8', 'photometric' or 'dL_dimage'")
         self.pc, self.W, self.H, self.fovx, self.fovy = pc, int(width), int(height), float(fovx), float(fovy)
@@ -119,6 +143,12 @@ class GraphedFrame:
         self.regularizers = regularizers
         if regularizers is not None and loss == "dL_dimage":
             raise ValueError("regularizers need a scalar loss ('l1_u8' or 'photometric')")
+        if optimizer is not None and not (isinstance(optimizer, Adam) and
+                                          all(g.get("capturable", False) for g in optimizer.param_groups)):
+            raise ValueError("optimizer must be a gaussianavatars_b200.Adam with capturable=True")
+        self.optimizer = optimizer
+        self.densify_stats = bool(densify_stats)
+        self._key = None
         self.headroom = float(headroom)
         dev = pc._xyz.device
         self.device = dev
@@ -197,7 +227,8 @@ class GraphedFrame:
     def _params(self):
         return list(self.pc.parameters())
 
-    def _body(self):
+    def _body(self, train: bool = False):
+        """One frame; with `train` (the captured step only) also the statistics and the optimizer step."""
         pc = self.pc
         for p in self._params():
             p.grad = None
@@ -235,6 +266,12 @@ class GraphedFrame:
             img.backward(self.dL_dimage)
         if self.after_backward is not None:
             self.after_backward()
+        if train:
+            skip = self.slot.flag
+            if self.densify_stats:
+                add_densification_stats(pc, out["viewspace_points"], out["radii"], skip_flag=skip)
+            if self.optimizer is not None:
+                self.optimizer.step(skip_flag=skip)
         if loss is not None:
             self.loss = loss.detach()
             self.loss_host.copy_(self.loss, non_blocking=True)
@@ -254,7 +291,8 @@ class GraphedFrame:
         hints = R.hints_of(self.pc)
         key = (self.device, self.W, self.H, self.pc._xyz.shape[0])
         n_max, lo, hi = 0, 0xFFFFFFFF, 0
-        blocks = self._warm if self._warm else [self.cam.clone()]
+        cam0 = self.cam.clone()
+        blocks = self._warm if self._warm else [cam0]
         # eager frames on a side stream (torch's recipe for whole-step capture): nothing autograd creates here may be
         # tied to the legacy default stream
         cur = torch.cuda.current_stream(self.device)
@@ -271,14 +309,38 @@ class GraphedFrame:
                     if d[1] > d[0]:  # union of the (already widened) depth-key ranges: one bucket grid fits every camera
                         lo, hi = min(lo, d[0]), max(hi, d[1])
         cur.wait_stream(side)
+        self.cam.copy_(cam0)   # the frame's own camera again: the captured step must not train on the last warm one
         torch.cuda.synchronize(self.device)
         # release what the eager frames left on the model / on this object (tensors with autograd history)
         self.pc.face_center = self.pc.face_orien_mat = self.pc.face_scaling = None
         self.image = self.radii = self.viewspace_points = self.loss = None
         return n_max, ((lo, hi) if hi > lo else (0, 0))
 
+    def _state_key(self):
+        """Everything a training capture baked in that eager code between replays may replace."""
+        pc = self.pc
+        b = getattr(pc, "binding", None)
+        key = [int(pc._xyz.shape[0]), int(getattr(pc, "active_sh_degree", 0)), None if b is None else b.data_ptr()]
+        key += [p.data_ptr() for p in self._params()]
+        if self.densify_stats:
+            key += [getattr(pc, n).data_ptr() for n in _STATS]
+        opt = self.optimizer
+        if opt is not None:
+            for g in opt.param_groups:
+                sched = g.get("lr_schedule")
+                key.append((tuple(sorted(sched.items())) if sched is not None else float(g["lr"]),
+                            tuple(g["betas"]), float(g["eps"])))
+                for p in g["params"]:
+                    st = opt.state.get(p, {})
+                    key.append((p.data_ptr(), p.shape) + tuple(st[k].data_ptr() for k in ("step", "exp_avg", "exp_avg_sq")
+                                                               if k in st))
+        return tuple(key)
+
     def capture(self, capacity: Optional[int] = None):
         dev = self.device
+        training = self.optimizer is not None or self.densify_stats
+        if self.optimizer is not None:
+            self.optimizer.init_state()   # created inside the capture, the state would be re-zeroed by every replay
         n_max, depth = self._learn_capacity()
         if capacity is None:
             capacity = self._capacity if self._capacity else int(n_max * self.headroom) + 16384
@@ -287,7 +349,7 @@ class GraphedFrame:
         R._capture_slot = self.slot
         try:
             with torch.cuda.graph(self.graph):
-                self._body()
+                self._body(train=training)
                 self.slot.flag_host.copy_(self.slot.flag, non_blocking=True)
         finally:
             R._capture_slot = None
@@ -295,12 +357,16 @@ class GraphedFrame:
         # GraphedFrame of the same model re-points .grad at its own when it captures
         self.grads = [p.grad for p in self._params()]
         self.flat_grad = getattr(self.pc, "flat_grad", None)
+        self._key = self._state_key() if training else None
         self.captures += 1
         return self
 
     # ---- replay ----------------------------------------------------------------------------------------------------
     def run(self, check: bool = False):
         if self.graph is None:
+            self.capture()
+        elif self._key is not None and self._state_key() != self._key:   # host-side compare: no sync
+            self.graph = None
             self.capture()
         if self._gt_ready is not None:   # a ground-truth upload is in flight on the copy stream
             torch.cuda.current_stream(self.device).wait_event(self._gt_ready)

@@ -5,12 +5,16 @@ CUDA launches behind the same C ABI:
                                                  (utils/loss_utils.py:17-18,36-63, train.py:131-132)
   Adam(param_groups, lr, betas, eps)          <- torch.optim.Adam(l, lr=0.0, eps=1e-15).step()
                                                  (scene/gaussian_model.py:213-232, train.py:207-210)
+  Adam(..., capturable=True)                  <- the same step with the step counters, the bias corrections and the
+     + expon_lr_schedule(...)                    xyz learning-rate schedule (update_learning_rate, train.py:106) on
+                                                 the device: capturable into a CUDA graph
 
 No CPU or eager fallback: both raise when the library is missing or a tensor is not a CUDA float32 tensor.
 """
 from __future__ import annotations
 
 import ctypes as C
+from typing import Optional
 
 import torch
 
@@ -73,32 +77,86 @@ def photometric_loss(image: torch.Tensor, gt: torch.Tensor, lambda_dssim: float 
 # ================================================================================================================
 # Adam: all parameter groups in one launch
 # ================================================================================================================
+def expon_lr_schedule(lr_init, lr_final, lr_delay_steps=0, lr_delay_mult=1.0, max_steps=1000000) -> dict:
+    """The reference's `get_expon_lr_func(lr_init, lr_final, lr_delay_steps, lr_delay_mult, max_steps)`
+    (utils/general_utils.py) as a parameter group's `"lr_schedule"` for a capturable `Adam`, which evaluates it on the
+    device at every step.  The reference's `xyz` schedule (scene/gaussian_model.py:224-227) is
+    `expon_lr_schedule(lr_init=position_lr_init * spatial_lr_scale, lr_final=position_lr_final * spatial_lr_scale,
+    lr_delay_mult=position_lr_delay_mult, max_steps=position_lr_max_steps)`."""
+    sched = dict(lr_init=float(lr_init), lr_final=float(lr_final), lr_delay_steps=int(lr_delay_steps),
+                 lr_delay_mult=float(lr_delay_mult), max_steps=int(max_steps))
+    if sched["lr_init"] < 0 or sched["lr_final"] < 0 or sched["lr_delay_steps"] < 0 or sched["lr_delay_mult"] < 0 \
+            or sched["max_steps"] <= 0:
+        raise ValueError(f"invalid learning-rate schedule {sched}")
+    return sched
+
+
 class Adam(torch.optim.Optimizer):
     """Drop-in for `torch.optim.Adam(param_groups, lr=0.0, eps=1e-15)` as the reference builds it.
 
     Same `param_groups` / `state` layout as torch's Adam (`state[p] = {"step", "exp_avg", "exp_avg_sq"}`), so the
     reference's densification surgery on the optimizer state (scene/gaussian_model.py:334-419) and
     `optimizer.state_dict()` checkpoints (scene/gaussian_model.py:89,111) work unchanged.  amsgrad, weight decay and
-    maximize are not part of the reference's configuration and are rejected."""
+    maximize are not part of the reference's configuration and are rejected.
 
-    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0, amsgrad=False, maximize=False):
+    capturable=True: torch's layout for `capturable=True` -- `state["step"]` is a float32 scalar on the parameter's
+    device -- and `step()` reads nothing on the host, so it can be captured into a CUDA graph (graph.GraphedFrame) and
+    replayed.  The step counters are incremented and the bias corrections formed on the device
+    (gab200_adam_step_device).  A group may then carry `"lr_schedule": expon_lr_schedule(...)`: its learning rate is
+    the reference's exponential schedule at the group's new step, which in train.py equals `iteration`, so
+    `update_learning_rate(iteration)` is no longer needed for it.  A constant `lr` written into a group between
+    replays is NOT seen by a captured step (it was baked in at capture).  Create the state before a capture
+    (`init_state()`): state created inside one would be re-zeroed by every replay."""
+
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0, amsgrad=False, maximize=False,
+                 capturable=False):
         if weight_decay != 0 or amsgrad or maximize:
             raise ValueError("gaussianavatars_b200.Adam implements the reference configuration only "
                              "(weight_decay=0, amsgrad=False, maximize=False)")
         if not 0.0 <= lr or not 0.0 <= eps or not 0.0 <= betas[0] < 1.0 or not 0.0 <= betas[1] < 1.0:
             raise ValueError("invalid Adam hyper-parameters")
-        super().__init__(params, dict(lr=lr, betas=betas, eps=eps))
+        # weight_decay is the one key torch.optim.Adam reads from a loaded group without filling in a default: with it
+        # a checkpoint of this optimizer loads into torch's Adam and steps there
+        super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=0.0, capturable=bool(capturable)))
+
+    def _new_state(self, p, capturable):
+        st = self.state[p]
+        if capturable:
+            st["step"] = torch.zeros((), dtype=torch.float32, device=p.device)
+        else:
+            st["step"] = torch.tensor(0.0, dtype=torch.float32)
+        st["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+        st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+        return st
 
     @torch.no_grad()
-    def step(self, closure=None):
+    def init_state(self):
+        """Creates the state (step 0, zero moments) of every parameter of a capturable group that has none yet --
+        what the first eager step() would create, which makes no step itself."""
+        for group in self.param_groups:
+            if group.get("capturable", False):
+                for p in group["params"]:
+                    if len(self.state[p]) == 0:
+                        self._new_state(p, True)
+
+    @torch.no_grad()
+    def step(self, closure=None, skip_flag: Optional[torch.Tensor] = None):
+        """skip_flag (capturable groups only): an int32 device tensor; when it holds a non-zero value as the step
+        executes, the step changes no parameter, moment or step counter (graph.GraphedFrame passes its sticky
+        instance-overflow flag)."""
         loss = None
         if closure is not None:
             with torch.enable_grad():
                 loss = closure()
         batches = {}   # (device, step, beta1, beta2, eps) -> list of segments; one launch per 8 segments
+        device_batches = {}   # capturable groups: (device, beta1, beta2, eps) -> list of segments
         keep = []
         for group in self.param_groups:
             beta1, beta2 = group["betas"]
+            capturable = group.get("capturable", False)
+            sched = group.get("lr_schedule")
+            if sched is not None and not capturable:
+                raise ValueError("a group's lr_schedule is evaluated on the device: it needs Adam(capturable=True)")
             for p in group["params"]:
                 if p.grad is None:
                     continue
@@ -107,15 +165,31 @@ class Adam(torch.optim.Optimizer):
                                        "(no CPU or eager fallback)")
                 st = self.state[p]
                 if len(st) == 0:
-                    st["step"] = torch.tensor(0.0, dtype=torch.float32)
-                    st["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
-                    st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
-                st["step"] += 1
+                    if capturable and torch.cuda.is_current_stream_capturing():
+                        raise RuntimeError("capturable Adam: call init_state() before capturing step()")
+                    st = self._new_state(p, capturable)
                 g = p.grad if p.grad.is_contiguous() else p.grad.contiguous()
                 m, v = st["exp_avg"], st["exp_avg_sq"]
                 if not (m.is_contiguous() and v.is_contiguous()):
                     raise RuntimeError("Adam state tensors must be contiguous")
                 keep.append(g)
+                if capturable:
+                    t = st["step"]
+                    if t.device != p.device or t.dtype != torch.float32 or t.numel() != 1:
+                        raise RuntimeError("capturable Adam keeps state['step'] as a float32 scalar on the "
+                                           "parameter's device")
+                    seg = N.AdamDeviceSegment(p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), p.numel(),
+                                              t.data_ptr(), float(group["lr"]))
+                    if sched is not None:
+                        seg.has_schedule = 1
+                        seg.lr_init, seg.lr_final = float(sched["lr_init"]), float(sched["lr_final"])
+                        seg.lr_delay_mult = float(sched.get("lr_delay_mult", 1.0))
+                        seg.lr_delay_steps = int(sched.get("lr_delay_steps", 0))
+                        seg.max_steps = int(sched["max_steps"])
+                    key = (p.device, float(beta1), float(beta2), float(group["eps"]))
+                    device_batches.setdefault(key, []).append(seg)
+                    continue
+                st["step"] += 1
                 seg = N.AdamSegment(p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), p.numel(), float(group["lr"]))
                 key = (p.device, int(st["step"]), float(beta1), float(beta2), float(group["eps"]))
                 batches.setdefault(key, []).append(seg)
@@ -125,6 +199,17 @@ class Adam(torch.optim.Optimizer):
                 stream = torch.cuda.current_stream(device).cuda_stream
                 N.check(N.lib().gab200_adam_step(len(segs), arr, step, beta1, beta2, eps, C.c_void_p(stream)),
                         "gab200_adam_step")
+        for (device, beta1, beta2, eps), segs in device_batches.items():
+            arr = (N.AdamDeviceSegment * len(segs))(*segs)
+            flag = None
+            if skip_flag is not None:
+                if skip_flag.device != device or skip_flag.dtype != torch.int32:
+                    raise TypeError(f"skip_flag must be an int32 tensor on {device}")
+                flag = skip_flag.data_ptr()
+            with torch.cuda.device(device):
+                stream = torch.cuda.current_stream(device).cuda_stream
+                N.check(N.lib().gab200_adam_step_device(len(segs), arr, beta1, beta2, eps, flag, C.c_void_p(stream)),
+                        "gab200_adam_step_device")
         return loss
 
 

@@ -315,6 +315,33 @@ typedef struct gab200_adam_segment {
 int32_t gab200_adam_step(int32_t num_segments, const gab200_adam_segment* segments, int64_t step, double beta1,
                          double beta2, double eps, void* stream);
 
+/* The same Adam step with nothing read from the host per step, so that it can be captured into a CUDA graph and
+ * replayed (torch's `capturable=True` layout).  Every segment owns a device float32 step counter (distinct per
+ * segment); the call first increments every counter on the device (one single-thread launch), then the Adam launch
+ * forms bias_correction1/2 and lr / bias_correction1 in double from the segment's new step -- the arithmetic of
+ * gab200_adam_step -- and rounds them to float once.  A segment with has_schedule = 1 takes its learning rate from
+ * the reference's exponential schedule (utils/general_utils.py get_expon_lr_func, evaluated in double at the new step:
+ * in train.py the optimizer steps once per iteration from 1, so that step is the iteration); otherwise from `lr`.
+ * skip_flag: DEVICE pointer or NULL.  When non-NULL and *skip_flag != 0 at execution time, both launches write
+ * nothing (no parameter, moment or step changes): a graph replay whose render overflowed its instance capacity
+ * (gab200_forward_args.overflow_flag) leaves the model untouched instead of applying wrong gradients.  Empty segments
+ * (n = 0) still count a step, as torch does. */
+typedef struct gab200_adam_device_segment {
+  float* param;
+  const float* grad;
+  float* exp_avg;
+  float* exp_avg_sq;
+  int64_t n;
+  float* step;            /* device float32 scalar */
+  double lr;              /* constant learning rate (has_schedule = 0) */
+  int32_t has_schedule;
+  int32_t reserved0;
+  double lr_init, lr_final, lr_delay_mult;   /* get_expon_lr_func(lr_init, lr_final, lr_delay_steps, lr_delay_mult, */
+  int64_t lr_delay_steps, max_steps;         /*                   max_steps); max_steps > 0                          */
+} gab200_adam_device_segment;
+int32_t gab200_adam_step_device(int32_t num_segments, const gab200_adam_device_segment* segments, double beta1,
+                                double beta2, double eps, const int32_t* skip_flag, void* stream);
+
 /* The position / scale regularisers of the mesh-bound training step (train.py:134-146), loss and gradient in one
  * launch each.  vis = radii > 0 of the frame just rendered.  loss[3] receives {xyz term, scale term, visible count};
  * sums: 3 doubles of device scratch shared by the forward and its backward.  The backward writes grad_xyz /
@@ -387,6 +414,15 @@ typedef struct gab200_densify_out {
   int32_t* noise_row_scratch;      /* [totals[2]] */
 } gab200_densify_out;
 size_t gab200_densify_scratch_bytes(int32_t P, int32_t num_faces);
+
+/* The densification statistics of one rendered frame, in place, in one launch over the P splats (no mask, no
+ * compaction, no host wait).  For every splat with radii > 0:
+ *   max_radii2D = max(max_radii2D, float(radii))                                   (train.py:197)
+ *   xyz_gradient_accum += ||viewspace_grad[:, :2]||,  denom += 1                    (scene/gaussian_model.py:517-519)
+ * viewspace_grad [P,3] (viewspace_points.grad), radii [P] int32, xyz_gradient_accum [P,1], denom [P,1],
+ * max_radii2D [P].  skip_flag: as gab200_adam_step_device (DEVICE pointer or NULL; non-zero = write nothing). */
+int32_t gab200_densify_stats(int32_t P, const float* viewspace_grad, const int32_t* radii, float* xyz_gradient_accum,
+                             float* denom, float* max_radii2D, const int32_t* skip_flag, void* stream);
 int32_t gab200_densify_plan(const gab200_densify_args* args, void* stream);
 int32_t gab200_densify_apply(const gab200_densify_args* args, const gab200_densify_out* out, void* stream);
 
