@@ -20,7 +20,7 @@ INPUT_BOUND_RAW = 1
 SYNC_EXACT, SYNC_LATE, SYNC_NONE = 0, 1, 2
 CTR_NOT_MIN_DEPTH_KEY, CTR_MAX_DEPTH_KEY, CTR_NUM_RENDERED, CTR_NUM_LISTED, CTR_BUCKET_OVERFLOW, CTR_CAPACITY, CTR_SEQ = range(7)
 NUM_COUNTERS = 8
-TUNE_HEAVY_FWD, TUNE_HEAVY_BWD, TUNE_DEPTH_SORT, TUNE_BWD_VARIANT, TUNE_TILE_SORT, TUNE_NVLS_CTAS = 0, 1, 2, 3, 4, 5
+TUNE_HEAVY_FWD, TUNE_HEAVY_BWD, TUNE_DEPTH_SORT, TUNE_TILE_SORT, TUNE_NVLS_CTAS = 0, 1, 2, 4, 5
 
 ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_size_t)
 

@@ -221,7 +221,7 @@ static int check_arch() {
 
 // tuning knobs (gab200_tune)
 static std::atomic<int> g_tune[GAB200_NUM_TUNABLES];
-static const int g_tune_default[GAB200_NUM_TUNABLES] = {32, 2048, 0, 4, 0, 0, 0, 0};  // see GAB200_TUNE_*
+static const int g_tune_default[GAB200_NUM_TUNABLES] = {32, 2048, 0, 0, 0, 0, 0, 0};  // see GAB200_TUNE_*
 int tune_get(int knob) {
   const int v = g_tune[knob].load(std::memory_order_relaxed);
   return v > 0 ? v - 1 : g_tune_default[knob];  // stored biased by one so that zero-initialised = "default"

@@ -17,16 +17,15 @@
 //   * splat records (48 B, three 16-B quads) are GATHERED straight into shared memory with cp.async (LDGSTS),
 //     double buffered one chunk ahead, ids one further chunk ahead: no register staging, no exposed L2 latency.
 //   * forward records, per sorted instance, which of the tile's eight 8x4 blocks it contributed to (one byte);
-//     backward visits a (splat, warp) pair only if one of the warp's blocks is set and then runs code SPECIALISED for
-//     that set of live bands: a warp-uniform switch over the 2^K - 1 live-band sets selects a straight-line body in
-//     which the live bands' dependency chains interleave (ILP) and dead bands cost nothing; lanes whose pixel did
-//     not contribute carry alpha = G = 0 through the same instructions (no divergence, no BSSY/BSYNC, no vote).
-//   * backward: per-lane partial sums over the K pixels collapse to three moments (S0,S1,S2) because dx is
-//     shared; eight of the nine per-splat gradient components are transposed through a conflict-free shared-memory
-//     tile (8 STS + 2 LDS.128 + 2 shuffles), the ninth takes 5 shuffles, and they leave the SM as ONE 9-lane
-//     RED.ADD.F32 pair per (warp, splat).
+//     backward visits a (splat, warp) pair only if one of the warp's blocks is set.
+//   * backward: one WARP task per (tile, half, band group) -- K = 2 on heavy tiles, K = 4 on light ones -- with a
+//     private TMA ring for its id/mask lists and no CTA barrier.  A visit with all K bands live is straight-line code
+//     in which the bands' dependency chains interleave (ILP); otherwise the live bands run under warp-uniform
+//     branches and dead bands cost nothing.  Lanes whose pixel did not contribute carry alpha = G = 0 through the
+//     same instructions (no divergence).  Per-lane partial sums over the K pixels collapse to three moments
+//     (S0,S1,S2) because dx is shared, and the nine per-splat gradient components leave through a three-stage
+//     pipelined shared-memory row reduction that ends in one 9-lane RED.ADD.F32 per (warp, splat).
 // Tensor cores are not used: there is no dense contraction on this path (north_star).
-#include <type_traits>
 #include "common.cuh"
 #include "kernels.cuh"
 
@@ -338,30 +337,6 @@ void launch_blend_forward(int W, int H, const uint2* ranges, const uint32_t* ord
 // =====================================================================================================
 // Backward
 // =====================================================================================================
-__device__ __forceinline__ float warp_reduce1(float v) {
-#pragma unroll
-  for (int m = 16; m > 0; m >>= 1) v += __shfl_xor_sync(FULLMASK, v, m);
-  return v;
-}
-
-// Warp sum of eight values per lane through shared memory.  Lanes store v[c] to row c (stride 36 floats: the 32
-// stores of a row and the quarter-warp phases of the 128-bit loads below are both bank-conflict free), then lane L
-// sums the eight values lanes 8 (L & 3) .. 8 (L & 3) + 7 left in row L >> 2 and two shuffles combine the four
-// partial sums: on return every lane holds the warp total of component (lane >> 2).
-#define RED_ROW 36
-#define RED_WORDS (8 * RED_ROW)
-__device__ __forceinline__ float warp_reduce8_smem(const float v[8], float* scratch, int lane) {
-#pragma unroll
-  for (int c = 0; c < 8; c++) scratch[c * RED_ROW + lane] = v[c];
-  __syncwarp();
-  const float4* src = reinterpret_cast<const float4*>(scratch + (lane >> 2) * RED_ROW + (lane & 3) * 8);
-  const float4 a = src[0], b = src[1];
-  float r = ((a.x + a.y) + (a.z + a.w)) + ((b.x + b.y) + (b.z + b.w));
-  r += __shfl_xor_sync(FULLMASK, r, 1);
-  r += __shfl_xor_sync(FULLMASK, r, 2);
-  return r;
-}
-
 // Per-pixel state of the reverse walk (K pixels per lane, one per band).
 template <int K>
 struct PixState {
@@ -374,140 +349,6 @@ struct PixState {
 };
 struct SplatSums {  // per-lane sums over the lane's pixels for one splat
   float S0, S1, S2, go, gr, gg, gb;
-};
-
-// ---- fp32 pairs -----------------------------------------------------------------------------------------------
-// Variants 8 and 9: the two bands of a pair run the same straight-line arithmetic, so their state lives in float2 and
-// each pair operation is two scalar IEEE fp32 operations with explicit round-to-nearest (Hopper has no packed fp32 FMA).  The
-// _rn intrinsics are never contracted or reassociated by the compiler, so every value rounds exactly as written.
-typedef float2 v2;
-__device__ __forceinline__ v2 bc2(float a) { return make_float2(a, a); }
-__device__ __forceinline__ v2 neg2(v2 a) { return make_float2(-a.x, -a.y); }
-__device__ __forceinline__ v2 add2(v2 a, v2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
-__device__ __forceinline__ v2 mul2(v2 a, v2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
-__device__ __forceinline__ v2 fma2(v2 a, v2 b, v2 c) {
-  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
-}
-
-// element i of a per-band array, whichever way it is stored
-__device__ __forceinline__ float& el(float* a, int i) { return a[i]; }
-__device__ __forceinline__ int& el(int* a, int i) { return a[i]; }
-__device__ __forceinline__ float& el(v2* a, int i) { return (i & 1) ? a[i >> 1].y : a[i >> 1].x; }
-
-// The same state with bands (2J, 2J+1) paired in float2 registers.
-template <int K>
-struct PixState2 {
-  v2 fy[K / 2], T[K / 2];
-  v2 ar[K / 2], ag[K / 2], ab[K / 2];
-  v2 dr[K / 2], dg[K / 2], db[K / 2];
-  v2 bgT[K / 2];
-  int nc[K];
-};
-struct SplatSums2 {  // (even band, odd band) partial sums, added at the end of the visit
-  v2 S0, S1, S2, go, gr, gg, gb;
-};
-// Bands 2J and 2J+1 of one visit, both live: visit_bands' arithmetic, element for element, two bands per instruction.
-template <int K, int J>
-__device__ __forceinline__ void visit_pair(PixState2<K>& p, int pos, float py, float tA, float dx, float Bp, float Cp,
-                                           float op, float cr, float cg, float cb, SplatSums2& s) {
-  const v2 dy = add2(bc2(py), neg2(p.fy[J]));
-  const v2 pw = fma2(mul2(bc2(Cp), dy), dy, mul2(fma2(bc2(Bp), dy, bc2(tA)), bc2(dx)));  // the forward's expression
-  const v2 G = make_float2(ex2_approx(pw.x), ex2_approx(pw.y));
-  const v2 a = mul2(bc2(op), G);
-  const v2 alpha = make_float2(fminf(0.99f, a.x), fminf(0.99f, a.y));
-  const bool vx = pos < p.nc[2 * J] && pw.x <= 0.f && alpha.x >= ALPHA_MIN;
-  const bool vy = pos < p.nc[2 * J + 1] && pw.y <= 0.f && alpha.y >= ALPHA_MIN;
-  const v2 om = add2(bc2(1.f), neg2(alpha));
-  const v2 al = make_float2(vx ? alpha.x : 0.f, vy ? alpha.y : 0.f);
-  const v2 Gv = make_float2(vx ? G.x : 0.f, vy ? G.y : 0.f);
-  const v2 ra = make_float2(vx ? rcp_approx(om.x) : 1.f, vy ? rcp_approx(om.y) : 1.f);
-  const v2 Tn = mul2(p.T[J], ra);
-  p.T[J] = Tn;
-  const v2 w = mul2(al, Tn);
-  s.gr = fma2(w, p.dr[J], s.gr);
-  s.gg = fma2(w, p.dg[J], s.gg);
-  s.gb = fma2(w, p.db[J], s.gb);
-  const v2 er = add2(bc2(cr), neg2(p.ar[J])), eg = add2(bc2(cg), neg2(p.ag[J])), eb = add2(bc2(cb), neg2(p.ab[J]));
-  v2 dLda = mul2(er, p.dr[J]);
-  dLda = fma2(eg, p.dg[J], dLda);
-  dLda = fma2(eb, p.db[J], dLda);
-  dLda = fma2(dLda, Tn, neg2(mul2(p.bgT[J], ra)));
-  p.ar[J] = fma2(al, er, p.ar[J]);
-  p.ag[J] = fma2(al, eg, p.ag[J]);
-  p.ab[J] = fma2(al, eb, p.ab[J]);
-  const v2 t = mul2(Gv, dLda);
-  s.go = add2(s.go, t);
-  const v2 s_ = mul2(bc2(op), t);
-  const v2 sd = mul2(s_, dy);
-  s.S0 = add2(s.S0, s_);
-  s.S1 = add2(s.S1, sd);
-  s.S2 = fma2(sd, dy, s.S2);
-}
-// One live band I of a pair-stored state (the other band of its pair is dead for this splat): scalar arithmetic on
-// the band's half of the registers, sums into the matching half of the accumulators.
-template <int K, int I>
-__device__ __forceinline__ void visit_single(PixState2<K>& p, int pos, float py, float tA, float dx, float Bp, float Cp,
-                                             float op, float cr, float cg, float cb, SplatSums2& s) {
-  const float dy = py - el(p.fy, I);
-  const float pw = fmaf(Cp * dy, dy, fmaf(Bp, dy, tA) * dx);
-  const float G = ex2_approx(pw);
-  const float alpha = fminf(0.99f, op * G);
-  const bool valid = pos < p.nc[I] && pw <= 0.f && alpha >= ALPHA_MIN;
-  const float al = valid ? alpha : 0.f;
-  const float Gv = valid ? G : 0.f;
-  const float ra = valid ? rcp_approx(1.f - alpha) : 1.f;
-  const float Tn = el(p.T, I) * ra;
-  el(p.T, I) = Tn;
-  const float w = al * Tn;
-  const float dr = el(p.dr, I), dg = el(p.dg, I), db = el(p.db, I);
-  el(&s.gr, I & 1) = fmaf(w, dr, el(&s.gr, I & 1));
-  el(&s.gg, I & 1) = fmaf(w, dg, el(&s.gg, I & 1));
-  el(&s.gb, I & 1) = fmaf(w, db, el(&s.gb, I & 1));
-  const float er = cr - el(p.ar, I), eg = cg - el(p.ag, I), eb = cb - el(p.ab, I);
-  float dLda = er * dr;
-  dLda = fmaf(eg, dg, dLda);
-  dLda = fmaf(eb, db, dLda);
-  dLda = fmaf(dLda, Tn, -el(p.bgT, I) * ra);
-  el(p.ar, I) = fmaf(al, er, el(p.ar, I));
-  el(p.ag, I) = fmaf(al, eg, el(p.ag, I));
-  el(p.ab, I) = fmaf(al, eb, el(p.ab, I));
-  const float t = Gv * dLda;
-  el(&s.go, I & 1) += t;
-  const float s_ = op * t;
-  const float sd = s_ * dy;
-  el(&s.S0, I & 1) += s_;
-  el(&s.S1, I & 1) += sd;
-  el(&s.S2, I & 1) = fmaf(sd, dy, el(&s.S2, I & 1));
-}
-// pairs one after the other; a pair with one live band takes the scalar form, a dead pair is skipped (uniform branches)
-template <int K, int J>
-struct PairLoop {
-  static __device__ __forceinline__ void run(uint32_t m, PixState2<K>& p, int pos, float py, float tA, float dx, float Bp,
-                                             float Cp, float op, float cr, float cg, float cb, SplatSums2& s) {
-    const uint32_t mm = (m >> (2 * J)) & 3u;
-    if (mm == 3u) visit_pair<K, J>(p, pos, py, tA, dx, Bp, Cp, op, cr, cg, cb, s);
-    else if (mm == 1u) visit_single<K, 2 * J>(p, pos, py, tA, dx, Bp, Cp, op, cr, cg, cb, s);
-    else if (mm == 2u) visit_single<K, 2 * J + 1>(p, pos, py, tA, dx, Bp, Cp, op, cr, cg, cb, s);
-    PairLoop<K, J + 1>::run(m, p, pos, py, tA, dx, Bp, Cp, op, cr, cg, cb, s);
-  }
-};
-template <int K>
-struct PairLoop<K, K / 2> {
-  static __device__ __forceinline__ void run(uint32_t, PixState2<K>&, int, float, float, float, float, float, float, float,
-                                             float, float, SplatSums2&) {}
-};
-template <int K, int J>
-struct PairAll {  // every band live: all pairs packed, straight line
-  static __device__ __forceinline__ void run(PixState2<K>& p, int pos, float py, float tA, float dx, float Bp, float Cp,
-                                             float op, float cr, float cg, float cb, SplatSums2& s) {
-    visit_pair<K, J>(p, pos, py, tA, dx, Bp, Cp, op, cr, cg, cb, s);
-    PairAll<K, J + 1>::run(p, pos, py, tA, dx, Bp, Cp, op, cr, cg, cb, s);
-  }
-};
-template <int K>
-struct PairAll<K, K / 2> {
-  static __device__ __forceinline__ void run(PixState2<K>&, int, float, float, float, float, float, float, float, float,
-                                             float, SplatSums2&) {}
 };
 
 // One (splat, warp) visit restricted to the live bands M (compile-time set): straight-line code, the bands'
@@ -570,228 +411,7 @@ struct BandLoop<K, K> {
                                              float, float, SplatSums&) {}
 };
 
-template <int K>
-__device__ __forceinline__ void visit_switch(uint32_t m, PixState<K>& p, int pos, float py, float tA, float dx,
-                                             float Bp, float Cp, float op, float cr, float cg, float cb,
-                                             SplatSums& s);
-#define GAB_VISIT(M) \
-  case M: visit_bands<K, M>(p, pos, py, tA, dx, Bp, Cp, op, cr, cg, cb, s); break;
-template <>
-__device__ __forceinline__ void visit_switch<2>(uint32_t m, PixState<2>& p, int pos, float py, float tA, float dx,
-                                                float Bp, float Cp, float op, float cr, float cg, float cb,
-                                                SplatSums& s) {
-  constexpr int K = 2;
-  switch (m) {
-    GAB_VISIT(1) GAB_VISIT(2) GAB_VISIT(3)
-    default: break;
-  }
-}
-template <>
-__device__ __forceinline__ void visit_switch<4>(uint32_t m, PixState<4>& p, int pos, float py, float tA, float dx,
-                                                float Bp, float Cp, float op, float cr, float cg, float cb,
-                                                SplatSums& s) {
-  constexpr int K = 4;
-  switch (m) {
-    GAB_VISIT(1) GAB_VISIT(2) GAB_VISIT(3) GAB_VISIT(4) GAB_VISIT(5) GAB_VISIT(6) GAB_VISIT(7) GAB_VISIT(8)
-    GAB_VISIT(9) GAB_VISIT(10) GAB_VISIT(11) GAB_VISIT(12) GAB_VISIT(13) GAB_VISIT(14) GAB_VISIT(15)
-    default: break;
-  }
-}
-#undef GAB_VISIT
-
-template <int K>
-__device__ __forceinline__ void backward_tile(int tile, int tl, GroupBarrier<256 / K> bar, SplatRec* buf0,
-                                              SplatRec* buf1, uint32_t* bid0, uint32_t* bid1, uint32_t* bm0,
-                                              uint32_t* bm1, int* s_max, uint32_t* ids_ring, uint8_t* mask_ring,
-                                              uint64_t* mbar, float* red, int W, int H, int gx,
-                                              const uint2* __restrict__ ranges,
-                                              const uint32_t* __restrict__ point_list,
-                                              const SplatRec* __restrict__ rec, const float* __restrict__ bg,
-                                              const float* __restrict__ final_T,
-                                              const uint32_t* __restrict__ n_contrib,
-                                              const float* __restrict__ dL_dpix,
-                                              const uint8_t* __restrict__ strip_mask, float* __restrict__ g2d) {
-  constexpr int NT = 256 / K;
-  const int tx = tile % gx, ty = tile / gx;
-  const int lane = tl & 31;
-  const BandGeom<K> geo(tl);
-  const int pixx = tx * GAB_TILE + geo.col;
-  const int pixy0 = ty * GAB_TILE + geo.row0;
-  const float fx = (float)pixx;
-  const uint2 range = ranges[tile];
-  const size_t HW = (size_t)H * W;
-  const float bg0 = bg[0], bg1 = bg[1], bg2 = bg[2];
-
-  PixState<K> p;
-  int my_max = 0;
-#pragma unroll
-  for (int i = 0; i < K; i++) {
-    const int y = pixy0 + 4 * i;
-    p.fy[i] = (float)y;
-    p.ar[i] = p.ag[i] = p.ab[i] = 0.f;
-    if (pixx < W && y < H) {
-      const size_t pix = (size_t)y * W + pixx;
-      p.T[i] = final_T[pix];
-      p.nc[i] = (int)n_contrib[pix];
-      p.dr[i] = dL_dpix[pix];
-      p.dg[i] = dL_dpix[HW + pix];
-      p.db[i] = dL_dpix[2 * HW + pix];
-    } else {
-      p.T[i] = 0.f; p.nc[i] = 0; p.dr[i] = p.dg[i] = p.db[i] = 0.f;
-    }
-    p.bgT[i] = p.T[i] * (bg0 * p.dr[i] + bg1 * p.dg[i] + bg2 * p.db[i]);
-    my_max = max(my_max, p.nc[i]);
-  }
-  // the tile only needs instances [0, max n_contrib): nothing behind the last contributor of any pixel matters
-  if (tl == 0) *s_max = 0;
-  bar.sync();
-  my_max = __reduce_max_sync(FULLMASK, my_max);
-  if (lane == 0 && my_max > 0) atomicMax(s_max, my_max);
-  bar.sync();
-  const int n = *s_max;
-  if (n == 0) return;
-  const int nchunks = (n + NT - 1) / NT;
-  const float half_W = 0.5f * (float)W, half_H = 0.5f * (float)H;
-
-  // reverse walk: chunk c covers positions n-1-c*NT-j (j = 0..NT-1), i.e. the ascending run [lo_c, lo_c + NT) with
-  // lo_c = max(0, n - (c+1) NT).  Ids and block masks of a chunk arrive by two TMA bulk copies on one mbarrier
-  // (same 16-B alignment treatment as in the forward), two chunks ahead.
-  constexpr int ID_STRIDE = NT + 4;    // u32 per ring slot
-  constexpr int MK_STRIDE = NT + 16;   // bytes per ring slot
-  constexpr uint32_t TX_BYTES = ID_STRIDE * 4 + MK_STRIDE;
-  auto chunk_lo = [&](int k) { return max(0, n - (k + 1) * NT); };
-  if (tl == 0) {
-#pragma unroll
-    for (int k = 0; k < ID_RING; k++) mbar_init(&mbar[k], 1);
-    mbar_fence_init();
-  }
-  bar.sync();
-  auto issue_lists = [&](int k) {
-    const uint32_t lo = range.x + (uint32_t)chunk_lo(k);
-    uint64_t* b = &mbar[k % ID_RING];
-    mbar_arrive_expect_tx(b, TX_BYTES);
-    bulk_copy_g2s(ids_ring + (k % ID_RING) * ID_STRIDE, point_list + (lo & ~3u), ID_STRIDE * 4, b);
-    bulk_copy_g2s(mask_ring + (k % ID_RING) * MK_STRIDE, strip_mask + (lo & ~15u), MK_STRIDE, b);
-  };
-  auto wait_lists = [&](int k) { mbar_wait(&mbar[k % ID_RING], (uint32_t)((k / ID_RING) & 1)); };
-  // this thread's (id, mask) of chunk k: reverse index p = k NT + tl  <->  position n-1-p
-  auto my_entry = [&](int k, uint32_t& id, uint32_t& mask) {
-    const int q = k * NT + tl;
-    id = 0xffffffffu;
-    mask = 0u;
-    if (q < n) {
-      const int lo = chunk_lo(k);
-      const uint32_t g0 = range.x + (uint32_t)lo;
-      const int rel = (n - 1 - q) - lo;
-      id = ids_ring[(k % ID_RING) * ID_STRIDE + (int)(g0 & 3u) + rel];
-      mask = mask_ring[(k % ID_RING) * MK_STRIDE + (int)(g0 & 15u) + rel];
-    }
-  };
-  if (tl == 0) {
-    issue_lists(0);
-    if (nchunks > 1) issue_lists(1);
-  }
-  uint32_t id_cur, mask_cur;
-  wait_lists(0);
-  my_entry(0, id_cur, mask_cur);
-  if (id_cur != 0xffffffffu && mask_cur != 0) gather_rec(&buf0[tl], rec + id_cur);
-  bid0[tl] = id_cur;
-  bm0[tl] = mask_cur;
-  cp_async_commit();
-
-  // this warp's K blocks inside the mask byte: bits geo.bit(0), geo.bit(0) + 2, ... (one half, consecutive bands)
-  const int bit0 = geo.bit(0);
-  auto my_bands = [&](uint32_t mask) {
-    uint32_t m = 0;
-#pragma unroll
-    for (int i = 0; i < K; i++) m |= ((mask >> (bit0 + 2 * i)) & 1u) << i;
-    return m;
-  };
-  float* red_w = red + (tl >> 5) * (2 * RED_WORDS);
-  uint32_t flip = 0;
-
-  for (int c = 0; c < nchunks; c++) {
-    const bool odd = (c & 1) != 0;
-    if (c + 1 < nchunks) {
-      wait_lists(c + 1);
-      my_entry(c + 1, id_cur, mask_cur);
-      SplatRec* nb = odd ? buf0 : buf1;
-      if (id_cur != 0xffffffffu && mask_cur != 0) gather_rec(&nb[tl], rec + id_cur);
-      (odd ? bid0 : bid1)[tl] = id_cur;
-      (odd ? bm0 : bm1)[tl] = mask_cur;
-    }
-    cp_async_commit();
-    if (tl == 0 && c + 2 < nchunks) issue_lists(c + 2);
-    cp_async_wait<1>();
-    bar.sync();
-    const SplatRec* cur = odd ? buf1 : buf0;
-    const uint32_t* cur_id = odd ? bid1 : bid0;
-    const uint32_t* cur_mask = odd ? bm1 : bm0;
-    const int cnt = min(NT, n - c * NT);
-    for (int gbase = 0; gbase < cnt; gbase += 32) {
-      // lane L looks at entry gbase + L: which of this warp's bands did it touch?  The warp then walks the entries
-      // with a non-empty set in order (ascending j = back to front).
-      const uint32_t mine = (gbase + lane < cnt) ? my_bands(cur_mask[gbase + lane]) : 0u;
-      uint32_t todo = __ballot_sync(FULLMASK, mine != 0u);
-      while (todo) {
-        const int jj = __ffs(todo) - 1;
-        todo &= todo - 1;
-        const uint32_t m = __shfl_sync(FULLMASK, mine, jj);
-        const int j = gbase + jj;
-        const int pos = n - 1 - c * NT - j;  // 0-based position in the tile's list; contributes to a pixel iff pos < nc
-        const float4 q0 = cur[j].q0;
-        const float4 q1 = cur[j].q1;
-        const float cbl = cur[j].q2.x;
-        const float dx = q0.x - fx;
-        const float tA = q0.z * dx;  // conic is stored pre-scaled: (A',B',C') = (-A/2, -B, -C/2) * log2(e)
-        SplatSums s;
-        s.S0 = s.S1 = s.S2 = s.go = s.gr = s.gg = s.gb = 0.f;
-        visit_switch<K>(m, p, pos, q0.y, tA, dx, q0.w, q1.x, q1.y, q1.z, q1.w, cbl, s);
-        const float A = q0.z * CONIC_UNSCALE_AC, B = q0.w * CONIC_UNSCALE_B, C = q1.x * CONIC_UNSCALE_AC;
-        float v[8];
-        const float dxS0 = dx * s.S0;
-        v[0] = (-A * dxS0 - B * s.S1) * half_W;  // dL/dmean2D.x (NDC units)
-        v[1] = (-C * s.S1 - B * dxS0) * half_H;  // dL/dmean2D.y
-        v[2] = -0.5f * dx * dxS0;                // dL/dconic.xx
-        v[3] = -0.5f * dx * s.S1;                // dL/dconic.xy (stored once)
-        v[4] = -0.5f * s.S2;                     // dL/dconic.yy
-        v[5] = s.go;                             // dL/dopacity
-        v[6] = s.gr;
-        v[7] = s.gg;
-        const float r8 = warp_reduce8_smem(v, red_w + flip, lane);
-        flip ^= RED_WORDS;  // the next visit stores into the other tile: its __syncwarp orders this one's loads
-        const float r1 = warp_reduce1(s.gb);
-        const uint32_t id = cur_id[j];
-        if ((lane & 3) == 0)
-          atomicAdd(g2d + (size_t)id * GAB_G2D_STRIDE + (lane >> 2), r8);
-        else if (lane == 1)
-          atomicAdd(g2d + (size_t)id * GAB_G2D_STRIDE + 8, r1);
-      }
-    }
-    bar.sync();
-  }
-  cp_async_wait<0>();
-}
-
-// =====================================================================================================
-// Backward, warp-independent form (variant 1..3 of GAB200_TUNE_BWD_VARIANT)
-// =====================================================================================================
-// Same pixel ownership and per-pair arithmetic as backward_tile above, different schedule:
-//   * a WARP is the unit of work: (tile, half, band group).  It stages its own id/mask lists (TMA bulk copies into a
-//     private 3-slot ring) and gathers only the records of entries that touch ITS blocks -- no CTA barrier anywhere,
-//     the two (four) warps of a tile drift apart freely, and each walks only up to ITS pixels' largest n_contrib.
-//   * the visit is one straight-line block (BANDS_ALWAYS: all K bands, dead lanes carry zeros) so the compiler can
-//     interleave the bands' chains with ...
-//   * ... a SOFTWARE-PIPELINED reduction: visit j stores its nine per-lane values as rows of a shared-memory tile;
-//     during visit j+1 eighteen lanes each add half a row (4 LDS.128) and store 18 partials; during visit j+2 nine
-//     lanes add the two halves and issue the RED.  No shuffle, no exposed shared-memory or shuffle latency: the
-//     loads of round 1/2 are issued at the top of a visit and consumed after its band math.
-#define BANDS_ALWAYS 1    // straight-line, every band every visit
-#define BANDS_UNIFORM 2   // each band under a warp-uniform branch (dead bands skipped, no interleaving)
-#define BANDS_HYBRID 3    // all bands live: straight-line; otherwise as BANDS_UNIFORM
-#define BANDS_SWITCH 4    // one straight-line body per live-band set (visit_switch)
-#define BANDS_PACKED 5    // as BANDS_HYBRID with the bands of a pair in packed fp32x2 arithmetic (FFMA2/FMUL2/FADD2)
-
+// Shared memory of one backward warp task.
 #define ROWS_STRIDE 36
 #define ROWS_WORDS (9 * ROWS_STRIDE)
 struct __align__(16) WarpSmem {
@@ -803,7 +423,18 @@ struct __align__(16) WarpSmem {
   uint64_t mbar[ID_RING];
 };
 
-template <int K, int MODE>
+// One warp task: the pixels of one (tile, half, band group), same ownership as the forward (BandGeom).
+//   * The WARP is the unit of work.  It stages its own id/mask lists (TMA bulk copies into a private 3-slot ring) and
+//     gathers only the records of entries that touch ITS blocks -- no CTA barrier anywhere, the warps of a tile drift
+//     apart freely, and each walks only up to ITS pixels' largest n_contrib.
+//   * A visit whose K bands are all live is one straight-line block, so the compiler interleaves the bands'
+//     dependency chains; otherwise each band runs under a warp-uniform branch and dead bands cost nothing (BandLoop).
+//   * The nine gradient components leave through a SOFTWARE-PIPELINED reduction: visit j stores its nine per-lane
+//     values as rows of a shared-memory tile; during visit j+1 eighteen lanes each add half a row (4 LDS.128) and
+//     store 18 partials; during visit j+2 nine lanes add the two halves and issue the RED.  No shuffle, no exposed
+//     shared-memory or shuffle latency: the loads of rounds 1 and 2 are issued at the top of a visit and consumed
+//     after its band math.
+template <int K>
 __device__ __forceinline__ void backward_task(int tile, int tl, WarpSmem& sm, int W, int H, int gx,
                                               const uint2* __restrict__ ranges,
                                               const uint32_t* __restrict__ point_list,
@@ -822,14 +453,13 @@ __device__ __forceinline__ void backward_task(int tile, int tl, WarpSmem& sm, in
   const size_t HW = (size_t)H * W;
   const float bg0 = bg[0], bg1 = bg[1], bg2 = bg[2];
 
-  constexpr bool PACKED = (MODE == BANDS_PACKED);
-  typename std::conditional<PACKED, PixState2<K>, PixState<K>>::type p;
+  PixState<K> p;
   int n = 0;
 #pragma unroll
   for (int i = 0; i < K; i++) {
     const int y = pixy0 + 4 * i;
-    el(p.fy, i) = (float)y;
-    el(p.ar, i) = el(p.ag, i) = el(p.ab, i) = 0.f;
+    p.fy[i] = (float)y;
+    p.ar[i] = p.ag[i] = p.ab[i] = 0.f;
     float T0 = 0.f, dr = 0.f, dg = 0.f, db = 0.f;
     p.nc[i] = 0;
     if (pixx < W && y < H) {
@@ -840,11 +470,11 @@ __device__ __forceinline__ void backward_task(int tile, int tl, WarpSmem& sm, in
       dg = dL_dpix[HW + pix];
       db = dL_dpix[2 * HW + pix];
     }
-    el(p.T, i) = T0;
-    el(p.dr, i) = dr;
-    el(p.dg, i) = dg;
-    el(p.db, i) = db;
-    el(p.bgT, i) = T0 * (bg0 * dr + bg1 * dg + bg2 * db);
+    p.T[i] = T0;
+    p.dr[i] = dr;
+    p.dg[i] = dg;
+    p.db[i] = db;
+    p.bgT[i] = T0 * (bg0 * dr + bg1 * dg + bg2 * db);
     n = max(n, p.nc[i]);
   }
   // this warp only needs instances [0, max n_contrib of ITS pixels)
@@ -907,17 +537,8 @@ __device__ __forceinline__ void backward_task(int tile, int tl, WarpSmem& sm, in
     const float4* r4 = reinterpret_cast<const float4*>(&sm.rows[par ^ 1][c1 * ROWS_STRIDE + h1 * 16]);
     const float4 a = r4[0], b = r4[1], c = r4[2], d = r4[3];
     if (id_part != 0xffffffffu && lane < 9) atomicAdd(g2d + (size_t)id_part * GAB_G2D_STRIDE + lane, pp.x + pp.y);
-    float s;
-    if constexpr (PACKED) {  // 7 packed adds + 1 instead of 15
-      const v2 u = add2(add2(add2(make_float2(a.x, a.y), make_float2(a.z, a.w)),
-                             add2(make_float2(b.x, b.y), make_float2(b.z, b.w))),
-                        add2(add2(make_float2(c.x, c.y), make_float2(c.z, c.w)),
-                             add2(make_float2(d.x, d.y), make_float2(d.z, d.w))));
-      s = u.x + u.y;
-    } else {
-      s = (((a.x + a.y) + (a.z + a.w)) + ((b.x + b.y) + (b.z + b.w))) +
-          (((c.x + c.y) + (c.z + c.w)) + ((d.x + d.y) + (d.z + d.w)));
-    }
+    const float s = (((a.x + a.y) + (a.z + a.w)) + ((b.x + b.y) + (b.z + b.w))) +
+                    (((c.x + c.y) + (c.z + c.w)) + ((d.x + d.y) + (d.z + d.w)));
     if (id_rows != 0xffffffffu && lane < 18) sm.part[par ^ 1][lane] = s;
   };
 
@@ -945,20 +566,8 @@ __device__ __forceinline__ void backward_task(int tile, int tl, WarpSmem& sm, in
       const float tA = q0.z * dx;
       SplatSums s;
       s.S0 = s.S1 = s.S2 = s.go = s.gr = s.gg = s.gb = 0.f;
-      if constexpr (PACKED) {
-        SplatSums2 s2;
-        s2.S0 = s2.S1 = s2.S2 = s2.go = s2.gr = s2.gg = s2.gb = make_float2(0.f, 0.f);
-        if (m == (1u << K) - 1u) PairAll<K, 0>::run(p, pos, q0.y, tA, dx, q0.w, q1.x, q1.y, q1.z, q1.w, cbl, s2);
-        else PairLoop<K, 0>::run(m, p, pos, q0.y, tA, dx, q0.w, q1.x, q1.y, q1.z, q1.w, cbl, s2);
-        s.S0 = s2.S0.x + s2.S0.y; s.S1 = s2.S1.x + s2.S1.y; s.S2 = s2.S2.x + s2.S2.y; s.go = s2.go.x + s2.go.y;
-        s.gr = s2.gr.x + s2.gr.y; s.gg = s2.gg.x + s2.gg.y; s.gb = s2.gb.x + s2.gb.y;
-      } else if (MODE == BANDS_ALWAYS || (MODE == BANDS_HYBRID && m == (1u << K) - 1u)) {
-        visit_bands<K, (1 << K) - 1>(p, pos, q0.y, tA, dx, q0.w, q1.x, q1.y, q1.z, q1.w, cbl, s);
-      } else if (MODE == BANDS_SWITCH) {
-        visit_switch<K>(m, p, pos, q0.y, tA, dx, q0.w, q1.x, q1.y, q1.z, q1.w, cbl, s);
-      } else {
-        BandLoop<K, 0>::run(m, p, pos, q0.y, tA, dx, q0.w, q1.x, q1.y, q1.z, q1.w, cbl, s);
-      }
+      if (m == (1u << K) - 1u) visit_bands<K, (1 << K) - 1>(p, pos, q0.y, tA, dx, q0.w, q1.x, q1.y, q1.z, q1.w, cbl, s);
+      else BandLoop<K, 0>::run(m, p, pos, q0.y, tA, dx, q0.w, q1.x, q1.y, q1.z, q1.w, cbl, s);
       const float A = q0.z * CONIC_UNSCALE_AC, B = q0.w * CONIC_UNSCALE_B, C = q1.x * CONIC_UNSCALE_AC;
       const float dxS0 = dx * s.S0;
       float* row = &sm.rows[par][lane];
@@ -990,70 +599,30 @@ __device__ __forceinline__ void backward_task(int tile, int tl, WarpSmem& sm, in
   }
 }
 
-template <int MODE, int MINB>
-__global__ void __launch_bounds__(128, MINB) blend_backward_warp_kernel(int W, int H, int gx, int tiles,
-                                                                      const uint2* __restrict__ ranges,
-                                                                      const uint32_t* __restrict__ order,
-                                                                      const uint32_t* __restrict__ order_info,
-                                                                      const uint32_t* __restrict__ point_list,
-                                                                      const SplatRec* __restrict__ rec,
-                                                                      const float* __restrict__ bg,
-                                                                      const float* __restrict__ final_T,
-                                                                      const uint32_t* __restrict__ n_contrib,
-                                                                      const float* __restrict__ dL_dpix,
-                                                                      const uint8_t* __restrict__ strip_mask,
-                                                                      float* __restrict__ g2d) {
+// CTA = 128 threads: CTAs [0, n_heavy) take one heavy tile on four warps, K = 2; the rest take two light tiles each,
+// two warps (the halves) per tile, K = 4.  5 CTAs per SM was the fastest occupancy measured on the H100.
+__global__ void __launch_bounds__(128, 5) blend_backward_kernel(int W, int H, int gx, int tiles,
+                                                                const uint2* __restrict__ ranges,
+                                                                const uint32_t* __restrict__ order,
+                                                                const uint32_t* __restrict__ order_info,
+                                                                const uint32_t* __restrict__ point_list,
+                                                                const SplatRec* __restrict__ rec,
+                                                                const float* __restrict__ bg,
+                                                                const float* __restrict__ final_T,
+                                                                const uint32_t* __restrict__ n_contrib,
+                                                                const float* __restrict__ dL_dpix,
+                                                                const uint8_t* __restrict__ strip_mask,
+                                                                float* __restrict__ g2d) {
   __shared__ WarpSmem sm[4];
   const int nh = (int)order_info[1];
   const int b = blockIdx.x, t = threadIdx.x, w = t >> 5;
   if (b < nh) {  // heavy tile: four warps, two bands each
-    backward_task<2, MODE>((int)order[b], t, sm[w], W, H, gx, ranges, point_list, rec, bg, final_T, n_contrib, dL_dpix,
-                           strip_mask, g2d);
+    backward_task<2>((int)order[b], t, sm[w], W, H, gx, ranges, point_list, rec, bg, final_T, n_contrib, dL_dpix,
+                     strip_mask, g2d);
   } else {       // two light tiles: two warps (the halves) each, four bands per warp
     const int slot = nh + 2 * (b - nh) + (w >> 1);
     if (slot >= tiles) return;
-    backward_task<4, MODE>((int)order[slot], t & 63, sm[w], W, H, gx, ranges, point_list, rec, bg, final_T, n_contrib,
-                           dL_dpix, strip_mask, g2d);
-  }
-}
-
-#ifndef BWD_MIN_BLOCKS
-#define BWD_MIN_BLOCKS 4
-#endif
-// CTA = 128 threads: CTAs [0, n_heavy) take one heavy tile with K = 2 (four warps); the rest take two light tiles
-// each, one per 64-thread group with K = 4.
-__global__ void __launch_bounds__(128, BWD_MIN_BLOCKS) blend_backward_kernel(int W, int H, int gx, int tiles,
-                                                             const uint2* __restrict__ ranges,
-                                                             const uint32_t* __restrict__ order,
-                                                             const uint32_t* __restrict__ order_info,
-                                                             const uint32_t* __restrict__ point_list,
-                                                             const SplatRec* __restrict__ rec,
-                                                             const float* __restrict__ bg,
-                                                             const float* __restrict__ final_T,
-                                                             const uint32_t* __restrict__ n_contrib,
-                                                             const float* __restrict__ dL_dpix,
-                                                             const uint8_t* __restrict__ strip_mask,
-                                                             float* __restrict__ g2d) {
-  __shared__ SplatRec buf[2][128];
-  __shared__ uint32_t bid[2][128];
-  __shared__ uint32_t bm[2][128];
-  __shared__ int s_max[2];
-  __shared__ __align__(16) uint32_t ids_ring[2][ID_RING * (64 + 4)];   // per 64-thread group; a 128-thread tile uses it flat
-  __shared__ __align__(16) uint8_t mask_ring[2][ID_RING * (64 + 16)];
-  __shared__ __align__(8) uint64_t mbar[2][ID_RING];
-  __shared__ __align__(16) float red[4 * 2 * RED_WORDS];  // per warp: two transposition tiles used alternately
-  const int nh = (int)order_info[1];
-  const int b = blockIdx.x, t = threadIdx.x;
-  if (b < nh) {
-    backward_tile<2>((int)order[b], t, GroupBarrier<128>{0}, buf[0], buf[1], bid[0], bid[1], bm[0], bm[1], &s_max[0],
-                     &ids_ring[0][0], &mask_ring[0][0], mbar[0], red, W, H, gx, ranges, point_list, rec, bg, final_T,
-                     n_contrib, dL_dpix, strip_mask, g2d);
-  } else {
-    const int g = t >> 6, slot = nh + 2 * (b - nh) + g;
-    if (slot >= tiles) return;
-    backward_tile<4>((int)order[slot], t & 63, GroupBarrier<64>{1 + g}, buf[0] + g * 64, buf[1] + g * 64,
-                     bid[0] + g * 64, bid[1] + g * 64, bm[0] + g * 64, bm[1] + g * 64, &s_max[g], ids_ring[g], mask_ring[g],
-                     mbar[g], red + g * (2 * 2 * RED_WORDS), W, H, gx, ranges, point_list, rec, bg, final_T, n_contrib,
+    backward_task<4>((int)order[slot], t & 63, sm[w], W, H, gx, ranges, point_list, rec, bg, final_T, n_contrib,
                      dL_dpix, strip_mask, g2d);
   }
 }
@@ -1065,25 +634,8 @@ void launch_blend_backward(int W, int H, const uint2* ranges, const uint32_t* or
   const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
   const int tiles = gx * gy;
   if (tiles == 0) return;
-#define GAB_BWD_WARP(MODE, MINB)                                                                                  \
-  blend_backward_warp_kernel<MODE, MINB><<<tiles, 128, 0, stream>>>(W, H, gx, tiles, ranges, order, order_info,      \
-                                                                    point_list, rec, bg, final_T, n_contrib, dL_dpix, \
-                                                                    strip_mask, g2d)
-  switch (tune_get(GAB200_TUNE_BWD_VARIANT)) {
-    case 1: GAB_BWD_WARP(BANDS_ALWAYS, 4); break;
-    case 2: GAB_BWD_WARP(BANDS_UNIFORM, 4); break;
-    case 3: GAB_BWD_WARP(BANDS_HYBRID, 4); break;
-    case 4: GAB_BWD_WARP(BANDS_HYBRID, 5); break;
-    case 5: GAB_BWD_WARP(BANDS_UNIFORM, 5); break;
-    case 6: GAB_BWD_WARP(BANDS_SWITCH, 4); break;
-    case 7: GAB_BWD_WARP(BANDS_UNIFORM, 6); break;
-    case 8: GAB_BWD_WARP(BANDS_PACKED, 4); break;
-    case 9: GAB_BWD_WARP(BANDS_PACKED, 5); break;
-    default:
-      blend_backward_kernel<<<tiles, 128, 0, stream>>>(W, H, gx, tiles, ranges, order, order_info, point_list, rec, bg,
-                                                       final_T, n_contrib, dL_dpix, strip_mask, g2d);
-  }
-#undef GAB_BWD_WARP
+  blend_backward_kernel<<<tiles, 128, 0, stream>>>(W, H, gx, tiles, ranges, order, order_info, point_list, rec, bg,
+                                                   final_T, n_contrib, dL_dpix, strip_mask, g2d);
   count_launch();
 }
 

@@ -51,8 +51,7 @@ __global__ void __launch_bounds__(PRE_NT) preprocess_kernel(gab200_forward_args 
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= a.P) return;
   // the other 44 bytes per splat: quaternion as one LDG.128, positions / scales / opacity as coalesced scalar loads
-  // (staging the two 12-byte-stride arrays through shared memory for 128-bit loads costs one more barrier for 24 of
-  // the 284 bytes -- load_raw_staged in splat_math.cuh)
+  // (staging them would cost a barrier for 24 of the 284 bytes)
   RawAttr raw;
   load_raw(a, i, raw);
   const float* my_sh = sh_s + threadIdx.x * sh_stride;

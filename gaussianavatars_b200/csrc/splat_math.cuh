@@ -146,8 +146,8 @@ struct BindCtx {
 
 // The 11 per-splat floats besides the SH coefficients (position, quaternion, scales, opacity; raw or activated
 // depending on the input mode).  The quaternion is one float4 (LDG.128) per thread; positions and scales have a
-// 12-byte stride and are read as coalesced scalars by default (load_raw) -- load_raw_staged brings them in through
-// shared memory with LDG.128 instead and is kept as the alternative (see preprocess.cu).
+// 12-byte stride and are read as coalesced scalars: staging them through shared memory for LDG.128 would cost a
+// barrier for 24 of the 284 bytes of a splat.
 struct RawAttr {
   float x[3], q[4], s[3], o;
 };
@@ -160,7 +160,7 @@ __device__ __forceinline__ void load_quat(const float* __restrict__ rot, size_t 
     q[0] = rot[4 * i]; q[1] = rot[4 * i + 1]; q[2] = rot[4 * i + 2]; q[3] = rot[4 * i + 3];
   }
 }
-// straight from global memory (kernels that do not stage: export, backward)
+// straight from global memory
 __device__ __forceinline__ void load_raw(const gab200_forward_args& a, int i, RawAttr& r) {
 #pragma unroll
   for (int k = 0; k < 3; k++) r.x[k] = a.means3D[3 * (size_t)i + k];
@@ -170,25 +170,6 @@ __device__ __forceinline__ void load_raw(const gab200_forward_args& a, int i, Ra
     for (int k = 0; k < 3; k++) r.s[k] = a.scales[3 * (size_t)i + k];
   }
   r.o = a.opacities[i];
-}
-// positions and scales of the block's NT splats -> shared memory (two [NT][3] tiles), then this thread's RawAttr
-template <int NT>
-__device__ __forceinline__ void load_raw_staged(const gab200_forward_args& a, int i, float* smem_xyz, float* smem_scale,
-                                                RawAttr& r) {
-  const int row0 = blockIdx.x * NT, rows = min(NT, a.P - row0);
-  stage_rows_in<NT>(smem_xyz, a.means3D, (size_t)row0, rows, 3, 3);
-  if (a.scales != nullptr) stage_rows_in<NT>(smem_scale, a.scales, (size_t)row0, rows, 3, 3);
-  __syncthreads();
-  if (i < a.P) {
-#pragma unroll
-    for (int k = 0; k < 3; k++) r.x[k] = smem_xyz[3 * threadIdx.x + k];
-    if (a.scales != nullptr) {
-#pragma unroll
-      for (int k = 0; k < 3; k++) r.s[k] = smem_scale[3 * threadIdx.x + k];
-    }
-    if (a.rotations != nullptr) load_quat(a.rotations, (size_t)i, r.q);
-    r.o = a.opacities[i];
-  }
 }
 
 __device__ __forceinline__ void bind_activate(const gab200_forward_args& a, int i, const RawAttr& raw, Activated& o,

@@ -458,13 +458,6 @@ enum {
   GAB200_TUNE_HEAVY_FWD = 0,   /* forward blend: a tile is "heavy" (1 px/thread, 8 warps) from this list length (default 32) */
   GAB200_TUNE_HEAVY_BWD = 1,   /* backward blend: a tile is "heavy" (K = 2, 4 warps) from this list length (default 2048) */
   GAB200_TUNE_DEPTH_SORT = 2,  /* 0 (default): bucket sort when a depth hint is given; 1: always cub radix sort */
-  GAB200_TUNE_BWD_VARIANT = 3, /* backward blend schedule (same arithmetic, same results up to summation order):
-                                  0 tile = CTA group, live-band-set specialised bodies; 1 warp-independent tasks,
-                                  straight-line bands, pipelined reduction; 2 / 3 as 1 with dead bands skipped by
-                                  uniform branches always / unless all bands are live; 4 (default), 5 = 3, 2 compiled for
-                                  5 CTAs per SM; 6 = 1 with specialised bodies; 7 = 2 for 6 CTAs per SM; 8 = 3 with the
-                                  two bands of a pair held in float2 registers; 9 = 8 for 5 CTAs per SM.  On an H100
-                                  (profiles/h100/bwd_variants.jsonl) 4 is the fastest and 8 the slowest of 2..9 */
   GAB200_TUNE_TILE_SORT = 4,   /* per-instance sort by tile: 0 (default) cub::DeviceRadixSort::SortPairs over the instances
                                   (5 launches + tile-range detection); 1 counting sort by tile + per-tile rank sort
                                   (csrc/tile_sort.cu: 3 launches, no memsets).  Identical sorted streams; the counting form
