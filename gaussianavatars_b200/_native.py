@@ -136,6 +136,36 @@ class RegularizeArgs(C.Structure):
     ]
 
 
+FLAME_J, FLAME_POSE_BASIS, FLAME_MAX_EXPR, FLAME_FRAME_FLOATS = 5, 36, 100, 128
+
+
+class FlameAssets(C.Structure):
+    """Mirror of gab200_flame_assets."""
+    _fields_ = [
+        ("abi_version", C.c_uint32), ("V", C.c_int32), ("n_shape", C.c_int32), ("n_expr", C.c_int32), ("J", C.c_int32),
+        ("parents", C.c_int32 * FLAME_J),
+        ("v_template", C.c_void_p), ("shapedirs", C.c_void_p), ("posedirs", C.c_void_p), ("J_regressor", C.c_void_p),
+        ("lbs_weights", C.c_void_p),
+    ]
+
+
+class FlameFrameArgs(C.Structure):
+    """Mirror of gab200_flame_frame_args."""
+    _fields_ = [
+        ("abi_version", C.c_uint32), ("T", C.c_int32), ("assets", C.POINTER(FlameAssets)), ("scratch", C.c_void_p),
+        ("timestep", C.c_void_p), ("expr", C.c_void_p), ("rotation", C.c_void_p), ("neck_pose", C.c_void_p),
+        ("jaw_pose", C.c_void_p), ("eyes_pose", C.c_void_p), ("translation", C.c_void_p), ("frame", C.c_void_p),
+    ]
+
+
+class FlameGrads(C.Structure):
+    """Mirror of gab200_flame_grads."""
+    _fields_ = [
+        ("expr", C.c_void_p), ("rotation", C.c_void_p), ("neck_pose", C.c_void_p), ("jaw_pose", C.c_void_p),
+        ("eyes_pose", C.c_void_p), ("translation", C.c_void_p),
+    ]
+
+
 ADAM_MAX_SEGMENTS = 8
 PHOTOMETRIC_SCRATCH_HEAD = 4
 
@@ -145,7 +175,8 @@ EXPORTED_SYMBOLS = ("gab200_forward", "gab200_backward", "gab200_mark_visible", 
                     "gab200_face_frame_backward", "gab200_host_times", "gab200_l1_loss_u8", "gab200_l1_loss_u8_backward",
                     "gab200_photometric_loss", "gab200_adam_step", "gab200_tune", "gab200_counters_ok",
                     "gab200_regularize_forward", "gab200_regularize_backward", "gab200_nvls_allreduce", "gab200_densify_scratch_bytes", "gab200_densify_plan", "gab200_densify_apply",
-                    "gab200_adam_step_device", "gab200_densify_stats")
+                    "gab200_adam_step_device", "gab200_densify_stats", "gab200_flame_scratch_bytes",
+                    "gab200_flame_prepare", "gab200_flame_forward", "gab200_flame_backward")
 
 _lib = None
 _lock = threading.Lock()
@@ -217,6 +248,15 @@ def lib():
                                               C.c_double, C.c_void_p, C.c_void_p]
         L.gab200_densify_stats.restype = C.c_int32
         L.gab200_densify_stats.argtypes = [C.c_int32] + [C.c_void_p] * 7
+        L.gab200_flame_scratch_bytes.restype = C.c_size_t
+        L.gab200_flame_scratch_bytes.argtypes = [C.c_int32, C.c_int32]
+        L.gab200_flame_prepare.restype = C.c_int32
+        L.gab200_flame_prepare.argtypes = [C.POINTER(FlameAssets), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gab200_flame_forward.restype = C.c_int32
+        L.gab200_flame_forward.argtypes = [C.POINTER(FlameFrameArgs), C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gab200_flame_backward.restype = C.c_int32
+        L.gab200_flame_backward.argtypes = [C.POINTER(FlameFrameArgs), C.c_void_p, C.c_void_p, C.POINTER(FlameGrads),
+                                            C.c_void_p]
         L.gab200_host_times.restype = None
         L.gab200_host_times.argtypes = [C.POINTER(C.c_double), C.c_int32]
         L.gab200_face_frame_forward.restype = C.c_int32

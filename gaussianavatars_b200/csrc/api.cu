@@ -878,6 +878,51 @@ int32_t gab200_densify_stats(int32_t P, const float* viewspace_grad, const int32
   return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
 }
 
+size_t gab200_flame_scratch_bytes(int32_t V, int32_t n_expr) {
+  return flame_scratch_bytes(V < 0 ? 0 : V, n_expr < 0 ? 0 : n_expr);
+}
+
+static bool flame_assets_ok(const gab200_flame_assets* a) {
+  if (a == nullptr || a->abi_version != GAB200_ABI_VERSION || a->V <= 0 || a->n_shape < 0 || a->n_expr < 0 ||
+      a->n_expr > GAB200_FLAME_MAX_EXPR || a->J != GAB200_FLAME_J || a->parents[0] != -1)
+    return false;
+  for (int i = 1; i < GAB200_FLAME_J; i++)
+    if (a->parents[i] < 0 || a->parents[i] >= i) return false;
+  return a->v_template && a->shapedirs && a->posedirs && a->J_regressor && a->lbs_weights;
+}
+
+static bool flame_frame_ok(const gab200_flame_frame_args* g) {
+  return g != nullptr && g->abi_version == GAB200_ABI_VERSION && flame_assets_ok(g->assets) && g->T > 0 &&
+         g->scratch && g->timestep && g->expr && g->rotation && g->neck_pose && g->jaw_pose && g->eyes_pose &&
+         g->translation && g->frame && ((uintptr_t)g->scratch & 255) == 0;
+}
+
+int32_t gab200_flame_prepare(const gab200_flame_assets* a, const float* shape, const float* static_offset,
+                             void* scratch, void* stream_) {
+  if (!flame_assets_ok(a) || scratch == nullptr || ((uintptr_t)scratch & 255) != 0 || (a->n_shape > 0 && !shape))
+    return GAB200_ERR_INVALID_ARGUMENT;
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  launch_flame_prepare(*a, shape, static_offset, scratch, (cudaStream_t)stream_);
+  return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
+int32_t gab200_flame_forward(const gab200_flame_frame_args* g, float* verts, float* verts_cano, void* stream_) {
+  if (!flame_frame_ok(g) || verts == nullptr) return GAB200_ERR_INVALID_ARGUMENT;
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  launch_flame_forward(*g, verts, verts_cano, (cudaStream_t)stream_);
+  return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
+int32_t gab200_flame_backward(const gab200_flame_frame_args* g, const float* dL_dverts, const float* dL_dverts_cano,
+                              const gab200_flame_grads* o, void* stream_) {
+  if (!flame_frame_ok(g) || dL_dverts == nullptr || o == nullptr || !o->expr || !o->rotation || !o->neck_pose ||
+      !o->jaw_pose || !o->eyes_pose || !o->translation)
+    return GAB200_ERR_INVALID_ARGUMENT;
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  launch_flame_backward(*g, dL_dverts, dL_dverts_cano, *o, (cudaStream_t)stream_);
+  return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
 int32_t gab200_export_binning(const gab200_forward_args* a, const gab200_frame_state* st, uint64_t* keys,
                               uint32_t* values, uint32_t* ranges, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;

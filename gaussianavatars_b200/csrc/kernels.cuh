@@ -185,6 +185,14 @@ cudaError_t launch_regularize_backward(const gab200_regularize_args& a, const fl
 // nvls.cu
 void launch_nvls_allreduce(float* mc, int64_t n, int rank, int world, cudaStream_t stream);
 
+// flame.cu
+size_t flame_scratch_bytes(int V, int n_expr);
+void launch_flame_prepare(const gab200_flame_assets& a, const float* shape, const float* static_offset, void* scratch,
+                          cudaStream_t stream);
+void launch_flame_forward(const gab200_flame_frame_args& g, float* verts, float* verts_cano, cudaStream_t stream);
+void launch_flame_backward(const gab200_flame_frame_args& g, const float* g_verts, const float* g_cano,
+                           const gab200_flame_grads& grads, cudaStream_t stream);
+
 // optim.cu
 void launch_adam(int num_segments, const gab200_adam_segment* segs, int64_t step, double beta1, double beta2, double eps,
                  cudaStream_t stream);

@@ -24,6 +24,12 @@ reference (train.py:106-210): after backward the graph also accumulates the dens
 Both are skipped on the device when the replay overflowed its capacity: such a replay changes no parameter, moment,
 step or statistic.  densify_and_prune / reset_opacity / oneupSHdegree stay eager calls between replays; `run()` notices
 the tensors or sizes they replaced and re-captures.
+
+When the model carries a FLAME head (`pc.flame`, a flame.FlameLBS, and `pc.flame_param`), the captured frame starts
+from the pose of the reference (select_mesh_by_timestep, scene/flame_gaussian_model.py:117-135) instead of given
+vertices: `set_inputs(timestep=t)` writes t into a device int32 that the replay reads, so changing the timestep never
+re-captures.  The gradients reach the FLAME tensors, and a capturable `Adam` holding their groups
+(flame.flame_param_groups) steps them in the same replay.
 """
 from __future__ import annotations
 
@@ -36,8 +42,10 @@ from .renderer import render
 from .rasterizer import l1_loss_u8
 from .densify import add_densification_stats
 from .training import Adam, binding_regularizers, photometric_loss
+from .flame import flame_pose
 
 _STATS = ("xyz_gradient_accum", "denom", "max_radii2D")
+_FLAME_KEYS = ("shape", "static_offset", "expr", "rotation", "neck_pose", "jaw_pose", "eyes_pose", "translation")
 
 
 class _Pipe:
@@ -155,7 +163,14 @@ class GraphedFrame:
         self.bg = bg.to(dev).float().contiguous()
         self.cam = torch.zeros(35, dtype=torch.float32, device=dev)
         self.camera = _GraphCamera(self.W, self.H, self.fovx, self.fovy, self.cam)
-        self.verts = pc.verts_rest.detach().clone().contiguous().requires_grad_(True)
+        self.flame = getattr(pc, "flame", None)
+        if self.flame is not None:   # the pose is computed inside the graph from this timestep
+            self.verts = None
+            self.timestep = torch.zeros(1, dtype=torch.int32, device=dev)
+            self.num_timesteps = int(pc.flame_param["expr"].shape[0])
+        else:
+            self.verts = pc.verts_rest.detach().clone().contiguous().requires_grad_(True)
+            self.timestep = None
         self.gt = torch.zeros((3, self.H, self.W), dtype=torch.uint8, device=dev) if loss != "dL_dimage" else None
         self.dL_dimage = torch.zeros((3, self.H, self.W), dtype=torch.float32, device=dev) if loss == "dL_dimage" else None
         self.cam_host = torch.zeros(35, dtype=torch.float32).pin_memory() if host_inputs else None  # staging
@@ -177,8 +192,18 @@ class GraphedFrame:
         self._warm = list(warm_cameras) if warm_cameras is not None else None
 
     # ---- inputs ------------------------------------------------------------------------------------------------
-    def set_inputs(self, camera=None, verts=None, gt_u8=None, dL_dimage=None):
-        """Copies new inputs into the static buffers (device tensors) / staging buffers (host_inputs)."""
+    def set_inputs(self, camera=None, verts=None, gt_u8=None, dL_dimage=None, timestep=None):
+        """Copies new inputs into the static buffers (device tensors) / staging buffers (host_inputs).  `timestep`
+        (a model with a FLAME head only) is a host int checked against the model's number of timesteps."""
+        if verts is not None and self.flame is not None:
+            raise ValueError("this frame poses its FLAME head itself: give set_inputs(timestep=...), not verts")
+        if timestep is not None:
+            if self.flame is None:
+                raise ValueError("timestep= needs a model with a FLAME head (pc.flame)")
+            t = int(timestep)
+            if not 0 <= t < self.num_timesteps:
+                raise IndexError(f"timestep {t} outside [0, {self.num_timesteps})")
+            self.timestep.fill_(t)
         if camera is not None:
             blk = camera if isinstance(camera, torch.Tensor) else camera_block(camera)
             if blk.device.type == "cpu" and self._uploads:
@@ -225,14 +250,19 @@ class GraphedFrame:
 
     # ---- the step body (run eagerly for warm-up, then captured) --------------------------------------------------
     def _params(self):
-        return list(self.pc.parameters())
+        """The tensors whose gradients the graph produces: the splat parameters, then the trained FLAME tensors."""
+        ps = list(self.pc.parameters())
+        if self.flame is not None:
+            ps += [self.pc.flame_param[k] for k in _FLAME_KEYS[2:] if self.pc.flame_param[k].requires_grad]
+        return ps
 
     def _body(self, train: bool = False):
         """One frame; with `train` (the captured step only) also the statistics and the optimizer step."""
         pc = self.pc
         for p in self._params():
             p.grad = None
-        self.verts.grad = None
+        if self.verts is not None:
+            self.verts.grad = None
         other = self._prefetch_target
         forked = other is not None or self.side_work is not None
         if forked:   # forked branch: runs while this frame computes
@@ -245,7 +275,11 @@ class GraphedFrame:
                         other.gt.copy_(other.gt_stage, non_blocking=True)
                 if self.side_work is not None and self.side_work_at == "start":
                     self.side_work()
-        pc.update_mesh_properties(self.verts)
+        if self.flame is not None:
+            verts, pc.verts_cano = flame_pose(self.flame, pc.flame_param, self.timestep)
+            pc.update_mesh_properties(verts[0])
+        else:
+            pc.update_mesh_properties(self.verts)
         out = render(self.camera, pc, _Pipe, self.bg)
         img = out["render"]
         if self.loss_kind in ("l1_u8", "photometric"):
@@ -313,6 +347,8 @@ class GraphedFrame:
         torch.cuda.synchronize(self.device)
         # release what the eager frames left on the model / on this object (tensors with autograd history)
         self.pc.face_center = self.pc.face_orien_mat = self.pc.face_scaling = None
+        if self.flame is not None:
+            self.pc.verts_cano = None
         self.image = self.radii = self.viewspace_points = self.loss = None
         return n_max, ((lo, hi) if hi > lo else (0, 0))
 
@@ -324,6 +360,11 @@ class GraphedFrame:
         key += [p.data_ptr() for p in self._params()]
         if self.densify_stats:
             key += [getattr(pc, n).data_ptr() for n in _STATS]
+        if self.flame is not None:   # the timestep is read on the device and is not part of the key
+            for k in _FLAME_KEYS:
+                t = pc.flame_param.get(k)
+                key.append(None if t is None else (t.data_ptr(), tuple(t.shape), bool(t.requires_grad)) +
+                           ((t._version,) if k in ("shape", "static_offset") else ()))
         opt = self.optimizer
         if opt is not None:
             for g in opt.param_groups:
@@ -357,7 +398,7 @@ class GraphedFrame:
         # GraphedFrame of the same model re-points .grad at its own when it captures
         self.grads = [p.grad for p in self._params()]
         self.flat_grad = getattr(self.pc, "flat_grad", None)
-        self._key = self._state_key() if training else None
+        self._key = self._state_key() if (training or self.flame is not None) else None
         self.captures += 1
         return self
 

@@ -8,7 +8,8 @@ scene/flame_gaussian_model.py:117-154).  The licensed FLAME assets are absent (S
                      reference route; the fused route never calls them)
 
 It is what bench.py and the tests feed to `render()`; a real FlameGaussianModel exposes the same names, so the
-renderer treats both alike.
+renderer treats both alike.  With `flame=` (a flame.FlameLBS) and `flame_param=` (the reference's per-timestep dict)
+`select_mesh_by_timestep` poses the mesh on the device as the reference does and keeps `verts_cano`.
 """
 from __future__ import annotations
 
@@ -73,12 +74,17 @@ def quat_mul_wxyz(p: torch.Tensor, q: torch.Tensor) -> torch.Tensor:
 class MeshBoundGaussians:
     def __init__(self, params: Dict[str, torch.Tensor], sh_degree: int, verts: Optional[torch.Tensor] = None,
                  faces: Optional[torch.Tensor] = None, pose_fn: Optional[Callable] = None, device="cuda",
-                 requires_grad: bool = False):
+                 requires_grad: bool = False, flame=None, flame_param: Optional[Dict[str, torch.Tensor]] = None):
         self.max_sh_degree = sh_degree
         self.active_sh_degree = sh_degree
         for k in ("_xyz", "_rotation", "_scaling", "_opacity", "_features_dc", "_features_rest"):
             t = params[k].to(device).contiguous()
             setattr(self, k, t.requires_grad_(requires_grad))
+        if (flame is None) != (flame_param is None):
+            raise ValueError("flame= and flame_param= go together")
+        self.flame, self.flame_param = flame, flame_param
+        if flame is not None and faces is None:
+            faces = flame.faces
         b = params.get("binding")
         self.binding = None if b is None else b.to(device=device, dtype=torch.int32).contiguous()
         self.verts_rest = None if verts is None else verts.to(device)
@@ -87,6 +93,7 @@ class MeshBoundGaussians:
         self.faces_i32 = None if faces is None else self.faces.to(torch.int32).contiguous()
         self.face_center = self.face_orien_mat = self.face_scaling = self._face_orien_quat = None
         self.verts = None
+        self.verts_cano = None
         self.timestep = None
 
     # ---- mesh ----
@@ -114,6 +121,12 @@ class MeshBoundGaussians:
 
     def select_mesh_by_timestep(self, timestep: int):
         self.timestep = timestep
+        if self.flame is not None:
+            from .flame import flame_pose
+
+            verts, self.verts_cano = flame_pose(self.flame, self.flame_param, timestep)
+            self.update_mesh_properties(verts[0])
+            return
         v = self.verts_rest if self.pose_fn is None else self.pose_fn(self.verts_rest, timestep)
         self.update_mesh_properties(v)
 

@@ -159,6 +159,67 @@ def pose_mesh(verts: torch.Tensor, timestep: int):
     return v
 
 
+FLAME_JOINT_CENTRES = np.array([[0.0, -0.12, -0.02], [0.0, -0.10, 0.0], [0.0, -0.06, 0.05], [0.035, 0.03, 0.09],
+                                [-0.035, 0.03, 0.09]], np.float64)   # root, neck, jaw, eyes
+
+
+def _smooth_fields(x: np.ndarray, n: int, rng, scale: float, n_waves: int = 12) -> np.ndarray:
+    """n smooth displacement fields over the points x (V,3): random mixtures of low-frequency plane waves.
+    Returns (V, 3, n)."""
+    omega = rng.normal(0, 12.0, size=(n_waves, 3))
+    phase = rng.uniform(0, 2 * np.pi, size=n_waves)
+    phi = np.sin(x @ omega.T + phase)                                  # (V, n_waves)
+    coef = rng.normal(0, scale / np.sqrt(n_waves / 2), size=(n_waves, 3 * n))
+    return (phi @ coef).reshape(x.shape[0], 3, n)
+
+
+def flame_like_assets(seed: int = 0, n_shape: int = 300, n_expr: int = 100) -> Dict[str, torch.Tensor]:
+    """FLAME-shaped assets on `head_mesh()` (the licensed model is not available): smooth shape / expression fields
+    scaled so that parameters of the demo's magnitudes (|shape| < 1, |expr| < 3) move the mesh by millimetres to
+    centimetres, small pose correctives, a J_regressor of local averages around a root, neck, jaw and two eyes, and
+    partition-of-unity skinning weights.  Buffer layouts of the reference FlameHead: v_template (V,3), shapedirs
+    (V,3,n_shape+n_expr), posedirs (36,3V), J_regressor (5,V), parents [-1,0,1,1,1], lbs_weights (V,5), faces (F,3)."""
+    rng = np.random.default_rng(seed)
+    verts, faces = head_mesh()
+    x = verts.numpy().astype(np.float64)
+    V = x.shape[0]
+    shapedirs = np.concatenate([_smooth_fields(x, n_shape, rng, 1e-3), _smooth_fields(x, n_expr, rng, 1.5e-3)], axis=2)
+    posedirs = _smooth_fields(x, 36, rng, 2e-3).transpose(2, 0, 1).reshape(36, 3 * V)
+    d2 = ((x[None, :, :] - FLAME_JOINT_CENTRES[:, None, :]) ** 2).sum(-1)   # (5, V)
+    J_regressor = np.exp(-d2 / (2 * 0.03 ** 2))
+    J_regressor /= J_regressor.sum(1, keepdims=True)
+    logits = -d2.T / (2 * 0.05 ** 2)
+    w = np.exp(logits - logits.max(1, keepdims=True))
+    lbs_weights = w / w.sum(1, keepdims=True)
+    f32 = lambda a: torch.tensor(np.ascontiguousarray(a), dtype=torch.float32)   # noqa: E731
+    return dict(v_template=verts.clone(), shapedirs=f32(shapedirs), posedirs=f32(posedirs), J_regressor=f32(J_regressor),
+                parents=torch.tensor([-1, 0, 1, 1, 1], dtype=torch.long), lbs_weights=f32(lbs_weights), faces=faces,
+                n_shape=n_shape, n_expr=n_expr)
+
+
+def flame_like_sequence(T: int, seed: int = 0, V: Optional[int] = None, n_shape: int = 300,
+                        n_expr: int = 100) -> Dict[str, torch.Tensor]:
+    """A reference-style `flame_param` dict (scene/flame_gaussian_model.py:61-71) with smooth per-timestep tracks of
+    the demo's magnitudes: expression (T,n_expr), rotation / neck / jaw (T,3), eyes (T,6), translation (T,3); a
+    fixed shape (n_shape,) and static offset (1,V,3); dynamic offsets (T,V,3) of zeros (unused by FLAME's forward)."""
+    rng = np.random.default_rng(seed)
+    V = V if V is not None else head_mesh()[0].shape[0]
+    ts = np.arange(T, dtype=np.float64)[:, None]
+
+    def track(n, amp):
+        f = rng.uniform(0.05, 0.4, size=(1, n))
+        p = rng.uniform(0, 2 * np.pi, size=(1, n))
+        return amp * np.sin(f * ts + p) * rng.uniform(0.3, 1.0, size=(1, n))
+
+    f32 = lambda a: torch.tensor(np.ascontiguousarray(a), dtype=torch.float32)   # noqa: E731
+    jaw = track(3, 0.03)
+    jaw[:, 0] = 0.12 * (1 + np.sin(0.3 * ts[:, 0])) / 2
+    return dict(shape=f32(rng.normal(0, 0.3, size=n_shape)), expr=f32(track(n_expr, 1.2)),
+                rotation=f32(track(3, 0.15)), neck_pose=f32(track(3, 0.05)), jaw_pose=f32(jaw),
+                eyes_pose=f32(track(6, 0.06)), translation=f32(track(3, 0.008)),
+                static_offset=f32(rng.normal(0, 5e-4, size=(1, V, 3))), dynamic_offset=torch.zeros(T, V, 3))
+
+
 SIZE0, SIZE_SIG = 0.19, 0.85
 
 

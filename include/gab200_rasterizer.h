@@ -426,6 +426,89 @@ int32_t gab200_densify_stats(int32_t P, const float* viewspace_grad, const int32
 int32_t gab200_densify_plan(const gab200_densify_args* args, void* stream);
 int32_t gab200_densify_apply(const gab200_densify_args* args, const gab200_densify_out* out, void* stream);
 
+/* FLAME head posing: blendshapes and linear blend skinning, forward and backward, for one timestep read from device
+ * memory.  Replaces FlameHead.forward + lbs (flame_model/flame.py:485-558, flame_model/lbs.py:25-304) as
+ * select_mesh_by_timestep calls it (scene/flame_gaussian_model.py:117-135): zero_centered_at_root_node = False,
+ * no landmarks, translation added after skinning, full_pose = [rotation, neck, jaw, eyes (6)],
+ * pose feature = (R_1..R_4 - I) flattened row-major, Rodrigues as lbs.py writes it (angle = |r + 1e-8|, exactly I at
+ * r = 0 with a finite gradient).  The reference's dynamic_offset argument is accepted there and never used, so it has
+ * no counterpart here.
+ *
+ * Only FLAME's kinematic layout is accepted: J = 5 joints (root, neck, jaw, two eyes), parents[0] = -1,
+ * 0 <= parents[i] < i, 36 = 9 (J - 1) pose-basis rows; 0 <= n_shape, 0 <= n_expr <= GAB200_FLAME_MAX_EXPR.
+ * Anything else is GAB200_ERR_INVALID_ARGUMENT.  All device arrays are float32 in the reference FlameHead buffer
+ * layouts:
+ *   v_template [V,3], shapedirs [V,3,n_shape+n_expr], posedirs [36,3V] (flame.py:117-119), J_regressor [J,V],
+ *   lbs_weights [V,J]. */
+#define GAB200_FLAME_J 5
+#define GAB200_FLAME_POSE_BASIS 36
+#define GAB200_FLAME_MAX_EXPR 100
+#define GAB200_FLAME_FRAME_FLOATS 128 /* per-call state: A [5,3,4] | pose feature [36] | posed joints [5,3] | pad */
+typedef struct gab200_flame_assets {
+  uint32_t abi_version;
+  int32_t V, n_shape, n_expr, J;
+  int32_t parents[GAB200_FLAME_J]; /* HOST ints */
+  const float* v_template;
+  const float* shapedirs;
+  const float* posedirs;
+  const float* J_regressor;
+  const float* lbs_weights;
+} gab200_flame_assets;
+
+/* Device scratch owned by the caller (256-byte aligned) holding what gab200_flame_prepare derives from the shape
+ * and the static offset, plus the backward's per-CTA partial sums.  One scratch serves one stream at a time. */
+size_t gab200_flame_scratch_bytes(int32_t V, int32_t n_expr);
+
+/* Run once per change of `shape` [n_shape] or `static_offset` [V,3] (NULL = zero), which the reference never trains
+ * (their optimizer groups are commented out, scene/flame_gaussian_model.py:180-183,209-217).  Writes into scratch:
+ *   v_base = v_template + shapedirs[..., :n_shape] . shape + static_offset     [V,3]
+ *   J_base = J_regressor . v_base                                              [5,3]
+ *   JS     = J_regressor . shapedirs[..., n_shape:]                            [5,3,n_expr]
+ *   the expression basis re-laid out component-major [n_expr,3V] for coalesced per-frame reads.
+ * This regroups the reference's sums (one einsum over all n_shape + n_expr components, then the joints regressed from
+ * the float32 v_shaped): results agree with it to rounding, not bit for bit. */
+int32_t gab200_flame_prepare(const gab200_flame_assets* assets, const float* shape, const float* static_offset,
+                             void* scratch, void* stream);
+
+/* One timestep of the reference's flame_param dict: the (T,.) tensors and the row index t in DEVICE memory, so that
+ * a captured CUDA graph poses whichever timestep the caller wrote before the replay.  A t outside [0, T) leaves the
+ * outputs unspecified but is memory-safe: every kernel returns without reading a parameter row or writing. */
+typedef struct gab200_flame_frame_args {
+  uint32_t abi_version;
+  int32_t T;
+  const gab200_flame_assets* assets;
+  const void* scratch;        /* prepared by gab200_flame_prepare for this shape / static offset */
+  const int32_t* timestep;    /* DEVICE int32 */
+  const float* expr;          /* [T, n_expr] */
+  const float* rotation;      /* [T, 3] */
+  const float* neck_pose;     /* [T, 3] */
+  const float* jaw_pose;      /* [T, 3] */
+  const float* eyes_pose;     /* [T, 6] */
+  const float* translation;   /* [T, 3] */
+  float* frame;               /* [GAB200_FLAME_FRAME_FLOATS] device: written by the forward, read by its backward */
+} gab200_flame_frame_args;
+
+/* Two launches, no host read: flame_joints_kernel (one CTA: joints, Rodrigues, rigid chain, pose feature) and
+ * flame_skin_kernel (blendshapes, pose correctives, skinning).  verts [V,3]; verts_cano [V,3] (the reference's
+ * v_shaped, returned for the laplacian term) or NULL. */
+int32_t gab200_flame_forward(const gab200_flame_frame_args* args, float* verts, float* verts_cano, void* stream);
+
+/* Gradients of the six (T,.) tensors, written in FULL: row t, and exact zeros in every other row (what autograd of the
+ * reference's [[timestep]] indexing produces).  dL_dverts [V,3]; dL_dverts_cano [V,3] or NULL (= 0).  Two launches
+ * (flame_skin_backward_kernel: per-CTA partial sums; flame_joints_backward_kernel: one CTA sums them in a fixed order
+ * and backpropagates through the chain and Rodrigues), no floating-point atomics: the same dL_dverts gives
+ * bit-identical gradients on every call. */
+typedef struct gab200_flame_grads {
+  float* expr;          /* [T, n_expr] */
+  float* rotation;      /* [T, 3] */
+  float* neck_pose;     /* [T, 3] */
+  float* jaw_pose;      /* [T, 3] */
+  float* eyes_pose;     /* [T, 6] */
+  float* translation;   /* [T, 3] */
+} gab200_flame_grads;
+int32_t gab200_flame_backward(const gab200_flame_frame_args* args, const float* dL_dverts, const float* dL_dverts_cano,
+                              const gab200_flame_grads* grads, void* stream);
+
 /* Debug/parity access to a finished forward: copies the sorted (key,value) stream and tile ranges to caller
  * DEVICE buffers: keys [N] u64, values [N] u32, ranges [tiles,2] u32. Any may be NULL. */
 int32_t gab200_export_binning(const gab200_forward_args* args, const gab200_frame_state* state, uint64_t* keys,

@@ -6,6 +6,13 @@ training iteration per step (train.py:106-210) -- xyz learning-rate schedule, po
               and with it a host wait per line), the learning rate written on the host, host-stepped Adam
   graph       GraphedFrame for frame -> backward, then the same eager statistics, host lr and host-stepped Adam
   graph_full  ONE replay of GraphedFrame(optimizer=capturable Adam with the xyz schedule, densify_stats=True)
+With a FLAME head (synthetic.flame_like_assets on the same mesh, 16 timesteps, the reference's FLAME optimizer groups
+trained as with not_finetune_flame_params=False):
+  eager_flame       the eager arm with the pose of select_mesh_by_timestep from the float32 reference-order
+                    restatement (tests/flame_oracle.py) + autograd, and torch's Adam on the FLAME groups
+  graph_full_flame  ONE replay of GraphedFrame on the FLAME model: pose, frame, statistics and Adam over the splat and
+                    FLAME groups
+graph_full stays beside them as the no-FLAME lower bound.
 One JSON line per resolution, with the GPU it ran on and its power limit.
 
     python scripts/train_step_graph.py            (ITERS=256 timed steps after 8 warm-up steps; P=150000)
@@ -19,6 +26,7 @@ from gaussianavatars_b200 import synthetic as syn
 from gaussianavatars_b200.graph import GraphedFrame, camera_block
 from gaussianavatars_b200.model import MeshBoundGaussians
 from gaussianavatars_b200.renderer import render
+from tests import flame_oracle as fo
 
 dev = torch.device("cuda:0")
 class Pipe: debug = False; compute_cov3D_python = False; convert_SHs_python = False
@@ -29,6 +37,9 @@ bg = torch.ones(3, device=dev)
 NAMES = ("xyz", "rotation", "scaling", "opacity", "f_dc", "f_rest")   # pc.parameters() order
 LRS = dict(xyz=0.0, rotation=1e-3, scaling=5e-3, opacity=5e-2, f_dc=2.5e-3, f_rest=1.25e-4)
 SCHED = g.expon_lr_schedule(lr_init=5e-3, lr_final=5e-5, lr_delay_mult=0.01, max_steps=600_000)   # OptimizationParams
+FLAME_ASSETS = syn.flame_like_assets(0)
+FLAME_SEQ = syn.flame_like_sequence(16, seed=1, V=FLAME_ASSETS["v_template"].shape[0])
+FLAME_SEQ.pop("dynamic_offset")
 
 
 def xyz_lr(it):
@@ -65,17 +76,46 @@ for (W, H) in ((550, 802), (1920, 1080)):
     cams = [syn.orbit_camera(W, H, azimuth_deg=-60 + 120 * (i + .5) / 16, elevation_deg=5 * math.sin(i)) for i in range(16)]
     gts = [torch.randint(0, 256, (3, H, W), dtype=torch.uint8, device=dev) for _ in range(2)]
     res = {"config": "3", "splats": P, "W": W, "H": H, "timed_steps": K, "gpu": name, "power_limit": power}
-    for arm in ("eager", "graph", "graph_full"):
-        pc = MeshBoundGaussians(params, 3, verts, faces, pose_fn=syn.pose_mesh, device=dev, requires_grad=True)
+    for arm in ("eager", "graph", "graph_full", "eager_flame", "graph_full_flame"):
+        flame = arm.endswith("_flame")
+        if flame:
+            a = FLAME_ASSETS
+            lbs = g.FlameLBS.from_arrays(a["v_template"], a["shapedirs"], a["posedirs"], a["J_regressor"], a["parents"],
+                                         a["lbs_weights"], a["faces"], a["n_shape"], a["n_expr"], device=dev)
+            fparam = {k: v.to(dev).clone().contiguous() for k, v in FLAME_SEQ.items()}
+            pc = MeshBoundGaussians(params, 3, None, None, device=dev, requires_grad=True, flame=lbs, flame_param=fparam)
+        else:
+            pc = MeshBoundGaussians(params, 3, verts, faces, pose_fn=syn.pose_mesh, device=dev, requires_grad=True)
         pc.xyz_gradient_accum = torch.zeros((P, 1), device=dev)
         pc.denom = torch.zeros((P, 1), device=dev)
         pc.max_radii2D = torch.zeros((P,), device=dev)
         groups = [{"params": [p], "lr": LRS[n], "name": n} for n, p in zip(NAMES, pc.parameters())]
-        if arm == "graph_full":
+        if arm.startswith("graph_full"):
             groups[0]["lr_schedule"] = SCHED
-        opt = g.Adam(groups, lr=0.0, eps=1e-15, capturable=arm == "graph_full")
-        posed = [syn.pose_mesh(pc.verts_rest, i).contiguous() for i in range(16)]
-        if arm == "eager":
+        if arm == "graph_full_flame":
+            groups += g.flame_param_groups(pc.flame_param)
+        opt = g.Adam(groups, lr=0.0, eps=1e-15, capturable=arm.startswith("graph_full"))
+        posed = None if flame else [syn.pose_mesh(pc.verts_rest, i).contiguous() for i in range(16)]
+        if arm == "eager_flame":
+            cd = [c.to(dev) for c in cams]
+            oa = fo.assets_as({k: FLAME_ASSETS[k] for k in ("v_template", "shapedirs", "posedirs", "J_regressor",
+                                                            "lbs_weights")} | {"parents": FLAME_ASSETS["parents"].tolist()},
+                              torch.float32, dev)
+            opt_f = torch.optim.Adam(g.flame_param_groups(pc.flame_param), lr=0.0, eps=1e-15)
+            def step(it):
+                opt.param_groups[0]["lr"] = xyz_lr(it)
+                opt.zero_grad(set_to_none=True)
+                opt_f.zero_grad(set_to_none=True)
+                v, pc.verts_cano, _ = fo.select_mesh_by_timestep(oa, pc.flame_param, it % 16)
+                pc.update_mesh_properties(v[0])
+                out = render(cd[it % 16], pc, Pipe, bg)
+                loss = g.photometric_loss(out["render"], gts[it % 2], 0.2)
+                lx, ls = g.binding_regularizers(pc._xyz, pc._scaling, out["radii"], pc.binding, pc.face_scaling)
+                (loss + lx + ls).backward()
+                reference_stats(pc, out["radii"], out["viewspace_points"].grad)
+                opt.step()
+                opt_f.step()
+        elif arm == "eager":
             cd = [c.to(dev) for c in cams]
             def step(it):
                 opt.param_groups[0]["lr"] = xyz_lr(it)
@@ -90,10 +130,13 @@ for (W, H) in ((550, 802), (1920, 1080)):
                 opt.step()
         else:
             blocks = [camera_block(c).to(dev) for c in cams]
-            kw = dict(optimizer=opt, densify_stats=True) if arm == "graph_full" else {}
+            kw = dict(optimizer=opt, densify_stats=True) if arm.startswith("graph_full") else {}
             fr = GraphedFrame(pc, W, H, cams[0].FoVx, cams[0].FoVy, bg, loss="photometric", lambda_dssim=0.2,
                               regularizers={}, warm_cameras=blocks, **kw)
-            fr.set_inputs(camera=blocks[0], verts=posed[0], gt_u8=gts[0])
+            if flame:
+                fr.set_inputs(camera=blocks[0], timestep=0, gt_u8=gts[0])
+            else:
+                fr.set_inputs(camera=blocks[0], verts=posed[0], gt_u8=gts[0])
             fr.capture()
             if arm == "graph":
                 def step(it):
@@ -102,12 +145,16 @@ for (W, H) in ((550, 802), (1920, 1080)):
                     fr.run()
                     reference_stats(pc, fr.radii, fr.viewspace_points.grad)
                     opt.step()
+            elif flame:
+                def step(it):
+                    fr.set_inputs(camera=blocks[it % 16], timestep=it % 16, gt_u8=gts[it % 2])
+                    fr.run()
             else:
                 def step(it):
                     fr.set_inputs(camera=blocks[it % 16], verts=posed[it % 16], gt_u8=gts[it % 2])
                     fr.run()
         res[arm + "_ms_per_step"] = round(timed(step), 4)
-        if arm != "eager":
+        if arm.startswith("graph"):
             res[arm + "_overflow"] = fr.overflowed()
             res[arm + "_captures"] = fr.captures
             res[arm + "_loss_finite"] = bool(torch.isfinite(fr.loss))
