@@ -176,7 +176,8 @@ EXPORTED_SYMBOLS = ("gab200_forward", "gab200_backward", "gab200_mark_visible", 
                     "gab200_photometric_loss", "gab200_adam_step", "gab200_tune", "gab200_counters_ok",
                     "gab200_regularize_forward", "gab200_regularize_backward", "gab200_nvls_allreduce", "gab200_densify_scratch_bytes", "gab200_densify_plan", "gab200_densify_apply",
                     "gab200_adam_step_device", "gab200_densify_stats", "gab200_flame_scratch_bytes",
-                    "gab200_flame_prepare", "gab200_flame_forward", "gab200_flame_backward")
+                    "gab200_flame_prepare", "gab200_flame_forward", "gab200_flame_backward",
+                    "gab200_forward_device_fov", "gab200_backward_device_fov")
 
 _lib = None
 _lock = threading.Lock()
@@ -209,6 +210,10 @@ def lib():
         L.gab200_forward.argtypes = [C.POINTER(ForwardArgs), C.POINTER(FrameState), C.c_void_p]
         L.gab200_backward.restype = C.c_int32
         L.gab200_backward.argtypes = [C.POINTER(BackwardArgs), C.c_void_p]
+        L.gab200_forward_device_fov.restype = C.c_int64
+        L.gab200_forward_device_fov.argtypes = [C.POINTER(ForwardArgs), C.c_void_p, C.POINTER(FrameState), C.c_void_p]
+        L.gab200_backward_device_fov.restype = C.c_int32
+        L.gab200_backward_device_fov.argtypes = [C.POINTER(BackwardArgs), C.c_void_p, C.c_void_p]
         L.gab200_mark_visible.restype = C.c_int32
         L.gab200_mark_visible.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gab200_bind_activate.restype = C.c_int32

@@ -337,6 +337,7 @@ const char* gab200_status_string(int32_t s) {
 namespace {
 struct Frame {
   const gab200_forward_args* a;
+  const float* tanfov;  // device float[2] (gab200_forward_device_fov) or NULL: a->tanfovx / tanfovy
   gab200_frame_state* st;
   cudaStream_t stream;
   GeomView g;
@@ -371,7 +372,7 @@ int enqueue_geometry(Frame& f, bool bucket, bool run_preprocess, uint32_t capaci
     if (f.counting) GAB_CUDA(cudaMemsetAsync(f.iv.tile_count, 0, sizeof(uint32_t) * (size_t)tiles, stream));
     StageScope sc(GAB200_STAGE_PREPROCESS, stream);
     launch_preprocess(*a, g.rec, g.aux, g.tiles_touched, f.nb ? g.clamped : nullptr, g.depth_keys[0], g.ids[0], g.buckets,
-                      f.counting ? f.iv.tile_count : nullptr, stream);
+                      f.counting ? f.iv.tile_count : nullptr, f.tanfov, stream);
   }
   GAB_STAGE_CHECK(f.dbg, stream);
   if (f.counting && run_preprocess) {
@@ -494,13 +495,14 @@ int wait_counters(Frame& f) {
 }
 }  // namespace
 
-int64_t gab200_forward(const gab200_forward_args* a, gab200_frame_state* st, void* stream_) {
+// gab200_forward and gab200_forward_device_fov (tanfov == NULL: the by-value tanfovx / tanfovy)
+static int64_t run_forward(const gab200_forward_args* a, const float* tanfov, gab200_frame_state* st, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   if (!validate(a) || st == nullptr) return GAB200_ERR_INVALID_ARGUMENT;
   if (check_arch() < 0) return GAB200_ERR_ARCH;
   memset(st, 0, sizeof(*st));
   Frame f;
-  f.a = a; f.st = st; f.stream = stream;
+  f.a = a; f.tanfov = tanfov; f.st = st; f.stream = stream;
   f.P = a->P; f.W = a->image_width; f.H = a->image_height;
   f.gx = (f.W + GAB_TILE - 1) / GAB_TILE; f.gy = (f.H + GAB_TILE - 1) / GAB_TILE;
   f.nb = a->need_backward != 0;
@@ -635,7 +637,17 @@ int64_t gab200_forward(const gab200_forward_args* a, gab200_frame_state* st, voi
   return N;
 }
 
-int32_t gab200_backward(const gab200_backward_args* b, void* stream_) {
+int64_t gab200_forward(const gab200_forward_args* a, gab200_frame_state* st, void* stream) {
+  return run_forward(a, nullptr, st, stream);
+}
+
+int64_t gab200_forward_device_fov(const gab200_forward_args* a, const float* tanfov, gab200_frame_state* st,
+                                  void* stream) {
+  return run_forward(a, tanfov, st, stream);
+}
+
+// gab200_backward and gab200_backward_device_fov
+static int32_t run_backward(const gab200_backward_args* b, const float* tanfov, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   if (b == nullptr || b->abi_version != GAB200_ABI_VERSION || b->fwd == nullptr || b->state == nullptr)
     return GAB200_ERR_INVALID_ARGUMENT;
@@ -687,10 +699,16 @@ int32_t gab200_backward(const gab200_backward_args* b, void* stream_) {
     const bool csr = bound && a->binding != nullptr && b->num_face_chunks > 0 && b->face_perm && b->face_chunk_face &&
                      b->face_chunk_start && b->face_chunk_end &&
                      (b->dL_dface_center || b->dL_dface_orien_mat || b->dL_dface_scaling);
-    launch_preprocess_backward(*b, g.rec, g.aux, g.clamped, g.g2d, csr ? g.face_scratch : nullptr, stream);
+    launch_preprocess_backward(*b, g.rec, g.aux, g.clamped, g.g2d, csr ? g.face_scratch : nullptr, tanfov, stream);
   }
   GAB_STAGE_CHECK(dbg, stream);
   return GAB200_OK;
+}
+
+int32_t gab200_backward(const gab200_backward_args* b, void* stream) { return run_backward(b, nullptr, stream); }
+
+int32_t gab200_backward_device_fov(const gab200_backward_args* b, const float* tanfov, void* stream) {
+  return run_backward(b, tanfov, stream);
 }
 
 int32_t gab200_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,

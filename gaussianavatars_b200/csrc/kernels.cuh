@@ -99,7 +99,7 @@ __device__ __forceinline__ uint32_t depth_bucket(uint32_t key, const DepthBucket
 // tile_count != nullptr: also count the instances of every tile (counting tile sort, tile_sort.cu)
 void launch_preprocess(const gab200_forward_args& a, SplatRec* rec, SplatAux* aux, uint32_t* tiles_touched,
                        uint8_t* clamped, uint32_t* depth_keys, uint32_t* ids, const DepthBuckets& buckets,
-                       uint32_t* tile_count, cudaStream_t stream);
+                       uint32_t* tile_count, const float* tanfov, cudaStream_t stream);
 // depth_keys [P] (by splat) -> sorted_ids [M] in (key, id) order and offsets [M] = inclusive instance counts
 // also publishes the frame counters (capacity, seq, overflow) of the bucket-sorted frame
 void launch_depth_bucket_sort(int P, const DepthBuckets& buckets, const uint32_t* depth_keys,
@@ -155,7 +155,8 @@ void launch_blend_backward(int W, int H, const uint2* ranges, const uint32_t* or
 
 // preprocess_bwd.cu
 void launch_preprocess_backward(const gab200_backward_args& b, const SplatRec* rec, const SplatAux* aux,
-                                const uint8_t* clamped, const float* g2d, float* face_scratch, cudaStream_t stream);
+                                const uint8_t* clamped, const float* g2d, float* face_scratch, const float* tanfov,
+                                cudaStream_t stream);
 #define GAB_FACE_GRAD_STRIDE 13  // per-splat face-frame gradient record: centre 3, orientation 9, scale 1
 
 // face_frame.cu

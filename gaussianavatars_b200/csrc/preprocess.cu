@@ -26,15 +26,18 @@ __device__ __forceinline__ void stage_camera(const gab200_forward_args& a, Camer
 
 // =====================================================================================================
 // K1: fused bind + activate + project + EWA + SH->RGB.  One thread per splat.
+// DEVFOV: (tanfovx, tanfovy) come from the device float[2] `tanfov` (gab200_forward_device_fov) instead of the
+// by-value args, so that a captured graph renders whatever field of view was written before the replay.
 // =====================================================================================================
-template <bool BOUND>
+template <bool BOUND, bool DEVFOV>
 __global__ void __launch_bounds__(PRE_NT) preprocess_kernel(gab200_forward_args a, SplatRec* __restrict__ rec,
                                                             SplatAux* __restrict__ aux,
                                                             uint32_t* __restrict__ tiles_touched,
                                                             uint8_t* __restrict__ clamped,
                                                             uint32_t* __restrict__ depth_keys,
                                                             uint32_t* __restrict__ ids, int exact_binning,
-                                                            DepthBuckets bk, uint32_t* __restrict__ tile_count) {
+                                                            DepthBuckets bk, uint32_t* __restrict__ tile_count,
+                                                            const float* __restrict__ tanfov) {
   __shared__ Camera cam;
   __shared__ float sh_s[PRE_NT * SH_SMEM_STRIDE_MAX];
   stage_camera(a, cam);
@@ -85,8 +88,17 @@ __global__ void __launch_bounds__(PRE_NT) preprocess_kernel(gab200_forward_args 
     opacity = raw.o;
   }
 
+  // DEVFOV: one broadcast load per thread; a device value that is zero, negative or not finite culls the splat
+  // before any tile index is formed (radius 0, no instances)
+  float dev_tx = 0.f, dev_ty = 0.f;
+  bool fov_ok = true;
+  if (DEVFOV) {
+    dev_tx = __ldg(tanfov);
+    dev_ty = __ldg(tanfov + 1);
+    fov_ok = dev_tx > 0.f && isfinite(dev_tx) && dev_ty > 0.f && isfinite(dev_ty);
+  }
   const float3 t = xform4x3(cam.V, p);
-  if (t.z > 0.2f) {
+  if (fov_ok && t.z > 0.2f) {
     const float hx = cam.Pm[0] * p.x + cam.Pm[4] * p.y + cam.Pm[8] * p.z + cam.Pm[12];
     const float hy = cam.Pm[1] * p.x + cam.Pm[5] * p.y + cam.Pm[9] * p.z + cam.Pm[13];
     const float hw = cam.Pm[3] * p.x + cam.Pm[7] * p.y + cam.Pm[11] * p.z + cam.Pm[15];
@@ -105,8 +117,9 @@ __global__ void __launch_bounds__(PRE_NT) preprocess_kernel(gab200_forward_args 
       }
     }
 
-    const float focal_x = (float)W / (2.0f * a.tanfovx), focal_y = (float)H / (2.0f * a.tanfovy);
-    const float limx = 1.3f * a.tanfovx, limy = 1.3f * a.tanfovy;
+    const float tanfovx = DEVFOV ? dev_tx : a.tanfovx, tanfovy = DEVFOV ? dev_ty : a.tanfovy;
+    const float focal_x = (float)W / (2.0f * tanfovx), focal_y = (float)H / (2.0f * tanfovy);
+    const float limx = 1.3f * tanfovx, limy = 1.3f * tanfovy;
     const float txtz = t.x / t.z, tytz = t.y / t.z;
     const float tcx = fminf(limx, fmaxf(-limx, txtz)) * t.z;
     const float tcy = fminf(limy, fmaxf(-limy, tytz)) * t.z;
@@ -250,15 +263,14 @@ __global__ void __launch_bounds__(PRE_NT) preprocess_kernel(gab200_forward_args 
 
 void launch_preprocess(const gab200_forward_args& a, SplatRec* rec, SplatAux* aux, uint32_t* tiles_touched,
                        uint8_t* clamped, uint32_t* depth_keys, uint32_t* ids, const DepthBuckets& buckets,
-                       uint32_t* tile_count, cudaStream_t stream) {
+                       uint32_t* tile_count, const float* tanfov, cudaStream_t stream) {
   const int threads = PRE_NT, blocks = (a.P + threads - 1) / threads;
   if (blocks == 0) return;
-  if (a.input_mode == GAB200_INPUT_BOUND_RAW)
-    preprocess_kernel<true><<<blocks, threads, 0, stream>>>(a, rec, aux, tiles_touched, clamped, depth_keys, ids,
-                                                            a.exact_binning, buckets, tile_count);
-  else
-    preprocess_kernel<false><<<blocks, threads, 0, stream>>>(a, rec, aux, tiles_touched, clamped, depth_keys, ids,
-                                                             a.exact_binning, buckets, tile_count);
+  const bool bound = a.input_mode == GAB200_INPUT_BOUND_RAW;
+  auto kernel = bound ? (tanfov ? preprocess_kernel<true, true> : preprocess_kernel<true, false>)
+                      : (tanfov ? preprocess_kernel<false, true> : preprocess_kernel<false, false>);
+  kernel<<<blocks, threads, 0, stream>>>(a, rec, aux, tiles_touched, clamped, depth_keys, ids, a.exact_binning, buckets,
+                                         tile_count, tanfov);
   count_launch();
 }
 

@@ -13,13 +13,15 @@
 
 namespace gab {
 
-template <bool BOUND, bool MC>
+// DEVFOV: (tanfovx, tanfovy) from the device float[2] `tanfov` the forward read (gab200_backward_device_fov).
+template <bool BOUND, bool MC, bool DEVFOV>
 __global__ void __launch_bounds__(PRE_NT, 12) preprocess_backward_kernel(gab200_backward_args b, gab200_forward_args a,
                                                                   const SplatRec* __restrict__ rec,
                                                                   const SplatAux* __restrict__ aux,
                                                                   const uint8_t* __restrict__ clamped,
                                                                   const float* __restrict__ g2d,
-                                                                  float* __restrict__ face_scratch) {
+                                                                  float* __restrict__ face_scratch,
+                                                                  const float* __restrict__ tanfov) {
   __shared__ Camera cam;
   __shared__ float fg_s[PRE_NT * GAB_FACE_GRAD_STRIDE];  // per-splat face-frame gradients, written out coalesced
   float* my_fg = fg_s + threadIdx.x * GAB_FACE_GRAD_STRIDE;
@@ -99,9 +101,11 @@ __global__ void __launch_bounds__(PRE_NT, 12) preprocess_backward_kernel(gab200_
 
     // ---- conic -> cov2D -> Sigma, t -> mean ----
     const float* V = cam.V;
-    const float fx = (float)W / (2.0f * a.tanfovx), fy = (float)H / (2.0f * a.tanfovy);
+    // visible splats only: the forward culled every splat when the device field of view was invalid
+    const float tanfovx = DEVFOV ? __ldg(tanfov) : a.tanfovx, tanfovy = DEVFOV ? __ldg(tanfov + 1) : a.tanfovy;
+    const float fx = (float)W / (2.0f * tanfovx), fy = (float)H / (2.0f * tanfovy);
     float3 t = xform4x3(V, m);
-    const float limx = 1.3f * a.tanfovx, limy = 1.3f * a.tanfovy;
+    const float limx = 1.3f * tanfovx, limy = 1.3f * tanfovy;
     const float txtz = t.x / t.z, tytz = t.y / t.z;
     const float x_grad_mul = (txtz < -limx || txtz > limx) ? 0.f : 1.f;
     const float y_grad_mul = (tytz < -limy || tytz > limy) ? 0.f : 1.f;
@@ -425,17 +429,20 @@ __global__ void __launch_bounds__(256) face_grad_reduce_kernel(int num_chunks, c
 }
 
 void launch_preprocess_backward(const gab200_backward_args& b, const SplatRec* rec, const SplatAux* aux,
-                                const uint8_t* clamped, const float* g2d, float* face_scratch, cudaStream_t stream) {
+                                const uint8_t* clamped, const float* g2d, float* face_scratch, const float* tanfov,
+                                cudaStream_t stream) {
   const gab200_forward_args& a = *b.fwd;
   const int threads = PRE_NT, blocks = (a.P + threads - 1) / threads;
   if (blocks == 0) return;
+  const bool dev = tanfov != nullptr;
   if (a.input_mode == GAB200_INPUT_BOUND_RAW) {
-    if (b.grads_are_multicast)
-      preprocess_backward_kernel<true, true><<<blocks, threads, 0, stream>>>(b, a, rec, aux, clamped, g2d, face_scratch);
-    else
-      preprocess_backward_kernel<true, false><<<blocks, threads, 0, stream>>>(b, a, rec, aux, clamped, g2d, face_scratch);
+    auto kernel = b.grads_are_multicast
+                      ? (dev ? preprocess_backward_kernel<true, true, true> : preprocess_backward_kernel<true, true, false>)
+                      : (dev ? preprocess_backward_kernel<true, false, true> : preprocess_backward_kernel<true, false, false>);
+    kernel<<<blocks, threads, 0, stream>>>(b, a, rec, aux, clamped, g2d, face_scratch, tanfov);
   } else {
-    preprocess_backward_kernel<false, false><<<blocks, threads, 0, stream>>>(b, a, rec, aux, clamped, g2d, nullptr);
+    auto kernel = dev ? preprocess_backward_kernel<false, false, true> : preprocess_backward_kernel<false, false, false>;
+    kernel<<<blocks, threads, 0, stream>>>(b, a, rec, aux, clamped, g2d, nullptr, tanfov);
   }
   count_launch();
   if (face_scratch != nullptr && b.num_face_chunks > 0) {

@@ -5,6 +5,12 @@
     frame.run()                                                                # enqueue one replay
     pc._xyz.grad, frame.verts.grad, frame.loss ...                             # static result tensors
 
+By default the field of view is the `fovx`/`fovy` given at construction, baked into the graph: every replay renders
+with it, so that mode is only correct for cameras that share one FoV.  With `per_camera_fov=True` the camera block
+also carries tan(FoVx/2), tan(FoVy/2) (`camera_block(cam, fov=True)`, 37 floats) and the kernels read them from device
+memory on every replay: one captured graph trains every camera of a calibrated rig (the reference gives each camera
+its own FoV, scene/dataset_readers.py).
+
 What is captured (the data flow of the reference training step, train.py:113-170, with the fused route of
 `render()`): [H2D copy of the camera block and the uint8 ground truth] -> per-face frame of the posed mesh
 (scene/flame_gaussian_model.py:137-147) -> fused binding + rasterizer forward (gaussian_renderer/__init__.py:19-101) ->
@@ -33,6 +39,7 @@ re-captures.  The gradients reach the FLAME tensors, and a capturable `Adam` hol
 """
 from __future__ import annotations
 
+import math
 from typing import Optional
 
 import torch
@@ -55,19 +62,34 @@ class _Pipe:
 
 
 class _GraphCamera:
-    """Camera whose matrices are views into the graph's static camera block."""
+    """Camera whose matrices (and, in a 37-float block, device field of view `tanfov`) are views into the graph's
+    static camera block."""
 
     def __init__(self, W, H, fovx, fovy, block):
         self.image_width, self.image_height, self.FoVx, self.FoVy = W, H, fovx, fovy
         self.world_view_transform = block[0:16].view(4, 4)
         self.full_proj_transform = block[16:32].view(4, 4)
         self.camera_center = block[32:35]
+        self.tanfov = block[35:37] if block.numel() == CAMERA_BLOCK_FOV else None
 
 
-def camera_block(cam) -> torch.Tensor:
-    """(35,) float32: world_view_transform (16) | full_proj_transform (16) | camera_center (3) of a camera object."""
-    return torch.cat((cam.world_view_transform.reshape(-1).float(), cam.full_proj_transform.reshape(-1).float(),
-                      cam.camera_center.reshape(-1).float()))
+CAMERA_BLOCK, CAMERA_BLOCK_FOV = 35, 37
+
+
+def tanfov_floats(fovx: float, fovy: float) -> torch.Tensor:
+    """(2,) float32 {tan(fovx/2), tan(fovy/2)}: computed in double and rounded once, as render()'s settings round
+    them on their way to the kernels."""
+    return torch.tensor([math.tan(fovx * 0.5), math.tan(fovy * 0.5)], dtype=torch.float32)
+
+
+def camera_block(cam, fov: bool = False) -> torch.Tensor:
+    """(35,) float32: world_view_transform (16) | full_proj_transform (16) | camera_center (3) of a camera object.
+    fov=True: (37,), followed by tan(FoVx/2), tan(FoVy/2) (a GraphedFrame with per_camera_fov=True)."""
+    parts = [cam.world_view_transform.reshape(-1).float(), cam.full_proj_transform.reshape(-1).float(),
+             cam.camera_center.reshape(-1).float()]
+    if fov:
+        parts.append(tanfov_floats(cam.FoVx, cam.FoVy).to(parts[0].device))
+    return torch.cat(parts)
 
 
 def pair_with_deferred_reduce(frames, buffers, side_work_at: str = "start"):
@@ -110,7 +132,7 @@ class GraphedFrame:
                  lambda_dssim: float = 0.2, host_inputs: bool = False, capacity: Optional[int] = None,
                  headroom: float = 1.25, after_backward=None, warm_cameras=None, regularizers: Optional[dict] = None,
                  before_backward=None, side_work=None, side_work_at: str = "start", optimizer: Optional[Adam] = None,
-                 densify_stats: bool = False):
+                 densify_stats: bool = False, per_camera_fov: bool = False):
         """loss: "l1_u8" (L1 vs a uint8 ground truth), "photometric" ((1-l) L1 + l (1-SSIM) vs a uint8 ground truth) or
         "dL_dimage" (the caller supplies dL/dimage in `self.dL_dimage`).
         host_inputs: the frame owns pinned STAGING tensors (`cam_stage` (35,) float32, `gt_stage` (3,H,W) uint8) that a
@@ -127,7 +149,8 @@ class GraphedFrame:
         side_work: optional callable captured on a FORKED branch of the graph that runs concurrently with the whole
         frame and is joined at its end -- e.g. the all-reduce of the PREVIOUS step's gradient buffer
         (dist.SymmetricGradBuffer.reduce of the other frame of an alternating pair), which then costs no step time.
-        warm_cameras: camera blocks (35,) rendered eagerly before the capture to size the instance capacity.
+        warm_cameras: camera blocks (35,) -- (37,) or camera objects with per_camera_fov -- rendered eagerly before the
+        capture to size the instance capacity.
         regularizers: keyword arguments of `binding_regularizers` (threshold_xyz, lambda_scale, ...; {} = the
         reference's defaults): the position / scale terms of train.py:134-146 are added to the loss inside the graph.
         densify_stats: after backward (and after_backward) the graph accumulates the densification statistics of the
@@ -139,10 +162,18 @@ class GraphedFrame:
         hyper-parameters) and run() re-captures (`captures` counts it) when any of it changed: after
         densify_and_prune, reset_opacity or oneupSHdegree.  A learning rate written into a group on the host every
         iteration therefore re-captures every iteration: give the group an `lr_schedule` instead.  Not combinable
-        with pair_with_deferred_reduce; a synchronous all-reduce in after_backward runs before the step."""
+        with pair_with_deferred_reduce; a synchronous all-reduce in after_backward runs before the step.
+        per_camera_fov: False (default): every replay renders with the fovx / fovy given here, baked into the graph --
+        correct only for cameras that share that FoV.  True: the camera block is 37 floats, the last two
+        tan(FoVx/2), tan(FoVy/2) (`camera_block(cam, fov=True)`), read by the kernels on every replay; fovx / fovy
+        only seed the initial block.  set_inputs(camera=), warm_cameras, the staging tensors and prefetch_for then
+        all carry 37 floats, and the warm-up sizes the capacity with each warm camera's own FoV.  The FoV is not
+        part of what triggers a re-capture."""
         if loss not in ("l1_u8", "photometric", "dL_dimage"):
             raise ValueError("loss must be 'l1_u8', 'photometric' or 'dL_dimage'")
         self.pc, self.W, self.H, self.fovx, self.fovy = pc, int(width), int(height), float(fovx), float(fovy)
+        self.per_camera_fov = bool(per_camera_fov)
+        nblk = CAMERA_BLOCK_FOV if self.per_camera_fov else CAMERA_BLOCK
         self.loss_kind, self.lambda_dssim, self.host_inputs = loss, float(lambda_dssim), bool(host_inputs)
         self.after_backward = after_backward
         self.before_backward = before_backward   # e.g. SymmetricGradBuffer.begin
@@ -161,7 +192,9 @@ class GraphedFrame:
         dev = pc._xyz.device
         self.device = dev
         self.bg = bg.to(dev).float().contiguous()
-        self.cam = torch.zeros(35, dtype=torch.float32, device=dev)
+        self.cam = torch.zeros(nblk, dtype=torch.float32, device=dev)
+        if self.per_camera_fov:
+            self.cam[CAMERA_BLOCK:] = tanfov_floats(self.fovx, self.fovy).to(dev)
         self.camera = _GraphCamera(self.W, self.H, self.fovx, self.fovy, self.cam)
         self.flame = getattr(pc, "flame", None)
         if self.flame is not None:   # the pose is computed inside the graph from this timestep
@@ -173,7 +206,9 @@ class GraphedFrame:
             self.timestep = None
         self.gt = torch.zeros((3, self.H, self.W), dtype=torch.uint8, device=dev) if loss != "dL_dimage" else None
         self.dL_dimage = torch.zeros((3, self.H, self.W), dtype=torch.float32, device=dev) if loss == "dL_dimage" else None
-        self.cam_host = torch.zeros(35, dtype=torch.float32).pin_memory() if host_inputs else None  # staging
+        self.cam_host = torch.zeros(nblk, dtype=torch.float32).pin_memory() if host_inputs else None  # staging
+        if self.cam_host is not None:
+            self.cam_host.copy_(self.cam)
         self.cam_stage = self.cam_host
         self.gt_stage = (torch.zeros((3, self.H, self.W), dtype=torch.uint8).pin_memory()
                          if host_inputs and self.gt is not None else None)
@@ -190,6 +225,16 @@ class GraphedFrame:
         self._uploads = bool(host_inputs)
         self._capacity = capacity
         self._warm = list(warm_cameras) if warm_cameras is not None else None
+        if self.per_camera_fov and self._warm is not None:
+            self._warm = [self._camera_tensor(c) for c in self._warm]
+
+    def _camera_tensor(self, camera):
+        """A camera object or block as this frame's block: 37 floats with per_camera_fov, else as given."""
+        blk = camera if isinstance(camera, torch.Tensor) else camera_block(camera, fov=self.per_camera_fov)
+        if self.per_camera_fov and blk.numel() != CAMERA_BLOCK_FOV:
+            raise ValueError(f"per_camera_fov=True: a camera block has {CAMERA_BLOCK_FOV} floats "
+                             f"(camera_block(cam, fov=True)), got {blk.numel()}")
+        return blk
 
     # ---- inputs ------------------------------------------------------------------------------------------------
     def set_inputs(self, camera=None, verts=None, gt_u8=None, dL_dimage=None, timestep=None):
@@ -205,7 +250,7 @@ class GraphedFrame:
                 raise IndexError(f"timestep {t} outside [0, {self.num_timesteps})")
             self.timestep.fill_(t)
         if camera is not None:
-            blk = camera if isinstance(camera, torch.Tensor) else camera_block(camera)
+            blk = self._camera_tensor(camera)
             if blk.device.type == "cpu" and self._uploads:
                 if not blk.is_pinned():      # stage pageable memory (after any upload still reading the staging copy)
                     self._side.synchronize()
@@ -230,6 +275,8 @@ class GraphedFrame:
         into `other`'s device inputs while it computes.  Call before capture()."""
         if not (self.host_inputs and other.host_inputs):
             raise ValueError("prefetching needs host_inputs=True on both frames")
+        if self.per_camera_fov != other.per_camera_fov:
+            raise ValueError("both frames of a prefetching pair must use the same per_camera_fov mode")
         self._prefetch_target = other
         return self
 

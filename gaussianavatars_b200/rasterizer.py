@@ -207,7 +207,20 @@ def visible_of(radii: torch.Tensor):
     return v[1] if v is not None and v[0] == radii.data_ptr() else None
 
 
-def _run_forward(a: N.ForwardArgs, device, need_backward: bool, hints: Optional[FrameHints] = None):
+def check_tanfov(tanfov: Optional[torch.Tensor], device):
+    """A camera's device field of view: a (2,) float32 tensor {tan(FoVx/2), tan(FoVy/2)} on `device`, or None."""
+    if tanfov is None:
+        return None
+    if not isinstance(tanfov, torch.Tensor) or tanfov.device != device or tanfov.dtype != torch.float32 or \
+            tanfov.numel() != 2 or not tanfov.is_contiguous():
+        raise ValueError(f"tanfov must be a contiguous (2,) float32 tensor on {device}")
+    return tanfov
+
+
+def _run_forward(a: N.ForwardArgs, device, need_backward: bool, hints: Optional[FrameHints] = None,
+                 tanfov: Optional[torch.Tensor] = None):
+    """tanfov: None (a.tanfovx / tanfovy) or the (2,) device tensor the kernels read instead
+    (gab200_forward_device_fov); the backward must then be given the same tensor."""
     global _last, _last_info
     H, W, P = a.image_height, a.image_width, a.P
     color = torch.empty((3, H, W), dtype=torch.float32, device=device)
@@ -235,7 +248,10 @@ def _run_forward(a: N.ForwardArgs, device, need_backward: bool, hints: Optional[
         a.frame_seq = hints.seq
     with torch.cuda.device(device):
         stream = torch.cuda.current_stream(device).cuda_stream
-        n = N.lib().gab200_forward(C.byref(a), C.byref(st), C.c_void_p(stream))
+        if tanfov is None:
+            n = N.lib().gab200_forward(C.byref(a), C.byref(st), C.c_void_p(stream))
+        else:
+            n = N.lib().gab200_forward_device_fov(C.byref(a), tanfov.data_ptr(), C.byref(st), C.c_void_p(stream))
     N.check(n, "gab200_forward")
     info = dict(num_rendered=int(st.num_rendered), capacity=int(st.binning_capacity), sync_mode=int(a.sync_mode),
                 depth_sort_path=int(st.depth_sort_path), attempts=int(st.attempts))
@@ -250,6 +266,17 @@ def _run_forward(a: N.ForwardArgs, device, need_backward: bool, hints: Optional[
         # pooled (inference) scratch stays valid until the next no_grad forward on this device
         _last = (a, st, holder, device)
     return color, radii, st, holder
+
+
+def _run_backward(b: N.BackwardArgs, device, tanfov: Optional[torch.Tensor] = None):
+    """gab200_backward, or gab200_backward_device_fov with the tensor the forward read."""
+    with torch.cuda.device(device):
+        stream = torch.cuda.current_stream(device).cuda_stream
+        if tanfov is None:
+            N.check(N.lib().gab200_backward(C.byref(b), C.c_void_p(stream)), "gab200_backward")
+        else:
+            N.check(N.lib().gab200_backward_device_fov(C.byref(b), tanfov.data_ptr(), C.c_void_p(stream)),
+                    "gab200_backward")
 
 
 class _RasterizeGaussians(torch.autograd.Function):
@@ -309,9 +336,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         b.dL_dmeans3D, b.dL_dmeans2D, b.dL_dopacity = d_means3D.data_ptr(), d_means2D.data_ptr(), d_opac.data_ptr()
         b.dL_dcolors, b.dL_dshs = d_colors.data_ptr(), N.ptr(d_sh)
         b.dL_dscales, b.dL_drotations, b.dL_dcov3D = N.ptr(d_scales), N.ptr(d_rots), d_cov.data_ptr()
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            N.check(N.lib().gab200_backward(C.byref(b), C.c_void_p(stream)), "gab200_backward")
+        _run_backward(b, device)
         ctx.holder = None
         return (d_means3D, d_means2D, d_sh, d_colors if colors_precomp is not None else None, d_opac, d_scales, d_rots,
                 d_cov if cov3Ds_precomp is not None else None, None)
@@ -403,7 +428,7 @@ def _face_csr(binding: torch.Tensor, num_faces: int, chunk: int = 16):
 class _RasterizeBound(torch.autograd.Function):
     @staticmethod
     def forward(ctx, _xyz, means2D, _rotation, _scaling, _opacity, f_dc, f_rest, face_center, face_orien_mat,
-                face_scaling, binding, colors_precomp, raster_settings, grad_sink=None):
+                face_scaling, binding, colors_precomp, raster_settings, grad_sink=None, tanfov=None):
         rs = raster_settings
         ctx.grad_sink = grad_sink
         device = _xyz.device
@@ -435,8 +460,10 @@ class _RasterizeBound(torch.autograd.Function):
             a.binding, a.num_faces = binding.data_ptr(), F
             a.face_center, a.face_orien_mat, a.face_scaling = face_center.data_ptr(), face_orien_mat.data_ptr(), \
                 face_scaling.data_ptr()
+        tanfov = check_tanfov(tanfov, device)
         color, radii, st, holder = _run_forward(a, device, need_bw,
-                                                hints_of(grad_sink) if grad_sink is not None else None)
+                                                hints_of(grad_sink) if grad_sink is not None else None, tanfov)
+        ctx.tanfov = tanfov
         if need_bw:
             ctx.args, ctx.state, ctx.holder = a, st, holder
             ctx.keep = (cams, _xyz, _rotation, _scaling, _opacity, f_dc, f_rest, face_center, face_orien_mat,
@@ -501,30 +528,32 @@ class _RasterizeBound(torch.autograd.Function):
             b.face_perm, b.face_chunk_face = perm.data_ptr(), c_face.data_ptr()
             b.face_chunk_start, b.face_chunk_end = c_start.data_ptr(), c_end.data_ptr()
             b.num_face_chunks = c_face.shape[0]
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            N.check(N.lib().gab200_backward(C.byref(b), C.c_void_p(stream)), "gab200_backward")
+        _run_backward(b, device, ctx.tanfov)
         ctx.holder = None
         if ctx.grad_sink is not None:  # dist.py: ONE all-reduce over this buffer instead of six
             ctx.grad_sink.flat_grad = flat
             ctx.grad_sink._gab200_mc_used = bool(use_symm)  # SymmetricGradBuffer.end() only trusts the replica if set
-        return (d_xyz, d_means2D, d_rot, d_scale, d_opac, d_dc, d_rest, d_fc, d_fR, d_fs, None, d_colors, None, None)
+        return (d_xyz, d_means2D, d_rot, d_scale, d_opac, d_dc, d_rest, d_fc, d_fR, d_fs, None, d_colors, None, None,
+                None)
 
 
 def rasterize_bound(raster_settings: GaussianRasterizationSettings, _xyz, _rotation, _scaling, _opacity,
                     features_dc, features_rest, binding=None, face_center=None, face_orien_mat=None,
-                    face_scaling=None, means2D=None, colors_precomp=None, grad_sink=None):
+                    face_scaling=None, means2D=None, colors_precomp=None, grad_sink=None, tanfov=None):
     """Fused binding + rasterization.  Returns (color (3,H,W), radii (P,) int32).
 
     binding=None is the identity frame (a plain GaussianModel, scene/gaussian_model.py:115-116,127-128,142-143).
-    `means2D` is the usual (P,3) gradient holder (its .grad receives dL/dmean2D in NDC units)."""
+    `means2D` is the usual (P,3) gradient holder (its .grad receives dL/dmean2D in NDC units).
+    `tanfov`: optional (2,) float32 device tensor {tan(FoVx/2), tan(FoVy/2)} read by the kernels in place of
+    raster_settings.tanfovx / tanfovy -- a CUDA graph replay renders whatever was written there before it.  Zero,
+    negative or non-finite values cull every splat (image = background)."""
     if means2D is None:
         means2D = torch.zeros((_xyz.shape[0], 3), dtype=torch.float32, device=_xyz.device)
     if _opacity.ndim == 1:
         _opacity = _opacity[:, None]
     return _RasterizeBound.apply(_xyz, means2D, _rotation, _scaling, _opacity, features_dc, features_rest,
                                  face_center, face_orien_mat, face_scaling, binding, colors_precomp, raster_settings,
-                                 grad_sink)
+                                 grad_sink, tanfov)
 
 
 def bind_activate(raster_settings_or_modifier, _xyz, _rotation, _scaling, _opacity, binding=None, face_center=None,

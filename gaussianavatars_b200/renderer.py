@@ -10,6 +10,9 @@
     (`rasterize_bound`): no getter, no torch.cat, no (P,3,3) temporaries, one flat gradient buffer.
 Camera matrices that live on the host are uploaded once and cached on the camera object (the reference re-uploads
 three tensors per call, gaussian_renderer/__init__.py:44-47).
+A camera may carry its field of view in device memory as `cam.tanfov`, a (2,) float32 CUDA tensor
+{tan(FoVx/2), tan(FoVy/2)} (graph.GraphedFrame(per_camera_fov=True) does): the fused route's kernels read it there
+instead of FoVx / FoVy; the reference route cannot and refuses such a camera.
 """
 from __future__ import annotations
 
@@ -61,7 +64,8 @@ def render_bound(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, ove
         fc, fR, fs = pc.face_center, pc.face_orien_mat, pc.face_scaling
     rendered_image, radii = rasterize_bound(rs, pc._xyz, pc._rotation, pc._scaling, pc._opacity, pc._features_dc,
                                             pc._features_rest, binding, fc, fR, fs, means2D=screenspace_points,
-                                            colors_precomp=override_color, grad_sink=pc)
+                                            colors_precomp=override_color, grad_sink=pc,
+                                            tanfov=getattr(viewpoint_camera, "tanfov", None))
     return {"render": rendered_image, "viewspace_points": screenspace_points, "visibility_filter": _visible(radii),
             "radii": radii}
 
@@ -80,6 +84,9 @@ def render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_
         return render_bound(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_color)
 
     # ---- reference route (data flow of gaussian_renderer/__init__.py:27-101) ----
+    if getattr(viewpoint_camera, "tanfov", None) is not None:
+        raise ValueError("a camera with a device field of view (cam.tanfov) needs the fused route: the reference route "
+                         "only takes FoVx / FoVy as host floats")
     xyz = pc.get_xyz
     device = xyz.device
     screenspace_points = torch.zeros_like(xyz, dtype=xyz.dtype, requires_grad=True, device=device) + 0

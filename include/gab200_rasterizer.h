@@ -100,7 +100,8 @@ typedef struct gab200_forward_args {
   int32_t sh_degree;       /* active SH degree D (0..3) */
   int32_t sh_coeffs;       /* M: coefficients stored per splat (1,4,9,16); 0 with colors_precomp */
   int32_t image_width, image_height;
-  float tanfovx, tanfovy, scale_modifier;
+  float tanfovx, tanfovy;   /* tan(FoV / 2); the *_device_fov entry points read them from device memory instead */
+  float scale_modifier;
   int32_t prefiltered;     /* accepted for signature parity; the near-plane cull is always applied */
   int32_t debug;           /* 1: synchronise + check after every stage (reference `debug=` flag) */
   int32_t need_backward;   /* 0: inference -- per-pixel state for backward is not written */
@@ -244,6 +245,18 @@ typedef struct gab200_backward_args {
 } gab200_backward_args;
 
 int32_t gab200_backward(const gab200_backward_args* args, void* stream);
+
+/* Per-camera field of view read from device memory, so that one captured CUDA graph can render every camera of a
+ * calibrated rig (the reference gives each camera its own FoVx / FoVy: scene/dataset_readers.py, render()).
+ * tanfov: DEVICE float[2] = {tan(FoVx / 2), tan(FoVy / 2)}, 4-byte aligned, read by the kernels when they run -- a
+ * graph replay uses whatever the caller wrote there before it.  args->tanfovx / tanfovy are ignored.  The arithmetic
+ * after the load is that of gab200_forward: the same float values give bit-identical results.  A value that is zero,
+ * negative or not finite culls every splat (radii 0, no instances, image = background); nothing is read or written
+ * out of bounds.  tanfov == NULL: exactly gab200_forward / gab200_backward.  Every sync mode is supported.
+ * The backward MUST be given the same pointer (holding the same values) as the forward whose state it consumes. */
+int64_t gab200_forward_device_fov(const gab200_forward_args* args, const float* tanfov, gab200_frame_state* state_out,
+                                  void* stream);
+int32_t gab200_backward_device_fov(const gab200_backward_args* args, const float* tanfov, void* stream);
 
 /* Frustum test only.  Replaces diff_gaussian_rasterization._C.mark_visible (GaussianRasterizer.markVisible). */
 int32_t gab200_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,

@@ -6,6 +6,8 @@ training iteration per step (train.py:106-210) -- xyz learning-rate schedule, po
               and with it a host wait per line), the learning rate written on the host, host-stepped Adam
   graph       GraphedFrame for frame -> backward, then the same eager statistics, host lr and host-stepped Adam
   graph_full  ONE replay of GraphedFrame(optimizer=capturable Adam with the xyz schedule, densify_stats=True)
+  graph_full_percam  the graph_full iteration over 16 cameras with DISTINCT fields of view (look_at_camera at the
+              orbit poses, FoV spread +-8 %): GraphedFrame(per_camera_fov=True), the FoV read on the device per replay
 With a FLAME head (synthetic.flame_like_assets on the same mesh, 16 timesteps, the reference's FLAME optimizer groups
 trained as with not_finetune_flame_params=False):
   eager_flame       the eager arm with the pose of select_mesh_by_timestep from the float32 reference-order
@@ -76,7 +78,13 @@ for (W, H) in ((550, 802), (1920, 1080)):
     cams = [syn.orbit_camera(W, H, azimuth_deg=-60 + 120 * (i + .5) / 16, elevation_deg=5 * math.sin(i)) for i in range(16)]
     gts = [torch.randint(0, 256, (3, H, W), dtype=torch.uint8, device=dev) for _ in range(2)]
     res = {"config": "3", "splats": P, "W": W, "H": H, "timed_steps": K, "gpu": name, "power_limit": power}
-    for arm in ("eager", "graph", "graph_full", "eager_flame", "graph_full_flame"):
+    # the same poses with distinct fields of view: 20 deg vertical (the orbit default) scaled by 0.92 .. 1.08
+    fov_cams = []
+    for i, c in enumerate(cams):
+        f = 1.0 + 0.08 * (2 * i / 15 - 1)
+        fov_cams.append(syn.look_at_camera(W, H, math.degrees(c.FoVx) * f, math.degrees(c.FoVy) * f,
+                                           w2c=c.world_view_transform.T.numpy()))
+    for arm in ("eager", "graph", "graph_full", "graph_full_percam", "eager_flame", "graph_full_flame"):
         flame = arm.endswith("_flame")
         if flame:
             a = FLAME_ASSETS
@@ -129,10 +137,12 @@ for (W, H) in ((550, 802), (1920, 1080)):
                 reference_stats(pc, out["radii"], out["viewspace_points"].grad)
                 opt.step()
         else:
-            blocks = [camera_block(c).to(dev) for c in cams]
+            percam = arm == "graph_full_percam"
+            blocks = [camera_block(c, fov=True).to(dev) for c in fov_cams] if percam else \
+                [camera_block(c).to(dev) for c in cams]
             kw = dict(optimizer=opt, densify_stats=True) if arm.startswith("graph_full") else {}
             fr = GraphedFrame(pc, W, H, cams[0].FoVx, cams[0].FoVy, bg, loss="photometric", lambda_dssim=0.2,
-                              regularizers={}, warm_cameras=blocks, **kw)
+                              regularizers={}, warm_cameras=blocks, per_camera_fov=percam, **kw)
             if flame:
                 fr.set_inputs(camera=blocks[0], timestep=0, gt_u8=gts[0])
             else:
