@@ -177,7 +177,7 @@ EXPORTED_SYMBOLS = ("gab200_forward", "gab200_backward", "gab200_mark_visible", 
                     "gab200_regularize_forward", "gab200_regularize_backward", "gab200_nvls_allreduce", "gab200_densify_scratch_bytes", "gab200_densify_plan", "gab200_densify_apply",
                     "gab200_adam_step_device", "gab200_densify_stats", "gab200_flame_scratch_bytes",
                     "gab200_flame_prepare", "gab200_flame_forward", "gab200_flame_backward",
-                    "gab200_forward_device_fov", "gab200_backward_device_fov")
+                    "gab200_forward_device_fov", "gab200_backward_device_fov", "gab200_forward_display")
 
 _lib = None
 _lock = threading.Lock()
@@ -213,6 +213,9 @@ def lib():
         L.gab200_forward_device_fov.restype = C.c_int64
         L.gab200_forward_device_fov.argtypes = [C.POINTER(ForwardArgs), C.c_void_p, C.POINTER(FrameState), C.c_void_p]
         L.gab200_backward_device_fov.restype = C.c_int32
+        L.gab200_forward_display.restype = C.c_int64
+        L.gab200_forward_display.argtypes = [C.POINTER(ForwardArgs), C.c_void_p, C.c_void_p, C.POINTER(FrameState),
+                                             C.c_void_p]
         L.gab200_backward_device_fov.argtypes = [C.POINTER(BackwardArgs), C.c_void_p, C.c_void_p]
         L.gab200_mark_visible.restype = C.c_int32
         L.gab200_mark_visible.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]

@@ -227,10 +227,11 @@ int tune_get(int knob) {
   return v > 0 ? v - 1 : g_tune_default[knob];  // stored biased by one so that zero-initialised = "default"
 }
 
-static bool validate(const gab200_forward_args* a) {
+// display_only: gab200_forward_display with a uint8 image and no backward, the one case out_color may be NULL
+static bool validate(const gab200_forward_args* a, bool display_only = false) {
   if (a == nullptr || a->abi_version != GAB200_ABI_VERSION) return false;
   if (a->P < 0 || a->image_width <= 0 || a->image_height <= 0) return false;
-  if (a->out_color == nullptr || (a->P > 0 && a->radii == nullptr)) return false;
+  if ((a->out_color == nullptr && !display_only) || (a->P > 0 && a->radii == nullptr)) return false;
   if (!a->bg || !a->viewmatrix || !a->projmatrix || !a->campos) return false;
   if (!a->alloc_geom || !a->alloc_binning || !a->alloc_image) return false;
   if (a->P == 0) return true;
@@ -338,6 +339,7 @@ namespace {
 struct Frame {
   const gab200_forward_args* a;
   const float* tanfov;  // device float[2] (gab200_forward_device_fov) or NULL: a->tanfovx / tanfovy
+  uint8_t* out_rgb8;    // [H,W,3] display image (gab200_forward_display) or NULL
   gab200_frame_state* st;
   cudaStream_t stream;
   GeomView g;
@@ -480,7 +482,7 @@ int enqueue_binning_blend(Frame& f, void* bin, int64_t cap, int64_t n_known, siz
   {
     StageScope sc(GAB200_STAGE_BLEND_FWD, stream);
     launch_blend_forward(f.W, f.H, f.iv.ranges, f.iv.order, f.iv.order_info, bv.vals[selector], f.g.rec, a->bg,
-                         a->out_color, f.iv.final_T, f.iv.n_contrib, bv.strip_mask, stream);
+                         a->out_color, f.iv.final_T, f.iv.n_contrib, bv.strip_mask, f.out_rgb8, stream);
   }
   GAB_STAGE_CHECK(f.dbg, stream);
   return GAB200_OK;
@@ -495,14 +497,17 @@ int wait_counters(Frame& f) {
 }
 }  // namespace
 
-// gab200_forward and gab200_forward_device_fov (tanfov == NULL: the by-value tanfovx / tanfovy)
-static int64_t run_forward(const gab200_forward_args* a, const float* tanfov, gab200_frame_state* st, void* stream_) {
+// gab200_forward, gab200_forward_device_fov and gab200_forward_display (tanfov == NULL: the by-value tanfovx /
+// tanfovy; out_rgb8 == NULL: no display image)
+static int64_t run_forward(const gab200_forward_args* a, const float* tanfov, uint8_t* out_rgb8,
+                           gab200_frame_state* st, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
-  if (!validate(a) || st == nullptr) return GAB200_ERR_INVALID_ARGUMENT;
+  if (!validate(a, out_rgb8 != nullptr && a != nullptr && a->need_backward == 0) || st == nullptr)
+    return GAB200_ERR_INVALID_ARGUMENT;
   if (check_arch() < 0) return GAB200_ERR_ARCH;
   memset(st, 0, sizeof(*st));
   Frame f;
-  f.a = a; f.tanfov = tanfov; f.st = st; f.stream = stream;
+  f.a = a; f.tanfov = tanfov; f.out_rgb8 = out_rgb8; f.st = st; f.stream = stream;
   f.P = a->P; f.W = a->image_width; f.H = a->image_height;
   f.gx = (f.W + GAB_TILE - 1) / GAB_TILE; f.gy = (f.H + GAB_TILE - 1) / GAB_TILE;
   f.nb = a->need_backward != 0;
@@ -638,12 +643,17 @@ static int64_t run_forward(const gab200_forward_args* a, const float* tanfov, ga
 }
 
 int64_t gab200_forward(const gab200_forward_args* a, gab200_frame_state* st, void* stream) {
-  return run_forward(a, nullptr, st, stream);
+  return run_forward(a, nullptr, nullptr, st, stream);
 }
 
 int64_t gab200_forward_device_fov(const gab200_forward_args* a, const float* tanfov, gab200_frame_state* st,
                                   void* stream) {
-  return run_forward(a, tanfov, st, stream);
+  return run_forward(a, tanfov, nullptr, st, stream);
+}
+
+int64_t gab200_forward_display(const gab200_forward_args* a, const float* tanfov, uint8_t* out_rgb8,
+                               gab200_frame_state* st, void* stream) {
+  return run_forward(a, tanfov, out_rgb8, st, stream);
 }
 
 // gab200_backward and gab200_backward_device_fov

@@ -122,17 +122,50 @@ struct BandGeom {
   __device__ __forceinline__ int bit(int i) const { return 2 * (band0 + i) + half; }
 };
 
+// ---- display epilogue: the image as interleaved uint8 [H,W,3], quantised as render.py:41 does it,
+// data.mul(255).add_(0.5).clamp_(0, 255) then the cast (truncation).  The multiply and the add are separately rounded
+// (no contraction into an fma), so the byte equals torch's two ops on the float the float path stores, bit for bit.
+#define BLEND_OUT_FLOAT 1  // [3,H,W] float32
+#define BLEND_OUT_U8 2     // [H,W,3] uint8
+__device__ __forceinline__ uint32_t quantize_u8(float c) {
+  return __float2uint_rz(fminf(fmaxf(__fadd_rn(__fmul_rn(c, 255.f), 0.5f), 0.f), 255.f));
+}
+// One row of a band is 8 lanes (lane = row * 8 + column) holding 8 consecutive pixels: 24 bytes = 6 words.  Lane
+// (row, j < 6) writes word j, bytes 4j .. 4j+3, which lie in pixels p0 = 4j/3 and p0 + 1 from byte 4j - 3 p0 of p0:
+// two shuffles per band, and the warp stores whole aligned 32-bit words instead of 96 scattered bytes.  A row whose
+// start is not word-aligned (W % 4 != 0) or that the image's right edge cuts stores bytes.  All 32 lanes call this.
+__device__ __forceinline__ void store_display(uint8_t* __restrict__ out, int W, int H, int pixx, int y, int lane,
+                                              float r, float g, float b) {
+  const uint32_t px = quantize_u8(r) | (quantize_u8(g) << 8) | (quantize_u8(b) << 16);
+  const int j = lane & 7, x0 = pixx - j;
+  const int p0 = min((4 * j) / 3, 6);
+  const uint32_t lo = __shfl_sync(FULLMASK, px, (lane & ~7) | p0);
+  const uint32_t hi = __shfl_sync(FULLMASK, px, (lane & ~7) | (p0 + 1));
+  const uint32_t word = (uint32_t)((((uint64_t)hi << 24) | lo) >> (8 * (4 * j - 3 * p0)));
+  if (y >= H) return;
+  const size_t row = (size_t)y * W;
+  if ((W & 3) == 0 && x0 + 8 <= W && ((uintptr_t)out & 3u) == 0) {
+    if (j < 6) reinterpret_cast<uint32_t*>(out)[(row + x0) / 4 * 3 + j] = word;
+  } else if (pixx < W) {
+    uint8_t* o = out + (row + pixx) * 3;
+    o[0] = (uint8_t)px;
+    o[1] = (uint8_t)(px >> 8);
+    o[2] = (uint8_t)(px >> 16);
+  }
+}
+
 // =====================================================================================================
 // Forward: one tile on a group of NT = 256/K threads (tl = thread index inside the group)
 // =====================================================================================================
-template <int K>
+template <int K, int OUT>
 __device__ __forceinline__ void forward_tile(int tile, int tl, GroupBarrier<256 / K> bar, SplatRec* buf0,
                                              SplatRec* buf1, uint32_t* smask, uint32_t* ids_ring, uint64_t* mbar,
                                              int W, int H, int gx,
                                              const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list,
                                              const SplatRec* __restrict__ rec, const float* __restrict__ bg,
                                              float* __restrict__ out_color, float* __restrict__ final_T,
-                                             uint32_t* __restrict__ n_contrib, uint8_t* __restrict__ strip_mask) {
+                                             uint32_t* __restrict__ n_contrib, uint8_t* __restrict__ strip_mask,
+                                             uint8_t* __restrict__ out_rgb8) {
   constexpr int NT = 256 / K;
   const int tx = tile % gx, ty = tile / gx;
   const int lane = tl & 31;
@@ -273,20 +306,28 @@ __device__ __forceinline__ void forward_tile(int tile, int tl, GroupBarrier<256 
     const int y = pixy0 + 4 * i;
     if (pixx < W && y < H) {
       const size_t pix = (size_t)y * W + pixx;
-      out_color[pix] = fmaf(T[i], bg0, Cr[i]);
-      out_color[HW + pix] = fmaf(T[i], bg1, Cg[i]);
-      out_color[2 * HW + pix] = fmaf(T[i], bg2, Cb[i]);
+      if (OUT & BLEND_OUT_FLOAT) {
+        out_color[pix] = fmaf(T[i], bg0, Cr[i]);
+        out_color[HW + pix] = fmaf(T[i], bg1, Cg[i]);
+        out_color[2 * HW + pix] = fmaf(T[i], bg2, Cb[i]);
+      }
       if (final_T != nullptr) {
         final_T[pix] = T[i];
         n_contrib[pix] = last[i];
       }
     }
   }
+  if (OUT & BLEND_OUT_U8) {
+#pragma unroll
+    for (int i = 0; i < K; i++)
+      store_display(out_rgb8, W, H, pixx, pixy0 + 4 * i, lane, fmaf(T[i], bg0, Cr[i]), fmaf(T[i], bg1, Cg[i]),
+                    fmaf(T[i], bg2, Cb[i]));
+  }
 }
 
 // CTA = 256 threads.  The first CTAs take KH heavy tiles each on 256/KH threads (KH = 1: all eight warps on one
 // tile); the following CTAs take four light tiles each, one per 64-thread group, K = 4.
-template <int KH>
+template <int KH, int OUT>
 __global__ void __launch_bounds__(256) blend_forward_kernel(int W, int H, int gx, int tiles,
                                                             const uint2* __restrict__ ranges,
                                                             const uint32_t* __restrict__ order,
@@ -296,7 +337,8 @@ __global__ void __launch_bounds__(256) blend_forward_kernel(int W, int H, int gx
                                                             const float* __restrict__ bg, float* __restrict__ out_color,
                                                             float* __restrict__ final_T,
                                                             uint32_t* __restrict__ n_contrib,
-                                                            uint8_t* __restrict__ strip_mask) {
+                                                            uint8_t* __restrict__ strip_mask,
+                                                            uint8_t* __restrict__ out_rgb8) {
   __shared__ SplatRec buf[2][256];
   __shared__ uint32_t smask[256];
   __shared__ __align__(16) uint32_t ids_ring[4][ID_RING * (64 + 4)];  // per 64-thread group; a 256-thread tile uses it flat
@@ -309,28 +351,32 @@ __global__ void __launch_bounds__(256) blend_forward_kernel(int W, int H, int gx
   if (b < heavy_ctas) {
     const int g = t / NTH, slot = b * GH + g;
     if (slot >= nh) return;
-    forward_tile<KH>((int)order[slot], t - g * NTH, GroupBarrier<NTH>{GH == 1 ? 0 : 1 + g}, buf[0] + g * NTH,
-                     buf[1] + g * NTH, smask + g * NTH, &ids_ring[0][0] + g * (ID_RING * (NTH + 4)), mbar[g], W, H, gx,
-                     ranges, point_list, rec, bg, out_color, final_T, n_contrib, strip_mask);
+    forward_tile<KH, OUT>((int)order[slot], t - g * NTH, GroupBarrier<NTH>{GH == 1 ? 0 : 1 + g}, buf[0] + g * NTH,
+                          buf[1] + g * NTH, smask + g * NTH, &ids_ring[0][0] + g * (ID_RING * (NTH + 4)), mbar[g], W,
+                          H, gx, ranges, point_list, rec, bg, out_color, final_T, n_contrib, strip_mask, out_rgb8);
   } else {
     const int g = t >> 6, slot = nh + 4 * (b - heavy_ctas) + g;
     if (slot >= tiles) return;
-    forward_tile<4>((int)order[slot], t & 63, GroupBarrier<64>{1 + g}, buf[0] + g * 64, buf[1] + g * 64,
-                    smask + g * 64, ids_ring[g], mbar[g], W, H, gx, ranges, point_list, rec, bg, out_color, final_T,
-                    n_contrib, strip_mask);
+    forward_tile<4, OUT>((int)order[slot], t & 63, GroupBarrier<64>{1 + g}, buf[0] + g * 64, buf[1] + g * 64,
+                         smask + g * 64, ids_ring[g], mbar[g], W, H, gx, ranges, point_list, rec, bg, out_color,
+                         final_T, n_contrib, strip_mask, out_rgb8);
   }
 }
 
 void launch_blend_forward(int W, int H, const uint2* ranges, const uint32_t* order, const uint32_t* order_info,
                           const uint32_t* point_list, const SplatRec* rec, const float* bg, float* out_color,
-                          float* final_T, uint32_t* n_contrib, uint8_t* strip_mask, cudaStream_t stream) {
+                          float* final_T, uint32_t* n_contrib, uint8_t* strip_mask, uint8_t* out_rgb8,
+                          cudaStream_t stream) {
   const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
   const int tiles = gx * gy;
   if (tiles == 0) return;
   // upper bound on CTAs: every tile heavy; surplus CTAs exit at once
   const int grid = tiles;
-  blend_forward_kernel<1><<<grid, 256, 0, stream>>>(W, H, gx, tiles, ranges, order, order_info, point_list, rec, bg,
-                                                    out_color, final_T, n_contrib, strip_mask);
+  auto kernel = out_rgb8 == nullptr ? blend_forward_kernel<1, BLEND_OUT_FLOAT>
+                : out_color == nullptr ? blend_forward_kernel<1, BLEND_OUT_U8>
+                                       : blend_forward_kernel<1, BLEND_OUT_FLOAT | BLEND_OUT_U8>;
+  kernel<<<grid, 256, 0, stream>>>(W, H, gx, tiles, ranges, order, order_info, point_list, rec, bg, out_color, final_T,
+                                   n_contrib, strip_mask, out_rgb8);
   count_launch();
 }
 

@@ -147,7 +147,7 @@ cudaError_t run_sort(void* temp, size_t temp_bytes, uint32_t* keys_a, uint32_t* 
 void launch_blend_forward(int W, int H, const uint2* ranges, const uint32_t* order, const uint32_t* order_info,
                           const uint32_t* point_list, const SplatRec* rec,
                           const float* bg, float* out_color, float* final_T, uint32_t* n_contrib, uint8_t* strip_mask,
-                          cudaStream_t stream);
+                          uint8_t* out_rgb8, cudaStream_t stream);  // out_color / out_rgb8: either may be NULL
 void launch_blend_backward(int W, int H, const uint2* ranges, const uint32_t* order, const uint32_t* order_info,
                            const uint32_t* point_list, const SplatRec* rec,
                            const float* bg, const float* final_T, const uint32_t* n_contrib, const float* dL_dpix,

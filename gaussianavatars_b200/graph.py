@@ -45,7 +45,7 @@ from typing import Optional
 import torch
 
 from . import rasterizer as R
-from .renderer import render
+from .renderer import _forward_only, render
 from .rasterizer import l1_loss_u8
 from .densify import add_densification_stats
 from .training import Adam, binding_regularizers, photometric_loss
@@ -498,4 +498,276 @@ class GraphedFrame:
         need = self.counters()["num_rendered"]
         cap = max(int(need * self.headroom) + 16384, int(self.slot.capacity * 1.5))
         self.graph = None
+        self.capture(capacity=cap)
+
+
+class GraphedRender:
+    """One PLAYBACK frame as ONE forward-only CUDA graph: what the reference's render.py, the fps benchmarks and the
+    viewer run per frame (select_mesh_by_timestep(t) -> render() -> the uint8 frame), with no backward, no loss and
+    no ground truth.
+
+        view = GraphedRender(pc, width, height, bg, outputs="u8", host_slots=2)
+        view.set_inputs(camera=cam, timestep=t)          # device buffers: never a re-capture
+        view.run()                                       # enqueue one replay
+        view.display, view.image, view.radii             # static result tensors ((H,W,3) uint8, (3,H,W) float32)
+
+    What is captured: [the FLAME pose of the device timestep (pc.flame), or the given vertices in `verts`] -> the
+    per-face frame (update_mesh_properties) -> the fused forward (need_backward = 0, GAB200_SYNC_NONE) writing the
+    float image and/or the display image (gab200_forward_display: bit for bit render.py's
+    mul(255).add_(0.5).clamp_(0, 255).permute(1, 2, 0).to(uint8)).  With mesh_update=False the graph renders the
+    face frame the model holds (pc.face_center ...) at capture: eager update_mesh_properties calls replace those
+    tensors and re-capture.
+
+    The camera is always the 37-float block with the field of view (`camera_block(cam, fov=True)`: a viewer zooms);
+    camera, timestep, vertices and background are device buffers written by `set_inputs`.  The parameters and the
+    rows of pc.flame_param are read by address on every replay, so in-place edits (a viewer's FLAME sliders) show in
+    the next one.  run() re-captures when the model, the image size or `scaling_modifier` changed (`captures` counts
+    it): P, active_sh_degree, the addresses of the parameters and of the binding, the FLAME tensors' addresses and
+    shapes and the in-place versions of shape / static_offset.
+
+    The instance capacity is sized and guarded as in GraphedFrame: eager frames over `warm_cameras` (x `headroom`),
+    a sticky overflow flag, `run(check=True)` re-captures with room and replays, `overflowed()`, `regrow()`.  The
+    graph owns its scratch (allocated during the capture, in the graph's private pool), so eager no_grad renders,
+    whose pooled scratch grows and moves, never touch it.
+
+    host_slots=k > 0: after each replay the display frame travels to a ring of k pinned host tensors on a copy
+    stream, one event per replay, so the copy of frame i overlaps replay i+1 (a consumer one replay behind never
+    waits for a transfer).  `host_frame(i)` waits for replay i's copy and returns its slot; slot i % k is rewritten
+    by replay i + k, not before."""
+
+    def __init__(self, pc, width: int, height: int, bg: torch.Tensor, outputs: str = "u8",
+                 scaling_modifier: float = 1.0, mesh_update: bool = True, host_slots: int = 0,
+                 capacity: Optional[int] = None, headroom: float = 1.25, warm_cameras=None, warm_timesteps=None):
+        """outputs: "u8" (the display image only: the float image is not written), "float" or "both".
+        warm_cameras: camera objects or 37-float blocks rendered eagerly before the capture to size the capacity (and
+        the depth-sort range); warm_timesteps: with a FLAME head, the timesteps each warm camera is rendered at
+        (default: the current one) -- a sequence played back whole sizes the graph once for all its frames."""
+        if outputs not in ("u8", "float", "both"):
+            raise ValueError("outputs must be 'u8', 'float' or 'both'")
+        if host_slots < 0 or (host_slots > 0 and outputs == "float"):
+            raise ValueError("host_slots copies the display image: it needs outputs 'u8' or 'both'")
+        self.pc, self.W, self.H = pc, int(width), int(height)
+        self.outputs, self.scaling_modifier, self.mesh_update = outputs, float(scaling_modifier), bool(mesh_update)
+        self.headroom, self._capacity = float(headroom), capacity
+        dev = pc._xyz.device
+        self.device = dev
+        self.bg = bg.to(dev).float().contiguous().clone()
+        self.cam = torch.zeros(CAMERA_BLOCK_FOV, dtype=torch.float32, device=dev)
+        self.cam[CAMERA_BLOCK:] = 1.0   # tan(45 deg): a harmless field of view until the first camera arrives
+        self.camera = _GraphCamera(self.W, self.H, math.pi / 2, math.pi / 2, self.cam)
+        self.flame = getattr(pc, "flame", None)
+        if self.flame is not None:
+            self.verts = None
+            self.timestep = torch.zeros(1, dtype=torch.int32, device=dev)
+            self.num_timesteps = int(pc.flame_param["expr"].shape[0])
+        else:
+            rest = getattr(pc, "verts_rest", None)
+            self.verts = None if rest is None else rest.detach().clone().contiguous()
+            self.timestep = None
+        self._warm = None if warm_cameras is None else [self._camera_tensor(c) for c in warm_cameras]
+        self._warm_t = None if warm_timesteps is None or self.flame is None else [int(t) for t in warm_timesteps]
+        self.host_slots = int(host_slots)
+        self.host = self._copy_stream = None
+        self._staged = self._host_events = self._stage_events = None
+        self.image = self.display = self.radii = None
+        self.graph = self.slot = self._key = None
+        self.replays = self.captures = 0
+
+    @staticmethod
+    def _camera_tensor(camera):
+        blk = camera if isinstance(camera, torch.Tensor) else camera_block(camera, fov=True)
+        if blk.numel() != CAMERA_BLOCK_FOV:
+            raise ValueError(f"a GraphedRender camera block has {CAMERA_BLOCK_FOV} floats "
+                             f"(camera_block(cam, fov=True)), got {blk.numel()}")
+        return blk
+
+    # ---- inputs ------------------------------------------------------------------------------------------------
+    def set_inputs(self, camera=None, timestep=None, verts=None, bg=None):
+        """Copies new inputs into the graph's device buffers; none of them re-captures.  A camera OBJECT of another
+        image size changes the frame's size (the next run() re-captures)."""
+        if verts is not None and self.flame is not None:
+            raise ValueError("this frame poses its FLAME head itself: give set_inputs(timestep=...), not verts")
+        if timestep is not None:
+            if self.flame is None:
+                raise ValueError("timestep= needs a model with a FLAME head (pc.flame)")
+            t = int(timestep)
+            if not 0 <= t < self.num_timesteps:
+                raise IndexError(f"timestep {t} outside [0, {self.num_timesteps})")
+            self.timestep.fill_(t)
+        if camera is not None:
+            blk = self._camera_tensor(camera)
+            if not isinstance(camera, torch.Tensor):
+                self.W, self.H = int(camera.image_width), int(camera.image_height)
+                self.camera.image_width, self.camera.image_height = self.W, self.H
+            self.cam.copy_(blk, non_blocking=True)
+        if verts is not None:
+            if self.verts is None:
+                self.verts = verts.detach().reshape(-1, 3).to(self.device).float().contiguous().clone()
+            else:
+                self.verts.copy_(verts.detach().reshape(self.verts.shape), non_blocking=True)
+        if bg is not None:
+            self.bg.copy_(bg, non_blocking=True)
+
+    # ---- the frame body (run eagerly for warm-up, then captured) -------------------------------------------------
+    def _body(self):
+        pc = self.pc
+        with torch.no_grad():
+            if self.mesh_update:
+                if self.flame is not None:
+                    verts, pc.verts_cano = flame_pose(self.flame, pc.flame_param, self.timestep)
+                    pc.update_mesh_properties(verts[0])
+                elif self.verts is not None:
+                    pc.update_mesh_properties(self.verts)
+            out = _forward_only(self.camera, pc, _Pipe, self.bg, self.scaling_modifier,
+                                self.outputs != "float", self.outputs != "u8")
+        self.image, self.display, self.radii = out["render"], out["display_u8"], out["radii"]
+
+    def _learn_capacity(self):
+        """Eager frames (sync modes EXACT then LATE) over the warm-up cameras: their instance counts size the graph."""
+        hints = R.hints_of(self.pc)
+        key = (self.device, self.W, self.H, self.pc._xyz.shape[0])
+        n_max, lo, hi = 0, 0xFFFFFFFF, 0
+        cam0 = self.cam.clone()
+        t0 = None if self.timestep is None else self.timestep.clone()
+        blocks = [b.to(self.device) for b in self._warm] if self._warm else [cam0]
+        steps = self._warm_t if self._warm_t else [None]
+        cur = torch.cuda.current_stream(self.device)
+        side = torch.cuda.Stream(device=self.device)
+        side.wait_stream(cur)
+        with torch.cuda.stream(side):
+            for rep in range(2):
+                for blk in blocks:
+                    for t in steps:
+                        self.cam.copy_(blk)
+                        if t is not None:
+                            self.timestep.fill_(t)
+                        self._body()
+                        n_max = max(n_max, int((hints.last or {}).get("num_rendered", 0)))
+                        d = hints.get(key)[1]
+                        if d[1] > d[0]:
+                            lo, hi = min(lo, d[0]), max(hi, d[1])
+            self.cam.copy_(cam0)
+            if t0 is not None:
+                self.timestep.copy_(t0)
+        cur.wait_stream(side)
+        torch.cuda.synchronize(self.device)
+        self.image = self.display = self.radii = None
+        return n_max, ((lo, hi) if hi > lo else (0, 0))
+
+    def _state_key(self):
+        """Everything the capture baked in that eager code between replays may replace."""
+        pc = self.pc
+        b = getattr(pc, "binding", None)
+        key = [int(pc._xyz.shape[0]), int(getattr(pc, "active_sh_degree", 0)), None if b is None else b.data_ptr(),
+               self.W, self.H, self.scaling_modifier]
+        key += [p.data_ptr() for p in pc.parameters()]
+        if self.flame is not None:
+            for k in _FLAME_KEYS:
+                t = pc.flame_param.get(k)
+                key.append(None if t is None else (t.data_ptr(), tuple(t.shape)) +
+                           ((t._version,) if k in ("shape", "static_offset") else ()))
+        if not self.mesh_update and b is not None:
+            key += [getattr(pc, n).data_ptr() for n in ("face_center", "face_orien_mat", "face_scaling")]
+        return tuple(key)
+
+    def capture(self, capacity: Optional[int] = None):
+        dev, pc = self.device, self.pc
+        self.camera.image_width, self.camera.image_height = self.W, self.H
+        n_max, depth = self._learn_capacity()
+        if capacity is None:
+            capacity = self._capacity if self._capacity else int(n_max * self.headroom) + 16384
+        self.graph = None
+        self.slot = R.CaptureSlot(dev, capacity, depth)
+        self.graph = torch.cuda.CUDAGraph()
+        R._capture_slot = self.slot
+        try:
+            with torch.cuda.graph(self.graph):
+                self._body()
+                self.slot.flag_host.copy_(self.slot.flag, non_blocking=True)
+        finally:
+            R._capture_slot = None
+        # the mesh tensors the replay writes (the model's attributes are replaced by any eager frame)
+        self._mesh = tuple(getattr(pc, n, None) for n in ("verts", "verts_cano", "face_center", "face_orien_mat",
+                                                          "face_scaling")) \
+            if self.mesh_update else None
+        self._key = self._state_key()
+        if self.host_slots:
+            self._make_ring()
+        self.captures += 1
+        return self
+
+    def _make_ring(self):
+        """Pinned host slots, two device staging copies of the display frame and their events."""
+        k, shape = self.host_slots, (self.H, self.W, 3)
+        if self.host is None or tuple(self.host[0].shape) != shape:
+            torch.cuda.synchronize(self.device)
+            self.host = [torch.empty(shape, dtype=torch.uint8).pin_memory() for _ in range(k)]
+            self._staged = [torch.empty(shape, dtype=torch.uint8, device=self.device) for _ in range(2)]
+        self._copy_stream = self._copy_stream or torch.cuda.Stream(device=self.device)
+        self._host_events = [None] * k     # per host slot: the copy into it, and which replay it holds
+        self._host_replay = [-1] * k
+        self._stage_events = [None, None]  # per staging buffer: the copy that last read it
+
+    def _ship(self):
+        """Replay i's display frame -> staging buffer i % 2 (on the main stream, right behind the replay) -> host slot
+        i % k (copy stream).  The main stream waits only for the copy of replay i - 2, long since done when replays
+        take longer than a transfer."""
+        i = self.replays - 1
+        s, h = i % 2, i % self.host_slots
+        cur = torch.cuda.current_stream(self.device)
+        if self._stage_events[s] is not None:
+            cur.wait_event(self._stage_events[s])
+        self._staged[s].copy_(self.display)
+        ready = torch.cuda.Event()
+        ready.record(cur)
+        self._copy_stream.wait_event(ready)
+        with torch.cuda.stream(self._copy_stream):
+            self.host[h].copy_(self._staged[s], non_blocking=True)
+            done = torch.cuda.Event()
+            done.record(self._copy_stream)
+        self._stage_events[s] = self._host_events[h] = done
+        self._host_replay[h] = i
+
+    def host_frame(self, replay: Optional[int] = None) -> torch.Tensor:
+        """The pinned (H,W,3) uint8 slot holding replay `replay` (default: the latest) once its copy has landed."""
+        if not self.host_slots:
+            raise ValueError("host_frame needs host_slots > 0")
+        i = self.replays - 1 if replay is None else int(replay)
+        h = i % self.host_slots
+        if self._host_replay[h] != i:
+            raise IndexError(f"replay {i} is not in the host ring (slot {h} holds replay {self._host_replay[h]})")
+        self._host_events[h].synchronize()
+        return self.host[h]
+
+    # ---- replay ----------------------------------------------------------------------------------------------------
+    def run(self, check: bool = False):
+        if self.graph is None or self._state_key() != self._key:   # host-side compare: no sync
+            self.capture()
+        self.graph.replay()
+        if check and self.overflowed(wait=True):
+            self.regrow()
+            self.graph.replay()
+            if self.overflowed(wait=True):
+                raise RuntimeError("GraphedRender: the frame still overflows its instance capacity after re-capture")
+        self.replays += 1
+        if self.host_slots:
+            self._ship()
+        return self
+
+    def overflowed(self, wait: bool = True) -> bool:
+        """True if any replay since the last (re-)capture needed more than the captured capacity."""
+        if self.slot is None:
+            return False
+        if wait:
+            torch.cuda.current_stream(self.device).synchronize()
+        return bool(int(self.slot.flag_host[0]) != 0)
+
+    def counters(self) -> dict:
+        return GraphedFrame.counters(self)
+
+    def regrow(self):
+        """Re-capture with the capacity the overflowing frame asked for (x headroom) and a fresh depth range."""
+        torch.cuda.synchronize(self.device)
+        need = self.counters()["num_rendered"]
+        cap = max(int(need * self.headroom) + 16384, int(self.slot.capacity * 1.5))
         self.capture(capacity=cap)

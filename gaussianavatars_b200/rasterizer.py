@@ -194,6 +194,7 @@ class CaptureSlot:
         self.flag_host = torch.zeros(1, dtype=torch.int32).pin_memory()
         self.seq = 1
         self.info = {}
+        self.scratch = None   # a captured forward-only frame's own scratch (see _run_forward)
 
 
 _capture_slot = None
@@ -217,22 +218,40 @@ def check_tanfov(tanfov: Optional[torch.Tensor], device):
     return tanfov
 
 
+def check_rgb8(rgb8: Optional[torch.Tensor], rs: GaussianRasterizationSettings, device):
+    """A display-image destination: a contiguous (H,W,3) uint8 tensor on `device`, or None."""
+    if rgb8 is None:
+        return None
+    shape = (int(rs.image_height), int(rs.image_width), 3)
+    if not isinstance(rgb8, torch.Tensor) or rgb8.device != device or rgb8.dtype != torch.uint8 or \
+            tuple(rgb8.shape) != shape or not rgb8.is_contiguous():
+        raise ValueError(f"rgb8 must be a contiguous {shape} uint8 tensor on {device}")
+    return rgb8
+
+
 def _run_forward(a: N.ForwardArgs, device, need_backward: bool, hints: Optional[FrameHints] = None,
-                 tanfov: Optional[torch.Tensor] = None):
+                 tanfov: Optional[torch.Tensor] = None, rgb8: Optional[torch.Tensor] = None, float_image: bool = True):
     """tanfov: None (a.tanfovx / tanfovy) or the (2,) device tensor the kernels read instead
-    (gab200_forward_device_fov); the backward must then be given the same tensor."""
+    (gab200_forward_device_fov); the backward must then be given the same tensor.
+    rgb8: None, or a (H,W,3) uint8 tensor the blend writes the display image into (gab200_forward_display);
+    float_image=False (with rgb8, no backward) skips the float image: the returned color is None."""
     global _last, _last_info
     H, W, P = a.image_height, a.image_width, a.P
-    color = torch.empty((3, H, W), dtype=torch.float32, device=device)
+    color = torch.empty((3, H, W), dtype=torch.float32, device=device) if float_image else None
     radii = torch.empty((P,), dtype=torch.int32, device=device)
     visible = torch.empty((P,), dtype=torch.bool, device=device)   # radii > 0, written by the preprocess kernel
-    a.out_color, a.radii, a.visibility = color.data_ptr(), radii.data_ptr(), visible.data_ptr()
+    a.out_color, a.radii, a.visibility = N.ptr(color), radii.data_ptr(), visible.data_ptr()
     _tls.visible = (radii.data_ptr(), visible)   # renderer.py hands it out as `visibility_filter`
-    cb, holder = N.begin_forward(device, need_backward)
+    slot = _capture_slot
+    # A forward-only frame captured into a graph must own its scratch: the pooled inference buffers are shared with
+    # every eager no_grad render and replaced when a larger frame comes along, so the graph's baked-in pointers would
+    # be overwritten or freed.  Allocated during the capture, the scratch lives in the graph's private pool.
+    cb, holder = N.begin_forward(device, need_backward or slot is not None)
+    if slot is not None and not need_backward:
+        slot.scratch = holder
     a.alloc_geom = a.alloc_binning = a.alloc_image = cb
     st = N.FrameState()
     key = (device, W, H, P)
-    slot = _capture_slot
     if slot is not None:      # graph capture: fixed capacity, no host wait; graph.py reads slot.counters after replays
         a.sync_mode = N.SYNC_NONE
         a.binning_hint = slot.capacity
@@ -248,7 +267,10 @@ def _run_forward(a: N.ForwardArgs, device, need_backward: bool, hints: Optional[
         a.frame_seq = hints.seq
     with torch.cuda.device(device):
         stream = torch.cuda.current_stream(device).cuda_stream
-        if tanfov is None:
+        if rgb8 is not None:
+            n = N.lib().gab200_forward_display(C.byref(a), N.ptr(tanfov), rgb8.data_ptr(), C.byref(st),
+                                               C.c_void_p(stream))
+        elif tanfov is None:
             n = N.lib().gab200_forward(C.byref(a), C.byref(st), C.c_void_p(stream))
         else:
             n = N.lib().gab200_forward_device_fov(C.byref(a), tanfov.data_ptr(), C.byref(st), C.c_void_p(stream))
@@ -428,7 +450,8 @@ def _face_csr(binding: torch.Tensor, num_faces: int, chunk: int = 16):
 class _RasterizeBound(torch.autograd.Function):
     @staticmethod
     def forward(ctx, _xyz, means2D, _rotation, _scaling, _opacity, f_dc, f_rest, face_center, face_orien_mat,
-                face_scaling, binding, colors_precomp, raster_settings, grad_sink=None, tanfov=None):
+                face_scaling, binding, colors_precomp, raster_settings, grad_sink=None, tanfov=None, rgb8=None,
+                float_image=True):
         rs = raster_settings
         ctx.grad_sink = grad_sink
         device = _xyz.device
@@ -461,8 +484,12 @@ class _RasterizeBound(torch.autograd.Function):
             a.face_center, a.face_orien_mat, a.face_scaling = face_center.data_ptr(), face_orien_mat.data_ptr(), \
                 face_scaling.data_ptr()
         tanfov = check_tanfov(tanfov, device)
+        rgb8 = check_rgb8(rgb8, rs, device)
+        if not float_image and (rgb8 is None or need_bw):
+            raise ValueError("float_image=False needs rgb8= and no gradient (the backward reads the float image's state)")
         color, radii, st, holder = _run_forward(a, device, need_bw,
-                                                hints_of(grad_sink) if grad_sink is not None else None, tanfov)
+                                                hints_of(grad_sink) if grad_sink is not None else None, tanfov,
+                                                rgb8, float_image)
         ctx.tanfov = tanfov
         if need_bw:
             ctx.args, ctx.state, ctx.holder = a, st, holder
@@ -534,26 +561,30 @@ class _RasterizeBound(torch.autograd.Function):
             ctx.grad_sink.flat_grad = flat
             ctx.grad_sink._gab200_mc_used = bool(use_symm)  # SymmetricGradBuffer.end() only trusts the replica if set
         return (d_xyz, d_means2D, d_rot, d_scale, d_opac, d_dc, d_rest, d_fc, d_fR, d_fs, None, d_colors, None, None,
-                None)
+                None, None, None)
 
 
 def rasterize_bound(raster_settings: GaussianRasterizationSettings, _xyz, _rotation, _scaling, _opacity,
                     features_dc, features_rest, binding=None, face_center=None, face_orien_mat=None,
-                    face_scaling=None, means2D=None, colors_precomp=None, grad_sink=None, tanfov=None):
+                    face_scaling=None, means2D=None, colors_precomp=None, grad_sink=None, tanfov=None, rgb8=None,
+                    float_image=True):
     """Fused binding + rasterization.  Returns (color (3,H,W), radii (P,) int32).
 
     binding=None is the identity frame (a plain GaussianModel, scene/gaussian_model.py:115-116,127-128,142-143).
     `means2D` is the usual (P,3) gradient holder (its .grad receives dL/dmean2D in NDC units).
     `tanfov`: optional (2,) float32 device tensor {tan(FoVx/2), tan(FoVy/2)} read by the kernels in place of
     raster_settings.tanfovx / tanfovy -- a CUDA graph replay renders whatever was written there before it.  Zero,
-    negative or non-finite values cull every splat (image = background)."""
+    negative or non-finite values cull every splat (image = background).
+    `rgb8`: optional contiguous (H,W,3) uint8 CUDA tensor that the forward blend also fills with the display image,
+    bit for bit torch's color.mul(255).add_(0.5).clamp_(0, 255).permute(1, 2, 0).to(torch.uint8)
+    (gab200_forward_display).  float_image=False (rgb8 given, no gradient) skips the float image: color is None."""
     if means2D is None:
         means2D = torch.zeros((_xyz.shape[0], 3), dtype=torch.float32, device=_xyz.device)
     if _opacity.ndim == 1:
         _opacity = _opacity[:, None]
     return _RasterizeBound.apply(_xyz, means2D, _rotation, _scaling, _opacity, features_dc, features_rest,
                                  face_center, face_orien_mat, face_scaling, binding, colors_precomp, raster_settings,
-                                 grad_sink, tanfov)
+                                 grad_sink, tanfov, rgb8, bool(float_image))
 
 
 def bind_activate(raster_settings_or_modifier, _xyz, _rotation, _scaling, _opacity, binding=None, face_center=None,

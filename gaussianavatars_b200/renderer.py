@@ -70,6 +70,38 @@ def render_bound(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, ove
             "radii": radii}
 
 
+def _forward_only(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, display: bool, float_image: bool):
+    """Fused route, forward only (no autograd): the float image and/or the display image."""
+    if not _has_raw(pc):
+        raise ValueError("render_display needs the fused route: a model exposing the raw parameters "
+                         "(_xyz, _rotation, _scaling, _opacity, _features_dc, _features_rest)")
+    device = pc._xyz.device
+    rs = _settings(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, device)
+    rgb8 = torch.empty((rs.image_height, rs.image_width, 3), dtype=torch.uint8, device=device) if display else None
+    binding = getattr(pc, "binding", None)
+    fc = fR = fs = None
+    d = lambda t: None if t is None else t.detach()  # noqa: E731  (no gradient: the forward keeps no backward state)
+    with torch.no_grad():
+        if binding is not None:
+            if getattr(pc, "face_center", None) is None:
+                pc.select_mesh_by_timestep(0)
+            fc, fR, fs = d(pc.face_center), d(pc.face_orien_mat), d(pc.face_scaling)
+        img, radii = rasterize_bound(rs, d(pc._xyz), d(pc._rotation), d(pc._scaling), d(pc._opacity),
+                                     d(pc._features_dc), d(pc._features_rest), binding, fc, fR, fs, grad_sink=pc,
+                                     tanfov=getattr(viewpoint_camera, "tanfov", None), rgb8=rgb8,
+                                     float_image=float_image)
+    return {"display_u8": rgb8, "render": img, "radii": radii, "visibility_filter": _visible(radii)}
+
+
+def render_display(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, float_image=False):
+    """One playback frame: the fused route's forward only, no autograd, with the image as the reference's render.py
+    and viewers consume it -- `display_u8`, a (H,W,3) uint8 tensor equal bit for bit to
+    render(...)["render"].mul(255).add_(0.5).clamp_(0, 255).permute(1, 2, 0).to(torch.uint8), written by the forward
+    blend itself (3 bytes per pixel instead of 12, no eager quantisation chain).  float_image=True also returns the
+    float (3,H,W) image as "render" (else None).  Returns {"display_u8", "render", "radii", "visibility_filter"}."""
+    return _forward_only(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, True, float_image)
+
+
 def _visible(radii):
     """`radii > 0` (gaussian_renderer/__init__.py:100): the forward wrote it next to the radii (one byte per splat)."""
     v = visible_of(radii)

@@ -258,6 +258,19 @@ int64_t gab200_forward_device_fov(const gab200_forward_args* args, const float* 
                                   void* stream);
 int32_t gab200_backward_device_fov(const gab200_backward_args* args, const float* tanfov, void* stream);
 
+/* Forward whose blend also writes the display image: out_rgb8, a DEVICE uint8 [H,W,3] (row-major, RGB interleaved),
+ * quantised as the reference's render.py does before it saves or shows a frame -- per channel of the float pixel c
+ * (the value out_color receives), q = (uint8) clamp(c * 255 + 0.5, 0, 255) with the multiply and the add rounded
+ * separately and truncation on the cast, i.e. torch's mul(255).add_(0.5).clamp_(0, 255).permute(1, 2, 0).to(uint8)
+ * of out_color, bit for bit.  It is written by the forward blend itself: 3 bytes per pixel instead of 12, no extra
+ * pass, and a D2H copy of the frame is a quarter of the float image's.
+ * args->out_color may be NULL only when out_rgb8 is not NULL and args->need_backward == 0 (the float image is then
+ * not written at all); any other NULL output is GAB200_ERR_INVALID_ARGUMENT.  tanfov: as gab200_forward_device_fov
+ * (NULL: args->tanfovx / tanfovy).  out_rgb8 == NULL: exactly gab200_forward_device_fov.  Every sync mode is
+ * supported; a frame the library re-enqueues (GAB200_SYNC_LATE) rewrites out_rgb8 with the EXACT frame's bytes. */
+int64_t gab200_forward_display(const gab200_forward_args* args, const float* tanfov, uint8_t* out_rgb8,
+                               gab200_frame_state* state_out, void* stream);
+
 /* Frustum test only.  Replaces diff_gaussian_rasterization._C.mark_visible (GaussianRasterizer.markVisible). */
 int32_t gab200_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,
                             uint8_t* present /* [P] 0/1 */, void* stream);
