@@ -182,10 +182,15 @@ def timestep_tensor(timestep: Union[int, torch.Tensor], T: int, device) -> torch
         if timestep.device != device or timestep.dtype != torch.int32 or timestep.numel() != 1:
             raise TypeError(f"a tensor timestep must be one int32 on {device}")
         return timestep
+    return torch.full((1,), check_timestep(timestep, T), dtype=torch.int32, device=device)
+
+
+def check_timestep(timestep, T: int) -> int:
+    """A host timestep as an int, checked against [0, T)."""
     t = int(timestep)
     if not 0 <= t < T:
         raise IndexError(f"timestep {t} outside [0, {T})")
-    return torch.full((1,), t, dtype=torch.int32, device=device)
+    return t
 
 
 def flame_pose(lbs: FlameLBS, flame_param: Dict[str, torch.Tensor], timestep: Union[int, torch.Tensor]):

@@ -49,7 +49,7 @@ from .renderer import _forward_only, render
 from .rasterizer import l1_loss_u8
 from .densify import add_densification_stats
 from .training import Adam, binding_regularizers, photometric_loss
-from .flame import flame_pose
+from .flame import check_timestep, flame_pose
 
 _STATS = ("xyz_gradient_accum", "denom", "max_radii2D")
 _FLAME_KEYS = ("shape", "static_offset", "expr", "rotation", "neck_pose", "jaw_pose", "eyes_pose", "translation")
@@ -127,7 +127,171 @@ def reduced_grads(buffers, k):
     return buffers[1 - k].all_views[0]
 
 
-class GraphedFrame:
+class _Captured:
+    """What a frame captured into one CUDA graph owns, whether it trains (GraphedFrame) or plays back (GraphedRender):
+    the static camera block, the pose input (a device FLAME timestep, or vertices), the instance capacity -- sized by
+    eager warm-up frames, guarded by the sticky overflow flag of the capture slot, grown by regrow() -- and the key of
+    what the capture baked in, which run() compares to know when to re-capture.  A subclass provides `_body(captured)`,
+    `_release()` (drop what the warm-up frames left behind), `_before_capture()` and `_after_capture()`, and extends
+    `_state_key()` with what only its own capture bakes in."""
+
+    def __init__(self, pc, width, height, fovx, fovy, bg, per_camera_fov, capacity, headroom, warm_cameras,
+                 warm_timesteps=None, verts_grad=False):
+        self.pc, self.W, self.H, self.fovx, self.fovy = pc, int(width), int(height), float(fovx), float(fovy)
+        self.per_camera_fov = bool(per_camera_fov)
+        self.headroom, self._capacity = float(headroom), capacity
+        dev = pc._xyz.device
+        self.device = dev
+        self.bg = bg.to(dev).float().contiguous()
+        self.cam = torch.zeros(CAMERA_BLOCK_FOV if self.per_camera_fov else CAMERA_BLOCK, dtype=torch.float32,
+                               device=dev)
+        if self.per_camera_fov:
+            self.cam[CAMERA_BLOCK:] = tanfov_floats(self.fovx, self.fovy).to(dev)
+        self.camera = _GraphCamera(self.W, self.H, self.fovx, self.fovy, self.cam)
+        self.flame = getattr(pc, "flame", None)
+        if self.flame is not None:   # the pose is computed inside the graph from this timestep
+            self.verts, self.timestep = None, torch.zeros(1, dtype=torch.int32, device=dev)
+            self.num_timesteps = int(pc.flame_param["expr"].shape[0])
+        else:   # verts_grad: the backward reaches the vertices, which the model must then have
+            rest = pc.verts_rest if verts_grad else getattr(pc, "verts_rest", None)
+            self.verts = None if rest is None else rest.detach().clone().contiguous().requires_grad_(verts_grad)
+            self.timestep = None
+        self._warm = None if warm_cameras is None else [self._camera_tensor(c) for c in warm_cameras]
+        self._warm_t = None if warm_timesteps is None or self.flame is None else [int(t) for t in warm_timesteps]
+        self.graph = self.slot = self._key = None
+        self.replays = self.captures = 0
+
+    def _camera_tensor(self, camera):
+        """A camera object or block as this frame's block: 37 floats with per_camera_fov, else as given."""
+        blk = camera if isinstance(camera, torch.Tensor) else camera_block(camera, fov=self.per_camera_fov)
+        if self.per_camera_fov and blk.numel() != CAMERA_BLOCK_FOV:
+            raise ValueError(f"a {type(self).__name__} camera block with the field of view has {CAMERA_BLOCK_FOV} "
+                             f"floats (camera_block(cam, fov=True)), got {blk.numel()}")
+        return blk
+
+    def _set_pose_input(self, verts, timestep):
+        """The checks of set_inputs' pose arguments; writes the timestep (a host int checked against the model's
+        number of timesteps) into the device int32 the replay reads."""
+        if verts is not None and self.flame is not None:
+            raise ValueError("this frame poses its FLAME head itself: give set_inputs(timestep=...), not verts")
+        if timestep is not None:
+            if self.flame is None:
+                raise ValueError("timestep= needs a model with a FLAME head (pc.flame)")
+            self.timestep.fill_(check_timestep(timestep, self.num_timesteps))
+
+    def _pose(self):
+        """The model's face frame from the FLAME pose of the device timestep, or from the given vertices."""
+        pc = self.pc
+        if self.flame is not None:
+            verts, pc.verts_cano = flame_pose(self.flame, pc.flame_param, self.timestep)
+            pc.update_mesh_properties(verts[0])
+        elif self.verts is not None:
+            pc.update_mesh_properties(self.verts)
+
+    # ---- capture ---------------------------------------------------------------------------------------------------
+    def _learn_capacity(self):
+        """Eager frames (sync modes EXACT then LATE) over the warm-up cameras, each at every warm-up timestep: their
+        instance counts size the graph."""
+        hints = R.hints_of(self.pc)
+        key = (self.device, self.W, self.H, self.pc._xyz.shape[0])
+        n_max, lo, hi = 0, 0xFFFFFFFF, 0
+        cam0 = self.cam.clone()
+        t0 = self.timestep.clone() if self._warm_t else None
+        blocks = self._warm if self._warm else [cam0]
+        steps = self._warm_t if self._warm_t else [None]
+        # eager frames on a side stream (torch's recipe for whole-step capture): nothing autograd creates here may be
+        # tied to the legacy default stream
+        cur = torch.cuda.current_stream(self.device)
+        side = torch.cuda.Stream(device=self.device)
+        side.wait_stream(cur)
+        with torch.cuda.stream(side):
+            for rep in range(2):
+                for blk in blocks:
+                    for t in steps:
+                        self.cam.copy_(blk)
+                        if t is not None:
+                            self.timestep.fill_(t)
+                        self._body()
+                        n_max = max(n_max, int((hints.last or {}).get("num_rendered", 0)))
+                        d = hints.get(key)[1]
+                        if d[1] > d[0]:  # union of the (already widened) depth-key ranges: one bucket grid fits all
+                            lo, hi = min(lo, d[0]), max(hi, d[1])
+        cur.wait_stream(side)
+        # the frame's own camera and timestep again: the captured frame must not render the last warm-up one
+        self.cam.copy_(cam0)
+        if t0 is not None:
+            self.timestep.copy_(t0)
+        torch.cuda.synchronize(self.device)
+        self._release()
+        return n_max, ((lo, hi) if hi > lo else (0, 0))
+
+    def _room_for(self, n: int) -> int:
+        """The instance capacity of a graph whose frames need n instances."""
+        return int(n * self.headroom) + 16384
+
+    def capture(self, capacity: Optional[int] = None):
+        self.graph = None
+        self._before_capture()
+        n_max, depth = self._learn_capacity()
+        if capacity is None:
+            capacity = self._capacity if self._capacity else self._room_for(n_max)
+        self.slot = R.CaptureSlot(self.device, capacity, depth)
+        self.graph = torch.cuda.CUDAGraph()
+        R._capture_slot = self.slot
+        try:
+            with torch.cuda.graph(self.graph):
+                self._body(captured=True)
+                self.slot.flag_host.copy_(self.slot.flag, non_blocking=True)
+        finally:
+            R._capture_slot = None
+        self._after_capture()
+        self._key = self._state_key()
+        self.captures += 1
+        return self
+
+    def _state_key(self):
+        """What a capture baked in that eager code between replays may replace: P, active_sh_degree, the addresses
+        of the binding and of the parameters and, with a FLAME head, the FLAME tensors' addresses and shapes and the
+        in-place versions of shape / static_offset.  The timestep is read on the device and is not part of it."""
+        pc = self.pc
+        b = getattr(pc, "binding", None)
+        key = [int(pc._xyz.shape[0]), int(getattr(pc, "active_sh_degree", 0)), None if b is None else b.data_ptr()]
+        key += [p.data_ptr() for p in pc.parameters()]
+        if self.flame is not None:
+            for k in _FLAME_KEYS:
+                t = pc.flame_param.get(k)
+                key.append(None if t is None else (t.data_ptr(), tuple(t.shape)) +
+                           ((t._version,) if k in ("shape", "static_offset") else ()))
+        return key
+
+    def _stale(self) -> bool:
+        """No graph yet, or the model no longer matches what the capture baked in (host-side compare: no sync).  A
+        frame whose key is None never re-captures."""
+        return self.graph is None or (self._key is not None and self._state_key() != self._key)
+
+    # ---- overflow --------------------------------------------------------------------------------------------------
+    def overflowed(self, wait: bool = True) -> bool:
+        """True if any replay since the last (re-)capture needed more than the captured capacity."""
+        if self.slot is None:
+            return False
+        if wait:
+            torch.cuda.current_stream(self.device).synchronize()
+        return bool(int(self.slot.flag_host[0]) != 0)
+
+    def counters(self) -> dict:
+        """Frame counters of the most recent finished replay (host copy; synchronise first for an exact answer)."""
+        c = self.slot.counters
+        return dict(num_rendered=int(c[R.N.CTR_NUM_RENDERED]) & 0xFFFFFFFF, capacity=int(c[R.N.CTR_CAPACITY]) & 0xFFFFFFFF,
+                    bucket_overflow=int(c[R.N.CTR_BUCKET_OVERFLOW]), listed=int(c[R.N.CTR_NUM_LISTED]) & 0xFFFFFFFF)
+
+    def regrow(self):
+        """Re-capture with the capacity the overflowing frame asked for (x headroom) and a fresh depth range."""
+        torch.cuda.synchronize(self.device)
+        need = self.counters()["num_rendered"]
+        self.capture(capacity=max(self._room_for(need), int(self.slot.capacity * 1.5)))
+
+
+class GraphedFrame(_Captured):
     def __init__(self, pc, width: int, height: int, fovx: float, fovy: float, bg: torch.Tensor, loss: str = "l1_u8",
                  lambda_dssim: float = 0.2, host_inputs: bool = False, capacity: Optional[int] = None,
                  headroom: float = 1.25, after_backward=None, warm_cameras=None, regularizers: Optional[dict] = None,
@@ -171,39 +335,22 @@ class GraphedFrame:
         part of what triggers a re-capture."""
         if loss not in ("l1_u8", "photometric", "dL_dimage"):
             raise ValueError("loss must be 'l1_u8', 'photometric' or 'dL_dimage'")
-        self.pc, self.W, self.H, self.fovx, self.fovy = pc, int(width), int(height), float(fovx), float(fovy)
-        self.per_camera_fov = bool(per_camera_fov)
-        nblk = CAMERA_BLOCK_FOV if self.per_camera_fov else CAMERA_BLOCK
+        if regularizers is not None and loss == "dL_dimage":
+            raise ValueError("regularizers need a scalar loss ('l1_u8' or 'photometric')")
+        if optimizer is not None and not (isinstance(optimizer, Adam) and
+                                          all(g.get("capturable", False) for g in optimizer.param_groups)):
+            raise ValueError("optimizer must be a gaussianavatars_b200.Adam with capturable=True")
+        super().__init__(pc, width, height, fovx, fovy, bg, per_camera_fov, capacity, headroom, warm_cameras,
+                         verts_grad=True)
         self.loss_kind, self.lambda_dssim, self.host_inputs = loss, float(lambda_dssim), bool(host_inputs)
         self.after_backward = after_backward
         self.before_backward = before_backward   # e.g. SymmetricGradBuffer.begin
         self.side_work = side_work
         self.side_work_at = side_work_at   # "start": beside the whole frame; "backward": forked after the forward
         self.regularizers = regularizers
-        if regularizers is not None and loss == "dL_dimage":
-            raise ValueError("regularizers need a scalar loss ('l1_u8' or 'photometric')")
-        if optimizer is not None and not (isinstance(optimizer, Adam) and
-                                          all(g.get("capturable", False) for g in optimizer.param_groups)):
-            raise ValueError("optimizer must be a gaussianavatars_b200.Adam with capturable=True")
         self.optimizer = optimizer
         self.densify_stats = bool(densify_stats)
-        self._key = None
-        self.headroom = float(headroom)
-        dev = pc._xyz.device
-        self.device = dev
-        self.bg = bg.to(dev).float().contiguous()
-        self.cam = torch.zeros(nblk, dtype=torch.float32, device=dev)
-        if self.per_camera_fov:
-            self.cam[CAMERA_BLOCK:] = tanfov_floats(self.fovx, self.fovy).to(dev)
-        self.camera = _GraphCamera(self.W, self.H, self.fovx, self.fovy, self.cam)
-        self.flame = getattr(pc, "flame", None)
-        if self.flame is not None:   # the pose is computed inside the graph from this timestep
-            self.verts = None
-            self.timestep = torch.zeros(1, dtype=torch.int32, device=dev)
-            self.num_timesteps = int(pc.flame_param["expr"].shape[0])
-        else:
-            self.verts = pc.verts_rest.detach().clone().contiguous().requires_grad_(True)
-            self.timestep = None
+        dev, nblk = self.device, self.cam.numel()
         self.gt = torch.zeros((3, self.H, self.W), dtype=torch.uint8, device=dev) if loss != "dL_dimage" else None
         self.dL_dimage = torch.zeros((3, self.H, self.W), dtype=torch.float32, device=dev) if loss == "dL_dimage" else None
         self.cam_host = torch.zeros(nblk, dtype=torch.float32).pin_memory() if host_inputs else None  # staging
@@ -217,38 +364,14 @@ class GraphedFrame:
         self.loss_host = torch.zeros((), dtype=torch.float32).pin_memory()
         self.loss = None
         self.image = self.radii = self.viewspace_points = None
-        self.graph = None
-        self.slot = None
-        self.replays = 0
-        self.captures = 0
         self._side = torch.cuda.Stream(device=dev) if (host_inputs or side_work is not None) else None
         self._uploads = bool(host_inputs)
-        self._capacity = capacity
-        self._warm = list(warm_cameras) if warm_cameras is not None else None
-        if self.per_camera_fov and self._warm is not None:
-            self._warm = [self._camera_tensor(c) for c in self._warm]
-
-    def _camera_tensor(self, camera):
-        """A camera object or block as this frame's block: 37 floats with per_camera_fov, else as given."""
-        blk = camera if isinstance(camera, torch.Tensor) else camera_block(camera, fov=self.per_camera_fov)
-        if self.per_camera_fov and blk.numel() != CAMERA_BLOCK_FOV:
-            raise ValueError(f"per_camera_fov=True: a camera block has {CAMERA_BLOCK_FOV} floats "
-                             f"(camera_block(cam, fov=True)), got {blk.numel()}")
-        return blk
 
     # ---- inputs ------------------------------------------------------------------------------------------------
     def set_inputs(self, camera=None, verts=None, gt_u8=None, dL_dimage=None, timestep=None):
         """Copies new inputs into the static buffers (device tensors) / staging buffers (host_inputs).  `timestep`
         (a model with a FLAME head only) is a host int checked against the model's number of timesteps."""
-        if verts is not None and self.flame is not None:
-            raise ValueError("this frame poses its FLAME head itself: give set_inputs(timestep=...), not verts")
-        if timestep is not None:
-            if self.flame is None:
-                raise ValueError("timestep= needs a model with a FLAME head (pc.flame)")
-            t = int(timestep)
-            if not 0 <= t < self.num_timesteps:
-                raise IndexError(f"timestep {t} outside [0, {self.num_timesteps})")
-            self.timestep.fill_(t)
+        self._set_pose_input(verts, timestep)
         if camera is not None:
             blk = self._camera_tensor(camera)
             if blk.device.type == "cpu" and self._uploads:
@@ -303,8 +426,9 @@ class GraphedFrame:
             ps += [self.pc.flame_param[k] for k in _FLAME_KEYS[2:] if self.pc.flame_param[k].requires_grad]
         return ps
 
-    def _body(self, train: bool = False):
-        """One frame; with `train` (the captured step only) also the statistics and the optimizer step."""
+    def _body(self, captured: bool = False):
+        """One frame; `captured` (the graph, not the warm-up frames) also accumulates the statistics and steps the
+        optimizer."""
         pc = self.pc
         for p in self._params():
             p.grad = None
@@ -322,11 +446,7 @@ class GraphedFrame:
                         other.gt.copy_(other.gt_stage, non_blocking=True)
                 if self.side_work is not None and self.side_work_at == "start":
                     self.side_work()
-        if self.flame is not None:
-            verts, pc.verts_cano = flame_pose(self.flame, pc.flame_param, self.timestep)
-            pc.update_mesh_properties(verts[0])
-        else:
-            pc.update_mesh_properties(self.verts)
+        self._pose()
         out = render(self.camera, pc, _Pipe, self.bg)
         img = out["render"]
         if self.loss_kind in ("l1_u8", "photometric"):
@@ -347,7 +467,7 @@ class GraphedFrame:
             img.backward(self.dL_dimage)
         if self.after_backward is not None:
             self.after_backward()
-        if train:
+        if captured:
             skip = self.slot.flag
             if self.densify_stats:
                 add_densification_stats(pc, out["viewspace_points"], out["radii"], skip_flag=skip)
@@ -367,51 +487,35 @@ class GraphedFrame:
                 self.side_work()
 
     # ---- capture ---------------------------------------------------------------------------------------------------
-    def _learn_capacity(self):
-        """Eager frames (sync modes EXACT then LATE) over the warm-up cameras: their instance counts size the graph."""
-        hints = R.hints_of(self.pc)
-        key = (self.device, self.W, self.H, self.pc._xyz.shape[0])
-        n_max, lo, hi = 0, 0xFFFFFFFF, 0
-        cam0 = self.cam.clone()
-        blocks = self._warm if self._warm else [cam0]
-        # eager frames on a side stream (torch's recipe for whole-step capture): nothing autograd creates here may be
-        # tied to the legacy default stream
-        cur = torch.cuda.current_stream(self.device)
-        side = torch.cuda.Stream(device=self.device)
-        side.wait_stream(cur)
-        with torch.cuda.stream(side):
-            for rep in range(2):
-                for blk in blocks:
-                    self.cam.copy_(blk)
-                    self._body()
-                    info = hints.last or {}
-                    n_max = max(n_max, int(info.get("num_rendered", 0)))
-                    d = hints.get(key)[1]
-                    if d[1] > d[0]:  # union of the (already widened) depth-key ranges: one bucket grid fits every camera
-                        lo, hi = min(lo, d[0]), max(hi, d[1])
-        cur.wait_stream(side)
-        self.cam.copy_(cam0)   # the frame's own camera again: the captured step must not train on the last warm one
-        torch.cuda.synchronize(self.device)
-        # release what the eager frames left on the model / on this object (tensors with autograd history)
+    def _release(self):
+        """What the warm-up frames left on the model / on this object: tensors with autograd history."""
         self.pc.face_center = self.pc.face_orien_mat = self.pc.face_scaling = None
         if self.flame is not None:
             self.pc.verts_cano = None
         self.image = self.radii = self.viewspace_points = self.loss = None
-        return n_max, ((lo, hi) if hi > lo else (0, 0))
+
+    def _before_capture(self):
+        if self.optimizer is not None:
+            self.optimizer.init_state()   # created inside the capture, the state would be re-zeroed by every replay
+
+    def _after_capture(self):
+        # the tensors autograd left in .grad during the capture ARE the graph's outputs: remember them, a second
+        # GraphedFrame of the same model re-points .grad at its own when it captures
+        self.grads = [p.grad for p in self._params()]
+        self.flat_grad = getattr(self.pc, "flat_grad", None)
 
     def _state_key(self):
-        """Everything a training capture baked in that eager code between replays may replace."""
+        """Everything a training capture baked in that eager code between replays may replace: beyond the shared key,
+        which FLAME tensors receive gradients, the statistics, every group's hyper-parameters and the addresses of
+        every moment and step.  None for a frame that neither trains nor poses a FLAME head: it never re-captures."""
         pc = self.pc
-        b = getattr(pc, "binding", None)
-        key = [int(pc._xyz.shape[0]), int(getattr(pc, "active_sh_degree", 0)), None if b is None else b.data_ptr()]
-        key += [p.data_ptr() for p in self._params()]
+        if self.optimizer is None and not self.densify_stats and self.flame is None:
+            return None
+        key = super()._state_key()
+        if self.flame is not None:
+            key += [t is not None and t.requires_grad for t in map(pc.flame_param.get, _FLAME_KEYS)]
         if self.densify_stats:
             key += [getattr(pc, n).data_ptr() for n in _STATS]
-        if self.flame is not None:   # the timestep is read on the device and is not part of the key
-            for k in _FLAME_KEYS:
-                t = pc.flame_param.get(k)
-                key.append(None if t is None else (t.data_ptr(), tuple(t.shape), bool(t.requires_grad)) +
-                           ((t._version,) if k in ("shape", "static_offset") else ()))
         opt = self.optimizer
         if opt is not None:
             for g in opt.param_groups:
@@ -422,86 +526,36 @@ class GraphedFrame:
                     st = opt.state.get(p, {})
                     key.append((p.data_ptr(), p.shape) + tuple(st[k].data_ptr() for k in ("step", "exp_avg", "exp_avg_sq")
                                                                if k in st))
-        return tuple(key)
-
-    def capture(self, capacity: Optional[int] = None):
-        dev = self.device
-        training = self.optimizer is not None or self.densify_stats
-        if self.optimizer is not None:
-            self.optimizer.init_state()   # created inside the capture, the state would be re-zeroed by every replay
-        n_max, depth = self._learn_capacity()
-        if capacity is None:
-            capacity = self._capacity if self._capacity else int(n_max * self.headroom) + 16384
-        self.slot = R.CaptureSlot(dev, capacity, depth)
-        self.graph = torch.cuda.CUDAGraph()
-        R._capture_slot = self.slot
-        try:
-            with torch.cuda.graph(self.graph):
-                self._body(train=training)
-                self.slot.flag_host.copy_(self.slot.flag, non_blocking=True)
-        finally:
-            R._capture_slot = None
-        # the tensors autograd left in .grad during the capture ARE the graph's outputs: remember them, a second
-        # GraphedFrame of the same model re-points .grad at its own when it captures
-        self.grads = [p.grad for p in self._params()]
-        self.flat_grad = getattr(self.pc, "flat_grad", None)
-        self._key = self._state_key() if (training or self.flame is not None) else None
-        self.captures += 1
-        return self
+        return key
 
     # ---- replay ----------------------------------------------------------------------------------------------------
     def run(self, check: bool = False):
-        if self.graph is None:
-            self.capture()
-        elif self._key is not None and self._state_key() != self._key:   # host-side compare: no sync
-            self.graph = None
+        if self._stale():
             self.capture()
         if self._gt_ready is not None:   # a ground-truth upload is in flight on the copy stream
             torch.cuda.current_stream(self.device).wait_event(self._gt_ready)
             self._gt_ready = None
-        self.graph.replay()
-        self.replays += 1
+        self._replay()
         if self._uploads:
             self._done = torch.cuda.Event()
             self._done.record()
-        for p, g in zip(self._params(), self.grads):
-            p.grad = g
-        self.pc.flat_grad = self.flat_grad
         if check and self.overflowed(wait=True):
             self.regrow()
-            self.graph.replay()
-            self.replays += 1
-            for p, g in zip(self._params(), self.grads):
-                p.grad = g
-            self.pc.flat_grad = self.flat_grad
+            self._replay()
             if self.overflowed(wait=True):
                 raise RuntimeError("GraphedFrame: the frame still overflows its instance capacity after re-capture")
         return self
 
-    def overflowed(self, wait: bool = True) -> bool:
-        """True if any replay since the last (re-)capture needed more than the captured capacity."""
-        if self.slot is None:
-            return False
-        if wait:
-            torch.cuda.current_stream(self.device).synchronize()
-        return bool(int(self.slot.flag_host[0]) != 0)
-
-    def counters(self) -> dict:
-        """Frame counters of the most recent finished replay (host copy; synchronise first for an exact answer)."""
-        c = self.slot.counters
-        return dict(num_rendered=int(c[R.N.CTR_NUM_RENDERED]) & 0xFFFFFFFF, capacity=int(c[R.N.CTR_CAPACITY]) & 0xFFFFFFFF,
-                    bucket_overflow=int(c[R.N.CTR_BUCKET_OVERFLOW]), listed=int(c[R.N.CTR_NUM_LISTED]) & 0xFFFFFFFF)
-
-    def regrow(self):
-        """Re-capture with the capacity the overflowing frame asked for (x headroom) and a fresh depth range."""
-        torch.cuda.synchronize(self.device)
-        need = self.counters()["num_rendered"]
-        cap = max(int(need * self.headroom) + 16384, int(self.slot.capacity * 1.5))
-        self.graph = None
-        self.capture(capacity=cap)
+    def _replay(self):
+        """One replay, counted, with .grad pointing at this graph's gradients again."""
+        self.graph.replay()
+        self.replays += 1
+        for p, g in zip(self._params(), self.grads):
+            p.grad = g
+        self.pc.flat_grad = self.flat_grad
 
 
-class GraphedRender:
+class GraphedRender(_Captured):
     """One PLAYBACK frame as ONE forward-only CUDA graph: what the reference's render.py, the fps benchmarks and the
     viewer run per frame (select_mesh_by_timestep(t) -> render() -> the uint8 frame), with no backward, no loss and
     no ground truth.
@@ -546,54 +600,21 @@ class GraphedRender:
             raise ValueError("outputs must be 'u8', 'float' or 'both'")
         if host_slots < 0 or (host_slots > 0 and outputs == "float"):
             raise ValueError("host_slots copies the display image: it needs outputs 'u8' or 'both'")
-        self.pc, self.W, self.H = pc, int(width), int(height)
+        # the background is an input (set_inputs writes it): the frame's own copy.  Field of view: tan(45 deg), a
+        # harmless one until the first camera arrives
+        super().__init__(pc, width, height, math.pi / 2, math.pi / 2, bg.clone(), True, capacity, headroom,
+                         warm_cameras, warm_timesteps)
         self.outputs, self.scaling_modifier, self.mesh_update = outputs, float(scaling_modifier), bool(mesh_update)
-        self.headroom, self._capacity = float(headroom), capacity
-        dev = pc._xyz.device
-        self.device = dev
-        self.bg = bg.to(dev).float().contiguous().clone()
-        self.cam = torch.zeros(CAMERA_BLOCK_FOV, dtype=torch.float32, device=dev)
-        self.cam[CAMERA_BLOCK:] = 1.0   # tan(45 deg): a harmless field of view until the first camera arrives
-        self.camera = _GraphCamera(self.W, self.H, math.pi / 2, math.pi / 2, self.cam)
-        self.flame = getattr(pc, "flame", None)
-        if self.flame is not None:
-            self.verts = None
-            self.timestep = torch.zeros(1, dtype=torch.int32, device=dev)
-            self.num_timesteps = int(pc.flame_param["expr"].shape[0])
-        else:
-            rest = getattr(pc, "verts_rest", None)
-            self.verts = None if rest is None else rest.detach().clone().contiguous()
-            self.timestep = None
-        self._warm = None if warm_cameras is None else [self._camera_tensor(c) for c in warm_cameras]
-        self._warm_t = None if warm_timesteps is None or self.flame is None else [int(t) for t in warm_timesteps]
         self.host_slots = int(host_slots)
         self.host = self._copy_stream = None
         self._staged = self._host_events = self._stage_events = None
         self.image = self.display = self.radii = None
-        self.graph = self.slot = self._key = None
-        self.replays = self.captures = 0
-
-    @staticmethod
-    def _camera_tensor(camera):
-        blk = camera if isinstance(camera, torch.Tensor) else camera_block(camera, fov=True)
-        if blk.numel() != CAMERA_BLOCK_FOV:
-            raise ValueError(f"a GraphedRender camera block has {CAMERA_BLOCK_FOV} floats "
-                             f"(camera_block(cam, fov=True)), got {blk.numel()}")
-        return blk
 
     # ---- inputs ------------------------------------------------------------------------------------------------
     def set_inputs(self, camera=None, timestep=None, verts=None, bg=None):
         """Copies new inputs into the graph's device buffers; none of them re-captures.  A camera OBJECT of another
         image size changes the frame's size (the next run() re-captures)."""
-        if verts is not None and self.flame is not None:
-            raise ValueError("this frame poses its FLAME head itself: give set_inputs(timestep=...), not verts")
-        if timestep is not None:
-            if self.flame is None:
-                raise ValueError("timestep= needs a model with a FLAME head (pc.flame)")
-            t = int(timestep)
-            if not 0 <= t < self.num_timesteps:
-                raise IndexError(f"timestep {t} outside [0, {self.num_timesteps})")
-            self.timestep.fill_(t)
+        self._set_pose_input(verts, timestep)
         if camera is not None:
             blk = self._camera_tensor(camera)
             if not isinstance(camera, torch.Tensor):
@@ -609,92 +630,36 @@ class GraphedRender:
             self.bg.copy_(bg, non_blocking=True)
 
     # ---- the frame body (run eagerly for warm-up, then captured) -------------------------------------------------
-    def _body(self):
-        pc = self.pc
+    def _body(self, captured: bool = False):
         with torch.no_grad():
             if self.mesh_update:
-                if self.flame is not None:
-                    verts, pc.verts_cano = flame_pose(self.flame, pc.flame_param, self.timestep)
-                    pc.update_mesh_properties(verts[0])
-                elif self.verts is not None:
-                    pc.update_mesh_properties(self.verts)
-            out = _forward_only(self.camera, pc, _Pipe, self.bg, self.scaling_modifier,
+                self._pose()
+            out = _forward_only(self.camera, self.pc, _Pipe, self.bg, self.scaling_modifier,
                                 self.outputs != "float", self.outputs != "u8")
         self.image, self.display, self.radii = out["render"], out["display_u8"], out["radii"]
 
-    def _learn_capacity(self):
-        """Eager frames (sync modes EXACT then LATE) over the warm-up cameras: their instance counts size the graph."""
-        hints = R.hints_of(self.pc)
-        key = (self.device, self.W, self.H, self.pc._xyz.shape[0])
-        n_max, lo, hi = 0, 0xFFFFFFFF, 0
-        cam0 = self.cam.clone()
-        t0 = None if self.timestep is None else self.timestep.clone()
-        blocks = [b.to(self.device) for b in self._warm] if self._warm else [cam0]
-        steps = self._warm_t if self._warm_t else [None]
-        cur = torch.cuda.current_stream(self.device)
-        side = torch.cuda.Stream(device=self.device)
-        side.wait_stream(cur)
-        with torch.cuda.stream(side):
-            for rep in range(2):
-                for blk in blocks:
-                    for t in steps:
-                        self.cam.copy_(blk)
-                        if t is not None:
-                            self.timestep.fill_(t)
-                        self._body()
-                        n_max = max(n_max, int((hints.last or {}).get("num_rendered", 0)))
-                        d = hints.get(key)[1]
-                        if d[1] > d[0]:
-                            lo, hi = min(lo, d[0]), max(hi, d[1])
-            self.cam.copy_(cam0)
-            if t0 is not None:
-                self.timestep.copy_(t0)
-        cur.wait_stream(side)
-        torch.cuda.synchronize(self.device)
+    # ---- capture ---------------------------------------------------------------------------------------------------
+    def _release(self):
         self.image = self.display = self.radii = None
-        return n_max, ((lo, hi) if hi > lo else (0, 0))
 
-    def _state_key(self):
-        """Everything the capture baked in that eager code between replays may replace."""
-        pc = self.pc
-        b = getattr(pc, "binding", None)
-        key = [int(pc._xyz.shape[0]), int(getattr(pc, "active_sh_degree", 0)), None if b is None else b.data_ptr(),
-               self.W, self.H, self.scaling_modifier]
-        key += [p.data_ptr() for p in pc.parameters()]
-        if self.flame is not None:
-            for k in _FLAME_KEYS:
-                t = pc.flame_param.get(k)
-                key.append(None if t is None else (t.data_ptr(), tuple(t.shape)) +
-                           ((t._version,) if k in ("shape", "static_offset") else ()))
-        if not self.mesh_update and b is not None:
-            key += [getattr(pc, n).data_ptr() for n in ("face_center", "face_orien_mat", "face_scaling")]
-        return tuple(key)
-
-    def capture(self, capacity: Optional[int] = None):
-        dev, pc = self.device, self.pc
+    def _before_capture(self):
         self.camera.image_width, self.camera.image_height = self.W, self.H
-        n_max, depth = self._learn_capacity()
-        if capacity is None:
-            capacity = self._capacity if self._capacity else int(n_max * self.headroom) + 16384
-        self.graph = None
-        self.slot = R.CaptureSlot(dev, capacity, depth)
-        self.graph = torch.cuda.CUDAGraph()
-        R._capture_slot = self.slot
-        try:
-            with torch.cuda.graph(self.graph):
-                self._body()
-                self.slot.flag_host.copy_(self.slot.flag, non_blocking=True)
-        finally:
-            R._capture_slot = None
+
+    def _after_capture(self):
         # the mesh tensors the replay writes (the model's attributes are replaced by any eager frame)
-        self._mesh = tuple(getattr(pc, n, None) for n in ("verts", "verts_cano", "face_center", "face_orien_mat",
-                                                          "face_scaling")) \
+        self._mesh = tuple(getattr(self.pc, n, None) for n in ("verts", "verts_cano", "face_center", "face_orien_mat",
+                                                               "face_scaling")) \
             if self.mesh_update else None
-        self._key = self._state_key()
         if self.host_slots:
             self._make_ring()
-        self.captures += 1
-        return self
+
+    def _state_key(self):
+        """Beyond the shared key: the image size, `scaling_modifier` and, with mesh_update=False, the addresses of
+        the face frame the graph renders."""
+        key = super()._state_key() + [self.W, self.H, self.scaling_modifier]
+        if not self.mesh_update and getattr(self.pc, "binding", None) is not None:
+            key += [getattr(self.pc, n).data_ptr() for n in ("face_center", "face_orien_mat", "face_scaling")]
+        return key
 
     def _make_ring(self):
         """Pinned host slots, two device staging copies of the display frame and their events."""
@@ -741,7 +706,7 @@ class GraphedRender:
 
     # ---- replay ----------------------------------------------------------------------------------------------------
     def run(self, check: bool = False):
-        if self.graph is None or self._state_key() != self._key:   # host-side compare: no sync
+        if self._stale():
             self.capture()
         self.graph.replay()
         if check and self.overflowed(wait=True):
@@ -753,21 +718,3 @@ class GraphedRender:
         if self.host_slots:
             self._ship()
         return self
-
-    def overflowed(self, wait: bool = True) -> bool:
-        """True if any replay since the last (re-)capture needed more than the captured capacity."""
-        if self.slot is None:
-            return False
-        if wait:
-            torch.cuda.current_stream(self.device).synchronize()
-        return bool(int(self.slot.flag_host[0]) != 0)
-
-    def counters(self) -> dict:
-        return GraphedFrame.counters(self)
-
-    def regrow(self):
-        """Re-capture with the capacity the overflowing frame asked for (x headroom) and a fresh depth range."""
-        torch.cuda.synchronize(self.device)
-        need = self.counters()["num_rendered"]
-        cap = max(int(need * self.headroom) + 16384, int(self.slot.capacity * 1.5))
-        self.capture(capacity=cap)

@@ -306,7 +306,7 @@ class _RasterizeGaussians(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                raster_settings):
+                raster_settings, hints=None):
         rs = raster_settings
         device = means3D.device
         if device.type != "cuda":
@@ -329,7 +329,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         a.means3D, a.opacities = N.ptr(means3D), N.ptr(opacities)
         a.scales, a.rotations, a.cov3D_precomp = N.ptr(scales), N.ptr(rotations), N.ptr(cov3Ds_precomp)
         a.shs, a.colors_precomp = N.ptr(sh), N.ptr(colors_precomp)
-        color, radii, st, holder = _run_forward(a, device, need_bw, _hints_for_next_call())
+        color, radii, st, holder = _run_forward(a, device, need_bw, hints)
         if need_bw:
             ctx.args, ctx.state, ctx.holder = a, st, holder
             ctx.keep = (cams, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, radii)
@@ -361,24 +361,13 @@ class _RasterizeGaussians(torch.autograd.Function):
         _run_backward(b, device)
         ctx.holder = None
         return (d_means3D, d_means2D, d_sh, d_colors if colors_precomp is not None else None, d_opac, d_scales, d_rots,
-                d_cov if cov3Ds_precomp is not None else None, None)
-
-
-_next_hints = None
-
-
-def _hints_for_next_call():
-    global _next_hints
-    h, _next_hints = _next_hints, None
-    return h
+                d_cov if cov3Ds_precomp is not None else None, None, None)
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                         raster_settings, hints: Optional[FrameHints] = None):
-    global _next_hints
-    _next_hints = hints  # autograd.Function.apply takes tensors and plain values; the hints object rides beside it
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                                     cov3Ds_precomp, raster_settings)
+                                     cov3Ds_precomp, raster_settings, hints)
 
 
 class GaussianRasterizer(nn.Module):

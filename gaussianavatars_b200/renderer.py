@@ -50,18 +50,22 @@ def _has_raw(pc):
     return all(hasattr(pc, n) for n in ("_xyz", "_rotation", "_scaling", "_opacity", "_features_dc", "_features_rest"))
 
 
+def _fused_frame(cam, pc, pipe, bg_color, scaling_modifier):
+    """The settings of a fused-route frame, the binding and the model's face frame (None without a binding)."""
+    rs = _settings(cam, pc, pipe, bg_color, scaling_modifier, pc._xyz.device)
+    binding = getattr(pc, "binding", None)
+    if binding is None:
+        return rs, None, (None, None, None)
+    if getattr(pc, "face_center", None) is None:
+        pc.select_mesh_by_timestep(0)  # as the reference getters do (scene/gaussian_model.py:119-120)
+    return rs, binding, (pc.face_center, pc.face_orien_mat, pc.face_scaling)
+
+
 def render_bound(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_color=None):
     """Fused route (see module docstring)."""
-    device = pc._xyz.device
-    rs = _settings(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, device)
-    P = pc._xyz.shape[0]
-    screenspace_points = torch.zeros((P, 3), dtype=pc._xyz.dtype, device=device, requires_grad=True)
-    binding = getattr(pc, "binding", None)
-    fc = fR = fs = None
-    if binding is not None:
-        if getattr(pc, "face_center", None) is None:
-            pc.select_mesh_by_timestep(0)  # as the reference getters do (scene/gaussian_model.py:119-120)
-        fc, fR, fs = pc.face_center, pc.face_orien_mat, pc.face_scaling
+    rs, binding, (fc, fR, fs) = _fused_frame(viewpoint_camera, pc, pipe, bg_color, scaling_modifier)
+    screenspace_points = torch.zeros((pc._xyz.shape[0], 3), dtype=pc._xyz.dtype, device=pc._xyz.device,
+                                     requires_grad=True)
     rendered_image, radii = rasterize_bound(rs, pc._xyz, pc._rotation, pc._scaling, pc._opacity, pc._features_dc,
                                             pc._features_rest, binding, fc, fR, fs, means2D=screenspace_points,
                                             colors_precomp=override_color, grad_sink=pc,
@@ -76,19 +80,13 @@ def _forward_only(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, displa
         raise ValueError("render_display needs the fused route: a model exposing the raw parameters "
                          "(_xyz, _rotation, _scaling, _opacity, _features_dc, _features_rest)")
     device = pc._xyz.device
-    rs = _settings(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, device)
-    rgb8 = torch.empty((rs.image_height, rs.image_width, 3), dtype=torch.uint8, device=device) if display else None
-    binding = getattr(pc, "binding", None)
-    fc = fR = fs = None
     d = lambda t: None if t is None else t.detach()  # noqa: E731  (no gradient: the forward keeps no backward state)
     with torch.no_grad():
-        if binding is not None:
-            if getattr(pc, "face_center", None) is None:
-                pc.select_mesh_by_timestep(0)
-            fc, fR, fs = d(pc.face_center), d(pc.face_orien_mat), d(pc.face_scaling)
+        rs, binding, (fc, fR, fs) = _fused_frame(viewpoint_camera, pc, pipe, bg_color, scaling_modifier)
+        rgb8 = torch.empty((rs.image_height, rs.image_width, 3), dtype=torch.uint8, device=device) if display else None
         img, radii = rasterize_bound(rs, d(pc._xyz), d(pc._rotation), d(pc._scaling), d(pc._opacity),
-                                     d(pc._features_dc), d(pc._features_rest), binding, fc, fR, fs, grad_sink=pc,
-                                     tanfov=getattr(viewpoint_camera, "tanfov", None), rgb8=rgb8,
+                                     d(pc._features_dc), d(pc._features_rest), binding, d(fc), d(fR), d(fs),
+                                     grad_sink=pc, tanfov=getattr(viewpoint_camera, "tanfov", None), rgb8=rgb8,
                                      float_image=float_image)
     return {"display_u8": rgb8, "render": img, "radii": radii, "visibility_filter": _visible(radii)}
 
