@@ -7,12 +7,12 @@ Nothing here falls back to CPU or eager PyTorch: the ops raise if libgaussianava
 from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, rasterize_gaussians, rasterize_bound,
                          bind_activate, set_exact_binning, face_frame, l1_loss_u8)
 from .renderer import render, render_bound, render_display
-from .training import photometric_loss, Adam, binding_regularizers, expon_lr_schedule
+from .training import photometric_loss, image_metrics, Adam, binding_regularizers, expon_lr_schedule
 from .io import load_ply, save_ply, load_flame_param, save_flame_param
 from .densify import densify_and_prune, densify_arrays, add_densification_stats
 from .flame import FlameLBS, flame_pose, flame_param_groups
 
 __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gaussians", "rasterize_bound",
            "bind_activate", "set_exact_binning", "face_frame", "l1_loss_u8", "render", "render_bound", "render_display",
-           "photometric_loss", "Adam", "binding_regularizers", "load_ply", "save_ply", "load_flame_param", "save_flame_param", "densify_and_prune", "densify_arrays",
+           "photometric_loss", "image_metrics", "Adam", "binding_regularizers", "load_ply", "save_ply", "load_flame_param", "save_flame_param", "densify_and_prune", "densify_arrays",
            "add_densification_stats", "expon_lr_schedule", "FlameLBS", "flame_pose", "flame_param_groups"]

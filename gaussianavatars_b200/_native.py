@@ -80,6 +80,19 @@ class PhotometricArgs(C.Structure):
     ]
 
 
+METRICS_FLOAT_CHW, METRICS_U8_HWC = 0, 1
+METRICS_FIELDS = 4
+
+
+class MetricsArgs(C.Structure):
+    """Mirror of gab200_metrics_args."""
+    _fields_ = [
+        ("abi_version", C.c_uint32), ("height", C.c_int32), ("width", C.c_int32), ("render_kind", C.c_int32),
+        ("render", C.c_void_p), ("gt", C.c_void_p), ("row", C.c_void_p), ("table", C.c_void_p),
+        ("table_rows", C.c_int32), ("skip_flag", C.c_void_p), ("scratch", C.c_void_p),
+    ]
+
+
 class AdamSegment(C.Structure):
     """Mirror of gab200_adam_segment."""
     _fields_ = [
@@ -177,7 +190,8 @@ EXPORTED_SYMBOLS = ("gab200_forward", "gab200_backward", "gab200_mark_visible", 
                     "gab200_regularize_forward", "gab200_regularize_backward", "gab200_nvls_allreduce", "gab200_densify_scratch_bytes", "gab200_densify_plan", "gab200_densify_apply",
                     "gab200_adam_step_device", "gab200_densify_stats", "gab200_flame_scratch_bytes",
                     "gab200_flame_prepare", "gab200_flame_forward", "gab200_flame_backward",
-                    "gab200_forward_device_fov", "gab200_backward_device_fov", "gab200_forward_display")
+                    "gab200_forward_device_fov", "gab200_backward_device_fov", "gab200_forward_display",
+                    "gab200_image_metrics", "gab200_image_metrics_scratch_bytes")
 
 _lib = None
 _lock = threading.Lock()
@@ -248,6 +262,10 @@ def lib():
         L.gab200_l1_loss_u8_backward.argtypes = [C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gab200_photometric_loss.restype = C.c_int32
         L.gab200_photometric_loss.argtypes = [C.POINTER(PhotometricArgs), C.c_void_p]
+        L.gab200_image_metrics.restype = C.c_int32
+        L.gab200_image_metrics.argtypes = [C.POINTER(MetricsArgs), C.c_void_p]
+        L.gab200_image_metrics_scratch_bytes.restype = C.c_size_t
+        L.gab200_image_metrics_scratch_bytes.argtypes = [C.c_int32, C.c_int32]
         L.gab200_adam_step.restype = C.c_int32
         L.gab200_adam_step.argtypes = [C.c_int32, C.POINTER(AdamSegment), C.c_int64, C.c_double, C.c_double,
                                        C.c_double, C.c_void_p]

@@ -32,6 +32,7 @@ SOURCES = {
     "face_frame.cu": [],
     "flame.cu": [],
     "loss.cu": [],
+    "metrics.cu": [],
     "optim.cu": [],
 }
 

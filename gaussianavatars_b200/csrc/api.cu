@@ -793,6 +793,21 @@ int32_t gab200_photometric_loss(const gab200_photometric_args* a, void* stream_)
   return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
 }
 
+size_t gab200_image_metrics_scratch_bytes(int32_t height, int32_t width) {
+  return height > 0 && width > 0 ? metrics_scratch_bytes(height, width) : 0;
+}
+
+int32_t gab200_image_metrics(const gab200_metrics_args* a, void* stream_) {
+  if (a == nullptr || a->abi_version != GAB200_ABI_VERSION || a->height <= 0 || a->width <= 0 || a->table_rows < 1 ||
+      !a->render || !a->gt || !a->table || !a->scratch || ((uintptr_t)a->scratch & 7) != 0 ||
+      (a->render_kind != GAB200_METRICS_FLOAT_CHW && a->render_kind != GAB200_METRICS_U8_HWC))
+    return GAB200_ERR_INVALID_ARGUMENT;
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  launch_image_metrics(a->height, a->width, a->render_kind, a->render, a->gt, a->row, a->table_rows, a->skip_flag,
+                       a->table, a->scratch, (cudaStream_t)stream_);
+  return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
 int32_t gab200_adam_step(int32_t num_segments, const gab200_adam_segment* segs, int64_t step, double beta1,
                          double beta2, double eps, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;

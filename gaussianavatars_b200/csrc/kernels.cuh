@@ -172,6 +172,11 @@ void launch_l1_loss_u8(int64_t n, const float* img, const uint8_t* gt, const flo
 void launch_photometric_loss(int C, int H, int W, const float* img, const void* gt, int gt_is_u8, float lambda,
                              float* grad, float* loss, float* scratch, cudaStream_t stream);
 
+// metrics.cu
+size_t metrics_scratch_bytes(int H, int W);
+void launch_image_metrics(int H, int W, int kind, const void* render, const uint8_t* gt, const int32_t* row, int rows,
+                          const int32_t* skip, float* table, void* scratch, cudaStream_t stream);
+
 // densify.cu
 size_t densify_scratch_bytes(int P, int F);
 cudaError_t launch_densify_plan(const gab200_densify_args& a, cudaStream_t stream);

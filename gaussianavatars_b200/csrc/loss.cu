@@ -5,6 +5,7 @@
 // same kernel that accumulates the loss.
 #include "common.cuh"
 #include "kernels.cuh"
+#include "ssim_tile.cuh"
 
 namespace gab {
 
@@ -85,48 +86,8 @@ void launch_l1_loss_u8(int64_t n, const float* img, const uint8_t* gt, const flo
 //   ds/dE[x^2] = -A1 A2 / (B1 B2^2)
 //   ds/dE[xy]  = 2 A1 / (B1 B2)
 
-constexpr int LT = 32;             // tile edge (outputs)
-constexpr int LHALO = 5;           // window_size // 2
-constexpr int LIN = LT + 2 * LHALO;
-constexpr int LTAPS = 2 * LHALO + 1;
-constexpr int LSEG_H = 8;          // outputs per thread, horizontal pass (168 work items per tile)
-constexpr int LLOAD_H = LSEG_H + LTAPS - 1;
-constexpr int LSEG = 4;            // outputs per thread, vertical pass (256 work items per tile)
-constexpr int LLOAD = LSEG + LTAPS - 1;
-constexpr int LROWS_PER_WARP = (LIN + 7) / 8;
-
-struct SsimWindow { float w[LTAPS]; };
-
-// value / 255 with a correctly rounded division: bit-identical to the reference's CPU-side
-// `torch.from_numpy(np.array(img)) / 255.0` (utils/general_utils.py:21-23); a multiply by 1/255 is off by one ulp
-// for some codes and flips sign(x - y).  The tile kernels divide once per code into a 256-entry shared table.
-__device__ __forceinline__ float u8_unit(uint8_t v) { return __fdiv_rn((float)v, 255.f); }
-
-template <typename GT> struct GtFetch;
-template <> struct GtFetch<uint8_t> {
-  float tab[256];
-  __device__ __forceinline__ void init(int tid) {
-    tab[tid] = u8_unit((uint8_t)tid);  // blockDim.x == 256
-    __syncthreads();
-  }
-  __device__ __forceinline__ float operator()(const uint8_t* p, int64_t i) const { return tab[p[i]]; }
-};
-template <> struct GtFetch<float> {
-  __device__ __forceinline__ void init(int) {}
-  __device__ __forceinline__ float operator()(const float* p, int64_t i) const { return p[i]; }
-};
-
-// 11-tap pass over a register window: out[o] = sum_t w[t] v[o + t]
-template <int NOUT>
-__device__ __forceinline__ void taps(const SsimWindow& win, const float (&v)[NOUT + LTAPS - 1], float (&out)[NOUT]) {
-#pragma unroll
-  for (int o = 0; o < NOUT; o++) {
-    float a = 0.f;
-#pragma unroll
-    for (int t = 0; t < LTAPS; t++) a = fmaf(win.w[t], v[o + t], a);
-    out[o] = a;
-  }
-}
+// The tile geometry (LT, LHALO, ...), SsimWindow, u8_unit, GtFetch and taps live in ssim_tile.cuh, shared with the
+// forward-only image metrics (metrics.cu).
 
 template <typename GT>
 __global__ void __launch_bounds__(256) ssim_stats_kernel(int H, int W, const float* __restrict__ img,
@@ -345,17 +306,7 @@ __global__ void __launch_bounds__(256) ssim_grad_kernel(int H, int W, const floa
 template <typename GT>
 static void launch_photometric_t(int C, int H, int W, const float* img, const GT* gt, float lambda, float* grad,
                                  float* loss, float* scratch, cudaStream_t stream) {
-  SsimWindow win;
-  {  // gaussian(11, 1.5) of utils/loss_utils.py:23-25, in float like the reference's torch.Tensor
-    // (the float32 taps are summed in double and rounded once: that reproduces torch.Tensor.sum()'s value)
-    float g[LTAPS];
-    double sum = 0.0;
-    for (int i = 0; i < LTAPS; i++) {
-      g[i] = (float)exp(-(double)((i - LHALO) * (i - LHALO)) / (2.0 * 1.5 * 1.5));
-      sum += (double)g[i];
-    }
-    for (int i = 0; i < LTAPS; i++) win.w[i] = g[i] / (float)sum;
-  }
+  const SsimWindow win = ssim_window();
   const int64_t n = (int64_t)C * H * W;
   const dim3 grid((W + LT - 1) / LT, (H + LT - 1) / LT, C);
   double* sums = reinterpret_cast<double*>(scratch);  // [2], zeroed by the caller (api.cu); the maps follow

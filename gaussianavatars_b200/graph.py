@@ -44,11 +44,12 @@ from typing import Optional
 
 import torch
 
+from . import _native as N
 from . import rasterizer as R
 from .renderer import _forward_only, render
 from .rasterizer import l1_loss_u8
 from .densify import add_densification_stats
-from .training import Adam, binding_regularizers, photometric_loss
+from .training import METRIC_NAMES, Adam, binding_regularizers, launch_image_metrics, metrics_scratch, photometric_loss
 from .flame import check_timestep, flame_pose
 
 _STATS = ("xyz_gradient_accum", "denom", "max_radii2D")
@@ -160,6 +161,8 @@ class _Captured:
         self._warm_t = None if warm_timesteps is None or self.flame is None else [int(t) for t in warm_timesteps]
         self.graph = self.slot = self._key = None
         self.replays = self.captures = 0
+        self._side = None                    # copy stream of host-input uploads (a subclass creates it)
+        self._gt_ready = self._done = None   # events ordering an upload against the replays that read its buffer
 
     def _camera_tensor(self, camera):
         """A camera object or block as this frame's block: 37 floats with per_camera_fov, else as given."""
@@ -187,6 +190,27 @@ class _Captured:
             pc.update_mesh_properties(verts[0])
         elif self.verts is not None:
             pc.update_mesh_properties(self.verts)
+
+    # ---- host inputs -----------------------------------------------------------------------------------------------
+    def _upload(self, dst, src_host):
+        """H2D on the copy stream: after the last replay that read `dst`, concurrently with the main stream."""
+        if self._done is not None:
+            self._side.wait_event(self._done)
+        with torch.cuda.stream(self._side):
+            dst.copy_(src_host, non_blocking=True)
+            self._gt_ready = torch.cuda.Event()
+            self._gt_ready.record(self._side)
+
+    def _await_upload(self):
+        """The main stream waits for an upload in flight on the copy stream (before the replay that reads it)."""
+        if self._gt_ready is not None:
+            torch.cuda.current_stream(self.device).wait_event(self._gt_ready)
+            self._gt_ready = None
+
+    def _mark_read(self):
+        """Records that the replays enqueued so far have read the uploaded buffers: the next upload waits for it."""
+        self._done = torch.cuda.Event()
+        self._done.record()
 
     # ---- capture ---------------------------------------------------------------------------------------------------
     def _learn_capacity(self):
@@ -360,7 +384,6 @@ class GraphedFrame(_Captured):
         self.gt_stage = (torch.zeros((3, self.H, self.W), dtype=torch.uint8).pin_memory()
                          if host_inputs and self.gt is not None else None)
         self._prefetch_target = None
-        self._gt_ready = self._done = None   # events ordering the ground-truth upload against the replays
         self.loss_host = torch.zeros((), dtype=torch.float32).pin_memory()
         self.loss = None
         self.image = self.radii = self.viewspace_points = None
@@ -408,15 +431,6 @@ class GraphedFrame(_Captured):
         self.cam.copy_(self.cam_stage, non_blocking=True)
         if self.gt_stage is not None:
             self.gt.copy_(self.gt_stage, non_blocking=True)
-
-    def _upload(self, dst, src_host):
-        """H2D on the copy stream: after the last replay that read `dst`, concurrently with the main stream."""
-        if self._done is not None:
-            self._side.wait_event(self._done)
-        with torch.cuda.stream(self._side):
-            dst.copy_(src_host, non_blocking=True)
-            self._gt_ready = torch.cuda.Event()
-            self._gt_ready.record(self._side)
 
     # ---- the step body (run eagerly for warm-up, then captured) --------------------------------------------------
     def _params(self):
@@ -532,13 +546,10 @@ class GraphedFrame(_Captured):
     def run(self, check: bool = False):
         if self._stale():
             self.capture()
-        if self._gt_ready is not None:   # a ground-truth upload is in flight on the copy stream
-            torch.cuda.current_stream(self.device).wait_event(self._gt_ready)
-            self._gt_ready = None
+        self._await_upload()   # a ground-truth upload in flight on the copy stream
         self._replay()
         if self._uploads:
-            self._done = torch.cuda.Event()
-            self._done.record()
+            self._mark_read()
         if check and self.overflowed(wait=True):
             self.regrow()
             self._replay()
@@ -718,3 +729,123 @@ class GraphedRender(_Captured):
         if self.host_slots:
             self._ship()
         return self
+
+
+class GraphedEval(GraphedRender):
+    """One EVALUATION view as ONE forward-only CUDA graph: a GraphedRender whose captured body ends in the image
+    metrics of the rendered view against its ground truth (training.image_metrics, gab200_image_metrics), written into
+    row `view` of a (views, 4) device table {l1, psnr, psnr_all, ssim}.  What the reference evaluates per val / test
+    view, in training_report (train.py:256-309: select_mesh_by_timestep -> render -> clamp -> l1_loss, psnr, ssim) and
+    in render.py + metrics.py (the PNG bytes of every view -> ssim, psnr):
+
+        ev = GraphedEval(pc, width, height, bg, views=len(cams), source="float", warm_cameras=cams)
+        for i, cam in enumerate(cams):
+            ev.set_inputs(camera=cam, timestep=cam.timestep, gt_u8=gt[i], view=i)   # device buffers: no re-capture
+            ev.run()                                                                # enqueue one replay
+        s = ev.scores()                    # one synchronisation: s["per_view"], s["l1"], s["psnr"], s["ssim"] ...
+
+    source="float": the graph renders the float image and scores it as train.py does (clamped to [0, 1]; psnr is the
+    mean of the three per-channel PSNRs).  source="u8": it renders the display image only (render.py's bytes) and
+    scores those as metrics.py reads them back (value/255); `psnr_all` is metrics.py's PSNR (one MSE over all
+    values).  With host_slots (source="u8" only) each replay also ships its display frame to the pinned host ring, so
+    one replay yields both the PNG bytes render.py would write and the view's scores.
+
+    camera, timestep, background, ground truth and view index are device buffers written by set_inputs: none of them
+    re-captures.  A HOST ground truth (pinned, for an upload that overlaps the replays) travels on a copy stream the
+    next replay waits for.  What re-captures is exactly what re-captures a GraphedRender.  The capacity is sized and
+    guarded as there; a replay that overflowed its capacity writes no row (the metrics launch reads the slot's sticky
+    overflow flag), so a truncated render never produces a score: `scores()` then raises, naming the rows to redo
+    after `regrow()`.  `run(check=True)` re-captures and replays an overflowing view at once.  The rendered images
+    stay in `image` / `display` for what this graph does not compute (LPIPS)."""
+
+    def __init__(self, pc, width: int, height: int, bg: torch.Tensor, views: int, source: str = "float",
+                 host_slots: int = 0, capacity: Optional[int] = None, headroom: float = 1.25, warm_cameras=None,
+                 warm_timesteps=None):
+        if source not in ("float", "u8"):
+            raise ValueError("source must be 'float' (train.py's evaluation of the float render) or 'u8' (the "
+                             "display bytes render.py writes, scored as metrics.py reads them)")
+        if host_slots and source != "u8":
+            raise ValueError("host_slots ships the display image: it needs source='u8'")
+        if int(views) < 1:
+            raise ValueError("views must be at least 1")
+        super().__init__(pc, width, height, bg, outputs="float" if source == "float" else "u8", host_slots=host_slots,
+                         capacity=capacity, headroom=headroom, warm_cameras=warm_cameras, warm_timesteps=warm_timesteps)
+        self.source, self.views = source, int(views)
+        self.table = torch.empty((self.views, N.METRICS_FIELDS), dtype=torch.float32, device=self.device)
+        self.reset()
+        self.view = torch.zeros(1, dtype=torch.int32, device=self.device)
+        self.gt = torch.zeros((3, self.H, self.W), dtype=torch.uint8, device=self.device)
+        self._metrics_scratch = None
+
+    def reset(self):
+        """Every row of the table back to NaN (no score)."""
+        self.table.fill_(float("nan"))
+
+    # ---- inputs ------------------------------------------------------------------------------------------------
+    def set_inputs(self, camera=None, timestep=None, gt_u8=None, view=None, verts=None, bg=None):
+        """As GraphedRender.set_inputs, plus the view's ground truth (uint8 (3,H,W), a device tensor or a pinned host
+        tensor) and its row in the table (a host int in [0, views)).  None of them re-captures."""
+        if view is not None:
+            view = int(view)
+            if not 0 <= view < self.views:
+                raise IndexError(f"view {view} outside the table's {self.views} rows")
+        size = (int(camera.image_height), int(camera.image_width)) \
+            if camera is not None and not isinstance(camera, torch.Tensor) else (self.H, self.W)
+        if gt_u8 is not None and (gt_u8.dtype != torch.uint8 or tuple(gt_u8.shape) != (3, *size)):
+            raise ValueError(f"gt_u8 must be a uint8 (3, {size[0]}, {size[1]}) tensor, got {gt_u8.dtype} "
+                             f"{tuple(gt_u8.shape)}")
+        super().set_inputs(camera=camera, timestep=timestep, verts=verts, bg=bg)
+        if tuple(self.gt.shape) != (3, self.H, self.W):   # a camera of another size (the next run() re-captures)
+            self._await_upload()
+            self.gt = torch.zeros((3, self.H, self.W), dtype=torch.uint8, device=self.device)
+        if gt_u8 is not None:
+            if gt_u8.device.type == "cpu" and self.device.type == "cuda":
+                if self._side is None:
+                    self._side = torch.cuda.Stream(device=self.device)
+                self._upload(self.gt, gt_u8)
+            else:
+                self._await_upload()   # an earlier host upload must not land after this copy
+                self.gt.copy_(gt_u8, non_blocking=True)
+        if view is not None:
+            self.view.fill_(view)
+
+    # ---- the frame body: the playback frame, then the metrics of what it rendered ------------------------------
+    def _body(self, captured: bool = False):
+        super()._body(captured)
+        if captured:   # the warm-up frames score nothing: they would write the current view's row
+            launch_image_metrics(self.image if self.source == "float" else self.display, self.gt, self.table,
+                                 row=self.view, skip_flag=self.slot.flag, scratch=self._metrics_scratch)
+
+    def _before_capture(self):
+        super()._before_capture()
+        self._metrics_scratch = metrics_scratch(self.H, self.W, self.device)
+
+    # ---- replay ----------------------------------------------------------------------------------------------------
+    def run(self, check: bool = False):
+        self._await_upload()
+        super().run(check)
+        if self._side is not None:
+            self._mark_read()
+        return self
+
+    def scores(self, n: Optional[int] = None) -> dict:
+        """Synchronises once and returns the first n rows (default: all): `per_view`, a (n, 4) float32 host tensor
+        {l1, psnr, psnr_all, ssim}, and the mean of each column as training_report forms its means (the per-view floats
+        summed in double, then divided by n: train.py:286-303).  `psnr` is train.py's PSNR, `psnr_all` metrics.py's.
+        Raises if a requested row holds no score (NaN): its replay overflowed the capacity (run(check=False)), or the
+        view was never run."""
+        n = self.views if n is None else int(n)
+        if not 1 <= n <= self.views:
+            raise IndexError(f"n must lie in [1, {self.views}]")
+        rows = self.table[:n].cpu()
+        missing = torch.isnan(rows).any(dim=1).nonzero().flatten().tolist()
+        if missing:
+            raise RuntimeError(f"GraphedEval: rows {missing} hold no score -- their replay overflowed the instance "
+                               "capacity (run(check=False)) or never ran: call regrow() and run those views again")
+        out = {"per_view": rows}
+        for i, name in enumerate(METRIC_NAMES):
+            total = 0.0
+            for v in rows[:, i].tolist():
+                total += v
+            out[name] = total / n
+        return out

@@ -3,13 +3,15 @@ CUDA launches behind the same C ABI:
 
   photometric_loss(image, gt, lambda_dssim)   <- l1_loss * (1 - lambda) + (1 - ssim) * lambda
                                                  (utils/loss_utils.py:17-18,36-63, train.py:131-132)
+  image_metrics(render, gt_u8)                <- clamp + l1_loss, psnr, ssim of one val / test view (train.py:277-288)
+                                                 and metrics.py:71-74 (evaluation, forward only)
   Adam(param_groups, lr, betas, eps)          <- torch.optim.Adam(l, lr=0.0, eps=1e-15).step()
                                                  (scene/gaussian_model.py:213-232, train.py:207-210)
   Adam(..., capturable=True)                  <- the same step with the step counters, the bias corrections and the
      + expon_lr_schedule(...)                    xyz learning-rate schedule (update_learning_rate, train.py:106) on
                                                  the device: capturable into a CUDA graph
 
-No CPU or eager fallback: both raise when the library is missing or a tensor is not a CUDA float32 tensor.
+No CPU or eager fallback: each raises when the library is missing or a tensor is not a CUDA tensor of the right dtype.
 """
 from __future__ import annotations
 
@@ -72,6 +74,87 @@ def photometric_loss(image: torch.Tensor, gt: torch.Tensor, lambda_dssim: float 
     returns the detached tensor [l1 mean, ssim mean, total] (for logging, train.py:159-166)."""
     total, parts = _PhotometricLoss.apply(image, gt, lambda_dssim)
     return (total, parts) if return_parts else total
+
+
+# ================================================================================================================
+# Evaluation metrics: l1, psnr (two definitions) and ssim of one view, forward only, in two launches
+# ================================================================================================================
+METRIC_NAMES = ("l1", "psnr", "psnr_all", "ssim")
+
+
+def check_metrics_inputs(render: torch.Tensor, gt_u8: torch.Tensor) -> int:
+    """The checks of image_metrics; returns the render kind (_native.METRICS_FLOAT_CHW or METRICS_U8_HWC)."""
+    device = render.device
+    if render.dtype == torch.float32 and render.dim() == 3 and render.shape[0] == 3:
+        kind, H, W = N.METRICS_FLOAT_CHW, int(render.shape[1]), int(render.shape[2])
+    elif render.dtype == torch.uint8 and render.dim() == 3 and render.shape[2] == 3:
+        kind, H, W = N.METRICS_U8_HWC, int(render.shape[0]), int(render.shape[1])
+    else:
+        raise TypeError("render must be a float32 (3, H, W) image or the uint8 (H, W, 3) display image, got "
+                        f"{render.dtype} {tuple(render.shape)}")
+    if gt_u8.dtype != torch.uint8:
+        raise TypeError(f"gt_u8 must be uint8 (value/255), got {gt_u8.dtype}")
+    if tuple(gt_u8.shape) != (3, H, W) or gt_u8.device != device:
+        raise ValueError(f"gt_u8 must have shape (3, {H}, {W}) on {device}, got {tuple(gt_u8.shape)} on {gt_u8.device}")
+    if H == 0 or W == 0:
+        raise ValueError("an empty image has no metrics")
+    if device.type != "cuda":
+        raise RuntimeError("gaussianavatars_b200 has no CPU path: tensors must be CUDA tensors")
+    return kind
+
+
+def metrics_scratch(height: int, width: int, device) -> torch.Tensor:
+    """Device scratch for one gab200_image_metrics call of this size (the per-tile partial sums)."""
+    nbytes = int(N.lib().gab200_image_metrics_scratch_bytes(int(height), int(width)))
+    return torch.empty(max(nbytes, 8), dtype=torch.uint8, device=device)
+
+
+def launch_image_metrics(render: torch.Tensor, gt_u8: torch.Tensor, table: torch.Tensor,
+                         row: Optional[torch.Tensor] = None, skip_flag: Optional[torch.Tensor] = None,
+                         scratch: Optional[torch.Tensor] = None):
+    """Enqueues the metrics of `render` against `gt_u8` into row `*row` (a device int32; None = row 0) of `table`, a
+    (rows, 4) float32 device tensor, on the current stream; nothing is written when `skip_flag` (device int32) holds a
+    non-zero value as the kernel runs.  Capturable: it reads nothing on the host."""
+    kind = check_metrics_inputs(render, gt_u8)
+    device = render.device
+    if table.dtype != torch.float32 or table.dim() != 2 or table.shape[1] != N.METRICS_FIELDS or \
+            table.device != device or not table.is_contiguous() or table.shape[0] < 1:
+        raise ValueError(f"table must be a contiguous float32 (rows, {N.METRICS_FIELDS}) tensor on {device}")
+    for t, n in ((row, "row"), (skip_flag, "skip_flag")):
+        if t is not None and (t.dtype != torch.int32 or t.device != device):
+            raise TypeError(f"{n} must be an int32 tensor on {device}")
+    r = render if render.is_contiguous() else render.contiguous()
+    g = gt_u8 if gt_u8.is_contiguous() else gt_u8.contiguous()
+    H, W = (int(r.shape[1]), int(r.shape[2])) if kind == N.METRICS_FLOAT_CHW else (int(r.shape[0]), int(r.shape[1]))
+    if scratch is None:
+        scratch = metrics_scratch(H, W, device)
+    elif scratch.numel() * scratch.element_size() < int(N.lib().gab200_image_metrics_scratch_bytes(H, W)):
+        raise ValueError("metrics scratch too small for this image size")
+    a = N.MetricsArgs()
+    a.abi_version, a.height, a.width, a.render_kind = N.ABI_VERSION, H, W, kind
+    a.render, a.gt, a.row, a.table = r.data_ptr(), g.data_ptr(), N.ptr(row), table.data_ptr()
+    a.table_rows, a.skip_flag, a.scratch = int(table.shape[0]), N.ptr(skip_flag), scratch.data_ptr()
+    with torch.cuda.device(device):
+        stream = torch.cuda.current_stream(device).cuda_stream
+        N.check(N.lib().gab200_image_metrics(C.byref(a), C.c_void_p(stream)), "gab200_image_metrics")
+    return table
+
+
+@torch.no_grad()
+def image_metrics(render: torch.Tensor, gt_u8: torch.Tensor) -> torch.Tensor:
+    """(4,) float32 device tensor {l1, psnr, psnr_all, ssim} of one view (include/gab200_rasterizer.h,
+    gab200_image_metrics), with no autograd and no host wait.
+
+    render: the float32 (3, H, W) image of render(), clamped to [0, 1] in the kernel as training_report clamps it
+    (train.py:277), or the uint8 (H, W, 3) display image of render_display() -- the bytes render.py writes as a PNG,
+    read back as value/255 as metrics.py reads them.  gt_u8: the uint8 (3, H, W) ground truth (value/255).
+      l1       = l1_loss(image, gt)                                  (train.py:286)
+      psnr     = psnr(image, gt).mean(): one PSNR per channel, averaged (train.py:287 passes a [3,H,W] image)
+      psnr_all = psnr over all values at once (metrics.py:73 passes [1,3,H,W] tensors)
+      ssim     = ssim(image, gt)                                     (train.py:288, metrics.py:72)
+    Sums run in double with a fixed reduction order: two calls on the same inputs give the same bits."""
+    table = torch.empty((1, N.METRICS_FIELDS), dtype=torch.float32, device=render.device)
+    return launch_image_metrics(render, gt_u8, table)[0]
 
 
 # ================================================================================================================

@@ -325,6 +325,50 @@ typedef struct gab200_photometric_args {
 } gab200_photometric_args;
 int32_t gab200_photometric_loss(const gab200_photometric_args* args, void* stream);
 
+/* Image metrics of one rendered view against its ground truth, forward only, in two launches with no host wait.
+ * Replaces the evaluation the reference runs per val / test view in training_report (train.py:277-288: clamp(0, 1) of
+ * the render, then l1_loss, psnr and ssim) and in metrics.py:71-74 (ssim and psnr of the PNG render.py wrote, read
+ * back as value/255): utils/image_utils.py:18-20 and utils/loss_utils.py:33-63 (11x11 Gaussian window, sigma 1.5,
+ * zero padding, C1 = 0.01^2, C2 = 0.03^2 -- the arithmetic of gab200_photometric_loss's SSIM).
+ *   render_kind GAB200_METRICS_FLOAT_CHW: render is float32 [3,H,W], clamped to [0, 1] in-kernel (train.py:277).
+ *   render_kind GAB200_METRICS_U8_HWC:    render is the display image uint8 [H,W,3] (gab200_forward_display), read as
+ *                                         value/255 correctly rounded (render.py's PNG bytes through to_tensor).
+ *   gt: uint8 [3,H,W], value/255 (PILtoTorch).
+ * The record written is GAB200_METRICS_FIELDS floats:
+ *   [0] l1       mean |render - gt| over all 3HW values
+ *   [1] psnr     mean over the three channels of 20 log10(1 / sqrt(MSE of the channel)): train.py passes a [3,H,W]
+ *                image to psnr(), whose view(img1.shape[0], -1) makes one PSNR per channel, then .mean()
+ *   [2] psnr_all 20 log10(1 / sqrt(MSE over all 3HW values)): metrics.py passes [1,3,H,W] tensors
+ *   [3] ssim     mean of the SSIM map over all 3HW values
+ * An MSE of 0 gives +inf.  Sums run in double and are reduced in a fixed order (no floating-point atomics): the same
+ * inputs give bit-identical records on every call.
+ * The record goes to row *row of `table` ([table_rows, GAB200_METRICS_FIELDS] float32); row is a DEVICE int32 read
+ * when the kernel runs (NULL = row 0), so a replayed CUDA graph can write a different row each time.  A row outside
+ * [0, table_rows) writes nothing.  skip_flag: DEVICE pointer or NULL, as gab200_adam_step_device: non-zero when the
+ * kernel runs = nothing is written (a graph replay whose render overflowed its instance capacity leaves its row as it
+ * was).  scratch: gab200_image_metrics_scratch_bytes(height, width) bytes of device memory, 8-byte aligned.
+ * Invalid arguments (GAB200_ERR_INVALID_ARGUMENT): a NULL args, render, gt, table or scratch, a non-positive height
+ * or width, table_rows < 1, an unknown render_kind, abi_version != GAB200_ABI_VERSION. */
+#define GAB200_METRICS_FIELDS 4
+typedef enum gab200_metrics_render_kind {
+  GAB200_METRICS_FLOAT_CHW = 0,
+  GAB200_METRICS_U8_HWC = 1
+} gab200_metrics_render_kind;
+typedef struct gab200_metrics_args {
+  uint32_t abi_version;
+  int32_t height, width;
+  int32_t render_kind;      /* gab200_metrics_render_kind */
+  const void* render;       /* float [3,H,W] | uint8 [H,W,3] */
+  const uint8_t* gt;        /* [3,H,W] */
+  const int32_t* row;       /* DEVICE int32 or NULL (= 0) */
+  float* table;             /* [table_rows, GAB200_METRICS_FIELDS] */
+  int32_t table_rows;
+  const int32_t* skip_flag; /* DEVICE int32 or NULL */
+  void* scratch;
+} gab200_metrics_args;
+size_t gab200_image_metrics_scratch_bytes(int32_t height, int32_t width);
+int32_t gab200_image_metrics(const gab200_metrics_args* args, void* stream);
+
 /* Adam over several parameter arrays in one launch (SURVEY.md 8f rank 3).  Replaces `gaussians.optimizer.step()` for
  * the splat parameter groups (scene/gaussian_model.py:213-232 builds `torch.optim.Adam(l, lr=0.0, eps=1e-15)` with one
  * group -- and one learning rate -- per array; train.py:207-209): amsgrad off, no weight decay, bias-corrected, `step`
