@@ -50,9 +50,12 @@ def quat_to_R(q):
 
 def render(means3D, means2D, opacities, viewmatrix, projmatrix, campos, W, H, tanfovx, tanfovy, bg, *, shs=None,
            sh_degree=0, colors_precomp=None, scales=None, rotations=None, cov3D_precomp=None, scale_modifier=1.0,
-           radii=None):
+           radii=None, rect_xy=None):
     """All tensor arguments float64.  `radii` (int, from the fp32 oracle) fixes the discrete tile rectangles so the
-    comparison is not at the mercy of ceil() knife edges.  Returns (image (3,H,W), aux dict)."""
+    comparison is not at the mercy of ceil() knife edges.  `rect_xy` ((P,2) float32 pixel centres, from the fp32
+    oracle) also takes the rectangles' centres from there, evaluated in float32 as the oracle does: a centre that
+    float32 puts exactly on a truncation edge (an integer pixel centre with (py + r + 15) / 16 integral, say) lands a
+    hair below it in float64 and would drop a whole tile row.  Returns (image (3,H,W), aux dict)."""
     dt = torch.float64
     P = means3D.shape[0]
     V = viewmatrix.reshape(16).to(dt)
@@ -114,12 +117,16 @@ def render(means3D, means2D, opacities, viewmatrix, projmatrix, campos, W, H, ta
         mid = 0.5 * (a + c)
         lam = mid + torch.sqrt(torch.clamp_min(mid * mid - det, 0.1))
         radii = torch.ceil(3.0 * torch.sqrt(lam)).to(torch.int64)
-    rad = radii.to(dt)
-    pxd, pyd = px.detach(), py.detach()
-    x0 = torch.clamp(((pxd - rad) / 16).trunc(), 0, gx)
-    y0 = torch.clamp(((pyd - rad) / 16).trunc(), 0, gy)
-    x1 = torch.clamp(((pxd + rad + 15) / 16).trunc(), 0, gx)
-    y1 = torch.clamp(((pyd + rad + 15) / 16).trunc(), 0, gy)
+    if rect_xy is None:
+        rad = radii.to(dt)
+        pxd, pyd = px.detach(), py.detach()
+    else:  # splat_oracle.c tile_rect, float32 throughout
+        rad = radii.to(torch.float32)
+        pxd, pyd = rect_xy[:, 0].to(torch.float32), rect_xy[:, 1].to(torch.float32)
+    x0 = torch.clamp(((pxd - rad) / 16).trunc(), 0, gx).to(dt)
+    y0 = torch.clamp(((pyd - rad) / 16).trunc(), 0, gy).to(dt)
+    x1 = torch.clamp(((pxd + rad + 15) / 16).trunc(), 0, gx).to(dt)
+    y1 = torch.clamp(((pyd + rad + 15) / 16).trunc(), 0, gy).to(dt)
     visible = in_front & (radii > 0) & ((x1 - x0) * (y1 - y0) > 0)
 
     order = torch.argsort(tz.detach().to(torch.float32), stable=True)  # fp32 depth bits decide, ties by id
