@@ -93,6 +93,25 @@ class MetricsArgs(C.Structure):
     ]
 
 
+MESH_POS_WORLD, MESH_POS_CLIP = 0, 1
+MESH_LIGHT_FRONT, MESH_LIGHT_CONSTANT = 0, 1
+MESH_BASE_NONE, MESH_BASE_FLOAT_CHW, MESH_BASE_U8_CHW = 0, 1, 2
+MESH_MAX_SIDE = 16384
+
+
+class MeshArgs(C.Structure):
+    """Mirror of gab200_mesh_args."""
+    _fields_ = [
+        ("abi_version", C.c_uint32), ("V", C.c_int32), ("F", C.c_int32), ("width", C.c_int32), ("height", C.c_int32),
+        ("pos_kind", C.c_int32), ("verts", C.c_void_p), ("faces", C.c_void_p), ("adjacency", C.c_void_p),
+        ("camera", C.c_void_p), ("face_colors", C.c_void_p), ("background", C.c_float * 3), ("lighting", C.c_int32),
+        ("antialias", C.c_int32), ("base_kind", C.c_int32), ("base", C.c_void_p), ("opacity", C.c_void_p),
+        ("out_u8", C.c_void_p), ("out_float", C.c_void_p), ("out_rgba", C.c_void_p), ("out_rast", C.c_void_p),
+        ("in_rast", C.c_void_p), ("in_color", C.c_void_p), ("out_color", C.c_void_p), ("channels", C.c_int32),
+        ("error_flag", C.c_void_p), ("scratch", C.c_void_p),
+    ]
+
+
 class AdamSegment(C.Structure):
     """Mirror of gab200_adam_segment."""
     _fields_ = [
@@ -191,7 +210,8 @@ EXPORTED_SYMBOLS = ("gab200_forward", "gab200_backward", "gab200_mark_visible", 
                     "gab200_adam_step_device", "gab200_densify_stats", "gab200_flame_scratch_bytes",
                     "gab200_flame_prepare", "gab200_flame_forward", "gab200_flame_backward",
                     "gab200_forward_device_fov", "gab200_backward_device_fov", "gab200_forward_display",
-                    "gab200_image_metrics", "gab200_image_metrics_scratch_bytes")
+                    "gab200_image_metrics", "gab200_image_metrics_scratch_bytes", "gab200_mesh_render",
+                    "gab200_mesh_scratch_bytes")
 
 _lib = None
 _lock = threading.Lock()
@@ -266,6 +286,10 @@ def lib():
         L.gab200_image_metrics.argtypes = [C.POINTER(MetricsArgs), C.c_void_p]
         L.gab200_image_metrics_scratch_bytes.restype = C.c_size_t
         L.gab200_image_metrics_scratch_bytes.argtypes = [C.c_int32, C.c_int32]
+        L.gab200_mesh_render.restype = C.c_int32
+        L.gab200_mesh_render.argtypes = [C.POINTER(MeshArgs), C.c_void_p]
+        L.gab200_mesh_scratch_bytes.restype = C.c_size_t
+        L.gab200_mesh_scratch_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
         L.gab200_adam_step.restype = C.c_int32
         L.gab200_adam_step.argtypes = [C.c_int32, C.POINTER(AdamSegment), C.c_int64, C.c_double, C.c_double,
                                        C.c_double, C.c_void_p]

@@ -2,7 +2,7 @@
 
     python -m gaussianavatars_b200.build [--force]
 
-preprocess.cu is compiled with --fmad=false (bit-reproducible keys, see its header); everything else with
+preprocess.cu and mesh.cu are compiled with --fmad=false (bit-reproducible keys, see their headers); everything else with
 default contraction.  The .so and the objects under csrc/_obj are build products (git-ignored).
 """
 from __future__ import annotations
@@ -33,6 +33,7 @@ SOURCES = {
     "flame.cu": [],
     "loss.cu": [],
     "metrics.cu": [],
+    "mesh.cu": ["--fmad=false"],
     "optim.cu": [],
 }
 

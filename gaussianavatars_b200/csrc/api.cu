@@ -808,6 +808,38 @@ int32_t gab200_image_metrics(const gab200_metrics_args* a, void* stream_) {
   return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
 }
 
+static const int kMeshMaxSide = 16384;  // snapped coordinates (guard band + image) stay below 2^24 / 256 px
+
+size_t gab200_mesh_scratch_bytes(int32_t num_faces, int32_t width, int32_t height) {
+  if (num_faces < 1 || width < 1 || height < 1 || width > kMeshMaxSide || height > kMeshMaxSide) return 0;
+  return mesh_scratch_bytes(num_faces, width, height);
+}
+
+static bool mesh_args_ok(const gab200_mesh_args* a) {
+  if (a == nullptr || a->abi_version != GAB200_ABI_VERSION || a->V < 1 || a->F < 1 || a->width < 1 || a->height < 1 ||
+      a->width > kMeshMaxSide || a->height > kMeshMaxSide || !a->verts || !a->faces || !a->scratch ||
+      ((uintptr_t)a->scratch & 255) != 0)
+    return false;
+  if (a->pos_kind != GAB200_MESH_POS_WORLD && a->pos_kind != GAB200_MESH_POS_CLIP) return false;
+  if (a->lighting != GAB200_MESH_LIGHT_FRONT && a->lighting != GAB200_MESH_LIGHT_CONSTANT) return false;
+  if (a->base_kind < GAB200_MESH_BASE_NONE || a->base_kind > GAB200_MESH_BASE_U8_CHW) return false;
+  if (a->antialias != 0 && a->antialias != 1) return false;
+  if (a->antialias && !a->adjacency) return false;
+  if (a->pos_kind == GAB200_MESH_POS_WORLD && !a->camera) return false;
+  const bool composite = a->out_u8 || a->out_float;
+  if (!composite && !a->out_rgba && !a->out_rast && !a->out_color) return false;
+  if ((composite || a->out_rgba) && a->pos_kind != GAB200_MESH_POS_WORLD) return false;
+  if (composite && (a->base_kind == GAB200_MESH_BASE_NONE || !a->base || !a->opacity)) return false;
+  if (a->out_color && (!a->in_color || a->channels < 1 || a->channels > 64)) return false;
+  return true;
+}
+
+int32_t gab200_mesh_render(const gab200_mesh_args* a, void* stream_) {
+  if (!mesh_args_ok(a)) return GAB200_ERR_INVALID_ARGUMENT;
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  return launch_mesh_render(*a, (cudaStream_t)stream_) == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
 int32_t gab200_adam_step(int32_t num_segments, const gab200_adam_segment* segs, int64_t step, double beta1,
                          double beta2, double eps, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;

@@ -177,6 +177,10 @@ size_t metrics_scratch_bytes(int H, int W);
 void launch_image_metrics(int H, int W, int kind, const void* render, const uint8_t* gt, const int32_t* row, int rows,
                           const int32_t* skip, float* table, void* scratch, cudaStream_t stream);
 
+// mesh.cu
+size_t mesh_scratch_bytes(int F, int W, int H);
+cudaError_t launch_mesh_render(const gab200_mesh_args& a, cudaStream_t stream);
+
 // densify.cu
 size_t densify_scratch_bytes(int P, int F);
 cudaError_t launch_densify_plan(const gab200_densify_args& a, cudaStream_t stream);

@@ -45,6 +45,7 @@ from typing import Optional
 import torch
 
 from . import _native as N
+from . import mesh as M
 from . import rasterizer as R
 from .renderer import _forward_only, render
 from .rasterizer import l1_loss_u8
@@ -598,11 +599,20 @@ class GraphedRender(_Captured):
     host_slots=k > 0: after each replay the display frame travels to a ring of k pinned host tensors on a copy
     stream, one event per replay, so the copy of frame i overlaps replay i+1 (a consumer one replay behind never
     waits for a transfer).  `host_frame(i)` waits for replay i's copy and returns its slot; slot i % k is rewritten
-    by replay i + k, not before."""
+    by replay i + k, not before.
+
+    mesh_opacity=o: the tracked mesh drawn over the avatar, as the reference's viewers do (train.py:82-93,
+    local_viewer.py's "show mesh"): the graph renders the float splat image, then the mesh overlay kernels
+    (mesh.mesh_overlay) composite the mesh of the vertices the graph just posed at opacity o and write `display`.
+    Pixels the mesh does not reach get the bytes the display epilogue would have written.  Opacity and face_colors
+    ((F,3), e.g. the viewer's splats-per-face colouring) are device buffers written by set_inputs: a slider or a colour
+    picker never re-captures.  `mesh_error` is a device int32 set to 1 when a face index is out of range."""
 
     def __init__(self, pc, width: int, height: int, bg: torch.Tensor, outputs: str = "u8",
                  scaling_modifier: float = 1.0, mesh_update: bool = True, host_slots: int = 0,
-                 capacity: Optional[int] = None, headroom: float = 1.25, warm_cameras=None, warm_timesteps=None):
+                 capacity: Optional[int] = None, headroom: float = 1.25, warm_cameras=None, warm_timesteps=None,
+                 mesh_opacity: Optional[float] = None, face_colors: Optional[torch.Tensor] = None,
+                 mesh_lighting: str = "front"):
         """outputs: "u8" (the display image only: the float image is not written), "float" or "both".
         warm_cameras: camera objects or 37-float blocks rendered eagerly before the capture to size the capacity (and
         the depth-sort range); warm_timesteps: with a FLAME head, the timesteps each warm camera is rendered at
@@ -620,11 +630,41 @@ class GraphedRender(_Captured):
         self.host = self._copy_stream = None
         self._staged = self._host_events = self._stage_events = None
         self.image = self.display = self.radii = None
+        self.mesh = mesh_opacity is not None
+        if self.mesh:
+            if outputs == "float":
+                raise ValueError("the mesh overlay writes the display image: it needs outputs 'u8' or 'both'")
+            if getattr(pc, "faces", None) is None:
+                raise ValueError("mesh_opacity needs a model with a mesh (pc.faces)")
+            if mesh_lighting not in M.LIGHTING:
+                raise ValueError(f"mesh_lighting must be one of {sorted(M.LIGHTING)}, got {mesh_lighting!r}")
+            self.mesh_lighting = mesh_lighting
+            self._opacity = M.opacity_pair(mesh_opacity, self.device)
+            self.face_colors = None
+            if face_colors is not None:
+                self._set_face_colors(face_colors)
+            self.mesh_error = torch.zeros(1, dtype=torch.int32, device=self.device)
+            self._adjacency = M._AdjacencyCache()
+
+    def _set_face_colors(self, face_colors):
+        fc = face_colors.detach().reshape(-1, 3)
+        if fc.shape[0] != self.pc.faces.shape[0]:
+            raise ValueError(f"face_colors must be (F,3) or (1,F,3) with F = {self.pc.faces.shape[0]}")
+        if self.face_colors is None:   # a new buffer: the next run() re-captures (its address joins the state key)
+            self.face_colors = fc.to(self.device, torch.float32).contiguous().clone()
+        else:
+            self.face_colors.copy_(fc, non_blocking=True)
 
     # ---- inputs ------------------------------------------------------------------------------------------------
-    def set_inputs(self, camera=None, timestep=None, verts=None, bg=None):
+    def set_inputs(self, camera=None, timestep=None, verts=None, bg=None, mesh_opacity=None, face_colors=None):
         """Copies new inputs into the graph's device buffers; none of them re-captures.  A camera OBJECT of another
         image size changes the frame's size (the next run() re-captures)."""
+        if (mesh_opacity is not None or face_colors is not None) and not self.mesh:
+            raise ValueError("mesh_opacity / face_colors need a GraphedRender built with mesh_opacity=")
+        if mesh_opacity is not None:
+            self._opacity.copy_(M.opacity_pair(mesh_opacity, "cpu"), non_blocking=True)
+        if face_colors is not None:
+            self._set_face_colors(face_colors)
         self._set_pose_input(verts, timestep)
         if camera is not None:
             blk = self._camera_tensor(camera)
@@ -646,8 +686,24 @@ class GraphedRender(_Captured):
             if self.mesh_update:
                 self._pose()
             out = _forward_only(self.camera, self.pc, _Pipe, self.bg, self.scaling_modifier,
-                                self.outputs != "float", self.outputs != "u8")
+                                self.outputs != "float" and not self.mesh, self.outputs != "u8" or self.mesh)
+            if self.mesh:
+                out["display_u8"] = self._overlay(out["render"])
         self.image, self.display, self.radii = out["render"], out["display_u8"], out["radii"]
+
+    def _overlay(self, image):
+        """The mesh of the vertices the frame just posed (pc.verts) over the float splat image -> (H,W,3) uint8."""
+        pc = self.pc
+        if pc.verts is None:
+            raise ValueError("the mesh overlay draws the posed vertices (pc.verts): pose the model first")
+        faces = getattr(pc, "faces_i32", None)
+        faces = pc.faces.to(torch.int32).contiguous() if faces is None else faces
+        display = torch.empty(self.H, self.W, 3, dtype=torch.uint8, device=self.device)
+        M.launch_mesh(verts=pc.verts.detach().reshape(-1, 3), faces=faces, width=self.W, height=self.H,
+                      camera=self.cam, adjacency=self._adjacency.get(pc.faces).to(self.device),
+                      face_colors=self.face_colors, lighting=self.mesh_lighting, antialias=True, base=image,
+                      opacity=self._opacity, out_u8=display, error_flag=self.mesh_error)
+        return display
 
     # ---- capture ---------------------------------------------------------------------------------------------------
     def _release(self):
@@ -665,9 +721,15 @@ class GraphedRender(_Captured):
             self._make_ring()
 
     def _state_key(self):
-        """Beyond the shared key: the image size, `scaling_modifier` and, with mesh_update=False, the addresses of
-        the face frame the graph renders."""
+        """Beyond the shared key: the image size, `scaling_modifier`, with the mesh overlay what its launch bakes in
+        (the faces' address and version, the adjacency, the colour buffer, the lighting) and, with mesh_update=False,
+        the addresses of the face frame (and of the vertices the overlay draws) the graph renders."""
         key = super()._state_key() + [self.W, self.H, self.scaling_modifier]
+        if self.mesh:
+            key += [self.pc.faces.data_ptr(), self.pc.faces._version, self._adjacency.get(self.pc.faces).data_ptr(),
+                    None if self.face_colors is None else self.face_colors.data_ptr(), self.mesh_lighting]
+            if not self.mesh_update:
+                key.append(None if self.pc.verts is None else self.pc.verts.data_ptr())
         if not self.mesh_update and getattr(self.pc, "binding", None) is not None:
             key += [getattr(self.pc, n).data_ptr() for n in ("face_center", "face_orien_mat", "face_scaling")]
         return key

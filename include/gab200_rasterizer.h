@@ -369,6 +369,92 @@ typedef struct gab200_metrics_args {
 size_t gab200_image_metrics_scratch_bytes(int32_t height, int32_t width);
 int32_t gab200_image_metrics(const gab200_metrics_args* args, void* stream);
 
+/* The tracked mesh drawn over an image, forward only, in four launches with no host wait (capturable).  Replaces
+ * what the reference's mesh renderer (mesh_renderer/__init__.py:183-274) asks of nvdiffrast -- dr.rasterize and
+ * dr.antialias -- and, fused, render.py's mesh composite (render.py:75-81) and its uint8 quantisation.
+ *   Geometry.  pos_kind GAB200_MESH_POS_WORLD: verts [V,3] world space, clip = [v,1] . full_proj_transform (the 16
+ *     floats at camera + 16; camera is the 35- or 37-float camera block world_view (16) | full_proj (16) | centre (3)
+ *     [| tan fov (2)]).  GAB200_MESH_POS_CLIP: verts [V,4] are clip coordinates (nvdiffrast's `pos`); camera unused.
+ *     Faces [F,3] int32.  A face is clipped against -w <= z <= w (nvdiffrast's clip volume) and a guard band of 2^15
+ *     pixels, and its vertices are snapped to 1/256 pixel.  Coverage: int64 edge functions at pixel centres with a
+ *     top-left fill rule -- watertight, no pixel covered twice along a shared edge.  No back-face culling.  Depth: z/w
+ *     at the pixel centre; the nearest face wins, ties go to the smaller face index.
+ *   Pixels.  Column c / row r has its centre at (c + 1/2, r + 1/2) with X = (x/w + 1) W / 2, Y = (y/w + 1) H / 2: row 0
+ *     is clip y = -1 (the top row of the splat image for a camera's own full_proj_transform; nvdiffrast's row 0 for
+ *     the reference's y-negated clip coordinates).  Images are row-major in that order.
+ *   Shading (POS_WORLD).  n = normalize(cross(v1 - v0, v2 - v0)) in the OpenGL camera frame (rows 1, 2 of the view
+ *     transform negated); diffuse = clamp(n.z, 0, 1) (GAB200_MESH_LIGHT_FRONT) or 1 (GAB200_MESH_LIGHT_CONSTANT);
+ *     rgba = (face_colors[f] (or 1) * diffuse, 1) where covered, (background, 0) elsewhere.
+ *   Antialiasing (antialias = 1; needs adjacency).  For every pair of horizontally or vertically adjacent pixels whose
+ *     winners differ, the occluder is the pixel whose face is nearer at its own centre (a covered pixel occludes the
+ *     background).  The occluder face's silhouette edges -- a mesh boundary, or the face across the edge lies on the
+ *     same side of the edge's projected line; a face with a vertex outside the clip volume has none -- with
+ *     |dx| <= |dy| are tested on horizontal pairs, the others on vertical ones: t = e(a) / (e(a) - e(b)), the crossing
+ *     on the segment between the centres counted from the occluder a, must lie in [0, 1] and within the edge's extent;
+ *     the smallest t wins.  t < 1/2: a moves toward b by 1/2 - t; t > 1/2: b moves toward a by t - 1/2.  Every delta is
+ *     taken from the un-antialiased colours and a pixel adds its deltas in the order left, right, up, down (no atomics:
+ *     the same inputs give the same bits).  This is the silhouette-coverage approximation of Laine et al. 2020,
+ *     "Modular Primitives for High-Performance Differentiable Rendering", section 3.3; it is not claimed to equal
+ *     nvdiffrast bit for bit.
+ *   adjacency [F,3] int32: adjacency[f][k] = the face across edge k = (faces[f][k], faces[f][(k+1) % 3]), or -1 when
+ *     no face or more than one other face shares that edge (a boundary).  It depends on faces only: build it once.
+ * Outputs (any may be NULL; at least one is required):
+ *   out_rgba  [H,W,4] float: the antialiased rgba (the reference's `rgba` before its flip)     POS_WORLD
+ *   out_u8    [H,W,3] uint8 / out_float [3,H,W] float: the composite
+ *               rgb * a * o + base * (a * (1 - o) + (1 - a))
+ *             in torch's evaluation order, every op rounded (render.py's expression), out_u8 quantised as render.py
+ *             does (mul(255).add_(0.5).clamp_(0, 255), truncation).  base: float [3,H,W] (GAB200_MESH_BASE_FLOAT_CHW)
+ *             or uint8 [3,H,W] read as value/255 correctly rounded (GAB200_MESH_BASE_U8_CHW).  opacity: DEVICE
+ *             float[2] = {o, 1 - o}, both rounded from the caller's double, as torch rounds its Python scalars;
+ *             read when the kernel runs (a replayed graph picks up a new opacity)                  POS_WORLD
+ *   out_rast  [H,W,4] float: nvdiffrast's rast_out -- perspective-correct barycentrics (u, v) of the original
+ *             triangle's vertices 0 and 1, z/w, face index + 1; zeros where nothing is covered
+ *   out_color [H,W,channels] float: antialias of the caller's image in_color [H,W,channels] (1..64 channels)
+ * in_rast [H,W,4] or NULL: the winners are taken from this rast_out (channel 2 z/w, channel 3 face index + 1) instead of
+ *   being rasterized: nvdiffrast's antialias(color, rast, pos, tri).
+ * error_flag: DEVICE int32 or NULL: 1 is ORed into it when a face has a vertex index outside [0, V); that face is not
+ *   drawn and nothing is read out of bounds.
+ * scratch: gab200_mesh_scratch_bytes(F, width, height) bytes of device memory, 256-byte aligned.
+ * Invalid arguments (GAB200_ERR_INVALID_ARGUMENT): abi_version, V < 1, F < 1, width / height outside [1, 16384], a
+ * NULL verts / faces / scratch, an unknown pos_kind / lighting / base_kind, POS_WORLD without camera, antialias
+ * without adjacency, no output, out_rgba / out_u8 / out_float with POS_CLIP, out_u8 / out_float without base or
+ * opacity, out_color without in_color or a channel count outside [1, 64]. */
+typedef enum gab200_mesh_pos_kind { GAB200_MESH_POS_WORLD = 0, GAB200_MESH_POS_CLIP = 1 } gab200_mesh_pos_kind;
+typedef enum gab200_mesh_lighting { GAB200_MESH_LIGHT_FRONT = 0, GAB200_MESH_LIGHT_CONSTANT = 1 } gab200_mesh_lighting;
+typedef enum gab200_mesh_base_kind {
+  GAB200_MESH_BASE_NONE = 0,
+  GAB200_MESH_BASE_FLOAT_CHW = 1,
+  GAB200_MESH_BASE_U8_CHW = 2
+} gab200_mesh_base_kind;
+typedef struct gab200_mesh_args {
+  uint32_t abi_version;
+  int32_t V, F, width, height;
+  int32_t pos_kind;            /* gab200_mesh_pos_kind */
+  const float* verts;          /* [V,3] | [V,4] */
+  const int32_t* faces;        /* [F,3] */
+  const int32_t* adjacency;    /* [F,3] or NULL (antialias = 0) */
+  const float* camera;         /* camera block (POS_WORLD) */
+  const float* face_colors;    /* [F,3] or NULL (albedo 1) */
+  float background[3];
+  int32_t lighting;            /* gab200_mesh_lighting */
+  int32_t antialias;           /* 0 | 1 */
+  int32_t base_kind;           /* gab200_mesh_base_kind */
+  const void* base;
+  const float* opacity;        /* DEVICE float[2] = {o, 1 - o} */
+  uint8_t* out_u8;             /* [H,W,3] */
+  float* out_float;            /* [3,H,W] */
+  float* out_rgba;             /* [H,W,4] */
+  float* out_rast;             /* [H,W,4] */
+  const float* in_rast;        /* [H,W,4] or NULL */
+  const float* in_color;       /* [H,W,channels] or NULL */
+  float* out_color;            /* [H,W,channels] */
+  int32_t channels;
+  int32_t* error_flag;         /* DEVICE int32 or NULL */
+  void* scratch;
+} gab200_mesh_args;
+size_t gab200_mesh_scratch_bytes(int32_t num_faces, int32_t width, int32_t height);
+int32_t gab200_mesh_render(const gab200_mesh_args* args, void* stream);
+
 /* Adam over several parameter arrays in one launch (SURVEY.md 8f rank 3).  Replaces `gaussians.optimizer.step()` for
  * the splat parameter groups (scene/gaussian_model.py:213-232 builds `torch.optim.Adam(l, lr=0.0, eps=1e-15)` with one
  * group -- and one learning rate -- per array; train.py:207-209): amsgrad off, no weight decay, bias-corrected, `step`
