@@ -50,12 +50,15 @@ def quat_to_R(q):
 
 def render(means3D, means2D, opacities, viewmatrix, projmatrix, campos, W, H, tanfovx, tanfovy, bg, *, shs=None,
            sh_degree=0, colors_precomp=None, scales=None, rotations=None, cov3D_precomp=None, scale_modifier=1.0,
-           radii=None, rect_xy=None):
+           radii=None, rect_xy=None, depths=None):
     """All tensor arguments float64.  `radii` (int, from the fp32 oracle) fixes the discrete tile rectangles so the
     comparison is not at the mercy of ceil() knife edges.  `rect_xy` ((P,2) float32 pixel centres, from the fp32
     oracle) also takes the rectangles' centres from there, evaluated in float32 as the oracle does: a centre that
     float32 puts exactly on a truncation edge (an integer pixel centre with (py + r + 15) / 16 integral, say) lands a
-    hair below it in float64 and would drop a whole tile row.  Returns (image (3,H,W), aux dict)."""
+    hair below it in float64 and would drop a whole tile row.  `depths` ((P,) float32 view-space depths, from the fp32
+    oracle) decides the blend order in place of this model's own depths rounded to float32: two splats a rounding
+    apart in depth composite in the oracle's order.  Returns (image (3,H,W), aux dict); aux also holds the discrete
+    decisions (`keep`, `alpha_clamped`, `colour_clamped`, `guard_clamped`) a caller can hold fixed."""
     dt = torch.float64
     P = means3D.shape[0]
     V = viewmatrix.reshape(16).to(dt)
@@ -103,12 +106,14 @@ def render(means3D, means2D, opacities, viewmatrix, projmatrix, campos, W, H, ta
 
     if colors_precomp is not None:
         rgb = colors_precomp
+        colour_clamped = torch.zeros_like(rgb, dtype=torch.bool)
     else:
         d = means3D - campos.reshape(1, 3)
         d = d / d.norm(dim=1, keepdim=True)
         B = sh_basis(sh_degree, d)
         nb = B.shape[1]
         rgb = (B[:, :, None] * shs[:, :nb, :]).sum(dim=1) + 0.5
+        colour_clamped = rgb.detach() < 0
         rgb = torch.clamp_min(rgb, 0.0)
 
     # discrete tile rectangles
@@ -129,7 +134,8 @@ def render(means3D, means2D, opacities, viewmatrix, projmatrix, campos, W, H, ta
     y1 = torch.clamp(((pyd + rad + 15) / 16).trunc(), 0, gy).to(dt)
     visible = in_front & (radii > 0) & ((x1 - x0) * (y1 - y0) > 0)
 
-    order = torch.argsort(tz.detach().to(torch.float32), stable=True)  # fp32 depth bits decide, ties by id
+    key = tz.detach() if depths is None else depths
+    order = torch.argsort(key.to(torch.float32), stable=True)  # fp32 depth bits decide, ties by id
     ys, xs = torch.meshgrid(torch.arange(H, dtype=dt), torch.arange(W, dtype=dt), indexing="ij")
     pixx, pixy = xs.reshape(-1, 1), ys.reshape(-1, 1)  # (HW,1)
     tilex, tiley = (pixx / 16).floor(), (pixy / 16).floor()
@@ -156,4 +162,6 @@ def render(means3D, means2D, opacities, viewmatrix, projmatrix, campos, W, H, ta
     T_final = torch.where(keep, one_minus, torch.ones_like(one_minus)).prod(dim=1)
     out = C + T_final[:, None] * bg.reshape(1, 3)
     img = out.t().reshape(3, H, W)
-    return img, dict(radii=radii, visible=visible, T_final=T_final.reshape(H, W), n_keep=keep.sum(dim=1).reshape(H, W))
+    return img, dict(radii=radii, visible=visible, T_final=T_final.reshape(H, W), n_keep=keep.sum(dim=1).reshape(H, W),
+                     keep=keep, alpha_clamped=og.detach() > 0.99, colour_clamped=colour_clamped,
+                     guard_clamped=torch.stack((cx, cy), dim=1))
