@@ -198,6 +198,9 @@ class FlameGrads(C.Structure):
     ]
 
 
+CAMERA_FLOATS = 37   # a gab200_forward_views camera row (GAB200_CAMERA_FLOATS)
+MAX_VIEWS = 65535
+
 ADAM_MAX_SEGMENTS = 8
 PHOTOMETRIC_SCRATCH_HEAD = 4
 
@@ -211,7 +214,7 @@ EXPORTED_SYMBOLS = ("gab200_forward", "gab200_backward", "gab200_mark_visible", 
                     "gab200_flame_prepare", "gab200_flame_forward", "gab200_flame_backward",
                     "gab200_forward_device_fov", "gab200_backward_device_fov", "gab200_forward_display",
                     "gab200_image_metrics", "gab200_image_metrics_scratch_bytes", "gab200_mesh_render",
-                    "gab200_mesh_scratch_bytes")
+                    "gab200_mesh_scratch_bytes", "gab200_forward_views")
 
 _lib = None
 _lock = threading.Lock()
@@ -251,6 +254,9 @@ def lib():
         L.gab200_forward_display.argtypes = [C.POINTER(ForwardArgs), C.c_void_p, C.c_void_p, C.POINTER(FrameState),
                                              C.c_void_p]
         L.gab200_backward_device_fov.argtypes = [C.POINTER(BackwardArgs), C.c_void_p, C.c_void_p]
+        L.gab200_forward_views.restype = C.c_int64
+        L.gab200_forward_views.argtypes = [C.POINTER(ForwardArgs), C.c_int32, C.c_void_p, C.c_void_p,
+                                           C.POINTER(FrameState), C.c_void_p]
         L.gab200_mark_visible.restype = C.c_int32
         L.gab200_mark_visible.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gab200_bind_activate.restype = C.c_int32

@@ -133,15 +133,17 @@ struct ImageView {
   uint32_t* n_contrib;
   size_t bytes;
 };
-static ImageView carve_image(void* base, int W, int H, bool need_backward) {
+// views > 1 (gab200_forward_views, forward only): the tile arrays of all views' tiles
+static ImageView carve_image(void* base, int W, int H, bool need_backward, int views = 1) {
   ImageView v;
   Carver c(base);
   const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
-  v.ranges = c.take<uint2>((size_t)gx * gy + 1);  // + 1: the slot the sentinel key of a capacity-padded sort maps to
-  v.order = c.take<uint32_t>((size_t)gx * gy);
+  const size_t tiles = (size_t)gx * gy * views;
+  v.ranges = c.take<uint2>(tiles + 1);  // + 1: the slot the sentinel key of a capacity-padded sort maps to
+  v.order = c.take<uint32_t>(tiles);
   v.order_info = c.take<uint32_t>(4);
-  v.tile_count = c.take<uint32_t>((size_t)gx * gy);
-  v.tile_cursor = c.take<uint32_t>((size_t)gx * gy);
+  v.tile_count = c.take<uint32_t>(tiles);
+  v.tile_cursor = c.take<uint32_t>(tiles);
   v.final_T = need_backward ? c.take<float>((size_t)W * H) : nullptr;
   v.n_contrib = need_backward ? c.take<uint32_t>((size_t)W * H) : nullptr;
   v.bytes = c.bytes();
@@ -339,12 +341,15 @@ namespace {
 struct Frame {
   const gab200_forward_args* a;
   const float* tanfov;  // device float[2] (gab200_forward_device_fov) or NULL: a->tanfovx / tanfovy
-  uint8_t* out_rgb8;    // [H,W,3] display image (gab200_forward_display) or NULL
+  uint8_t* out_rgb8;    // [H,W,3] display image (gab200_forward_display) or NULL; [views,H,W,3] with `cameras`
   gab200_frame_state* st;
   cudaStream_t stream;
   GeomView g;
   ImageView iv;
   int P, W, H, gx, gy;
+  int tiles;                        // of the whole frame: gx * gy * views
+  int views = 1;                    // gab200_forward_views: P = views * a->P virtual splats (view k: k * a->P + i) ...
+  const float* cameras = nullptr;   // ... rendered with row k of this device table, else NULL
   bool nb, dbg;
   uint32_t* ctr_host;   // where the counters land on the host
   cudaEvent_t ctr_event;
@@ -368,13 +373,17 @@ int enqueue_geometry(Frame& f, bool bucket, bool run_preprocess, uint32_t capaci
     d.scale = (float)((double)d.nb / ((double)(d.hi - d.lo) + 1.0));
     d.enabled = 1;
   }
-  const int tiles = f.gx * f.gy;
+  const int tiles = f.tiles;
   if (run_preprocess) {
     GAB_CUDA(cudaMemsetAsync(d.counts, 0, g.bucket_clear_bytes, stream));
     if (f.counting) GAB_CUDA(cudaMemsetAsync(f.iv.tile_count, 0, sizeof(uint32_t) * (size_t)tiles, stream));
     StageScope sc(GAB200_STAGE_PREPROCESS, stream);
-    launch_preprocess(*a, g.rec, g.aux, g.tiles_touched, f.nb ? g.clamped : nullptr, g.depth_keys[0], g.ids[0], g.buckets,
-                      f.counting ? f.iv.tile_count : nullptr, f.tanfov, stream);
+    if (f.cameras != nullptr)
+      launch_preprocess_views(*a, f.views, f.cameras, g.rec, g.aux, g.tiles_touched, g.depth_keys[0], g.ids[0],
+                              g.buckets, f.counting ? f.iv.tile_count : nullptr, stream);
+    else
+      launch_preprocess(*a, g.rec, g.aux, g.tiles_touched, f.nb ? g.clamped : nullptr, g.depth_keys[0], g.ids[0],
+                        g.buckets, f.counting ? f.iv.tile_count : nullptr, f.tanfov, stream);
   }
   GAB_STAGE_CHECK(f.dbg, stream);
   if (f.counting && run_preprocess) {
@@ -413,6 +422,16 @@ int enqueue_geometry(Frame& f, bool bucket, bool run_preprocess, uint32_t capaci
   return GAB200_OK;
 }
 
+// key emission of the frame's (virtual) splats in depth order
+void emit(const Frame& f, const uint32_t* offsets, uint32_t cap, uint32_t* cursor, const BinView& bv) {
+  if (f.cameras != nullptr)
+    launch_emit_keys_views(f.P, f.gx, f.gy, f.g.rec, f.g.aux, f.g.ids[f.selA], offsets, f.order_count, f.g.buckets.meta,
+                           cap, cursor, bv.keys[0], bv.vals[0], f.a->exact_binning, f.a->P, f.stream);
+  else
+    launch_emit_keys(f.P, f.gx, f.gy, f.g.rec, f.g.aux, f.g.ids[f.selA], offsets, f.order_count, f.g.buckets.meta, cap,
+                     cursor, bv.keys[0], bv.vals[0], f.a->exact_binning, f.stream);
+}
+
 // emit -> per-instance tile sort -> ranges -> tile order -> blend, for a binning buffer of `cap` instances.
 // n_known >= 0: exactly that many instances exist (no padding); n_known < 0: the count is only on the device -- the
 // tile sort runs over the whole capacity, unused slots carry the sentinel key and sort behind every tile.
@@ -420,7 +439,7 @@ int enqueue_binning_blend(Frame& f, void* bin, int64_t cap, int64_t n_known, siz
   const gab200_forward_args* a = f.a;
   gab200_frame_state* st = f.st;
   cudaStream_t stream = f.stream;
-  const int tiles = f.gx * f.gy;
+  const int tiles = f.tiles;
   BinView bv = carve_binning(bin, cap, f.nb, sort_temp);
   st->binning_capacity = cap;
   st->binning_buffer = bin;
@@ -441,8 +460,7 @@ int enqueue_binning_blend(Frame& f, void* bin, int64_t cap, int64_t n_known, siz
     if (n_sort > 0) {
       {
         StageScope sc(GAB200_STAGE_EMIT_KEYS, stream);
-        launch_emit_keys(f.P, f.gx, f.gy, f.g.rec, f.g.aux, f.g.ids[f.selA], nullptr, f.order_count, f.g.buckets.meta,
-                         (uint32_t)cap, f.iv.tile_cursor, bv.keys[0], bv.vals[0], a->exact_binning, stream);
+        emit(f, nullptr, (uint32_t)cap, f.iv.tile_cursor, bv);
       }
       GAB_STAGE_CHECK(f.dbg, stream);
       {
@@ -458,8 +476,7 @@ int enqueue_binning_blend(Frame& f, void* bin, int64_t cap, int64_t n_known, siz
       if (n_known < 0) GAB_CUDA(cudaMemsetAsync(bv.keys[0], 0xff, sizeof(uint32_t) * (size_t)cap, stream));
       {
         StageScope sc(GAB200_STAGE_EMIT_KEYS, stream);
-        launch_emit_keys(f.P, f.gx, f.gy, f.g.rec, f.g.aux, f.g.ids[f.selA], f.g.offsets, f.order_count, f.g.buckets.meta,
-                         (uint32_t)cap, nullptr, bv.keys[0], bv.vals[0], a->exact_binning, stream);
+        emit(f, f.g.offsets, (uint32_t)cap, nullptr, bv);
       }
       GAB_STAGE_CHECK(f.dbg, stream);
       {
@@ -481,8 +498,12 @@ int enqueue_binning_blend(Frame& f, void* bin, int64_t cap, int64_t n_known, siz
   st->sorted_selector = selector;
   {
     StageScope sc(GAB200_STAGE_BLEND_FWD, stream);
-    launch_blend_forward(f.W, f.H, f.iv.ranges, f.iv.order, f.iv.order_info, bv.vals[selector], f.g.rec, a->bg,
-                         a->out_color, f.iv.final_T, f.iv.n_contrib, bv.strip_mask, f.out_rgb8, stream);
+    if (f.cameras != nullptr)
+      launch_blend_forward_views(f.views, f.W, f.H, f.iv.ranges, f.iv.order, f.iv.order_info, bv.vals[selector], f.g.rec,
+                                 a->bg, a->out_color, f.out_rgb8, stream);
+    else
+      launch_blend_forward(f.W, f.H, f.iv.ranges, f.iv.order, f.iv.order_info, bv.vals[selector], f.g.rec, a->bg,
+                           a->out_color, f.iv.final_T, f.iv.n_contrib, bv.strip_mask, f.out_rgb8, stream);
   }
   GAB_STAGE_CHECK(f.dbg, stream);
   return GAB200_OK;
@@ -498,9 +519,10 @@ int wait_counters(Frame& f) {
 }  // namespace
 
 // gab200_forward, gab200_forward_device_fov and gab200_forward_display (tanfov == NULL: the by-value tanfovx /
-// tanfovy; out_rgb8 == NULL: no display image)
+// tanfovy; out_rgb8 == NULL: no display image), and gab200_forward_views (cameras != NULL: `views` cameras, validated
+// by the caller, as one frame of views * P virtual splats)
 static int64_t run_forward(const gab200_forward_args* a, const float* tanfov, uint8_t* out_rgb8,
-                           gab200_frame_state* st, void* stream_) {
+                           gab200_frame_state* st, void* stream_, int views = 1, const float* cameras = nullptr) {
   cudaStream_t stream = (cudaStream_t)stream_;
   if (!validate(a, out_rgb8 != nullptr && a != nullptr && a->need_backward == 0) || st == nullptr)
     return GAB200_ERR_INVALID_ARGUMENT;
@@ -508,8 +530,10 @@ static int64_t run_forward(const gab200_forward_args* a, const float* tanfov, ui
   memset(st, 0, sizeof(*st));
   Frame f;
   f.a = a; f.tanfov = tanfov; f.out_rgb8 = out_rgb8; f.st = st; f.stream = stream;
-  f.P = a->P; f.W = a->image_width; f.H = a->image_height;
+  f.P = a->P * views; f.W = a->image_width; f.H = a->image_height;
   f.gx = (f.W + GAB_TILE - 1) / GAB_TILE; f.gy = (f.H + GAB_TILE - 1) / GAB_TILE;
+  f.tiles = f.gx * f.gy * views;
+  f.views = views; f.cameras = cameras;
   f.nb = a->need_backward != 0;
   f.dbg = a->debug != 0;
   f.counting = tune_get(GAB200_TUNE_TILE_SORT) == 1;
@@ -533,13 +557,13 @@ static int64_t run_forward(const gab200_forward_args* a, const float* tanfov, ui
   void* geom = a->alloc_geom(a->alloc_user, gsz.bytes);
   if (geom == nullptr) return GAB200_ERR_ALLOC;
   f.g = carve_geom(geom, P, f.nb, tempA);
-  ImageView isz = carve_image(nullptr, f.W, f.H, f.nb);
+  ImageView isz = carve_image(nullptr, f.W, f.H, f.nb, views);
   void* img = a->alloc_image(a->alloc_user, isz.bytes);
   if (img == nullptr) return GAB200_ERR_ALLOC;
-  f.iv = carve_image(img, f.W, f.H, f.nb);
+  f.iv = carve_image(img, f.W, f.H, f.nb, views);
   st->geom_buffer = geom; st->geom_bytes = f.g.bytes;
   st->image_buffer = img; st->image_bytes = f.iv.bytes;
-  st->sort_bits = (int)tile_bits((uint32_t)(f.gx * f.gy));  // stage B: tile id only
+  st->sort_bits = (int)tile_bits((uint32_t)f.tiles);  // stage B: tile id only
   st->depth_bits = 32;                                      // stage A: the full fp32 depth pattern
   st->device_counters = f.g.buckets.meta;
   st->attempts = 1;
@@ -654,6 +678,19 @@ int64_t gab200_forward_device_fov(const gab200_forward_args* a, const float* tan
 int64_t gab200_forward_display(const gab200_forward_args* a, const float* tanfov, uint8_t* out_rgb8,
                                gab200_frame_state* st, void* stream) {
   return run_forward(a, tanfov, out_rgb8, st, stream);
+}
+
+int64_t gab200_forward_views(const gab200_forward_args* a, int32_t views, const float* cameras, uint8_t* out_rgb8,
+                             gab200_frame_state* st, void* stream) {
+  if (a == nullptr || a->need_backward != 0 || views < 1 || views > 65535 || cameras == nullptr || st == nullptr)
+    return GAB200_ERR_INVALID_ARGUMENT;
+  gab200_forward_args v = *a;
+  v.viewmatrix = v.projmatrix = v.campos = cameras;  // ignored: every view reads its row of the table
+  if (!validate(&v, out_rgb8 != nullptr)) return GAB200_ERR_INVALID_ARGUMENT;
+  const int64_t view_tiles = (((int64_t)v.image_width + GAB_TILE - 1) / GAB_TILE) *
+                             (((int64_t)v.image_height + GAB_TILE - 1) / GAB_TILE);
+  if ((int64_t)views * v.P > INT32_MAX || (int64_t)views * view_tiles > INT32_MAX) return GAB200_ERR_INVALID_ARGUMENT;
+  return run_forward(&v, nullptr, out_rgb8, st, stream, views, cameras);
 }
 
 // gab200_backward and gab200_backward_device_fov

@@ -380,6 +380,59 @@ void launch_blend_forward(int W, int H, const uint2* ranges, const uint32_t* ord
   count_launch();
 }
 
+// gab200_forward_views: the tiles of K views as one list of K * view_tiles global tiles, scheduled heaviest-first
+// together (small views fill the GPU side by side).  Global tile g is tile g % view_tiles of view g / view_tiles: the
+// tile's range and the view's images are offset, and forward_tile renders it exactly as the single-view kernel does.
+// Forward only (no final_T, n_contrib or block masks).
+template <int OUT>
+__global__ void __launch_bounds__(256) blend_forward_views_kernel(int W, int H, int gx, int tiles, int view_tiles,
+                                                                  const uint2* __restrict__ ranges,
+                                                                  const uint32_t* __restrict__ order,
+                                                                  const uint32_t* __restrict__ order_info,
+                                                                  const uint32_t* __restrict__ point_list,
+                                                                  const SplatRec* __restrict__ rec,
+                                                                  const float* __restrict__ bg,
+                                                                  float* __restrict__ out_color,
+                                                                  uint8_t* __restrict__ out_rgb8) {
+  __shared__ SplatRec buf[2][256];
+  __shared__ uint32_t smask[256];
+  __shared__ __align__(16) uint32_t ids_ring[4][ID_RING * (64 + 4)];
+  __shared__ __align__(8) uint64_t mbar[4][ID_RING];
+  const int nh = (int)order_info[0];
+  const int b = blockIdx.x, t = threadIdx.x;
+  const bool heavy = b < nh;  // one heavy tile on all 256 threads, else four light tiles on 64 threads each
+  const int g = heavy ? 0 : t >> 6;
+  const int slot = heavy ? b : nh + 4 * (b - nh) + g;
+  if (slot >= (heavy ? nh : tiles)) return;
+  const int tile = (int)order[slot];
+  const int view = tile / view_tiles, local = tile - view * view_tiles;
+  const size_t HW = (size_t)H * W;
+  float* color = (OUT & BLEND_OUT_FLOAT) ? out_color + (size_t)view * 3 * HW : nullptr;
+  uint8_t* rgb8 = (OUT & BLEND_OUT_U8) ? out_rgb8 + (size_t)view * 3 * HW : nullptr;
+  const uint2* view_ranges = ranges + (size_t)view * view_tiles;
+  if (heavy)
+    forward_tile<1, OUT>(local, t, GroupBarrier<256>{0}, buf[0], buf[1], smask, &ids_ring[0][0], mbar[0], W, H, gx,
+                         view_ranges, point_list, rec, bg, color, nullptr, nullptr, nullptr, rgb8);
+  else
+    forward_tile<4, OUT>(local, t & 63, GroupBarrier<64>{1 + g}, buf[0] + g * 64, buf[1] + g * 64, smask + g * 64,
+                         ids_ring[g], mbar[g], W, H, gx, view_ranges, point_list, rec, bg, color, nullptr, nullptr,
+                         nullptr, rgb8);
+}
+
+void launch_blend_forward_views(int views, int W, int H, const uint2* ranges, const uint32_t* order,
+                                const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
+                                const float* bg, float* out_color, uint8_t* out_rgb8, cudaStream_t stream) {
+  const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
+  const int view_tiles = gx * gy, tiles = views * view_tiles;
+  if (tiles == 0) return;
+  auto kernel = out_rgb8 == nullptr ? blend_forward_views_kernel<BLEND_OUT_FLOAT>
+                : out_color == nullptr ? blend_forward_views_kernel<BLEND_OUT_U8>
+                                       : blend_forward_views_kernel<BLEND_OUT_FLOAT | BLEND_OUT_U8>;
+  kernel<<<tiles, 256, 0, stream>>>(W, H, gx, tiles, view_tiles, ranges, order, order_info, point_list, rec, bg,
+                                    out_color, out_rgb8);
+  count_launch();
+}
+
 // =====================================================================================================
 // Backward
 // =====================================================================================================

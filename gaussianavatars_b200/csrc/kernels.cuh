@@ -100,6 +100,11 @@ __device__ __forceinline__ uint32_t depth_bucket(uint32_t key, const DepthBucket
 void launch_preprocess(const gab200_forward_args& a, SplatRec* rec, SplatAux* aux, uint32_t* tiles_touched,
                        uint8_t* clamped, uint32_t* depth_keys, uint32_t* ids, const DepthBuckets& buckets,
                        uint32_t* tile_count, const float* tanfov, cudaStream_t stream);
+// gab200_forward_views: grid (splat blocks, views); camera row k of `cameras` renders virtual splats k * P + i
+// (rec / aux / tiles / depth keys / ids / radii / visibility), tile counts at k * (gx * gy) + the tile in the view
+void launch_preprocess_views(const gab200_forward_args& a, int views, const float* cameras, SplatRec* rec, SplatAux* aux,
+                             uint32_t* tiles_touched, uint32_t* depth_keys, uint32_t* ids, const DepthBuckets& buckets,
+                             uint32_t* tile_count, cudaStream_t stream);
 // depth_keys [P] (by splat) -> sorted_ids [M] in (key, id) order and offsets [M] = inclusive instance counts
 // also publishes the frame counters (capacity, seq, overflow) of the bucket-sorted frame
 void launch_depth_bucket_sort(int P, const DepthBuckets& buckets, const uint32_t* depth_keys,
@@ -118,6 +123,12 @@ void launch_publish_counters(uint32_t* counters, const uint32_t* offsets, int P,
 void launch_emit_keys(int P, int gx, int gy, const SplatRec* rec, const SplatAux* aux, const uint32_t* order,
                       const uint32_t* offsets, const uint32_t* order_count, const uint32_t* counters, uint32_t capacity,
                       uint32_t* cursor, uint32_t* keys, uint32_t* vals, int exact_binning, cudaStream_t stream);
+// the same over the P virtual splats of a multi-view frame, view_splats per view: instances of virtual splat v go to
+// the tiles (v / view_splats) * (gx * gy) + the tile in the view
+void launch_emit_keys_views(int P, int gx, int gy, const SplatRec* rec, const SplatAux* aux, const uint32_t* order,
+                            const uint32_t* offsets, const uint32_t* order_count, const uint32_t* counters, uint32_t cap,
+                            uint32_t* cursor, uint32_t* keys, uint32_t* vals, int exact_binning, int view_splats,
+                            cudaStream_t stream);
 // keys[0..N) sorted; entries with key >= tiles are padding (sentinel) behind the last real instance
 void launch_tile_ranges(int64_t N, uint32_t tiles, const uint32_t* keys, uint2* ranges, cudaStream_t stream);
 void launch_expand_keys(int64_t N, const uint32_t* tile_keys, const uint32_t* ids, const SplatAux* aux, uint64_t* out,
@@ -148,6 +159,11 @@ void launch_blend_forward(int W, int H, const uint2* ranges, const uint32_t* ord
                           const uint32_t* point_list, const SplatRec* rec,
                           const float* bg, float* out_color, float* final_T, uint32_t* n_contrib, uint8_t* strip_mask,
                           uint8_t* out_rgb8, cudaStream_t stream);  // out_color / out_rgb8: either may be NULL
+// `views` images of one size: global tile g is tile g % (gx * gy) of view g / (gx * gy); out_color [views,3,H,W],
+// out_rgb8 [views,H,W,3] (either may be NULL); forward only
+void launch_blend_forward_views(int views, int W, int H, const uint2* ranges, const uint32_t* order,
+                                const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
+                                const float* bg, float* out_color, uint8_t* out_rgb8, cudaStream_t stream);
 void launch_blend_backward(int W, int H, const uint2* ranges, const uint32_t* order, const uint32_t* order_info,
                            const uint32_t* point_list, const SplatRec* rec,
                            const float* bg, const float* final_T, const uint32_t* n_contrib, const float* dL_dpix,

@@ -47,7 +47,7 @@ import torch
 from . import _native as N
 from . import mesh as M
 from . import rasterizer as R
-from .renderer import _forward_only, render
+from .renderer import _forward_only, _views_forward, camera_table, render
 from .rasterizer import l1_loss_u8
 from .densify import add_densification_stats
 from .training import METRIC_NAMES, Adam, binding_regularizers, launch_image_metrics, metrics_scratch, photometric_loss
@@ -145,11 +145,12 @@ class _Captured:
         dev = pc._xyz.device
         self.device = dev
         self.bg = bg.to(dev).float().contiguous()
-        self.cam = torch.zeros(CAMERA_BLOCK_FOV if self.per_camera_fov else CAMERA_BLOCK, dtype=torch.float32,
-                               device=dev)
+        self.K = getattr(self, "K", 1)   # cameras per replay (GraphedRender(views_per_replay=K)): a (K, 37) table
+        nblk = CAMERA_BLOCK_FOV if self.per_camera_fov else CAMERA_BLOCK
+        self.cam = torch.zeros((self.K, nblk) if self.K > 1 else nblk, dtype=torch.float32, device=dev)
         if self.per_camera_fov:
-            self.cam[CAMERA_BLOCK:] = tanfov_floats(self.fovx, self.fovy).to(dev)
-        self.camera = _GraphCamera(self.W, self.H, self.fovx, self.fovy, self.cam)
+            self.cam[..., CAMERA_BLOCK:] = tanfov_floats(self.fovx, self.fovy).to(dev)
+        self.camera = _GraphCamera(self.W, self.H, self.fovx, self.fovy, self.cam) if self.K == 1 else None
         self.flame = getattr(pc, "flame", None)
         if self.flame is not None:   # the pose is computed inside the graph from this timestep
             self.verts, self.timestep = None, torch.zeros(1, dtype=torch.int32, device=dev)
@@ -217,8 +218,10 @@ class _Captured:
     def _learn_capacity(self):
         """Eager frames (sync modes EXACT then LATE) over the warm-up cameras, each at every warm-up timestep: their
         instance counts size the graph."""
-        hints = R.hints_of(self.pc)
-        key = (self.device, self.W, self.H, self.pc._xyz.shape[0])
+        if self.K > 1:   # a K-view frame learns from K-view frames only (rasterizer.view_hints_of)
+            hints, key = R.view_hints_of(self.pc), (self.device, self.W, self.H, self.pc._xyz.shape[0], self.K)
+        else:
+            hints, key = R.hints_of(self.pc), (self.device, self.W, self.H, self.pc._xyz.shape[0])
         n_max, lo, hi = 0, 0xFFFFFFFF, 0
         cam0 = self.cam.clone()
         t0 = self.timestep.clone() if self._warm_t else None
@@ -612,13 +615,23 @@ class GraphedRender(_Captured):
                  scaling_modifier: float = 1.0, mesh_update: bool = True, host_slots: int = 0,
                  capacity: Optional[int] = None, headroom: float = 1.25, warm_cameras=None, warm_timesteps=None,
                  mesh_opacity: Optional[float] = None, face_colors: Optional[torch.Tensor] = None,
-                 mesh_lighting: str = "front"):
+                 mesh_lighting: str = "front", views_per_replay: int = 1):
         """outputs: "u8" (the display image only: the float image is not written), "float" or "both".
         warm_cameras: camera objects or 37-float blocks rendered eagerly before the capture to size the capacity (and
         the depth-sort range); warm_timesteps: with a FLAME head, the timesteps each warm camera is rendered at
-        (default: the current one) -- a sequence played back whole sizes the graph once for all its frames."""
+        (default: the current one) -- a sequence played back whole sizes the graph once for all its frames.
+        views_per_replay=K > 1: every replay renders K cameras of one timestep in one forward
+        (gab200_forward_views): the head is posed once, set_inputs(cameras=...) takes K cameras (or a (K, 37) table),
+        warm_cameras is a list of such camera groups, and display / image / radii / the host slots carry a leading K
+        dimension.  Not combinable with the mesh overlay."""
         if outputs not in ("u8", "float", "both"):
             raise ValueError("outputs must be 'u8', 'float' or 'both'")
+        if isinstance(views_per_replay, bool) or not isinstance(views_per_replay, int) or \
+                not 1 <= views_per_replay <= N.MAX_VIEWS:
+            raise ValueError(f"views_per_replay must be an int in [1, {N.MAX_VIEWS}]")
+        if views_per_replay > 1 and mesh_opacity is not None:
+            raise ValueError("the mesh overlay draws one camera per replay: it needs views_per_replay=1")
+        self.K = int(views_per_replay)
         if host_slots < 0 or (host_slots > 0 and outputs == "float"):
             raise ValueError("host_slots copies the display image: it needs outputs 'u8' or 'both'")
         # the background is an input (set_inputs writes it): the frame's own copy.  Field of view: tan(45 deg), a
@@ -655,10 +668,30 @@ class GraphedRender(_Captured):
         else:
             self.face_colors.copy_(fc, non_blocking=True)
 
+    def _camera_tensor(self, camera):
+        """With views_per_replay=K > 1: a group of K camera objects (one image size) or a (K, 37) table."""
+        if self.K == 1:
+            return super()._camera_tensor(camera)
+        if isinstance(camera, torch.Tensor):
+            if tuple(camera.shape) != (self.K, CAMERA_BLOCK_FOV):
+                raise ValueError(f"a camera table of this frame is ({self.K}, {CAMERA_BLOCK_FOV}), got "
+                                 f"{tuple(camera.shape)}")
+            return camera.float()
+        cams = list(camera)
+        if len(cams) != self.K:
+            raise ValueError(f"this frame renders {self.K} cameras per replay, got {len(cams)}")
+        return camera_table(cams, self.device)
+
     # ---- inputs ------------------------------------------------------------------------------------------------
-    def set_inputs(self, camera=None, timestep=None, verts=None, bg=None, mesh_opacity=None, face_colors=None):
+    def set_inputs(self, camera=None, timestep=None, verts=None, bg=None, mesh_opacity=None, face_colors=None,
+                   cameras=None):
         """Copies new inputs into the graph's device buffers; none of them re-captures.  A camera OBJECT of another
-        image size changes the frame's size (the next run() re-captures)."""
+        image size changes the frame's size (the next run() re-captures).  views_per_replay=K > 1: `cameras` (K
+        camera objects of one size, or a (K, 37) table) instead of `camera`."""
+        if (camera is not None and self.K > 1) or (cameras is not None and self.K == 1):
+            raise ValueError("a frame with views_per_replay > 1 takes cameras=, one with a single view camera=")
+        if cameras is not None:
+            camera = cameras
         if (mesh_opacity is not None or face_colors is not None) and not self.mesh:
             raise ValueError("mesh_opacity / face_colors need a GraphedRender built with mesh_opacity=")
         if mesh_opacity is not None:
@@ -669,8 +702,10 @@ class GraphedRender(_Captured):
         if camera is not None:
             blk = self._camera_tensor(camera)
             if not isinstance(camera, torch.Tensor):
-                self.W, self.H = int(camera.image_width), int(camera.image_height)
-                self.camera.image_width, self.camera.image_height = self.W, self.H
+                first = camera if self.K == 1 else list(camera)[0]
+                self.W, self.H = int(first.image_width), int(first.image_height)
+                if self.camera is not None:
+                    self.camera.image_width, self.camera.image_height = self.W, self.H
             self.cam.copy_(blk, non_blocking=True)
         if verts is not None:
             if self.verts is None:
@@ -685,8 +720,12 @@ class GraphedRender(_Captured):
         with torch.no_grad():
             if self.mesh_update:
                 self._pose()
-            out = _forward_only(self.camera, self.pc, _Pipe, self.bg, self.scaling_modifier,
-                                self.outputs != "float" and not self.mesh, self.outputs != "u8" or self.mesh)
+            if self.K > 1:   # the K cameras of the table in one forward
+                out = _views_forward(self.cam, self.W, self.H, self.pc, _Pipe, self.bg, self.scaling_modifier,
+                                     self.outputs != "float", self.outputs != "u8")
+            else:
+                out = _forward_only(self.camera, self.pc, _Pipe, self.bg, self.scaling_modifier,
+                                    self.outputs != "float" and not self.mesh, self.outputs != "u8" or self.mesh)
             if self.mesh:
                 out["display_u8"] = self._overlay(out["render"])
         self.image, self.display, self.radii = out["render"], out["display_u8"], out["radii"]
@@ -710,7 +749,8 @@ class GraphedRender(_Captured):
         self.image = self.display = self.radii = None
 
     def _before_capture(self):
-        self.camera.image_width, self.camera.image_height = self.W, self.H
+        if self.camera is not None:
+            self.camera.image_width, self.camera.image_height = self.W, self.H
 
     def _after_capture(self):
         # the mesh tensors the replay writes (the model's attributes are replaced by any eager frame)
@@ -736,7 +776,7 @@ class GraphedRender(_Captured):
 
     def _make_ring(self):
         """Pinned host slots, two device staging copies of the display frame and their events."""
-        k, shape = self.host_slots, (self.H, self.W, 3)
+        k, shape = self.host_slots, (self.H, self.W, 3) if self.K == 1 else (self.K, self.H, self.W, 3)
         if self.host is None or tuple(self.host[0].shape) != shape:
             torch.cuda.synchronize(self.device)
             self.host = [torch.empty(shape, dtype=torch.uint8).pin_memory() for _ in range(k)]
@@ -767,7 +807,7 @@ class GraphedRender(_Captured):
         self._host_replay[h] = i
 
     def host_frame(self, replay: Optional[int] = None) -> torch.Tensor:
-        """The pinned (H,W,3) uint8 slot holding replay `replay` (default: the latest) once its copy has landed."""
+        """The pinned (H,W,3) uint8 slot ((K,H,W,3) with views_per_replay=K) holding replay `replay` (default: the latest) once its copy has landed."""
         if not self.host_slots:
             raise ValueError("host_frame needs host_slots > 0")
         i = self.replays - 1 if replay is None else int(replay)
@@ -822,7 +862,11 @@ class GraphedEval(GraphedRender):
 
     def __init__(self, pc, width: int, height: int, bg: torch.Tensor, views: int, source: str = "float",
                  host_slots: int = 0, capacity: Optional[int] = None, headroom: float = 1.25, warm_cameras=None,
-                 warm_timesteps=None):
+                 warm_timesteps=None, views_per_replay: int = 1):
+        """views_per_replay=K > 1: one replay renders K cameras of one timestep in one forward and scores them into
+        rows view .. view + K - 1 (set_inputs(cameras=K cameras, gt_u8=(K,3,H,W), view=first row)); warm_cameras is a
+        list of K-camera groups.  K is fixed per capture: a last group of fewer views is the business of a
+        single-view (or smaller) GraphedEval."""
         if source not in ("float", "u8"):
             raise ValueError("source must be 'float' (train.py's evaluation of the float render) or 'u8' (the "
                              "display bytes render.py writes, scored as metrics.py reads them)")
@@ -830,13 +874,21 @@ class GraphedEval(GraphedRender):
             raise ValueError("host_slots ships the display image: it needs source='u8'")
         if int(views) < 1:
             raise ValueError("views must be at least 1")
+        if isinstance(views_per_replay, int) and views_per_replay > int(views):
+            raise ValueError(f"views_per_replay={views_per_replay} exceeds the table's {int(views)} rows")
         super().__init__(pc, width, height, bg, outputs="float" if source == "float" else "u8", host_slots=host_slots,
-                         capacity=capacity, headroom=headroom, warm_cameras=warm_cameras, warm_timesteps=warm_timesteps)
+                         capacity=capacity, headroom=headroom, warm_cameras=warm_cameras, warm_timesteps=warm_timesteps,
+                         views_per_replay=views_per_replay)
         self.source, self.views = source, int(views)
         self.table = torch.empty((self.views, N.METRICS_FIELDS), dtype=torch.float32, device=self.device)
         self.reset()
         self.view = torch.zeros(1, dtype=torch.int32, device=self.device)
-        self.gt = torch.zeros((3, self.H, self.W), dtype=torch.uint8, device=self.device)
+        # K > 1: the rows of the replay's views, view + k, one device int32 each
+        self.rows = torch.arange(self.K, dtype=torch.int32, device=self.device) if self.K > 1 else None
+        self.gt = torch.zeros(self._gt_shape(), dtype=torch.uint8, device=self.device)
+
+    def _gt_shape(self):
+        return (3, self.H, self.W) if self.K == 1 else (self.K, 3, self.H, self.W)
         self._metrics_scratch = None
 
     def reset(self):
@@ -844,22 +896,25 @@ class GraphedEval(GraphedRender):
         self.table.fill_(float("nan"))
 
     # ---- inputs ------------------------------------------------------------------------------------------------
-    def set_inputs(self, camera=None, timestep=None, gt_u8=None, view=None, verts=None, bg=None):
+    def set_inputs(self, camera=None, timestep=None, gt_u8=None, view=None, verts=None, bg=None, cameras=None):
         """As GraphedRender.set_inputs, plus the view's ground truth (uint8 (3,H,W), a device tensor or a pinned host
-        tensor) and its row in the table (a host int in [0, views)).  None of them re-captures."""
+        tensor) and its row in the table (a host int in [0, views)).  None of them re-captures.  views_per_replay=K >
+        1: `cameras` (K), gt_u8 (K,3,H,W), and `view` is the first of the K rows (view + K <= views)."""
         if view is not None:
             view = int(view)
-            if not 0 <= view < self.views:
-                raise IndexError(f"view {view} outside the table's {self.views} rows")
-        size = (int(camera.image_height), int(camera.image_width)) \
-            if camera is not None and not isinstance(camera, torch.Tensor) else (self.H, self.W)
-        if gt_u8 is not None and (gt_u8.dtype != torch.uint8 or tuple(gt_u8.shape) != (3, *size)):
-            raise ValueError(f"gt_u8 must be a uint8 (3, {size[0]}, {size[1]}) tensor, got {gt_u8.dtype} "
-                             f"{tuple(gt_u8.shape)}")
-        super().set_inputs(camera=camera, timestep=timestep, verts=verts, bg=bg)
-        if tuple(self.gt.shape) != (3, self.H, self.W):   # a camera of another size (the next run() re-captures)
+            if not 0 <= view <= self.views - self.K:
+                raise IndexError(f"rows {view} .. {view + self.K - 1} outside the table's {self.views} rows")
+        group = camera if self.K == 1 else (None if cameras is None or isinstance(cameras, torch.Tensor)
+                                            else list(cameras)[0])
+        size = (int(group.image_height), int(group.image_width)) \
+            if group is not None and not isinstance(group, torch.Tensor) else (self.H, self.W)
+        want = (3, *size) if self.K == 1 else (self.K, 3, *size)
+        if gt_u8 is not None and (gt_u8.dtype != torch.uint8 or tuple(gt_u8.shape) != want):
+            raise ValueError(f"gt_u8 must be a uint8 {want} tensor, got {gt_u8.dtype} {tuple(gt_u8.shape)}")
+        super().set_inputs(camera=camera, timestep=timestep, verts=verts, bg=bg, cameras=cameras)
+        if tuple(self.gt.shape) != self._gt_shape():   # a camera of another size (the next run() re-captures)
             self._await_upload()
-            self.gt = torch.zeros((3, self.H, self.W), dtype=torch.uint8, device=self.device)
+            self.gt = torch.zeros(self._gt_shape(), dtype=torch.uint8, device=self.device)
         if gt_u8 is not None:
             if gt_u8.device.type == "cpu" and self.device.type == "cuda":
                 if self._side is None:
@@ -870,13 +925,21 @@ class GraphedEval(GraphedRender):
                 self.gt.copy_(gt_u8, non_blocking=True)
         if view is not None:
             self.view.fill_(view)
+            if self.rows is not None:
+                self.rows.copy_(torch.arange(view, view + self.K, dtype=torch.int32), non_blocking=True)
 
     # ---- the frame body: the playback frame, then the metrics of what it rendered ------------------------------
     def _body(self, captured: bool = False):
         super()._body(captured)
         if captured:   # the warm-up frames score nothing: they would write the current view's row
-            launch_image_metrics(self.image if self.source == "float" else self.display, self.gt, self.table,
-                                 row=self.view, skip_flag=self.slot.flag, scratch=self._metrics_scratch)
+            rendered = self.image if self.source == "float" else self.display
+            if self.K == 1:
+                launch_image_metrics(rendered, self.gt, self.table, row=self.view, skip_flag=self.slot.flag,
+                                     scratch=self._metrics_scratch)
+            else:   # one launch per view, each into its own row; an overflowed replay writes none of them
+                for k in range(self.K):
+                    launch_image_metrics(rendered[k], self.gt[k], self.table, row=self.rows[k:k + 1],
+                                         skip_flag=self.slot.flag, scratch=self._metrics_scratch)
 
     def _before_capture(self):
         super()._before_capture()

@@ -576,6 +576,122 @@ def rasterize_bound(raster_settings: GaussianRasterizationSettings, _xyz, _rotat
                                  grad_sink, tanfov, rgb8, bool(float_image))
 
 
+# ================================================================================================================
+# Several cameras of one splat set in one forward (gab200_forward_views)
+# ================================================================================================================
+def view_hints_of(obj) -> "FrameHints":
+    """The FrameHints of a model's multi-view frames, kept apart from its single-view ones (`hints_of`): a K-view
+    frame's instance count and depth range are those of K cameras together, and single-view frames must go on
+    learning only from single-view frames."""
+    h = getattr(obj, "_gab200_view_hints", None)
+    if h is None:
+        h = FrameHints()
+        try:
+            obj._gab200_view_hints = h
+        except Exception:
+            return FrameHints()
+    return h
+
+
+def check_camera_table(cameras, device) -> torch.Tensor:
+    """A multi-view camera table: a contiguous (K, 37) float32 tensor on `device`, 1 <= K <= 65535, row k =
+    camera_block(cam_k, fov=True)."""
+    if not isinstance(cameras, torch.Tensor) or cameras.device != device or cameras.dtype != torch.float32 or \
+            cameras.ndim != 2 or cameras.shape[1] != N.CAMERA_FLOATS or not 1 <= cameras.shape[0] <= N.MAX_VIEWS or \
+            not cameras.is_contiguous():
+        raise ValueError(f"cameras must be a contiguous (K, {N.CAMERA_FLOATS}) float32 tensor on {device} with "
+                         f"1 <= K <= {N.MAX_VIEWS} (rows: camera_block(cam, fov=True))")
+    return cameras
+
+
+def rasterize_bound_views(raster_settings: GaussianRasterizationSettings, cameras: torch.Tensor, _xyz, _rotation,
+                          _scaling, _opacity, features_dc, features_rest, binding=None, face_center=None,
+                          face_orien_mat=None, face_scaling=None, colors_precomp=None, hints: Optional[FrameHints] = None,
+                          display: bool = True, float_image: bool = False):
+    """Fused binding + rasterization of K cameras in ONE forward (gab200_forward_views), forward only.
+
+    `cameras`: (K, 37) float32 device table, row k = camera_block(cam_k, fov=True); each view uses its own matrices,
+    centre and field of view.  raster_settings gives what the views share: image size, background, scale_modifier,
+    sh_degree, debug (its viewmatrix / projmatrix / campos / tanfov* are not read).  Returns (color (K,3,H,W) or None,
+    display (K,H,W,3) uint8 or None, radii (K,P) int32, visibility (K,P) bool), every one bit for bit the K
+    single-camera forwards' (rasterize_bound(..., rgb8=...)).  `hints`: the capacity / depth hints of these frames
+    (view_hints_of(model)); the model's single-view hints are not touched.  No autograd: an input that requires a
+    gradient while grad mode is on is refused."""
+    tensors = [t for t in (_xyz, _rotation, _scaling, _opacity, features_dc, features_rest, face_center,
+                           face_orien_mat, face_scaling, colors_precomp) if t is not None]
+    if torch.is_grad_enabled() and any(t.requires_grad for t in tensors):
+        raise ValueError("rasterize_bound_views is forward only: call it under torch.no_grad() or with detached inputs")
+    if not (display or float_image):
+        raise ValueError("rasterize_bound_views needs display=True and/or float_image=True")
+    rs = raster_settings
+    device = _xyz.device
+    if device.type != "cuda":
+        raise RuntimeError("gaussianavatars_b200 has no CPU path: tensors must be CUDA tensors")
+    cameras = check_camera_table(cameras, device)
+    K, P, H, W = int(cameras.shape[0]), int(_xyz.shape[0]), int(rs.image_height), int(rs.image_width)
+    a = N.ForwardArgs()
+    a.abi_version, a.input_mode, a.P = N.ABI_VERSION, N.INPUT_BOUND_RAW, P
+    a.sh_degree, a.image_width, a.image_height = int(rs.sh_degree), W, H
+    a.scale_modifier, a.prefiltered, a.debug = float(rs.scale_modifier), int(bool(rs.prefiltered)), int(bool(rs.debug))
+    a.need_backward, a.exact_binning = 0, int(_EXACT_BINNING)
+    bg = _cam(rs.bg, "bg", device)
+    a.bg = bg.data_ptr()
+    if _opacity.ndim == 1:
+        _opacity = _opacity[:, None]
+    keep = [_f32c(t, n, device) for t, n in ((_xyz, "_xyz"), (_rotation, "_rotation"), (_scaling, "_scaling"),
+                                              (_opacity, "_opacity"), (features_dc, "_features_dc"),
+                                              (features_rest, "_features_rest"), (colors_precomp, "colors_precomp"))]
+    _xyz, _rotation, _scaling, _opacity, f_dc, f_rest, colors_precomp = keep
+    a.sh_coeffs = 1 + (0 if f_rest is None else f_rest.shape[1])
+    a.means3D, a.rotations, a.scales, a.opacities = _xyz.data_ptr(), _rotation.data_ptr(), _scaling.data_ptr(), \
+        _opacity.data_ptr()
+    a.sh_dc, a.sh_rest, a.colors_precomp = N.ptr(f_dc), N.ptr(f_rest), N.ptr(colors_precomp)
+    if binding is not None:
+        binding = _face_csr(binding, face_center.shape[0])[0] if (binding.dtype != torch.int32 or
+                                                                  not binding.is_contiguous()) else binding
+        face = [_f32c(t, n, device) for t, n in ((face_center, "face_center"), (face_orien_mat, "face_orien_mat"),
+                                                  (face_scaling, "face_scaling"))]
+        keep += face + [binding]
+        a.binding, a.num_faces = binding.data_ptr(), face[0].shape[0]
+        a.face_center, a.face_orien_mat, a.face_scaling = (t.data_ptr() for t in face)
+    color = torch.empty((K, 3, H, W), dtype=torch.float32, device=device) if float_image else None
+    rgb8 = torch.empty((K, H, W, 3), dtype=torch.uint8, device=device) if display else None
+    radii = torch.empty((K, P), dtype=torch.int32, device=device)
+    visible = torch.empty((K, P), dtype=torch.bool, device=device)
+    a.out_color, a.radii, a.visibility = N.ptr(color), radii.data_ptr(), visible.data_ptr()
+    slot = _capture_slot
+    cb, holder = N.begin_forward(device, slot is not None)   # captured: the graph owns its scratch (see _run_forward)
+    if slot is not None:
+        slot.scratch = holder
+    a.alloc_geom = a.alloc_binning = a.alloc_image = cb
+    st = N.FrameState()
+    key = (device, W, H, P, K)
+    if slot is not None:
+        a.sync_mode, a.binning_hint = N.SYNC_NONE, slot.capacity
+        a.depth_hint_lo, a.depth_hint_hi = slot.depth_range
+        a.frame_seq, a.counters_host, a.overflow_flag = slot.seq, slot.counters.data_ptr(), slot.flag.data_ptr()
+    else:
+        hints = hints if hints is not None else FrameHints()
+        a.binning_hint, (a.depth_hint_lo, a.depth_hint_hi) = hints.get(key)
+        a.sync_mode = N.SYNC_LATE if (_SYNC_POLICY == "late" and a.binning_hint > 0) else N.SYNC_EXACT
+        hints.seq = (hints.seq + 1) & 0x7FFFFFFF
+        a.frame_seq = hints.seq
+    with torch.cuda.device(device):
+        stream = torch.cuda.current_stream(device).cuda_stream
+        n = N.lib().gab200_forward_views(C.byref(a), K, cameras.data_ptr(), N.ptr(rgb8), C.byref(st),
+                                         C.c_void_p(stream))
+    N.check(n, "gab200_forward_views")
+    info = dict(num_rendered=int(st.num_rendered), capacity=int(st.binning_capacity), sync_mode=int(a.sync_mode),
+                depth_sort_path=int(st.depth_sort_path), attempts=int(st.attempts), views=K)
+    if slot is not None:
+        slot.info = info
+    else:
+        hints.put(key, n, _widen_depth_range(st.depth_key_min, st.depth_key_max)
+                  if st.depth_key_min <= st.depth_key_max else (0, 0))
+        hints.last = info
+    return color, rgb8, radii, visible
+
+
 def bind_activate(raster_settings_or_modifier, _xyz, _rotation, _scaling, _opacity, binding=None, face_center=None,
                   face_orien_mat=None, face_scaling=None):
     """Exports what the fused preprocess computes for the binding (no autograd): world means3D (P,3), opacities (P,1),

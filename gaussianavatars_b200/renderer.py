@@ -13,6 +13,7 @@ three tensors per call, gaussian_renderer/__init__.py:44-47).
 A camera may carry its field of view in device memory as `cam.tanfov`, a (2,) float32 CUDA tensor
 {tan(FoVx/2), tan(FoVy/2)} (graph.GraphedFrame(per_camera_fov=True) does): the fused route's kernels read it there
 instead of FoVx / FoVy; the reference route cannot and refuses such a camera.
+`render_views(cameras, ...)` renders every camera of a rig (one image size) in one forward, forward only.
 """
 from __future__ import annotations
 
@@ -20,7 +21,8 @@ import math
 
 import torch
 
-from .rasterizer import GaussianRasterizationSettings, GaussianRasterizer, hints_of, rasterize_bound, visible_of
+from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, check_camera_table, hints_of,
+                         rasterize_bound, rasterize_bound_views, view_hints_of, visible_of)
 
 
 def _camera_block(cam, device):
@@ -98,6 +100,67 @@ def render_display(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, f
     blend itself (3 bytes per pixel instead of 12, no eager quantisation chain).  float_image=True also returns the
     float (3,H,W) image as "render" (else None).  Returns {"display_u8", "render", "radii", "visibility_filter"}."""
     return _forward_only(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, True, float_image)
+
+
+def camera_table(cameras, device) -> torch.Tensor:
+    """(K, 37) float32 device table of camera objects: row k = graph.camera_block(cam_k, fov=True), with the camera's
+    device field of view (`cam.tanfov`) when it carries one."""
+    from .graph import camera_block
+    rows = []
+    for cam in cameras:
+        row = camera_block(cam, fov=True).to(device)
+        tanfov = getattr(cam, "tanfov", None)
+        if tanfov is not None:
+            row[35:] = tanfov.to(device)
+        rows.append(row)
+    return torch.stack(rows).contiguous()
+
+
+def render_views(cameras, pc, pipe, bg_color, scaling_modifier=1.0, float_image=False, width=None, height=None):
+    """Every camera of a rig in ONE forward (gab200_forward_views): the fused route, forward only, no autograd.
+    `cameras`: a list of camera objects of one image size (each with its own matrices and field of view), or a
+    (K, 37) float32 device table of camera_block(cam, fov=True) rows together with `width` and `height`.  Returns
+    {"display_u8": (K,H,W,3) uint8, "render": (K,3,H,W) float32 or None (float_image=False), "radii": (K,P) int32,
+    "visibility_filter": (K,P) bool}; view k equals render_display(cameras[k], ...) bit for bit."""
+    if not _has_raw(pc):
+        raise ValueError("render_views needs the fused route: a model exposing the raw parameters "
+                         "(_xyz, _rotation, _scaling, _opacity, _features_dc, _features_rest)")
+    device = pc._xyz.device
+    if isinstance(cameras, torch.Tensor):
+        if width is None or height is None:
+            raise ValueError("a camera table carries no image size: give width= and height=")
+        table, W, H = check_camera_table(cameras, device), int(width), int(height)
+    else:
+        cameras = list(cameras)
+        if not cameras:
+            raise ValueError("render_views needs at least one camera")
+        sizes = {(int(c.image_width), int(c.image_height)) for c in cameras}
+        if len(sizes) != 1:
+            raise ValueError(f"render_views renders cameras of one image size, got {sorted(sizes)}")
+        (W, H), = sizes
+        table = camera_table(cameras, device)
+    return _views_forward(table, W, H, pc, pipe, bg_color, scaling_modifier, True, float_image)
+
+
+def _views_forward(table, W, H, pc, pipe, bg_color, scaling_modifier, display: bool, float_image: bool):
+    """The fused route's K-view forward of a (K, 37) device camera table (render_views, GraphedRender)."""
+    d = lambda t: None if t is None else t.detach()  # noqa: E731
+    with torch.no_grad():
+        rs = GaussianRasterizationSettings(image_height=H, image_width=W, tanfovx=1.0, tanfovy=1.0, bg=bg_color,
+                                           scale_modifier=scaling_modifier, viewmatrix=None, projmatrix=None,
+                                           sh_degree=pc.active_sh_degree, campos=None, prefiltered=False,
+                                           debug=bool(getattr(pipe, "debug", False)))
+        binding = getattr(pc, "binding", None)
+        fc = fR = fs = None
+        if binding is not None:
+            if getattr(pc, "face_center", None) is None:
+                pc.select_mesh_by_timestep(0)
+            fc, fR, fs = pc.face_center, pc.face_orien_mat, pc.face_scaling
+        img, rgb8, radii, visible = rasterize_bound_views(
+            rs, table, d(pc._xyz), d(pc._rotation), d(pc._scaling), d(pc._opacity), d(pc._features_dc),
+            d(pc._features_rest), binding, d(fc), d(fR), d(fs), hints=view_hints_of(pc), display=display,
+            float_image=float_image)
+    return {"display_u8": rgb8, "render": img, "radii": radii, "visibility_filter": visible}
 
 
 def _visible(radii):

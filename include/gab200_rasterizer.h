@@ -271,6 +271,30 @@ int32_t gab200_backward_device_fov(const gab200_backward_args* args, const float
 int64_t gab200_forward_display(const gab200_forward_args* args, const float* tanfov, uint8_t* out_rgb8,
                                gab200_frame_state* state_out, void* stream);
 
+/* Every camera of a rig in one forward: `views` cameras render one splat set, the way a calibrated capture is
+ * rendered and evaluated (all views of a timestep share the pose, so they need one pass, not one each).
+ * cameras: DEVICE float[views][GAB200_CAMERA_FLOATS]; row k = world_view_transform (16) | full_proj_transform (16) |
+ * camera_center (3) | tan(FoVx/2), tan(FoVy/2) -- the 37-float camera block with the field of view.  The kernels read
+ * the table when they run, so a graph replay renders whatever was written there before it.  args->viewmatrix,
+ * projmatrix, campos, tanfovx and tanfovy are ignored; image size, background, scale_modifier, SH degree and the splat
+ * inputs (either input mode, colors_precomp included) are shared by all views.
+ * Outputs: args->out_color [views,3,H,W] float and/or out_rgb8 [views,H,W,3] uint8 (quantised as gab200_forward_display
+ * does); either may be NULL, not both.  args->radii [views,P]; args->visibility [views,P] or NULL.
+ * The frame is K * P virtual splats -- splat i seen by camera k is virtual splat k * P + i and owns the global tiles
+ * k * T .. k * T + T - 1 (T = tiles of one view) -- sorted and blended as one frame.  The stable per-splat depth sort
+ * restricted to view k is camera k's own order and tiles of different views are disjoint, so every output (float
+ * image, bytes, radii, visibility) is bit for bit that of `views` calls of gab200_forward_display with the same
+ * cameras; views == 1 is that call.  A row whose tan(FoV/2) is zero, negative or not finite culls only its view (all
+ * background).
+ * Forward only: need_backward != 0 is GAB200_ERR_INVALID_ARGUMENT.  Every sync mode works as in gab200_forward;
+ * binning_hint is the capacity of the whole K-view frame, and the counters, the sticky overflow_flag and the LATE
+ * re-enqueue behave as documented there.  Before any device work, GAB200_ERR_INVALID_ARGUMENT for: views < 1 or
+ * > 65535, cameras == NULL, views * P > INT32_MAX, views * T > INT32_MAX (the 32-bit tile key), and every error of
+ * gab200_forward_display. */
+#define GAB200_CAMERA_FLOATS 37
+int64_t gab200_forward_views(const gab200_forward_args* args, int32_t views, const float* cameras, uint8_t* out_rgb8,
+                             gab200_frame_state* state_out, void* stream);
+
 /* Frustum test only.  Replaces diff_gaussian_rasterization._C.mark_visible (GaussianRasterizer.markVisible). */
 int32_t gab200_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,
                             uint8_t* present /* [P] 0/1 */, void* stream);
