@@ -60,10 +60,11 @@ static uint32_t depth_bucket_count(int P) {
   while (nb < 8192 && (int64_t)nb * 64 < P) nb <<= 1;
   return nb;
 }
-// The layout is a pure function of (P, need_backward): the only size that depends on anything else (cub's temp
-// storage for the stage-A radix sort, `sort_temp`) is carved LAST, so the backward -- which passes 0 for it, on
-// whatever host thread autograd picked -- sees every other array at the forward's offset.
-static GeomView carve_geom(void* base, int P, bool need_backward, size_t sort_temp) {
+// The layout is a pure function of (P, need_backward, face_rows): the only size that depends on anything else (cub's
+// temp storage for the stage-A radix sort, `sort_temp`) is carved LAST, so the backward -- which passes 0 for it, on
+// whatever host thread autograd picked -- sees every other array at the forward's offset.  face_rows: rows of the
+// face-frame scratch, one per REAL splat (a multi-view training frame has P = views * real splats), < 0: P.
+static GeomView carve_geom(void* base, int P, bool need_backward, size_t sort_temp, int face_rows = -1) {
   GeomView g;
   Carver c(base);
   g.rec = c.take<SplatRec>((size_t)P);
@@ -76,7 +77,8 @@ static GeomView carve_geom(void* base, int P, bool need_backward, size_t sort_te
   g.ids[0] = c.take<uint32_t>((size_t)P);
   g.ids[1] = c.take<uint32_t>((size_t)P);
   g.g2d = need_backward ? c.take<float>((size_t)P * GAB_G2D_STRIDE) : nullptr;
-  g.face_scratch = need_backward ? c.take<float>((size_t)P * GAB_FACE_GRAD_STRIDE) : nullptr;
+  g.face_scratch =
+      need_backward ? c.take<float>((size_t)(face_rows < 0 ? P : face_rows) * GAB_FACE_GRAD_STRIDE) : nullptr;
   g.scan_temp_bytes = scan_temp_bytes(P);
   g.scan_temp = c.take<char>(g.scan_temp_bytes);
   {
@@ -133,7 +135,8 @@ struct ImageView {
   uint32_t* n_contrib;
   size_t bytes;
 };
-// views > 1 (gab200_forward_views, forward only): the tile arrays of all views' tiles
+// views > 1 (gab200_forward_views[_train]): the tile arrays of all views' tiles, and the per-pixel state of all views'
+// pixels
 static ImageView carve_image(void* base, int W, int H, bool need_backward, int views = 1) {
   ImageView v;
   Carver c(base);
@@ -144,8 +147,8 @@ static ImageView carve_image(void* base, int W, int H, bool need_backward, int v
   v.order_info = c.take<uint32_t>(4);
   v.tile_count = c.take<uint32_t>(tiles);
   v.tile_cursor = c.take<uint32_t>(tiles);
-  v.final_T = need_backward ? c.take<float>((size_t)W * H) : nullptr;
-  v.n_contrib = need_backward ? c.take<uint32_t>((size_t)W * H) : nullptr;
+  v.final_T = need_backward ? c.take<float>((size_t)W * H * views) : nullptr;
+  v.n_contrib = need_backward ? c.take<uint32_t>((size_t)W * H * views) : nullptr;
   v.bytes = c.bytes();
   return v;
 }
@@ -380,7 +383,7 @@ int enqueue_geometry(Frame& f, bool bucket, bool run_preprocess, uint32_t capaci
     StageScope sc(GAB200_STAGE_PREPROCESS, stream);
     if (f.cameras != nullptr)
       launch_preprocess_views(*a, f.views, f.cameras, g.rec, g.aux, g.tiles_touched, g.depth_keys[0], g.ids[0],
-                              g.buckets, f.counting ? f.iv.tile_count : nullptr, stream);
+                              g.buckets, f.counting ? f.iv.tile_count : nullptr, f.nb ? g.clamped : nullptr, stream);
     else
       launch_preprocess(*a, g.rec, g.aux, g.tiles_touched, f.nb ? g.clamped : nullptr, g.depth_keys[0], g.ids[0],
                         g.buckets, f.counting ? f.iv.tile_count : nullptr, f.tanfov, stream);
@@ -498,7 +501,11 @@ int enqueue_binning_blend(Frame& f, void* bin, int64_t cap, int64_t n_known, siz
   st->sorted_selector = selector;
   {
     StageScope sc(GAB200_STAGE_BLEND_FWD, stream);
-    if (f.cameras != nullptr)
+    if (f.cameras != nullptr && f.nb)
+      launch_blend_forward_views_train(f.views, f.W, f.H, f.iv.ranges, f.iv.order, f.iv.order_info, bv.vals[selector],
+                                       f.g.rec, a->bg, a->out_color, f.iv.final_T, f.iv.n_contrib, bv.strip_mask,
+                                       stream);
+    else if (f.cameras != nullptr)
       launch_blend_forward_views(f.views, f.W, f.H, f.iv.ranges, f.iv.order, f.iv.order_info, bv.vals[selector], f.g.rec,
                                  a->bg, a->out_color, f.out_rgb8, stream);
     else
@@ -519,8 +526,8 @@ int wait_counters(Frame& f) {
 }  // namespace
 
 // gab200_forward, gab200_forward_device_fov and gab200_forward_display (tanfov == NULL: the by-value tanfovx /
-// tanfovy; out_rgb8 == NULL: no display image), and gab200_forward_views (cameras != NULL: `views` cameras, validated
-// by the caller, as one frame of views * P virtual splats)
+// tanfovy; out_rgb8 == NULL: no display image), and gab200_forward_views[_train] (cameras != NULL: `views` cameras,
+// validated by the caller, as one frame of views * P virtual splats; need_backward: the training form)
 static int64_t run_forward(const gab200_forward_args* a, const float* tanfov, uint8_t* out_rgb8,
                            gab200_frame_state* st, void* stream_, int views = 1, const float* cameras = nullptr) {
   cudaStream_t stream = (cudaStream_t)stream_;
@@ -553,10 +560,10 @@ static int64_t run_forward(const gab200_forward_args* a, const float* tanfov, ui
 
   // ---- geometry + image buffers ----
   const size_t tempA = cached_sort_temp_bytes(P > 0 ? P : 1, 32);
-  GeomView gsz = carve_geom(nullptr, P, f.nb, tempA);
+  GeomView gsz = carve_geom(nullptr, P, f.nb, tempA, a->P);
   void* geom = a->alloc_geom(a->alloc_user, gsz.bytes);
   if (geom == nullptr) return GAB200_ERR_ALLOC;
-  f.g = carve_geom(geom, P, f.nb, tempA);
+  f.g = carve_geom(geom, P, f.nb, tempA, a->P);
   ImageView isz = carve_image(nullptr, f.W, f.H, f.nb, views);
   void* img = a->alloc_image(a->alloc_user, isz.bytes);
   if (img == nullptr) return GAB200_ERR_ALLOC;
@@ -568,6 +575,7 @@ static int64_t run_forward(const gab200_forward_args* a, const float* tanfov, ui
   st->device_counters = f.g.buckets.meta;
   st->attempts = 1;
   st->depth_key_min = 1; st->depth_key_max = 0;  // "nothing visible" until the counters say otherwise
+  st->reserved0 = (cameras != nullptr && f.nb) ? views : 0;  // the K a multi-view backward must be called with
 
   const double t0 = now_us();
   if (P == 0) {  // nothing to bin: background image, empty ranges
@@ -693,6 +701,82 @@ int64_t gab200_forward_views(const gab200_forward_args* a, int32_t views, const 
   return run_forward(&v, nullptr, out_rgb8, st, stream, views, cameras);
 }
 
+// the argument checks gab200_forward_views_train and gab200_backward_views share: the camera table, the limits of the
+// multi-view frame, and the one input form the training kernels exist for (BOUND_RAW with SH colours)
+static bool validate_views_train(const gab200_forward_args* a, int32_t views, const float* cameras,
+                                 gab200_forward_args& v) {
+  if (a == nullptr || views < 1 || views > 65535 || cameras == nullptr) return false;
+  v = *a;
+  v.viewmatrix = v.projmatrix = v.campos = cameras;  // ignored: every view reads its row of the table
+  v.need_backward = 1;
+  if (!validate(&v)) return false;
+  if (v.input_mode != GAB200_INPUT_BOUND_RAW || v.colors_precomp != nullptr) return false;
+  const int64_t view_tiles = (((int64_t)v.image_width + GAB_TILE - 1) / GAB_TILE) *
+                             (((int64_t)v.image_height + GAB_TILE - 1) / GAB_TILE);
+  return (int64_t)views * v.P <= INT32_MAX && (int64_t)views * view_tiles <= INT32_MAX;
+}
+
+int64_t gab200_forward_views_train(const gab200_forward_args* a, int32_t views, const float* cameras,
+                                   gab200_frame_state* st, void* stream) {
+  gab200_forward_args v;
+  if (!validate_views_train(a, views, cameras, v) || st == nullptr) return GAB200_ERR_INVALID_ARGUMENT;
+  return run_forward(&v, nullptr, nullptr, st, stream, views, cameras);
+}
+
+int32_t gab200_backward_views(const gab200_backward_args* b, int32_t views, const float* cameras, void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  if (b == nullptr || b->abi_version != GAB200_ABI_VERSION || b->fwd == nullptr || b->state == nullptr)
+    return GAB200_ERR_INVALID_ARGUMENT;
+  gab200_forward_args v;
+  if (!validate_views_train(b->fwd, views, cameras, v)) return GAB200_ERR_INVALID_ARGUMENT;
+  const gab200_frame_state* st = b->state;
+  if (st->reserved0 != views || b->grads_are_multicast || b->dL_dout_color == nullptr) return GAB200_ERR_INVALID_ARGUMENT;
+  if (b->dL_dsh_dc == nullptr || (v.sh_coeffs > 1 && b->dL_dsh_rest == nullptr)) return GAB200_ERR_INVALID_ARGUMENT;
+  if (st->geom_buffer == nullptr || st->image_buffer == nullptr || st->binning_buffer == nullptr)
+    return GAB200_ERR_INVALID_ARGUMENT;
+  const int P = v.P, W = v.image_width, H = v.image_height;
+  const bool dbg = v.debug != 0;
+  if (P == 0) return GAB200_OK;
+  GeomView g = carve_geom(st->geom_buffer, views * P, true, 0, P);
+  ImageView iv = carve_image(st->image_buffer, W, H, true, views);
+  BinView bv = carve_binning(st->binning_buffer, st->binning_capacity, true, 0);
+  if (g.bytes > st->geom_bytes || iv.bytes > st->image_bytes || bv.bytes > st->binning_bytes)
+    return GAB200_ERR_INVALID_ARGUMENT;  // not the buffers this forward carved
+  cudaStreamCaptureStatus cap_status = cudaStreamCaptureStatusNone;
+  GAB_CUDA(cudaStreamIsCapturing(stream, &cap_status));
+  struct CaptureGuard {
+    bool prev;
+    explicit CaptureGuard(bool c) : prev(t_capturing) { t_capturing = c; }
+    ~CaptureGuard() { t_capturing = prev; }
+  } capture_guard(cap_status != cudaStreamCaptureStatusNone);
+
+  GAB_CUDA(cudaMemsetAsync(g.g2d, 0, sizeof(float) * (size_t)views * P * GAB_G2D_STRIDE, stream));
+  if (v.binding != nullptr) {
+    const size_t F = (size_t)v.num_faces;
+    if (b->dL_dface_center) GAB_CUDA(cudaMemsetAsync(b->dL_dface_center, 0, sizeof(float) * 3 * F, stream));
+    if (b->dL_dface_orien_mat) GAB_CUDA(cudaMemsetAsync(b->dL_dface_orien_mat, 0, sizeof(float) * 9 * F, stream));
+    if (b->dL_dface_scaling) GAB_CUDA(cudaMemsetAsync(b->dL_dface_scaling, 0, sizeof(float) * F, stream));
+  }
+  if (st->num_rendered != 0) {
+    StageScope sc(GAB200_STAGE_BLEND_BWD, stream);
+    launch_blend_backward_views(views, W, H, iv.ranges, iv.order, iv.order_info, bv.vals[st->sorted_selector], g.rec,
+                                v.bg, iv.final_T, iv.n_contrib, b->dL_dout_color, bv.strip_mask, g.g2d, stream);
+  }
+  GAB_STAGE_CHECK(dbg, stream);
+  {
+    StageScope sc(GAB200_STAGE_PREPROCESS_BWD, stream);
+    const bool csr = v.binding != nullptr && b->num_face_chunks > 0 && b->face_perm && b->face_chunk_face &&
+                     b->face_chunk_start && b->face_chunk_end &&
+                     (b->dL_dface_center || b->dL_dface_orien_mat || b->dL_dface_scaling);
+    gab200_backward_args bb = *b;
+    bb.fwd = &v;
+    launch_preprocess_backward_views(bb, views, cameras, g.aux, g.clamped, g.g2d, csr ? g.face_scratch : nullptr,
+                                     stream);
+  }
+  GAB_STAGE_CHECK(dbg, stream);
+  return GAB200_OK;
+}
+
 // gab200_backward and gab200_backward_device_fov
 static int32_t run_backward(const gab200_backward_args* b, const float* tanfov, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
@@ -701,6 +785,7 @@ static int32_t run_backward(const gab200_backward_args* b, const float* tanfov, 
   const gab200_forward_args* a = b->fwd;
   const gab200_frame_state* st = b->state;
   if (!validate(a) || !a->need_backward || b->dL_dout_color == nullptr) return GAB200_ERR_INVALID_ARGUMENT;
+  if (st->reserved0 != 0) return GAB200_ERR_INVALID_ARGUMENT;  // a multi-view frame: gab200_backward_views
   if (st->geom_buffer == nullptr || st->image_buffer == nullptr || st->binning_buffer == nullptr)
     return GAB200_ERR_INVALID_ARGUMENT;
   const int P = a->P, W = a->image_width, H = a->image_height;

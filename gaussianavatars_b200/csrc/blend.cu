@@ -433,6 +433,59 @@ void launch_blend_forward_views(int views, int W, int H, const uint2* ranges, co
   count_launch();
 }
 
+// gab200_forward_views_train: blend_forward_views_kernel with the float image only, keeping what the backward reads --
+// final_T and n_contrib at the view's offset, and the block mask of every instance (indexed by its position in the
+// sorted stream, which is global already).
+__global__ void __launch_bounds__(256) blend_forward_views_train_kernel(int W, int H, int gx, int tiles, int view_tiles,
+                                                                        const uint2* __restrict__ ranges,
+                                                                        const uint32_t* __restrict__ order,
+                                                                        const uint32_t* __restrict__ order_info,
+                                                                        const uint32_t* __restrict__ point_list,
+                                                                        const SplatRec* __restrict__ rec,
+                                                                        const float* __restrict__ bg,
+                                                                        float* __restrict__ out_color,
+                                                                        float* __restrict__ final_T,
+                                                                        uint32_t* __restrict__ n_contrib,
+                                                                        uint8_t* __restrict__ strip_mask) {
+  __shared__ SplatRec buf[2][256];
+  __shared__ uint32_t smask[256];
+  __shared__ __align__(16) uint32_t ids_ring[4][ID_RING * (64 + 4)];
+  __shared__ __align__(8) uint64_t mbar[4][ID_RING];
+  const int nh = (int)order_info[0];
+  const int b = blockIdx.x, t = threadIdx.x;
+  const bool heavy = b < nh;
+  const int g = heavy ? 0 : t >> 6;
+  const int slot = heavy ? b : nh + 4 * (b - nh) + g;
+  if (slot >= (heavy ? nh : tiles)) return;
+  const int tile = (int)order[slot];
+  const int view = tile / view_tiles, local = tile - view * view_tiles;
+  const size_t HW = (size_t)H * W;
+  float* color = out_color + (size_t)view * 3 * HW;
+  float* vT = final_T + (size_t)view * HW;
+  uint32_t* vn = n_contrib + (size_t)view * HW;
+  const uint2* view_ranges = ranges + (size_t)view * view_tiles;
+  if (heavy)
+    forward_tile<1, BLEND_OUT_FLOAT>(local, t, GroupBarrier<256>{0}, buf[0], buf[1], smask, &ids_ring[0][0], mbar[0], W,
+                                     H, gx, view_ranges, point_list, rec, bg, color, vT, vn, strip_mask, nullptr);
+  else
+    forward_tile<4, BLEND_OUT_FLOAT>(local, t & 63, GroupBarrier<64>{1 + g}, buf[0] + g * 64, buf[1] + g * 64,
+                                     smask + g * 64, ids_ring[g], mbar[g], W, H, gx, view_ranges, point_list, rec, bg,
+                                     color, vT, vn, strip_mask, nullptr);
+}
+
+void launch_blend_forward_views_train(int views, int W, int H, const uint2* ranges, const uint32_t* order,
+                                      const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
+                                      const float* bg, float* out_color, float* final_T, uint32_t* n_contrib,
+                                      uint8_t* strip_mask, cudaStream_t stream) {
+  const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
+  const int view_tiles = gx * gy, tiles = views * view_tiles;
+  if (tiles == 0) return;
+  blend_forward_views_train_kernel<<<tiles, 256, 0, stream>>>(W, H, gx, tiles, view_tiles, ranges, order, order_info,
+                                                              point_list, rec, bg, out_color, final_T, n_contrib,
+                                                              strip_mask);
+  count_launch();
+}
+
 // =====================================================================================================
 // Backward
 // =====================================================================================================
@@ -735,6 +788,54 @@ void launch_blend_backward(int W, int H, const uint2* ranges, const uint32_t* or
   if (tiles == 0) return;
   blend_backward_kernel<<<tiles, 128, 0, stream>>>(W, H, gx, tiles, ranges, order, order_info, point_list, rec, bg,
                                                    final_T, n_contrib, dL_dpix, strip_mask, g2d);
+  count_launch();
+}
+
+// gab200_backward_views: blend_backward_kernel over the K * view_tiles global tiles of a multi-view frame.  Global tile
+// g is tile g % view_tiles of view g / view_tiles; its range, final_T, n_contrib and dL/dpixel are offset by view as
+// the multi-view forward offsets them.  The point list holds virtual splat ids and the block masks are indexed by
+// stream position, so records, masks and the K * P rows of g2d need no offset; backward_task runs unchanged.
+__global__ void __launch_bounds__(128, 5) blend_backward_views_kernel(int W, int H, int gx, int tiles, int view_tiles,
+                                                                      const uint2* __restrict__ ranges,
+                                                                      const uint32_t* __restrict__ order,
+                                                                      const uint32_t* __restrict__ order_info,
+                                                                      const uint32_t* __restrict__ point_list,
+                                                                      const SplatRec* __restrict__ rec,
+                                                                      const float* __restrict__ bg,
+                                                                      const float* __restrict__ final_T,
+                                                                      const uint32_t* __restrict__ n_contrib,
+                                                                      const float* __restrict__ dL_dpix,
+                                                                      const uint8_t* __restrict__ strip_mask,
+                                                                      float* __restrict__ g2d) {
+  __shared__ WarpSmem sm[4];
+  const int nh = (int)order_info[1];
+  const int b = blockIdx.x, t = threadIdx.x, w = t >> 5;
+  const bool heavy = b < nh;
+  const int slot = heavy ? b : nh + 2 * (b - nh) + (w >> 1);
+  if (!heavy && slot >= tiles) return;
+  const int tile = (int)order[slot];
+  const int view = tile / view_tiles, local = tile - view * view_tiles;
+  const size_t HW = (size_t)H * W;
+  const uint2* vr = ranges + (size_t)view * view_tiles;
+  const float* vT = final_T + (size_t)view * HW;
+  const uint32_t* vn = n_contrib + (size_t)view * HW;
+  const float* vd = dL_dpix + (size_t)view * 3 * HW;
+  if (heavy)
+    backward_task<2>(local, t, sm[w], W, H, gx, vr, point_list, rec, bg, vT, vn, vd, strip_mask, g2d);
+  else
+    backward_task<4>(local, t & 63, sm[w], W, H, gx, vr, point_list, rec, bg, vT, vn, vd, strip_mask, g2d);
+}
+
+void launch_blend_backward_views(int views, int W, int H, const uint2* ranges, const uint32_t* order,
+                                 const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
+                                 const float* bg, const float* final_T, const uint32_t* n_contrib, const float* dL_dpix,
+                                 const uint8_t* strip_mask, float* g2d, cudaStream_t stream) {
+  const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
+  const int view_tiles = gx * gy, tiles = views * view_tiles;
+  if (tiles == 0) return;
+  blend_backward_views_kernel<<<tiles, 128, 0, stream>>>(W, H, gx, tiles, view_tiles, ranges, order, order_info,
+                                                         point_list, rec, bg, final_T, n_contrib, dL_dpix, strip_mask,
+                                                         g2d);
   count_launch();
 }
 

@@ -101,10 +101,11 @@ void launch_preprocess(const gab200_forward_args& a, SplatRec* rec, SplatAux* au
                        uint8_t* clamped, uint32_t* depth_keys, uint32_t* ids, const DepthBuckets& buckets,
                        uint32_t* tile_count, const float* tanfov, cudaStream_t stream);
 // gab200_forward_views: grid (splat blocks, views); camera row k of `cameras` renders virtual splats k * P + i
-// (rec / aux / tiles / depth keys / ids / radii / visibility), tile counts at k * (gx * gy) + the tile in the view
+// (rec / aux / tiles / depth keys / ids / radii / visibility), tile counts at k * (gx * gy) + the tile in the view;
+// clamped != nullptr (gab200_forward_views_train, BOUND_RAW only): also the colour clamp bits at k * P + i
 void launch_preprocess_views(const gab200_forward_args& a, int views, const float* cameras, SplatRec* rec, SplatAux* aux,
                              uint32_t* tiles_touched, uint32_t* depth_keys, uint32_t* ids, const DepthBuckets& buckets,
-                             uint32_t* tile_count, cudaStream_t stream);
+                             uint32_t* tile_count, uint8_t* clamped, cudaStream_t stream);
 // depth_keys [P] (by splat) -> sorted_ids [M] in (key, id) order and offsets [M] = inclusive instance counts
 // also publishes the frame counters (capacity, seq, overflow) of the bucket-sorted frame
 void launch_depth_bucket_sort(int P, const DepthBuckets& buckets, const uint32_t* depth_keys,
@@ -164,15 +165,32 @@ void launch_blend_forward(int W, int H, const uint2* ranges, const uint32_t* ord
 void launch_blend_forward_views(int views, int W, int H, const uint2* ranges, const uint32_t* order,
                                 const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
                                 const float* bg, float* out_color, uint8_t* out_rgb8, cudaStream_t stream);
+// the training form of the multi-view forward: out_color required, no display image; final_T / n_contrib
+// [views,H,W] and the per-instance block masks are kept for launch_blend_backward_views
+void launch_blend_forward_views_train(int views, int W, int H, const uint2* ranges, const uint32_t* order,
+                                      const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
+                                      const float* bg, float* out_color, float* final_T, uint32_t* n_contrib,
+                                      uint8_t* strip_mask, cudaStream_t stream);
 void launch_blend_backward(int W, int H, const uint2* ranges, const uint32_t* order, const uint32_t* order_info,
                            const uint32_t* point_list, const SplatRec* rec,
                            const float* bg, const float* final_T, const uint32_t* n_contrib, const float* dL_dpix,
                            const uint8_t* strip_mask, float* g2d, cudaStream_t stream);
+// the same over the tiles of `views` images: dL_dpix [views,3,H,W]; g2d rows of the views * P virtual splats
+void launch_blend_backward_views(int views, int W, int H, const uint2* ranges, const uint32_t* order,
+                                 const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
+                                 const float* bg, const float* final_T, const uint32_t* n_contrib, const float* dL_dpix,
+                                 const uint8_t* strip_mask, float* g2d, cudaStream_t stream);
 
 // preprocess_bwd.cu
 void launch_preprocess_backward(const gab200_backward_args& b, const SplatRec* rec, const SplatAux* aux,
                                 const uint8_t* clamped, const float* g2d, float* face_scratch, const float* tanfov,
                                 cudaStream_t stream);
+// gab200_backward_views (BOUND_RAW, no colors_precomp, no multicast): one thread per real splat sums the gradients of
+// its `views` virtual splats (camera row k of `cameras`; rec / aux / clamped / g2d rows k * P + i) and stores each
+// parameter gradient once; dL_dmeans2D [views,P,3]; face-frame gradients as launch_preprocess_backward's
+void launch_preprocess_backward_views(const gab200_backward_args& b, int views, const float* cameras,
+                                      const SplatAux* aux, const uint8_t* clamped, const float* g2d,
+                                      float* face_scratch, cudaStream_t stream);
 #define GAB_FACE_GRAD_STRIDE 13  // per-splat face-frame gradient record: centre 3, orientation 9, scale 1
 
 // face_frame.cu

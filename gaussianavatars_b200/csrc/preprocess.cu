@@ -80,6 +80,32 @@ __global__ void __launch_bounds__(PRE_NT) preprocess_views_kernel(gab200_forward
 #undef GAB_PRE_OUT
 }
 
+// gab200_forward_views_train: preprocess_views_kernel for BOUND_RAW inputs that also keeps the per-channel colour
+// clamp bits of every virtual splat, which the multi-view backward reads
+__global__ void __launch_bounds__(PRE_NT) preprocess_views_train_kernel(gab200_forward_args a,
+                                                                        const float* __restrict__ cameras,
+                                                                        SplatRec* __restrict__ rec,
+                                                                        SplatAux* __restrict__ aux,
+                                                                        uint32_t* __restrict__ tiles_touched,
+                                                                        uint8_t* __restrict__ clamped,
+                                                                        uint32_t* __restrict__ depth_keys,
+                                                                        uint32_t* __restrict__ ids, int exact_binning,
+                                                                        DepthBuckets bk,
+                                                                        uint32_t* __restrict__ view_counts) {
+  constexpr bool BOUND = true, DEVFOV = true;
+  __shared__ Camera cam;
+  __shared__ float sh_s[PRE_NT * SH_SMEM_STRIDE_MAX];
+  const int view = (int)blockIdx.y;
+  const float* row = cameras + (size_t)view * GAB200_CAMERA_FLOATS;
+  stage_camera_row(row, cam);
+  const float* tanfov = row + 35;
+  const int view_tiles = ((a.image_width + GAB_TILE - 1) / GAB_TILE) * ((a.image_height + GAB_TILE - 1) / GAB_TILE);
+  uint32_t* const tile_count = view_counts != nullptr ? view_counts + view * view_tiles : nullptr;
+#define GAB_PRE_OUT (view * a.P + i)
+#include "preprocess_splat.inc"
+#undef GAB_PRE_OUT
+}
+
 void launch_preprocess(const gab200_forward_args& a, SplatRec* rec, SplatAux* aux, uint32_t* tiles_touched,
                        uint8_t* clamped, uint32_t* depth_keys, uint32_t* ids, const DepthBuckets& buckets,
                        uint32_t* tile_count, const float* tanfov, cudaStream_t stream) {
@@ -95,9 +121,15 @@ void launch_preprocess(const gab200_forward_args& a, SplatRec* rec, SplatAux* au
 
 void launch_preprocess_views(const gab200_forward_args& a, int views, const float* cameras, SplatRec* rec, SplatAux* aux,
                              uint32_t* tiles_touched, uint32_t* depth_keys, uint32_t* ids, const DepthBuckets& buckets,
-                             uint32_t* tile_count, cudaStream_t stream) {
+                             uint32_t* tile_count, uint8_t* clamped, cudaStream_t stream) {
   const int threads = PRE_NT, blocks = (a.P + threads - 1) / threads;
   if (blocks == 0) return;
+  if (clamped != nullptr) {  // training frame (BOUND_RAW, checked by the caller)
+    preprocess_views_train_kernel<<<dim3(blocks, views), threads, 0, stream>>>(
+        a, cameras, rec, aux, tiles_touched, clamped, depth_keys, ids, a.exact_binning, buckets, tile_count);
+    count_launch();
+    return;
+  }
   auto kernel = a.input_mode == GAB200_INPUT_BOUND_RAW ? preprocess_views_kernel<true> : preprocess_views_kernel<false>;
   kernel<<<dim3(blocks, views), threads, 0, stream>>>(a, cameras, rec, aux, tiles_touched, depth_keys, ids,
                                                       a.exact_binning, buckets, tile_count);

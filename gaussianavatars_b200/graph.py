@@ -47,7 +47,9 @@ import torch
 from . import _native as N
 from . import mesh as M
 from . import rasterizer as R
-from .renderer import _forward_only, _views_forward, camera_table, render
+from types import SimpleNamespace
+
+from .renderer import _forward_only, _views_forward, camera_table, render, render_views_train
 from .rasterizer import l1_loss_u8
 from .densify import add_densification_stats
 from .training import METRIC_NAMES, Adam, binding_regularizers, launch_image_metrics, metrics_scratch, photometric_loss
@@ -129,6 +131,11 @@ def reduced_grads(buffers, k):
     return buffers[1 - k].all_views[0]
 
 
+def _check_views_per_replay(k):
+    if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= N.MAX_VIEWS:
+        raise ValueError(f"views_per_replay must be an int in [1, {N.MAX_VIEWS}]")
+
+
 class _Captured:
     """What a frame captured into one CUDA graph owns, whether it trains (GraphedFrame) or plays back (GraphedRender):
     the static camera block, the pose input (a device FLAME timestep, or vertices), the instance capacity -- sized by
@@ -136,6 +143,8 @@ class _Captured:
     what the capture baked in, which run() compares to know when to re-capture.  A subclass provides `_body(captured)`,
     `_release()` (drop what the warm-up frames left behind), `_before_capture()` and `_after_capture()`, and extends
     `_state_key()` with what only its own capture bakes in."""
+
+    K = 1   # cameras per replay (views_per_replay); a subclass sets it before __init__
 
     def __init__(self, pc, width, height, fovx, fovy, bg, per_camera_fov, capacity, headroom, warm_cameras,
                  warm_timesteps=None, verts_grad=False):
@@ -167,7 +176,18 @@ class _Captured:
         self._gt_ready = self._done = None   # events ordering an upload against the replays that read its buffer
 
     def _camera_tensor(self, camera):
-        """A camera object or block as this frame's block: 37 floats with per_camera_fov, else as given."""
+        """A camera object or block as this frame's block: 37 floats with per_camera_fov, else as given.  A frame of K > 1
+        views per replay: a group of K camera objects (one image size) or a (K, 37) table."""
+        if self.K > 1:
+            if isinstance(camera, torch.Tensor):
+                if tuple(camera.shape) != (self.K, CAMERA_BLOCK_FOV):
+                    raise ValueError(f"a camera table of this frame is ({self.K}, {CAMERA_BLOCK_FOV}), got "
+                                     f"{tuple(camera.shape)}")
+                return camera.float()
+            cams = list(camera)
+            if len(cams) != self.K:
+                raise ValueError(f"this frame renders {self.K} cameras per replay, got {len(cams)}")
+            return camera_table(cams, self.device)
         blk = camera if isinstance(camera, torch.Tensor) else camera_block(camera, fov=self.per_camera_fov)
         if self.per_camera_fov and blk.numel() != CAMERA_BLOCK_FOV:
             raise ValueError(f"a {type(self).__name__} camera block with the field of view has {CAMERA_BLOCK_FOV} "
@@ -324,7 +344,7 @@ class GraphedFrame(_Captured):
                  lambda_dssim: float = 0.2, host_inputs: bool = False, capacity: Optional[int] = None,
                  headroom: float = 1.25, after_backward=None, warm_cameras=None, regularizers: Optional[dict] = None,
                  before_backward=None, side_work=None, side_work_at: str = "start", optimizer: Optional[Adam] = None,
-                 densify_stats: bool = False, per_camera_fov: bool = False):
+                 densify_stats: bool = False, per_camera_fov: bool = False, views_per_replay: int = 1):
         """loss: "l1_u8" (L1 vs a uint8 ground truth), "photometric" ((1-l) L1 + l (1-SSIM) vs a uint8 ground truth) or
         "dL_dimage" (the caller supplies dL/dimage in `self.dL_dimage`).
         host_inputs: the frame owns pinned STAGING tensors (`cam_stage` (35,) float32, `gt_stage` (3,H,W) uint8) that a
@@ -360,7 +380,16 @@ class GraphedFrame(_Captured):
         tan(FoVx/2), tan(FoVy/2) (`camera_block(cam, fov=True)`), read by the kernels on every replay; fovx / fovy
         only seed the initial block.  set_inputs(camera=), warm_cameras, the staging tensors and prefetch_for then
         all carry 37 floats, and the warm-up sizes the capacity with each warm camera's own FoV.  The FoV is not
-        part of what triggers a re-capture."""
+        part of what triggers a re-capture.
+        views_per_replay=K > 1: one replay is one training iteration over K cameras of one timestep
+        (renderer.render_views_train: one forward and one backward for the K views, the gradients summed over them).
+        The camera input is a (K, 37) device table (per_camera_fov is implied): set_inputs(cameras=K camera objects
+        of one image size, or a (K, 37) table), warm_cameras is a list of such groups, and gt_u8 / dL_dimage /
+        gt_stage / image are (K,3,H,W), cam_stage (K,37), radii (K,P), viewspace_points (K,P,3).  The loss is
+        K x the batch loss (one mean over the K images), i.e. the sum of the K per-view losses, plus the regularisers
+        once per view with that view's radii; densify_stats feeds the K rows to the statistics in view order; the
+        optimizer takes ONE step per replay.  Changing cameras, timestep or ground truth never re-captures.
+        views_per_replay=1 is the single-camera frame."""
         if loss not in ("l1_u8", "photometric", "dL_dimage"):
             raise ValueError("loss must be 'l1_u8', 'photometric' or 'dL_dimage'")
         if regularizers is not None and loss == "dL_dimage":
@@ -368,8 +397,10 @@ class GraphedFrame(_Captured):
         if optimizer is not None and not (isinstance(optimizer, Adam) and
                                           all(g.get("capturable", False) for g in optimizer.param_groups)):
             raise ValueError("optimizer must be a gaussianavatars_b200.Adam with capturable=True")
-        super().__init__(pc, width, height, fovx, fovy, bg, per_camera_fov, capacity, headroom, warm_cameras,
-                         verts_grad=True)
+        _check_views_per_replay(views_per_replay)
+        self.K = int(views_per_replay)
+        super().__init__(pc, width, height, fovx, fovy, bg, per_camera_fov or self.K > 1, capacity, headroom,
+                         warm_cameras, verts_grad=True)
         self.loss_kind, self.lambda_dssim, self.host_inputs = loss, float(lambda_dssim), bool(host_inputs)
         self.after_backward = after_backward
         self.before_backward = before_backward   # e.g. SymmetricGradBuffer.begin
@@ -378,14 +409,15 @@ class GraphedFrame(_Captured):
         self.regularizers = regularizers
         self.optimizer = optimizer
         self.densify_stats = bool(densify_stats)
-        dev, nblk = self.device, self.cam.numel()
-        self.gt = torch.zeros((3, self.H, self.W), dtype=torch.uint8, device=dev) if loss != "dL_dimage" else None
-        self.dL_dimage = torch.zeros((3, self.H, self.W), dtype=torch.float32, device=dev) if loss == "dL_dimage" else None
-        self.cam_host = torch.zeros(nblk, dtype=torch.float32).pin_memory() if host_inputs else None  # staging
+        dev = self.device
+        img = self._gt_shape()
+        self.gt = torch.zeros(img, dtype=torch.uint8, device=dev) if loss != "dL_dimage" else None
+        self.dL_dimage = torch.zeros(img, dtype=torch.float32, device=dev) if loss == "dL_dimage" else None
+        self.cam_host = torch.zeros(self.cam.shape, dtype=torch.float32).pin_memory() if host_inputs else None  # staging
         if self.cam_host is not None:
             self.cam_host.copy_(self.cam)
         self.cam_stage = self.cam_host
-        self.gt_stage = (torch.zeros((3, self.H, self.W), dtype=torch.uint8).pin_memory()
+        self.gt_stage = (torch.zeros(img, dtype=torch.uint8).pin_memory()
                          if host_inputs and self.gt is not None else None)
         self._prefetch_target = None
         self.loss_host = torch.zeros((), dtype=torch.float32).pin_memory()
@@ -394,10 +426,26 @@ class GraphedFrame(_Captured):
         self._side = torch.cuda.Stream(device=dev) if (host_inputs or side_work is not None) else None
         self._uploads = bool(host_inputs)
 
+    def _gt_shape(self):
+        return (3, self.H, self.W) if self.K == 1 else (self.K, 3, self.H, self.W)
+
     # ---- inputs ------------------------------------------------------------------------------------------------
-    def set_inputs(self, camera=None, verts=None, gt_u8=None, dL_dimage=None, timestep=None):
+    def set_inputs(self, camera=None, verts=None, gt_u8=None, dL_dimage=None, timestep=None, cameras=None):
         """Copies new inputs into the static buffers (device tensors) / staging buffers (host_inputs).  `timestep`
-        (a model with a FLAME head only) is a host int checked against the model's number of timesteps."""
+        (a model with a FLAME head only) is a host int checked against the model's number of timesteps.
+        views_per_replay=K > 1: `cameras` (K camera objects of the frame's image size, or a (K, 37) table) instead of
+        `camera`; gt_u8 / dL_dimage are (K,3,H,W)."""
+        if (camera is not None and self.K > 1) or (cameras is not None and self.K == 1):
+            raise ValueError("a frame with views_per_replay > 1 takes cameras=, one with a single view camera=")
+        if cameras is not None:
+            camera = cameras
+        for name, t in (("gt_u8", gt_u8), ("dL_dimage", dL_dimage)):
+            if t is not None and self.K > 1 and tuple(t.shape) != self._gt_shape():
+                raise ValueError(f"{name} of this frame is {self._gt_shape()}, got {tuple(t.shape)}")
+        if camera is not None and self.K > 1 and not isinstance(camera, torch.Tensor):
+            sizes = {(int(c.image_width), int(c.image_height)) for c in camera}
+            if sizes != {(self.W, self.H)}:
+                raise ValueError(f"the cameras of this frame are {self.W}x{self.H}, got {sorted(sizes)}")
         self._set_pose_input(verts, timestep)
         if camera is not None:
             blk = self._camera_tensor(camera)
@@ -427,6 +475,8 @@ class GraphedFrame(_Captured):
             raise ValueError("prefetching needs host_inputs=True on both frames")
         if self.per_camera_fov != other.per_camera_fov:
             raise ValueError("both frames of a prefetching pair must use the same per_camera_fov mode")
+        if self.K != other.K:
+            raise ValueError("both frames of a prefetching pair must render the same number of views per replay")
         self._prefetch_target = other
         return self
 
@@ -465,14 +515,21 @@ class GraphedFrame(_Captured):
                 if self.side_work is not None and self.side_work_at == "start":
                     self.side_work()
         self._pose()
-        out = render(self.camera, pc, _Pipe, self.bg)
+        if self.K > 1:   # the K cameras of the table in one forward and one backward
+            out = render_views_train(self.cam, pc, _Pipe, self.bg, width=self.W, height=self.H)
+        else:
+            out = render(self.camera, pc, _Pipe, self.bg)
         img = out["render"]
+        radii_rows = [out["radii"]] if self.K == 1 else list(out["radii"])
         if self.loss_kind in ("l1_u8", "photometric"):
             loss = l1_loss_u8(img, self.gt) if self.loss_kind == "l1_u8" else photometric_loss(img, self.gt, self.lambda_dssim)
+            if self.K > 1:   # one mean over the K images: K x it is the sum of the per-view losses
+                loss = loss * float(self.K)
             if self.regularizers is not None:
-                lx, ls = binding_regularizers(pc._xyz, pc._scaling, out["radii"], getattr(pc, "binding", None),
-                                              getattr(pc, "face_scaling", None), **self.regularizers)
-                loss = loss + lx + ls
+                for radii in radii_rows:   # train.py:134-146 per view, with that view's visibility
+                    lx, ls = binding_regularizers(pc._xyz, pc._scaling, radii, getattr(pc, "binding", None),
+                                                  getattr(pc, "face_scaling", None), **self.regularizers)
+                    loss = loss + lx + ls
             self._fork_side_at_backward()
             if self.before_backward is not None:
                 self.before_backward()
@@ -488,7 +545,12 @@ class GraphedFrame(_Captured):
         if captured:
             skip = self.slot.flag
             if self.densify_stats:
-                add_densification_stats(pc, out["viewspace_points"], out["radii"], skip_flag=skip)
+                if self.K == 1:
+                    add_densification_stats(pc, out["viewspace_points"], out["radii"], skip_flag=skip)
+                else:   # the K views' rows in view order: the state after K single-view frames
+                    vp = out["viewspace_points"].grad
+                    for k in range(self.K):
+                        add_densification_stats(pc, SimpleNamespace(grad=vp[k]), out["radii"][k], skip_flag=skip)
             if self.optimizer is not None:
                 self.optimizer.step(skip_flag=skip)
         if loss is not None:
@@ -626,9 +688,7 @@ class GraphedRender(_Captured):
         dimension.  Not combinable with the mesh overlay."""
         if outputs not in ("u8", "float", "both"):
             raise ValueError("outputs must be 'u8', 'float' or 'both'")
-        if isinstance(views_per_replay, bool) or not isinstance(views_per_replay, int) or \
-                not 1 <= views_per_replay <= N.MAX_VIEWS:
-            raise ValueError(f"views_per_replay must be an int in [1, {N.MAX_VIEWS}]")
+        _check_views_per_replay(views_per_replay)
         if views_per_replay > 1 and mesh_opacity is not None:
             raise ValueError("the mesh overlay draws one camera per replay: it needs views_per_replay=1")
         self.K = int(views_per_replay)
@@ -667,20 +727,6 @@ class GraphedRender(_Captured):
             self.face_colors = fc.to(self.device, torch.float32).contiguous().clone()
         else:
             self.face_colors.copy_(fc, non_blocking=True)
-
-    def _camera_tensor(self, camera):
-        """With views_per_replay=K > 1: a group of K camera objects (one image size) or a (K, 37) table."""
-        if self.K == 1:
-            return super()._camera_tensor(camera)
-        if isinstance(camera, torch.Tensor):
-            if tuple(camera.shape) != (self.K, CAMERA_BLOCK_FOV):
-                raise ValueError(f"a camera table of this frame is ({self.K}, {CAMERA_BLOCK_FOV}), got "
-                                 f"{tuple(camera.shape)}")
-            return camera.float()
-        cams = list(camera)
-        if len(cams) != self.K:
-            raise ValueError(f"this frame renders {self.K} cameras per replay, got {len(cams)}")
-        return camera_table(cams, self.device)
 
     # ---- inputs ------------------------------------------------------------------------------------------------
     def set_inputs(self, camera=None, timestep=None, verts=None, bg=None, mesh_opacity=None, face_colors=None,

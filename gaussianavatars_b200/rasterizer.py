@@ -692,6 +692,172 @@ def rasterize_bound_views(raster_settings: GaussianRasterizationSettings, camera
     return color, rgb8, radii, visible
 
 
+class _RasterizeBoundViews(torch.autograd.Function):
+    """The K cameras of one timestep as one training frame (gab200_forward_views_train / gab200_backward_views)."""
+
+    @staticmethod
+    def forward(ctx, _xyz, means2D, _rotation, _scaling, _opacity, f_dc, f_rest, face_center, face_orien_mat,
+                face_scaling, binding, cameras, raster_settings, grad_sink, hints):
+        rs = raster_settings
+        ctx.grad_sink = grad_sink
+        device = _xyz.device
+        K, P, H, W = int(cameras.shape[0]), int(_xyz.shape[0]), int(rs.image_height), int(rs.image_width)
+        a = N.ForwardArgs()
+        a.abi_version, a.input_mode, a.P = N.ABI_VERSION, N.INPUT_BOUND_RAW, P
+        a.sh_degree, a.image_width, a.image_height = int(rs.sh_degree), W, H
+        a.scale_modifier, a.prefiltered, a.debug = float(rs.scale_modifier), int(bool(rs.prefiltered)), int(bool(rs.debug))
+        a.need_backward, a.exact_binning = 1, int(_EXACT_BINNING)
+        bg = _cam(rs.bg, "bg", device)
+        a.bg = bg.data_ptr()
+        _xyz, _rotation = _f32c(_xyz, "_xyz", device), _f32c(_rotation, "_rotation", device)
+        _scaling, _opacity = _f32c(_scaling, "_scaling", device), _f32c(_opacity, "_opacity", device)
+        f_dc, f_rest = _f32c(f_dc, "_features_dc", device), _f32c(f_rest, "_features_rest", device)
+        M = 1 + (0 if f_rest is None else f_rest.shape[1])
+        a.sh_coeffs = M
+        a.means3D, a.rotations, a.scales, a.opacities = _xyz.data_ptr(), _rotation.data_ptr(), _scaling.data_ptr(), \
+            _opacity.data_ptr()
+        a.sh_dc, a.sh_rest = N.ptr(f_dc), N.ptr(f_rest)
+        F = 0
+        binding_orig = binding
+        if binding is not None:
+            if binding.dtype != torch.int32 or not binding.is_contiguous():
+                binding = _face_csr(binding_orig, face_center.shape[0])[0]
+            face_center = _f32c(face_center, "face_center", device)
+            face_orien_mat = _f32c(face_orien_mat, "face_orien_mat", device)
+            face_scaling = _f32c(face_scaling, "face_scaling", device)
+            F = face_center.shape[0]
+            a.binding, a.num_faces = binding.data_ptr(), F
+            a.face_center, a.face_orien_mat, a.face_scaling = face_center.data_ptr(), face_orien_mat.data_ptr(), \
+                face_scaling.data_ptr()
+        color = torch.empty((K, 3, H, W), dtype=torch.float32, device=device)
+        radii = torch.empty((K, P), dtype=torch.int32, device=device)
+        visible = torch.empty((K, P), dtype=torch.bool, device=device)
+        a.out_color, a.radii, a.visibility = color.data_ptr(), radii.data_ptr(), visible.data_ptr()
+        _tls.visible = (radii.data_ptr(), visible)
+        slot = _capture_slot
+        cb, holder = N.begin_forward(device, True)
+        a.alloc_geom = a.alloc_binning = a.alloc_image = cb
+        st = N.FrameState()
+        key = (device, W, H, P, K)
+        if slot is not None:
+            a.sync_mode, a.binning_hint = N.SYNC_NONE, slot.capacity
+            a.depth_hint_lo, a.depth_hint_hi = slot.depth_range
+            a.frame_seq, a.counters_host, a.overflow_flag = slot.seq, slot.counters.data_ptr(), slot.flag.data_ptr()
+        else:
+            a.binning_hint, (a.depth_hint_lo, a.depth_hint_hi) = hints.get(key)
+            a.sync_mode = N.SYNC_LATE if (_SYNC_POLICY == "late" and a.binning_hint > 0) else N.SYNC_EXACT
+            hints.seq = (hints.seq + 1) & 0x7FFFFFFF
+            a.frame_seq = hints.seq
+        with torch.cuda.device(device):
+            stream = torch.cuda.current_stream(device).cuda_stream
+            n = N.lib().gab200_forward_views_train(C.byref(a), K, cameras.data_ptr(), C.byref(st), C.c_void_p(stream))
+        N.check(n, "gab200_forward_views_train")
+        info = dict(num_rendered=int(st.num_rendered), capacity=int(st.binning_capacity), sync_mode=int(a.sync_mode),
+                    depth_sort_path=int(st.depth_sort_path), attempts=int(st.attempts), views=K)
+        if slot is not None:
+            slot.info = info
+        else:
+            hints.put(key, n, _widen_depth_range(st.depth_key_min, st.depth_key_max)
+                      if st.depth_key_min <= st.depth_key_max else (0, 0))
+            hints.last = info
+        ctx.args, ctx.state, ctx.holder = a, st, holder
+        ctx.keep = (bg, cameras, _xyz, _rotation, _scaling, _opacity, f_dc, f_rest, face_center, face_orien_mat,
+                    face_scaling, binding)
+        ctx.dims = (K, P, M, F)
+        ctx.face_shapes = None if binding is None else (face_center.shape, face_orien_mat.shape, face_scaling.shape)
+        ctx.want_face = binding is not None and any(ctx.needs_input_grad[7:10])
+        ctx.csr = _face_csr(binding_orig, F)[1] if ctx.want_face else None
+        ctx.mark_non_differentiable(radii)
+        return color, radii
+
+    @staticmethod
+    def backward(ctx, grad_out_color, _grad_radii):
+        a, st = ctx.args, ctx.state
+        K, P, M, F = ctx.dims
+        cameras = ctx.keep[1]
+        device = cameras.device
+        g = grad_out_color if grad_out_color.is_contiguous() else grad_out_color.contiguous()
+        # the flat per-splat gradient buffer of _RasterizeBound: [_xyz 3 | _rotation 4 | _scaling 3 | _opacity 1 |
+        # f_dc 3 | f_rest 3(M-1)], holding the sum over the K views
+        widths = (3, 4, 3, 1, 3, 3 * (M - 1))
+        symm = getattr(ctx.grad_sink, "symm_grad", None) if ctx.grad_sink is not None else None
+        use_symm = symm is not None and symm.enabled and symm.numel == P * sum(widths)
+        flat = symm.flat if use_symm else torch.empty((P * sum(widths),), dtype=torch.float32, device=device)
+        views, off = [], 0
+        for w in widths:
+            views.append(flat[off:off + P * w])
+            off += P * w
+        d_xyz, d_rot, d_scale, d_opac = views[0].view(P, 3), views[1].view(P, 4), views[2].view(P, 3), views[3].view(P, 1)
+        d_dc = views[4].view(P, 1, 3)
+        d_rest = views[5].view(P, M - 1, 3) if M > 1 else None
+        d_means2D = torch.empty((K, P, 3), dtype=torch.float32, device=device)
+        d_fc = d_fR = d_fs = None
+        if ctx.want_face:
+            fshape = ctx.face_shapes
+            d_fc = torch.empty(fshape[0], dtype=torch.float32, device=device)
+            d_fR = torch.empty(fshape[1], dtype=torch.float32, device=device)
+            d_fs = torch.empty(fshape[2], dtype=torch.float32, device=device)
+        b = N.BackwardArgs()
+        b.abi_version = N.ABI_VERSION
+        b.fwd, b.state = C.pointer(a), C.pointer(st)
+        b.dL_dout_color = g.data_ptr()
+        b.dL_dmeans3D, b.dL_dopacity, b.dL_dmeans2D = d_xyz.data_ptr(), d_opac.data_ptr(), d_means2D.data_ptr()
+        b.dL_dsh_dc, b.dL_dsh_rest = d_dc.data_ptr(), N.ptr(d_rest)
+        b.dL_dscales, b.dL_drotations = d_scale.data_ptr(), d_rot.data_ptr()
+        b.dL_dface_center, b.dL_dface_orien_mat, b.dL_dface_scaling = N.ptr(d_fc), N.ptr(d_fR), N.ptr(d_fs)
+        if ctx.csr is not None:
+            perm, c_face, c_start, c_end = ctx.csr
+            b.face_perm, b.face_chunk_face = perm.data_ptr(), c_face.data_ptr()
+            b.face_chunk_start, b.face_chunk_end = c_start.data_ptr(), c_end.data_ptr()
+            b.num_face_chunks = c_face.shape[0]
+        with torch.cuda.device(device):
+            stream = torch.cuda.current_stream(device).cuda_stream
+            N.check(N.lib().gab200_backward_views(C.byref(b), K, cameras.data_ptr(), C.c_void_p(stream)),
+                    "gab200_backward_views")
+        ctx.holder = None
+        if ctx.grad_sink is not None:  # dist.py all-reduces this buffer, as after a single-view backward
+            ctx.grad_sink.flat_grad = flat
+            ctx.grad_sink._gab200_mc_used = bool(use_symm)
+        return (d_xyz, d_means2D, d_rot, d_scale, d_opac, d_dc, d_rest, d_fc, d_fR, d_fs, None, None, None, None, None)
+
+
+def rasterize_bound_views_train(raster_settings: GaussianRasterizationSettings, cameras: torch.Tensor, _xyz, _rotation,
+                                _scaling, _opacity, features_dc, features_rest, binding=None, face_center=None,
+                                face_orien_mat=None, face_scaling=None, means2D=None, colors_precomp=None,
+                                grad_sink=None, hints: Optional[FrameHints] = None):
+    """Fused binding + rasterization of the K cameras of one timestep as ONE training frame, differentiable.
+
+    `cameras` and `raster_settings` as in rasterize_bound_views.  Returns (color (K,3,H,W), radii (K,P) int32); images
+    and radii equal the K single-camera forwards' bit for bit.  The backward writes the sum over the views of every
+    single-camera gradient: the raw parameters (into the flat per-splat buffer of rasterize_bound, handed to
+    `grad_sink.flat_grad`) and the face frame.  `means2D` is a (K,P,3) holder whose .grad row k receives camera k's
+    dL/dmean2D.  `hints`: the capacity / depth hints of these frames (default: view_hints_of(grad_sink)).  The kernels
+    exist for SH colours and plain stores only: colors_precomp, and a grad_sink whose symmetric gradient buffer is in
+    "push" (multicast) mode, are refused."""
+    if colors_precomp is not None:
+        raise ValueError("rasterize_bound_views_train takes SH colours only (no colors_precomp)")
+    symm = getattr(grad_sink, "symm_grad", None) if grad_sink is not None else None
+    if symm is not None and symm.enabled and getattr(symm, "mode", "push") == "push":
+        raise ValueError("rasterize_bound_views_train writes plain gradients: use the symmetric gradient buffer in "
+                         "'two_shot' or 'plain' mode, not 'push'")
+    device = _xyz.device
+    if device.type != "cuda":
+        raise RuntimeError("gaussianavatars_b200 has no CPU path: tensors must be CUDA tensors")
+    cameras = check_camera_table(cameras, device)
+    K, P = int(cameras.shape[0]), int(_xyz.shape[0])
+    if means2D is None:
+        means2D = torch.zeros((K, P, 3), dtype=torch.float32, device=device)
+    elif tuple(means2D.shape) != (K, P, 3):
+        raise ValueError(f"means2D must be a ({K}, {P}, 3) holder, got {tuple(means2D.shape)}")
+    if _opacity.ndim == 1:
+        _opacity = _opacity[:, None]
+    if hints is None:
+        hints = view_hints_of(grad_sink) if grad_sink is not None else FrameHints()
+    return _RasterizeBoundViews.apply(_xyz, means2D, _rotation, _scaling, _opacity, features_dc, features_rest,
+                                      face_center, face_orien_mat, face_scaling, binding, cameras, raster_settings,
+                                      grad_sink, hints)
+
+
 def bind_activate(raster_settings_or_modifier, _xyz, _rotation, _scaling, _opacity, binding=None, face_center=None,
                   face_orien_mat=None, face_scaling=None):
     """Exports what the fused preprocess computes for the binding (no autograd): world means3D (P,3), opacities (P,1),

@@ -13,7 +13,8 @@ three tensors per call, gaussian_renderer/__init__.py:44-47).
 A camera may carry its field of view in device memory as `cam.tanfov`, a (2,) float32 CUDA tensor
 {tan(FoVx/2), tan(FoVy/2)} (graph.GraphedFrame(per_camera_fov=True) does): the fused route's kernels read it there
 instead of FoVx / FoVy; the reference route cannot and refuses such a camera.
-`render_views(cameras, ...)` renders every camera of a rig (one image size) in one forward, forward only.
+`render_views(cameras, ...)` renders every camera of a rig (one image size) in one forward, forward only;
+`render_views_train(cameras, ...)` is its differentiable form, for a training step over every camera of a timestep.
 """
 from __future__ import annotations
 
@@ -22,7 +23,8 @@ import math
 import torch
 
 from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, check_camera_table, hints_of,
-                         rasterize_bound, rasterize_bound_views, view_hints_of, visible_of)
+                         rasterize_bound, rasterize_bound_views, rasterize_bound_views_train, view_hints_of,
+                         visible_of)
 
 
 def _camera_block(cam, device):
@@ -122,40 +124,71 @@ def render_views(cameras, pc, pipe, bg_color, scaling_modifier=1.0, float_image=
     (K, 37) float32 device table of camera_block(cam, fov=True) rows together with `width` and `height`.  Returns
     {"display_u8": (K,H,W,3) uint8, "render": (K,3,H,W) float32 or None (float_image=False), "radii": (K,P) int32,
     "visibility_filter": (K,P) bool}; view k equals render_display(cameras[k], ...) bit for bit."""
+    table, W, H = _views_table(cameras, pc, width, height, "render_views")
+    return _views_forward(table, W, H, pc, pipe, bg_color, scaling_modifier, True, float_image)
+
+
+def _views_table(cameras, pc, width, height, what):
+    """(table, W, H) of render_views' `cameras` argument: camera objects of one size, or a table with its size."""
     if not _has_raw(pc):
-        raise ValueError("render_views needs the fused route: a model exposing the raw parameters "
+        raise ValueError(f"{what} needs the fused route: a model exposing the raw parameters "
                          "(_xyz, _rotation, _scaling, _opacity, _features_dc, _features_rest)")
     device = pc._xyz.device
     if isinstance(cameras, torch.Tensor):
         if width is None or height is None:
             raise ValueError("a camera table carries no image size: give width= and height=")
-        table, W, H = check_camera_table(cameras, device), int(width), int(height)
-    else:
-        cameras = list(cameras)
-        if not cameras:
-            raise ValueError("render_views needs at least one camera")
-        sizes = {(int(c.image_width), int(c.image_height)) for c in cameras}
-        if len(sizes) != 1:
-            raise ValueError(f"render_views renders cameras of one image size, got {sorted(sizes)}")
-        (W, H), = sizes
-        table = camera_table(cameras, device)
-    return _views_forward(table, W, H, pc, pipe, bg_color, scaling_modifier, True, float_image)
+        return check_camera_table(cameras, device), int(width), int(height)
+    cameras = list(cameras)
+    if not cameras:
+        raise ValueError(f"{what} needs at least one camera")
+    sizes = {(int(c.image_width), int(c.image_height)) for c in cameras}
+    if len(sizes) != 1:
+        raise ValueError(f"{what} renders cameras of one image size, got {sorted(sizes)}")
+    (W, H), = sizes
+    return camera_table(cameras, device), W, H
+
+
+def _views_settings(W, H, pc, pipe, bg_color, scaling_modifier):
+    return GaussianRasterizationSettings(image_height=H, image_width=W, tanfovx=1.0, tanfovy=1.0, bg=bg_color,
+                                         scale_modifier=scaling_modifier, viewmatrix=None, projmatrix=None,
+                                         sh_degree=pc.active_sh_degree, campos=None, prefiltered=False,
+                                         debug=bool(getattr(pipe, "debug", False)))
+
+
+def _face_frame_of(pc):
+    binding = getattr(pc, "binding", None)
+    if binding is None:
+        return None, (None, None, None)
+    if getattr(pc, "face_center", None) is None:
+        pc.select_mesh_by_timestep(0)
+    return binding, (pc.face_center, pc.face_orien_mat, pc.face_scaling)
+
+
+def render_views_train(cameras, pc, pipe, bg_color, scaling_modifier=1.0, width=None, height=None):
+    """The training form of render_views: every camera of one timestep (the model's current face frame) in ONE
+    differentiable forward (gab200_forward_views_train).  Returns render()'s dict with a leading K:
+    {"render": (K,3,H,W), "viewspace_points": (K,P,3) holder whose .grad row k is camera k's dL/dmean2D,
+    "visibility_filter": (K,P) bool, "radii": (K,P) int32}; view k's image and radii equal render(cameras[k], ...)
+    bit for bit.  A loss summed over the views backpropagates, in one backward, the sum of the K single-view
+    gradients into the model's parameters and face frame."""
+    table, W, H = _views_table(cameras, pc, width, height, "render_views_train")
+    rs = _views_settings(W, H, pc, pipe, bg_color, scaling_modifier)
+    binding, (fc, fR, fs) = _face_frame_of(pc)
+    K, P = int(table.shape[0]), int(pc._xyz.shape[0])
+    screenspace_points = torch.zeros((K, P, 3), dtype=pc._xyz.dtype, device=pc._xyz.device, requires_grad=True)
+    image, radii = rasterize_bound_views_train(rs, table, pc._xyz, pc._rotation, pc._scaling, pc._opacity,
+                                               pc._features_dc, pc._features_rest, binding, fc, fR, fs,
+                                               means2D=screenspace_points, grad_sink=pc)
+    return {"render": image, "viewspace_points": screenspace_points, "visibility_filter": _visible(radii),
+            "radii": radii}
 
 
 def _views_forward(table, W, H, pc, pipe, bg_color, scaling_modifier, display: bool, float_image: bool):
     """The fused route's K-view forward of a (K, 37) device camera table (render_views, GraphedRender)."""
     d = lambda t: None if t is None else t.detach()  # noqa: E731
     with torch.no_grad():
-        rs = GaussianRasterizationSettings(image_height=H, image_width=W, tanfovx=1.0, tanfovy=1.0, bg=bg_color,
-                                           scale_modifier=scaling_modifier, viewmatrix=None, projmatrix=None,
-                                           sh_degree=pc.active_sh_degree, campos=None, prefiltered=False,
-                                           debug=bool(getattr(pipe, "debug", False)))
-        binding = getattr(pc, "binding", None)
-        fc = fR = fs = None
-        if binding is not None:
-            if getattr(pc, "face_center", None) is None:
-                pc.select_mesh_by_timestep(0)
-            fc, fR, fs = pc.face_center, pc.face_orien_mat, pc.face_scaling
+        rs = _views_settings(W, H, pc, pipe, bg_color, scaling_modifier)
+        binding, (fc, fR, fs) = _face_frame_of(pc)
         img, rgb8, radii, visible = rasterize_bound_views(
             rs, table, d(pc._xyz), d(pc._rotation), d(pc._scaling), d(pc._opacity), d(pc._features_dc),
             d(pc._features_rest), binding, d(fc), d(fR), d(fs), hints=view_hints_of(pc), display=display,

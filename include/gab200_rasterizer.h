@@ -183,7 +183,8 @@ typedef struct gab200_frame_state {
   int32_t depth_sort_path;    /* 0: radix sort (no hint); 1: bucket sort; 2: bucket sort overflowed, radix sort redone */
   int32_t attempts;           /* 1 + number of times stages were re-enqueued (GAB200_SYNC_LATE only; else 1) */
   int32_t tile_sort_path;     /* 0: cub::DeviceRadixSort over the instances; 1: counting sort by tile + per-tile rank sort */
-  int32_t reserved0;
+  int32_t reserved0;          /* K of a gab200_forward_views_train frame (its backward is gab200_backward_views with the
+                                 same K); 0 for every other forward */
   const uint32_t* device_counters; /* GAB200_NUM_COUNTERS words inside the geometry buffer (valid as long as it is) */
 } gab200_frame_state;
 
@@ -294,6 +295,34 @@ int64_t gab200_forward_display(const gab200_forward_args* args, const float* tan
 #define GAB200_CAMERA_FLOATS 37
 int64_t gab200_forward_views(const gab200_forward_args* args, int32_t views, const float* cameras, uint8_t* out_rgb8,
                              gab200_frame_state* state_out, void* stream);
+
+/* Training over every camera of one timestep: the K-view frame of gab200_forward_views, kept for a backward.
+ * It is gab200_forward_views with need_backward = 1 (args->need_backward is not read): args->out_color [views,3,H,W] is
+ * required and no display image is written; radii [views,P] and visibility [views,P] | NULL as there.  Images, radii
+ * and visibility are bit for bit those of gab200_forward_views and of `views` single-camera forwards.  The state keeps
+ * what the backward reads for all K * P virtual splats and K * H * W pixels (final transmittance, contributor counts,
+ * per-instance block masks, colour clamp bits, records) and records K in state_out->reserved0; the struct layout and
+ * GAB200_ABI_VERSION are unchanged.  Every sync mode, binning_hint, the counters, the sticky overflow_flag and the
+ * LATE re-enqueue behave as in gab200_forward_views.  Before any device work, GAB200_ERR_INVALID_ARGUMENT for every
+ * error of gab200_forward_views except a NULL out_rgb8 (there is none), and for input_mode GAB200_INPUT_ACTIVATED and
+ * colors_precomp != NULL: training uses BOUND_RAW splats with SH colours only. */
+int64_t gab200_forward_views_train(const gab200_forward_args* args, int32_t views, const float* cameras,
+                                   gab200_frame_state* state_out, void* stream);
+
+/* Gradients of a gab200_forward_views_train frame, summed over its views: every output is what the sum over k of
+ * gab200_backward of camera k's single-view frame would hold (float sums in another order).  args->fwd is the forward's
+ * args, args->state its state, `views` and `cameras` the forward's (the table must hold the same values).
+ * dL_dout_color [views,3,H,W]; dL_dmeans2D [views,P,3] | NULL (row k: camera k's dL/dmean2D, x,y in NDC units, z = 0);
+ * dL_dmeans3D, dL_drotations, dL_dscales, dL_dopacity, dL_dsh_dc, dL_dsh_rest: the RAW-parameter gradients [P,...],
+ * written in full (zeros where no view gave a gradient), each stored once -- one thread per splat sums the views in
+ * order, without atomics.  dL_dface_* are zeroed and accumulated as in gab200_backward, through the CSR chunks when
+ * given, else with atomics.  dL_dcolors, dL_dshs and dL_dcov3D are not read.
+ * Before any device work, GAB200_ERR_INVALID_ARGUMENT for: views outside [1, 65535], cameras == NULL, every limit of
+ * gab200_forward_views_train, a state whose reserved0 != views (a single-view state, or another K),
+ * GAB200_INPUT_ACTIVATED, colors_precomp != NULL, grads_are_multicast != 0, a NULL dL_dout_color / dL_dsh_dc /
+ * dL_dsh_rest (sh_coeffs > 1), and scratch buffers that are not the forward's.  gab200_backward and
+ * gab200_backward_device_fov refuse a multi-view state. */
+int32_t gab200_backward_views(const gab200_backward_args* args, int32_t views, const float* cameras, void* stream);
 
 /* Frustum test only.  Replaces diff_gaussian_rasterization._C.mark_visible (GaussianRasterizer.markVisible). */
 int32_t gab200_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,
