@@ -360,6 +360,9 @@ struct Frame {
   const uint32_t* order_count = nullptr;  // device count of listed splats (bucket path), else all P are listed
   bool counting = true;                   // tile sort: counting sort + per-tile rank sort (tile_sort.cu), else cub radix
   uint32_t scan_clamp = 0xffffffffu;      // capacity the tile ranges were cut at by the last tile scan
+  bool da = false;                        // gab200_forward_depth_alpha: records with z, the two planes below
+  float* out_alpha = nullptr;             // [H,W] or NULL
+  float* out_depth = nullptr;             // [H,W] or NULL
 };
 
 // preprocess (+ bucket bookkeeping when `bucket`) -> per-splat depth order + emission offsets -> counters published
@@ -386,7 +389,7 @@ int enqueue_geometry(Frame& f, bool bucket, bool run_preprocess, uint32_t capaci
                               g.buckets, f.counting ? f.iv.tile_count : nullptr, f.nb ? g.clamped : nullptr, stream);
     else
       launch_preprocess(*a, g.rec, g.aux, g.tiles_touched, f.nb ? g.clamped : nullptr, g.depth_keys[0], g.ids[0],
-                        g.buckets, f.counting ? f.iv.tile_count : nullptr, f.tanfov, stream);
+                        g.buckets, f.counting ? f.iv.tile_count : nullptr, f.tanfov, stream, f.da);
   }
   GAB_STAGE_CHECK(f.dbg, stream);
   if (f.counting && run_preprocess) {
@@ -505,6 +508,10 @@ int enqueue_binning_blend(Frame& f, void* bin, int64_t cap, int64_t n_known, siz
       launch_blend_forward_views_train(f.views, f.W, f.H, f.iv.ranges, f.iv.order, f.iv.order_info, bv.vals[selector],
                                        f.g.rec, a->bg, a->out_color, f.iv.final_T, f.iv.n_contrib, bv.strip_mask,
                                        stream);
+    else if (f.da)
+      launch_blend_forward_depth(f.W, f.H, f.iv.ranges, f.iv.order, f.iv.order_info, bv.vals[selector], f.g.rec, a->bg,
+                                 a->out_color, f.iv.final_T, f.iv.n_contrib, bv.strip_mask, f.out_rgb8, f.out_alpha,
+                                 f.out_depth, stream);
     else if (f.cameras != nullptr)
       launch_blend_forward_views(f.views, f.W, f.H, f.iv.ranges, f.iv.order, f.iv.order_info, bv.vals[selector], f.g.rec,
                                  a->bg, a->out_color, f.out_rgb8, stream);
@@ -527,9 +534,11 @@ int wait_counters(Frame& f) {
 
 // gab200_forward, gab200_forward_device_fov and gab200_forward_display (tanfov == NULL: the by-value tanfovx /
 // tanfovy; out_rgb8 == NULL: no display image), and gab200_forward_views[_train] (cameras != NULL: `views` cameras,
-// validated by the caller, as one frame of views * P virtual splats; need_backward: the training form)
+// validated by the caller, as one frame of views * P virtual splats; need_backward: the training form), and
+// gab200_forward_depth_alpha (da: the alpha / depth planes, either may be NULL, validated by the caller)
 static int64_t run_forward(const gab200_forward_args* a, const float* tanfov, uint8_t* out_rgb8,
-                           gab200_frame_state* st, void* stream_, int views = 1, const float* cameras = nullptr) {
+                           gab200_frame_state* st, void* stream_, int views = 1, const float* cameras = nullptr,
+                           bool da = false, float* out_alpha = nullptr, float* out_depth = nullptr) {
   cudaStream_t stream = (cudaStream_t)stream_;
   if (!validate(a, out_rgb8 != nullptr && a != nullptr && a->need_backward == 0) || st == nullptr)
     return GAB200_ERR_INVALID_ARGUMENT;
@@ -541,6 +550,7 @@ static int64_t run_forward(const gab200_forward_args* a, const float* tanfov, ui
   f.gx = (f.W + GAB_TILE - 1) / GAB_TILE; f.gy = (f.H + GAB_TILE - 1) / GAB_TILE;
   f.tiles = f.gx * f.gy * views;
   f.views = views; f.cameras = cameras;
+  f.da = da; f.out_alpha = out_alpha; f.out_depth = out_depth;
   f.nb = a->need_backward != 0;
   f.dbg = a->debug != 0;
   f.counting = tune_get(GAB200_TUNE_TILE_SORT) == 1;
@@ -576,6 +586,7 @@ static int64_t run_forward(const gab200_forward_args* a, const float* tanfov, ui
   st->attempts = 1;
   st->depth_key_min = 1; st->depth_key_max = 0;  // "nothing visible" until the counters say otherwise
   st->reserved0 = (cameras != nullptr && f.nb) ? views : 0;  // the K a multi-view backward must be called with
+  st->depth_prefix = (da && f.nb) ? 1u : 0u;                 // the records carry z: gab200_backward_depth_alpha may run
 
   const double t0 = now_us();
   if (P == 0) {  // nothing to bin: background image, empty ranges
@@ -688,6 +699,12 @@ int64_t gab200_forward_display(const gab200_forward_args* a, const float* tanfov
   return run_forward(a, tanfov, out_rgb8, st, stream);
 }
 
+int64_t gab200_forward_depth_alpha(const gab200_forward_args* a, const float* tanfov, float* out_alpha, float* out_depth,
+                                   uint8_t* out_rgb8, gab200_frame_state* st, void* stream) {
+  if (out_alpha == nullptr && out_depth == nullptr) return GAB200_ERR_INVALID_ARGUMENT;
+  return run_forward(a, tanfov, out_rgb8, st, stream, 1, nullptr, true, out_alpha, out_depth);
+}
+
 int64_t gab200_forward_views(const gab200_forward_args* a, int32_t views, const float* cameras, uint8_t* out_rgb8,
                              gab200_frame_state* st, void* stream) {
   if (a == nullptr || a->need_backward != 0 || views < 1 || views > 65535 || cameras == nullptr || st == nullptr)
@@ -777,8 +794,9 @@ int32_t gab200_backward_views(const gab200_backward_args* b, int32_t views, cons
   return GAB200_OK;
 }
 
-// gab200_backward and gab200_backward_device_fov
-static int32_t run_backward(const gab200_backward_args* b, const float* tanfov, void* stream_) {
+// gab200_backward and gab200_backward_device_fov, and gab200_backward_depth_alpha (da: the plane gradients, NULL = 0)
+static int32_t run_backward(const gab200_backward_args* b, const float* tanfov, void* stream_, bool da = false,
+                            const float* dL_dalpha = nullptr, const float* dL_ddepth = nullptr) {
   cudaStream_t stream = (cudaStream_t)stream_;
   if (b == nullptr || b->abi_version != GAB200_ABI_VERSION || b->fwd == nullptr || b->state == nullptr)
     return GAB200_ERR_INVALID_ARGUMENT;
@@ -786,6 +804,8 @@ static int32_t run_backward(const gab200_backward_args* b, const float* tanfov, 
   const gab200_frame_state* st = b->state;
   if (!validate(a) || !a->need_backward || b->dL_dout_color == nullptr) return GAB200_ERR_INVALID_ARGUMENT;
   if (st->reserved0 != 0) return GAB200_ERR_INVALID_ARGUMENT;  // a multi-view frame: gab200_backward_views
+  // the depth plane's backward reads z from the records: only a gab200_forward_depth_alpha state has it; plain stores
+  if (da && (st->depth_prefix != 1u || b->grads_are_multicast)) return GAB200_ERR_INVALID_ARGUMENT;
   if (st->geom_buffer == nullptr || st->image_buffer == nullptr || st->binning_buffer == nullptr)
     return GAB200_ERR_INVALID_ARGUMENT;
   const int P = a->P, W = a->image_width, H = a->image_height;
@@ -822,8 +842,13 @@ static int32_t run_backward(const gab200_backward_args* b, const float* tanfov, 
   }
   if (st->num_rendered != 0) {  // -1: only the device knows (GAB200_SYNC_NONE); empty tile lists cost nothing
     StageScope sc(GAB200_STAGE_BLEND_BWD, stream);
-    launch_blend_backward(W, H, iv.ranges, iv.order, iv.order_info, bv.vals[st->sorted_selector], g.rec, a->bg, iv.final_T, iv.n_contrib,
-                          b->dL_dout_color, bv.strip_mask, g.g2d, stream);
+    if (da)
+      launch_blend_backward_depth(W, H, iv.ranges, iv.order, iv.order_info, bv.vals[st->sorted_selector], g.rec, a->bg,
+                                  iv.final_T, iv.n_contrib, b->dL_dout_color, bv.strip_mask, g.g2d, dL_dalpha,
+                                  dL_ddepth, stream);
+    else
+      launch_blend_backward(W, H, iv.ranges, iv.order, iv.order_info, bv.vals[st->sorted_selector], g.rec, a->bg,
+                            iv.final_T, iv.n_contrib, b->dL_dout_color, bv.strip_mask, g.g2d, stream);
   }
   GAB_STAGE_CHECK(dbg, stream);
   {
@@ -831,7 +856,7 @@ static int32_t run_backward(const gab200_backward_args* b, const float* tanfov, 
     const bool csr = bound && a->binding != nullptr && b->num_face_chunks > 0 && b->face_perm && b->face_chunk_face &&
                      b->face_chunk_start && b->face_chunk_end &&
                      (b->dL_dface_center || b->dL_dface_orien_mat || b->dL_dface_scaling);
-    launch_preprocess_backward(*b, g.rec, g.aux, g.clamped, g.g2d, csr ? g.face_scratch : nullptr, tanfov, stream);
+    launch_preprocess_backward(*b, g.rec, g.aux, g.clamped, g.g2d, csr ? g.face_scratch : nullptr, tanfov, stream, da);
   }
   GAB_STAGE_CHECK(dbg, stream);
   return GAB200_OK;
@@ -841,6 +866,11 @@ int32_t gab200_backward(const gab200_backward_args* b, void* stream) { return ru
 
 int32_t gab200_backward_device_fov(const gab200_backward_args* b, const float* tanfov, void* stream) {
   return run_backward(b, tanfov, stream);
+}
+
+int32_t gab200_backward_depth_alpha(const gab200_backward_args* b, const float* tanfov, const float* dL_dalpha,
+                                    const float* dL_ddepth, void* stream) {
+  return run_backward(b, tanfov, stream, true, dL_dalpha, dL_ddepth);
 }
 
 int32_t gab200_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,

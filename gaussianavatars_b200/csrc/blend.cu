@@ -26,6 +26,8 @@
 //     (S0,S1,S2) because dx is shared, and the nine per-splat gradient components leave through a three-stage
 //     pipelined shared-memory row reduction that ends in one 9-lane RED.ADD.F32 per (warp, splat).
 // Tensor cores are not used: there is no dense contraction on this path (north_star).
+#include <type_traits>
+
 #include "common.cuh"
 #include "kernels.cuh"
 
@@ -88,6 +90,8 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       "r"(parity)
       : "memory");
 }
+#define GAB_FWD_DEPTH_CTAS 2  // CTAs per SM the depth-plane blend kernels are bounded for (DESIGN.md section 4)
+#define GAB_BWD_DEPTH_CTAS 5
 #define ID_RING 3  // id chunks in flight: being gathered from, next, and the one the copy engine is filling
 
 // Barrier of one thread group (NT threads, hardware barrier `id`); id 0 with NT = blockDim is __syncthreads().
@@ -157,7 +161,9 @@ __device__ __forceinline__ void store_display(uint8_t* __restrict__ out, int W, 
 // =====================================================================================================
 // Forward: one tile on a group of NT = 256/K threads (tl = thread index inside the group)
 // =====================================================================================================
-template <int K, int OUT>
+// DA (gab200_forward_depth_alpha): also the accumulated alpha 1 - T_final and the depth sum_i w_i z_i of the same walk,
+// z_i = q2.w of a record written by preprocess_depth_kernel; out_alpha / out_depth [H,W] (either may be NULL).
+template <int K, int OUT, bool DA = false>
 __device__ __forceinline__ void forward_tile(int tile, int tl, GroupBarrier<256 / K> bar, SplatRec* buf0,
                                              SplatRec* buf1, uint32_t* smask, uint32_t* ids_ring, uint64_t* mbar,
                                              int W, int H, int gx,
@@ -165,7 +171,8 @@ __device__ __forceinline__ void forward_tile(int tile, int tl, GroupBarrier<256 
                                              const SplatRec* __restrict__ rec, const float* __restrict__ bg,
                                              float* __restrict__ out_color, float* __restrict__ final_T,
                                              uint32_t* __restrict__ n_contrib, uint8_t* __restrict__ strip_mask,
-                                             uint8_t* __restrict__ out_rgb8) {
+                                             uint8_t* __restrict__ out_rgb8, float* __restrict__ out_alpha = nullptr,
+                                             float* __restrict__ out_depth = nullptr) {
   constexpr int NT = 256 / K;
   const int tx = tile % gx, ty = tile / gx;
   const int lane = tl & 31;
@@ -183,12 +190,14 @@ __device__ __forceinline__ void forward_tile(int tile, int tl, GroupBarrier<256 
   smask[tl] = 0;
 
   float T[K], Cr[K], Cg[K], Cb[K];
+  float D[DA ? K : 1];
   uint32_t last[K];
   uint32_t done = 0;
   constexpr uint32_t ALL = (1u << K) - 1u;
 #pragma unroll
   for (int i = 0; i < K; i++) {
     T[i] = 1.f; Cr[i] = Cg[i] = Cb[i] = 0.f; last[i] = 0;
+    if (DA) D[i] = 0.f;
     if (pixx >= W || pixy0 + 4 * i >= H) done |= 1u << i;
   }
 
@@ -272,6 +281,7 @@ __device__ __forceinline__ void forward_tile(int tile, int tl, GroupBarrier<256 
               Cr[i] = fmaf(q1.z, w, Cr[i]);
               Cg[i] = fmaf(q1.w, w, Cg[i]);
               Cb[i] = fmaf(r->q2.x, w, Cb[i]);
+              if (DA) D[i] = fmaf(r->q2.w, w, D[i]);
               T[i] = test_T;
               last[i] = pos0 + (uint32_t)(gbase + jj) + 1u;
               lb[i] |= 1u << jj;
@@ -314,6 +324,10 @@ __device__ __forceinline__ void forward_tile(int tile, int tl, GroupBarrier<256 
       if (final_T != nullptr) {
         final_T[pix] = T[i];
         n_contrib[pix] = last[i];
+      }
+      if (DA) {
+        if (out_alpha != nullptr) out_alpha[pix] = 1.0f - T[i];
+        if (out_depth != nullptr) out_depth[pix] = D[i];
       }
     }
   }
@@ -377,6 +391,57 @@ void launch_blend_forward(int W, int H, const uint2* ranges, const uint32_t* ord
                                        : blend_forward_kernel<1, BLEND_OUT_FLOAT | BLEND_OUT_U8>;
   kernel<<<grid, 256, 0, stream>>>(W, H, gx, tiles, ranges, order, order_info, point_list, rec, bg, out_color, final_T,
                                    n_contrib, strip_mask, out_rgb8);
+  count_launch();
+}
+
+// gab200_forward_depth_alpha: blend_forward_kernel<1, OUT> with the alpha and depth planes (forward_tile<.., DA>).  The
+// records must come from preprocess_depth_kernel (z in q2.w).
+template <int OUT>
+__global__ void __launch_bounds__(256, GAB_FWD_DEPTH_CTAS) blend_forward_depth_kernel(int W, int H, int gx, int tiles,
+                                                                  const uint2* __restrict__ ranges,
+                                                                  const uint32_t* __restrict__ order,
+                                                                  const uint32_t* __restrict__ order_info,
+                                                                  const uint32_t* __restrict__ point_list,
+                                                                  const SplatRec* __restrict__ rec,
+                                                                  const float* __restrict__ bg,
+                                                                  float* __restrict__ out_color,
+                                                                  float* __restrict__ final_T,
+                                                                  uint32_t* __restrict__ n_contrib,
+                                                                  uint8_t* __restrict__ strip_mask,
+                                                                  uint8_t* __restrict__ out_rgb8,
+                                                                  float* __restrict__ out_alpha,
+                                                                  float* __restrict__ out_depth) {
+  __shared__ SplatRec buf[2][256];
+  __shared__ uint32_t smask[256];
+  __shared__ __align__(16) uint32_t ids_ring[4][ID_RING * (64 + 4)];
+  __shared__ __align__(8) uint64_t mbar[4][ID_RING];
+  const int nh = (int)order_info[0];
+  const int b = blockIdx.x, t = threadIdx.x;
+  if (b < nh) {
+    forward_tile<1, OUT, true>((int)order[b], t, GroupBarrier<256>{0}, buf[0], buf[1], smask, &ids_ring[0][0], mbar[0],
+                               W, H, gx, ranges, point_list, rec, bg, out_color, final_T, n_contrib, strip_mask,
+                               out_rgb8, out_alpha, out_depth);
+  } else {
+    const int g = t >> 6, slot = nh + 4 * (b - nh) + g;
+    if (slot >= tiles) return;
+    forward_tile<4, OUT, true>((int)order[slot], t & 63, GroupBarrier<64>{1 + g}, buf[0] + g * 64, buf[1] + g * 64,
+                               smask + g * 64, ids_ring[g], mbar[g], W, H, gx, ranges, point_list, rec, bg, out_color,
+                               final_T, n_contrib, strip_mask, out_rgb8, out_alpha, out_depth);
+  }
+}
+
+void launch_blend_forward_depth(int W, int H, const uint2* ranges, const uint32_t* order, const uint32_t* order_info,
+                                const uint32_t* point_list, const SplatRec* rec, const float* bg, float* out_color,
+                                float* final_T, uint32_t* n_contrib, uint8_t* strip_mask, uint8_t* out_rgb8,
+                                float* out_alpha, float* out_depth, cudaStream_t stream) {
+  const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
+  const int tiles = gx * gy;
+  if (tiles == 0) return;
+  auto kernel = out_rgb8 == nullptr ? blend_forward_depth_kernel<BLEND_OUT_FLOAT>
+                : out_color == nullptr ? blend_forward_depth_kernel<BLEND_OUT_U8>
+                                       : blend_forward_depth_kernel<BLEND_OUT_FLOAT | BLEND_OUT_U8>;
+  kernel<<<tiles, 256, 0, stream>>>(W, H, gx, tiles, ranges, order, order_info, point_list, rec, bg, out_color, final_T,
+                                    n_contrib, strip_mask, out_rgb8, out_alpha, out_depth);
   count_launch();
 }
 
@@ -496,20 +561,34 @@ struct PixState {
   float T[K];                 // transmittance in front of the splat being visited (starts at final_T)
   float ar[K], ag[K], ab[K];  // colour composited behind the splat being visited
   float dr[K], dg[K], db[K];  // dL/dpixel
-  float bgT[K];               // final_T * (bg . dL/dpixel)
+  float bgT[K];               // final_T * (bg . dL/dpixel)  (DA: final_T * (bg . dL/dpixel - dL/dalpha))
   int nc[K];                  // n_contrib: only list positions below it contributed to the pixel
 };
 struct SplatSums {  // per-lane sums over the lane's pixels for one splat
   float S0, S1, S2, go, gr, gg, gb;
 };
+// DA (depth plane): a fourth channel with colour z and background 0, and dL/dalpha folded into bgT
+template <int K>
+struct PixStateDA : PixState<K> {
+  float az[K];  // depth composited behind the splat being visited
+  float dD[K];  // dL/ddepth
+};
+struct SplatSumsDA : SplatSums {
+  float gz;     // dL/dz
+};
+template <int K, bool DA>
+using PixStateT = std::conditional_t<DA, PixStateDA<K>, PixState<K>>;
+template <bool DA>
+using SplatSumsT = std::conditional_t<DA, SplatSumsDA, SplatSums>;
 
 // One (splat, warp) visit restricted to the live bands M (compile-time set): straight-line code, the bands'
 // dependency chains are independent and interleave.  A lane whose pixel did not receive this splat in the forward
 // (beyond its n_contrib, outside the footprint, alpha < 1/255) runs the same instructions with alpha = G = 0 and
 // T multiplied by exactly 1: every one of its contributions is an exact zero.
-template <int K, int M>
-__device__ __forceinline__ void visit_bands(PixState<K>& p, int pos, float py, float tA, float dx, float Bp, float Cp,
-                                            float op, float cr, float cg, float cb, SplatSums& s) {
+template <int K, int M, bool DA = false>
+__device__ __forceinline__ void visit_bands(PixStateT<K, DA>& p, int pos, float py, float tA, float dx, float Bp,
+                                            float Cp, float op, float cr, float cg, float cb, SplatSumsT<DA>& s,
+                                            float cz = 0.f) {
 #pragma unroll
   for (int i = 0; i < K; i++) {
     if (!((M >> i) & 1)) continue;
@@ -532,11 +611,18 @@ __device__ __forceinline__ void visit_bands(PixState<K>& p, int pos, float py, f
     float dLda = er * p.dr[i];
     dLda = fmaf(eg, p.dg[i], dLda);
     dLda = fmaf(eb, p.db[i], dLda);
+    float ez = 0.f;
+    if constexpr (DA) {
+      ez = cz - p.az[i];
+      dLda = fmaf(ez, p.dD[i], dLda);
+      s.gz = fmaf(w, p.dD[i], s.gz);
+    }
     dLda = fmaf(dLda, Tn, -p.bgT[i] * ra);
     // colour behind the NEXT (nearer) splat: this one composited over what was behind it
     p.ar[i] = fmaf(al, er, p.ar[i]);
     p.ag[i] = fmaf(al, eg, p.ag[i]);
     p.ab[i] = fmaf(al, eb, p.ab[i]);
+    if constexpr (DA) p.az[i] = fmaf(al, ez, p.az[i]);
     const float t = Gv * dLda;  // G dL/dalpha
     s.go += t;
     const float s_ = op * t;    // G dL/dG
@@ -549,31 +635,33 @@ __device__ __forceinline__ void visit_bands(PixState<K>& p, int pos, float py, f
 
 // Dead bands skipped with warp-uniform branches, live bands one after the other (template recursion keeps the band
 // index a compile-time constant, so p.X[i] stays in registers).
-template <int K, int I>
+template <int K, int I, bool DA = false>
 struct BandLoop {
-  static __device__ __forceinline__ void run(uint32_t m, PixState<K>& p, int pos, float py, float tA, float dx, float Bp,
-                                             float Cp, float op, float cr, float cg, float cb, SplatSums& s) {
-    if (m & (1u << I)) visit_bands<K, (1 << I)>(p, pos, py, tA, dx, Bp, Cp, op, cr, cg, cb, s);
-    BandLoop<K, I + 1>::run(m, p, pos, py, tA, dx, Bp, Cp, op, cr, cg, cb, s);
+  static __device__ __forceinline__ void run(uint32_t m, PixStateT<K, DA>& p, int pos, float py, float tA, float dx,
+                                             float Bp, float Cp, float op, float cr, float cg, float cb,
+                                             SplatSumsT<DA>& s, float cz = 0.f) {
+    if (m & (1u << I)) visit_bands<K, (1 << I), DA>(p, pos, py, tA, dx, Bp, Cp, op, cr, cg, cb, s, cz);
+    BandLoop<K, I + 1, DA>::run(m, p, pos, py, tA, dx, Bp, Cp, op, cr, cg, cb, s, cz);
   }
 };
-template <int K>
-struct BandLoop<K, K> {
-  static __device__ __forceinline__ void run(uint32_t, PixState<K>&, int, float, float, float, float, float, float, float,
-                                             float, float, SplatSums&) {}
+template <int K, bool DA>
+struct BandLoop<K, K, DA> {
+  static __device__ __forceinline__ void run(uint32_t, PixStateT<K, DA>&, int, float, float, float, float, float, float,
+                                             float, float, float, SplatSumsT<DA>&, float = 0.f) {}
 };
 
-// Shared memory of one backward warp task.
+// Shared memory of one backward warp task: NR gradient components per splat (9; 10 with the depth plane's dL/dz).
 #define ROWS_STRIDE 36
-#define ROWS_WORDS (9 * ROWS_STRIDE)
-struct __align__(16) WarpSmem {
+template <int NR>
+struct __align__(16) WarpSmemT {
   SplatRec rec[2][32];
-  float rows[2][ROWS_WORDS];        // [visit parity][component][lane], row stride 36 floats
-  float part[2][32];                // [visit parity][component * 2 + half]  (18 used)
+  float rows[2][NR * ROWS_STRIDE];  // [visit parity][component][lane], row stride 36 floats
+  float part[2][32];                // [visit parity][component * 2 + half]  (2 NR used)
   uint32_t ids[ID_RING][32 + 4];
   uint8_t masks[ID_RING][32 + 16];
   uint64_t mbar[ID_RING];
 };
+using WarpSmem = WarpSmemT<9>;
 
 // One warp task: the pixels of one (tile, half, band group), same ownership as the forward (BandGeom).
 //   * The WARP is the unit of work.  It stages its own id/mask lists (TMA bulk copies into a private 3-slot ring) and
@@ -586,15 +674,20 @@ struct __align__(16) WarpSmem {
 //     store 18 partials; during visit j+2 nine lanes add the two halves and issue the RED.  No shuffle, no exposed
 //     shared-memory or shuffle latency: the loads of rounds 1 and 2 are issued at the top of a visit and consumed
 //     after its band math.
-template <int K>
-__device__ __forceinline__ void backward_task(int tile, int tl, WarpSmem& sm, int W, int H, int gx,
+// DA (gab200_backward_depth_alpha): records from preprocess_depth_kernel (z in q2.w); dL_dalpha / dL_ddepth [H,W] or
+// NULL (zero); a tenth component, dL/dz, leaves for g2d slot 9.
+template <int K, bool DA = false>
+__device__ __forceinline__ void backward_task(int tile, int tl, WarpSmemT<DA ? 10 : 9>& sm, int W, int H, int gx,
                                               const uint2* __restrict__ ranges,
                                               const uint32_t* __restrict__ point_list,
                                               const SplatRec* __restrict__ rec, const float* __restrict__ bg,
                                               const float* __restrict__ final_T,
                                               const uint32_t* __restrict__ n_contrib,
                                               const float* __restrict__ dL_dpix,
-                                              const uint8_t* __restrict__ strip_mask, float* __restrict__ g2d) {
+                                              const uint8_t* __restrict__ strip_mask, float* __restrict__ g2d,
+                                              const float* __restrict__ dL_dalpha = nullptr,
+                                              const float* __restrict__ dL_ddepth = nullptr) {
+  constexpr int NR = DA ? 10 : 9;
   const int tx = tile % gx, ty = tile / gx;
   const int lane = tl & 31;
   const BandGeom<K> geo(tl);
@@ -605,14 +698,14 @@ __device__ __forceinline__ void backward_task(int tile, int tl, WarpSmem& sm, in
   const size_t HW = (size_t)H * W;
   const float bg0 = bg[0], bg1 = bg[1], bg2 = bg[2];
 
-  PixState<K> p;
+  PixStateT<K, DA> p;
   int n = 0;
 #pragma unroll
   for (int i = 0; i < K; i++) {
     const int y = pixy0 + 4 * i;
     p.fy[i] = (float)y;
     p.ar[i] = p.ag[i] = p.ab[i] = 0.f;
-    float T0 = 0.f, dr = 0.f, dg = 0.f, db = 0.f;
+    float T0 = 0.f, dr = 0.f, dg = 0.f, db = 0.f, dA = 0.f, dZ = 0.f;
     p.nc[i] = 0;
     if (pixx < W && y < H) {
       const size_t pix = (size_t)y * W + pixx;
@@ -621,12 +714,22 @@ __device__ __forceinline__ void backward_task(int tile, int tl, WarpSmem& sm, in
       dr = dL_dpix[pix];
       dg = dL_dpix[HW + pix];
       db = dL_dpix[2 * HW + pix];
+      if constexpr (DA) {
+        if (dL_dalpha != nullptr) dA = dL_dalpha[pix];
+        if (dL_ddepth != nullptr) dZ = dL_ddepth[pix];
+      }
     }
     p.T[i] = T0;
     p.dr[i] = dr;
     p.dg[i] = dg;
     p.db[i] = db;
-    p.bgT[i] = T0 * (bg0 * dr + bg1 * dg + bg2 * db);
+    if constexpr (DA) {  // alpha = 1 - T_final: dL/dT_final gains -dL/dalpha, which joins the background term
+      p.bgT[i] = T0 * ((bg0 * dr + bg1 * dg + bg2 * db) - dA);
+      p.az[i] = 0.f;
+      p.dD[i] = dZ;
+    } else {
+      p.bgT[i] = T0 * (bg0 * dr + bg1 * dg + bg2 * db);
+    }
     n = max(n, p.nc[i]);
   }
   // this warp only needs instances [0, max n_contrib of ITS pixels)
@@ -679,19 +782,19 @@ __device__ __forceinline__ void backward_task(int tile, int tl, WarpSmem& sm, in
   // reduction pipeline state: ids of the two visits whose sums are still on their way out
   uint32_t id1 = 0xffffffffu, id2 = 0xffffffffu;  // visit j-1 (rows written), visit j-2 (partials written)
   uint32_t par = 0;                                // parity of the current visit
-  // round 1 (lane < 18): component c1 = lane / 2, half h1 = lane & 1: sum of rows[c1][16 h1 .. 16 h1 + 15]
-  const int c1 = min(lane >> 1, 8), h1 = lane & 1;
-  // round 2 (lane < 9): component lane: part[2 lane] + part[2 lane + 1]
+  // round 1 (lane < 2 NR): component c1 = lane / 2, half h1 = lane & 1: sum of rows[c1][16 h1 .. 16 h1 + 15]
+  const int c1 = min(lane >> 1, NR - 1), h1 = lane & 1;
+  // round 2 (lane < NR): component lane: part[2 lane] + part[2 lane + 1]
   auto reduce_step = [&](uint32_t id_rows, uint32_t id_part) {
     // partials of the visit before last -> global
-    const float2 pp = *reinterpret_cast<const float2*>(&sm.part[par][2 * min(lane, 8)]);
+    const float2 pp = *reinterpret_cast<const float2*>(&sm.part[par][2 * min(lane, NR - 1)]);
     // rows of the last visit -> partials
     const float4* r4 = reinterpret_cast<const float4*>(&sm.rows[par ^ 1][c1 * ROWS_STRIDE + h1 * 16]);
     const float4 a = r4[0], b = r4[1], c = r4[2], d = r4[3];
-    if (id_part != 0xffffffffu && lane < 9) atomicAdd(g2d + (size_t)id_part * GAB_G2D_STRIDE + lane, pp.x + pp.y);
+    if (id_part != 0xffffffffu && lane < NR) atomicAdd(g2d + (size_t)id_part * GAB_G2D_STRIDE + lane, pp.x + pp.y);
     const float s = (((a.x + a.y) + (a.z + a.w)) + ((b.x + b.y) + (b.z + b.w))) +
                     (((c.x + c.y) + (c.z + c.w)) + ((d.x + d.y) + (d.z + d.w)));
-    if (id_rows != 0xffffffffu && lane < 18) sm.part[par ^ 1][lane] = s;
+    if (id_rows != 0xffffffffu && lane < 2 * NR) sm.part[par ^ 1][lane] = s;
   };
 
   for (int c = 0; c < nchunks; c++) {
@@ -713,13 +816,16 @@ __device__ __forceinline__ void backward_task(int tile, int tl, WarpSmem& sm, in
       const float4 q0 = cur[jj].q0;
       const float4 q1 = cur[jj].q1;
       const float cbl = cur[jj].q2.x;
+      const float czl = DA ? cur[jj].q2.w : 0.f;
       reduce_step(id1, id2);
       const float dx = q0.x - fx;
       const float tA = q0.z * dx;
-      SplatSums s;
+      SplatSumsT<DA> s;
       s.S0 = s.S1 = s.S2 = s.go = s.gr = s.gg = s.gb = 0.f;
-      if (m == (1u << K) - 1u) visit_bands<K, (1 << K) - 1>(p, pos, q0.y, tA, dx, q0.w, q1.x, q1.y, q1.z, q1.w, cbl, s);
-      else BandLoop<K, 0>::run(m, p, pos, q0.y, tA, dx, q0.w, q1.x, q1.y, q1.z, q1.w, cbl, s);
+      if constexpr (DA) s.gz = 0.f;
+      if (m == (1u << K) - 1u)
+        visit_bands<K, (1 << K) - 1, DA>(p, pos, q0.y, tA, dx, q0.w, q1.x, q1.y, q1.z, q1.w, cbl, s, czl);
+      else BandLoop<K, 0, DA>::run(m, p, pos, q0.y, tA, dx, q0.w, q1.x, q1.y, q1.z, q1.w, cbl, s, czl);
       const float A = q0.z * CONIC_UNSCALE_AC, B = q0.w * CONIC_UNSCALE_B, C = q1.x * CONIC_UNSCALE_AC;
       const float dxS0 = dx * s.S0;
       float* row = &sm.rows[par][lane];
@@ -732,6 +838,7 @@ __device__ __forceinline__ void backward_task(int tile, int tl, WarpSmem& sm, in
       row[6 * ROWS_STRIDE] = s.gr;
       row[7 * ROWS_STRIDE] = s.gg;
       row[8 * ROWS_STRIDE] = s.gb;
+      if constexpr (DA) row[9 * ROWS_STRIDE] = s.gz;         // dL/dz (view-space depth)
       id2 = id1;
       id1 = id0;
       par ^= 1;
@@ -788,6 +895,41 @@ void launch_blend_backward(int W, int H, const uint2* ranges, const uint32_t* or
   if (tiles == 0) return;
   blend_backward_kernel<<<tiles, 128, 0, stream>>>(W, H, gx, tiles, ranges, order, order_info, point_list, rec, bg,
                                                    final_T, n_contrib, dL_dpix, strip_mask, g2d);
+  count_launch();
+}
+
+// gab200_backward_depth_alpha: blend_backward_kernel with the alpha and depth plane gradients (backward_task<K, true>).
+// Its own occupancy bound: see DESIGN.md section 4 for the registers of both bounds.
+__global__ void __launch_bounds__(128, GAB_BWD_DEPTH_CTAS) blend_backward_depth_kernel(
+    int W, int H, int gx, int tiles, const uint2* __restrict__ ranges, const uint32_t* __restrict__ order,
+    const uint32_t* __restrict__ order_info, const uint32_t* __restrict__ point_list, const SplatRec* __restrict__ rec,
+    const float* __restrict__ bg, const float* __restrict__ final_T, const uint32_t* __restrict__ n_contrib,
+    const float* __restrict__ dL_dpix, const uint8_t* __restrict__ strip_mask, float* __restrict__ g2d,
+    const float* __restrict__ dL_dalpha, const float* __restrict__ dL_ddepth) {
+  __shared__ WarpSmemT<10> sm[4];
+  const int nh = (int)order_info[1];
+  const int b = blockIdx.x, t = threadIdx.x, w = t >> 5;
+  if (b < nh) {
+    backward_task<2, true>((int)order[b], t, sm[w], W, H, gx, ranges, point_list, rec, bg, final_T, n_contrib, dL_dpix,
+                           strip_mask, g2d, dL_dalpha, dL_ddepth);
+  } else {
+    const int slot = nh + 2 * (b - nh) + (w >> 1);
+    if (slot >= tiles) return;
+    backward_task<4, true>((int)order[slot], t & 63, sm[w], W, H, gx, ranges, point_list, rec, bg, final_T, n_contrib,
+                           dL_dpix, strip_mask, g2d, dL_dalpha, dL_ddepth);
+  }
+}
+
+void launch_blend_backward_depth(int W, int H, const uint2* ranges, const uint32_t* order, const uint32_t* order_info,
+                                 const uint32_t* point_list, const SplatRec* rec, const float* bg, const float* final_T,
+                                 const uint32_t* n_contrib, const float* dL_dpix, const uint8_t* strip_mask, float* g2d,
+                                 const float* dL_dalpha, const float* dL_ddepth, cudaStream_t stream) {
+  const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
+  const int tiles = gx * gy;
+  if (tiles == 0) return;
+  blend_backward_depth_kernel<<<tiles, 128, 0, stream>>>(W, H, gx, tiles, ranges, order, order_info, point_list, rec,
+                                                         bg, final_T, n_contrib, dL_dpix, strip_mask, g2d, dL_dalpha,
+                                                         dL_ddepth);
   count_launch();
 }
 

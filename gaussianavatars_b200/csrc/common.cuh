@@ -32,7 +32,8 @@ struct __align__(16) SplatAux {
 };
 
 // Per-splat 2-D gradient record accumulated by blend-backward (RED.ADD) and consumed by preprocess-backward:
-//   (dL/dndc.x, dL/dndc.y, dL/dconic.xx, dL/dconic.xy, dL/dconic.yy, dL/dopacity, dL/dr, dL/dg, dL/db, pad*3)
+//   (dL/dndc.x, dL/dndc.y, dL/dconic.xx, dL/dconic.xy, dL/dconic.yy, dL/dopacity, dL/dr, dL/dg, dL/db,
+//    dL/dz (depth plane only; else pad), pad*2)
 #define GAB_G2D_STRIDE 12
 
 struct Camera {  // staged once per block in shared memory

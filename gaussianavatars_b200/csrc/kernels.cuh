@@ -96,10 +96,11 @@ __device__ __forceinline__ uint32_t depth_bucket(uint32_t key, const DepthBucket
   const uint32_t b = (uint32_t)(__uint2float_rz(key - d.lo) * d.scale);
   return b < d.nb ? b : d.nb - 1u;
 }
-// tile_count != nullptr: also count the instances of every tile (counting tile sort, tile_sort.cu)
+// tile_count != nullptr: also count the instances of every tile (counting tile sort, tile_sort.cu); rec_depth: the
+// records carry the view-space depth in q2.w (gab200_forward_depth_alpha)
 void launch_preprocess(const gab200_forward_args& a, SplatRec* rec, SplatAux* aux, uint32_t* tiles_touched,
                        uint8_t* clamped, uint32_t* depth_keys, uint32_t* ids, const DepthBuckets& buckets,
-                       uint32_t* tile_count, const float* tanfov, cudaStream_t stream);
+                       uint32_t* tile_count, const float* tanfov, cudaStream_t stream, bool rec_depth = false);
 // gab200_forward_views: grid (splat blocks, views); camera row k of `cameras` renders virtual splats k * P + i
 // (rec / aux / tiles / depth keys / ids / radii / visibility), tile counts at k * (gx * gy) + the tile in the view;
 // clamped != nullptr (gab200_forward_views_train, BOUND_RAW only): also the colour clamp bits at k * P + i
@@ -160,6 +161,11 @@ void launch_blend_forward(int W, int H, const uint2* ranges, const uint32_t* ord
                           const uint32_t* point_list, const SplatRec* rec,
                           const float* bg, float* out_color, float* final_T, uint32_t* n_contrib, uint8_t* strip_mask,
                           uint8_t* out_rgb8, cudaStream_t stream);  // out_color / out_rgb8: either may be NULL
+// launch_blend_forward plus the accumulated alpha and the depth planes [H,W] (either may be NULL); records with z in q2.w
+void launch_blend_forward_depth(int W, int H, const uint2* ranges, const uint32_t* order, const uint32_t* order_info,
+                                const uint32_t* point_list, const SplatRec* rec, const float* bg, float* out_color,
+                                float* final_T, uint32_t* n_contrib, uint8_t* strip_mask, uint8_t* out_rgb8,
+                                float* out_alpha, float* out_depth, cudaStream_t stream);
 // `views` images of one size: global tile g is tile g % (gx * gy) of view g / (gx * gy); out_color [views,3,H,W],
 // out_rgb8 [views,H,W,3] (either may be NULL); forward only
 void launch_blend_forward_views(int views, int W, int H, const uint2* ranges, const uint32_t* order,
@@ -175,6 +181,11 @@ void launch_blend_backward(int W, int H, const uint2* ranges, const uint32_t* or
                            const uint32_t* point_list, const SplatRec* rec,
                            const float* bg, const float* final_T, const uint32_t* n_contrib, const float* dL_dpix,
                            const uint8_t* strip_mask, float* g2d, cudaStream_t stream);
+// launch_blend_backward plus the plane gradients dL_dalpha / dL_ddepth [H,W] (NULL: zero); dL/dz -> g2d slot 9
+void launch_blend_backward_depth(int W, int H, const uint2* ranges, const uint32_t* order, const uint32_t* order_info,
+                                 const uint32_t* point_list, const SplatRec* rec, const float* bg, const float* final_T,
+                                 const uint32_t* n_contrib, const float* dL_dpix, const uint8_t* strip_mask, float* g2d,
+                                 const float* dL_dalpha, const float* dL_ddepth, cudaStream_t stream);
 // the same over the tiles of `views` images: dL_dpix [views,3,H,W]; g2d rows of the views * P virtual splats
 void launch_blend_backward_views(int views, int W, int H, const uint2* ranges, const uint32_t* order,
                                  const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
@@ -182,9 +193,11 @@ void launch_blend_backward_views(int views, int W, int H, const uint2* ranges, c
                                  const uint8_t* strip_mask, float* g2d, cudaStream_t stream);
 
 // preprocess_bwd.cu
+// depth: g2d slot 9 holds dL/dz (gab200_backward_depth_alpha), added to dL/dmean through the view matrix's third row;
+// no multicast
 void launch_preprocess_backward(const gab200_backward_args& b, const SplatRec* rec, const SplatAux* aux,
                                 const uint8_t* clamped, const float* g2d, float* face_scratch, const float* tanfov,
-                                cudaStream_t stream);
+                                cudaStream_t stream, bool depth = false);
 // gab200_backward_views (BOUND_RAW, no colors_precomp, no multicast): one thread per real splat sums the gradients of
 // its `views` virtual splats (camera row k of `cameras`; rec / aux / clamped / g2d rows k * P + i) and stores each
 // parameter gradient once; dL_dmeans2D [views,P,3]; face-frame gradients as launch_preprocess_backward's

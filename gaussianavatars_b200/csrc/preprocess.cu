@@ -55,6 +55,27 @@ __global__ void __launch_bounds__(PRE_NT) preprocess_kernel(gab200_forward_args 
 #undef GAB_PRE_OUT
 }
 
+// gab200_forward_depth_alpha: preprocess_kernel whose records also carry the view-space depth z in q2.w, read by the
+// depth plane of the blend (forward and backward)
+template <bool BOUND, bool DEVFOV>
+__global__ void __launch_bounds__(PRE_NT) preprocess_depth_kernel(gab200_forward_args a, SplatRec* __restrict__ rec,
+                                                                  SplatAux* __restrict__ aux,
+                                                                  uint32_t* __restrict__ tiles_touched,
+                                                                  uint8_t* __restrict__ clamped,
+                                                                  uint32_t* __restrict__ depth_keys,
+                                                                  uint32_t* __restrict__ ids, int exact_binning,
+                                                                  DepthBuckets bk, uint32_t* __restrict__ tile_count,
+                                                                  const float* __restrict__ tanfov) {
+  __shared__ Camera cam;
+  __shared__ float sh_s[PRE_NT * SH_SMEM_STRIDE_MAX];
+  stage_camera(a, cam);
+#define GAB_PRE_OUT i
+#define GAB_PRE_REC_DEPTH
+#include "preprocess_splat.inc"
+#undef GAB_PRE_REC_DEPTH
+#undef GAB_PRE_OUT
+}
+
 // gab200_forward_views: grid.y = view.  Camera row `view` of the table, its field of view read as DEVFOV reads it;
 // outputs at the virtual splat view * P + i, tile counts in the view's slice.
 template <bool BOUND>
@@ -108,12 +129,15 @@ __global__ void __launch_bounds__(PRE_NT) preprocess_views_train_kernel(gab200_f
 
 void launch_preprocess(const gab200_forward_args& a, SplatRec* rec, SplatAux* aux, uint32_t* tiles_touched,
                        uint8_t* clamped, uint32_t* depth_keys, uint32_t* ids, const DepthBuckets& buckets,
-                       uint32_t* tile_count, const float* tanfov, cudaStream_t stream) {
+                       uint32_t* tile_count, const float* tanfov, cudaStream_t stream, bool rec_depth) {
   const int threads = PRE_NT, blocks = (a.P + threads - 1) / threads;
   if (blocks == 0) return;
   const bool bound = a.input_mode == GAB200_INPUT_BOUND_RAW;
   auto kernel = bound ? (tanfov ? preprocess_kernel<true, true> : preprocess_kernel<true, false>)
                       : (tanfov ? preprocess_kernel<false, true> : preprocess_kernel<false, false>);
+  if (rec_depth)
+    kernel = bound ? (tanfov ? preprocess_depth_kernel<true, true> : preprocess_depth_kernel<true, false>)
+                   : (tanfov ? preprocess_depth_kernel<false, true> : preprocess_depth_kernel<false, false>);
   kernel<<<blocks, threads, 0, stream>>>(a, rec, aux, tiles_touched, clamped, depth_keys, ids, a.exact_binning, buckets,
                                          tile_count, tanfov);
   count_launch();

@@ -22,175 +22,24 @@ __global__ void __launch_bounds__(PRE_NT, 12) preprocess_backward_kernel(gab200_
                                                                   const float* __restrict__ g2d,
                                                                   float* __restrict__ face_scratch,
                                                                   const float* __restrict__ tanfov) {
-  __shared__ Camera cam;
-  __shared__ float fg_s[PRE_NT * GAB_FACE_GRAD_STRIDE];  // per-splat face-frame gradients, written out coalesced
-  float* my_fg = fg_s + threadIdx.x * GAB_FACE_GRAD_STRIDE;
-  if (BOUND && face_scratch != nullptr) {
-#pragma unroll
-    for (int k = 0; k < GAB_FACE_GRAD_STRIDE; k++) my_fg[k] = 0.f;
-  }
-  {
-    int t = threadIdx.x;
-    if (t < 16) cam.V[t] = a.viewmatrix[t];
-    else if (t < 32) cam.Pm[t - 16] = a.projmatrix[t - 16];
-    else if (t < 35) cam.campos[t - 32] = a.campos[t - 32];
-    __syncthreads();
-  }
-  // SH coefficients in (for the view-direction term) and SH gradients out share one shared-memory tile:
-  // coalesced 128-bit global accesses, conflict-free (odd stride) per-thread row accesses.
-  __shared__ float sh_s[PRE_NT * SH_SMEM_STRIDE_MAX];
-  const int M = a.sh_coeffs;
-  const int sh_width = BOUND ? 3 * (M - 1) : 3 * M;
-  const int sh_stride = sh_width | 1;
-  const int row0 = blockIdx.x * PRE_NT;
-  const int rows = min(PRE_NT, a.P - row0);
-  const float* sh_src = BOUND ? a.sh_rest : a.shs;
-  const bool stage_sh = a.colors_precomp == nullptr && sh_src != nullptr && sh_width > 0;
-  if (stage_sh) {
-    if (a.sh_degree > 0) stage_rows_in<PRE_NT>(sh_s, sh_src, (size_t)row0, rows, sh_width, sh_stride);
-    __syncthreads();
-  }
-  float* my_sh = sh_s + threadIdx.x * sh_stride;
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  const bool active = idx < a.P;
-  const int i = active ? idx : a.P - 1;
-  const int W = a.image_width, H = a.image_height;
-  const int radius = aux[i].radius;
+  constexpr bool DEPTH = false;
+#include "preprocess_bwd_splat.inc"
+}
 
-  float gm[3] = {0.f, 0.f, 0.f}, gcov[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-  float gscale[3] = {0.f, 0.f, 0.f}, grot[4] = {0.f, 0.f, 0.f, 0.f};
-  float g_op = 0.f, g2x = 0.f, g2y = 0.f, gcol[3] = {0.f, 0.f, 0.f};
-  const bool use_sh = (a.colors_precomp == nullptr);
-  const bool visible = active && radius > 0;
-
-  Activated act;
-  BindCtx ctx;
-  float3 m;
-  float c3[6];
-  float Rw[9], s[3];  // world rotation and s = mod * scale (when computed from scale/rotation)
-  const bool from_sr = BOUND || (a.cov3D_precomp == nullptr);
-
-  if (visible) {
-    const float* g = g2d + (size_t)i * GAB_G2D_STRIDE;
-    g2x = g[0]; g2y = g[1];
-    const float gA = g[2], gB = g[3], gC = g[4];
-    g_op = g[5];
-    gcol[0] = g[6]; gcol[1] = g[7]; gcol[2] = g[8];
-
-    if (BOUND) {
-      bind_activate(a, i, act, ctx);
-      m = act.mean;
-#pragma unroll
-      for (int k = 0; k < 9; k++) Rw[k] = act.R[k];
-#pragma unroll
-      for (int k = 0; k < 3; k++) s[k] = a.scale_modifier * act.s[k];
-      cov3d_from_R(Rw, s, c3);
-    } else {
-      m = make_float3(a.means3D[3 * (size_t)i], a.means3D[3 * (size_t)i + 1], a.means3D[3 * (size_t)i + 2]);
-      if (a.cov3D_precomp != nullptr) {
-#pragma unroll
-        for (int k = 0; k < 6; k++) c3[k] = a.cov3D_precomp[6 * (size_t)i + k];
-      } else {
-        quat_to_R(a.rotations[4 * (size_t)i], a.rotations[4 * (size_t)i + 1], a.rotations[4 * (size_t)i + 2],
-                  a.rotations[4 * (size_t)i + 3], Rw);
-#pragma unroll
-        for (int k = 0; k < 3; k++) s[k] = a.scale_modifier * a.scales[3 * (size_t)i + k];
-        cov3d_from_R(Rw, s, c3);
-      }
-    }
-
-#include "preprocess_bwd_view.inc"
-  }
-
-  // ---- SH: dL/dsh written for every splat (zeros when invisible), direction term -> gm ----
-  if (use_sh) {
-    float gRGB[3] = {0.f, 0.f, 0.f};
-    float B[16];
-#pragma unroll
-    for (int k = 0; k < 16; k++) B[k] = 0.f;
-    const int nb = (a.sh_degree + 1) * (a.sh_degree + 1);
-    if (visible) {
-      const uint8_t cl = clamped[i];
-#pragma unroll
-      for (int ch = 0; ch < 3; ch++) gRGB[ch] = ((cl >> ch) & 1) ? 0.f : gcol[ch];
-#include "preprocess_bwd_shdir.inc"
-    }
-    // this thread is done reading its own row: overwrite it with the gradient row, then the block writes it out
-    if (BOUND) {
-      if (active && (!MC || visible)) {
-        float* gdc = b.dL_dsh_dc + 3 * (size_t)i;
-        put<MC>(gdc + 0, B[0] * gRGB[0]); put<MC>(gdc + 1, B[0] * gRGB[1]); put<MC>(gdc + 2, B[0] * gRGB[2]);
-      }
-      for (int k = 1; k < M; k++) {
-        const float bk = (k < nb) ? B[k] : 0.f;
-        my_sh[3 * (k - 1) + 0] = bk * gRGB[0];
-        my_sh[3 * (k - 1) + 1] = bk * gRGB[1];
-        my_sh[3 * (k - 1) + 2] = bk * gRGB[2];
-      }
-    } else {
-      for (int k = 0; k < M; k++) {
-        const float bk = (k < nb) ? B[k] : 0.f;
-        my_sh[3 * k + 0] = bk * gRGB[0];
-        my_sh[3 * k + 1] = bk * gRGB[1];
-        my_sh[3 * k + 2] = bk * gRGB[2];
-      }
-    }
-  }
-  if (stage_sh) {
-    __syncthreads();
-    float* dst = BOUND ? b.dL_dsh_rest : b.dL_dshs;
-    if (dst != nullptr) stage_rows_out<PRE_NT, MC>(sh_s, dst, (size_t)row0, rows, sh_width, sh_stride);
-    // multicast reductions are weak operations: order them before anything this grid's completion is used to
-    // signal (the group barrier that follows the kernel on the stream)
-    if (MC) __threadfence_system();
-  }
-
-  // ---- Sigma -> (scale, rotation) [-> binding chain] ----
-  float g_xyz[3] = {gm[0], gm[1], gm[2]};
-  float g_opacity_out = g_op;
-  if (visible && from_sr) {
-#include "preprocess_bwd_chain.inc"
-  } else if (visible && BOUND) {
-    // unreachable: BOUND always has scale/rotation
-  }
-
-  if (BOUND && face_scratch != nullptr) {
-    __syncthreads();
-    stage_rows_out<PRE_NT>(fg_s, face_scratch, (size_t)row0, rows, GAB_FACE_GRAD_STRIDE, GAB_FACE_GRAD_STRIDE);
-  }
-
-  // ---- stores ----
-  if (!active) return;
-  const bool emit_param = !MC || visible;  // multicast mode: splats without gradient add nothing
-  if (b.dL_dmeans3D != nullptr && emit_param) {
-    put<MC>(b.dL_dmeans3D + 3 * (size_t)i + 0, g_xyz[0]);
-    put<MC>(b.dL_dmeans3D + 3 * (size_t)i + 1, g_xyz[1]);
-    put<MC>(b.dL_dmeans3D + 3 * (size_t)i + 2, g_xyz[2]);
-  }
-  if (b.dL_dmeans2D != nullptr) {
-    b.dL_dmeans2D[3 * (size_t)i + 0] = g2x;
-    b.dL_dmeans2D[3 * (size_t)i + 1] = g2y;
-    b.dL_dmeans2D[3 * (size_t)i + 2] = 0.f;
-  }
-  if (b.dL_dopacity != nullptr && emit_param) put<MC>(b.dL_dopacity + i, g_opacity_out);
-  if (b.dL_dcolors != nullptr) {
-    b.dL_dcolors[3 * (size_t)i + 0] = gcol[0];
-    b.dL_dcolors[3 * (size_t)i + 1] = gcol[1];
-    b.dL_dcolors[3 * (size_t)i + 2] = gcol[2];
-  }
-  if (b.dL_dcov3D != nullptr) {
-#pragma unroll
-    for (int k = 0; k < 6; k++) b.dL_dcov3D[6 * (size_t)i + k] = gcov[k];
-  }
-  if (b.dL_dscales != nullptr && emit_param) {
-#pragma unroll
-    for (int k = 0; k < 3; k++) put<MC>(b.dL_dscales + 3 * (size_t)i + k, gscale[k]);
-  }
-  if (b.dL_drotations != nullptr && emit_param) {
-#pragma unroll
-    for (int k = 0; k < 4; k++) put<MC>(b.dL_drotations + 4 * (size_t)i + k, grot[k]);
-  }
-  if (MC) __threadfence_system();
+// gab200_backward_depth_alpha: preprocess_backward_kernel that also adds dL/dz (g2d slot 9) to dL/dmean through the third
+// row of the view matrix, before the binding chain.  Plain stores only.  Bounded for 8 CTAs per SM (up to 128 registers):
+// under the 12 of preprocess_backward_kernel (80 registers) its BOUND instances spill.
+template <bool BOUND, bool DEVFOV>
+__global__ void __launch_bounds__(PRE_NT, 8) preprocess_backward_depth_kernel(gab200_backward_args b,
+                                                                        gab200_forward_args a,
+                                                                        const SplatRec* __restrict__ rec,
+                                                                        const SplatAux* __restrict__ aux,
+                                                                        const uint8_t* __restrict__ clamped,
+                                                                        const float* __restrict__ g2d,
+                                                                        float* __restrict__ face_scratch,
+                                                                        const float* __restrict__ tanfov) {
+  constexpr bool MC = false, DEPTH = true;
+#include "preprocess_bwd_splat.inc"
 }
 
 // gab200_backward_views (BOUND_RAW): one thread per REAL splat i walks the views in order.  Per view k it stages camera
@@ -364,12 +213,18 @@ __global__ void __launch_bounds__(256) face_grad_reduce_kernel(int num_chunks, c
 
 void launch_preprocess_backward(const gab200_backward_args& b, const SplatRec* rec, const SplatAux* aux,
                                 const uint8_t* clamped, const float* g2d, float* face_scratch, const float* tanfov,
-                                cudaStream_t stream) {
+                                cudaStream_t stream, bool depth) {
   const gab200_forward_args& a = *b.fwd;
   const int threads = PRE_NT, blocks = (a.P + threads - 1) / threads;
   if (blocks == 0) return;
   const bool dev = tanfov != nullptr;
-  if (a.input_mode == GAB200_INPUT_BOUND_RAW) {
+  if (depth) {  // multicast refused by the caller
+    auto kernel = a.input_mode == GAB200_INPUT_BOUND_RAW
+                      ? (dev ? preprocess_backward_depth_kernel<true, true> : preprocess_backward_depth_kernel<true, false>)
+                      : (dev ? preprocess_backward_depth_kernel<false, true> : preprocess_backward_depth_kernel<false, false>);
+    kernel<<<blocks, threads, 0, stream>>>(b, a, rec, aux, clamped, g2d,
+                                           a.input_mode == GAB200_INPUT_BOUND_RAW ? face_scratch : nullptr, tanfov);
+  } else if (a.input_mode == GAB200_INPUT_BOUND_RAW) {
     auto kernel = b.grads_are_multicast
                       ? (dev ? preprocess_backward_kernel<true, true, true> : preprocess_backward_kernel<true, true, false>)
                       : (dev ? preprocess_backward_kernel<true, false, true> : preprocess_backward_kernel<true, false, false>);

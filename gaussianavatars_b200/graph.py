@@ -677,7 +677,7 @@ class GraphedRender(_Captured):
                  scaling_modifier: float = 1.0, mesh_update: bool = True, host_slots: int = 0,
                  capacity: Optional[int] = None, headroom: float = 1.25, warm_cameras=None, warm_timesteps=None,
                  mesh_opacity: Optional[float] = None, face_colors: Optional[torch.Tensor] = None,
-                 mesh_lighting: str = "front", views_per_replay: int = 1):
+                 mesh_lighting: str = "front", views_per_replay: int = 1, depth_alpha: bool = False):
         """outputs: "u8" (the display image only: the float image is not written), "float" or "both".
         warm_cameras: camera objects or 37-float blocks rendered eagerly before the capture to size the capacity (and
         the depth-sort range); warm_timesteps: with a FLAME head, the timesteps each warm camera is rendered at
@@ -685,10 +685,16 @@ class GraphedRender(_Captured):
         views_per_replay=K > 1: every replay renders K cameras of one timestep in one forward
         (gab200_forward_views): the head is posed once, set_inputs(cameras=...) takes K cameras (or a (K, 37) table),
         warm_cameras is a list of such camera groups, and display / image / radii / the host slots carry a leading K
-        dimension.  Not combinable with the mesh overlay."""
+        dimension.  Not combinable with the mesh overlay.
+        depth_alpha=True: every replay also refreshes `alpha` and `depth`, (1,H,W) float32 static tensors -- the
+        splats' accumulated opacity and alpha-weighted view-space depth from the same blend (gab200_forward_depth_alpha;
+        with the mesh overlay they remain the splats').  Single-view replays only."""
         if outputs not in ("u8", "float", "both"):
             raise ValueError("outputs must be 'u8', 'float' or 'both'")
         _check_views_per_replay(views_per_replay)
+        if depth_alpha and views_per_replay > 1:
+            raise ValueError("depth_alpha renders one camera per replay: it needs views_per_replay=1 (the K-view "
+                             "forward has no alpha / depth planes)")
         if views_per_replay > 1 and mesh_opacity is not None:
             raise ValueError("the mesh overlay draws one camera per replay: it needs views_per_replay=1")
         self.K = int(views_per_replay)
@@ -702,7 +708,8 @@ class GraphedRender(_Captured):
         self.host_slots = int(host_slots)
         self.host = self._copy_stream = None
         self._staged = self._host_events = self._stage_events = None
-        self.image = self.display = self.radii = None
+        self.image = self.display = self.radii = self.alpha = self.depth = None
+        self.depth_alpha = bool(depth_alpha)
         self.mesh = mesh_opacity is not None
         if self.mesh:
             if outputs == "float":
@@ -771,10 +778,12 @@ class GraphedRender(_Captured):
                                      self.outputs != "float", self.outputs != "u8")
             else:
                 out = _forward_only(self.camera, self.pc, _Pipe, self.bg, self.scaling_modifier,
-                                    self.outputs != "float" and not self.mesh, self.outputs != "u8" or self.mesh)
+                                    self.outputs != "float" and not self.mesh, self.outputs != "u8" or self.mesh,
+                                    self.depth_alpha)
             if self.mesh:
                 out["display_u8"] = self._overlay(out["render"])
         self.image, self.display, self.radii = out["render"], out["display_u8"], out["radii"]
+        self.alpha, self.depth = out.get("alpha"), out.get("depth")
 
     def _overlay(self, image):
         """The mesh of the vertices the frame just posed (pc.verts) over the float splat image -> (H,W,3) uint8."""
@@ -792,7 +801,7 @@ class GraphedRender(_Captured):
 
     # ---- capture ---------------------------------------------------------------------------------------------------
     def _release(self):
-        self.image = self.display = self.radii = None
+        self.image = self.display = self.radii = self.alpha = self.depth = None
 
     def _before_capture(self):
         if self.camera is not None:

@@ -230,11 +230,13 @@ def check_rgb8(rgb8: Optional[torch.Tensor], rs: GaussianRasterizationSettings, 
 
 
 def _run_forward(a: N.ForwardArgs, device, need_backward: bool, hints: Optional[FrameHints] = None,
-                 tanfov: Optional[torch.Tensor] = None, rgb8: Optional[torch.Tensor] = None, float_image: bool = True):
+                 tanfov: Optional[torch.Tensor] = None, rgb8: Optional[torch.Tensor] = None, float_image: bool = True,
+                 planes: Optional[tuple] = None):
     """tanfov: None (a.tanfovx / tanfovy) or the (2,) device tensor the kernels read instead
     (gab200_forward_device_fov); the backward must then be given the same tensor.
     rgb8: None, or a (H,W,3) uint8 tensor the blend writes the display image into (gab200_forward_display);
-    float_image=False (with rgb8, no backward) skips the float image: the returned color is None."""
+    float_image=False (with rgb8, no backward) skips the float image: the returned color is None.
+    planes: None, or (alpha, depth) (1,H,W) float32 tensors the blend also fills (gab200_forward_depth_alpha)."""
     global _last, _last_info
     H, W, P = a.image_height, a.image_width, a.P
     color = torch.empty((3, H, W), dtype=torch.float32, device=device) if float_image else None
@@ -267,7 +269,10 @@ def _run_forward(a: N.ForwardArgs, device, need_backward: bool, hints: Optional[
         a.frame_seq = hints.seq
     with torch.cuda.device(device):
         stream = torch.cuda.current_stream(device).cuda_stream
-        if rgb8 is not None:
+        if planes is not None:
+            n = N.lib().gab200_forward_depth_alpha(C.byref(a), N.ptr(tanfov), planes[0].data_ptr(),
+                                                   planes[1].data_ptr(), N.ptr(rgb8), C.byref(st), C.c_void_p(stream))
+        elif rgb8 is not None:
             n = N.lib().gab200_forward_display(C.byref(a), N.ptr(tanfov), rgb8.data_ptr(), C.byref(st),
                                                C.c_void_p(stream))
         elif tanfov is None:
@@ -290,11 +295,17 @@ def _run_forward(a: N.ForwardArgs, device, need_backward: bool, hints: Optional[
     return color, radii, st, holder
 
 
-def _run_backward(b: N.BackwardArgs, device, tanfov: Optional[torch.Tensor] = None):
-    """gab200_backward, or gab200_backward_device_fov with the tensor the forward read."""
+def _run_backward(b: N.BackwardArgs, device, tanfov: Optional[torch.Tensor] = None,
+                  plane_grads: Optional[tuple] = None):
+    """gab200_backward, or gab200_backward_device_fov with the tensor the forward read; plane_grads: (dL/dalpha,
+    dL/ddepth), each a contiguous (1,H,W) tensor or None, of a depth_alpha frame (gab200_backward_depth_alpha)."""
     with torch.cuda.device(device):
         stream = torch.cuda.current_stream(device).cuda_stream
-        if tanfov is None:
+        if plane_grads is not None:
+            N.check(N.lib().gab200_backward_depth_alpha(C.byref(b), N.ptr(tanfov), N.ptr(plane_grads[0]),
+                                                        N.ptr(plane_grads[1]), C.c_void_p(stream)),
+                    "gab200_backward_depth_alpha")
+        elif tanfov is None:
             N.check(N.lib().gab200_backward(C.byref(b), C.c_void_p(stream)), "gab200_backward")
         else:
             N.check(N.lib().gab200_backward_device_fov(C.byref(b), tanfov.data_ptr(), C.c_void_p(stream)),
@@ -391,7 +402,13 @@ class GaussianRasterizer(nn.Module):
         return out.bool()
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
-                cov3D_precomp=None):
+                cov3D_precomp=None, depth_alpha=False):
+        """The reference's (color, radii).  depth_alpha=True is refused: the alpha / depth planes are on the fused
+        route, rasterize_bound(..., depth_alpha=True) or render(..., depth_alpha=True)."""
+        if depth_alpha:
+            raise ValueError("GaussianRasterizer (the drop-in for diff_gaussian_rasterization) returns the reference's "
+                             "(color, radii) only: for the alpha and depth planes use the fused route, "
+                             "rasterize_bound(..., depth_alpha=True) or render(..., depth_alpha=True)")
         if (shs is None and colors_precomp is None) or (shs is not None and colors_precomp is not None):
             raise Exception('Please provide excatly one of either SHs or precomputed colors!')
         if ((scales is None or rotations is None) and cov3D_precomp is None) or \
@@ -440,7 +457,7 @@ class _RasterizeBound(torch.autograd.Function):
     @staticmethod
     def forward(ctx, _xyz, means2D, _rotation, _scaling, _opacity, f_dc, f_rest, face_center, face_orien_mat,
                 face_scaling, binding, colors_precomp, raster_settings, grad_sink=None, tanfov=None, rgb8=None,
-                float_image=True):
+                float_image=True, depth_alpha=False):
         rs = raster_settings
         ctx.grad_sink = grad_sink
         device = _xyz.device
@@ -476,10 +493,15 @@ class _RasterizeBound(torch.autograd.Function):
         rgb8 = check_rgb8(rgb8, rs, device)
         if not float_image and (rgb8 is None or need_bw):
             raise ValueError("float_image=False needs rgb8= and no gradient (the backward reads the float image's state)")
+        planes = None
+        if depth_alpha:
+            planes = (torch.empty((1, rs.image_height, rs.image_width), dtype=torch.float32, device=device),
+                      torch.empty((1, rs.image_height, rs.image_width), dtype=torch.float32, device=device))
         color, radii, st, holder = _run_forward(a, device, need_bw,
                                                 hints_of(grad_sink) if grad_sink is not None else None, tanfov,
-                                                rgb8, float_image)
+                                                rgb8, float_image, planes)
         ctx.tanfov = tanfov
+        ctx.depth_alpha = bool(depth_alpha)
         if need_bw:
             ctx.args, ctx.state, ctx.holder = a, st, holder
             ctx.keep = (cams, _xyz, _rotation, _scaling, _opacity, f_dc, f_rest, face_center, face_orien_mat,
@@ -491,10 +513,12 @@ class _RasterizeBound(torch.autograd.Function):
             ctx.want_face = binding is not None and any(ctx.needs_input_grad[7:10])
             ctx.csr = _face_csr(binding_orig, F)[1] if ctx.want_face else None
         ctx.mark_non_differentiable(radii)
+        if planes is not None:
+            return color, radii, planes[0], planes[1]
         return color, radii
 
     @staticmethod
-    def backward(ctx, grad_out_color, _grad_radii):
+    def backward(ctx, grad_out_color, _grad_radii, *grad_planes):
         a, st = ctx.args, ctx.state
         P, M, F = ctx.dims
         device = ctx.keep[1].device
@@ -544,20 +568,24 @@ class _RasterizeBound(torch.autograd.Function):
             b.face_perm, b.face_chunk_face = perm.data_ptr(), c_face.data_ptr()
             b.face_chunk_start, b.face_chunk_end = c_start.data_ptr(), c_end.data_ptr()
             b.num_face_chunks = c_face.shape[0]
-        _run_backward(b, device, ctx.tanfov)
+        plane_grads = None
+        if ctx.depth_alpha:   # gradients of the alpha / depth planes (None: the loss does not read that plane)
+            plane_grads = tuple(None if t is None else (t if t.is_contiguous() else t.contiguous()) for t in grad_planes)
+        _run_backward(b, device, ctx.tanfov, plane_grads)
         ctx.holder = None
         if ctx.grad_sink is not None:  # dist.py: ONE all-reduce over this buffer instead of six
             ctx.grad_sink.flat_grad = flat
             ctx.grad_sink._gab200_mc_used = bool(use_symm)  # SymmetricGradBuffer.end() only trusts the replica if set
         return (d_xyz, d_means2D, d_rot, d_scale, d_opac, d_dc, d_rest, d_fc, d_fR, d_fs, None, d_colors, None, None,
-                None, None, None)
+                None, None, None, None)
 
 
 def rasterize_bound(raster_settings: GaussianRasterizationSettings, _xyz, _rotation, _scaling, _opacity,
                     features_dc, features_rest, binding=None, face_center=None, face_orien_mat=None,
                     face_scaling=None, means2D=None, colors_precomp=None, grad_sink=None, tanfov=None, rgb8=None,
-                    float_image=True):
-    """Fused binding + rasterization.  Returns (color (3,H,W), radii (P,) int32).
+                    float_image=True, depth_alpha=False):
+    """Fused binding + rasterization.  Returns (color (3,H,W), radii (P,) int32); with depth_alpha=True
+    (color, radii, alpha (1,H,W), depth (1,H,W)).
 
     binding=None is the identity frame (a plain GaussianModel, scene/gaussian_model.py:115-116,127-128,142-143).
     `means2D` is the usual (P,3) gradient holder (its .grad receives dL/dmean2D in NDC units).
@@ -566,14 +594,23 @@ def rasterize_bound(raster_settings: GaussianRasterizationSettings, _xyz, _rotat
     negative or non-finite values cull every splat (image = background).
     `rgb8`: optional contiguous (H,W,3) uint8 CUDA tensor that the forward blend also fills with the display image,
     bit for bit torch's color.mul(255).add_(0.5).clamp_(0, 255).permute(1, 2, 0).to(torch.uint8)
-    (gab200_forward_display).  float_image=False (rgb8 given, no gradient) skips the float image: color is None."""
+    (gab200_forward_display).  float_image=False (rgb8 given, no gradient) skips the float image: color is None.
+    depth_alpha=True (gab200_forward_depth_alpha): also the accumulated alpha 1 - T_final and the alpha-weighted
+    view-space depth sum_i w_i z_i (not normalised: depth / alpha is a viewer's depth) of the same blend, both
+    differentiable; the colour image, radii and display bytes are those of depth_alpha=False bit for bit.  The gradients
+    are plain stores: a grad_sink whose symmetric gradient buffer is in "push" (multicast) mode is refused."""
+    if depth_alpha:
+        symm = getattr(grad_sink, "symm_grad", None) if grad_sink is not None else None
+        if symm is not None and symm.enabled and getattr(symm, "mode", "push") == "push":
+            raise ValueError("rasterize_bound(depth_alpha=True) writes plain gradients: use the symmetric gradient "
+                             "buffer in 'two_shot' or 'plain' mode, not 'push'")
     if means2D is None:
         means2D = torch.zeros((_xyz.shape[0], 3), dtype=torch.float32, device=_xyz.device)
     if _opacity.ndim == 1:
         _opacity = _opacity[:, None]
     return _RasterizeBound.apply(_xyz, means2D, _rotation, _scaling, _opacity, features_dc, features_rest,
                                  face_center, face_orien_mat, face_scaling, binding, colors_precomp, raster_settings,
-                                 grad_sink, tanfov, rgb8, bool(float_image))
+                                 grad_sink, tanfov, rgb8, bool(float_image), bool(depth_alpha))
 
 
 # ================================================================================================================

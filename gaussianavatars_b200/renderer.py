@@ -15,6 +15,8 @@ A camera may carry its field of view in device memory as `cam.tanfov`, a (2,) fl
 instead of FoVx / FoVy; the reference route cannot and refuses such a camera.
 `render_views(cameras, ...)` renders every camera of a rig (one image size) in one forward, forward only;
 `render_views_train(cameras, ...)` is its differentiable form, for a training step over every camera of a timestep.
+`depth_alpha=True` (render, render_bound, render_display; fused route only) adds "alpha" (1,H,W), the accumulated
+opacity 1 - T_final, and "depth" (1,H,W), the alpha-weighted view-space depth, both from the colour blend itself.
 """
 from __future__ import annotations
 
@@ -65,21 +67,26 @@ def _fused_frame(cam, pc, pipe, bg_color, scaling_modifier):
     return rs, binding, (pc.face_center, pc.face_orien_mat, pc.face_scaling)
 
 
-def render_bound(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_color=None):
-    """Fused route (see module docstring)."""
+def render_bound(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_color=None, depth_alpha=False):
+    """Fused route (see module docstring).  depth_alpha=True adds the differentiable "alpha" and "depth" planes."""
     rs, binding, (fc, fR, fs) = _fused_frame(viewpoint_camera, pc, pipe, bg_color, scaling_modifier)
     screenspace_points = torch.zeros((pc._xyz.shape[0], 3), dtype=pc._xyz.dtype, device=pc._xyz.device,
                                      requires_grad=True)
-    rendered_image, radii = rasterize_bound(rs, pc._xyz, pc._rotation, pc._scaling, pc._opacity, pc._features_dc,
-                                            pc._features_rest, binding, fc, fR, fs, means2D=screenspace_points,
-                                            colors_precomp=override_color, grad_sink=pc,
-                                            tanfov=getattr(viewpoint_camera, "tanfov", None))
-    return {"render": rendered_image, "viewspace_points": screenspace_points, "visibility_filter": _visible(radii),
-            "radii": radii}
+    out = rasterize_bound(rs, pc._xyz, pc._rotation, pc._scaling, pc._opacity, pc._features_dc, pc._features_rest,
+                          binding, fc, fR, fs, means2D=screenspace_points, colors_precomp=override_color, grad_sink=pc,
+                          tanfov=getattr(viewpoint_camera, "tanfov", None), depth_alpha=depth_alpha)
+    rendered_image, radii = out[0], out[1]
+    res = {"render": rendered_image, "viewspace_points": screenspace_points, "visibility_filter": _visible(radii),
+           "radii": radii}
+    if depth_alpha:
+        res["alpha"], res["depth"] = out[2], out[3]
+    return res
 
 
-def _forward_only(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, display: bool, float_image: bool):
-    """Fused route, forward only (no autograd): the float image and/or the display image."""
+def _forward_only(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, display: bool, float_image: bool,
+                  depth_alpha: bool = False):
+    """Fused route, forward only (no autograd): the float image and/or the display image [and the alpha / depth
+    planes]."""
     if not _has_raw(pc):
         raise ValueError("render_display needs the fused route: a model exposing the raw parameters "
                          "(_xyz, _rotation, _scaling, _opacity, _features_dc, _features_rest)")
@@ -88,20 +95,26 @@ def _forward_only(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, displa
     with torch.no_grad():
         rs, binding, (fc, fR, fs) = _fused_frame(viewpoint_camera, pc, pipe, bg_color, scaling_modifier)
         rgb8 = torch.empty((rs.image_height, rs.image_width, 3), dtype=torch.uint8, device=device) if display else None
-        img, radii = rasterize_bound(rs, d(pc._xyz), d(pc._rotation), d(pc._scaling), d(pc._opacity),
-                                     d(pc._features_dc), d(pc._features_rest), binding, d(fc), d(fR), d(fs),
-                                     grad_sink=pc, tanfov=getattr(viewpoint_camera, "tanfov", None), rgb8=rgb8,
-                                     float_image=float_image)
-    return {"display_u8": rgb8, "render": img, "radii": radii, "visibility_filter": _visible(radii)}
+        out = rasterize_bound(rs, d(pc._xyz), d(pc._rotation), d(pc._scaling), d(pc._opacity), d(pc._features_dc),
+                              d(pc._features_rest), binding, d(fc), d(fR), d(fs), grad_sink=pc,
+                              tanfov=getattr(viewpoint_camera, "tanfov", None), rgb8=rgb8, float_image=float_image,
+                              depth_alpha=depth_alpha)
+    img, radii = out[0], out[1]
+    res = {"display_u8": rgb8, "render": img, "radii": radii, "visibility_filter": _visible(radii)}
+    if depth_alpha:
+        res["alpha"], res["depth"] = out[2], out[3]
+    return res
 
 
-def render_display(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, float_image=False):
+def render_display(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, float_image=False, depth_alpha=False):
     """One playback frame: the fused route's forward only, no autograd, with the image as the reference's render.py
     and viewers consume it -- `display_u8`, a (H,W,3) uint8 tensor equal bit for bit to
     render(...)["render"].mul(255).add_(0.5).clamp_(0, 255).permute(1, 2, 0).to(torch.uint8), written by the forward
     blend itself (3 bytes per pixel instead of 12, no eager quantisation chain).  float_image=True also returns the
-    float (3,H,W) image as "render" (else None).  Returns {"display_u8", "render", "radii", "visibility_filter"}."""
-    return _forward_only(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, True, float_image)
+    float (3,H,W) image as "render" (else None).  Returns {"display_u8", "render", "radii", "visibility_filter"};
+    depth_alpha=True adds "alpha" and "depth" (1,H,W) float32, from the same blend (the viewers' opacity / depth modes;
+    a normalised depth is depth / alpha)."""
+    return _forward_only(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, True, float_image, depth_alpha)
 
 
 def camera_table(cameras, device) -> torch.Tensor:
@@ -202,12 +215,17 @@ def _visible(radii):
     return v if v is not None else radii > 0
 
 
-def render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_color=None, fused=None):
+def render(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_color=None, fused=None,
+           depth_alpha=False):
     python_paths = bool(getattr(pipe, "compute_cov3D_python", False)) or bool(getattr(pipe, "convert_SHs_python", False))
     if fused is None:
         fused = _has_raw(pc) and not python_paths
     if fused:
-        return render_bound(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_color)
+        return render_bound(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_color, depth_alpha)
+    if depth_alpha:
+        raise ValueError("depth_alpha=True needs the fused route (render_bound / rasterize_bound on a model exposing the "
+                         "raw parameters, without compute_cov3D_python / convert_SHs_python): the reference route's "
+                         "GaussianRasterizer returns only (color, radii)")
 
     # ---- reference route (data flow of gaussian_renderer/__init__.py:27-101) ----
     if getattr(viewpoint_camera, "tanfov", None) is not None:

@@ -175,7 +175,8 @@ typedef struct gab200_frame_state {
   int32_t sort_bits;          /* key width of the per-instance (stage B) radix sort: bits(tile id) */
   int32_t depth_bits;         /* key width of the per-splat (stage A) radix sort: 32 (the fp32 depth pattern); the two
                                  stable stages together are the reference's LSD sort of (tile << 32 | depth) */
-  uint32_t depth_prefix;      /* reserved (0) */
+  uint32_t depth_prefix;      /* 1: a gab200_forward_depth_alpha frame kept for a backward -- its records carry the
+                                 view-space depth that gab200_backward_depth_alpha reads; 0 for every other forward */
   int64_t binning_capacity;   /* instances the binning buffer was carved for (>= num_rendered; = binning_hint when the
                                  speculative allocation was large enough) */
   uint32_t depth_key_min;     /* smallest / largest depth key among the splats that emitted instances (min > max: none) */
@@ -271,6 +272,33 @@ int32_t gab200_backward_device_fov(const gab200_backward_args* args, const float
  * supported; a frame the library re-enqueues (GAB200_SYNC_LATE) rewrites out_rgb8 with the EXACT frame's bytes. */
 int64_t gab200_forward_display(const gab200_forward_args* args, const float* tanfov, uint8_t* out_rgb8,
                                gab200_frame_state* state_out, void* stream);
+
+/* Opacity and depth beside the colour, from the same blend.  For each pixel the splats are walked exactly as the colour
+ * blend walks them: the same list, the same alpha, the same 1/255 skip, the same T < 1e-4 stop.
+ *   alpha = 1.0f - T_final, rounded once in fp32, where T_final is the transmittance the colour image uses as its
+ *           background weight, so image = C + (1 - alpha) * bg holds exactly;
+ *   depth = sum_i w_i z_i, accumulated as D = fmaf(z_i, w_i, D) in the same order and at the same point as the colour
+ *           channels, with w_i = alpha_i T_i and z_i the splat's view-space depth (the fp32 value whose bits form its
+ *           depth sort key: t.z = V[2] x + V[6] y + V[10] z + V[14] of the world-space mean).  Not normalised: a
+ *           viewer's normalised depth is depth / alpha.  Inverse depth is not offered.
+ * gab200_forward_depth_alpha is gab200_forward_display plus out_alpha and out_depth, DEVICE float [H,W] each; either may
+ * be NULL, not both (GAB200_ERR_INVALID_ARGUMENT before any device work).  The colour image, display bytes, radii,
+ * visibility and the backward state are those of gab200_forward_display bit for bit.  Every sync mode works; a frame
+ * the library re-enqueues (GAB200_SYNC_LATE) rewrites both planes with the EXACT frame's values.  With need_backward,
+ * state_out->depth_prefix = 1: the records carry z.
+ * gab200_backward_depth_alpha is gab200_backward_device_fov (tanfov: the forward's, or NULL) plus dL_dalpha and
+ * dL_ddepth, DEVICE float [H,W] each or NULL (= zero):
+ *   dL/dalpha joins the background term: dL/dT_final gains -dL/dalpha;
+ *   dL/ddepth is a fourth colour channel with c = z and bg = 0; each splat receives dL/dz = sum_pixels w dL/ddepth,
+ *           which reaches the 3-D mean through t.z (then the binding chain and the face frame like every mean gradient);
+ *   dL_dmeans2D includes the alpha and depth contributions (the gradient of the whole loss).
+ * Before any device work, GAB200_ERR_INVALID_ARGUMENT for every error of gab200_backward, for a state whose
+ * depth_prefix != 1 (a plain forward's, or a multi-view frame's) and for grads_are_multicast != 0.  gab200_backward on a
+ * depth-alpha state is valid: the same backward with both plane gradients zero. */
+int64_t gab200_forward_depth_alpha(const gab200_forward_args* args, const float* tanfov, float* out_alpha,
+                                   float* out_depth, uint8_t* out_rgb8, gab200_frame_state* state_out, void* stream);
+int32_t gab200_backward_depth_alpha(const gab200_backward_args* args, const float* tanfov, const float* dL_dalpha,
+                                    const float* dL_ddepth, void* stream);
 
 /* Every camera of a rig in one forward: `views` cameras render one splat set, the way a calibrated capture is
  * rendered and evaluated (all views of a timestep share the pose, so they need one pass, not one each).
