@@ -215,7 +215,9 @@ EXPORTED_SYMBOLS = ("gab200_forward", "gab200_backward", "gab200_mark_visible", 
                     "gab200_forward_device_fov", "gab200_backward_device_fov", "gab200_forward_display",
                     "gab200_image_metrics", "gab200_image_metrics_scratch_bytes", "gab200_mesh_render",
                     "gab200_mesh_scratch_bytes", "gab200_forward_views", "gab200_forward_views_train",
-                    "gab200_backward_views", "gab200_forward_depth_alpha", "gab200_backward_depth_alpha")
+                    "gab200_backward_views", "gab200_forward_depth_alpha", "gab200_backward_depth_alpha",
+                    "gab200_forward_views_depth_alpha", "gab200_forward_views_train_depth_alpha",
+                    "gab200_backward_views_depth_alpha")
 
 _lib = None
 _lock = threading.Lock()
@@ -269,6 +271,16 @@ def lib():
         L.gab200_backward_depth_alpha.restype = C.c_int32
         L.gab200_backward_depth_alpha.argtypes = [C.POINTER(BackwardArgs), C.c_void_p, C.c_void_p, C.c_void_p,
                                                   C.c_void_p]
+        L.gab200_forward_views_depth_alpha.restype = C.c_int64
+        L.gab200_forward_views_depth_alpha.argtypes = [C.POINTER(ForwardArgs), C.c_int32, C.c_void_p, C.c_void_p,
+                                                       C.c_void_p, C.c_void_p, C.POINTER(FrameState), C.c_void_p]
+        L.gab200_forward_views_train_depth_alpha.restype = C.c_int64
+        L.gab200_forward_views_train_depth_alpha.argtypes = [C.POINTER(ForwardArgs), C.c_int32, C.c_void_p,
+                                                             C.c_void_p, C.c_void_p, C.POINTER(FrameState),
+                                                             C.c_void_p]
+        L.gab200_backward_views_depth_alpha.restype = C.c_int32
+        L.gab200_backward_views_depth_alpha.argtypes = [C.POINTER(BackwardArgs), C.c_int32, C.c_void_p, C.c_void_p,
+                                                        C.c_void_p, C.c_void_p]
         L.gab200_mark_visible.restype = C.c_int32
         L.gab200_mark_visible.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gab200_bind_activate.restype = C.c_int32

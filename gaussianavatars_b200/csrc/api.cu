@@ -386,7 +386,8 @@ int enqueue_geometry(Frame& f, bool bucket, bool run_preprocess, uint32_t capaci
     StageScope sc(GAB200_STAGE_PREPROCESS, stream);
     if (f.cameras != nullptr)
       launch_preprocess_views(*a, f.views, f.cameras, g.rec, g.aux, g.tiles_touched, g.depth_keys[0], g.ids[0],
-                              g.buckets, f.counting ? f.iv.tile_count : nullptr, f.nb ? g.clamped : nullptr, stream);
+                              g.buckets, f.counting ? f.iv.tile_count : nullptr, f.nb ? g.clamped : nullptr, stream,
+                              f.da);
     else
       launch_preprocess(*a, g.rec, g.aux, g.tiles_touched, f.nb ? g.clamped : nullptr, g.depth_keys[0], g.ids[0],
                         g.buckets, f.counting ? f.iv.tile_count : nullptr, f.tanfov, stream, f.da);
@@ -504,7 +505,11 @@ int enqueue_binning_blend(Frame& f, void* bin, int64_t cap, int64_t n_known, siz
   st->sorted_selector = selector;
   {
     StageScope sc(GAB200_STAGE_BLEND_FWD, stream);
-    if (f.cameras != nullptr && f.nb)
+    if (f.cameras != nullptr && f.da)
+      launch_blend_forward_views_depth(f.views, f.W, f.H, f.iv.ranges, f.iv.order, f.iv.order_info, bv.vals[selector],
+                                       f.g.rec, a->bg, a->out_color, f.nb ? f.iv.final_T : nullptr, f.iv.n_contrib,
+                                       bv.strip_mask, f.out_rgb8, f.out_alpha, f.out_depth, stream);
+    else if (f.cameras != nullptr && f.nb)
       launch_blend_forward_views_train(f.views, f.W, f.H, f.iv.ranges, f.iv.order, f.iv.order_info, bv.vals[selector],
                                        f.g.rec, a->bg, a->out_color, f.iv.final_T, f.iv.n_contrib, bv.strip_mask,
                                        stream);
@@ -535,7 +540,7 @@ int wait_counters(Frame& f) {
 // gab200_forward, gab200_forward_device_fov and gab200_forward_display (tanfov == NULL: the by-value tanfovx /
 // tanfovy; out_rgb8 == NULL: no display image), and gab200_forward_views[_train] (cameras != NULL: `views` cameras,
 // validated by the caller, as one frame of views * P virtual splats; need_backward: the training form), and
-// gab200_forward_depth_alpha (da: the alpha / depth planes, either may be NULL, validated by the caller)
+// gab200_forward[_views[_train]]_depth_alpha (da: the alpha / depth planes, either may be NULL, validated by the caller)
 static int64_t run_forward(const gab200_forward_args* a, const float* tanfov, uint8_t* out_rgb8,
                            gab200_frame_state* st, void* stream_, int views = 1, const float* cameras = nullptr,
                            bool da = false, float* out_alpha = nullptr, float* out_depth = nullptr) {
@@ -705,8 +710,10 @@ int64_t gab200_forward_depth_alpha(const gab200_forward_args* a, const float* ta
   return run_forward(a, tanfov, out_rgb8, st, stream, 1, nullptr, true, out_alpha, out_depth);
 }
 
-int64_t gab200_forward_views(const gab200_forward_args* a, int32_t views, const float* cameras, uint8_t* out_rgb8,
-                             gab200_frame_state* st, void* stream) {
+// gab200_forward_views, and gab200_forward_views_depth_alpha (da: the planes, not both NULL -- checked by the caller)
+static int64_t run_forward_views(const gab200_forward_args* a, int32_t views, const float* cameras, uint8_t* out_rgb8,
+                                 gab200_frame_state* st, void* stream, bool da = false, float* out_alpha = nullptr,
+                                 float* out_depth = nullptr) {
   if (a == nullptr || a->need_backward != 0 || views < 1 || views > 65535 || cameras == nullptr || st == nullptr)
     return GAB200_ERR_INVALID_ARGUMENT;
   gab200_forward_args v = *a;
@@ -715,7 +722,19 @@ int64_t gab200_forward_views(const gab200_forward_args* a, int32_t views, const 
   const int64_t view_tiles = (((int64_t)v.image_width + GAB_TILE - 1) / GAB_TILE) *
                              (((int64_t)v.image_height + GAB_TILE - 1) / GAB_TILE);
   if ((int64_t)views * v.P > INT32_MAX || (int64_t)views * view_tiles > INT32_MAX) return GAB200_ERR_INVALID_ARGUMENT;
-  return run_forward(&v, nullptr, out_rgb8, st, stream, views, cameras);
+  return run_forward(&v, nullptr, out_rgb8, st, stream, views, cameras, da, out_alpha, out_depth);
+}
+
+int64_t gab200_forward_views(const gab200_forward_args* a, int32_t views, const float* cameras, uint8_t* out_rgb8,
+                             gab200_frame_state* st, void* stream) {
+  return run_forward_views(a, views, cameras, out_rgb8, st, stream);
+}
+
+int64_t gab200_forward_views_depth_alpha(const gab200_forward_args* a, int32_t views, const float* cameras,
+                                         float* out_alpha, float* out_depth, uint8_t* out_rgb8, gab200_frame_state* st,
+                                         void* stream) {
+  if (out_alpha == nullptr && out_depth == nullptr) return GAB200_ERR_INVALID_ARGUMENT;
+  return run_forward_views(a, views, cameras, out_rgb8, st, stream, true, out_alpha, out_depth);
 }
 
 // the argument checks gab200_forward_views_train and gab200_backward_views share: the camera table, the limits of the
@@ -740,7 +759,19 @@ int64_t gab200_forward_views_train(const gab200_forward_args* a, int32_t views, 
   return run_forward(&v, nullptr, nullptr, st, stream, views, cameras);
 }
 
-int32_t gab200_backward_views(const gab200_backward_args* b, int32_t views, const float* cameras, void* stream_) {
+int64_t gab200_forward_views_train_depth_alpha(const gab200_forward_args* a, int32_t views, const float* cameras,
+                                               float* out_alpha, float* out_depth, gab200_frame_state* st,
+                                               void* stream) {
+  gab200_forward_args v;
+  if (!validate_views_train(a, views, cameras, v) || st == nullptr) return GAB200_ERR_INVALID_ARGUMENT;
+  if (out_alpha == nullptr && out_depth == nullptr) return GAB200_ERR_INVALID_ARGUMENT;
+  return run_forward(&v, nullptr, nullptr, st, stream, views, cameras, true, out_alpha, out_depth);
+}
+
+// gab200_backward_views, and gab200_backward_views_depth_alpha (da: the plane gradients, NULL = 0)
+static int32_t run_backward_views(const gab200_backward_args* b, int32_t views, const float* cameras, void* stream_,
+                                  bool da = false, const float* dL_dalpha = nullptr,
+                                  const float* dL_ddepth = nullptr) {
   cudaStream_t stream = (cudaStream_t)stream_;
   if (b == nullptr || b->abi_version != GAB200_ABI_VERSION || b->fwd == nullptr || b->state == nullptr)
     return GAB200_ERR_INVALID_ARGUMENT;
@@ -748,6 +779,7 @@ int32_t gab200_backward_views(const gab200_backward_args* b, int32_t views, cons
   if (!validate_views_train(b->fwd, views, cameras, v)) return GAB200_ERR_INVALID_ARGUMENT;
   const gab200_frame_state* st = b->state;
   if (st->reserved0 != views || b->grads_are_multicast || b->dL_dout_color == nullptr) return GAB200_ERR_INVALID_ARGUMENT;
+  if (da && st->depth_prefix != 1u) return GAB200_ERR_INVALID_ARGUMENT;  // the records of a plain K-view frame carry no z
   if (b->dL_dsh_dc == nullptr || (v.sh_coeffs > 1 && b->dL_dsh_rest == nullptr)) return GAB200_ERR_INVALID_ARGUMENT;
   if (st->geom_buffer == nullptr || st->image_buffer == nullptr || st->binning_buffer == nullptr)
     return GAB200_ERR_INVALID_ARGUMENT;
@@ -776,8 +808,13 @@ int32_t gab200_backward_views(const gab200_backward_args* b, int32_t views, cons
   }
   if (st->num_rendered != 0) {
     StageScope sc(GAB200_STAGE_BLEND_BWD, stream);
-    launch_blend_backward_views(views, W, H, iv.ranges, iv.order, iv.order_info, bv.vals[st->sorted_selector], g.rec,
-                                v.bg, iv.final_T, iv.n_contrib, b->dL_dout_color, bv.strip_mask, g.g2d, stream);
+    if (da)
+      launch_blend_backward_views_depth(views, W, H, iv.ranges, iv.order, iv.order_info, bv.vals[st->sorted_selector],
+                                        g.rec, v.bg, iv.final_T, iv.n_contrib, b->dL_dout_color, bv.strip_mask, g.g2d,
+                                        dL_dalpha, dL_ddepth, stream);
+    else
+      launch_blend_backward_views(views, W, H, iv.ranges, iv.order, iv.order_info, bv.vals[st->sorted_selector], g.rec,
+                                  v.bg, iv.final_T, iv.n_contrib, b->dL_dout_color, bv.strip_mask, g.g2d, stream);
   }
   GAB_STAGE_CHECK(dbg, stream);
   {
@@ -788,10 +825,19 @@ int32_t gab200_backward_views(const gab200_backward_args* b, int32_t views, cons
     gab200_backward_args bb = *b;
     bb.fwd = &v;
     launch_preprocess_backward_views(bb, views, cameras, g.aux, g.clamped, g.g2d, csr ? g.face_scratch : nullptr,
-                                     stream);
+                                     stream, da);
   }
   GAB_STAGE_CHECK(dbg, stream);
   return GAB200_OK;
+}
+
+int32_t gab200_backward_views(const gab200_backward_args* b, int32_t views, const float* cameras, void* stream) {
+  return run_backward_views(b, views, cameras, stream);
+}
+
+int32_t gab200_backward_views_depth_alpha(const gab200_backward_args* b, int32_t views, const float* cameras,
+                                          const float* dL_dalpha, const float* dL_ddepth, void* stream) {
+  return run_backward_views(b, views, cameras, stream, true, dL_dalpha, dL_ddepth);
 }
 
 // gab200_backward and gab200_backward_device_fov, and gab200_backward_depth_alpha (da: the plane gradients, NULL = 0)

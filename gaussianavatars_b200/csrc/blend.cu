@@ -551,6 +551,62 @@ void launch_blend_forward_views_train(int views, int W, int H, const uint2* rang
   count_launch();
 }
 
+// gab200_forward_views_depth_alpha and gab200_forward_views_train_depth_alpha: blend_forward_views_kernel with the alpha
+// and depth planes (forward_tile<.., DA>), written at view k's offset k * H * W; records from preprocess_views_depth_kernel
+// (z in q2.w).  final_T != nullptr (the training form, OUT = BLEND_OUT_FLOAT): also final_T, n_contrib and the block
+// masks, as blend_forward_views_train_kernel keeps them.  Bounded as blend_forward_depth_kernel.
+template <int OUT>
+__global__ void __launch_bounds__(256, GAB_FWD_DEPTH_CTAS) blend_forward_views_depth_kernel(
+    int W, int H, int gx, int tiles, int view_tiles, const uint2* __restrict__ ranges, const uint32_t* __restrict__ order,
+    const uint32_t* __restrict__ order_info, const uint32_t* __restrict__ point_list, const SplatRec* __restrict__ rec,
+    const float* __restrict__ bg, float* __restrict__ out_color, float* __restrict__ final_T,
+    uint32_t* __restrict__ n_contrib, uint8_t* __restrict__ strip_mask, uint8_t* __restrict__ out_rgb8,
+    float* __restrict__ out_alpha, float* __restrict__ out_depth) {
+  __shared__ SplatRec buf[2][256];
+  __shared__ uint32_t smask[256];
+  __shared__ __align__(16) uint32_t ids_ring[4][ID_RING * (64 + 4)];
+  __shared__ __align__(8) uint64_t mbar[4][ID_RING];
+  const int nh = (int)order_info[0];
+  const int b = blockIdx.x, t = threadIdx.x;
+  const bool heavy = b < nh;
+  const int g = heavy ? 0 : t >> 6;
+  const int slot = heavy ? b : nh + 4 * (b - nh) + g;
+  if (slot >= (heavy ? nh : tiles)) return;
+  const int tile = (int)order[slot];
+  const int view = tile / view_tiles, local = tile - view * view_tiles;
+  const size_t HW = (size_t)H * W, off = (size_t)view * HW;
+  float* color = (OUT & BLEND_OUT_FLOAT) ? out_color + 3 * off : nullptr;
+  uint8_t* rgb8 = (OUT & BLEND_OUT_U8) ? out_rgb8 + 3 * off : nullptr;
+  float* vT = final_T != nullptr ? final_T + off : nullptr;
+  uint32_t* vn = final_T != nullptr ? n_contrib + off : nullptr;
+  float* va = out_alpha != nullptr ? out_alpha + off : nullptr;
+  float* vd = out_depth != nullptr ? out_depth + off : nullptr;
+  const uint2* view_ranges = ranges + (size_t)view * view_tiles;
+  if (heavy)
+    forward_tile<1, OUT, true>(local, t, GroupBarrier<256>{0}, buf[0], buf[1], smask, &ids_ring[0][0], mbar[0], W, H,
+                               gx, view_ranges, point_list, rec, bg, color, vT, vn, strip_mask, rgb8, va, vd);
+  else
+    forward_tile<4, OUT, true>(local, t & 63, GroupBarrier<64>{1 + g}, buf[0] + g * 64, buf[1] + g * 64,
+                               smask + g * 64, ids_ring[g], mbar[g], W, H, gx, view_ranges, point_list, rec, bg, color,
+                               vT, vn, strip_mask, rgb8, va, vd);
+}
+
+void launch_blend_forward_views_depth(int views, int W, int H, const uint2* ranges, const uint32_t* order,
+                                      const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
+                                      const float* bg, float* out_color, float* final_T, uint32_t* n_contrib,
+                                      uint8_t* strip_mask, uint8_t* out_rgb8, float* out_alpha, float* out_depth,
+                                      cudaStream_t stream) {
+  const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
+  const int view_tiles = gx * gy, tiles = views * view_tiles;
+  if (tiles == 0) return;
+  auto kernel = out_rgb8 == nullptr ? blend_forward_views_depth_kernel<BLEND_OUT_FLOAT>
+                : out_color == nullptr ? blend_forward_views_depth_kernel<BLEND_OUT_U8>
+                                       : blend_forward_views_depth_kernel<BLEND_OUT_FLOAT | BLEND_OUT_U8>;
+  kernel<<<tiles, 256, 0, stream>>>(W, H, gx, tiles, view_tiles, ranges, order, order_info, point_list, rec, bg,
+                                    out_color, final_T, n_contrib, strip_mask, out_rgb8, out_alpha, out_depth);
+  count_launch();
+}
+
 // =====================================================================================================
 // Backward
 // =====================================================================================================
@@ -978,6 +1034,49 @@ void launch_blend_backward_views(int views, int W, int H, const uint2* ranges, c
   blend_backward_views_kernel<<<tiles, 128, 0, stream>>>(W, H, gx, tiles, view_tiles, ranges, order, order_info,
                                                          point_list, rec, bg, final_T, n_contrib, dL_dpix, strip_mask,
                                                          g2d);
+  count_launch();
+}
+
+// gab200_backward_views_depth_alpha: blend_backward_views_kernel with the plane gradients (backward_task<K, true>):
+// dL/dalpha and dL/ddepth are read at view k's offset, dL/dz leaves for g2d slot 9 of the virtual splat's row.
+// Bounded as blend_backward_depth_kernel.
+__global__ void __launch_bounds__(128, GAB_BWD_DEPTH_CTAS) blend_backward_views_depth_kernel(
+    int W, int H, int gx, int tiles, int view_tiles, const uint2* __restrict__ ranges,
+    const uint32_t* __restrict__ order, const uint32_t* __restrict__ order_info, const uint32_t* __restrict__ point_list,
+    const SplatRec* __restrict__ rec, const float* __restrict__ bg, const float* __restrict__ final_T,
+    const uint32_t* __restrict__ n_contrib, const float* __restrict__ dL_dpix, const uint8_t* __restrict__ strip_mask,
+    float* __restrict__ g2d, const float* __restrict__ dL_dalpha, const float* __restrict__ dL_ddepth) {
+  __shared__ WarpSmemT<10> sm[4];
+  const int nh = (int)order_info[1];
+  const int b = blockIdx.x, t = threadIdx.x, w = t >> 5;
+  const bool heavy = b < nh;
+  const int slot = heavy ? b : nh + 2 * (b - nh) + (w >> 1);
+  if (!heavy && slot >= tiles) return;
+  const int tile = (int)order[slot];
+  const int view = tile / view_tiles, local = tile - view * view_tiles;
+  const size_t HW = (size_t)H * W, off = (size_t)view * HW;
+  const uint2* vr = ranges + (size_t)view * view_tiles;
+  const float* va = dL_dalpha != nullptr ? dL_dalpha + off : nullptr;
+  const float* vz = dL_ddepth != nullptr ? dL_ddepth + off : nullptr;
+  if (heavy)
+    backward_task<2, true>(local, t, sm[w], W, H, gx, vr, point_list, rec, bg, final_T + off, n_contrib + off,
+                           dL_dpix + 3 * off, strip_mask, g2d, va, vz);
+  else
+    backward_task<4, true>(local, t & 63, sm[w], W, H, gx, vr, point_list, rec, bg, final_T + off, n_contrib + off,
+                           dL_dpix + 3 * off, strip_mask, g2d, va, vz);
+}
+
+void launch_blend_backward_views_depth(int views, int W, int H, const uint2* ranges, const uint32_t* order,
+                                       const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
+                                       const float* bg, const float* final_T, const uint32_t* n_contrib,
+                                       const float* dL_dpix, const uint8_t* strip_mask, float* g2d,
+                                       const float* dL_dalpha, const float* dL_ddepth, cudaStream_t stream) {
+  const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
+  const int view_tiles = gx * gy, tiles = views * view_tiles;
+  if (tiles == 0) return;
+  blend_backward_views_depth_kernel<<<tiles, 128, 0, stream>>>(W, H, gx, tiles, view_tiles, ranges, order, order_info,
+                                                               point_list, rec, bg, final_T, n_contrib, dL_dpix,
+                                                               strip_mask, g2d, dL_dalpha, dL_ddepth);
   count_launch();
 }
 

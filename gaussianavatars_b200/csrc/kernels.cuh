@@ -103,10 +103,11 @@ void launch_preprocess(const gab200_forward_args& a, SplatRec* rec, SplatAux* au
                        uint32_t* tile_count, const float* tanfov, cudaStream_t stream, bool rec_depth = false);
 // gab200_forward_views: grid (splat blocks, views); camera row k of `cameras` renders virtual splats k * P + i
 // (rec / aux / tiles / depth keys / ids / radii / visibility), tile counts at k * (gx * gy) + the tile in the view;
-// clamped != nullptr (gab200_forward_views_train, BOUND_RAW only): also the colour clamp bits at k * P + i
+// clamped != nullptr (gab200_forward_views_train, BOUND_RAW only): also the colour clamp bits at k * P + i;
+// rec_depth: the records carry the view-space depth in q2.w (gab200_forward_views[_train]_depth_alpha)
 void launch_preprocess_views(const gab200_forward_args& a, int views, const float* cameras, SplatRec* rec, SplatAux* aux,
                              uint32_t* tiles_touched, uint32_t* depth_keys, uint32_t* ids, const DepthBuckets& buckets,
-                             uint32_t* tile_count, uint8_t* clamped, cudaStream_t stream);
+                             uint32_t* tile_count, uint8_t* clamped, cudaStream_t stream, bool rec_depth = false);
 // depth_keys [P] (by splat) -> sorted_ids [M] in (key, id) order and offsets [M] = inclusive instance counts
 // also publishes the frame counters (capacity, seq, overflow) of the bucket-sorted frame
 void launch_depth_bucket_sort(int P, const DepthBuckets& buckets, const uint32_t* depth_keys,
@@ -177,6 +178,13 @@ void launch_blend_forward_views_train(int views, int W, int H, const uint2* rang
                                       const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
                                       const float* bg, float* out_color, float* final_T, uint32_t* n_contrib,
                                       uint8_t* strip_mask, cudaStream_t stream);
+// either multi-view forward plus the alpha and depth planes [views,H,W] (either may be NULL); records with z in q2.w.
+// final_T != NULL: the training form (out_color only; final_T / n_contrib / block masks kept as above)
+void launch_blend_forward_views_depth(int views, int W, int H, const uint2* ranges, const uint32_t* order,
+                                      const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
+                                      const float* bg, float* out_color, float* final_T, uint32_t* n_contrib,
+                                      uint8_t* strip_mask, uint8_t* out_rgb8, float* out_alpha, float* out_depth,
+                                      cudaStream_t stream);
 void launch_blend_backward(int W, int H, const uint2* ranges, const uint32_t* order, const uint32_t* order_info,
                            const uint32_t* point_list, const SplatRec* rec,
                            const float* bg, const float* final_T, const uint32_t* n_contrib, const float* dL_dpix,
@@ -191,6 +199,13 @@ void launch_blend_backward_views(int views, int W, int H, const uint2* ranges, c
                                  const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
                                  const float* bg, const float* final_T, const uint32_t* n_contrib, const float* dL_dpix,
                                  const uint8_t* strip_mask, float* g2d, cudaStream_t stream);
+// launch_blend_backward_views plus the plane gradients dL_dalpha / dL_ddepth [views,H,W] (NULL: zero); dL/dz -> g2d
+// slot 9 of each virtual splat's row
+void launch_blend_backward_views_depth(int views, int W, int H, const uint2* ranges, const uint32_t* order,
+                                       const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
+                                       const float* bg, const float* final_T, const uint32_t* n_contrib,
+                                       const float* dL_dpix, const uint8_t* strip_mask, float* g2d,
+                                       const float* dL_dalpha, const float* dL_ddepth, cudaStream_t stream);
 
 // preprocess_bwd.cu
 // depth: g2d slot 9 holds dL/dz (gab200_backward_depth_alpha), added to dL/dmean through the view matrix's third row;
@@ -200,10 +215,12 @@ void launch_preprocess_backward(const gab200_backward_args& b, const SplatRec* r
                                 cudaStream_t stream, bool depth = false);
 // gab200_backward_views (BOUND_RAW, no colors_precomp, no multicast): one thread per real splat sums the gradients of
 // its `views` virtual splats (camera row k of `cameras`; rec / aux / clamped / g2d rows k * P + i) and stores each
-// parameter gradient once; dL_dmeans2D [views,P,3]; face-frame gradients as launch_preprocess_backward's
+// parameter gradient once; dL_dmeans2D [views,P,3]; face-frame gradients as launch_preprocess_backward's.
+// depth: g2d slot 9 holds each virtual splat's dL/dz (gab200_backward_views_depth_alpha), added through view k's own
+// view-matrix row
 void launch_preprocess_backward_views(const gab200_backward_args& b, int views, const float* cameras,
                                       const SplatAux* aux, const uint8_t* clamped, const float* g2d,
-                                      float* face_scratch, cudaStream_t stream);
+                                      float* face_scratch, cudaStream_t stream, bool depth = false);
 #define GAB_FACE_GRAD_STRIDE 13  // per-splat face-frame gradient record: centre 3, orientation 9, scale 1
 
 // face_frame.cu

@@ -127,6 +127,36 @@ __global__ void __launch_bounds__(PRE_NT) preprocess_views_train_kernel(gab200_f
 #undef GAB_PRE_OUT
 }
 
+// gab200_forward_views_depth_alpha / gab200_forward_views_train_depth_alpha: preprocess_views_kernel whose records also
+// carry the view-space depth z of virtual splat view * P + i in q2.w.  clamped != nullptr (the training form, BOUND_RAW
+// only): also the colour clamp bits, as preprocess_views_train_kernel keeps them.
+template <bool BOUND>
+__global__ void __launch_bounds__(PRE_NT) preprocess_views_depth_kernel(gab200_forward_args a,
+                                                                        const float* __restrict__ cameras,
+                                                                        SplatRec* __restrict__ rec,
+                                                                        SplatAux* __restrict__ aux,
+                                                                        uint32_t* __restrict__ tiles_touched,
+                                                                        uint8_t* __restrict__ clamped,
+                                                                        uint32_t* __restrict__ depth_keys,
+                                                                        uint32_t* __restrict__ ids, int exact_binning,
+                                                                        DepthBuckets bk,
+                                                                        uint32_t* __restrict__ view_counts) {
+  constexpr bool DEVFOV = true;
+  __shared__ Camera cam;
+  __shared__ float sh_s[PRE_NT * SH_SMEM_STRIDE_MAX];
+  const int view = (int)blockIdx.y;
+  const float* row = cameras + (size_t)view * GAB200_CAMERA_FLOATS;
+  stage_camera_row(row, cam);
+  const float* tanfov = row + 35;
+  const int view_tiles = ((a.image_width + GAB_TILE - 1) / GAB_TILE) * ((a.image_height + GAB_TILE - 1) / GAB_TILE);
+  uint32_t* const tile_count = view_counts != nullptr ? view_counts + view * view_tiles : nullptr;
+#define GAB_PRE_OUT (view * a.P + i)
+#define GAB_PRE_REC_DEPTH
+#include "preprocess_splat.inc"
+#undef GAB_PRE_REC_DEPTH
+#undef GAB_PRE_OUT
+}
+
 void launch_preprocess(const gab200_forward_args& a, SplatRec* rec, SplatAux* aux, uint32_t* tiles_touched,
                        uint8_t* clamped, uint32_t* depth_keys, uint32_t* ids, const DepthBuckets& buckets,
                        uint32_t* tile_count, const float* tanfov, cudaStream_t stream, bool rec_depth) {
@@ -145,9 +175,17 @@ void launch_preprocess(const gab200_forward_args& a, SplatRec* rec, SplatAux* au
 
 void launch_preprocess_views(const gab200_forward_args& a, int views, const float* cameras, SplatRec* rec, SplatAux* aux,
                              uint32_t* tiles_touched, uint32_t* depth_keys, uint32_t* ids, const DepthBuckets& buckets,
-                             uint32_t* tile_count, uint8_t* clamped, cudaStream_t stream) {
+                             uint32_t* tile_count, uint8_t* clamped, cudaStream_t stream, bool rec_depth) {
   const int threads = PRE_NT, blocks = (a.P + threads - 1) / threads;
   if (blocks == 0) return;
+  if (rec_depth) {  // clamped != nullptr only for the training frame (BOUND_RAW, checked by the caller)
+    auto kernel = a.input_mode == GAB200_INPUT_BOUND_RAW ? preprocess_views_depth_kernel<true>
+                                                         : preprocess_views_depth_kernel<false>;
+    kernel<<<dim3(blocks, views), threads, 0, stream>>>(a, cameras, rec, aux, tiles_touched, clamped, depth_keys, ids,
+                                                        a.exact_binning, buckets, tile_count);
+    count_launch();
+    return;
+  }
   if (clamped != nullptr) {  // training frame (BOUND_RAW, checked by the caller)
     preprocess_views_train_kernel<<<dim3(blocks, views), threads, 0, stream>>>(
         a, cameras, rec, aux, tiles_touched, clamped, depth_keys, ids, a.exact_binning, buckets, tile_count);

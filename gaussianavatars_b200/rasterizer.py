@@ -644,7 +644,7 @@ def check_camera_table(cameras, device) -> torch.Tensor:
 def rasterize_bound_views(raster_settings: GaussianRasterizationSettings, cameras: torch.Tensor, _xyz, _rotation,
                           _scaling, _opacity, features_dc, features_rest, binding=None, face_center=None,
                           face_orien_mat=None, face_scaling=None, colors_precomp=None, hints: Optional[FrameHints] = None,
-                          display: bool = True, float_image: bool = False):
+                          display: bool = True, float_image: bool = False, depth_alpha: bool = False):
     """Fused binding + rasterization of K cameras in ONE forward (gab200_forward_views), forward only.
 
     `cameras`: (K, 37) float32 device table, row k = camera_block(cam_k, fov=True); each view uses its own matrices,
@@ -653,7 +653,10 @@ def rasterize_bound_views(raster_settings: GaussianRasterizationSettings, camera
     display (K,H,W,3) uint8 or None, radii (K,P) int32, visibility (K,P) bool), every one bit for bit the K
     single-camera forwards' (rasterize_bound(..., rgb8=...)).  `hints`: the capacity / depth hints of these frames
     (view_hints_of(model)); the model's single-view hints are not touched.  No autograd: an input that requires a
-    gradient while grad mode is on is refused."""
+    gradient while grad mode is on is refused.
+    depth_alpha=True (gab200_forward_views_depth_alpha): also returns alpha and depth, (K,1,H,W) float32 each, the planes
+    of rasterize_bound(..., depth_alpha=True) for every view; the other outputs are those of depth_alpha=False bit for
+    bit."""
     tensors = [t for t in (_xyz, _rotation, _scaling, _opacity, features_dc, features_rest, face_center,
                            face_orien_mat, face_scaling, colors_precomp) if t is not None]
     if torch.is_grad_enabled() and any(t.requires_grad for t in tensors):
@@ -696,6 +699,10 @@ def rasterize_bound_views(raster_settings: GaussianRasterizationSettings, camera
     radii = torch.empty((K, P), dtype=torch.int32, device=device)
     visible = torch.empty((K, P), dtype=torch.bool, device=device)
     a.out_color, a.radii, a.visibility = N.ptr(color), radii.data_ptr(), visible.data_ptr()
+    planes = None
+    if depth_alpha:
+        planes = (torch.empty((K, 1, H, W), dtype=torch.float32, device=device),
+                  torch.empty((K, 1, H, W), dtype=torch.float32, device=device))
     slot = _capture_slot
     cb, holder = N.begin_forward(device, slot is not None)   # captured: the graph owns its scratch (see _run_forward)
     if slot is not None:
@@ -715,8 +722,13 @@ def rasterize_bound_views(raster_settings: GaussianRasterizationSettings, camera
         a.frame_seq = hints.seq
     with torch.cuda.device(device):
         stream = torch.cuda.current_stream(device).cuda_stream
-        n = N.lib().gab200_forward_views(C.byref(a), K, cameras.data_ptr(), N.ptr(rgb8), C.byref(st),
-                                         C.c_void_p(stream))
+        if planes is not None:
+            n = N.lib().gab200_forward_views_depth_alpha(C.byref(a), K, cameras.data_ptr(), planes[0].data_ptr(),
+                                                         planes[1].data_ptr(), N.ptr(rgb8), C.byref(st),
+                                                         C.c_void_p(stream))
+        else:
+            n = N.lib().gab200_forward_views(C.byref(a), K, cameras.data_ptr(), N.ptr(rgb8), C.byref(st),
+                                             C.c_void_p(stream))
     N.check(n, "gab200_forward_views")
     info = dict(num_rendered=int(st.num_rendered), capacity=int(st.binning_capacity), sync_mode=int(a.sync_mode),
                 depth_sort_path=int(st.depth_sort_path), attempts=int(st.attempts), views=K)
@@ -726,6 +738,8 @@ def rasterize_bound_views(raster_settings: GaussianRasterizationSettings, camera
         hints.put(key, n, _widen_depth_range(st.depth_key_min, st.depth_key_max)
                   if st.depth_key_min <= st.depth_key_max else (0, 0))
         hints.last = info
+    if planes is not None:
+        return color, rgb8, radii, visible, planes[0], planes[1]
     return color, rgb8, radii, visible
 
 
@@ -734,7 +748,7 @@ class _RasterizeBoundViews(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, _xyz, means2D, _rotation, _scaling, _opacity, f_dc, f_rest, face_center, face_orien_mat,
-                face_scaling, binding, cameras, raster_settings, grad_sink, hints):
+                face_scaling, binding, cameras, raster_settings, grad_sink, hints, depth_alpha=False):
         rs = raster_settings
         ctx.grad_sink = grad_sink
         device = _xyz.device
@@ -771,6 +785,10 @@ class _RasterizeBoundViews(torch.autograd.Function):
         visible = torch.empty((K, P), dtype=torch.bool, device=device)
         a.out_color, a.radii, a.visibility = color.data_ptr(), radii.data_ptr(), visible.data_ptr()
         _tls.visible = (radii.data_ptr(), visible)
+        planes = None
+        if depth_alpha:
+            planes = (torch.empty((K, 1, H, W), dtype=torch.float32, device=device),
+                      torch.empty((K, 1, H, W), dtype=torch.float32, device=device))
         slot = _capture_slot
         cb, holder = N.begin_forward(device, True)
         a.alloc_geom = a.alloc_binning = a.alloc_image = cb
@@ -787,7 +805,13 @@ class _RasterizeBoundViews(torch.autograd.Function):
             a.frame_seq = hints.seq
         with torch.cuda.device(device):
             stream = torch.cuda.current_stream(device).cuda_stream
-            n = N.lib().gab200_forward_views_train(C.byref(a), K, cameras.data_ptr(), C.byref(st), C.c_void_p(stream))
+            if planes is not None:
+                n = N.lib().gab200_forward_views_train_depth_alpha(C.byref(a), K, cameras.data_ptr(),
+                                                                   planes[0].data_ptr(), planes[1].data_ptr(),
+                                                                   C.byref(st), C.c_void_p(stream))
+            else:
+                n = N.lib().gab200_forward_views_train(C.byref(a), K, cameras.data_ptr(), C.byref(st),
+                                                       C.c_void_p(stream))
         N.check(n, "gab200_forward_views_train")
         info = dict(num_rendered=int(st.num_rendered), capacity=int(st.binning_capacity), sync_mode=int(a.sync_mode),
                     depth_sort_path=int(st.depth_sort_path), attempts=int(st.attempts), views=K)
@@ -804,11 +828,14 @@ class _RasterizeBoundViews(torch.autograd.Function):
         ctx.face_shapes = None if binding is None else (face_center.shape, face_orien_mat.shape, face_scaling.shape)
         ctx.want_face = binding is not None and any(ctx.needs_input_grad[7:10])
         ctx.csr = _face_csr(binding_orig, F)[1] if ctx.want_face else None
+        ctx.depth_alpha = planes is not None
         ctx.mark_non_differentiable(radii)
+        if planes is not None:
+            return color, radii, planes[0], planes[1]
         return color, radii
 
     @staticmethod
-    def backward(ctx, grad_out_color, _grad_radii):
+    def backward(ctx, grad_out_color, _grad_radii, *grad_planes):
         a, st = ctx.args, ctx.state
         K, P, M, F = ctx.dims
         cameras = ctx.keep[1]
@@ -849,19 +876,26 @@ class _RasterizeBoundViews(torch.autograd.Function):
             b.num_face_chunks = c_face.shape[0]
         with torch.cuda.device(device):
             stream = torch.cuda.current_stream(device).cuda_stream
-            N.check(N.lib().gab200_backward_views(C.byref(b), K, cameras.data_ptr(), C.c_void_p(stream)),
-                    "gab200_backward_views")
+            if ctx.depth_alpha:   # gradients of the (K,1,H,W) alpha / depth planes (None: the loss does not read one)
+                ga, gd = (None if t is None else (t if t.is_contiguous() else t.contiguous()) for t in grad_planes)
+                N.check(N.lib().gab200_backward_views_depth_alpha(C.byref(b), K, cameras.data_ptr(), N.ptr(ga),
+                                                                  N.ptr(gd), C.c_void_p(stream)),
+                        "gab200_backward_views_depth_alpha")
+            else:
+                N.check(N.lib().gab200_backward_views(C.byref(b), K, cameras.data_ptr(), C.c_void_p(stream)),
+                        "gab200_backward_views")
         ctx.holder = None
         if ctx.grad_sink is not None:  # dist.py all-reduces this buffer, as after a single-view backward
             ctx.grad_sink.flat_grad = flat
             ctx.grad_sink._gab200_mc_used = bool(use_symm)
-        return (d_xyz, d_means2D, d_rot, d_scale, d_opac, d_dc, d_rest, d_fc, d_fR, d_fs, None, None, None, None, None)
+        return (d_xyz, d_means2D, d_rot, d_scale, d_opac, d_dc, d_rest, d_fc, d_fR, d_fs, None, None, None, None, None,
+                None)
 
 
 def rasterize_bound_views_train(raster_settings: GaussianRasterizationSettings, cameras: torch.Tensor, _xyz, _rotation,
                                 _scaling, _opacity, features_dc, features_rest, binding=None, face_center=None,
                                 face_orien_mat=None, face_scaling=None, means2D=None, colors_precomp=None,
-                                grad_sink=None, hints: Optional[FrameHints] = None):
+                                grad_sink=None, hints: Optional[FrameHints] = None, depth_alpha: bool = False):
     """Fused binding + rasterization of the K cameras of one timestep as ONE training frame, differentiable.
 
     `cameras` and `raster_settings` as in rasterize_bound_views.  Returns (color (K,3,H,W), radii (K,P) int32); images
@@ -870,7 +904,11 @@ def rasterize_bound_views_train(raster_settings: GaussianRasterizationSettings, 
     `grad_sink.flat_grad`) and the face frame.  `means2D` is a (K,P,3) holder whose .grad row k receives camera k's
     dL/dmean2D.  `hints`: the capacity / depth hints of these frames (default: view_hints_of(grad_sink)).  The kernels
     exist for SH colours and plain stores only: colors_precomp, and a grad_sink whose symmetric gradient buffer is in
-    "push" (multicast) mode, are refused."""
+    "push" (multicast) mode, are refused.
+    depth_alpha=True (gab200_forward_views_train_depth_alpha / gab200_backward_views_depth_alpha): returns (color,
+    radii, alpha (K,1,H,W), depth (K,1,H,W)), each view's planes those of rasterize_bound(..., depth_alpha=True),
+    differentiable in all three images; the backward writes the sum over the views of the single-camera gradients of
+    the whole loss (a mask or depth term included)."""
     if colors_precomp is not None:
         raise ValueError("rasterize_bound_views_train takes SH colours only (no colors_precomp)")
     symm = getattr(grad_sink, "symm_grad", None) if grad_sink is not None else None
@@ -892,7 +930,7 @@ def rasterize_bound_views_train(raster_settings: GaussianRasterizationSettings, 
         hints = view_hints_of(grad_sink) if grad_sink is not None else FrameHints()
     return _RasterizeBoundViews.apply(_xyz, means2D, _rotation, _scaling, _opacity, features_dc, features_rest,
                                       face_center, face_orien_mat, face_scaling, binding, cameras, raster_settings,
-                                      grad_sink, hints)
+                                      grad_sink, hints, bool(depth_alpha))
 
 
 def bind_activate(raster_settings_or_modifier, _xyz, _rotation, _scaling, _opacity, binding=None, face_center=None,

@@ -16,7 +16,8 @@ instead of FoVx / FoVy; the reference route cannot and refuses such a camera.
 `render_views(cameras, ...)` renders every camera of a rig (one image size) in one forward, forward only;
 `render_views_train(cameras, ...)` is its differentiable form, for a training step over every camera of a timestep.
 `depth_alpha=True` (render, render_bound, render_display; fused route only) adds "alpha" (1,H,W), the accumulated
-opacity 1 - T_final, and "depth" (1,H,W), the alpha-weighted view-space depth, both from the colour blend itself.
+opacity 1 - T_final, and "depth" (1,H,W), the alpha-weighted view-space depth, both from the colour blend itself;
+on render_views and render_views_train it adds them for every camera, (K,1,H,W).
 """
 from __future__ import annotations
 
@@ -131,14 +132,16 @@ def camera_table(cameras, device) -> torch.Tensor:
     return torch.stack(rows).contiguous()
 
 
-def render_views(cameras, pc, pipe, bg_color, scaling_modifier=1.0, float_image=False, width=None, height=None):
+def render_views(cameras, pc, pipe, bg_color, scaling_modifier=1.0, float_image=False, width=None, height=None,
+                 depth_alpha=False):
     """Every camera of a rig in ONE forward (gab200_forward_views): the fused route, forward only, no autograd.
     `cameras`: a list of camera objects of one image size (each with its own matrices and field of view), or a
     (K, 37) float32 device table of camera_block(cam, fov=True) rows together with `width` and `height`.  Returns
     {"display_u8": (K,H,W,3) uint8, "render": (K,3,H,W) float32 or None (float_image=False), "radii": (K,P) int32,
-    "visibility_filter": (K,P) bool}; view k equals render_display(cameras[k], ...) bit for bit."""
+    "visibility_filter": (K,P) bool}; view k equals render_display(cameras[k], ...) bit for bit.  depth_alpha=True adds
+    "alpha" and "depth", (K,1,H,W) float32, view k's those of render_display(cameras[k], ..., depth_alpha=True)."""
     table, W, H = _views_table(cameras, pc, width, height, "render_views")
-    return _views_forward(table, W, H, pc, pipe, bg_color, scaling_modifier, True, float_image)
+    return _views_forward(table, W, H, pc, pipe, bg_color, scaling_modifier, True, float_image, depth_alpha)
 
 
 def _views_table(cameras, pc, width, height, what):
@@ -177,36 +180,47 @@ def _face_frame_of(pc):
     return binding, (pc.face_center, pc.face_orien_mat, pc.face_scaling)
 
 
-def render_views_train(cameras, pc, pipe, bg_color, scaling_modifier=1.0, width=None, height=None):
+def render_views_train(cameras, pc, pipe, bg_color, scaling_modifier=1.0, width=None, height=None, depth_alpha=False):
     """The training form of render_views: every camera of one timestep (the model's current face frame) in ONE
     differentiable forward (gab200_forward_views_train).  Returns render()'s dict with a leading K:
     {"render": (K,3,H,W), "viewspace_points": (K,P,3) holder whose .grad row k is camera k's dL/dmean2D,
     "visibility_filter": (K,P) bool, "radii": (K,P) int32}; view k's image and radii equal render(cameras[k], ...)
     bit for bit.  A loss summed over the views backpropagates, in one backward, the sum of the K single-view
-    gradients into the model's parameters and face frame."""
+    gradients into the model's parameters and face frame.  depth_alpha=True adds the differentiable "alpha" and "depth"
+    planes, (K,1,H,W), view k's those of render(cameras[k], ..., depth_alpha=True): a mask or depth term of every view
+    joins the same loss and the same backward."""
     table, W, H = _views_table(cameras, pc, width, height, "render_views_train")
     rs = _views_settings(W, H, pc, pipe, bg_color, scaling_modifier)
     binding, (fc, fR, fs) = _face_frame_of(pc)
     K, P = int(table.shape[0]), int(pc._xyz.shape[0])
     screenspace_points = torch.zeros((K, P, 3), dtype=pc._xyz.dtype, device=pc._xyz.device, requires_grad=True)
-    image, radii = rasterize_bound_views_train(rs, table, pc._xyz, pc._rotation, pc._scaling, pc._opacity,
-                                               pc._features_dc, pc._features_rest, binding, fc, fR, fs,
-                                               means2D=screenspace_points, grad_sink=pc)
-    return {"render": image, "viewspace_points": screenspace_points, "visibility_filter": _visible(radii),
-            "radii": radii}
+    out = rasterize_bound_views_train(rs, table, pc._xyz, pc._rotation, pc._scaling, pc._opacity, pc._features_dc,
+                                      pc._features_rest, binding, fc, fR, fs, means2D=screenspace_points, grad_sink=pc,
+                                      depth_alpha=depth_alpha)
+    image, radii = out[0], out[1]
+    res = {"render": image, "viewspace_points": screenspace_points, "visibility_filter": _visible(radii),
+           "radii": radii}
+    if depth_alpha:
+        res["alpha"], res["depth"] = out[2], out[3]
+    return res
 
 
-def _views_forward(table, W, H, pc, pipe, bg_color, scaling_modifier, display: bool, float_image: bool):
+def _views_forward(table, W, H, pc, pipe, bg_color, scaling_modifier, display: bool, float_image: bool,
+                   depth_alpha: bool = False):
     """The fused route's K-view forward of a (K, 37) device camera table (render_views, GraphedRender)."""
     d = lambda t: None if t is None else t.detach()  # noqa: E731
     with torch.no_grad():
         rs = _views_settings(W, H, pc, pipe, bg_color, scaling_modifier)
         binding, (fc, fR, fs) = _face_frame_of(pc)
-        img, rgb8, radii, visible = rasterize_bound_views(
+        out = rasterize_bound_views(
             rs, table, d(pc._xyz), d(pc._rotation), d(pc._scaling), d(pc._opacity), d(pc._features_dc),
             d(pc._features_rest), binding, d(fc), d(fR), d(fs), hints=view_hints_of(pc), display=display,
-            float_image=float_image)
-    return {"display_u8": rgb8, "render": img, "radii": radii, "visibility_filter": visible}
+            float_image=float_image, depth_alpha=depth_alpha)
+    img, rgb8, radii, visible = out[:4]
+    res = {"display_u8": rgb8, "render": img, "radii": radii, "visibility_filter": visible}
+    if depth_alpha:
+        res["alpha"], res["depth"] = out[4], out[5]
+    return res
 
 
 def _visible(radii):

@@ -175,8 +175,9 @@ typedef struct gab200_frame_state {
   int32_t sort_bits;          /* key width of the per-instance (stage B) radix sort: bits(tile id) */
   int32_t depth_bits;         /* key width of the per-splat (stage A) radix sort: 32 (the fp32 depth pattern); the two
                                  stable stages together are the reference's LSD sort of (tile << 32 | depth) */
-  uint32_t depth_prefix;      /* 1: a gab200_forward_depth_alpha frame kept for a backward -- its records carry the
-                                 view-space depth that gab200_backward_depth_alpha reads; 0 for every other forward */
+  uint32_t depth_prefix;      /* 1: a gab200_forward_depth_alpha or gab200_forward_views_train_depth_alpha frame kept for
+                                 a backward -- its records carry the view-space depth that gab200_backward_depth_alpha /
+                                 gab200_backward_views_depth_alpha read; 0 for every other forward */
   int64_t binning_capacity;   /* instances the binning buffer was carved for (>= num_rendered; = binning_hint when the
                                  speculative allocation was large enough) */
   uint32_t depth_key_min;     /* smallest / largest depth key among the splats that emitted instances (min > max: none) */
@@ -351,6 +352,34 @@ int64_t gab200_forward_views_train(const gab200_forward_args* args, int32_t view
  * dL_dsh_rest (sh_coeffs > 1), and scratch buffers that are not the forward's.  gab200_backward and
  * gab200_backward_device_fov refuse a multi-view state. */
 int32_t gab200_backward_views(const gab200_backward_args* args, int32_t views, const float* cameras, void* stream);
+
+/* Opacity and depth for every camera of a K-view frame: the planes of gab200_forward_depth_alpha (same definitions, same
+ * walk) for each view of gab200_forward_views / gab200_forward_views_train, and their gradients.
+ * gab200_forward_views_depth_alpha is gab200_forward_views plus out_alpha and out_depth, DEVICE float [views,H,W] each
+ * (view k's plane at offset k * H * W); either may be NULL, not both.  Every output is bit for bit that of `views` calls
+ * of gab200_forward_depth_alpha with the same cameras (planes included), and colour, bytes, radii and visibility are
+ * those of gab200_forward_views.  Before any device work, GAB200_ERR_INVALID_ARGUMENT for every error of
+ * gab200_forward_views and for both planes NULL.
+ * gab200_forward_views_train_depth_alpha is gab200_forward_views_train plus the two planes, as above.  The state records
+ * K in state_out->reserved0 and sets state_out->depth_prefix = 1 (the records carry z).  Before any device work,
+ * GAB200_ERR_INVALID_ARGUMENT for every error of gab200_forward_views_train and for both planes NULL.
+ * Both forwards: every sync mode, binning_hint, the counters, the sticky overflow_flag and the LATE re-enqueue (which
+ * rewrites both planes with the EXACT frame's values) behave as in gab200_forward_views.
+ * gab200_backward_views_depth_alpha is gab200_backward_views plus dL_dalpha and dL_ddepth, DEVICE float [views,H,W]
+ * each or NULL (= zero).  Every output is what the sum over k of gab200_backward_depth_alpha of camera k's single-view
+ * frame would hold (float sums in another order): each view's dL/dz reaches the mean through that view's own view
+ * matrix before the sums over the views.  Before any device work, GAB200_ERR_INVALID_ARGUMENT for every error of
+ * gab200_backward_views and for a state whose depth_prefix != 1 (a plain K-view frame's).  gab200_backward_views on a
+ * K-view depth-alpha state is valid: the colour backward, both plane gradients zero.  gab200_backward_depth_alpha
+ * refuses a K-view state. */
+int64_t gab200_forward_views_depth_alpha(const gab200_forward_args* args, int32_t views, const float* cameras,
+                                         float* out_alpha, float* out_depth, uint8_t* out_rgb8,
+                                         gab200_frame_state* state_out, void* stream);
+int64_t gab200_forward_views_train_depth_alpha(const gab200_forward_args* args, int32_t views, const float* cameras,
+                                               float* out_alpha, float* out_depth, gab200_frame_state* state_out,
+                                               void* stream);
+int32_t gab200_backward_views_depth_alpha(const gab200_backward_args* args, int32_t views, const float* cameras,
+                                          const float* dL_dalpha, const float* dL_ddepth, void* stream);
 
 /* Frustum test only.  Replaces diff_gaussian_rasterization._C.mark_visible (GaussianRasterizer.markVisible). */
 int32_t gab200_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,
