@@ -209,6 +209,29 @@ struct PinnedSlot {
 };
 static thread_local PinnedSlot t_slot;
 
+// GAB200_SYNC_NONE: nothing on the host waits for the counters inside the frame, so their copy runs on a branch forked
+// from the frame's stream after the depth sort and joined at the end of the forward.  On the frame's own stream the
+// copy would sit between the depth sort and the key emission, with a copy-engine hand-over on either side of it.
+// One branch stream per device and host thread.
+struct CounterBranch {
+  cudaStream_t side = nullptr;
+  cudaEvent_t fork = nullptr, join = nullptr;
+  bool ok() {
+    if (side == nullptr) {
+      if (cudaStreamCreateWithFlags(&side, cudaStreamNonBlocking) != cudaSuccess) return false;
+      if (cudaEventCreateWithFlags(&fork, cudaEventDisableTiming) != cudaSuccess) return false;
+      if (cudaEventCreateWithFlags(&join, cudaEventDisableTiming) != cudaSuccess) return false;
+    }
+    return true;
+  }
+};
+static thread_local CounterBranch t_branch[64];
+static CounterBranch* counter_branch() {
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return nullptr;
+  return t_branch[dev].ok() ? &t_branch[dev] : nullptr;
+}
+
 static int check_arch() {
   constexpr int MAX_DEV = 64;
   static std::atomic<int> cached[MAX_DEV];  // per device: 0 unknown, 1 ok, -1 bad
@@ -356,6 +379,7 @@ struct Frame {
   bool nb, dbg;
   uint32_t* ctr_host;   // where the counters land on the host
   cudaEvent_t ctr_event;
+  CounterBranch* branch = nullptr;  // GAB200_SYNC_NONE: the counters' copy is forked onto this branch
   int selA = 0;                           // which half of the stage-A double buffer holds the depth order
   const uint32_t* order_count = nullptr;  // device count of listed splats (bucket path), else all P are listed
   bool counting = true;                   // tile sort: counting sort + per-tile rank sort (tile_sort.cu), else cub radix
@@ -423,20 +447,29 @@ int enqueue_geometry(Frame& f, bool bucket, bool run_preprocess, uint32_t capaci
                               a->sync_mode == GAB200_SYNC_NONE ? a->overflow_flag : nullptr, stream);
   }
   GAB_STAGE_CHECK(f.dbg, stream);
-  GAB_CUDA(cudaMemcpyAsync(f.ctr_host, g.buckets.meta, sizeof(uint32_t) * GAB200_NUM_COUNTERS, cudaMemcpyDeviceToHost,
-                           stream));
+  if (f.branch != nullptr) {
+    GAB_CUDA(cudaEventRecord(f.branch->fork, stream));
+    GAB_CUDA(cudaStreamWaitEvent(f.branch->side, f.branch->fork, 0));
+    GAB_CUDA(cudaMemcpyAsync(f.ctr_host, g.buckets.meta, sizeof(uint32_t) * GAB200_NUM_COUNTERS,
+                             cudaMemcpyDeviceToHost, f.branch->side));
+    GAB_CUDA(cudaEventRecord(f.branch->join, f.branch->side));
+  } else {
+    GAB_CUDA(cudaMemcpyAsync(f.ctr_host, g.buckets.meta, sizeof(uint32_t) * GAB200_NUM_COUNTERS,
+                             cudaMemcpyDeviceToHost, stream));
+  }
   if (f.ctr_event) GAB_CUDA(cudaEventRecord(f.ctr_event, stream));
   return GAB200_OK;
 }
 
 // key emission of the frame's (virtual) splats in depth order
-void emit(const Frame& f, const uint32_t* offsets, uint32_t cap, uint32_t* cursor, const BinView& bv) {
+void emit(const Frame& f, const uint32_t* offsets, uint32_t cap, uint32_t* cursor, const BinView& bv,
+          const EmitClears& clr) {
   if (f.cameras != nullptr)
     launch_emit_keys_views(f.P, f.gx, f.gy, f.g.rec, f.g.aux, f.g.ids[f.selA], offsets, f.order_count, f.g.buckets.meta,
-                           cap, cursor, bv.keys[0], bv.vals[0], f.a->exact_binning, f.a->P, f.stream);
+                           cap, cursor, bv.keys[0], bv.vals[0], f.a->exact_binning, f.a->P, clr, f.stream);
   else
     launch_emit_keys(f.P, f.gx, f.gy, f.g.rec, f.g.aux, f.g.ids[f.selA], offsets, f.order_count, f.g.buckets.meta, cap,
-                     cursor, bv.keys[0], bv.vals[0], f.a->exact_binning, f.stream);
+                     cursor, bv.keys[0], bv.vals[0], f.a->exact_binning, clr, f.stream);
 }
 
 // emit -> per-instance tile sort -> ranges -> tile order -> blend, for a binning buffer of `cap` instances.
@@ -454,7 +487,10 @@ int enqueue_binning_blend(Frame& f, void* bin, int64_t cap, int64_t n_known, siz
   const int64_t n_sort = n_known >= 0 ? n_known : cap;
   const bool counting = f.counting && f.P > 0;
   st->tile_sort_path = counting ? 1 : 0;
-  if (bv.strip_mask != nullptr && n_sort > 0) GAB_CUDA(cudaMemsetAsync(bv.strip_mask, 0, (size_t)n_sort, stream));
+  // the emission grid clears the block masks (and, for the radix sort, the ranges and the padding keys) before it emits
+  EmitClears clr;
+  clr.mask = n_sort > 0 ? bv.strip_mask : nullptr;
+  clr.n_mask = (uint32_t)n_sort;
   int selector = 0;
   if (counting) {
     if (redo) {  // the cursors were consumed (and the ranges possibly cut at a smaller capacity) by the first attempt
@@ -467,7 +503,7 @@ int enqueue_binning_blend(Frame& f, void* bin, int64_t cap, int64_t n_known, siz
     if (n_sort > 0) {
       {
         StageScope sc(GAB200_STAGE_EMIT_KEYS, stream);
-        emit(f, nullptr, (uint32_t)cap, f.iv.tile_cursor, bv);
+        emit(f, nullptr, (uint32_t)cap, f.iv.tile_cursor, bv, clr);
       }
       GAB_STAGE_CHECK(f.dbg, stream);
       {
@@ -478,12 +514,14 @@ int enqueue_binning_blend(Frame& f, void* bin, int64_t cap, int64_t n_known, siz
       GAB_STAGE_CHECK(f.dbg, stream);
     }
   } else {
-    GAB_CUDA(cudaMemsetAsync(f.iv.ranges, 0, sizeof(uint2) * ((size_t)tiles + 1), stream));
+    if (n_sort == 0) GAB_CUDA(cudaMemsetAsync(f.iv.ranges, 0, sizeof(uint2) * ((size_t)tiles + 1), stream));
     if (n_sort > 0) {
-      if (n_known < 0) GAB_CUDA(cudaMemsetAsync(bv.keys[0], 0xff, sizeof(uint32_t) * (size_t)cap, stream));
+      clr.ranges = f.iv.ranges;
+      clr.n_ranges = (uint32_t)tiles + 1;
+      clr.sentinel = n_known < 0;
       {
         StageScope sc(GAB200_STAGE_EMIT_KEYS, stream);
-        emit(f, f.g.offsets, (uint32_t)cap, nullptr, bv);
+        emit(f, f.g.offsets, (uint32_t)cap, nullptr, bv, clr);
       }
       GAB_STAGE_CHECK(f.dbg, stream);
       {
@@ -611,6 +649,9 @@ static int64_t run_forward(const gab200_forward_args* a, const float* tanfov, ui
     if (!t_slot.ok()) return GAB200_ERR_CUDA;
     f.ctr_event = t_slot.ev;
     if (f.ctr_host == nullptr) f.ctr_host = t_slot.host;
+  } else {
+    f.branch = counter_branch();
+    if (f.branch == nullptr) return GAB200_ERR_CUDA;
   }
   bool bucket = a->depth_hint_hi > a->depth_hint_lo && tune_get(GAB200_TUNE_DEPTH_SORT) == 0;
   int64_t cap = speculative ? (int64_t)a->binning_hint : 0;
@@ -641,6 +682,7 @@ static int64_t run_forward(const gab200_forward_args* a, const float* tanfov, ui
   }
   st->depth_sort_path = bucket ? 1 : 0;
   if (mode == GAB200_SYNC_NONE) {
+    GAB_CUDA(cudaStreamWaitEvent(stream, f.branch->join, 0));  // the counters' copy rejoins the frame's stream
     st->num_rendered = st->num_candidates = -1;
     g_host_ns[5].fetch_add(1, std::memory_order_relaxed);
     return 0;
@@ -799,8 +841,13 @@ static int32_t run_backward_views(const gab200_backward_args* b, int32_t views, 
     ~CaptureGuard() { t_capturing = prev; }
   } capture_guard(cap_status != cudaStreamCaptureStatusNone);
 
+  // csr: the per-splat kernel writes per-splat face gradients and clears the face gradients that face_grad_reduce
+  // then adds them into; otherwise it adds into them itself, cleared here
+  const bool csr = v.binding != nullptr && b->num_face_chunks > 0 && b->face_perm && b->face_chunk_face &&
+                   b->face_chunk_start && b->face_chunk_end &&
+                   (b->dL_dface_center || b->dL_dface_orien_mat || b->dL_dface_scaling);
   GAB_CUDA(cudaMemsetAsync(g.g2d, 0, sizeof(float) * (size_t)views * P * GAB_G2D_STRIDE, stream));
-  if (v.binding != nullptr) {
+  if (v.binding != nullptr && !csr) {
     const size_t F = (size_t)v.num_faces;
     if (b->dL_dface_center) GAB_CUDA(cudaMemsetAsync(b->dL_dface_center, 0, sizeof(float) * 3 * F, stream));
     if (b->dL_dface_orien_mat) GAB_CUDA(cudaMemsetAsync(b->dL_dface_orien_mat, 0, sizeof(float) * 9 * F, stream));
@@ -819,9 +866,6 @@ static int32_t run_backward_views(const gab200_backward_args* b, int32_t views, 
   GAB_STAGE_CHECK(dbg, stream);
   {
     StageScope sc(GAB200_STAGE_PREPROCESS_BWD, stream);
-    const bool csr = v.binding != nullptr && b->num_face_chunks > 0 && b->face_perm && b->face_chunk_face &&
-                     b->face_chunk_start && b->face_chunk_end &&
-                     (b->dL_dface_center || b->dL_dface_orien_mat || b->dL_dface_scaling);
     gab200_backward_args bb = *b;
     bb.fwd = &v;
     launch_preprocess_backward_views(bb, views, cameras, g.aux, g.clamped, g.g2d, csr ? g.face_scratch : nullptr,
@@ -873,8 +917,12 @@ static int32_t run_backward(const gab200_backward_args* b, const float* tanfov, 
   if (g.bytes > st->geom_bytes || iv.bytes > st->image_bytes || bv.bytes > st->binning_bytes)
     return GAB200_ERR_INVALID_ARGUMENT;  // not the buffers this forward carved
 
+  // csr: as in run_backward_views, the per-splat kernel clears the face gradients face_grad_reduce adds into
+  const bool csr = bound && a->binding != nullptr && b->num_face_chunks > 0 && b->face_perm && b->face_chunk_face &&
+                   b->face_chunk_start && b->face_chunk_end &&
+                   (b->dL_dface_center || b->dL_dface_orien_mat || b->dL_dface_scaling);
   GAB_CUDA(cudaMemsetAsync(g.g2d, 0, sizeof(float) * (size_t)P * GAB_G2D_STRIDE, stream));
-  if (bound && a->binding != nullptr) {
+  if (bound && a->binding != nullptr && !csr) {
     const size_t F = (size_t)a->num_faces;
     if (b->dL_dface_center) GAB_CUDA(cudaMemsetAsync(b->dL_dface_center, 0, sizeof(float) * 3 * F, stream));
     if (b->dL_dface_orien_mat) GAB_CUDA(cudaMemsetAsync(b->dL_dface_orien_mat, 0, sizeof(float) * 9 * F, stream));
@@ -899,9 +947,6 @@ static int32_t run_backward(const gab200_backward_args* b, const float* tanfov, 
   GAB_STAGE_CHECK(dbg, stream);
   {
     StageScope sc(GAB200_STAGE_PREPROCESS_BWD, stream);
-    const bool csr = bound && a->binding != nullptr && b->num_face_chunks > 0 && b->face_perm && b->face_chunk_face &&
-                     b->face_chunk_start && b->face_chunk_end &&
-                     (b->dL_dface_center || b->dL_dface_orien_mat || b->dL_dface_scaling);
     launch_preprocess_backward(*b, g.rec, g.aux, g.clamped, g.g2d, csr ? g.face_scratch : nullptr, tanfov, stream, da);
   }
   GAB_STAGE_CHECK(dbg, stream);

@@ -359,6 +359,8 @@ __global__ void __launch_bounds__(256) blend_forward_kernel(int W, int H, int gx
   __shared__ __align__(8) uint64_t mbar[4][ID_RING];
   constexpr int GH = KH;  // heavy tiles per CTA (256/KH threads each)
   constexpr int NTH = 256 / KH;
+  pdl_wait();
+  pdl_trigger();
   const int nh = (int)order_info[0];
   const int heavy_ctas = (nh + GH - 1) / GH;
   const int b = blockIdx.x, t = threadIdx.x;
@@ -389,9 +391,8 @@ void launch_blend_forward(int W, int H, const uint2* ranges, const uint32_t* ord
   auto kernel = out_rgb8 == nullptr ? blend_forward_kernel<1, BLEND_OUT_FLOAT>
                 : out_color == nullptr ? blend_forward_kernel<1, BLEND_OUT_U8>
                                        : blend_forward_kernel<1, BLEND_OUT_FLOAT | BLEND_OUT_U8>;
-  kernel<<<grid, 256, 0, stream>>>(W, H, gx, tiles, ranges, order, order_info, point_list, rec, bg, out_color, final_T,
-                                   n_contrib, strip_mask, out_rgb8);
-  count_launch();
+  launch_pdl(kernel, grid, 256, 0, stream, W, H, gx, tiles, ranges, order, order_info, point_list, rec, bg, out_color,
+             final_T, n_contrib, strip_mask, out_rgb8);
 }
 
 // gab200_forward_depth_alpha: blend_forward_kernel<1, OUT> with the alpha and depth planes (forward_tile<.., DA>).  The
@@ -415,6 +416,8 @@ __global__ void __launch_bounds__(256, GAB_FWD_DEPTH_CTAS) blend_forward_depth_k
   __shared__ uint32_t smask[256];
   __shared__ __align__(16) uint32_t ids_ring[4][ID_RING * (64 + 4)];
   __shared__ __align__(8) uint64_t mbar[4][ID_RING];
+  pdl_wait();
+  pdl_trigger();
   const int nh = (int)order_info[0];
   const int b = blockIdx.x, t = threadIdx.x;
   if (b < nh) {
@@ -440,9 +443,8 @@ void launch_blend_forward_depth(int W, int H, const uint2* ranges, const uint32_
   auto kernel = out_rgb8 == nullptr ? blend_forward_depth_kernel<BLEND_OUT_FLOAT>
                 : out_color == nullptr ? blend_forward_depth_kernel<BLEND_OUT_U8>
                                        : blend_forward_depth_kernel<BLEND_OUT_FLOAT | BLEND_OUT_U8>;
-  kernel<<<tiles, 256, 0, stream>>>(W, H, gx, tiles, ranges, order, order_info, point_list, rec, bg, out_color, final_T,
-                                    n_contrib, strip_mask, out_rgb8, out_alpha, out_depth);
-  count_launch();
+  launch_pdl(kernel, tiles, 256, 0, stream, W, H, gx, tiles, ranges, order, order_info, point_list, rec, bg, out_color,
+             final_T, n_contrib, strip_mask, out_rgb8, out_alpha, out_depth);
 }
 
 // gab200_forward_views: the tiles of K views as one list of K * view_tiles global tiles, scheduled heaviest-first
@@ -463,6 +465,8 @@ __global__ void __launch_bounds__(256) blend_forward_views_kernel(int W, int H, 
   __shared__ uint32_t smask[256];
   __shared__ __align__(16) uint32_t ids_ring[4][ID_RING * (64 + 4)];
   __shared__ __align__(8) uint64_t mbar[4][ID_RING];
+  pdl_wait();
+  pdl_trigger();
   const int nh = (int)order_info[0];
   const int b = blockIdx.x, t = threadIdx.x;
   const bool heavy = b < nh;  // one heavy tile on all 256 threads, else four light tiles on 64 threads each
@@ -493,9 +497,8 @@ void launch_blend_forward_views(int views, int W, int H, const uint2* ranges, co
   auto kernel = out_rgb8 == nullptr ? blend_forward_views_kernel<BLEND_OUT_FLOAT>
                 : out_color == nullptr ? blend_forward_views_kernel<BLEND_OUT_U8>
                                        : blend_forward_views_kernel<BLEND_OUT_FLOAT | BLEND_OUT_U8>;
-  kernel<<<tiles, 256, 0, stream>>>(W, H, gx, tiles, view_tiles, ranges, order, order_info, point_list, rec, bg,
-                                    out_color, out_rgb8);
-  count_launch();
+  launch_pdl(kernel, tiles, 256, 0, stream, W, H, gx, tiles, view_tiles, ranges, order, order_info, point_list, rec, bg,
+             out_color, out_rgb8);
 }
 
 // gab200_forward_views_train: blend_forward_views_kernel with the float image only, keeping what the backward reads --
@@ -516,6 +519,8 @@ __global__ void __launch_bounds__(256) blend_forward_views_train_kernel(int W, i
   __shared__ uint32_t smask[256];
   __shared__ __align__(16) uint32_t ids_ring[4][ID_RING * (64 + 4)];
   __shared__ __align__(8) uint64_t mbar[4][ID_RING];
+  pdl_wait();
+  pdl_trigger();
   const int nh = (int)order_info[0];
   const int b = blockIdx.x, t = threadIdx.x;
   const bool heavy = b < nh;
@@ -545,10 +550,8 @@ void launch_blend_forward_views_train(int views, int W, int H, const uint2* rang
   const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
   const int view_tiles = gx * gy, tiles = views * view_tiles;
   if (tiles == 0) return;
-  blend_forward_views_train_kernel<<<tiles, 256, 0, stream>>>(W, H, gx, tiles, view_tiles, ranges, order, order_info,
-                                                              point_list, rec, bg, out_color, final_T, n_contrib,
-                                                              strip_mask);
-  count_launch();
+  launch_pdl(blend_forward_views_train_kernel, tiles, 256, 0, stream, W, H, gx, tiles, view_tiles, ranges, order,
+             order_info, point_list, rec, bg, out_color, final_T, n_contrib, strip_mask);
 }
 
 // gab200_forward_views_depth_alpha and gab200_forward_views_train_depth_alpha: blend_forward_views_kernel with the alpha
@@ -566,6 +569,8 @@ __global__ void __launch_bounds__(256, GAB_FWD_DEPTH_CTAS) blend_forward_views_d
   __shared__ uint32_t smask[256];
   __shared__ __align__(16) uint32_t ids_ring[4][ID_RING * (64 + 4)];
   __shared__ __align__(8) uint64_t mbar[4][ID_RING];
+  pdl_wait();
+  pdl_trigger();
   const int nh = (int)order_info[0];
   const int b = blockIdx.x, t = threadIdx.x;
   const bool heavy = b < nh;
@@ -602,9 +607,8 @@ void launch_blend_forward_views_depth(int views, int W, int H, const uint2* rang
   auto kernel = out_rgb8 == nullptr ? blend_forward_views_depth_kernel<BLEND_OUT_FLOAT>
                 : out_color == nullptr ? blend_forward_views_depth_kernel<BLEND_OUT_U8>
                                        : blend_forward_views_depth_kernel<BLEND_OUT_FLOAT | BLEND_OUT_U8>;
-  kernel<<<tiles, 256, 0, stream>>>(W, H, gx, tiles, view_tiles, ranges, order, order_info, point_list, rec, bg,
-                                    out_color, final_T, n_contrib, strip_mask, out_rgb8, out_alpha, out_depth);
-  count_launch();
+  launch_pdl(kernel, tiles, 256, 0, stream, W, H, gx, tiles, view_tiles, ranges, order, order_info, point_list, rec, bg,
+             out_color, final_T, n_contrib, strip_mask, out_rgb8, out_alpha, out_depth);
 }
 
 // =====================================================================================================
@@ -929,6 +933,8 @@ __global__ void __launch_bounds__(128, 5) blend_backward_kernel(int W, int H, in
                                                                 const uint8_t* __restrict__ strip_mask,
                                                                 float* __restrict__ g2d) {
   __shared__ WarpSmem sm[4];
+  pdl_wait();
+  pdl_trigger();
   const int nh = (int)order_info[1];
   const int b = blockIdx.x, t = threadIdx.x, w = t >> 5;
   if (b < nh) {  // heavy tile: four warps, two bands each
@@ -949,9 +955,8 @@ void launch_blend_backward(int W, int H, const uint2* ranges, const uint32_t* or
   const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
   const int tiles = gx * gy;
   if (tiles == 0) return;
-  blend_backward_kernel<<<tiles, 128, 0, stream>>>(W, H, gx, tiles, ranges, order, order_info, point_list, rec, bg,
-                                                   final_T, n_contrib, dL_dpix, strip_mask, g2d);
-  count_launch();
+  launch_pdl(blend_backward_kernel, tiles, 128, 0, stream, W, H, gx, tiles, ranges, order, order_info, point_list, rec,
+             bg, final_T, n_contrib, dL_dpix, strip_mask, g2d);
 }
 
 // gab200_backward_depth_alpha: blend_backward_kernel with the alpha and depth plane gradients (backward_task<K, true>).
@@ -963,6 +968,8 @@ __global__ void __launch_bounds__(128, GAB_BWD_DEPTH_CTAS) blend_backward_depth_
     const float* __restrict__ dL_dpix, const uint8_t* __restrict__ strip_mask, float* __restrict__ g2d,
     const float* __restrict__ dL_dalpha, const float* __restrict__ dL_ddepth) {
   __shared__ WarpSmemT<10> sm[4];
+  pdl_wait();
+  pdl_trigger();
   const int nh = (int)order_info[1];
   const int b = blockIdx.x, t = threadIdx.x, w = t >> 5;
   if (b < nh) {
@@ -983,10 +990,8 @@ void launch_blend_backward_depth(int W, int H, const uint2* ranges, const uint32
   const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
   const int tiles = gx * gy;
   if (tiles == 0) return;
-  blend_backward_depth_kernel<<<tiles, 128, 0, stream>>>(W, H, gx, tiles, ranges, order, order_info, point_list, rec,
-                                                         bg, final_T, n_contrib, dL_dpix, strip_mask, g2d, dL_dalpha,
-                                                         dL_ddepth);
-  count_launch();
+  launch_pdl(blend_backward_depth_kernel, tiles, 128, 0, stream, W, H, gx, tiles, ranges, order, order_info, point_list,
+             rec, bg, final_T, n_contrib, dL_dpix, strip_mask, g2d, dL_dalpha, dL_ddepth);
 }
 
 // gab200_backward_views: blend_backward_kernel over the K * view_tiles global tiles of a multi-view frame.  Global tile
@@ -1006,6 +1011,8 @@ __global__ void __launch_bounds__(128, 5) blend_backward_views_kernel(int W, int
                                                                       const uint8_t* __restrict__ strip_mask,
                                                                       float* __restrict__ g2d) {
   __shared__ WarpSmem sm[4];
+  pdl_wait();
+  pdl_trigger();
   const int nh = (int)order_info[1];
   const int b = blockIdx.x, t = threadIdx.x, w = t >> 5;
   const bool heavy = b < nh;
@@ -1031,10 +1038,8 @@ void launch_blend_backward_views(int views, int W, int H, const uint2* ranges, c
   const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
   const int view_tiles = gx * gy, tiles = views * view_tiles;
   if (tiles == 0) return;
-  blend_backward_views_kernel<<<tiles, 128, 0, stream>>>(W, H, gx, tiles, view_tiles, ranges, order, order_info,
-                                                         point_list, rec, bg, final_T, n_contrib, dL_dpix, strip_mask,
-                                                         g2d);
-  count_launch();
+  launch_pdl(blend_backward_views_kernel, tiles, 128, 0, stream, W, H, gx, tiles, view_tiles, ranges, order, order_info,
+             point_list, rec, bg, final_T, n_contrib, dL_dpix, strip_mask, g2d);
 }
 
 // gab200_backward_views_depth_alpha: blend_backward_views_kernel with the plane gradients (backward_task<K, true>):
@@ -1047,6 +1052,8 @@ __global__ void __launch_bounds__(128, GAB_BWD_DEPTH_CTAS) blend_backward_views_
     const uint32_t* __restrict__ n_contrib, const float* __restrict__ dL_dpix, const uint8_t* __restrict__ strip_mask,
     float* __restrict__ g2d, const float* __restrict__ dL_dalpha, const float* __restrict__ dL_ddepth) {
   __shared__ WarpSmemT<10> sm[4];
+  pdl_wait();
+  pdl_trigger();
   const int nh = (int)order_info[1];
   const int b = blockIdx.x, t = threadIdx.x, w = t >> 5;
   const bool heavy = b < nh;
@@ -1074,10 +1081,8 @@ void launch_blend_backward_views_depth(int views, int W, int H, const uint2* ran
   const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
   const int view_tiles = gx * gy, tiles = views * view_tiles;
   if (tiles == 0) return;
-  blend_backward_views_depth_kernel<<<tiles, 128, 0, stream>>>(W, H, gx, tiles, view_tiles, ranges, order, order_info,
-                                                               point_list, rec, bg, final_T, n_contrib, dL_dpix,
-                                                               strip_mask, g2d, dL_dalpha, dL_ddepth);
-  count_launch();
+  launch_pdl(blend_backward_views_depth_kernel, tiles, 128, 0, stream, W, H, gx, tiles, view_tiles, ranges, order,
+             order_info, point_list, rec, bg, final_T, n_contrib, dL_dpix, strip_mask, g2d, dL_dalpha, dL_ddepth);
 }
 
 }  // namespace gab

@@ -35,6 +35,8 @@ __global__ void __launch_bounds__(256) face_frame_fwd_kernel(int F, const float*
                                                              const int32_t* __restrict__ faces,
                                                              float* __restrict__ fc, float* __restrict__ fR,
                                                              float* __restrict__ fs) {
+  pdl_wait();
+  pdl_trigger();
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= F) return;
   const V3 v0 = ld3(verts + 3 * (size_t)faces[3 * f]), v1 = ld3(verts + 3 * (size_t)faces[3 * f + 1]),
@@ -62,6 +64,8 @@ __global__ void __launch_bounds__(256) face_frame_bwd_kernel(int F, const float*
                                                              const float* __restrict__ g_fR,
                                                              const float* __restrict__ g_fs,
                                                              float* __restrict__ g_verts) {
+  pdl_wait();
+  pdl_trigger();
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= F) return;
   const int i0 = faces[3 * f], i1 = faces[3 * f + 1], i2 = faces[3 * f + 2];
@@ -108,14 +112,12 @@ __global__ void __launch_bounds__(256) face_frame_bwd_kernel(int F, const float*
 void launch_face_frame_forward(int F, const float* verts, const int32_t* faces, float* fc, float* fR, float* fs,
                                cudaStream_t stream) {
   if (F == 0) return;
-  face_frame_fwd_kernel<<<(F + 255) / 256, 256, 0, stream>>>(F, verts, faces, fc, fR, fs);
-  count_launch();
+  launch_pdl(face_frame_fwd_kernel, (F + 255) / 256, 256, 0, stream, F, verts, faces, fc, fR, fs);
 }
 void launch_face_frame_backward(int F, const float* verts, const int32_t* faces, const float* g_fc, const float* g_fR,
                                 const float* g_fs, float* g_verts, cudaStream_t stream) {
   if (F == 0) return;
-  face_frame_bwd_kernel<<<(F + 255) / 256, 256, 0, stream>>>(F, verts, faces, g_fc, g_fR, g_fs, g_verts);
-  count_launch();
+  launch_pdl(face_frame_bwd_kernel, (F + 255) / 256, 256, 0, stream, F, verts, faces, g_fc, g_fR, g_fs, g_verts);
 }
 
 }  // namespace gab

@@ -23,6 +23,26 @@ namespace gab {
 void count_launch();
 int tune_get(int knob);  // api.cu: current value of a gab200_tune() knob
 
+// Programmatic dependent launch (sm_90).  A kernel launched through launch_pdl may start while the kernel before it on
+// the stream is still draining (stream capture turns this into a programmatic graph edge), so its launch and the
+// CTAs' start-up overlap the predecessor's tail.  Every such kernel calls pdl_wait() in every CTA before it reads or
+// writes global memory -- it returns once the predecessor grid has completed and its writes are visible, and since
+// the predecessor waited the same way, once every earlier kernel has -- and then pdl_trigger(), which lets the next
+// kernel launch once all of this grid's CTAs have been scheduled.  Both are no-ops in a kernel launched without the
+// attribute.  Only kernel parameters and shared memory are touched above the wait: the camera, bg and dL/dimage may
+// be written by a kernel just before (a loss kernel, a torch copy), so they are read after it like everything else.
+template <typename... Params, typename... Args>
+void launch_pdl(void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr.val.programmaticStreamSerializationAllowed = 1;
+  const cudaLaunchConfig_t cfg = {grid, block, smem, stream, &attr, 1};
+  cudaLaunchKernelEx(&cfg, kernel, static_cast<Args&&>(args)...);
+  count_launch();
+}
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
 // Exact per-tile-row span of the region where a splat can reach alpha >= 1/255:
 //   q(d) = 1/2 (A dx^2 + C dy^2) + B dx dy <= ln(255 * opacity)          (the blend's own accept test)
 // For tile row ty the pixel centres have dy in [16 ty - py, 16 ty + 15 - py]; the x-extent of the ellipse over
@@ -121,17 +141,26 @@ void launch_mark_visible(int P, const float* means3D, const float* V, uint8_t* p
 // bucket-sorted one, whose kernels wrote them), capacity and sequence number
 void launch_publish_counters(uint32_t* counters, const uint32_t* offsets, int P, uint32_t capacity, uint32_t seq,
                              uint32_t* sticky_overflow, cudaStream_t stream);
+// Buffers the emission grid clears before the tile sort (preprocess.cu emit_clears); zero / null: nothing to clear
+struct EmitClears {
+  bool sentinel = false;      // keys past the device count up to the capacity get the sentinel 0xffffffff
+  uint8_t* mask = nullptr;    // block masks [0, n_mask) zeroed
+  uint32_t n_mask = 0;
+  uint2* ranges = nullptr;    // tile ranges [0, n_ranges) zeroed
+  uint32_t n_ranges = 0;
+};
 // `capacity`: instances the key/value arrays hold -- anything beyond is dropped (the frame's counters say so);
 // counters[BUCKET_OVERFLOW] != 0 (depth order unusable) emits nothing.
 void launch_emit_keys(int P, int gx, int gy, const SplatRec* rec, const SplatAux* aux, const uint32_t* order,
                       const uint32_t* offsets, const uint32_t* order_count, const uint32_t* counters, uint32_t capacity,
-                      uint32_t* cursor, uint32_t* keys, uint32_t* vals, int exact_binning, cudaStream_t stream);
+                      uint32_t* cursor, uint32_t* keys, uint32_t* vals, int exact_binning, const EmitClears& clr,
+                      cudaStream_t stream);
 // the same over the P virtual splats of a multi-view frame, view_splats per view: instances of virtual splat v go to
 // the tiles (v / view_splats) * (gx * gy) + the tile in the view
 void launch_emit_keys_views(int P, int gx, int gy, const SplatRec* rec, const SplatAux* aux, const uint32_t* order,
                             const uint32_t* offsets, const uint32_t* order_count, const uint32_t* counters, uint32_t cap,
                             uint32_t* cursor, uint32_t* keys, uint32_t* vals, int exact_binning, int view_splats,
-                            cudaStream_t stream);
+                            const EmitClears& clr, cudaStream_t stream);
 // keys[0..N) sorted; entries with key >= tiles are padding (sentinel) behind the last real instance
 void launch_tile_ranges(int64_t N, uint32_t tiles, const uint32_t* keys, uint2* ranges, cudaStream_t stream);
 void launch_expand_keys(int64_t N, const uint32_t* tile_keys, const uint32_t* ids, const SplatAux* aux, uint64_t* out,

@@ -49,6 +49,8 @@ __global__ void __launch_bounds__(PRE_NT) preprocess_kernel(gab200_forward_args 
                                                             const float* __restrict__ tanfov) {
   __shared__ Camera cam;
   __shared__ float sh_s[PRE_NT * SH_SMEM_STRIDE_MAX];
+  pdl_wait();
+  pdl_trigger();
   stage_camera(a, cam);
 #define GAB_PRE_OUT i
 #include "preprocess_splat.inc"
@@ -68,6 +70,8 @@ __global__ void __launch_bounds__(PRE_NT) preprocess_depth_kernel(gab200_forward
                                                                   const float* __restrict__ tanfov) {
   __shared__ Camera cam;
   __shared__ float sh_s[PRE_NT * SH_SMEM_STRIDE_MAX];
+  pdl_wait();
+  pdl_trigger();
   stage_camera(a, cam);
 #define GAB_PRE_OUT i
 #define GAB_PRE_REC_DEPTH
@@ -91,6 +95,8 @@ __global__ void __launch_bounds__(PRE_NT) preprocess_views_kernel(gab200_forward
   __shared__ float sh_s[PRE_NT * SH_SMEM_STRIDE_MAX];
   const int view = (int)blockIdx.y;
   const float* row = cameras + (size_t)view * GAB200_CAMERA_FLOATS;
+  pdl_wait();
+  pdl_trigger();
   stage_camera_row(row, cam);
   const float* tanfov = row + 35;
   uint8_t* const clamped = nullptr;
@@ -118,6 +124,8 @@ __global__ void __launch_bounds__(PRE_NT) preprocess_views_train_kernel(gab200_f
   __shared__ float sh_s[PRE_NT * SH_SMEM_STRIDE_MAX];
   const int view = (int)blockIdx.y;
   const float* row = cameras + (size_t)view * GAB200_CAMERA_FLOATS;
+  pdl_wait();
+  pdl_trigger();
   stage_camera_row(row, cam);
   const float* tanfov = row + 35;
   const int view_tiles = ((a.image_width + GAB_TILE - 1) / GAB_TILE) * ((a.image_height + GAB_TILE - 1) / GAB_TILE);
@@ -146,6 +154,8 @@ __global__ void __launch_bounds__(PRE_NT) preprocess_views_depth_kernel(gab200_f
   __shared__ float sh_s[PRE_NT * SH_SMEM_STRIDE_MAX];
   const int view = (int)blockIdx.y;
   const float* row = cameras + (size_t)view * GAB200_CAMERA_FLOATS;
+  pdl_wait();
+  pdl_trigger();
   stage_camera_row(row, cam);
   const float* tanfov = row + 35;
   const int view_tiles = ((a.image_width + GAB_TILE - 1) / GAB_TILE) * ((a.image_height + GAB_TILE - 1) / GAB_TILE);
@@ -168,9 +178,8 @@ void launch_preprocess(const gab200_forward_args& a, SplatRec* rec, SplatAux* au
   if (rec_depth)
     kernel = bound ? (tanfov ? preprocess_depth_kernel<true, true> : preprocess_depth_kernel<true, false>)
                    : (tanfov ? preprocess_depth_kernel<false, true> : preprocess_depth_kernel<false, false>);
-  kernel<<<blocks, threads, 0, stream>>>(a, rec, aux, tiles_touched, clamped, depth_keys, ids, a.exact_binning, buckets,
-                                         tile_count, tanfov);
-  count_launch();
+  launch_pdl(kernel, blocks, threads, 0, stream, a, rec, aux, tiles_touched, clamped, depth_keys, ids, a.exact_binning,
+             buckets, tile_count, tanfov);
 }
 
 void launch_preprocess_views(const gab200_forward_args& a, int views, const float* cameras, SplatRec* rec, SplatAux* aux,
@@ -181,21 +190,18 @@ void launch_preprocess_views(const gab200_forward_args& a, int views, const floa
   if (rec_depth) {  // clamped != nullptr only for the training frame (BOUND_RAW, checked by the caller)
     auto kernel = a.input_mode == GAB200_INPUT_BOUND_RAW ? preprocess_views_depth_kernel<true>
                                                          : preprocess_views_depth_kernel<false>;
-    kernel<<<dim3(blocks, views), threads, 0, stream>>>(a, cameras, rec, aux, tiles_touched, clamped, depth_keys, ids,
-                                                        a.exact_binning, buckets, tile_count);
-    count_launch();
+    launch_pdl(kernel, dim3(blocks, views), threads, 0, stream, a, cameras, rec, aux, tiles_touched, clamped, depth_keys,
+               ids, a.exact_binning, buckets, tile_count);
     return;
   }
   if (clamped != nullptr) {  // training frame (BOUND_RAW, checked by the caller)
-    preprocess_views_train_kernel<<<dim3(blocks, views), threads, 0, stream>>>(
-        a, cameras, rec, aux, tiles_touched, clamped, depth_keys, ids, a.exact_binning, buckets, tile_count);
-    count_launch();
+    launch_pdl(preprocess_views_train_kernel, dim3(blocks, views), threads, 0, stream, a, cameras, rec, aux,
+               tiles_touched, clamped, depth_keys, ids, a.exact_binning, buckets, tile_count);
     return;
   }
   auto kernel = a.input_mode == GAB200_INPUT_BOUND_RAW ? preprocess_views_kernel<true> : preprocess_views_kernel<false>;
-  kernel<<<dim3(blocks, views), threads, 0, stream>>>(a, cameras, rec, aux, tiles_touched, depth_keys, ids,
-                                                      a.exact_binning, buckets, tile_count);
-  count_launch();
+  launch_pdl(kernel, dim3(blocks, views), threads, 0, stream, a, cameras, rec, aux, tiles_touched, depth_keys, ids,
+             a.exact_binning, buckets, tile_count);
 }
 
 // =====================================================================================================
@@ -253,6 +259,8 @@ __global__ void __launch_bounds__(DS_NT) depth_scatter_kernel(int P, DepthBucket
   __shared__ uint32_t s_flag;
   const int tid = threadIdx.x, nb = (int)bk.nb;
   if (tid == 0) s_flag = 0;
+  pdl_wait();
+  pdl_trigger();
   uint32_t over = 0;
   for (int b = tid; b < nb; b += DS_NT) {
     const uint32_t c = bk.counts[b];
@@ -302,6 +310,8 @@ __global__ void __launch_bounds__(DB_NT) depth_bucket_kernel(DepthBuckets bk, co
   __shared__ uint32_t st[GAB_DEPTH_BUCKET_CAP];
   __shared__ uint32_t warp_tot[DB_NT / 32];
   const int b = blockIdx.x, tid = threadIdx.x;
+  pdl_wait();
+  pdl_trigger();
   const int n = (int)bk.counts[b];
   if (n == 0 || n > GAB_DEPTH_BUCKET_CAP) return;  // overflow: the host redoes the frame on the radix path
   const uint32_t start = bk.start[b], tbase = bk.tile_base[b];
@@ -344,11 +354,9 @@ void launch_depth_bucket_sort(int P, const DepthBuckets& bk, const uint32_t* dep
                               uint32_t* scratch_keys, uint32_t* sorted_ids, uint32_t* offsets, uint32_t capacity,
                               uint32_t seq, uint32_t* sticky_overflow, cudaStream_t stream) {
   if (P <= 0) return;
-  depth_scatter_kernel<<<(P + DS_NT - 1) / DS_NT, DS_NT, bk.nb * sizeof(uint32_t), stream>>>(
-      P, bk, depth_keys, scratch_keys, sorted_ids, capacity, seq, sticky_overflow);
-  count_launch();
-  depth_bucket_kernel<<<bk.nb, DB_NT, 0, stream>>>(bk, scratch_keys, sorted_ids, tiles_touched, offsets);
-  count_launch();
+  launch_pdl(depth_scatter_kernel, (P + DS_NT - 1) / DS_NT, DS_NT, bk.nb * sizeof(uint32_t), stream, P, bk, depth_keys,
+             scratch_keys, sorted_ids, capacity, seq, sticky_overflow);
+  launch_pdl(depth_bucket_kernel, bk.nb, DB_NT, 0, stream, bk, scratch_keys, sorted_ids, tiles_touched, offsets);
 }
 
 // =====================================================================================================
@@ -416,6 +424,25 @@ void launch_mark_visible(int P, const float* means3D, const float* V, uint8_t* p
 
 // VIEWS (gab200_forward_views): splat i of the depth order is virtual splat view * view_splats + local; its instances
 // go to the tiles view * view_tiles + the tile in the view.
+// The clears the radix tile sort needs before it, done by the emission grid instead of memset nodes on the frame's
+// stream (each such node is a boundary of its own, and a kernel behind a memset cannot launch early): the ranges
+// [0, n_ranges), the block masks [0, n_mask) (16-B stores: the binning buffer's slack covers the round-up) and, with
+// `sentinel` (count only on the device), the padding keys [n, cap) behind the n = min(N, cap) instances the emission
+// writes -- all cap keys when a depth bucket overflowed and nothing is emitted.
+__device__ __forceinline__ void emit_clears(const uint32_t* counters, const uint32_t* order_count, uint32_t cap,
+                                            uint32_t* keys, bool sentinel, uint8_t* mask, uint32_t n_mask,
+                                            uint2* ranges, uint32_t n_ranges) {
+  const uint32_t stride = gridDim.x * blockDim.x, t = blockIdx.x * blockDim.x + threadIdx.x;
+  for (uint32_t j = t; j < n_ranges; j += stride) ranges[j] = make_uint2(0u, 0u);
+  if (mask != nullptr)
+    for (uint32_t j = t; j < (n_mask + 15u) / 16u; j += stride) reinterpret_cast<uint4*>(mask)[j] = make_uint4(0, 0, 0, 0);
+  if (sentinel) {
+    uint32_t n = counters[GAB200_CTR_NUM_RENDERED_HI] != 0 ? cap : min(counters[GAB200_CTR_NUM_RENDERED], cap);
+    if (order_count != nullptr && counters[GAB200_CTR_BUCKET_OVERFLOW] != 0) n = 0;
+    for (uint32_t j = n + t; j < cap; j += stride) keys[j] = 0xffffffffu;
+  }
+}
+
 template <bool VIEWS>
 __device__ __forceinline__ void emit_keys(int P, int gx, int gy, const SplatRec* rec, const SplatAux* aux,
                                           const uint32_t* order, const uint32_t* offsets, const uint32_t* order_count,
@@ -537,7 +564,12 @@ __global__ void __launch_bounds__(256) emit_keys_kernel(int P, int gx, int gy, c
                                                         const uint32_t* __restrict__ counters, uint32_t cap,
                                                         uint32_t* __restrict__ cursor,
                                                         uint32_t* __restrict__ keys, uint32_t* __restrict__ vals,
-                                                        int exact_binning) {
+                                                        int exact_binning, bool sentinel, uint8_t* __restrict__ mask,
+                                                        uint32_t n_mask, uint2* __restrict__ ranges,
+                                                        uint32_t n_ranges) {
+  pdl_wait();
+  pdl_trigger();
+  emit_clears(counters, order_count, cap, keys, sentinel, mask, n_mask, ranges, n_ranges);
   emit_keys<false>(P, gx, gy, rec, aux, order, offsets, order_count, counters, cap, cursor, keys, vals, exact_binning, 1u,
                    0u);
 }
@@ -551,13 +583,20 @@ __global__ void __launch_bounds__(256) emit_keys_views_kernel(int P, int gx, int
                                                               uint32_t* __restrict__ cursor,
                                                               uint32_t* __restrict__ keys, uint32_t* __restrict__ vals,
                                                               int exact_binning, uint32_t view_splats,
-                                                              uint32_t view_tiles) {
+                                                              uint32_t view_tiles, bool sentinel,
+                                                              uint8_t* __restrict__ mask, uint32_t n_mask,
+                                                              uint2* __restrict__ ranges, uint32_t n_ranges) {
+  pdl_wait();
+  pdl_trigger();
+  emit_clears(counters, order_count, cap, keys, sentinel, mask, n_mask, ranges, n_ranges);
   emit_keys<true>(P, gx, gy, rec, aux, order, offsets, order_count, counters, cap, cursor, keys, vals, exact_binning,
                   view_splats, view_tiles);
 }
 
 __global__ void publish_counters_kernel(uint32_t* __restrict__ counters, const uint32_t* __restrict__ offsets, int P,
                                         uint32_t capacity, uint32_t seq, uint32_t* __restrict__ sticky_overflow) {
+  pdl_wait();
+  pdl_trigger();
   if (P > 0) {  // radix-sorted frame: every splat is listed; N is the last inclusive offset (unless already counted)
     if (offsets != nullptr) counters[GAB200_CTR_NUM_RENDERED] = offsets[P - 1];
     counters[GAB200_CTR_NUM_LISTED] = (uint32_t)P;
@@ -573,41 +612,41 @@ __global__ void publish_counters_kernel(uint32_t* __restrict__ counters, const u
 }
 void launch_publish_counters(uint32_t* counters, const uint32_t* offsets, int P, uint32_t capacity, uint32_t seq,
                              uint32_t* sticky_overflow, cudaStream_t stream) {
-  publish_counters_kernel<<<1, 1, 0, stream>>>(counters, offsets, P, capacity, seq, sticky_overflow);
-  count_launch();
+  launch_pdl(publish_counters_kernel, 1, 1, 0, stream, counters, offsets, P, capacity, seq, sticky_overflow);
 }
 
 void launch_emit_keys(int P, int gx, int gy, const SplatRec* rec, const SplatAux* aux, const uint32_t* order,
                       const uint32_t* offsets, const uint32_t* order_count, const uint32_t* counters, uint32_t cap,
-                      uint32_t* cursor, uint32_t* keys, uint32_t* vals, int exact_binning, cudaStream_t stream) {
+                      uint32_t* cursor, uint32_t* keys, uint32_t* vals, int exact_binning, const EmitClears& clr,
+                      cudaStream_t stream) {
   const int warps = (P + 31) / 32;
   const int threads = 256, blocks = (warps * 32 + threads - 1) / threads;
   if (blocks == 0) return;
-  emit_keys_kernel<<<blocks, threads, 0, stream>>>(P, gx, gy, rec, aux, order, offsets, order_count, counters, cap, cursor,
-                                                   keys, vals, exact_binning);
-  count_launch();
+  launch_pdl(emit_keys_kernel, blocks, threads, 0, stream, P, gx, gy, rec, aux, order, offsets, order_count, counters,
+             cap, cursor, keys, vals, exact_binning, clr.sentinel, clr.mask, clr.n_mask, clr.ranges, clr.n_ranges);
 }
 
 void launch_emit_keys_views(int P, int gx, int gy, const SplatRec* rec, const SplatAux* aux, const uint32_t* order,
                             const uint32_t* offsets, const uint32_t* order_count, const uint32_t* counters, uint32_t cap,
                             uint32_t* cursor, uint32_t* keys, uint32_t* vals, int exact_binning, int view_splats,
-                            cudaStream_t stream) {
+                            const EmitClears& clr, cudaStream_t stream) {
   const int warps = (P + 31) / 32;
   const int threads = 256, blocks = (warps * 32 + threads - 1) / threads;
   if (blocks == 0) return;
-  emit_keys_views_kernel<<<blocks, threads, 0, stream>>>(P, gx, gy, rec, aux, order, offsets, order_count, counters, cap,
-                                                         cursor, keys, vals, exact_binning, (uint32_t)view_splats,
-                                                         (uint32_t)(gx * gy));
-  count_launch();
+  launch_pdl(emit_keys_views_kernel, blocks, threads, 0, stream, P, gx, gy, rec, aux, order, offsets, order_count,
+             counters, cap, cursor, keys, vals, exact_binning, (uint32_t)view_splats, (uint32_t)(gx * gy),
+             clr.sentinel, clr.mask, clr.n_mask, clr.ranges, clr.n_ranges);
 }
 
 // =====================================================================================================
-// K5: tile ranges from key transitions in the sorted stream (ranges pre-zeroed by the caller).
+// K5: tile ranges from key transitions in the sorted stream (ranges zeroed by the emission, EmitClears).
 // =====================================================================================================
 // Keys >= tiles are the padding of a capacity-sized sort (sentinel 0xffffffff): they sort behind every real instance
 // and all of them land in the spare slot ranges[tiles], which nobody reads.
 __global__ void __launch_bounds__(256) tile_ranges_kernel(int64_t N, uint32_t tiles, const uint32_t* __restrict__ keys,
                                                           uint2* __restrict__ ranges) {
+  pdl_wait();
+  pdl_trigger();
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= N) return;
   const uint32_t cur = min(keys[idx], tiles);
@@ -641,8 +680,7 @@ void launch_tile_ranges(int64_t N, uint32_t tiles, const uint32_t* keys, uint2* 
   if (N == 0) return;
   const int threads = 256;
   const int64_t blocks = (N + threads - 1) / threads;
-  tile_ranges_kernel<<<(unsigned)blocks, threads, 0, stream>>>(N, tiles, keys, ranges);
-  count_launch();
+  launch_pdl(tile_ranges_kernel, (unsigned)blocks, threads, 0, stream, N, tiles, keys, ranges);
 }
 
 }  // namespace gab

@@ -83,6 +83,8 @@ __global__ void __launch_bounds__(256) face_grad_reduce_kernel(int num_chunks, c
                                                                const int32_t* __restrict__ chunk_end,
                                                                const float* __restrict__ fg, float* __restrict__ d_fc,
                                                                float* __restrict__ d_fR, float* __restrict__ d_fs) {
+  pdl_wait();
+  pdl_trigger();
   const int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 4, c = threadIdx.x & 15;
   if (g >= num_chunks || c >= GAB_FACE_GRAD_STRIDE) return;
   const int s0 = chunk_start[g], s1 = chunk_end[g];
@@ -112,24 +114,22 @@ void launch_preprocess_backward(const gab200_backward_args& b, const SplatRec* r
     auto kernel = a.input_mode == GAB200_INPUT_BOUND_RAW
                       ? (dev ? preprocess_backward_depth_kernel<true, true> : preprocess_backward_depth_kernel<true, false>)
                       : (dev ? preprocess_backward_depth_kernel<false, true> : preprocess_backward_depth_kernel<false, false>);
-    kernel<<<blocks, threads, 0, stream>>>(b, a, rec, aux, clamped, g2d,
-                                           a.input_mode == GAB200_INPUT_BOUND_RAW ? face_scratch : nullptr, tanfov);
+    launch_pdl(kernel, blocks, threads, 0, stream, b, a, rec, aux, clamped, g2d,
+               a.input_mode == GAB200_INPUT_BOUND_RAW ? face_scratch : nullptr, tanfov);
   } else if (a.input_mode == GAB200_INPUT_BOUND_RAW) {
     auto kernel = b.grads_are_multicast
                       ? (dev ? preprocess_backward_kernel<true, true, true> : preprocess_backward_kernel<true, true, false>)
                       : (dev ? preprocess_backward_kernel<true, false, true> : preprocess_backward_kernel<true, false, false>);
-    kernel<<<blocks, threads, 0, stream>>>(b, a, rec, aux, clamped, g2d, face_scratch, tanfov);
+    launch_pdl(kernel, blocks, threads, 0, stream, b, a, rec, aux, clamped, g2d, face_scratch, tanfov);
   } else {
     auto kernel = dev ? preprocess_backward_kernel<false, false, true> : preprocess_backward_kernel<false, false, false>;
-    kernel<<<blocks, threads, 0, stream>>>(b, a, rec, aux, clamped, g2d, nullptr, tanfov);
+    launch_pdl(kernel, blocks, threads, 0, stream, b, a, rec, aux, clamped, g2d, nullptr, tanfov);
   }
-  count_launch();
   if (face_scratch != nullptr && b.num_face_chunks > 0) {
     const int groups_per_block = 256 / 16;
-    face_grad_reduce_kernel<<<(b.num_face_chunks + groups_per_block - 1) / groups_per_block, 256, 0, stream>>>(
-        b.num_face_chunks, b.face_perm, b.face_chunk_face, b.face_chunk_start, b.face_chunk_end, face_scratch,
-        b.dL_dface_center, b.dL_dface_orien_mat, b.dL_dface_scaling);
-    count_launch();
+    launch_pdl(face_grad_reduce_kernel, (b.num_face_chunks + groups_per_block - 1) / groups_per_block, 256, 0, stream,
+               b.num_face_chunks, b.face_perm, b.face_chunk_face, b.face_chunk_start, b.face_chunk_end, face_scratch,
+               b.dL_dface_center, b.dL_dface_orien_mat, b.dL_dface_scaling);
   }
 }
 
@@ -140,14 +140,12 @@ void launch_preprocess_backward_views(const gab200_backward_args& b, int views, 
   const int threads = PRE_NT, blocks = (a.P + threads - 1) / threads;
   if (blocks == 0) return;
   auto kernel = depth ? preprocess_backward_views_depth_kernel : preprocess_backward_views_kernel;
-  kernel<<<blocks, threads, 0, stream>>>(b, a, views, cameras, aux, clamped, g2d, face_scratch);
-  count_launch();
+  launch_pdl(kernel, blocks, threads, 0, stream, b, a, views, cameras, aux, clamped, g2d, face_scratch);
   if (face_scratch != nullptr && b.num_face_chunks > 0) {
     const int groups_per_block = 256 / 16;
-    face_grad_reduce_kernel<<<(b.num_face_chunks + groups_per_block - 1) / groups_per_block, 256, 0, stream>>>(
-        b.num_face_chunks, b.face_perm, b.face_chunk_face, b.face_chunk_start, b.face_chunk_end, face_scratch,
-        b.dL_dface_center, b.dL_dface_orien_mat, b.dL_dface_scaling);
-    count_launch();
+    launch_pdl(face_grad_reduce_kernel, (b.num_face_chunks + groups_per_block - 1) / groups_per_block, 256, 0, stream,
+               b.num_face_chunks, b.face_perm, b.face_chunk_face, b.face_chunk_start, b.face_chunk_end, face_scratch,
+               b.dL_dface_center, b.dL_dface_orien_mat, b.dL_dface_scaling);
   }
 }
 

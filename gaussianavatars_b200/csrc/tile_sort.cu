@@ -54,6 +54,8 @@ __global__ void __launch_bounds__(SCAN_NT) tile_scan_order_kernel(int tiles, con
   for (int k = tid; k < ORDER_WARPS * (ORDER_NB + 1); k += SCAN_NT) (&hist[0][0])[k] = 0;
   if (tid == 0) { s_carry = 0; s_long = 0; }
   __syncthreads();
+  pdl_wait();  // shared-memory set-up above overlaps the predecessor; ranges / counts / order below
+  pdl_trigger();
   if (tile_count != nullptr) {
     // ---- exclusive scan of the counts, SCAN_NT tiles per round ----
     for (int base = 0; base < tiles; base += SCAN_NT) {
@@ -158,9 +160,8 @@ void launch_tile_scan_order(int tiles, const uint32_t* tile_count, uint32_t clam
                             uint32_t* order, uint32_t* order_info, uint32_t* counters, int heavy_fwd, int heavy_bwd,
                             cudaStream_t stream) {
   if (tiles == 0) return;
-  tile_scan_order_kernel<<<1, SCAN_NT, 0, stream>>>(tiles, tile_count, clamp, ranges, cursor, order, order_info,
-                                                    counters, heavy_fwd, heavy_bwd);
-  count_launch();
+  launch_pdl(tile_scan_order_kernel, 1, SCAN_NT, 0, stream, tiles, tile_count, clamp, ranges, cursor, order, order_info,
+             counters, heavy_fwd, heavy_bwd);
 }
 
 // =====================================================================================================

@@ -289,7 +289,6 @@ class _Captured:
         try:
             with torch.cuda.graph(self.graph):
                 self._body(captured=True)
-                self.slot.flag_host.copy_(self.slot.flag, non_blocking=True)
         finally:
             R._capture_slot = None
         self._after_capture()
@@ -319,11 +318,14 @@ class _Captured:
 
     # ---- overflow --------------------------------------------------------------------------------------------------
     def overflowed(self, wait: bool = True) -> bool:
-        """True if any replay since the last (re-)capture needed more than the captured capacity."""
+        """True if any replay since the last (re-)capture needed more than the captured capacity.  The sticky flag stays
+        on the device (a copy of it inside the graph would be the last node of every replay): wait=True reads it behind
+        the replays enqueued so far; wait=False returns what the last wait=True read found."""
         if self.slot is None:
             return False
         if wait:
             torch.cuda.current_stream(self.device).synchronize()
+            self.slot.flag_host.copy_(self.slot.flag)
         return bool(int(self.slot.flag_host[0]) != 0)
 
     def counters(self) -> dict:
