@@ -16,6 +16,8 @@
 //     issue-bound.
 //   * splat records (48 B, three 16-B quads) are GATHERED straight into shared memory with cp.async (LDGSTS),
 //     double buffered one chunk ahead, ids one further chunk ahead: no register staging, no exposed L2 latency.
+//   * forward: per 32-splat group, each warp tests the splats' alpha boxes against its pixels (reaches_rect) and walks
+//     only the live ones, through a per-warp list of their offsets.
 //   * forward records, per sorted instance, which of the tile's eight 8x4 blocks it contributed to (one byte);
 //     backward visits a (splat, warp) pair only if one of the warp's blocks is set.
 //   * backward: one WARP task per (tile, half, band group) -- K = 2 on heavy tiles, K = 4 on light ones -- with a
@@ -158,6 +160,29 @@ __device__ __forceinline__ void store_display(uint8_t* __restrict__ out, int W, 
   }
 }
 
+// Can splat r reach alpha >= 1/255 at a pixel centre of the rectangle [x0, x1] x [y0, y1]?  The test of the splat's
+// alpha box against the rectangle: (rx, ry) = q2.yz are TileSpan's extents of the ellipse
+//   q(d) = 1/2 (A dx^2 + C dy^2) + B dx dy <= tau = ln(255 opacity) + 0.01,   rx = sqrt(2 tau C / det) + 0.02 px
+// (ry likewise with A), 1e30 for a degenerate conic and -1 when tau <= 0 (no alpha reaches 1/255: never live).  A
+// NaN centre or extent counts as live.
+// Why a skipped splat is one the unculled walk would not have changed anything for: a pixel centre outside the box
+// lies outside the ellipse q = tau, so its exact alpha is below e^-0.01 / 255 = 0.990 / 255.  The walk computes pw in
+// float (two fmaf and a product, rounding error at most ~4 ulp of the largest term |A'| dx^2, |B' dx dy|, |C'| dy^2,
+// whose sum is at most (kappa + 1) |pw| for a conic of condition number kappa), ex2.approx.ftz (relative error below
+// 2^-22, PTX ISA) and op * G, and accepts alpha >= 1/255.  Accepting a pixel whose exact alpha is below 0.990 / 255
+// takes an error of 0.0144 in pw (the 0.01 log margin in log2 units); with |pw| <= 8 near the boundary, the rounding
+// stays below that for kappa up to ~7e3, and ex2's error is five orders of magnitude short of it.  The +0.02 px
+// margin adds 2 tau 0.02 / rx to q at the box edge on top.  Such a pixel fails `pw <= 0 && alpha >= 1/255` in the
+// walk: no T, colour, depth, `done`, `last` or block-mask bit changes, so skipping the splat for the whole warp leaves
+// every output bit-identical.  The binning (TileSpan::row) drops whole tiles on the same margins; this test applies
+// them to the warp's 8x4 blocks.  tests/test_gpu_forward_cull.py checks the claim in float32 on the adversarial rigs.
+__device__ __forceinline__ bool reaches_rect(const SplatRec& r, float x0, float x1, float y0, float y1) {
+  const float4 q0 = r.q0, q2 = r.q2;
+  const float ex = fmaxf(fmaxf(x0 - q0.x, q0.x - x1), 0.f);  // distance from the centre to the rectangle, per axis
+  const float ey = fmaxf(fmaxf(y0 - q0.y, q0.y - y1), 0.f);
+  return !(ex > q2.y) && !(ey > q2.z);
+}
+
 // =====================================================================================================
 // Forward: one tile on a group of NT = 256/K threads (tl = thread index inside the group)
 // =====================================================================================================
@@ -188,6 +213,11 @@ __device__ __forceinline__ void forward_tile(int tile, int tl, GroupBarrier<256 
   const uint32_t* ids = point_list + range.x;
   const bool want_mask = strip_mask != nullptr;
   smask[tl] = 0;
+  // the warp's pixel rectangle: columns of its half, rows of its K bands (pixels past the image edge included)
+  const float rx0 = (float)(pixx - (lane & 7)), rx1 = rx0 + 7.f;
+  const float ry0 = (float)(ty * GAB_TILE + geo.band0 * 4), ry1 = ry0 + (float)(4 * K - 1);
+  __shared__ uint8_t live_idx[8][32];  // per warp of the CTA: the group offsets of the live splats, in list order
+  uint8_t* my_idx = live_idx[threadIdx.x >> 5];
 
   float T[K], Cr[K], Cg[K], Cb[K];
   float D[DA ? K : 1];
@@ -256,12 +286,20 @@ __device__ __forceinline__ void forward_tile(int tile, int tl, GroupBarrier<256 
     uint32_t lb[K];
 #pragma unroll
     for (int i = 0; i < K; i++) lb[i] = 0;
-    // 32-splat groups: the inner loop is branch-light and unrolled; the per-group epilogue publishes the strip bits
-    // and tests saturation once per group
+    // 32-splat groups: lane L first tests splat gbase+L against the warp's rectangle (reaches_rect) and the ballot's
+    // set bits are compacted into a list of group offsets, so the inner loop walks only those splats, branch-light
+    // and unrolled, with every record address independent of the previous iteration; the per-group epilogue
+    // publishes the strip bits and tests saturation once per group.
     for (int gbase = 0; gbase < cnt; gbase += 32) {
       const int gend = min(32, cnt - gbase);
+      const uint32_t live = __ballot_sync(FULLMASK, lane < gend && reaches_rect(cur[gbase + lane], rx0, rx1, ry0, ry1));
+      const int nlive = __popc(live);
+      __syncwarp();  // the previous group's walk has read the list
+      if ((live >> lane) & 1u) my_idx[__popc(live & ((1u << lane) - 1u))] = (uint8_t)lane;
+      __syncwarp();
 #pragma unroll 4
-      for (int jj = 0; jj < gend; jj++) {
+      for (int k = 0; k < nlive; k++) {
+        const int jj = my_idx[k];
         const SplatRec* r = cur + gbase + jj;
         const float4 q0 = r->q0;
         const float4 q1 = r->q1;

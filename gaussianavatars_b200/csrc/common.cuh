@@ -17,7 +17,8 @@ namespace gab {
 //   q0 = (px, py, A', B')   q1 = (C', opacity, r, g)   q2 = (b, rx, ry, 0)
 // with the conic pre-scaled for the blend exponent in log2 units: (A',B',C') = (-conic.xx/2, -conic.xy, -conic.yy/2)*log2 e
 // (rx, ry) = half extents of the axis-aligned box around the region where the splat can reach alpha >= 1/255
-// (negative: nowhere) -- the blend-forward warps use it to skip splats that cannot touch their pixel strip.
+// (negative: nowhere; 1e30: unbounded), from the TileSpan that culls the instance list.  Read only by the forward
+// blend (blend.cu `reaches_rect`): each warp walks only the splats whose box meets its pixel rectangle.
 struct __align__(16) SplatRec {
   float4 q0, q1, q2;
 };
