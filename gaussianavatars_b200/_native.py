@@ -217,7 +217,7 @@ EXPORTED_SYMBOLS = ("gab200_forward", "gab200_backward", "gab200_mark_visible", 
                     "gab200_mesh_scratch_bytes", "gab200_forward_views", "gab200_forward_views_train",
                     "gab200_backward_views", "gab200_forward_depth_alpha", "gab200_backward_depth_alpha",
                     "gab200_forward_views_depth_alpha", "gab200_forward_views_train_depth_alpha",
-                    "gab200_backward_views_depth_alpha")
+                    "gab200_backward_views_depth_alpha", "gab200_composite_rgba")
 
 _lib = None
 _lock = threading.Lock()
@@ -310,6 +310,9 @@ def lib():
         L.gab200_l1_loss_u8.argtypes = [C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gab200_l1_loss_u8_backward.restype = C.c_int32
         L.gab200_l1_loss_u8_backward.argtypes = [C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gab200_composite_rgba.restype = C.c_int32
+        L.gab200_composite_rgba.argtypes = [C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_void_p]
         L.gab200_photometric_loss.restype = C.c_int32
         L.gab200_photometric_loss.argtypes = [C.POINTER(PhotometricArgs), C.c_void_p]
         L.gab200_image_metrics.restype = C.c_int32

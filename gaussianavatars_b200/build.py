@@ -32,6 +32,7 @@ SOURCES = {
     "face_frame.cu": [],
     "flame.cu": [],
     "loss.cu": [],
+    "composite.cu": [],
     "metrics.cu": [],
     "mesh.cu": ["--fmad=false"],
     "optim.cu": [],

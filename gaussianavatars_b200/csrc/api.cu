@@ -1020,6 +1020,15 @@ int32_t gab200_l1_loss_u8_backward(int64_t n, const float* img, const uint8_t* g
   return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
 }
 
+int32_t gab200_composite_rgba(int64_t views, int32_t height, int32_t width, const uint8_t* rgba, const float* bg,
+                              uint8_t* rgb_out, uint8_t* mask_out, void* stream_) {
+  if (views < 0 || height < 0 || width < 0) return GAB200_ERR_INVALID_ARGUMENT;
+  if (views * height * width > 0 && (!rgba || !bg || !rgb_out)) return GAB200_ERR_INVALID_ARGUMENT;
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  launch_composite_rgba(views, height, width, rgba, bg, rgb_out, mask_out, (cudaStream_t)stream_);
+  return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
 int32_t gab200_photometric_loss(const gab200_photometric_args* a, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   if (a == nullptr || a->abi_version != GAB200_ABI_VERSION || a->channels < 0 || a->height < 0 || a->width < 0 ||

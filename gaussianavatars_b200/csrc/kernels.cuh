@@ -265,6 +265,10 @@ void launch_l1_loss_u8(int64_t n, const float* img, const uint8_t* gt, const flo
 void launch_photometric_loss(int C, int H, int W, const float* img, const void* gt, int gt_is_u8, float lambda,
                              float* grad, float* loss, float* scratch, cudaStream_t stream);
 
+// composite.cu
+void launch_composite_rgba(int64_t views, int H, int W, const uint8_t* rgba, const float* bg, uint8_t* rgb,
+                           uint8_t* mask, cudaStream_t stream);
+
 // metrics.cu
 size_t metrics_scratch_bytes(int H, int W);
 void launch_image_metrics(int H, int W, int kind, const void* render, const uint8_t* gt, const int32_t* row, int rows,

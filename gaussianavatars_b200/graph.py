@@ -52,7 +52,8 @@ from types import SimpleNamespace
 from .renderer import _forward_only, _views_forward, camera_table, render, render_views_train
 from .rasterizer import l1_loss_u8
 from .densify import add_densification_stats
-from .training import METRIC_NAMES, Adam, binding_regularizers, launch_image_metrics, metrics_scratch, photometric_loss
+from .training import (METRIC_NAMES, Adam, binding_regularizers, launch_composite_rgba, launch_image_metrics,
+                       metrics_scratch, photometric_loss)
 from .flame import check_timestep, flame_pose
 
 _STATS = ("xyz_gradient_accum", "denom", "max_radii2D")
@@ -346,7 +347,8 @@ class GraphedFrame(_Captured):
                  lambda_dssim: float = 0.2, host_inputs: bool = False, capacity: Optional[int] = None,
                  headroom: float = 1.25, after_backward=None, warm_cameras=None, regularizers: Optional[dict] = None,
                  before_backward=None, side_work=None, side_work_at: str = "start", optimizer: Optional[Adam] = None,
-                 densify_stats: bool = False, per_camera_fov: bool = False, views_per_replay: int = 1):
+                 densify_stats: bool = False, per_camera_fov: bool = False, views_per_replay: int = 1,
+                 rgba: bool = False, lambda_mask: float = 0.0):
         """loss: "l1_u8" (L1 vs a uint8 ground truth), "photometric" ((1-l) L1 + l (1-SSIM) vs a uint8 ground truth) or
         "dL_dimage" (the caller supplies dL/dimage in `self.dL_dimage`).
         host_inputs: the frame owns pinned STAGING tensors (`cam_stage` (35,) float32, `gt_stage` (3,H,W) uint8) that a
@@ -391,11 +393,29 @@ class GraphedFrame(_Captured):
         K x the batch loss (one mean over the K images), i.e. the sum of the K per-view losses, plus the regularisers
         once per view with that view's radii; densify_stats feeds the K rows to the statistics in view order; the
         optimizer takes ONE step per replay.  Changing cameras, timestep or ground truth never re-captures.
-        views_per_replay=1 is the single-camera frame."""
+        views_per_replay=1 is the single-camera frame.
+        rgba=True: the ground truth arrives as the capture's decoded RGBA frame(s) -- `set_inputs(gt_rgba=...)`, uint8
+        (H,W,4) or (K,H,W,4), in place of gt_u8, which is refused -- and the graph makes the (3,H,W) / (K,3,H,W) uint8
+        ground truth itself before the loss: the reference loader's composite onto `bg`, bit for bit
+        (training.composite_rgba).  `gt` holds the composite, `mask` the alpha bytes ((1,H,W) / (K,1,H,W)); gt_stage
+        is the pinned (H,W,4) / (K,H,W,4) RGBA frame.  A loader then only decodes the PNG.
+        lambda_mask > 0 (needs rgba=True): the frame renders the alpha plane as well (render(depth_alpha=True)),
+        exposes `alpha` and `depth`, and adds the foreground-mask term  K * lambda_mask * l1_loss_u8(alpha, mask),
+        the sum over the views of lambda_mask * mean|alpha - mask/255|, to the loss before the regularisers.  Both
+        are construction constants: they never re-capture."""
         if loss not in ("l1_u8", "photometric", "dL_dimage"):
             raise ValueError("loss must be 'l1_u8', 'photometric' or 'dL_dimage'")
         if regularizers is not None and loss == "dL_dimage":
             raise ValueError("regularizers need a scalar loss ('l1_u8' or 'photometric')")
+        if rgba and loss == "dL_dimage":
+            raise ValueError("rgba=True makes the ground truth of a scalar loss ('l1_u8' or 'photometric'): "
+                             "loss='dL_dimage' reads none")
+        lambda_mask = float(lambda_mask)
+        if not lambda_mask >= 0.0 or not math.isfinite(lambda_mask):
+            raise ValueError(f"lambda_mask must be a finite value >= 0, got {lambda_mask}")
+        if lambda_mask > 0.0 and not rgba:
+            raise ValueError("the mask term compares the alpha plane with the capture's alpha: lambda_mask > 0 "
+                             "needs rgba=True")
         if optimizer is not None and not (isinstance(optimizer, Adam) and
                                           all(g.get("capturable", False) for g in optimizer.param_groups)):
             raise ValueError("optimizer must be a gaussianavatars_b200.Adam with capturable=True")
@@ -411,34 +431,54 @@ class GraphedFrame(_Captured):
         self.regularizers = regularizers
         self.optimizer = optimizer
         self.densify_stats = bool(densify_stats)
+        self.rgba, self.lambda_mask = bool(rgba), lambda_mask
         dev = self.device
         img = self._gt_shape()
         self.gt = torch.zeros(img, dtype=torch.uint8, device=dev) if loss != "dL_dimage" else None
+        lead = () if self.K == 1 else (self.K,)
+        # rgba: the static RGBA input the composite reads, and the mask it writes beside gt
+        self.gt_rgba = torch.zeros(lead + (self.H, self.W, 4), dtype=torch.uint8, device=dev) if self.rgba else None
+        self.mask = torch.zeros(lead + (1, self.H, self.W), dtype=torch.uint8, device=dev) if self.rgba else None
+        gt_in = self._gt_input()
         self.dL_dimage = torch.zeros(img, dtype=torch.float32, device=dev) if loss == "dL_dimage" else None
         self.cam_host = torch.zeros(self.cam.shape, dtype=torch.float32).pin_memory() if host_inputs else None  # staging
         if self.cam_host is not None:
             self.cam_host.copy_(self.cam)
         self.cam_stage = self.cam_host
-        self.gt_stage = (torch.zeros(img, dtype=torch.uint8).pin_memory()
-                         if host_inputs and self.gt is not None else None)
+        self.gt_stage = (torch.zeros(gt_in.shape, dtype=torch.uint8).pin_memory()
+                         if host_inputs and gt_in is not None else None)
         self._prefetch_target = None
         self.loss_host = torch.zeros((), dtype=torch.float32).pin_memory()
         self.loss = None
-        self.image = self.radii = self.viewspace_points = None
+        self.image = self.radii = self.viewspace_points = self.alpha = self.depth = None
         self._side = torch.cuda.Stream(device=dev) if (host_inputs or side_work is not None) else None
         self._uploads = bool(host_inputs)
 
     def _gt_shape(self):
         return (3, self.H, self.W) if self.K == 1 else (self.K, 3, self.H, self.W)
 
+    def _gt_input(self):
+        """The device tensor the ground truth is written into: the RGBA frame(s) with rgba=True, else gt."""
+        return self.gt_rgba if self.rgba else self.gt
+
     # ---- inputs ------------------------------------------------------------------------------------------------
-    def set_inputs(self, camera=None, verts=None, gt_u8=None, dL_dimage=None, timestep=None, cameras=None):
+    def set_inputs(self, camera=None, verts=None, gt_u8=None, dL_dimage=None, timestep=None, cameras=None,
+                   gt_rgba=None):
         """Copies new inputs into the static buffers (device tensors) / staging buffers (host_inputs).  `timestep`
         (a model with a FLAME head only) is a host int checked against the model's number of timesteps.
         views_per_replay=K > 1: `cameras` (K camera objects of the frame's image size, or a (K, 37) table) instead of
-        `camera`; gt_u8 / dL_dimage are (K,3,H,W)."""
+        `camera`; gt_u8 / dL_dimage are (K,3,H,W).  rgba=True: `gt_rgba`, the decoded uint8 RGBA frame (H,W,4) or
+        (K,H,W,4), instead of gt_u8."""
         if (camera is not None and self.K > 1) or (cameras is not None and self.K == 1):
             raise ValueError("a frame with views_per_replay > 1 takes cameras=, one with a single view camera=")
+        if gt_u8 is not None and self.rgba:
+            raise ValueError("this frame composites its ground truth from the RGBA frame: give gt_rgba=, not gt_u8")
+        if gt_rgba is not None:
+            if not self.rgba:
+                raise ValueError("gt_rgba= needs a frame built with rgba=True")
+            if gt_rgba.dtype != torch.uint8 or tuple(gt_rgba.shape) != tuple(self.gt_rgba.shape):
+                raise ValueError(f"gt_rgba of this frame is a uint8 {tuple(self.gt_rgba.shape)} tensor, got "
+                                 f"{gt_rgba.dtype} {tuple(gt_rgba.shape)}")
         if cameras is not None:
             camera = cameras
         for name, t in (("gt_u8", gt_u8), ("dL_dimage", dL_dimage)):
@@ -462,11 +502,13 @@ class GraphedFrame(_Captured):
         if verts is not None:
             with torch.no_grad():
                 self.verts.copy_(verts.reshape(self.verts.shape), non_blocking=True)
-        if gt_u8 is not None:
-            if gt_u8.device.type == "cpu" and self._uploads:
-                self._upload(self.gt, gt_u8)
+        gt_src = gt_rgba if gt_rgba is not None else gt_u8
+        if gt_src is not None:
+            dst = self._gt_input()
+            if gt_src.device.type == "cpu" and self._uploads:
+                self._upload(dst, gt_src)
             else:
-                self.gt.copy_(gt_u8, non_blocking=True)
+                dst.copy_(gt_src, non_blocking=True)
         if dL_dimage is not None:
             self.dL_dimage.copy_(dL_dimage, non_blocking=True)
 
@@ -479,6 +521,9 @@ class GraphedFrame(_Captured):
             raise ValueError("both frames of a prefetching pair must use the same per_camera_fov mode")
         if self.K != other.K:
             raise ValueError("both frames of a prefetching pair must render the same number of views per replay")
+        if self.rgba != other.rgba:
+            raise ValueError("both frames of a prefetching pair must take the same ground truth (rgba=True on both "
+                             "or on neither)")
         self._prefetch_target = other
         return self
 
@@ -486,7 +531,7 @@ class GraphedFrame(_Captured):
         """Eager upload of this frame's own staging tensors (the first step of a prefetching pair)."""
         self.cam.copy_(self.cam_stage, non_blocking=True)
         if self.gt_stage is not None:
-            self.gt.copy_(self.gt_stage, non_blocking=True)
+            self._gt_input().copy_(self.gt_stage, non_blocking=True)
 
     # ---- the step body (run eagerly for warm-up, then captured) --------------------------------------------------
     def _params(self):
@@ -513,20 +558,25 @@ class GraphedFrame(_Captured):
                 if other is not None:   # the other frame's next inputs travel
                     other.cam.copy_(other.cam_stage, non_blocking=True)
                     if other.gt_stage is not None:
-                        other.gt.copy_(other.gt_stage, non_blocking=True)
+                        other._gt_input().copy_(other.gt_stage, non_blocking=True)
                 if self.side_work is not None and self.side_work_at == "start":
                     self.side_work()
         self._pose()
+        planes = self.lambda_mask > 0.0   # the mask term reads the alpha plane
         if self.K > 1:   # the K cameras of the table in one forward and one backward
-            out = render_views_train(self.cam, pc, _Pipe, self.bg, width=self.W, height=self.H)
+            out = render_views_train(self.cam, pc, _Pipe, self.bg, width=self.W, height=self.H, depth_alpha=planes)
         else:
-            out = render(self.camera, pc, _Pipe, self.bg)
+            out = render(self.camera, pc, _Pipe, self.bg, depth_alpha=planes)
         img = out["render"]
         radii_rows = [out["radii"]] if self.K == 1 else list(out["radii"])
+        if self.rgba:   # the loader's composite of the RGBA input: gt and mask for this replay's loss
+            launch_composite_rgba(self.gt_rgba, self.bg, self.gt, self.mask)
         if self.loss_kind in ("l1_u8", "photometric"):
             loss = l1_loss_u8(img, self.gt) if self.loss_kind == "l1_u8" else photometric_loss(img, self.gt, self.lambda_dssim)
             if self.K > 1:   # one mean over the K images: K x it is the sum of the per-view losses
                 loss = loss * float(self.K)
+            if planes:   # one mean over the K alpha planes, K x it: the sum of the per-view mask terms
+                loss = loss + l1_loss_u8(out["alpha"], self.mask) * (float(self.K) * self.lambda_mask)
             if self.regularizers is not None:
                 for radii in radii_rows:   # train.py:134-146 per view, with that view's visibility
                     lx, ls = binding_regularizers(pc._xyz, pc._scaling, radii, getattr(pc, "binding", None),
@@ -561,6 +611,8 @@ class GraphedFrame(_Captured):
         if forked:   # join the branch (a captured fork must end inside the graph)
             torch.cuda.current_stream(self.device).wait_stream(self._side)
         self.image, self.radii, self.viewspace_points = img.detach(), out["radii"], out["viewspace_points"]
+        if planes:
+            self.alpha, self.depth = out["alpha"].detach(), out["depth"].detach()
 
     def _fork_side_at_backward(self):
         if self.side_work is not None and self.side_work_at == "backward":
@@ -574,7 +626,7 @@ class GraphedFrame(_Captured):
         self.pc.face_center = self.pc.face_orien_mat = self.pc.face_scaling = None
         if self.flame is not None:
             self.pc.verts_cano = None
-        self.image = self.radii = self.viewspace_points = self.loss = None
+        self.image = self.radii = self.viewspace_points = self.loss = self.alpha = self.depth = None
 
     def _before_capture(self):
         if self.optimizer is not None:

@@ -3,6 +3,8 @@ CUDA launches behind the same C ABI:
 
   photometric_loss(image, gt, lambda_dssim)   <- l1_loss * (1 - lambda) + (1 - ssim) * lambda
                                                  (utils/loss_utils.py:17-18,36-63, train.py:131-132)
+  composite_rgba(rgba_u8, bg)                 <- the loader's RGBA composite onto the background, and the alpha
+                                                 mask it drops (scene/__init__.py:48-51)
   image_metrics(render, gt_u8)                <- clamp + l1_loss, psnr, ssim of one val / test view (train.py:277-288)
                                                  and metrics.py:71-74 (evaluation, forward only)
   Adam(param_groups, lr, betas, eps)          <- torch.optim.Adam(l, lr=0.0, eps=1e-15).step()
@@ -74,6 +76,65 @@ def photometric_loss(image: torch.Tensor, gt: torch.Tensor, lambda_dssim: float 
     returns the detached tensor [l1 mean, ssim mean, total] (for logging, train.py:159-166)."""
     total, parts = _PhotometricLoss.apply(image, gt, lambda_dssim)
     return (total, parts) if return_parts else total
+
+
+# ================================================================================================================
+# The loader's RGBA composite: a capture's decoded RGBA frames -> the uint8 ground truth and the alpha mask, one launch
+# ================================================================================================================
+def check_rgba(rgba_u8: torch.Tensor) -> int:
+    """The checks of composite_rgba; returns the number of frames (1 for an (H,W,4) frame)."""
+    if not isinstance(rgba_u8, torch.Tensor) or rgba_u8.dtype != torch.uint8 or rgba_u8.dim() not in (3, 4) or \
+            rgba_u8.shape[-1] != 4:
+        raise TypeError("rgba must be a uint8 (H, W, 4) or (K, H, W, 4) tensor, got "
+                        f"{getattr(rgba_u8, 'dtype', type(rgba_u8))} {tuple(getattr(rgba_u8, 'shape', ()))}")
+    if rgba_u8.device.type != "cuda":
+        raise RuntimeError("gaussianavatars_b200 has no CPU path: tensors must be CUDA tensors")
+    return 1 if rgba_u8.dim() == 3 else int(rgba_u8.shape[0])
+
+
+def launch_composite_rgba(rgba_u8: torch.Tensor, bg: torch.Tensor, gt_out: torch.Tensor,
+                          mask_out: Optional[torch.Tensor] = None):
+    """Enqueues gab200_composite_rgba on the current stream: rgba (H,W,4) / (K,H,W,4) uint8 -> gt_out (3,H,W) /
+    (K,3,H,W) uint8 and mask_out (1,H,W) / (K,1,H,W) uint8 (None: not written).  bg: 3 float32 on the device, read by
+    the kernel.  Capturable: it reads nothing on the host."""
+    views = check_rgba(rgba_u8)
+    device = rgba_u8.device
+    H, W = int(rgba_u8.shape[-3]), int(rgba_u8.shape[-2])
+    lead = () if rgba_u8.dim() == 3 else (views,)
+    for t, n, c in ((gt_out, "gt_out", 3), (mask_out, "mask_out", 1)):
+        if t is not None and (t.dtype != torch.uint8 or tuple(t.shape) != lead + (c, H, W) or t.device != device
+                              or not t.is_contiguous()):
+            raise ValueError(f"{n} must be a contiguous uint8 {lead + (c, H, W)} tensor on {device}")
+    if bg.dtype != torch.float32 or bg.numel() != 3 or bg.device != device or not bg.is_contiguous():
+        raise ValueError(f"bg must be 3 contiguous float32 values on {device}")
+    src = rgba_u8 if rgba_u8.is_contiguous() else rgba_u8.contiguous()
+    with torch.cuda.device(device):
+        stream = torch.cuda.current_stream(device).cuda_stream
+        N.check(N.lib().gab200_composite_rgba(views, H, W, src.data_ptr(), bg.data_ptr(), gt_out.data_ptr(),
+                                              N.ptr(mask_out), C.c_void_p(stream)), "gab200_composite_rgba")
+    return gt_out, mask_out
+
+
+@torch.no_grad()
+def composite_rgba(rgba_u8: torch.Tensor, bg) -> tuple:
+    """(gt_u8, mask_u8) of decoded RGBA capture frames, computed on the device: what the reference's loader
+    (CameraDataset.__getitem__, scene/__init__.py:48-51) makes of `np.array(Image.open(p).convert("RGBA"))` on the
+    host, bit for bit, plus the alpha channel it throws away.
+
+    rgba_u8: a CUDA uint8 (H, W, 4) frame or (K, H, W, 4) frames.  bg: the camera's background (3 values, 0 or 1 per
+    channel in the reference; other colours go through the same formula).  Returns the uint8 ground truth (3, H, W) /
+    (K, 3, H, W) -- trunc((c/255 * a/255 + bg * (1 - a/255)) * 255) in float64, the loader's bytes -- and the alpha
+    bytes (1, H, W) / (K, 1, H, W), the foreground mask (value/255) of a mask loss."""
+    views = check_rgba(rgba_u8)
+    device = rgba_u8.device
+    H, W = int(rgba_u8.shape[-3]), int(rgba_u8.shape[-2])
+    lead = () if rgba_u8.dim() == 3 else (views,)
+    b = torch.as_tensor(bg, dtype=torch.float32).reshape(-1).to(device).contiguous()
+    if b.numel() != 3:
+        raise ValueError(f"bg must hold 3 values, got {b.numel()}")
+    gt = torch.empty(lead + (3, H, W), dtype=torch.uint8, device=device)
+    mask = torch.empty(lead + (1, H, W), dtype=torch.uint8, device=device)
+    return launch_composite_rgba(rgba_u8, b, gt, mask)
 
 
 # ================================================================================================================

@@ -413,6 +413,17 @@ int32_t gab200_l1_loss_u8(int64_t n, const float* img, const uint8_t* gt, float*
 int32_t gab200_l1_loss_u8_backward(int64_t n, const float* img, const uint8_t* gt, const float* upstream, float* grad,
                                    void* stream);
 
+/* The ground truth the reference's loader makes from a capture's RGBA frame (CameraDataset.__getitem__,
+ * scene/__init__.py:48-51), in one launch: for every colour byte c and alpha byte a of `views` interleaved
+ * [height, width, 4] uint8 frames,
+ *   rgb_out = trunc((c / 255.0 * (a / 255.0) + bg[ch] * (1 - a / 255.0)) * 255.0)
+ * evaluated in double precision in exactly that order (no contraction), written planar as [views, 3, height, width]
+ * uint8 -- the loader's bytes, bit for bit -- and mask_out = a as [views, 1, height, width] uint8 (may be NULL).
+ * bg: 3 floats in device memory, read on every launch.  The loader's backgrounds are 0 or 1 per channel; any other
+ * colour goes through the same formula (converted to double), which the loader would give for that colour as well. */
+int32_t gab200_composite_rgba(int64_t views, int32_t height, int32_t width, const uint8_t* rgba, const float* bg,
+                              uint8_t* rgb_out, uint8_t* mask_out, void* stream);
+
 /* Photometric training loss of the reference with its gradient, in two launches (SURVEY.md 8f rank 2):
  *   total = (1 - lambda_dssim) * mean|img - gt| + lambda_dssim * (1 - mean SSIM(img, gt))
  * Replaces `l1_loss(image, gt) * (1 - lambda)` + `(1 - ssim(image, gt)) * lambda` and their autograd
