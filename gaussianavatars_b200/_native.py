@@ -217,7 +217,8 @@ EXPORTED_SYMBOLS = ("gab200_forward", "gab200_backward", "gab200_mark_visible", 
                     "gab200_mesh_scratch_bytes", "gab200_forward_views", "gab200_forward_views_train",
                     "gab200_backward_views", "gab200_forward_depth_alpha", "gab200_backward_depth_alpha",
                     "gab200_forward_views_depth_alpha", "gab200_forward_views_train_depth_alpha",
-                    "gab200_backward_views_depth_alpha", "gab200_composite_rgba")
+                    "gab200_backward_views_depth_alpha", "gab200_composite_rgba",
+                    "gab200_frame_encode_plan", "gab200_frame_encode", "gab200_frame_decode")
 
 _lib = None
 _lock = threading.Lock()
@@ -313,6 +314,15 @@ def lib():
         L.gab200_composite_rgba.restype = C.c_int32
         L.gab200_composite_rgba.argtypes = [C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                             C.c_void_p, C.c_void_p]
+        L.gab200_frame_encode_plan.restype = C.c_int32
+        L.gab200_frame_encode_plan.argtypes = [C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                               C.c_void_p]
+        L.gab200_frame_encode.restype = C.c_int32
+        L.gab200_frame_encode.argtypes = [C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gab200_frame_decode.restype = C.c_int32
+        L.gab200_frame_decode.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gab200_photometric_loss.restype = C.c_int32
         L.gab200_photometric_loss.argtypes = [C.POINTER(PhotometricArgs), C.c_void_p]
         L.gab200_image_metrics.restype = C.c_int32

@@ -33,6 +33,7 @@ SOURCES = {
     "flame.cu": [],
     "loss.cu": [],
     "composite.cu": [],
+    "frames.cu": [],
     "metrics.cu": [],
     "mesh.cu": ["--fmad=false"],
     "optim.cu": [],

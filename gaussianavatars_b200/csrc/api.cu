@@ -1029,6 +1029,37 @@ int32_t gab200_composite_rgba(int64_t views, int32_t height, int32_t width, cons
   return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
 }
 
+int32_t gab200_frame_encode_plan(int64_t frames, int32_t height, int32_t width, const uint8_t* gt, const uint8_t* mask,
+                                 uint32_t* record_units, void* stream_) {
+  if (frames < 0 || height < 0 || width < 0) return GAB200_ERR_INVALID_ARGUMENT;
+  if (frames * height * width > 0 && (!gt || !record_units)) return GAB200_ERR_INVALID_ARGUMENT;
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  if (height > 0 && width > 0) launch_frame_encode_plan(frames, height, width, gt, mask, record_units, (cudaStream_t)stream_);
+  return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
+int32_t gab200_frame_encode(int64_t frames, int32_t height, int32_t width, const uint8_t* gt, const uint8_t* mask,
+                            const int64_t* frame_base, const uint32_t* tile_off, uint8_t* arena, void* stream_) {
+  if (frames < 0 || height < 0 || width < 0) return GAB200_ERR_INVALID_ARGUMENT;
+  if (frames * height * width > 0 && (!gt || !frame_base || !tile_off || !arena)) return GAB200_ERR_INVALID_ARGUMENT;
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  if (height > 0 && width > 0)
+    launch_frame_encode(frames, height, width, gt, mask, frame_base, tile_off, arena, (cudaStream_t)stream_);
+  return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
+int32_t gab200_frame_decode(int32_t views, int32_t height, int32_t width, const int32_t* ids, const uint8_t* arena,
+                            const int64_t* frame_base, const uint32_t* tile_off, uint8_t* gt_out, uint8_t* mask_out,
+                            void* stream_) {
+  if (views < 0 || height < 0 || width < 0) return GAB200_ERR_INVALID_ARGUMENT;
+  if ((int64_t)views * height * width > 0 && (!ids || !arena || !frame_base || !tile_off || !gt_out))
+    return GAB200_ERR_INVALID_ARGUMENT;
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  if (height > 0 && width > 0)
+    launch_frame_decode(views, height, width, ids, arena, frame_base, tile_off, gt_out, mask_out, (cudaStream_t)stream_);
+  return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
 int32_t gab200_photometric_loss(const gab200_photometric_args* a, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   if (a == nullptr || a->abi_version != GAB200_ABI_VERSION || a->channels < 0 || a->height < 0 || a->width < 0 ||

@@ -269,6 +269,15 @@ void launch_photometric_loss(int C, int H, int W, const float* img, const void* 
 void launch_composite_rgba(int64_t views, int H, int W, const uint8_t* rgba, const float* bg, uint8_t* rgb,
                            uint8_t* mask, cudaStream_t stream);
 
+// frames.cu
+int frame_tiles(int H, int W);
+void launch_frame_encode_plan(int64_t frames, int H, int W, const uint8_t* gt, const uint8_t* mask, uint32_t* units,
+                              cudaStream_t stream);
+void launch_frame_encode(int64_t frames, int H, int W, const uint8_t* gt, const uint8_t* mask,
+                         const int64_t* frame_base, const uint32_t* tile_off, uint8_t* arena, cudaStream_t stream);
+void launch_frame_decode(int views, int H, int W, const int32_t* ids, const uint8_t* arena, const int64_t* frame_base,
+                         const uint32_t* tile_off, uint8_t* gt, uint8_t* mask, cudaStream_t stream);
+
 // metrics.cu
 size_t metrics_scratch_bytes(int H, int W);
 void launch_image_metrics(int H, int W, int kind, const void* render, const uint8_t* gt, const int32_t* row, int rows,

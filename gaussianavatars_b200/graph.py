@@ -348,7 +348,7 @@ class GraphedFrame(_Captured):
                  headroom: float = 1.25, after_backward=None, warm_cameras=None, regularizers: Optional[dict] = None,
                  before_backward=None, side_work=None, side_work_at: str = "start", optimizer: Optional[Adam] = None,
                  densify_stats: bool = False, per_camera_fov: bool = False, views_per_replay: int = 1,
-                 rgba: bool = False, lambda_mask: float = 0.0):
+                 rgba: bool = False, lambda_mask: float = 0.0, frames=None):
         """loss: "l1_u8" (L1 vs a uint8 ground truth), "photometric" ((1-l) L1 + l (1-SSIM) vs a uint8 ground truth) or
         "dL_dimage" (the caller supplies dL/dimage in `self.dL_dimage`).
         host_inputs: the frame owns pinned STAGING tensors (`cam_stage` (35,) float32, `gt_stage` (3,H,W) uint8) that a
@@ -402,7 +402,21 @@ class GraphedFrame(_Captured):
         lambda_mask > 0 (needs rgba=True): the frame renders the alpha plane as well (render(depth_alpha=True)),
         exposes `alpha` and `depth`, and adds the foreground-mask term  K * lambda_mask * l1_loss_u8(alpha, mask),
         the sum over the views of lambda_mask * mean|alpha - mask/255|, to the loss before the regularisers.  Both
-        are construction constants: they never re-capture."""
+        are construction constants: they never re-capture.
+        frames=store (a frames.FrameStore of this frame's size, composited over this frame's bg): the ground truth and
+        the mask are decoded inside the graph, at the point where rgba=True composites them, from the store's frames
+        that `set_inputs(frames=...)` names -- K ids (an int when K = 1), each checked on the host against len(store)
+        and written to a device int32 table without a host wait.  gt_u8 / gt_rgba are refused; lambda_mask > 0 uses
+        the store's mask.  Only the camera table, the timestep and the K ids travel from the host per iteration; with
+        host_inputs the ids are staged in the pinned `frames_stage` ((K,) int32, written by stage_frames) and travel
+        beside cam_stage.  Changing ids never re-captures; a store that grew (its arena or index moved) does.  Not
+        combinable with rgba=True or loss='dL_dimage'."""
+        if frames is not None and rgba:
+            raise ValueError("frames= decodes the ground truth from the frame store: rgba=True composites it from an "
+                             "RGBA input instead; use one of them")
+        if frames is not None and loss == "dL_dimage":
+            raise ValueError("frames= decodes the ground truth of a scalar loss ('l1_u8' or 'photometric'): "
+                             "loss='dL_dimage' reads none")
         if loss not in ("l1_u8", "photometric", "dL_dimage"):
             raise ValueError("loss must be 'l1_u8', 'photometric' or 'dL_dimage'")
         if regularizers is not None and loss == "dL_dimage":
@@ -413,7 +427,7 @@ class GraphedFrame(_Captured):
         lambda_mask = float(lambda_mask)
         if not lambda_mask >= 0.0 or not math.isfinite(lambda_mask):
             raise ValueError(f"lambda_mask must be a finite value >= 0, got {lambda_mask}")
-        if lambda_mask > 0.0 and not rgba:
+        if lambda_mask > 0.0 and not rgba and frames is None:
             raise ValueError("the mask term compares the alpha plane with the capture's alpha: lambda_mask > 0 "
                              "needs rgba=True")
         if optimizer is not None and not (isinstance(optimizer, Adam) and
@@ -432,13 +446,21 @@ class GraphedFrame(_Captured):
         self.optimizer = optimizer
         self.densify_stats = bool(densify_stats)
         self.rgba, self.lambda_mask = bool(rgba), lambda_mask
+        self.frames = frames
         dev = self.device
+        if frames is not None:
+            self._check_store(frames)
         img = self._gt_shape()
         self.gt = torch.zeros(img, dtype=torch.uint8, device=dev) if loss != "dL_dimage" else None
         lead = () if self.K == 1 else (self.K,)
         # rgba: the static RGBA input the composite reads, and the mask it writes beside gt
         self.gt_rgba = torch.zeros(lead + (self.H, self.W, 4), dtype=torch.uint8, device=dev) if self.rgba else None
-        self.mask = torch.zeros(lead + (1, self.H, self.W), dtype=torch.uint8, device=dev) if self.rgba else None
+        self.mask = (torch.zeros(lead + (1, self.H, self.W), dtype=torch.uint8, device=dev)
+                     if self.rgba or frames is not None else None)
+        # frames: the device table of the K frame ids the decode reads (id 0 until set_inputs names others)
+        self.frame_ids = torch.zeros(self.K, dtype=torch.int32, device=dev) if frames is not None else None
+        self.frames_stage = (torch.zeros(self.K, dtype=torch.int32).pin_memory()
+                             if frames is not None and host_inputs else None)
         gt_in = self._gt_input()
         self.dL_dimage = torch.zeros(img, dtype=torch.float32, device=dev) if loss == "dL_dimage" else None
         self.cam_host = torch.zeros(self.cam.shape, dtype=torch.float32).pin_memory() if host_inputs else None  # staging
@@ -458,19 +480,59 @@ class GraphedFrame(_Captured):
         return (3, self.H, self.W) if self.K == 1 else (self.K, 3, self.H, self.W)
 
     def _gt_input(self):
-        """The device tensor the ground truth is written into: the RGBA frame(s) with rgba=True, else gt."""
+        """The device tensor the ground truth is written into: the RGBA frame(s) with rgba=True, else gt; None with a
+        frame store (the graph decodes gt itself)."""
+        if self.frames is not None:
+            return None
         return self.gt_rgba if self.rgba else self.gt
+
+    def _check_store(self, store):
+        from .frames import FrameStore
+        if not isinstance(store, FrameStore):
+            raise ValueError(f"frames must be a gaussianavatars_b200.FrameStore, got {type(store).__name__}")
+        if (store.W, store.H) != (self.W, self.H):
+            raise ValueError(f"the frame store holds {store.W}x{store.H} frames, this frame renders {self.W}x{self.H}")
+        if store.device != self.device:
+            raise ValueError(f"the frame store lives on {store.device}, this frame on {self.device}")
+        if not torch.equal(store.bg, self.bg):
+            raise ValueError(f"the frame store's frames are composited over {store.bg.tolist()}, this frame renders "
+                             f"over {self.bg.tolist()}: the backgrounds must be equal")
+        if len(store) == 0:
+            raise ValueError("the frame store holds no frames: add them before building the frame")
+
+    def _frame_list(self, frames) -> list:
+        """set_inputs' / stage_frames' ids: K ints (an int when K = 1), each checked against len(store)."""
+        if self.frames is None:
+            raise ValueError("frames= needs a GraphedFrame built with frames=store")
+        if isinstance(frames, int) and not isinstance(frames, bool) and self.K > 1:
+            raise ValueError(f"this frame trains {self.K} views per replay: give {self.K} frame ids")
+        ids = self.frames.check_ids(frames)
+        if len(ids) != self.K:
+            raise ValueError(f"this frame trains {self.K} views per replay, got {len(ids)} frame ids")
+        return ids
+
+    def stage_frames(self, frames):
+        """host_inputs: checks the ids and writes them into the pinned `frames_stage`, which the other frame of a
+        prefetching pair copies in its graph (or upload_staged).  The caller keeps the stage as it keeps cam_stage:
+        not rewritten while a replay that copies it may be running."""
+        if self.frames_stage is None:
+            raise ValueError("stage_frames needs a frame built with frames=store and host_inputs=True")
+        self.frames_stage.copy_(torch.tensor(self._frame_list(frames), dtype=torch.int32))
 
     # ---- inputs ------------------------------------------------------------------------------------------------
     def set_inputs(self, camera=None, verts=None, gt_u8=None, dL_dimage=None, timestep=None, cameras=None,
-                   gt_rgba=None):
+                   gt_rgba=None, frames=None):
         """Copies new inputs into the static buffers (device tensors) / staging buffers (host_inputs).  `timestep`
         (a model with a FLAME head only) is a host int checked against the model's number of timesteps.
         views_per_replay=K > 1: `cameras` (K camera objects of the frame's image size, or a (K, 37) table) instead of
         `camera`; gt_u8 / dL_dimage are (K,3,H,W).  rgba=True: `gt_rgba`, the decoded uint8 RGBA frame (H,W,4) or
-        (K,H,W,4), instead of gt_u8."""
+        (K,H,W,4), instead of gt_u8.  frames=store: `frames`, the K frame ids to decode (an int when K = 1)."""
         if (camera is not None and self.K > 1) or (cameras is not None and self.K == 1):
             raise ValueError("a frame with views_per_replay > 1 takes cameras=, one with a single view camera=")
+        if (gt_u8 is not None or gt_rgba is not None) and self.frames is not None:
+            raise ValueError("this frame decodes its ground truth from the frame store: give frames=, not gt_u8 / "
+                             "gt_rgba")
+        ids = self._frame_list(frames) if frames is not None else None
         if gt_u8 is not None and self.rgba:
             raise ValueError("this frame composites its ground truth from the RGBA frame: give gt_rgba=, not gt_u8")
         if gt_rgba is not None:
@@ -511,6 +573,15 @@ class GraphedFrame(_Captured):
                 dst.copy_(gt_src, non_blocking=True)
         if dL_dimage is not None:
             self.dL_dimage.copy_(dL_dimage, non_blocking=True)
+        if ids is not None:
+            if self._uploads:   # through the pinned stage, on the copy stream, like a host camera
+                self._side.synchronize()
+                self.stage_frames(ids)
+                self._upload(self.frame_ids, self.frames_stage)
+            elif self.K == 1:   # a fill, like the timestep
+                self.frame_ids.fill_(ids[0])
+            else:   # a pinned block of the caching allocator: the copy does not wait on the host
+                self.frame_ids.copy_(torch.tensor(ids, dtype=torch.int32).pin_memory(), non_blocking=True)
 
     def prefetch_for(self, other: "GraphedFrame"):
         """This frame's graph will, on a forked branch, copy `other`'s pinned staging tensors (cam_stage, gt_stage)
@@ -524,6 +595,9 @@ class GraphedFrame(_Captured):
         if self.rgba != other.rgba:
             raise ValueError("both frames of a prefetching pair must take the same ground truth (rgba=True on both "
                              "or on neither)")
+        if (self.frames is None) != (other.frames is None):
+            raise ValueError("both frames of a prefetching pair must take the same ground truth (frames= on both or "
+                             "on neither)")
         self._prefetch_target = other
         return self
 
@@ -532,6 +606,8 @@ class GraphedFrame(_Captured):
         self.cam.copy_(self.cam_stage, non_blocking=True)
         if self.gt_stage is not None:
             self._gt_input().copy_(self.gt_stage, non_blocking=True)
+        if self.frames_stage is not None:
+            self.frame_ids.copy_(self.frames_stage, non_blocking=True)
 
     # ---- the step body (run eagerly for warm-up, then captured) --------------------------------------------------
     def _params(self):
@@ -559,6 +635,8 @@ class GraphedFrame(_Captured):
                     other.cam.copy_(other.cam_stage, non_blocking=True)
                     if other.gt_stage is not None:
                         other._gt_input().copy_(other.gt_stage, non_blocking=True)
+                    if other.frames_stage is not None:
+                        other.frame_ids.copy_(other.frames_stage, non_blocking=True)
                 if self.side_work is not None and self.side_work_at == "start":
                     self.side_work()
         self._pose()
@@ -571,6 +649,8 @@ class GraphedFrame(_Captured):
         radii_rows = [out["radii"]] if self.K == 1 else list(out["radii"])
         if self.rgba:   # the loader's composite of the RGBA input: gt and mask for this replay's loss
             launch_composite_rgba(self.gt_rgba, self.bg, self.gt, self.mask)
+        elif self.frames is not None:   # the same gt and mask, decoded from the store's frames of the device ids
+            self.frames.launch_decode(self.frame_ids, self.gt, self.mask)
         if self.loss_kind in ("l1_u8", "photometric"):
             loss = l1_loss_u8(img, self.gt) if self.loss_kind == "l1_u8" else photometric_loss(img, self.gt, self.lambda_dssim)
             if self.K > 1:   # one mean over the K images: K x it is the sum of the per-view losses
@@ -641,11 +721,14 @@ class GraphedFrame(_Captured):
     def _state_key(self):
         """Everything a training capture baked in that eager code between replays may replace: beyond the shared key,
         which FLAME tensors receive gradients, the statistics, every group's hyper-parameters and the addresses of
-        every moment and step.  None for a frame that neither trains nor poses a FLAME head: it never re-captures."""
+        every moment and step, and with a frame store the addresses of its arena and index.  None for a frame that
+        neither trains, poses a FLAME head nor reads a store: it never re-captures."""
         pc = self.pc
-        if self.optimizer is None and not self.densify_stats and self.flame is None:
+        if self.optimizer is None and not self.densify_stats and self.flame is None and self.frames is None:
             return None
         key = super()._state_key()
+        if self.frames is not None:
+            key.append(self.frames.pointers())
         if self.flame is not None:
             key += [t is not None and t.requires_grad for t in map(pc.flame_param.get, _FLAME_KEYS)]
         if self.densify_stats:

@@ -424,6 +424,30 @@ int32_t gab200_l1_loss_u8_backward(int64_t n, const float* img, const uint8_t* g
 int32_t gab200_composite_rgba(int64_t views, int32_t height, int32_t width, const uint8_t* rgba, const float* bg,
                               uint8_t* rgb_out, uint8_t* mask_out, void* stream);
 
+/* The tile-packed lossless frame store (csrc/frames.cu, gaussianavatars_b200.frames.FrameStore): a frame is four
+ * uint8 planes -- R, G, B of the composited ground truth, M its alpha (255 without a mask) -- coded per 16x16 tile
+ * (row-major, edge-replicated) and plane as base = v(0,0), the mod-256 2-D difference d(y,x) = q(y,x) - q(y,x-1) -
+ * q(y-1,x) + q(y-1,x-1) of q = v - base, zigzagged into b bits (b = bit length of the tile's largest residual).
+ * Record, 8-byte aligned: 4 bases | uint16 of the 4 widths (plane p in bits 4p..4p+3) | 2 zero bytes | R, G, B, M
+ * payloads of 32 b bytes (value 16 y + x at bits [i b, i b + b) of a little-endian bit stream): 8 + 32 sum(b) bytes.
+ * Index: frame_base[f] (int64, byte offset into the arena), tile_off[f * n_tiles + t] (uint32, 8-byte units from the
+ * frame's base).  n_tiles = ceil(height/16) * ceil(width/16).
+ *
+ * Plan: the record size, in 8-byte units, of every tile of `frames` frames gt [frames, 3, height, width] and mask
+ * [frames, 1, height, width] (NULL: 255) -> record_units[frames * n_tiles]. */
+int32_t gab200_frame_encode_plan(int64_t frames, int32_t height, int32_t width, const uint8_t* gt, const uint8_t* mask,
+                                 uint32_t* record_units, void* stream);
+/* Encode: the same frames' records, tile t of frame f at arena + frame_base[f] + 8 * tile_off[f * n_tiles + t] (the
+ * caller's scan of the planned sizes; frame_base / tile_off here are the rows of the frames being encoded). */
+int32_t gab200_frame_encode(int64_t frames, int32_t height, int32_t width, const uint8_t* gt, const uint8_t* mask,
+                            const int64_t* frame_base, const uint32_t* tile_off, uint8_t* arena, void* stream);
+/* Decode frames ids[0 .. views) (a device int32 table) -> gt_out [views, 3, height, width] and mask_out [views, 1,
+ * height, width] (NULL: not written).  Reads nothing on the host: capturable.  The ids are not checked on the device:
+ * each must index a frame of the arena. */
+int32_t gab200_frame_decode(int32_t views, int32_t height, int32_t width, const int32_t* ids, const uint8_t* arena,
+                            const int64_t* frame_base, const uint32_t* tile_off, uint8_t* gt_out, uint8_t* mask_out,
+                            void* stream);
+
 /* Photometric training loss of the reference with its gradient, in two launches (SURVEY.md 8f rank 2):
  *   total = (1 - lambda_dssim) * mean|img - gt| + lambda_dssim * (1 - mean SSIM(img, gt))
  * Replaces `l1_loss(image, gt) * (1 - lambda)` + `(1 - ssim(image, gt)) * lambda` and their autograd
