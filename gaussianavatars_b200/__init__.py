@@ -9,6 +9,7 @@ from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, rast
 from .renderer import render, render_bound, render_display, render_views, render_views_train
 from .training import photometric_loss, image_metrics, Adam, binding_regularizers, expon_lr_schedule, composite_rgba
 from .frames import FrameStore
+from .schedule import ViewSchedule, epoch_order
 from .io import load_ply, save_ply, load_flame_param, save_flame_param
 from .densify import densify_and_prune, densify_arrays, add_densification_stats
 from .flame import FlameLBS, flame_pose, flame_param_groups
@@ -19,4 +20,5 @@ __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gau
            "render_views_train",
            "photometric_loss", "image_metrics", "Adam", "binding_regularizers", "load_ply", "save_ply", "load_flame_param", "save_flame_param", "densify_and_prune", "densify_arrays",
            "add_densification_stats", "expon_lr_schedule", "FlameLBS", "flame_pose", "flame_param_groups",
-           "mesh_overlay", "MeshRenderer", "composite_rgba", "FrameStore"]
+           "mesh_overlay", "MeshRenderer", "composite_rgba", "FrameStore",
+           "ViewSchedule", "epoch_order"]

@@ -218,7 +218,8 @@ EXPORTED_SYMBOLS = ("gab200_forward", "gab200_backward", "gab200_mark_visible", 
                     "gab200_backward_views", "gab200_forward_depth_alpha", "gab200_backward_depth_alpha",
                     "gab200_forward_views_depth_alpha", "gab200_forward_views_train_depth_alpha",
                     "gab200_backward_views_depth_alpha", "gab200_composite_rgba",
-                    "gab200_frame_encode_plan", "gab200_frame_encode", "gab200_frame_decode")
+                    "gab200_frame_encode_plan", "gab200_frame_encode", "gab200_frame_decode",
+                    "gab200_schedule_sample", "gab200_schedule_commit")
 
 _lib = None
 _lock = threading.Lock()
@@ -323,6 +324,10 @@ def lib():
         L.gab200_frame_decode.restype = C.c_int32
         L.gab200_frame_decode.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gab200_schedule_sample.restype = C.c_int32
+        L.gab200_schedule_sample.argtypes = [C.c_int32, C.c_int32, C.c_int32] + [C.c_void_p] * 11
+        L.gab200_schedule_commit.restype = C.c_int32
+        L.gab200_schedule_commit.argtypes = [C.c_int32] + [C.c_void_p] * 6
         L.gab200_photometric_loss.restype = C.c_int32
         L.gab200_photometric_loss.argtypes = [C.POINTER(PhotometricArgs), C.c_void_p]
         L.gab200_image_metrics.restype = C.c_int32

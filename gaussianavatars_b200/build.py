@@ -34,6 +34,7 @@ SOURCES = {
     "loss.cu": [],
     "composite.cu": [],
     "frames.cu": [],
+    "schedule.cu": [],
     "metrics.cu": [],
     "mesh.cu": ["--fmad=false"],
     "optim.cu": [],

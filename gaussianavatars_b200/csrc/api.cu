@@ -1060,6 +1060,28 @@ int32_t gab200_frame_decode(int32_t views, int32_t height, int32_t width, const 
   return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
 }
 
+int32_t gab200_schedule_sample(int32_t records, int32_t views, int32_t length, const float* cams,
+                               const int32_t* timesteps, const int32_t* frame_ids, const int32_t* order,
+                               const int32_t* cursor, float* cam_out, int32_t* timestep_out, int32_t* ids_out,
+                               int32_t* rows_out, int32_t* exhausted, void* stream_) {
+  if (records < 1 || views < 1 || views > 65535 || length < 1 || (int64_t)records * views > INT32_MAX)
+    return GAB200_ERR_INVALID_ARGUMENT;
+  if (!cams || !order || !cursor || !cam_out || !exhausted) return GAB200_ERR_INVALID_ARGUMENT;
+  if ((timestep_out && !timesteps) || (ids_out && !frame_ids)) return GAB200_ERR_INVALID_ARGUMENT;
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  launch_schedule_sample(records, views, length, cams, timesteps, frame_ids, order, cursor, cam_out, timestep_out,
+                         ids_out, rows_out, exhausted, (cudaStream_t)stream_);
+  return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
+int32_t gab200_schedule_commit(int32_t length, const int32_t* overflow_flag, const int32_t* exhausted,
+                               const float* loss, float* losses, int32_t* cursor, void* stream_) {
+  if (length < 1 || !exhausted || !cursor || (losses && !loss)) return GAB200_ERR_INVALID_ARGUMENT;
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  launch_schedule_commit(length, overflow_flag, exhausted, loss, losses, cursor, (cudaStream_t)stream_);
+  return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
 int32_t gab200_photometric_loss(const gab200_photometric_args* a, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   if (a == nullptr || a->abi_version != GAB200_ABI_VERSION || a->channels < 0 || a->height < 0 || a->width < 0 ||

@@ -278,6 +278,14 @@ void launch_frame_encode(int64_t frames, int H, int W, const uint8_t* gt, const 
 void launch_frame_decode(int views, int H, int W, const int32_t* ids, const uint8_t* arena, const int64_t* frame_base,
                          const uint32_t* tile_off, uint8_t* gt, uint8_t* mask, cudaStream_t stream);
 
+// schedule.cu
+void launch_schedule_sample(int records, int views, int length, const float* cams, const int32_t* timesteps,
+                            const int32_t* frame_ids, const int32_t* order, const int32_t* cursor, float* cam_out,
+                            int32_t* timestep_out, int32_t* ids_out, int32_t* rows_out, int32_t* exhausted,
+                            cudaStream_t stream);
+void launch_schedule_commit(int length, const int32_t* overflow_flag, const int32_t* exhausted, const float* loss,
+                            float* losses, int32_t* cursor, cudaStream_t stream);
+
 // metrics.cu
 size_t metrics_scratch_bytes(int H, int W);
 void launch_image_metrics(int H, int W, int kind, const void* render, const uint8_t* gt, const int32_t* row, int rows,

@@ -39,6 +39,7 @@ re-captures.  The gradients reach the FLAME tensors, and a capturable `Adam` hol
 """
 from __future__ import annotations
 
+import ctypes as C
 import math
 from typing import Optional
 
@@ -146,6 +147,7 @@ class _Captured:
     `_state_key()` with what only its own capture bakes in."""
 
     K = 1   # cameras per replay (views_per_replay); a subclass sets it before __init__
+    schedule = None   # a schedule.ViewSchedule the replays follow (_use_schedule)
 
     def __init__(self, pc, width, height, fovx, fovy, bg, per_camera_fov, capacity, headroom, warm_cameras,
                  warm_timesteps=None, verts_grad=False):
@@ -171,6 +173,7 @@ class _Captured:
             self.timestep = None
         self._warm = None if warm_cameras is None else [self._camera_tensor(c) for c in warm_cameras]
         self._warm_t = None if warm_timesteps is None or self.flame is None else [int(t) for t in warm_timesteps]
+        self._warm_pairs = None   # (block, timestep) pairs rendered in place of the warm cameras x warm timesteps
         self.graph = self.slot = self._key = None
         self.replays = self.captures = 0
         self._side = None                    # copy stream of host-input uploads (a subclass creates it)
@@ -245,9 +248,11 @@ class _Captured:
             hints, key = R.hints_of(self.pc), (self.device, self.W, self.H, self.pc._xyz.shape[0])
         n_max, lo, hi = 0, 0xFFFFFFFF, 0
         cam0 = self.cam.clone()
-        t0 = self.timestep.clone() if self._warm_t else None
+        pairs = self._warm_pairs
+        t0 = self.timestep.clone() if self._warm_t or (pairs and self.timestep is not None) else None
         blocks = self._warm if self._warm else [cam0]
         steps = self._warm_t if self._warm_t else [None]
+        runs = pairs if pairs else [(blk, t) for blk in blocks for t in steps]
         # eager frames on a side stream (torch's recipe for whole-step capture): nothing autograd creates here may be
         # tied to the legacy default stream
         cur = torch.cuda.current_stream(self.device)
@@ -255,16 +260,15 @@ class _Captured:
         side.wait_stream(cur)
         with torch.cuda.stream(side):
             for rep in range(2):
-                for blk in blocks:
-                    for t in steps:
-                        self.cam.copy_(blk)
-                        if t is not None:
-                            self.timestep.fill_(t)
-                        self._body()
-                        n_max = max(n_max, int((hints.last or {}).get("num_rendered", 0)))
-                        d = hints.get(key)[1]
-                        if d[1] > d[0]:  # union of the (already widened) depth-key ranges: one bucket grid fits all
-                            lo, hi = min(lo, d[0]), max(hi, d[1])
+                for blk, t in runs:
+                    self.cam.copy_(blk)
+                    if t is not None:
+                        self.timestep.fill_(t)
+                    self._body()
+                    n_max = max(n_max, int((hints.last or {}).get("num_rendered", 0)))
+                    d = hints.get(key)[1]
+                    if d[1] > d[0]:  # union of the (already widened) depth-key ranges: one bucket grid fits all
+                        lo, hi = min(lo, d[0]), max(hi, d[1])
         cur.wait_stream(side)
         # the frame's own camera and timestep again: the captured frame must not render the last warm-up one
         self.cam.copy_(cam0)
@@ -317,6 +321,114 @@ class _Captured:
         frame whose key is None never re-captures."""
         return self.graph is None or (self._key is not None and self._state_key() != self._key)
 
+    def _check_store(self, store):
+        from .frames import FrameStore
+        if not isinstance(store, FrameStore):
+            raise ValueError(f"frames must be a gaussianavatars_b200.FrameStore, got {type(store).__name__}")
+        if (store.W, store.H) != (self.W, self.H):
+            raise ValueError(f"the frame store holds {store.W}x{store.H} frames, this frame renders {self.W}x{self.H}")
+        if store.device != self.device:
+            raise ValueError(f"the frame store lives on {store.device}, this frame on {self.device}")
+        if not torch.equal(store.bg, self.bg):
+            raise ValueError(f"the frame store's frames are composited over {store.bg.tolist()}, this frame renders "
+                             f"over {self.bg.tolist()}: the backgrounds must be equal")
+        if len(store) == 0:
+            raise ValueError("the frame store holds no frames: add them before building the frame")
+
+    # ---- a device-resident view schedule (schedule.ViewSchedule) ---------------------------------------------------
+    def _use_schedule(self, schedule, store, log: bool):
+        """Checks `schedule` against this frame and creates what the frame owns to follow it: the device `cursor`
+        (the iteration the next replay runs), the `exhausted` word the sampler raises past the end of the order and,
+        with log, the `losses` log ((L,) float32, NaN until its iteration commits).  Without warm cameras, the warm-up
+        renders up to 16 records spread over the table, each at its own timestep."""
+        from .schedule import ViewSchedule
+        if not isinstance(schedule, ViewSchedule):
+            raise ValueError(f"schedule must be a gaussianavatars_b200.ViewSchedule, got {type(schedule).__name__}")
+        schedule.check_for(type(self).__name__, self.W, self.H, self.K, self.device,
+                           self.num_timesteps if self.flame is not None else None, store)
+        if self.flame is None and self.verts is not None:
+            raise ValueError("this model is posed by host vertices: a schedule poses the model from its timesteps, "
+                             "which needs a FLAME head (pc.flame), or a model without a mesh")
+        self.schedule = schedule
+        dev = self.device
+        self.cursor = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.exhausted = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.losses = torch.full((schedule.L,), float("nan"), dtype=torch.float32, device=dev) if log else None
+        self._cursor_host = self._pending = 0   # the cursor last read on the host, replays enqueued since
+        if self._warm is None:
+            ts = schedule.timesteps_host
+            self._warm_pairs = [(schedule.cams[r] if self.K > 1 else schedule.cams[r, 0], None if ts is None else ts[r])
+                                for r in schedule.warm_records()]
+
+    def set_cursor(self, i: int):
+        """The next replay runs iteration i of the schedule (resuming from a checkpoint; 0 rewinds).  Enqueued behind
+        the replays so far; clears the exhausted word."""
+        if self.schedule is None:
+            raise ValueError("set_cursor needs a frame built with schedule=")
+        i = int(i)
+        if not 0 <= i <= self.schedule.L:
+            raise IndexError(f"the cursor lies in [0, {self.schedule.L}], got {i}")
+        self.cursor.fill_(i)
+        self.exhausted.zero_()
+        self._cursor_host, self._pending = i, 0
+
+    def _launch_sample(self, ids=None, rows=None):
+        """gab200_schedule_sample: record order[cursor] -> the camera block, the timestep, `ids`, `rows`."""
+        s = self.schedule
+        stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        t_out = self.timestep if s.timesteps is not None else None
+        N.check(N.lib().gab200_schedule_sample(s.R, s.K, s.L, s.cams.data_ptr(), N.ptr(s.timesteps),
+                                               N.ptr(s.frame_ids), s.order.data_ptr(), self.cursor.data_ptr(),
+                                               self.cam.data_ptr(), N.ptr(t_out), N.ptr(ids), N.ptr(rows),
+                                               self.exhausted.data_ptr(), stream), "gab200_schedule_sample")
+
+    def _launch_commit(self, loss=None):
+        """gab200_schedule_commit: unless this replay overflowed (the slot's sticky flag) or found the schedule
+        exhausted, log `loss` at the cursor and advance it."""
+        stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        N.check(N.lib().gab200_schedule_commit(self.schedule.L, self.slot.flag.data_ptr(), self.exhausted.data_ptr(),
+                                               N.ptr(loss if self.losses is not None else None), N.ptr(self.losses),
+                                               self.cursor.data_ptr(), stream), "gab200_schedule_commit")
+
+    def _run_scheduled(self, n: int, check: bool):
+        """n replays of the schedule's next iterations.  Refused on the host when they could run past the end of the
+        order (the cursor last read plus the replays enqueued since: no sync).  check: one synchronisation, then the
+        cursor and the overflow flag; after an overflow, regrow() and replay the iterations that did not commit.
+        Returns the iterations committed since the cursor was last read (check=True), else None."""
+        if self.schedule is None:
+            raise ValueError("a scheduled run needs a frame built with schedule=")
+        n, L = int(n), self.schedule.L
+        if n < 0:
+            raise ValueError(f"the number of iterations must be >= 0, got {n}")
+        if self._cursor_host + self._pending + n > L:
+            raise ValueError(f"{n} more iterations could run past the schedule's {L}: the cursor reaches up to "
+                             f"{self._cursor_host + self._pending} (set_cursor rewinds)")
+        if self._stale():
+            self.capture()
+        for _ in range(n):
+            self._replay_scheduled()
+        self._pending += n
+        if not check:
+            return None
+        start, want, grown_at = self._cursor_host, self._cursor_host + self._pending, None
+        while True:
+            over = self.overflowed(wait=True)   # waits for the replays; then the cursor is a plain read
+            c = int(self.cursor.item())
+            if c == want:
+                break
+            if not over:
+                raise RuntimeError(f"{type(self).__name__}: the schedule's cursor stopped at {c} of {want} without an "
+                                   "overflow (exhausted: the cursor was moved past the order)")
+            if grown_at == c:
+                raise RuntimeError(f"{type(self).__name__}: iteration {c} still overflows its instance capacity after "
+                                   "re-capture")
+            grown_at = c
+            self.regrow()   # an overflowed replay and the ones behind it committed nothing: redo them from c
+            for _ in range(want - c):
+                self._replay_scheduled()
+        self._cursor_host, self._pending = want, 0
+        return want - start
+
     # ---- overflow --------------------------------------------------------------------------------------------------
     def overflowed(self, wait: bool = True) -> bool:
         """True if any replay since the last (re-)capture needed more than the captured capacity.  The sticky flag stays
@@ -348,7 +460,7 @@ class GraphedFrame(_Captured):
                  headroom: float = 1.25, after_backward=None, warm_cameras=None, regularizers: Optional[dict] = None,
                  before_backward=None, side_work=None, side_work_at: str = "start", optimizer: Optional[Adam] = None,
                  densify_stats: bool = False, per_camera_fov: bool = False, views_per_replay: int = 1,
-                 rgba: bool = False, lambda_mask: float = 0.0, frames=None):
+                 rgba: bool = False, lambda_mask: float = 0.0, frames=None, schedule=None):
         """loss: "l1_u8" (L1 vs a uint8 ground truth), "photometric" ((1-l) L1 + l (1-SSIM) vs a uint8 ground truth) or
         "dL_dimage" (the caller supplies dL/dimage in `self.dL_dimage`).
         host_inputs: the frame owns pinned STAGING tensors (`cam_stage` (35,) float32, `gt_stage` (3,H,W) uint8) that a
@@ -410,7 +522,26 @@ class GraphedFrame(_Captured):
         the store's mask.  Only the camera table, the timestep and the K ids travel from the host per iteration; with
         host_inputs the ids are staged in the pinned `frames_stage` ((K,) int32, written by stage_frames) and travel
         beside cam_stage.  Changing ids never re-captures; a store that grew (its arena or index moved) does.  Not
-        combinable with rgba=True or loss='dL_dimage'."""
+        combinable with rgba=True or loss='dL_dimage'.
+        schedule=s (a schedule.ViewSchedule): every captured replay runs the next iteration of the schedule by itself.
+        A sampler kernel at its head copies record order[cursor] -- the camera table, the timestep, the K frame ids --
+        into the frame's inputs, and a commit kernel at its end (after the optimizer step) logs the detached loss in
+        `losses[cursor]` and advances the device `cursor`, unless the replay overflowed its capacity.
+        run_iterations(n) enqueues n replays with no host input; set_cursor(i) resumes; loss_history(a, b) reads the
+        log.  The warm-up renders `warm_cameras` if given, else up to 16 records of the table at their own timesteps.
+        per_camera_fov is implied.  Refused: host_inputs, prefetch_for, loss='dL_dimage', rgba=True, a model posed by
+        host vertices, and set_inputs(camera=, cameras=, timestep=, frames=).  The cursor and the log survive a
+        re-capture (densify_and_prune, reset_opacity, oneupSHdegree between runs); the schedule never re-captures."""
+        if schedule is not None:
+            if host_inputs:
+                raise ValueError("schedule= samples the inputs on the device: host_inputs=True stages them on the host; "
+                                 "use one of them")
+            if loss == "dL_dimage":
+                raise ValueError("schedule= trains on a scalar loss ('l1_u8' or 'photometric'): loss='dL_dimage' "
+                                 "takes a host-written gradient")
+            if rgba:
+                raise ValueError("schedule= cannot feed rgba=True: nothing on the device holds the RGBA frames to "
+                                 "composite; add them to a FrameStore and give frames=store")
         if frames is not None and rgba:
             raise ValueError("frames= decodes the ground truth from the frame store: rgba=True composites it from an "
                              "RGBA input instead; use one of them")
@@ -435,8 +566,8 @@ class GraphedFrame(_Captured):
             raise ValueError("optimizer must be a gaussianavatars_b200.Adam with capturable=True")
         _check_views_per_replay(views_per_replay)
         self.K = int(views_per_replay)
-        super().__init__(pc, width, height, fovx, fovy, bg, per_camera_fov or self.K > 1, capacity, headroom,
-                         warm_cameras, verts_grad=True)
+        super().__init__(pc, width, height, fovx, fovy, bg, per_camera_fov or self.K > 1 or schedule is not None,
+                         capacity, headroom, warm_cameras, verts_grad=True)
         self.loss_kind, self.lambda_dssim, self.host_inputs = loss, float(lambda_dssim), bool(host_inputs)
         self.after_backward = after_backward
         self.before_backward = before_backward   # e.g. SymmetricGradBuffer.begin
@@ -475,6 +606,8 @@ class GraphedFrame(_Captured):
         self.image = self.radii = self.viewspace_points = self.alpha = self.depth = None
         self._side = torch.cuda.Stream(device=dev) if (host_inputs or side_work is not None) else None
         self._uploads = bool(host_inputs)
+        if schedule is not None:
+            self._use_schedule(schedule, frames, log=True)
 
     def _gt_shape(self):
         return (3, self.H, self.W) if self.K == 1 else (self.K, 3, self.H, self.W)
@@ -485,20 +618,6 @@ class GraphedFrame(_Captured):
         if self.frames is not None:
             return None
         return self.gt_rgba if self.rgba else self.gt
-
-    def _check_store(self, store):
-        from .frames import FrameStore
-        if not isinstance(store, FrameStore):
-            raise ValueError(f"frames must be a gaussianavatars_b200.FrameStore, got {type(store).__name__}")
-        if (store.W, store.H) != (self.W, self.H):
-            raise ValueError(f"the frame store holds {store.W}x{store.H} frames, this frame renders {self.W}x{self.H}")
-        if store.device != self.device:
-            raise ValueError(f"the frame store lives on {store.device}, this frame on {self.device}")
-        if not torch.equal(store.bg, self.bg):
-            raise ValueError(f"the frame store's frames are composited over {store.bg.tolist()}, this frame renders "
-                             f"over {self.bg.tolist()}: the backgrounds must be equal")
-        if len(store) == 0:
-            raise ValueError("the frame store holds no frames: add them before building the frame")
 
     def _frame_list(self, frames) -> list:
         """set_inputs' / stage_frames' ids: K ints (an int when K = 1), each checked against len(store)."""
@@ -527,6 +646,9 @@ class GraphedFrame(_Captured):
         views_per_replay=K > 1: `cameras` (K camera objects of the frame's image size, or a (K, 37) table) instead of
         `camera`; gt_u8 / dL_dimage are (K,3,H,W).  rgba=True: `gt_rgba`, the decoded uint8 RGBA frame (H,W,4) or
         (K,H,W,4), instead of gt_u8.  frames=store: `frames`, the K frame ids to decode (an int when K = 1)."""
+        if self.schedule is not None and any(x is not None for x in (camera, cameras, timestep, frames)):
+            raise ValueError("this frame samples its camera, timestep and frame ids from its schedule on the device: "
+                             "set_inputs(camera=, cameras=, timestep=, frames=) is refused (set_cursor moves it)")
         if (camera is not None and self.K > 1) or (cameras is not None and self.K == 1):
             raise ValueError("a frame with views_per_replay > 1 takes cameras=, one with a single view camera=")
         if (gt_u8 is not None or gt_rgba is not None) and self.frames is not None:
@@ -586,6 +708,8 @@ class GraphedFrame(_Captured):
     def prefetch_for(self, other: "GraphedFrame"):
         """This frame's graph will, on a forked branch, copy `other`'s pinned staging tensors (cam_stage, gt_stage)
         into `other`'s device inputs while it computes.  Call before capture()."""
+        if getattr(self, "schedule", None) is not None or getattr(other, "schedule", None) is not None:
+            raise ValueError("a frame with schedule= takes no host inputs: it cannot join a prefetching pair")
         if not (self.host_inputs and other.host_inputs):
             raise ValueError("prefetching needs host_inputs=True on both frames")
         if self.per_camera_fov != other.per_camera_fov:
@@ -625,6 +749,8 @@ class GraphedFrame(_Captured):
             p.grad = None
         if self.verts is not None:
             self.verts.grad = None
+        if captured and self.schedule is not None:   # this replay's record: camera table, timestep, frame ids
+            self._launch_sample(ids=self.frame_ids)
         other = self._prefetch_target
         forked = other is not None or self.side_work is not None
         if forked:   # forked branch: runs while this frame computes
@@ -690,6 +816,8 @@ class GraphedFrame(_Captured):
             self.loss_host.copy_(self.loss, non_blocking=True)
         if forked:   # join the branch (a captured fork must end inside the graph)
             torch.cuda.current_stream(self.device).wait_stream(self._side)
+        if captured and self.schedule is not None:   # log the loss and advance the cursor, unless this replay overflowed
+            self._launch_commit(self.loss)
         self.image, self.radii, self.viewspace_points = img.detach(), out["radii"], out["viewspace_points"]
         if planes:
             self.alpha, self.depth = out["alpha"].detach(), out["depth"].detach()
@@ -747,6 +875,9 @@ class GraphedFrame(_Captured):
 
     # ---- replay ----------------------------------------------------------------------------------------------------
     def run(self, check: bool = False):
+        if self.schedule is not None:   # one iteration of the schedule
+            self._run_scheduled(1, check)
+            return self
         if self._stale():
             self.capture()
         self._await_upload()   # a ground-truth upload in flight on the copy stream
@@ -767,6 +898,25 @@ class GraphedFrame(_Captured):
         for p, g in zip(self._params(), self.grads):
             p.grad = g
         self.pc.flat_grad = self.flat_grad
+
+    _replay_scheduled = _replay
+
+    def run_iterations(self, n: int, check: bool = True):
+        """schedule=: n training iterations of the schedule as n back-to-back replays, with no host input between
+        them (re-capturing first if the model changed).  Refused on the host, before anything runs, when they could
+        pass the end of the order.  check=True synchronises once at the end and reads the cursor and the overflow
+        flag: if a replay overflowed its capacity, it skipped its statistics, its Adam step and its commit, and so did
+        every replay behind it in the run (the sticky flag) -- wasted work, not wrong work; the frame then regrows and
+        replays from the record that overflowed.  Returns the number of iterations committed (n, when no unchecked
+        run came before); check=False returns None and reads nothing."""
+        return self._run_scheduled(n, check)
+
+    def loss_history(self, a: int = 0, b: Optional[int] = None) -> torch.Tensor:
+        """The logged losses of iterations a .. b - 1 of the schedule as a host tensor (one synchronisation); NaN for
+        an iteration not committed yet."""
+        if self.schedule is None:
+            raise ValueError("loss_history needs a frame built with schedule=")
+        return self.losses[a:b].cpu()
 
 
 class GraphedRender(_Captured):
@@ -1054,11 +1204,18 @@ class GraphedEval(GraphedRender):
 
     def __init__(self, pc, width: int, height: int, bg: torch.Tensor, views: int, source: str = "float",
                  host_slots: int = 0, capacity: Optional[int] = None, headroom: float = 1.25, warm_cameras=None,
-                 warm_timesteps=None, views_per_replay: int = 1):
+                 warm_timesteps=None, views_per_replay: int = 1, schedule=None, frames=None):
         """views_per_replay=K > 1: one replay renders K cameras of one timestep in one forward and scores them into
         rows view .. view + K - 1 (set_inputs(cameras=K cameras, gt_u8=(K,3,H,W), view=first row)); warm_cameras is a
         list of K-camera groups.  K is fixed per capture: a last group of fewer views is the business of a
-        single-view (or smaller) GraphedEval."""
+        single-view (or smaller) GraphedEval.
+        schedule=s with frames=store (a schedule.ViewSchedule of R records of K cameras, and the FrameStore its ids
+        index; views >= R * K): every replay runs the next record of the schedule with no host input.  A sampler kernel
+        copies record r = order[cursor] into the camera table, the timestep, the frame ids and the rows r * K ..
+        r * K + K - 1; the store's decode writes `gt`; the view is rendered and scored into those rows; a commit kernel
+        advances the cursor unless the replay overflowed.  run_all() scores the rest of the order; reset() also
+        rewinds the cursor; set_inputs is refused.  The warm-up renders `warm_cameras` if given, else up to 16 records
+        at their own timesteps."""
         if source not in ("float", "u8"):
             raise ValueError("source must be 'float' (train.py's evaluation of the float render) or 'u8' (the "
                              "display bytes render.py writes, scored as metrics.py reads them)")
@@ -1073,6 +1230,18 @@ class GraphedEval(GraphedRender):
                          views_per_replay=views_per_replay)
         self.source, self.views = source, int(views)
         self.table = torch.empty((self.views, N.METRICS_FIELDS), dtype=torch.float32, device=self.device)
+        self.frames = frames
+        self.frame_ids = None
+        if (schedule is None) != (frames is None):
+            raise ValueError("a GraphedEval scores a schedule's records against their frames: give schedule= and "
+                             "frames= together")
+        if schedule is not None:
+            self._check_store(frames)
+            self._use_schedule(schedule, frames, log=False)
+            if schedule.R * self.K > self.views:
+                raise ValueError(f"the schedule's {schedule.R} records of {self.K} views score {schedule.R * self.K} "
+                                 f"rows, the table has {self.views}")
+            self.frame_ids = torch.zeros(self.K, dtype=torch.int32, device=self.device)
         self.reset()
         self.view = torch.zeros(1, dtype=torch.int32, device=self.device)
         # K > 1: the rows of the replay's views, view + k, one device int32 each
@@ -1084,14 +1253,19 @@ class GraphedEval(GraphedRender):
         self._metrics_scratch = None
 
     def reset(self):
-        """Every row of the table back to NaN (no score)."""
+        """Every row of the table back to NaN (no score); with a schedule, the cursor back to its first record."""
         self.table.fill_(float("nan"))
+        if self.schedule is not None:
+            self.set_cursor(0)
 
     # ---- inputs ------------------------------------------------------------------------------------------------
     def set_inputs(self, camera=None, timestep=None, gt_u8=None, view=None, verts=None, bg=None, cameras=None):
         """As GraphedRender.set_inputs, plus the view's ground truth (uint8 (3,H,W), a device tensor or a pinned host
         tensor) and its row in the table (a host int in [0, views)).  None of them re-captures.  views_per_replay=K >
         1: `cameras` (K), gt_u8 (K,3,H,W), and `view` is the first of the K rows (view + K <= views)."""
+        if self.schedule is not None:
+            raise ValueError("this GraphedEval samples every input from its schedule on the device: set_inputs is "
+                             "refused (reset() or set_cursor() move it)")
         if view is not None:
             view = int(view)
             if not 0 <= view <= self.views - self.K:
@@ -1122,6 +1296,9 @@ class GraphedEval(GraphedRender):
 
     # ---- the frame body: the playback frame, then the metrics of what it rendered ------------------------------
     def _body(self, captured: bool = False):
+        if captured and self.schedule is not None:   # this replay's record, its rows, and its ground truth
+            self._launch_sample(ids=self.frame_ids, rows=self.view if self.K == 1 else self.rows)
+            self.frames.launch_decode(self.frame_ids, self.gt, None)
         super()._body(captured)
         if captured:   # the warm-up frames score nothing: they would write the current view's row
             rendered = self.image if self.source == "float" else self.display
@@ -1132,18 +1309,45 @@ class GraphedEval(GraphedRender):
                 for k in range(self.K):
                     launch_image_metrics(rendered[k], self.gt[k], self.table, row=self.rows[k:k + 1],
                                          skip_flag=self.slot.flag, scratch=self._metrics_scratch)
+            if self.schedule is not None:
+                self._launch_commit()
 
     def _before_capture(self):
         super()._before_capture()
         self._metrics_scratch = metrics_scratch(self.H, self.W, self.device)
 
+    def _state_key(self):
+        """Beyond a GraphedRender's key: with a frame store, the addresses of its arena and index."""
+        key = super()._state_key()
+        if self.frames is not None:
+            key.append(self.frames.pointers())
+        return key
+
     # ---- replay ----------------------------------------------------------------------------------------------------
     def run(self, check: bool = False):
+        if self.schedule is not None:   # the schedule's next record
+            self._run_scheduled(1, check)
+            return self
         self._await_upload()
         super().run(check)
         if self._side is not None:
             self._mark_read()
         return self
+
+    def _replay_scheduled(self):
+        self.graph.replay()
+        self.replays += 1
+        if self.host_slots:
+            self._ship()
+
+    def run_all(self, check: bool = True) -> Optional[int]:
+        """schedule=: scores every record of the order not scored yet, as back-to-back replays with no host input (R
+        replays after reset() with the identity order).  check=True synchronises once; a replay that overflowed its
+        capacity wrote no row and committed nothing, nor did the replays behind it, so the frame regrows and redoes
+        the records from the cursor on.  Returns the number of records scored (check=True), else None."""
+        if self.schedule is None:
+            raise ValueError("run_all needs a GraphedEval built with schedule= and frames=")
+        return self._run_scheduled(self.schedule.L - self._cursor_host - self._pending, check)
 
     def scores(self, n: Optional[int] = None) -> dict:
         """Synchronises once and returns the first n rows (default: all): `per_view`, a (n, 4) float32 host tensor

@@ -448,6 +448,25 @@ int32_t gab200_frame_decode(int32_t views, int32_t height, int32_t width, const 
                             const int64_t* frame_base, const uint32_t* tile_off, uint8_t* gt_out, uint8_t* mask_out,
                             void* stream);
 
+/* A device-resident view schedule (csrc/schedule.cu, gaussianavatars_b200.schedule.ViewSchedule): `records` records
+ * of `views` cameras each -- cams [records, views, GAB200_CAMERA_FLOATS] float32, timesteps [records] int32 (may be
+ * NULL), frame_ids [records, views] int32 (may be NULL) -- visited in the order order[0 .. length).  `cursor` is one
+ * device int32, the iteration the next replay runs.  Both launches read nothing on the host: capturable.
+ *
+ * Sample (one CTA, a plain launch): c = *cursor, r = order[c]; cam_out [views, GAB200_CAMERA_FLOATS] = cams[r],
+ * *timestep_out = timesteps[r], ids_out[k] = frame_ids[r * views + k], rows_out[k] = r * views + k (each output may
+ * be NULL: not written; timestep_out / ids_out need their table).  If c lies outside [0, length) or r outside
+ * [0, records), nothing is read or written but *exhausted = 1. */
+int32_t gab200_schedule_sample(int32_t records, int32_t views, int32_t length, const float* cams,
+                               const int32_t* timesteps, const int32_t* frame_ids, const int32_t* order,
+                               const int32_t* cursor, float* cam_out, int32_t* timestep_out, int32_t* ids_out,
+                               int32_t* rows_out, int32_t* exhausted, void* stream);
+/* Commit (one thread, a plain launch at the end of the replay): nothing if *overflow_flag (may be NULL) or *exhausted
+ * is set or *cursor lies outside [0, length); else losses[*cursor] = *loss (losses may be NULL: no log) and
+ * *cursor += 1. */
+int32_t gab200_schedule_commit(int32_t length, const int32_t* overflow_flag, const int32_t* exhausted,
+                               const float* loss, float* losses, int32_t* cursor, void* stream);
+
 /* Photometric training loss of the reference with its gradient, in two launches (SURVEY.md 8f rank 2):
  *   total = (1 - lambda_dssim) * mean|img - gt| + lambda_dssim * (1 - mean SSIM(img, gt))
  * Replaces `l1_loss(image, gt) * (1 - lambda)` + `(1 - ssim(image, gt)) * lambda` and their autograd
