@@ -408,13 +408,8 @@ int enqueue_geometry(Frame& f, bool bucket, bool run_preprocess, uint32_t capaci
     GAB_CUDA(cudaMemsetAsync(d.counts, 0, g.bucket_clear_bytes, stream));
     if (f.counting) GAB_CUDA(cudaMemsetAsync(f.iv.tile_count, 0, sizeof(uint32_t) * (size_t)tiles, stream));
     StageScope sc(GAB200_STAGE_PREPROCESS, stream);
-    if (f.cameras != nullptr)
-      launch_preprocess_views(*a, f.views, f.cameras, g.rec, g.aux, g.tiles_touched, g.depth_keys[0], g.ids[0],
-                              g.buckets, f.counting ? f.iv.tile_count : nullptr, f.nb ? g.clamped : nullptr, stream,
-                              f.da);
-    else
-      launch_preprocess(*a, g.rec, g.aux, g.tiles_touched, f.nb ? g.clamped : nullptr, g.depth_keys[0], g.ids[0],
-                        g.buckets, f.counting ? f.iv.tile_count : nullptr, f.tanfov, stream, f.da);
+    launch_preprocess(*a, f.views, f.cameras, f.tanfov, g.rec, g.aux, g.tiles_touched, f.nb ? g.clamped : nullptr,
+                      g.depth_keys[0], g.ids[0], g.buckets, f.counting ? f.iv.tile_count : nullptr, f.da, stream);
   }
   GAB_STAGE_CHECK(f.dbg, stream);
   if (f.counting && run_preprocess) {
@@ -543,24 +538,9 @@ int enqueue_binning_blend(Frame& f, void* bin, int64_t cap, int64_t n_known, siz
   st->sorted_selector = selector;
   {
     StageScope sc(GAB200_STAGE_BLEND_FWD, stream);
-    if (f.cameras != nullptr && f.da)
-      launch_blend_forward_views_depth(f.views, f.W, f.H, f.iv.ranges, f.iv.order, f.iv.order_info, bv.vals[selector],
-                                       f.g.rec, a->bg, a->out_color, f.nb ? f.iv.final_T : nullptr, f.iv.n_contrib,
-                                       bv.strip_mask, f.out_rgb8, f.out_alpha, f.out_depth, stream);
-    else if (f.cameras != nullptr && f.nb)
-      launch_blend_forward_views_train(f.views, f.W, f.H, f.iv.ranges, f.iv.order, f.iv.order_info, bv.vals[selector],
-                                       f.g.rec, a->bg, a->out_color, f.iv.final_T, f.iv.n_contrib, bv.strip_mask,
-                                       stream);
-    else if (f.da)
-      launch_blend_forward_depth(f.W, f.H, f.iv.ranges, f.iv.order, f.iv.order_info, bv.vals[selector], f.g.rec, a->bg,
-                                 a->out_color, f.iv.final_T, f.iv.n_contrib, bv.strip_mask, f.out_rgb8, f.out_alpha,
-                                 f.out_depth, stream);
-    else if (f.cameras != nullptr)
-      launch_blend_forward_views(f.views, f.W, f.H, f.iv.ranges, f.iv.order, f.iv.order_info, bv.vals[selector], f.g.rec,
-                                 a->bg, a->out_color, f.out_rgb8, stream);
-    else
-      launch_blend_forward(f.W, f.H, f.iv.ranges, f.iv.order, f.iv.order_info, bv.vals[selector], f.g.rec, a->bg,
-                           a->out_color, f.iv.final_T, f.iv.n_contrib, bv.strip_mask, f.out_rgb8, stream);
+    launch_blend_forward(f.views, f.W, f.H, f.iv.ranges, f.iv.order, f.iv.order_info, bv.vals[selector], f.g.rec, a->bg,
+                         a->out_color, f.iv.final_T, f.iv.n_contrib, bv.strip_mask, f.out_rgb8, f.out_alpha,
+                         f.out_depth, stream);
   }
   GAB_STAGE_CHECK(f.dbg, stream);
   return GAB200_OK;
@@ -810,23 +790,38 @@ int64_t gab200_forward_views_train_depth_alpha(const gab200_forward_args* a, int
   return run_forward(&v, nullptr, nullptr, st, stream, views, cameras, true, out_alpha, out_depth);
 }
 
-// gab200_backward_views, and gab200_backward_views_depth_alpha (da: the plane gradients, NULL = 0)
-static int32_t run_backward_views(const gab200_backward_args* b, int32_t views, const float* cameras, void* stream_,
-                                  bool da = false, const float* dL_dalpha = nullptr,
-                                  const float* dL_ddepth = nullptr) {
+// gab200_backward, gab200_backward_device_fov and gab200_backward_depth_alpha (cameras == NULL), and
+// gab200_backward_views[_depth_alpha] (`views` cameras); da: the plane gradients, NULL = 0
+static int32_t run_backward(const gab200_backward_args* b, const float* tanfov, int32_t views, const float* cameras,
+                            void* stream_, bool da = false, const float* dL_dalpha = nullptr,
+                            const float* dL_ddepth = nullptr) {
   cudaStream_t stream = (cudaStream_t)stream_;
   if (b == nullptr || b->abi_version != GAB200_ABI_VERSION || b->fwd == nullptr || b->state == nullptr)
     return GAB200_ERR_INVALID_ARGUMENT;
-  gab200_forward_args v;
-  if (!validate_views_train(b->fwd, views, cameras, v)) return GAB200_ERR_INVALID_ARGUMENT;
   const gab200_frame_state* st = b->state;
-  if (st->reserved0 != views || b->grads_are_multicast || b->dL_dout_color == nullptr) return GAB200_ERR_INVALID_ARGUMENT;
-  if (da && st->depth_prefix != 1u) return GAB200_ERR_INVALID_ARGUMENT;  // the records of a plain K-view frame carry no z
-  if (b->dL_dsh_dc == nullptr || (v.sh_coeffs > 1 && b->dL_dsh_rest == nullptr)) return GAB200_ERR_INVALID_ARGUMENT;
+  const gab200_forward_args* a = b->fwd;
+  gab200_forward_args v;  // a multi-view frame's arguments as its forward ran them
+  if (cameras != nullptr) {
+    if (!validate_views_train(b->fwd, views, cameras, v)) return GAB200_ERR_INVALID_ARGUMENT;
+    if (st->reserved0 != views || b->grads_are_multicast || b->dL_dout_color == nullptr)
+      return GAB200_ERR_INVALID_ARGUMENT;
+    if (da && st->depth_prefix != 1u) return GAB200_ERR_INVALID_ARGUMENT;  // the records of a plain K-view frame carry no z
+    if (b->dL_dsh_dc == nullptr || (v.sh_coeffs > 1 && b->dL_dsh_rest == nullptr)) return GAB200_ERR_INVALID_ARGUMENT;
+    a = &v;
+  } else {
+    if (!validate(a) || !a->need_backward || b->dL_dout_color == nullptr) return GAB200_ERR_INVALID_ARGUMENT;
+    if (st->reserved0 != 0) return GAB200_ERR_INVALID_ARGUMENT;  // a multi-view frame: gab200_backward_views
+    // the depth plane's backward reads z from the records: only a gab200_forward_depth_alpha state has it; plain stores
+    if (da && (st->depth_prefix != 1u || b->grads_are_multicast)) return GAB200_ERR_INVALID_ARGUMENT;
+    if (a->input_mode == GAB200_INPUT_BOUND_RAW && a->colors_precomp == nullptr &&
+        (b->dL_dsh_dc == nullptr || (a->sh_coeffs > 1 && b->dL_dsh_rest == nullptr)))
+      return GAB200_ERR_INVALID_ARGUMENT;
+  }
   if (st->geom_buffer == nullptr || st->image_buffer == nullptr || st->binning_buffer == nullptr)
     return GAB200_ERR_INVALID_ARGUMENT;
-  const int P = v.P, W = v.image_width, H = v.image_height;
-  const bool dbg = v.debug != 0;
+  const int P = a->P, W = a->image_width, H = a->image_height;
+  const bool dbg = a->debug != 0;
+  const bool bound = a->input_mode == GAB200_INPUT_BOUND_RAW;
   if (P == 0) return GAB200_OK;
   GeomView g = carve_geom(st->geom_buffer, views * P, true, 0, P);
   ImageView iv = carve_image(st->image_buffer, W, H, true, views);
@@ -843,85 +838,10 @@ static int32_t run_backward_views(const gab200_backward_args* b, int32_t views, 
 
   // csr: the per-splat kernel writes per-splat face gradients and clears the face gradients that face_grad_reduce
   // then adds them into; otherwise it adds into them itself, cleared here
-  const bool csr = v.binding != nullptr && b->num_face_chunks > 0 && b->face_perm && b->face_chunk_face &&
-                   b->face_chunk_start && b->face_chunk_end &&
-                   (b->dL_dface_center || b->dL_dface_orien_mat || b->dL_dface_scaling);
-  GAB_CUDA(cudaMemsetAsync(g.g2d, 0, sizeof(float) * (size_t)views * P * GAB_G2D_STRIDE, stream));
-  if (v.binding != nullptr && !csr) {
-    const size_t F = (size_t)v.num_faces;
-    if (b->dL_dface_center) GAB_CUDA(cudaMemsetAsync(b->dL_dface_center, 0, sizeof(float) * 3 * F, stream));
-    if (b->dL_dface_orien_mat) GAB_CUDA(cudaMemsetAsync(b->dL_dface_orien_mat, 0, sizeof(float) * 9 * F, stream));
-    if (b->dL_dface_scaling) GAB_CUDA(cudaMemsetAsync(b->dL_dface_scaling, 0, sizeof(float) * F, stream));
-  }
-  if (st->num_rendered != 0) {
-    StageScope sc(GAB200_STAGE_BLEND_BWD, stream);
-    if (da)
-      launch_blend_backward_views_depth(views, W, H, iv.ranges, iv.order, iv.order_info, bv.vals[st->sorted_selector],
-                                        g.rec, v.bg, iv.final_T, iv.n_contrib, b->dL_dout_color, bv.strip_mask, g.g2d,
-                                        dL_dalpha, dL_ddepth, stream);
-    else
-      launch_blend_backward_views(views, W, H, iv.ranges, iv.order, iv.order_info, bv.vals[st->sorted_selector], g.rec,
-                                  v.bg, iv.final_T, iv.n_contrib, b->dL_dout_color, bv.strip_mask, g.g2d, stream);
-  }
-  GAB_STAGE_CHECK(dbg, stream);
-  {
-    StageScope sc(GAB200_STAGE_PREPROCESS_BWD, stream);
-    gab200_backward_args bb = *b;
-    bb.fwd = &v;
-    launch_preprocess_backward_views(bb, views, cameras, g.aux, g.clamped, g.g2d, csr ? g.face_scratch : nullptr,
-                                     stream, da);
-  }
-  GAB_STAGE_CHECK(dbg, stream);
-  return GAB200_OK;
-}
-
-int32_t gab200_backward_views(const gab200_backward_args* b, int32_t views, const float* cameras, void* stream) {
-  return run_backward_views(b, views, cameras, stream);
-}
-
-int32_t gab200_backward_views_depth_alpha(const gab200_backward_args* b, int32_t views, const float* cameras,
-                                          const float* dL_dalpha, const float* dL_ddepth, void* stream) {
-  return run_backward_views(b, views, cameras, stream, true, dL_dalpha, dL_ddepth);
-}
-
-// gab200_backward and gab200_backward_device_fov, and gab200_backward_depth_alpha (da: the plane gradients, NULL = 0)
-static int32_t run_backward(const gab200_backward_args* b, const float* tanfov, void* stream_, bool da = false,
-                            const float* dL_dalpha = nullptr, const float* dL_ddepth = nullptr) {
-  cudaStream_t stream = (cudaStream_t)stream_;
-  if (b == nullptr || b->abi_version != GAB200_ABI_VERSION || b->fwd == nullptr || b->state == nullptr)
-    return GAB200_ERR_INVALID_ARGUMENT;
-  const gab200_forward_args* a = b->fwd;
-  const gab200_frame_state* st = b->state;
-  if (!validate(a) || !a->need_backward || b->dL_dout_color == nullptr) return GAB200_ERR_INVALID_ARGUMENT;
-  if (st->reserved0 != 0) return GAB200_ERR_INVALID_ARGUMENT;  // a multi-view frame: gab200_backward_views
-  // the depth plane's backward reads z from the records: only a gab200_forward_depth_alpha state has it; plain stores
-  if (da && (st->depth_prefix != 1u || b->grads_are_multicast)) return GAB200_ERR_INVALID_ARGUMENT;
-  if (st->geom_buffer == nullptr || st->image_buffer == nullptr || st->binning_buffer == nullptr)
-    return GAB200_ERR_INVALID_ARGUMENT;
-  const int P = a->P, W = a->image_width, H = a->image_height;
-  const bool dbg = a->debug != 0;
-  const bool bound = a->input_mode == GAB200_INPUT_BOUND_RAW;
-  if (bound && a->colors_precomp == nullptr && (b->dL_dsh_dc == nullptr || (a->sh_coeffs > 1 && b->dL_dsh_rest == nullptr)))
-    return GAB200_ERR_INVALID_ARGUMENT;
-  if (P == 0) return GAB200_OK;
-  cudaStreamCaptureStatus cap_status = cudaStreamCaptureStatusNone;
-  GAB_CUDA(cudaStreamIsCapturing(stream, &cap_status));
-  struct CaptureGuard {
-    bool prev;
-    explicit CaptureGuard(bool c) : prev(t_capturing) { t_capturing = c; }
-    ~CaptureGuard() { t_capturing = prev; }
-  } capture_guard(cap_status != cudaStreamCaptureStatusNone);
-  GeomView g = carve_geom(st->geom_buffer, P, true, 0);
-  ImageView iv = carve_image(st->image_buffer, W, H, true);
-  BinView bv = carve_binning(st->binning_buffer, st->binning_capacity, true, 0);
-  if (g.bytes > st->geom_bytes || iv.bytes > st->image_bytes || bv.bytes > st->binning_bytes)
-    return GAB200_ERR_INVALID_ARGUMENT;  // not the buffers this forward carved
-
-  // csr: as in run_backward_views, the per-splat kernel clears the face gradients face_grad_reduce adds into
   const bool csr = bound && a->binding != nullptr && b->num_face_chunks > 0 && b->face_perm && b->face_chunk_face &&
                    b->face_chunk_start && b->face_chunk_end &&
                    (b->dL_dface_center || b->dL_dface_orien_mat || b->dL_dface_scaling);
-  GAB_CUDA(cudaMemsetAsync(g.g2d, 0, sizeof(float) * (size_t)P * GAB_G2D_STRIDE, stream));
+  GAB_CUDA(cudaMemsetAsync(g.g2d, 0, sizeof(float) * (size_t)views * P * GAB_G2D_STRIDE, stream));
   if (bound && a->binding != nullptr && !csr) {
     const size_t F = (size_t)a->num_faces;
     if (b->dL_dface_center) GAB_CUDA(cudaMemsetAsync(b->dL_dface_center, 0, sizeof(float) * 3 * F, stream));
@@ -929,39 +849,54 @@ static int32_t run_backward(const gab200_backward_args* b, const float* tanfov, 
     if (b->dL_dface_scaling) GAB_CUDA(cudaMemsetAsync(b->dL_dface_scaling, 0, sizeof(float) * F, stream));
   }
   if (b->grads_are_multicast && !bound) return GAB200_ERR_INVALID_ARGUMENT;
-  if (bound && a->colors_precomp != nullptr && !b->grads_are_multicast) {
+  if (bound && a->colors_precomp != nullptr && !b->grads_are_multicast) {  // single view only: K views take SH colours
     if (b->dL_dsh_dc) GAB_CUDA(cudaMemsetAsync(b->dL_dsh_dc, 0, sizeof(float) * 3 * (size_t)P, stream));
     if (b->dL_dsh_rest && a->sh_coeffs > 1)
       GAB_CUDA(cudaMemsetAsync(b->dL_dsh_rest, 0, sizeof(float) * 3 * (size_t)(a->sh_coeffs - 1) * P, stream));
   }
   if (st->num_rendered != 0) {  // -1: only the device knows (GAB200_SYNC_NONE); empty tile lists cost nothing
     StageScope sc(GAB200_STAGE_BLEND_BWD, stream);
-    if (da)
-      launch_blend_backward_depth(W, H, iv.ranges, iv.order, iv.order_info, bv.vals[st->sorted_selector], g.rec, a->bg,
-                                  iv.final_T, iv.n_contrib, b->dL_dout_color, bv.strip_mask, g.g2d, dL_dalpha,
-                                  dL_ddepth, stream);
-    else
-      launch_blend_backward(W, H, iv.ranges, iv.order, iv.order_info, bv.vals[st->sorted_selector], g.rec, a->bg,
-                            iv.final_T, iv.n_contrib, b->dL_dout_color, bv.strip_mask, g.g2d, stream);
+    launch_blend_backward(views, W, H, iv.ranges, iv.order, iv.order_info, bv.vals[st->sorted_selector], g.rec, a->bg,
+                          iv.final_T, iv.n_contrib, b->dL_dout_color, bv.strip_mask, g.g2d, da, dL_dalpha, dL_ddepth,
+                          stream);
   }
   GAB_STAGE_CHECK(dbg, stream);
   {
     StageScope sc(GAB200_STAGE_PREPROCESS_BWD, stream);
-    launch_preprocess_backward(*b, g.rec, g.aux, g.clamped, g.g2d, csr ? g.face_scratch : nullptr, tanfov, stream, da);
+    if (cameras != nullptr) {
+      gab200_backward_args bb = *b;
+      bb.fwd = &v;
+      launch_preprocess_backward_views(bb, views, cameras, g.aux, g.clamped, g.g2d, csr ? g.face_scratch : nullptr,
+                                       stream, da);
+    } else {
+      launch_preprocess_backward(*b, g.rec, g.aux, g.clamped, g.g2d, csr ? g.face_scratch : nullptr, tanfov, stream,
+                                 da);
+    }
   }
   GAB_STAGE_CHECK(dbg, stream);
   return GAB200_OK;
 }
 
-int32_t gab200_backward(const gab200_backward_args* b, void* stream) { return run_backward(b, nullptr, stream); }
+int32_t gab200_backward_views(const gab200_backward_args* b, int32_t views, const float* cameras, void* stream) {
+  return run_backward(b, nullptr, views, cameras, stream);
+}
+
+int32_t gab200_backward_views_depth_alpha(const gab200_backward_args* b, int32_t views, const float* cameras,
+                                          const float* dL_dalpha, const float* dL_ddepth, void* stream) {
+  return run_backward(b, nullptr, views, cameras, stream, true, dL_dalpha, dL_ddepth);
+}
+
+int32_t gab200_backward(const gab200_backward_args* b, void* stream) {
+  return run_backward(b, nullptr, 1, nullptr, stream);
+}
 
 int32_t gab200_backward_device_fov(const gab200_backward_args* b, const float* tanfov, void* stream) {
-  return run_backward(b, tanfov, stream);
+  return run_backward(b, tanfov, 1, nullptr, stream);
 }
 
 int32_t gab200_backward_depth_alpha(const gab200_backward_args* b, const float* tanfov, const float* dL_dalpha,
                                     const float* dL_ddepth, void* stream) {
-  return run_backward(b, tanfov, stream, true, dL_dalpha, dL_ddepth);
+  return run_backward(b, tanfov, 1, nullptr, stream, true, dL_dalpha, dL_ddepth);
 }
 
 int32_t gab200_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,

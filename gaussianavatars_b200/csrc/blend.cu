@@ -93,6 +93,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
 }
 #define GAB_FWD_DEPTH_CTAS 2  // CTAs per SM the depth-plane blend kernels are bounded for (DESIGN.md section 4)
+#define GAB_FWD_VIEWS_TRAIN_CTAS 3  // ... and the K-view training forward
 #define GAB_BWD_DEPTH_CTAS 5
 #define ID_RING 3  // id chunks in flight: being gathered from, next, and the one the copy engine is filling
 
@@ -133,6 +134,7 @@ struct BandGeom {
 // (no contraction into an fma), so the byte equals torch's two ops on the float the float path stores, bit for bit.
 #define BLEND_OUT_FLOAT 1  // [3,H,W] float32
 #define BLEND_OUT_U8 2     // [H,W,3] uint8
+#define BLEND_OUT_TRAIN 4  // final_T and n_contrib [H,W] and the block masks, which the backward reads
 __device__ __forceinline__ uint32_t quantize_u8(float c) {
   return __float2uint_rz(fminf(fmaxf(__fadd_rn(__fmul_rn(c, 255.f), 0.5f), 0.f), 255.f));
 }
@@ -186,18 +188,38 @@ __device__ __forceinline__ bool reaches_rect(const SplatRec& r, float x0, float 
 // =====================================================================================================
 // Forward: one tile on a group of NT = 256/K threads (tl = thread index inside the group)
 // =====================================================================================================
-// DA (gab200_forward_depth_alpha): also the accumulated alpha 1 - T_final and the depth sum_i w_i z_i of the same walk,
-// z_i = q2.w of a record written by preprocess_depth_kernel; out_alpha / out_depth [H,W] (either may be NULL).
-template <int K, int OUT, bool DA = false>
+// OUT: which images are written (BLEND_OUT_*).  Without BLEND_OUT_TRAIN the training outputs (final_T, n_contrib and
+// the block masks) are absent at compile time; with it they are written where final_T / strip_mask are non-null.
+// DA (gab200_forward*_depth_alpha): also the accumulated alpha 1 - T_final and the depth sum_i w_i z_i of the same
+// walk, z_i = q2.w of a record written by the preprocess with DA; out_alpha / out_depth [H,W] (either may be NULL).
+// VIEWS (gab200_forward_views*): `tile` is global tile g of K views, tile g % view_tiles of view g / view_tiles: the
+// tile's range and the view's per-pixel outputs are offset by view, then the tile is rendered exactly as a single
+// view.  The block masks are indexed by position in the sorted stream, which is global already.
+template <int K, int OUT, bool DA, bool VIEWS>
 __device__ __forceinline__ void forward_tile(int tile, int tl, GroupBarrier<256 / K> bar, SplatRec* buf0,
                                              SplatRec* buf1, uint32_t* smask, uint32_t* ids_ring, uint64_t* mbar,
-                                             int W, int H, int gx,
+                                             int W, int H, int gx, int view_tiles,
                                              const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list,
                                              const SplatRec* __restrict__ rec, const float* __restrict__ bg,
                                              float* __restrict__ out_color, float* __restrict__ final_T,
                                              uint32_t* __restrict__ n_contrib, uint8_t* __restrict__ strip_mask,
-                                             uint8_t* __restrict__ out_rgb8, float* __restrict__ out_alpha = nullptr,
-                                             float* __restrict__ out_depth = nullptr) {
+                                             uint8_t* __restrict__ out_rgb8, float* __restrict__ out_alpha,
+                                             float* __restrict__ out_depth) {
+  constexpr bool TRAIN = DA || (OUT & BLEND_OUT_TRAIN) != 0;
+  if (VIEWS) {
+    const int view = tile / view_tiles;
+    const size_t off = (size_t)view * H * W;
+    tile -= view * view_tiles;
+    ranges += (size_t)view * view_tiles;
+    if (OUT & BLEND_OUT_FLOAT) out_color += 3 * off;
+    if (OUT & BLEND_OUT_U8) out_rgb8 += 3 * off;
+    if (TRAIN && final_T != nullptr) {
+      final_T += off;
+      n_contrib += off;
+    }
+    if (DA && out_alpha != nullptr) out_alpha += off;
+    if (DA && out_depth != nullptr) out_depth += off;
+  }
   constexpr int NT = 256 / K;
   const int tx = tile % gx, ty = tile / gx;
   const int lane = tl & 31;
@@ -211,7 +233,7 @@ __device__ __forceinline__ void forward_tile(int tile, int tl, GroupBarrier<256 
   const uint2 range = ranges[tile];
   const int n = (int)(range.y - range.x);
   const uint32_t* ids = point_list + range.x;
-  const bool want_mask = strip_mask != nullptr;
+  const bool want_mask = TRAIN && strip_mask != nullptr;
   smask[tl] = 0;
   // the warp's pixel rectangle: columns of its half, rows of its K bands (pixels past the image edge included)
   const float rx0 = (float)(pixx - (lane & 7)), rx1 = rx0 + 7.f;
@@ -359,7 +381,7 @@ __device__ __forceinline__ void forward_tile(int tile, int tl, GroupBarrier<256 
         out_color[HW + pix] = fmaf(T[i], bg1, Cg[i]);
         out_color[2 * HW + pix] = fmaf(T[i], bg2, Cb[i]);
       }
-      if (final_T != nullptr) {
+      if (TRAIN && final_T != nullptr) {
         final_T[pix] = T[i];
         n_contrib[pix] = last[i];
       }
@@ -377,227 +399,16 @@ __device__ __forceinline__ void forward_tile(int tile, int tl, GroupBarrier<256 
   }
 }
 
-// CTA = 256 threads.  The first CTAs take KH heavy tiles each on 256/KH threads (KH = 1: all eight warps on one
-// tile); the following CTAs take four light tiles each, one per 64-thread group, K = 4.
-template <int KH, int OUT>
-__global__ void __launch_bounds__(256) blend_forward_kernel(int W, int H, int gx, int tiles,
-                                                            const uint2* __restrict__ ranges,
-                                                            const uint32_t* __restrict__ order,
-                                                            const uint32_t* __restrict__ order_info,
-                                                            const uint32_t* __restrict__ point_list,
-                                                            const SplatRec* __restrict__ rec,
-                                                            const float* __restrict__ bg, float* __restrict__ out_color,
-                                                            float* __restrict__ final_T,
-                                                            uint32_t* __restrict__ n_contrib,
-                                                            uint8_t* __restrict__ strip_mask,
-                                                            uint8_t* __restrict__ out_rgb8) {
-  __shared__ SplatRec buf[2][256];
-  __shared__ uint32_t smask[256];
-  __shared__ __align__(16) uint32_t ids_ring[4][ID_RING * (64 + 4)];  // per 64-thread group; a 256-thread tile uses it flat
-  __shared__ __align__(8) uint64_t mbar[4][ID_RING];
-  constexpr int GH = KH;  // heavy tiles per CTA (256/KH threads each)
-  constexpr int NTH = 256 / KH;
-  pdl_wait();
-  pdl_trigger();
-  const int nh = (int)order_info[0];
-  const int heavy_ctas = (nh + GH - 1) / GH;
-  const int b = blockIdx.x, t = threadIdx.x;
-  if (b < heavy_ctas) {
-    const int g = t / NTH, slot = b * GH + g;
-    if (slot >= nh) return;
-    forward_tile<KH, OUT>((int)order[slot], t - g * NTH, GroupBarrier<NTH>{GH == 1 ? 0 : 1 + g}, buf[0] + g * NTH,
-                          buf[1] + g * NTH, smask + g * NTH, &ids_ring[0][0] + g * (ID_RING * (NTH + 4)), mbar[g], W,
-                          H, gx, ranges, point_list, rec, bg, out_color, final_T, n_contrib, strip_mask, out_rgb8);
-  } else {
-    const int g = t >> 6, slot = nh + 4 * (b - heavy_ctas) + g;
-    if (slot >= tiles) return;
-    forward_tile<4, OUT>((int)order[slot], t & 63, GroupBarrier<64>{1 + g}, buf[0] + g * 64, buf[1] + g * 64,
-                         smask + g * 64, ids_ring[g], mbar[g], W, H, gx, ranges, point_list, rec, bg, out_color,
-                         final_T, n_contrib, strip_mask, out_rgb8);
-  }
-}
-
-void launch_blend_forward(int W, int H, const uint2* ranges, const uint32_t* order, const uint32_t* order_info,
-                          const uint32_t* point_list, const SplatRec* rec, const float* bg, float* out_color,
-                          float* final_T, uint32_t* n_contrib, uint8_t* strip_mask, uint8_t* out_rgb8,
-                          cudaStream_t stream) {
-  const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
-  const int tiles = gx * gy;
-  if (tiles == 0) return;
-  // upper bound on CTAs: every tile heavy; surplus CTAs exit at once
-  const int grid = tiles;
-  auto kernel = out_rgb8 == nullptr ? blend_forward_kernel<1, BLEND_OUT_FLOAT>
-                : out_color == nullptr ? blend_forward_kernel<1, BLEND_OUT_U8>
-                                       : blend_forward_kernel<1, BLEND_OUT_FLOAT | BLEND_OUT_U8>;
-  launch_pdl(kernel, grid, 256, 0, stream, W, H, gx, tiles, ranges, order, order_info, point_list, rec, bg, out_color,
-             final_T, n_contrib, strip_mask, out_rgb8);
-}
-
-// gab200_forward_depth_alpha: blend_forward_kernel<1, OUT> with the alpha and depth planes (forward_tile<.., DA>).  The
-// records must come from preprocess_depth_kernel (z in q2.w).
-template <int OUT>
-__global__ void __launch_bounds__(256, GAB_FWD_DEPTH_CTAS) blend_forward_depth_kernel(int W, int H, int gx, int tiles,
-                                                                  const uint2* __restrict__ ranges,
-                                                                  const uint32_t* __restrict__ order,
-                                                                  const uint32_t* __restrict__ order_info,
-                                                                  const uint32_t* __restrict__ point_list,
-                                                                  const SplatRec* __restrict__ rec,
-                                                                  const float* __restrict__ bg,
-                                                                  float* __restrict__ out_color,
-                                                                  float* __restrict__ final_T,
-                                                                  uint32_t* __restrict__ n_contrib,
-                                                                  uint8_t* __restrict__ strip_mask,
-                                                                  uint8_t* __restrict__ out_rgb8,
-                                                                  float* __restrict__ out_alpha,
-                                                                  float* __restrict__ out_depth) {
-  __shared__ SplatRec buf[2][256];
-  __shared__ uint32_t smask[256];
-  __shared__ __align__(16) uint32_t ids_ring[4][ID_RING * (64 + 4)];
-  __shared__ __align__(8) uint64_t mbar[4][ID_RING];
-  pdl_wait();
-  pdl_trigger();
-  const int nh = (int)order_info[0];
-  const int b = blockIdx.x, t = threadIdx.x;
-  if (b < nh) {
-    forward_tile<1, OUT, true>((int)order[b], t, GroupBarrier<256>{0}, buf[0], buf[1], smask, &ids_ring[0][0], mbar[0],
-                               W, H, gx, ranges, point_list, rec, bg, out_color, final_T, n_contrib, strip_mask,
-                               out_rgb8, out_alpha, out_depth);
-  } else {
-    const int g = t >> 6, slot = nh + 4 * (b - nh) + g;
-    if (slot >= tiles) return;
-    forward_tile<4, OUT, true>((int)order[slot], t & 63, GroupBarrier<64>{1 + g}, buf[0] + g * 64, buf[1] + g * 64,
-                               smask + g * 64, ids_ring[g], mbar[g], W, H, gx, ranges, point_list, rec, bg, out_color,
-                               final_T, n_contrib, strip_mask, out_rgb8, out_alpha, out_depth);
-  }
-}
-
-void launch_blend_forward_depth(int W, int H, const uint2* ranges, const uint32_t* order, const uint32_t* order_info,
-                                const uint32_t* point_list, const SplatRec* rec, const float* bg, float* out_color,
-                                float* final_T, uint32_t* n_contrib, uint8_t* strip_mask, uint8_t* out_rgb8,
-                                float* out_alpha, float* out_depth, cudaStream_t stream) {
-  const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
-  const int tiles = gx * gy;
-  if (tiles == 0) return;
-  auto kernel = out_rgb8 == nullptr ? blend_forward_depth_kernel<BLEND_OUT_FLOAT>
-                : out_color == nullptr ? blend_forward_depth_kernel<BLEND_OUT_U8>
-                                       : blend_forward_depth_kernel<BLEND_OUT_FLOAT | BLEND_OUT_U8>;
-  launch_pdl(kernel, tiles, 256, 0, stream, W, H, gx, tiles, ranges, order, order_info, point_list, rec, bg, out_color,
-             final_T, n_contrib, strip_mask, out_rgb8, out_alpha, out_depth);
-}
-
-// gab200_forward_views: the tiles of K views as one list of K * view_tiles global tiles, scheduled heaviest-first
-// together (small views fill the GPU side by side).  Global tile g is tile g % view_tiles of view g / view_tiles: the
-// tile's range and the view's images are offset, and forward_tile renders it exactly as the single-view kernel does.
-// Forward only (no final_T, n_contrib or block masks).
-template <int OUT>
-__global__ void __launch_bounds__(256) blend_forward_views_kernel(int W, int H, int gx, int tiles, int view_tiles,
-                                                                  const uint2* __restrict__ ranges,
-                                                                  const uint32_t* __restrict__ order,
-                                                                  const uint32_t* __restrict__ order_info,
-                                                                  const uint32_t* __restrict__ point_list,
-                                                                  const SplatRec* __restrict__ rec,
-                                                                  const float* __restrict__ bg,
-                                                                  float* __restrict__ out_color,
-                                                                  uint8_t* __restrict__ out_rgb8) {
-  __shared__ SplatRec buf[2][256];
-  __shared__ uint32_t smask[256];
-  __shared__ __align__(16) uint32_t ids_ring[4][ID_RING * (64 + 4)];
-  __shared__ __align__(8) uint64_t mbar[4][ID_RING];
-  pdl_wait();
-  pdl_trigger();
-  const int nh = (int)order_info[0];
-  const int b = blockIdx.x, t = threadIdx.x;
-  const bool heavy = b < nh;  // one heavy tile on all 256 threads, else four light tiles on 64 threads each
-  const int g = heavy ? 0 : t >> 6;
-  const int slot = heavy ? b : nh + 4 * (b - nh) + g;
-  if (slot >= (heavy ? nh : tiles)) return;
-  const int tile = (int)order[slot];
-  const int view = tile / view_tiles, local = tile - view * view_tiles;
-  const size_t HW = (size_t)H * W;
-  float* color = (OUT & BLEND_OUT_FLOAT) ? out_color + (size_t)view * 3 * HW : nullptr;
-  uint8_t* rgb8 = (OUT & BLEND_OUT_U8) ? out_rgb8 + (size_t)view * 3 * HW : nullptr;
-  const uint2* view_ranges = ranges + (size_t)view * view_tiles;
-  if (heavy)
-    forward_tile<1, OUT>(local, t, GroupBarrier<256>{0}, buf[0], buf[1], smask, &ids_ring[0][0], mbar[0], W, H, gx,
-                         view_ranges, point_list, rec, bg, color, nullptr, nullptr, nullptr, rgb8);
-  else
-    forward_tile<4, OUT>(local, t & 63, GroupBarrier<64>{1 + g}, buf[0] + g * 64, buf[1] + g * 64, smask + g * 64,
-                         ids_ring[g], mbar[g], W, H, gx, view_ranges, point_list, rec, bg, color, nullptr, nullptr,
-                         nullptr, rgb8);
-}
-
-void launch_blend_forward_views(int views, int W, int H, const uint2* ranges, const uint32_t* order,
-                                const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
-                                const float* bg, float* out_color, uint8_t* out_rgb8, cudaStream_t stream) {
-  const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
-  const int view_tiles = gx * gy, tiles = views * view_tiles;
-  if (tiles == 0) return;
-  auto kernel = out_rgb8 == nullptr ? blend_forward_views_kernel<BLEND_OUT_FLOAT>
-                : out_color == nullptr ? blend_forward_views_kernel<BLEND_OUT_U8>
-                                       : blend_forward_views_kernel<BLEND_OUT_FLOAT | BLEND_OUT_U8>;
-  launch_pdl(kernel, tiles, 256, 0, stream, W, H, gx, tiles, view_tiles, ranges, order, order_info, point_list, rec, bg,
-             out_color, out_rgb8);
-}
-
-// gab200_forward_views_train: blend_forward_views_kernel with the float image only, keeping what the backward reads --
-// final_T and n_contrib at the view's offset, and the block mask of every instance (indexed by its position in the
-// sorted stream, which is global already).
-__global__ void __launch_bounds__(256) blend_forward_views_train_kernel(int W, int H, int gx, int tiles, int view_tiles,
-                                                                        const uint2* __restrict__ ranges,
-                                                                        const uint32_t* __restrict__ order,
-                                                                        const uint32_t* __restrict__ order_info,
-                                                                        const uint32_t* __restrict__ point_list,
-                                                                        const SplatRec* __restrict__ rec,
-                                                                        const float* __restrict__ bg,
-                                                                        float* __restrict__ out_color,
-                                                                        float* __restrict__ final_T,
-                                                                        uint32_t* __restrict__ n_contrib,
-                                                                        uint8_t* __restrict__ strip_mask) {
-  __shared__ SplatRec buf[2][256];
-  __shared__ uint32_t smask[256];
-  __shared__ __align__(16) uint32_t ids_ring[4][ID_RING * (64 + 4)];
-  __shared__ __align__(8) uint64_t mbar[4][ID_RING];
-  pdl_wait();
-  pdl_trigger();
-  const int nh = (int)order_info[0];
-  const int b = blockIdx.x, t = threadIdx.x;
-  const bool heavy = b < nh;
-  const int g = heavy ? 0 : t >> 6;
-  const int slot = heavy ? b : nh + 4 * (b - nh) + g;
-  if (slot >= (heavy ? nh : tiles)) return;
-  const int tile = (int)order[slot];
-  const int view = tile / view_tiles, local = tile - view * view_tiles;
-  const size_t HW = (size_t)H * W;
-  float* color = out_color + (size_t)view * 3 * HW;
-  float* vT = final_T + (size_t)view * HW;
-  uint32_t* vn = n_contrib + (size_t)view * HW;
-  const uint2* view_ranges = ranges + (size_t)view * view_tiles;
-  if (heavy)
-    forward_tile<1, BLEND_OUT_FLOAT>(local, t, GroupBarrier<256>{0}, buf[0], buf[1], smask, &ids_ring[0][0], mbar[0], W,
-                                     H, gx, view_ranges, point_list, rec, bg, color, vT, vn, strip_mask, nullptr);
-  else
-    forward_tile<4, BLEND_OUT_FLOAT>(local, t & 63, GroupBarrier<64>{1 + g}, buf[0] + g * 64, buf[1] + g * 64,
-                                     smask + g * 64, ids_ring[g], mbar[g], W, H, gx, view_ranges, point_list, rec, bg,
-                                     color, vT, vn, strip_mask, nullptr);
-}
-
-void launch_blend_forward_views_train(int views, int W, int H, const uint2* ranges, const uint32_t* order,
-                                      const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
-                                      const float* bg, float* out_color, float* final_T, uint32_t* n_contrib,
-                                      uint8_t* strip_mask, cudaStream_t stream) {
-  const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
-  const int view_tiles = gx * gy, tiles = views * view_tiles;
-  if (tiles == 0) return;
-  launch_pdl(blend_forward_views_train_kernel, tiles, 256, 0, stream, W, H, gx, tiles, view_tiles, ranges, order,
-             order_info, point_list, rec, bg, out_color, final_T, n_contrib, strip_mask);
-}
-
-// gab200_forward_views_depth_alpha and gab200_forward_views_train_depth_alpha: blend_forward_views_kernel with the alpha
-// and depth planes (forward_tile<.., DA>), written at view k's offset k * H * W; records from preprocess_views_depth_kernel
-// (z in q2.w).  final_T != nullptr (the training form, OUT = BLEND_OUT_FLOAT): also final_T, n_contrib and the block
-// masks, as blend_forward_views_train_kernel keeps them.  Bounded as blend_forward_depth_kernel.
-template <int OUT>
-__global__ void __launch_bounds__(256, GAB_FWD_DEPTH_CTAS) blend_forward_views_depth_kernel(
+// CTA = 256 threads.  CTAs [0, n_heavy) take one heavy tile each on all eight warps; the following CTAs take four
+// light tiles each, one per 64-thread group, K = 4.
+// The view split and the training outputs are compile-time properties: either one at run time takes the plain forms
+// from 64 registers (4 CTAs per SM) to 80 or more.  Occupancy bounds (DESIGN.md section 4): the plane forms
+// GAB_FWD_DEPTH_CTAS, the K-view training form 3 (unbounded, ptxas holds it to 64 registers and spills); the plain
+// forms are left to ptxas (minimum 0: no bound, which is not the same as 1).
+template <int OUT, bool DA, bool VIEWS>
+__global__ void __launch_bounds__(256, DA                                 ? GAB_FWD_DEPTH_CTAS
+                                       : VIEWS && (OUT & BLEND_OUT_TRAIN) ? GAB_FWD_VIEWS_TRAIN_CTAS
+                                                                          : 0) blend_forward_kernel(
     int W, int H, int gx, int tiles, int view_tiles, const uint2* __restrict__ ranges, const uint32_t* __restrict__ order,
     const uint32_t* __restrict__ order_info, const uint32_t* __restrict__ point_list, const SplatRec* __restrict__ rec,
     const float* __restrict__ bg, float* __restrict__ out_color, float* __restrict__ final_T,
@@ -605,46 +416,52 @@ __global__ void __launch_bounds__(256, GAB_FWD_DEPTH_CTAS) blend_forward_views_d
     float* __restrict__ out_alpha, float* __restrict__ out_depth) {
   __shared__ SplatRec buf[2][256];
   __shared__ uint32_t smask[256];
-  __shared__ __align__(16) uint32_t ids_ring[4][ID_RING * (64 + 4)];
+  __shared__ __align__(16) uint32_t ids_ring[4][ID_RING * (64 + 4)];  // per 64-thread group; a 256-thread tile uses it flat
   __shared__ __align__(8) uint64_t mbar[4][ID_RING];
   pdl_wait();
   pdl_trigger();
   const int nh = (int)order_info[0];
   const int b = blockIdx.x, t = threadIdx.x;
-  const bool heavy = b < nh;
-  const int g = heavy ? 0 : t >> 6;
-  const int slot = heavy ? b : nh + 4 * (b - nh) + g;
-  if (slot >= (heavy ? nh : tiles)) return;
-  const int tile = (int)order[slot];
-  const int view = tile / view_tiles, local = tile - view * view_tiles;
-  const size_t HW = (size_t)H * W, off = (size_t)view * HW;
-  float* color = (OUT & BLEND_OUT_FLOAT) ? out_color + 3 * off : nullptr;
-  uint8_t* rgb8 = (OUT & BLEND_OUT_U8) ? out_rgb8 + 3 * off : nullptr;
-  float* vT = final_T != nullptr ? final_T + off : nullptr;
-  uint32_t* vn = final_T != nullptr ? n_contrib + off : nullptr;
-  float* va = out_alpha != nullptr ? out_alpha + off : nullptr;
-  float* vd = out_depth != nullptr ? out_depth + off : nullptr;
-  const uint2* view_ranges = ranges + (size_t)view * view_tiles;
-  if (heavy)
-    forward_tile<1, OUT, true>(local, t, GroupBarrier<256>{0}, buf[0], buf[1], smask, &ids_ring[0][0], mbar[0], W, H,
-                               gx, view_ranges, point_list, rec, bg, color, vT, vn, strip_mask, rgb8, va, vd);
-  else
-    forward_tile<4, OUT, true>(local, t & 63, GroupBarrier<64>{1 + g}, buf[0] + g * 64, buf[1] + g * 64,
-                               smask + g * 64, ids_ring[g], mbar[g], W, H, gx, view_ranges, point_list, rec, bg, color,
-                               vT, vn, strip_mask, rgb8, va, vd);
+  if (b < nh) {
+    forward_tile<1, OUT, DA, VIEWS>((int)order[b], t, GroupBarrier<256>{0}, buf[0], buf[1], smask, &ids_ring[0][0],
+                                    mbar[0], W, H, gx, view_tiles, ranges, point_list, rec, bg, out_color, final_T,
+                                    n_contrib, strip_mask, out_rgb8, out_alpha, out_depth);
+  } else {
+    const int g = t >> 6, slot = nh + 4 * (b - nh) + g;
+    if (slot >= tiles) return;
+    forward_tile<4, OUT, DA, VIEWS>((int)order[slot], t & 63, GroupBarrier<64>{1 + g}, buf[0] + g * 64,
+                                    buf[1] + g * 64, smask + g * 64, ids_ring[g], mbar[g], W, H, gx, view_tiles, ranges,
+                                    point_list, rec, bg, out_color, final_T, n_contrib, strip_mask, out_rgb8,
+                                    out_alpha, out_depth);
+  }
 }
 
-void launch_blend_forward_views_depth(int views, int W, int H, const uint2* ranges, const uint32_t* order,
-                                      const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
-                                      const float* bg, float* out_color, float* final_T, uint32_t* n_contrib,
-                                      uint8_t* strip_mask, uint8_t* out_rgb8, float* out_alpha, float* out_depth,
-                                      cudaStream_t stream) {
+template <bool DA, bool VIEWS>
+static decltype(&blend_forward_kernel<BLEND_OUT_FLOAT, DA, VIEWS>) blend_forward_instance(int out) {
+  constexpr int F = BLEND_OUT_FLOAT, U = BLEND_OUT_U8, T = BLEND_OUT_TRAIN;
+  if constexpr (!DA) {  // the plane forms keep the training outputs at run time whatever OUT says
+    if (out == (F | T)) return blend_forward_kernel<F | T, DA, VIEWS>;
+    if (out == (F | U | T)) return blend_forward_kernel<F | U | T, DA, VIEWS>;
+  }
+  out &= F | U;
+  return out == F ? blend_forward_kernel<F, DA, VIEWS>
+         : out == U ? blend_forward_kernel<U, DA, VIEWS>
+                    : blend_forward_kernel<F | U, DA, VIEWS>;
+}
+
+void launch_blend_forward(int views, int W, int H, const uint2* ranges, const uint32_t* order,
+                          const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec, const float* bg,
+                          float* out_color, float* final_T, uint32_t* n_contrib, uint8_t* strip_mask, uint8_t* out_rgb8,
+                          float* out_alpha, float* out_depth, cudaStream_t stream) {
   const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
   const int view_tiles = gx * gy, tiles = views * view_tiles;
   if (tiles == 0) return;
-  auto kernel = out_rgb8 == nullptr ? blend_forward_views_depth_kernel<BLEND_OUT_FLOAT>
-                : out_color == nullptr ? blend_forward_views_depth_kernel<BLEND_OUT_U8>
-                                       : blend_forward_views_depth_kernel<BLEND_OUT_FLOAT | BLEND_OUT_U8>;
+  const int out = (out_color != nullptr ? BLEND_OUT_FLOAT : 0) | (out_rgb8 != nullptr ? BLEND_OUT_U8 : 0) |
+                  (final_T != nullptr ? BLEND_OUT_TRAIN : 0);
+  const bool da = out_alpha != nullptr || out_depth != nullptr;
+  auto kernel = da ? (views > 1 ? blend_forward_instance<true, true>(out) : blend_forward_instance<true, false>(out))
+                   : (views > 1 ? blend_forward_instance<false, true>(out) : blend_forward_instance<false, false>(out));
+  // upper bound on CTAs: every tile heavy; surplus CTAs exit at once
   launch_pdl(kernel, tiles, 256, 0, stream, W, H, gx, tiles, view_tiles, ranges, order, order_info, point_list, rec, bg,
              out_color, final_T, n_contrib, strip_mask, out_rgb8, out_alpha, out_depth);
 }
@@ -759,7 +576,6 @@ struct __align__(16) WarpSmemT {
   uint8_t masks[ID_RING][32 + 16];
   uint64_t mbar[ID_RING];
 };
-using WarpSmem = WarpSmemT<9>;
 
 // One warp task: the pixels of one (tile, half, band group), same ownership as the forward (BandGeom).
 //   * The WARP is the unit of work.  It stages its own id/mask lists (TMA bulk copies into a private 3-slot ring) and
@@ -772,9 +588,9 @@ using WarpSmem = WarpSmemT<9>;
 //     store 18 partials; during visit j+2 nine lanes add the two halves and issue the RED.  No shuffle, no exposed
 //     shared-memory or shuffle latency: the loads of rounds 1 and 2 are issued at the top of a visit and consumed
 //     after its band math.
-// DA (gab200_backward_depth_alpha): records from preprocess_depth_kernel (z in q2.w); dL_dalpha / dL_ddepth [H,W] or
+// DA (gab200_backward_depth_alpha): records from the preprocess with DA (z in q2.w); dL_dalpha / dL_ddepth [H,W] or
 // NULL (zero); a tenth component, dL/dz, leaves for g2d slot 9.
-template <int K, bool DA = false>
+template <int K, bool DA>
 __device__ __forceinline__ void backward_task(int tile, int tl, WarpSmemT<DA ? 10 : 9>& sm, int W, int H, int gx,
                                               const uint2* __restrict__ ranges,
                                               const uint32_t* __restrict__ point_list,
@@ -783,8 +599,8 @@ __device__ __forceinline__ void backward_task(int tile, int tl, WarpSmemT<DA ? 1
                                               const uint32_t* __restrict__ n_contrib,
                                               const float* __restrict__ dL_dpix,
                                               const uint8_t* __restrict__ strip_mask, float* __restrict__ g2d,
-                                              const float* __restrict__ dL_dalpha = nullptr,
-                                              const float* __restrict__ dL_ddepth = nullptr) {
+                                              const float* __restrict__ dL_dalpha,
+                                              const float* __restrict__ dL_ddepth) {
   constexpr int NR = DA ? 10 : 9;
   const int tx = tile % gx, ty = tile / gx;
   const int lane = tl & 31;
@@ -958,138 +774,20 @@ __device__ __forceinline__ void backward_task(int tile, int tl, WarpSmemT<DA ? 1
 
 // CTA = 128 threads: CTAs [0, n_heavy) take one heavy tile on four warps, K = 2; the rest take two light tiles each,
 // two warps (the halves) per tile, K = 4.  5 CTAs per SM was the fastest occupancy measured on the H100.
-__global__ void __launch_bounds__(128, 5) blend_backward_kernel(int W, int H, int gx, int tiles,
-                                                                const uint2* __restrict__ ranges,
-                                                                const uint32_t* __restrict__ order,
-                                                                const uint32_t* __restrict__ order_info,
-                                                                const uint32_t* __restrict__ point_list,
-                                                                const SplatRec* __restrict__ rec,
-                                                                const float* __restrict__ bg,
-                                                                const float* __restrict__ final_T,
-                                                                const uint32_t* __restrict__ n_contrib,
-                                                                const float* __restrict__ dL_dpix,
-                                                                const uint8_t* __restrict__ strip_mask,
-                                                                float* __restrict__ g2d) {
-  __shared__ WarpSmem sm[4];
-  pdl_wait();
-  pdl_trigger();
-  const int nh = (int)order_info[1];
-  const int b = blockIdx.x, t = threadIdx.x, w = t >> 5;
-  if (b < nh) {  // heavy tile: four warps, two bands each
-    backward_task<2>((int)order[b], t, sm[w], W, H, gx, ranges, point_list, rec, bg, final_T, n_contrib, dL_dpix,
-                     strip_mask, g2d);
-  } else {       // two light tiles: two warps (the halves) each, four bands per warp
-    const int slot = nh + 2 * (b - nh) + (w >> 1);
-    if (slot >= tiles) return;
-    backward_task<4>((int)order[slot], t & 63, sm[w], W, H, gx, ranges, point_list, rec, bg, final_T, n_contrib,
-                     dL_dpix, strip_mask, g2d);
-  }
-}
-
-void launch_blend_backward(int W, int H, const uint2* ranges, const uint32_t* order, const uint32_t* order_info,
-                           const uint32_t* point_list, const SplatRec* rec, const float* bg, const float* final_T,
-                           const uint32_t* n_contrib, const float* dL_dpix, const uint8_t* strip_mask, float* g2d,
-                           cudaStream_t stream) {
-  const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
-  const int tiles = gx * gy;
-  if (tiles == 0) return;
-  launch_pdl(blend_backward_kernel, tiles, 128, 0, stream, W, H, gx, tiles, ranges, order, order_info, point_list, rec,
-             bg, final_T, n_contrib, dL_dpix, strip_mask, g2d);
-}
-
-// gab200_backward_depth_alpha: blend_backward_kernel with the alpha and depth plane gradients (backward_task<K, true>).
-// Its own occupancy bound: see DESIGN.md section 4 for the registers of both bounds.
-__global__ void __launch_bounds__(128, GAB_BWD_DEPTH_CTAS) blend_backward_depth_kernel(
-    int W, int H, int gx, int tiles, const uint2* __restrict__ ranges, const uint32_t* __restrict__ order,
-    const uint32_t* __restrict__ order_info, const uint32_t* __restrict__ point_list, const SplatRec* __restrict__ rec,
-    const float* __restrict__ bg, const float* __restrict__ final_T, const uint32_t* __restrict__ n_contrib,
-    const float* __restrict__ dL_dpix, const uint8_t* __restrict__ strip_mask, float* __restrict__ g2d,
-    const float* __restrict__ dL_dalpha, const float* __restrict__ dL_ddepth) {
-  __shared__ WarpSmemT<10> sm[4];
-  pdl_wait();
-  pdl_trigger();
-  const int nh = (int)order_info[1];
-  const int b = blockIdx.x, t = threadIdx.x, w = t >> 5;
-  if (b < nh) {
-    backward_task<2, true>((int)order[b], t, sm[w], W, H, gx, ranges, point_list, rec, bg, final_T, n_contrib, dL_dpix,
-                           strip_mask, g2d, dL_dalpha, dL_ddepth);
-  } else {
-    const int slot = nh + 2 * (b - nh) + (w >> 1);
-    if (slot >= tiles) return;
-    backward_task<4, true>((int)order[slot], t & 63, sm[w], W, H, gx, ranges, point_list, rec, bg, final_T, n_contrib,
-                           dL_dpix, strip_mask, g2d, dL_dalpha, dL_ddepth);
-  }
-}
-
-void launch_blend_backward_depth(int W, int H, const uint2* ranges, const uint32_t* order, const uint32_t* order_info,
-                                 const uint32_t* point_list, const SplatRec* rec, const float* bg, const float* final_T,
-                                 const uint32_t* n_contrib, const float* dL_dpix, const uint8_t* strip_mask, float* g2d,
-                                 const float* dL_dalpha, const float* dL_ddepth, cudaStream_t stream) {
-  const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
-  const int tiles = gx * gy;
-  if (tiles == 0) return;
-  launch_pdl(blend_backward_depth_kernel, tiles, 128, 0, stream, W, H, gx, tiles, ranges, order, order_info, point_list,
-             rec, bg, final_T, n_contrib, dL_dpix, strip_mask, g2d, dL_dalpha, dL_ddepth);
-}
-
-// gab200_backward_views: blend_backward_kernel over the K * view_tiles global tiles of a multi-view frame.  Global tile
-// g is tile g % view_tiles of view g / view_tiles; its range, final_T, n_contrib and dL/dpixel are offset by view as
+// DA (gab200_backward*_depth_alpha): the alpha and depth plane gradients (backward_task<K, true>), either may be NULL
+// (zero); bounded for GAB_BWD_DEPTH_CTAS CTAs per SM (DESIGN.md section 4 has the registers of both bounds).
+// VIEWS (gab200_backward_views*): the K * view_tiles global tiles of a multi-view frame.  Global tile g is tile
+// g % view_tiles of view g / view_tiles; its range, final_T, n_contrib and the pixel gradients are offset by view as
 // the multi-view forward offsets them.  The point list holds virtual splat ids and the block masks are indexed by
 // stream position, so records, masks and the K * P rows of g2d need no offset; backward_task runs unchanged.
-__global__ void __launch_bounds__(128, 5) blend_backward_views_kernel(int W, int H, int gx, int tiles, int view_tiles,
-                                                                      const uint2* __restrict__ ranges,
-                                                                      const uint32_t* __restrict__ order,
-                                                                      const uint32_t* __restrict__ order_info,
-                                                                      const uint32_t* __restrict__ point_list,
-                                                                      const SplatRec* __restrict__ rec,
-                                                                      const float* __restrict__ bg,
-                                                                      const float* __restrict__ final_T,
-                                                                      const uint32_t* __restrict__ n_contrib,
-                                                                      const float* __restrict__ dL_dpix,
-                                                                      const uint8_t* __restrict__ strip_mask,
-                                                                      float* __restrict__ g2d) {
-  __shared__ WarpSmem sm[4];
-  pdl_wait();
-  pdl_trigger();
-  const int nh = (int)order_info[1];
-  const int b = blockIdx.x, t = threadIdx.x, w = t >> 5;
-  const bool heavy = b < nh;
-  const int slot = heavy ? b : nh + 2 * (b - nh) + (w >> 1);
-  if (!heavy && slot >= tiles) return;
-  const int tile = (int)order[slot];
-  const int view = tile / view_tiles, local = tile - view * view_tiles;
-  const size_t HW = (size_t)H * W;
-  const uint2* vr = ranges + (size_t)view * view_tiles;
-  const float* vT = final_T + (size_t)view * HW;
-  const uint32_t* vn = n_contrib + (size_t)view * HW;
-  const float* vd = dL_dpix + (size_t)view * 3 * HW;
-  if (heavy)
-    backward_task<2>(local, t, sm[w], W, H, gx, vr, point_list, rec, bg, vT, vn, vd, strip_mask, g2d);
-  else
-    backward_task<4>(local, t & 63, sm[w], W, H, gx, vr, point_list, rec, bg, vT, vn, vd, strip_mask, g2d);
-}
-
-void launch_blend_backward_views(int views, int W, int H, const uint2* ranges, const uint32_t* order,
-                                 const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
-                                 const float* bg, const float* final_T, const uint32_t* n_contrib, const float* dL_dpix,
-                                 const uint8_t* strip_mask, float* g2d, cudaStream_t stream) {
-  const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
-  const int view_tiles = gx * gy, tiles = views * view_tiles;
-  if (tiles == 0) return;
-  launch_pdl(blend_backward_views_kernel, tiles, 128, 0, stream, W, H, gx, tiles, view_tiles, ranges, order, order_info,
-             point_list, rec, bg, final_T, n_contrib, dL_dpix, strip_mask, g2d);
-}
-
-// gab200_backward_views_depth_alpha: blend_backward_views_kernel with the plane gradients (backward_task<K, true>):
-// dL/dalpha and dL/ddepth are read at view k's offset, dL/dz leaves for g2d slot 9 of the virtual splat's row.
-// Bounded as blend_backward_depth_kernel.
-__global__ void __launch_bounds__(128, GAB_BWD_DEPTH_CTAS) blend_backward_views_depth_kernel(
+template <bool DA, bool VIEWS>
+__global__ void __launch_bounds__(128, DA ? GAB_BWD_DEPTH_CTAS : 5) blend_backward_kernel(
     int W, int H, int gx, int tiles, int view_tiles, const uint2* __restrict__ ranges,
     const uint32_t* __restrict__ order, const uint32_t* __restrict__ order_info, const uint32_t* __restrict__ point_list,
     const SplatRec* __restrict__ rec, const float* __restrict__ bg, const float* __restrict__ final_T,
     const uint32_t* __restrict__ n_contrib, const float* __restrict__ dL_dpix, const uint8_t* __restrict__ strip_mask,
     float* __restrict__ g2d, const float* __restrict__ dL_dalpha, const float* __restrict__ dL_ddepth) {
-  __shared__ WarpSmemT<10> sm[4];
+  __shared__ WarpSmemT<DA ? 10 : 9> sm[4];
   pdl_wait();
   pdl_trigger();
   const int nh = (int)order_info[1];
@@ -1098,29 +796,31 @@ __global__ void __launch_bounds__(128, GAB_BWD_DEPTH_CTAS) blend_backward_views_
   const int slot = heavy ? b : nh + 2 * (b - nh) + (w >> 1);
   if (!heavy && slot >= tiles) return;
   const int tile = (int)order[slot];
-  const int view = tile / view_tiles, local = tile - view * view_tiles;
-  const size_t HW = (size_t)H * W, off = (size_t)view * HW;
+  const int view = VIEWS ? tile / view_tiles : 0, local = tile - view * view_tiles;
+  const size_t off = (size_t)view * H * W;
   const uint2* vr = ranges + (size_t)view * view_tiles;
   const float* va = dL_dalpha != nullptr ? dL_dalpha + off : nullptr;
   const float* vz = dL_ddepth != nullptr ? dL_ddepth + off : nullptr;
-  if (heavy)
-    backward_task<2, true>(local, t, sm[w], W, H, gx, vr, point_list, rec, bg, final_T + off, n_contrib + off,
-                           dL_dpix + 3 * off, strip_mask, g2d, va, vz);
-  else
-    backward_task<4, true>(local, t & 63, sm[w], W, H, gx, vr, point_list, rec, bg, final_T + off, n_contrib + off,
-                           dL_dpix + 3 * off, strip_mask, g2d, va, vz);
+  if (heavy)  // heavy tile: four warps, two bands each
+    backward_task<2, DA>(local, t, sm[w], W, H, gx, vr, point_list, rec, bg, final_T + off, n_contrib + off,
+                         dL_dpix + 3 * off, strip_mask, g2d, va, vz);
+  else        // two light tiles: two warps (the halves) each, four bands per warp
+    backward_task<4, DA>(local, t & 63, sm[w], W, H, gx, vr, point_list, rec, bg, final_T + off, n_contrib + off,
+                         dL_dpix + 3 * off, strip_mask, g2d, va, vz);
 }
 
-void launch_blend_backward_views_depth(int views, int W, int H, const uint2* ranges, const uint32_t* order,
-                                       const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
-                                       const float* bg, const float* final_T, const uint32_t* n_contrib,
-                                       const float* dL_dpix, const uint8_t* strip_mask, float* g2d,
-                                       const float* dL_dalpha, const float* dL_ddepth, cudaStream_t stream) {
+void launch_blend_backward(int views, int W, int H, const uint2* ranges, const uint32_t* order,
+                           const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec, const float* bg,
+                           const float* final_T, const uint32_t* n_contrib, const float* dL_dpix,
+                           const uint8_t* strip_mask, float* g2d, bool da, const float* dL_dalpha,
+                           const float* dL_ddepth, cudaStream_t stream) {
   const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
   const int view_tiles = gx * gy, tiles = views * view_tiles;
   if (tiles == 0) return;
-  launch_pdl(blend_backward_views_depth_kernel, tiles, 128, 0, stream, W, H, gx, tiles, view_tiles, ranges, order,
-             order_info, point_list, rec, bg, final_T, n_contrib, dL_dpix, strip_mask, g2d, dL_dalpha, dL_ddepth);
+  auto kernel = da ? (views > 1 ? blend_backward_kernel<true, true> : blend_backward_kernel<true, false>)
+                   : (views > 1 ? blend_backward_kernel<false, true> : blend_backward_kernel<false, false>);
+  launch_pdl(kernel, tiles, 128, 0, stream, W, H, gx, tiles, view_tiles, ranges, order, order_info, point_list, rec, bg,
+             final_T, n_contrib, dL_dpix, strip_mask, g2d, dL_dalpha, dL_ddepth);
 }
 
 }  // namespace gab

@@ -116,18 +116,17 @@ __device__ __forceinline__ uint32_t depth_bucket(uint32_t key, const DepthBucket
   const uint32_t b = (uint32_t)(__uint2float_rz(key - d.lo) * d.scale);
   return b < d.nb ? b : d.nb - 1u;
 }
-// tile_count != nullptr: also count the instances of every tile (counting tile sort, tile_sort.cu); rec_depth: the
-// records carry the view-space depth in q2.w (gab200_forward_depth_alpha)
-void launch_preprocess(const gab200_forward_args& a, SplatRec* rec, SplatAux* aux, uint32_t* tiles_touched,
-                       uint8_t* clamped, uint32_t* depth_keys, uint32_t* ids, const DepthBuckets& buckets,
-                       uint32_t* tile_count, const float* tanfov, cudaStream_t stream, bool rec_depth = false);
-// gab200_forward_views: grid (splat blocks, views); camera row k of `cameras` renders virtual splats k * P + i
-// (rec / aux / tiles / depth keys / ids / radii / visibility), tile counts at k * (gx * gy) + the tile in the view;
-// clamped != nullptr (gab200_forward_views_train, BOUND_RAW only): also the colour clamp bits at k * P + i;
-// rec_depth: the records carry the view-space depth in q2.w (gab200_forward_views[_train]_depth_alpha)
-void launch_preprocess_views(const gab200_forward_args& a, int views, const float* cameras, SplatRec* rec, SplatAux* aux,
-                             uint32_t* tiles_touched, uint32_t* depth_keys, uint32_t* ids, const DepthBuckets& buckets,
-                             uint32_t* tile_count, uint8_t* clamped, cudaStream_t stream, bool rec_depth = false);
+// cameras == NULL: the camera of `a`, its field of view from the device float[2] `tanfov`
+// (gab200_forward_device_fov) or, when that is NULL, a.tanfovx / tanfovy.  Otherwise `views` cameras
+// (gab200_forward_views*): grid (splat blocks, views); camera row k of `cameras` renders virtual splats k * P + i
+// (rec / aux / tiles / depth keys / ids / radii / visibility / clamp bits), tile counts at k * (gx * gy) + the tile
+// in the view.  clamped != nullptr: also the colour clamp bits (the backward reads them); tile_count != nullptr: also
+// count the instances of every tile (counting tile sort, tile_sort.cu); rec_depth: the records carry the view-space
+// depth in q2.w (the depth_alpha forms)
+void launch_preprocess(const gab200_forward_args& a, int views, const float* cameras, const float* tanfov,
+                       SplatRec* rec, SplatAux* aux, uint32_t* tiles_touched, uint8_t* clamped, uint32_t* depth_keys,
+                       uint32_t* ids, const DepthBuckets& buckets, uint32_t* tile_count, bool rec_depth,
+                       cudaStream_t stream);
 // depth_keys [P] (by splat) -> sorted_ids [M] in (key, id) order and offsets [M] = inclusive instance counts
 // also publishes the frame counters (capacity, seq, overflow) of the bucket-sorted frame
 void launch_depth_bucket_sort(int P, const DepthBuckets& buckets, const uint32_t* depth_keys,
@@ -187,55 +186,21 @@ cudaError_t run_sort(void* temp, size_t temp_bytes, uint32_t* keys_a, uint32_t* 
                      uint32_t* vals_b, int64_t N, int end_bit, int* selector_out, cudaStream_t stream);
 
 // blend.cu
-void launch_blend_forward(int W, int H, const uint2* ranges, const uint32_t* order, const uint32_t* order_info,
-                          const uint32_t* point_list, const SplatRec* rec,
-                          const float* bg, float* out_color, float* final_T, uint32_t* n_contrib, uint8_t* strip_mask,
-                          uint8_t* out_rgb8, cudaStream_t stream);  // out_color / out_rgb8: either may be NULL
-// launch_blend_forward plus the accumulated alpha and the depth planes [H,W] (either may be NULL); records with z in q2.w
-void launch_blend_forward_depth(int W, int H, const uint2* ranges, const uint32_t* order, const uint32_t* order_info,
-                                const uint32_t* point_list, const SplatRec* rec, const float* bg, float* out_color,
-                                float* final_T, uint32_t* n_contrib, uint8_t* strip_mask, uint8_t* out_rgb8,
-                                float* out_alpha, float* out_depth, cudaStream_t stream);
-// `views` images of one size: global tile g is tile g % (gx * gy) of view g / (gx * gy); out_color [views,3,H,W],
-// out_rgb8 [views,H,W,3] (either may be NULL); forward only
-void launch_blend_forward_views(int views, int W, int H, const uint2* ranges, const uint32_t* order,
-                                const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
-                                const float* bg, float* out_color, uint8_t* out_rgb8, cudaStream_t stream);
-// the training form of the multi-view forward: out_color required, no display image; final_T / n_contrib
-// [views,H,W] and the per-instance block masks are kept for launch_blend_backward_views
-void launch_blend_forward_views_train(int views, int W, int H, const uint2* ranges, const uint32_t* order,
-                                      const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
-                                      const float* bg, float* out_color, float* final_T, uint32_t* n_contrib,
-                                      uint8_t* strip_mask, cudaStream_t stream);
-// either multi-view forward plus the alpha and depth planes [views,H,W] (either may be NULL); records with z in q2.w.
-// final_T != NULL: the training form (out_color only; final_T / n_contrib / block masks kept as above)
-void launch_blend_forward_views_depth(int views, int W, int H, const uint2* ranges, const uint32_t* order,
-                                      const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
-                                      const float* bg, float* out_color, float* final_T, uint32_t* n_contrib,
-                                      uint8_t* strip_mask, uint8_t* out_rgb8, float* out_alpha, float* out_depth,
-                                      cudaStream_t stream);
-void launch_blend_backward(int W, int H, const uint2* ranges, const uint32_t* order, const uint32_t* order_info,
-                           const uint32_t* point_list, const SplatRec* rec,
-                           const float* bg, const float* final_T, const uint32_t* n_contrib, const float* dL_dpix,
-                           const uint8_t* strip_mask, float* g2d, cudaStream_t stream);
-// launch_blend_backward plus the plane gradients dL_dalpha / dL_ddepth [H,W] (NULL: zero); dL/dz -> g2d slot 9
-void launch_blend_backward_depth(int W, int H, const uint2* ranges, const uint32_t* order, const uint32_t* order_info,
-                                 const uint32_t* point_list, const SplatRec* rec, const float* bg, const float* final_T,
-                                 const uint32_t* n_contrib, const float* dL_dpix, const uint8_t* strip_mask, float* g2d,
-                                 const float* dL_dalpha, const float* dL_ddepth, cudaStream_t stream);
-// the same over the tiles of `views` images: dL_dpix [views,3,H,W]; g2d rows of the views * P virtual splats
-void launch_blend_backward_views(int views, int W, int H, const uint2* ranges, const uint32_t* order,
-                                 const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
-                                 const float* bg, const float* final_T, const uint32_t* n_contrib, const float* dL_dpix,
-                                 const uint8_t* strip_mask, float* g2d, cudaStream_t stream);
-// launch_blend_backward_views plus the plane gradients dL_dalpha / dL_ddepth [views,H,W] (NULL: zero); dL/dz -> g2d
-// slot 9 of each virtual splat's row
-void launch_blend_backward_views_depth(int views, int W, int H, const uint2* ranges, const uint32_t* order,
-                                       const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec,
-                                       const float* bg, const float* final_T, const uint32_t* n_contrib,
-                                       const float* dL_dpix, const uint8_t* strip_mask, float* g2d,
-                                       const float* dL_dalpha, const float* dL_ddepth, cudaStream_t stream);
-
+// `views` images of one size (1: a single view): global tile g is tile g % (gx * gy) of view g / (gx * gy).
+// out_color [views,3,H,W] / out_rgb8 [views,H,W,3]: either may be NULL.  final_T != NULL (the training forms): also
+// final_T / n_contrib [views,H,W] and the per-instance block masks, kept for launch_blend_backward.
+// out_alpha / out_depth [views,H,W]: the accumulated alpha and depth planes (either may be NULL; records with z in q2.w)
+void launch_blend_forward(int views, int W, int H, const uint2* ranges, const uint32_t* order,
+                          const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec, const float* bg,
+                          float* out_color, float* final_T, uint32_t* n_contrib, uint8_t* strip_mask, uint8_t* out_rgb8,
+                          float* out_alpha, float* out_depth, cudaStream_t stream);
+// the same tiles: dL_dpix [views,3,H,W]; g2d rows of the views * P virtual splats.  da: also the plane gradients
+// dL_dalpha / dL_ddepth [views,H,W] (NULL: zero); dL/dz -> g2d slot 9 of each virtual splat's row
+void launch_blend_backward(int views, int W, int H, const uint2* ranges, const uint32_t* order,
+                           const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec, const float* bg,
+                           const float* final_T, const uint32_t* n_contrib, const float* dL_dpix,
+                           const uint8_t* strip_mask, float* g2d, bool da, const float* dL_dalpha,
+                           const float* dL_ddepth, cudaStream_t stream);
 // preprocess_bwd.cu
 // depth: g2d slot 9 holds dL/dz (gab200_backward_depth_alpha), added to dL/dmean through the view matrix's third row;
 // no multicast

@@ -16,192 +16,294 @@ namespace gab {
 #define REC_SCALE_AC (-0.5f * 1.4426950408889634f)
 #define REC_SCALE_B (-1.4426950408889634f)
 
-__device__ __forceinline__ void stage_camera(const gab200_forward_args& a, Camera& cam) {
+// the camera of a block: viewmatrix (16) | projmatrix (16) | campos (3)
+__device__ __forceinline__ void stage_camera(const float* __restrict__ V, const float* __restrict__ Pm,
+                                             const float* __restrict__ campos, Camera& cam) {
   int t = threadIdx.x;
-  if (t < 16) cam.V[t] = a.viewmatrix[t];
-  else if (t < 32) cam.Pm[t - 16] = a.projmatrix[t - 16];
-  else if (t < 35) cam.campos[t - 32] = a.campos[t - 32];
-  __syncthreads();
-}
-// one row of a gab200_forward_views camera table: viewmatrix (16) | projmatrix (16) | campos (3) | tan(FoV/2) (2)
-__device__ __forceinline__ void stage_camera_row(const float* __restrict__ row, Camera& cam) {
-  int t = threadIdx.x;
-  if (t < 16) cam.V[t] = row[t];
-  else if (t < 32) cam.Pm[t - 16] = row[t];
-  else if (t < 35) cam.campos[t - 32] = row[t];
+  if (t < 16) cam.V[t] = V[t];
+  else if (t < 32) cam.Pm[t - 16] = Pm[t - 16];
+  else if (t < 35) cam.campos[t - 32] = campos[t - 32];
   __syncthreads();
 }
 
 // =====================================================================================================
 // K1: fused bind + activate + project + EWA + SH->RGB.  One thread per splat.
-// DEVFOV: (tanfovx, tanfovy) come from the device float[2] `tanfov` (gab200_forward_device_fov) instead of the
-// by-value args, so that a captured graph renders whatever field of view was written before the replay.
-// preprocess_views_kernel (gab200_forward_views): the same per splat, for camera row blockIdx.y of a table.
+// CAM: where the camera comes from.
+//   CAM_ARGS   : the by-value matrices and tanfovx / tanfovy of `a` (gab200_forward).
+//   CAM_DEVFOV : the same matrices, (tanfovx, tanfovy) from the device float[2] `tanfov` (gab200_forward_device_fov),
+//                so that a captured graph renders whatever field of view was written before the replay.
+//   CAM_TABLE  : row blockIdx.y of the device camera table (gab200_forward_views*), its field of view read as
+//                CAM_DEVFOV reads it; outputs at the virtual splat view * P + i, tile counts in the view's slice.
+// DA: the record also carries the view-space depth z in q2.w, read by the depth plane of the blend (forward and
+// backward).  clamped != nullptr: the per-channel colour clamp bits, which the backward reads.
 // =====================================================================================================
-template <bool BOUND, bool DEVFOV>
-__global__ void __launch_bounds__(PRE_NT) preprocess_kernel(gab200_forward_args a, SplatRec* __restrict__ rec,
+enum { CAM_ARGS, CAM_DEVFOV, CAM_TABLE };
+template <bool BOUND, int CAM, bool DA>
+__global__ void __launch_bounds__(PRE_NT) preprocess_kernel(gab200_forward_args a, const float* __restrict__ cameras,
+                                                            const float* __restrict__ tanfov, SplatRec* __restrict__ rec,
                                                             SplatAux* __restrict__ aux,
                                                             uint32_t* __restrict__ tiles_touched,
                                                             uint8_t* __restrict__ clamped,
                                                             uint32_t* __restrict__ depth_keys,
                                                             uint32_t* __restrict__ ids, int exact_binning,
-                                                            DepthBuckets bk, uint32_t* __restrict__ tile_count,
-                                                            const float* __restrict__ tanfov) {
+                                                            DepthBuckets bk, uint32_t* __restrict__ tile_count) {
   __shared__ Camera cam;
   __shared__ float sh_s[PRE_NT * SH_SMEM_STRIDE_MAX];
+  const int view = CAM == CAM_TABLE ? (int)blockIdx.y : 0;
   pdl_wait();
   pdl_trigger();
-  stage_camera(a, cam);
-#define GAB_PRE_OUT i
-#include "preprocess_splat.inc"
-#undef GAB_PRE_OUT
+  if (CAM == CAM_TABLE) {
+    const float* row = cameras + (size_t)view * GAB200_CAMERA_FLOATS;
+    stage_camera(row, row + 16, row + 32, cam);
+    tanfov = row + 35;
+    const int view_tiles = ((a.image_width + GAB_TILE - 1) / GAB_TILE) * ((a.image_height + GAB_TILE - 1) / GAB_TILE);
+    if (tile_count != nullptr) tile_count += view * view_tiles;
+  } else {
+    stage_camera(a.viewmatrix, a.projmatrix, a.campos, cam);
+  }
+  // SH coefficients of the block's splats: coalesced 128-bit loads -> shared memory (row stride odd: conflict-free)
+  const int sh_width = BOUND ? 3 * (a.sh_coeffs - 1) : 3 * a.sh_coeffs;
+  const int sh_stride = sh_width | 1;
+  const float* sh_src = BOUND ? a.sh_rest : a.shs;
+  const bool use_sh = a.colors_precomp == nullptr && sh_src != nullptr && sh_width > 0;
+  if (use_sh) {
+    const int row0 = blockIdx.x * PRE_NT;
+    stage_rows_in<PRE_NT>(sh_s, sh_src, (size_t)row0, min(PRE_NT, a.P - row0), sh_width, sh_stride);
+    __syncthreads();
+  }
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= a.P) return;
+  const int o = CAM == CAM_TABLE ? view * a.P + i : i;  // where the outputs of splat i go; inputs are read at i
+  // the other 44 bytes per splat: quaternion as one LDG.128, positions / scales / opacity as coalesced scalar loads
+  // (staging them would cost a barrier for 24 of the 284 bytes)
+  RawAttr raw;
+  load_raw(a, i, raw);
+  const float* my_sh = sh_s + threadIdx.x * sh_stride;
+  const int W = a.image_width, H = a.image_height;
+  const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
+
+  SplatRec out;
+  out.q0 = make_float4(0.f, 0.f, 0.f, 0.f);
+  out.q1 = make_float4(0.f, 0.f, 0.f, 0.f);
+  out.q2 = make_float4(0.f, 0.f, 0.f, 0.f);
+  int radius_out = 0;
+  float depth_out = 0.f;
+  uint32_t tiles_out = 0;
+  uint8_t clamp_bits = 0;
+
+  float3 p;
+  float opacity;
+  float c3[6];
+  bool have_cov = false;
+  if (BOUND) {
+    Activated act;
+    BindCtx bctx;
+    bind_activate(a, i, raw, act, bctx);
+    p = act.mean;
+    opacity = act.opacity;
+    float s[3] = {a.scale_modifier * act.s[0], a.scale_modifier * act.s[1], a.scale_modifier * act.s[2]};
+    cov3d_from_R(act.R, s, c3);
+    have_cov = true;
+  } else {
+    p = make_float3(raw.x[0], raw.x[1], raw.x[2]);
+    opacity = raw.o;
+  }
+
+  // a device field of view: one broadcast load per thread; a device value that is zero, negative or not finite culls the splat
+  // before any tile index is formed (radius 0, no instances)
+  float dev_tx = 0.f, dev_ty = 0.f;
+  bool fov_ok = true;
+  if (CAM != CAM_ARGS) {
+    dev_tx = __ldg(tanfov);
+    dev_ty = __ldg(tanfov + 1);
+    fov_ok = dev_tx > 0.f && isfinite(dev_tx) && dev_ty > 0.f && isfinite(dev_ty);
+  }
+  const float3 t = xform4x3(cam.V, p);
+  if (fov_ok && t.z > 0.2f) {
+    const float hx = cam.Pm[0] * p.x + cam.Pm[4] * p.y + cam.Pm[8] * p.z + cam.Pm[12];
+    const float hy = cam.Pm[1] * p.x + cam.Pm[5] * p.y + cam.Pm[9] * p.z + cam.Pm[13];
+    const float hw = cam.Pm[3] * p.x + cam.Pm[7] * p.y + cam.Pm[11] * p.z + cam.Pm[15];
+    const float p_w = 1.0f / (hw + 0.0000001f);
+    const float ndc_x = hx * p_w, ndc_y = hy * p_w;
+
+    if (!have_cov) {
+      if (a.cov3D_precomp != nullptr) {
+#pragma unroll
+        for (int k = 0; k < 6; k++) c3[k] = a.cov3D_precomp[6 * (size_t)i + k];
+      } else {
+        float R[9];
+        quat_to_R(raw.q[0], raw.q[1], raw.q[2], raw.q[3], R);
+        float s[3] = {a.scale_modifier * raw.s[0], a.scale_modifier * raw.s[1], a.scale_modifier * raw.s[2]};
+        cov3d_from_R(R, s, c3);
+      }
+    }
+
+    const float tanfovx = CAM != CAM_ARGS ? dev_tx : a.tanfovx, tanfovy = CAM != CAM_ARGS ? dev_ty : a.tanfovy;
+    const float focal_x = (float)W / (2.0f * tanfovx), focal_y = (float)H / (2.0f * tanfovy);
+    const float limx = 1.3f * tanfovx, limy = 1.3f * tanfovy;
+    const float txtz = t.x / t.z, tytz = t.y / t.z;
+    const float tcx = fminf(limx, fmaxf(-limx, txtz)) * t.z;
+    const float tcy = fminf(limy, fmaxf(-limy, tytz)) * t.z;
+    const float j00 = focal_x / t.z, j02 = -(focal_x * tcx) / (t.z * t.z);
+    const float j11 = focal_y / t.z, j12 = -(focal_y * tcy) / (t.z * t.z);
+    float T0[3], T1[3];
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+      T0[c] = j00 * cam.V[4 * c + 0] + j02 * cam.V[4 * c + 2];
+      T1[c] = j11 * cam.V[4 * c + 1] + j12 * cam.V[4 * c + 2];
+    }
+    const float S[9] = {c3[0], c3[1], c3[2], c3[1], c3[3], c3[4], c3[2], c3[4], c3[5]};
+    float u[3], v[3];
+#pragma unroll
+    for (int r = 0; r < 3; r++) {
+      u[r] = S[3 * r + 0] * T0[0] + S[3 * r + 1] * T0[1] + S[3 * r + 2] * T0[2];
+      v[r] = S[3 * r + 0] * T1[0] + S[3 * r + 1] * T1[1] + S[3 * r + 2] * T1[2];
+    }
+    float ca = T0[0] * u[0] + T0[1] * u[1] + T0[2] * u[2];
+    float cb = T0[0] * v[0] + T0[1] * v[1] + T0[2] * v[2];
+    float cc = T1[0] * v[0] + T1[1] * v[1] + T1[2] * v[2];
+    ca += 0.3f;
+    cc += 0.3f;
+    const float det = ca * cc - cb * cb;
+    if (det != 0.0f) {
+      const float det_inv = 1.f / det;
+      const float conic_x = cc * det_inv, conic_y = -cb * det_inv, conic_z = ca * det_inv;
+      const float mid = 0.5f * (ca + cc);
+      const float sq = sqrtf(fmaxf(0.1f, mid * mid - det));
+      const float lambda1 = mid + sq, lambda2 = mid - sq;
+      const float my_radius = ceilf(3.f * sqrtf(fmaxf(lambda1, lambda2)));
+      const float px = ndc2pix(ndc_x, W), py = ndc2pix(ndc_y, H);
+      int x0, y0, x1, y1;
+      tile_rect(px, py, (int)my_radius, gx, gy, x0, y0, x1, y1);
+      if ((x1 - x0) * (y1 - y0) != 0) {
+        float rgb[3];
+        if (a.colors_precomp != nullptr) {
+          rgb[0] = a.colors_precomp[3 * (size_t)i];
+          rgb[1] = a.colors_precomp[3 * (size_t)i + 1];
+          rgb[2] = a.colors_precomp[3 * (size_t)i + 2];
+        } else {
+          float3 d = make_float3(p.x - cam.campos[0], p.y - cam.campos[1], p.z - cam.campos[2]);
+          const float len = sqrtf(d.x * d.x + d.y * d.y + d.z * d.z);
+          d.x = d.x / len; d.y = d.y / len; d.z = d.z / len;
+          float B[16];
+          sh_basis(a.sh_degree, d, B);
+          const int nb = (a.sh_degree + 1) * (a.sh_degree + 1);
+          float acc[3] = {0.f, 0.f, 0.f};
+          if (BOUND) {
+            const float* dc = a.sh_dc + 3 * (size_t)i;
+            acc[0] = acc[0] + B[0] * dc[0];
+            acc[1] = acc[1] + B[0] * dc[1];
+            acc[2] = acc[2] + B[0] * dc[2];
+            const float* rest = my_sh;
+            for (int k = 1; k < nb; k++) {
+              acc[0] = acc[0] + B[k] * rest[3 * (k - 1) + 0];
+              acc[1] = acc[1] + B[k] * rest[3 * (k - 1) + 1];
+              acc[2] = acc[2] + B[k] * rest[3 * (k - 1) + 2];
+            }
+          } else {
+            const float* sh = my_sh;
+            for (int k = 0; k < nb; k++) {
+              acc[0] = acc[0] + B[k] * sh[3 * k + 0];
+              acc[1] = acc[1] + B[k] * sh[3 * k + 1];
+              acc[2] = acc[2] + B[k] * sh[3 * k + 2];
+            }
+          }
+#pragma unroll
+          for (int ch = 0; ch < 3; ch++) {
+            float r = acc[ch] + 0.5f;
+            if (r < 0.f) clamp_bits |= (1u << ch);
+            rgb[ch] = fmaxf(r, 0.f);
+          }
+        }
+        radius_out = (int)my_radius;
+        // conic pre-scaled for the blend kernels' exponent in log2 units: pw = A' dx^2 + B' dx dy + C' dy^2
+        out.q0 = make_float4(px, py, conic_x * REC_SCALE_AC, conic_y * REC_SCALE_B);
+        out.q1 = make_float4(conic_z * REC_SCALE_AC, opacity, rgb[0], rgb[1]);
+        // the span test must see exactly the values key emission will read back from the record
+        TileSpan span(px, py, (conic_x * REC_SCALE_AC) / REC_SCALE_AC, (conic_y * REC_SCALE_B) / REC_SCALE_B,
+                      (conic_z * REC_SCALE_AC) / REC_SCALE_AC, opacity, x0, x1);
+        const float ext_x = !span.any ? -1.f : (span.full ? 1.0e30f : span.dxmax + 0.02f);
+        const float ext_y = !span.any ? -1.f : (span.full ? 1.0e30f : span.ymax + 0.02f);
+        // instance count of the splat; with `tile_count` (counting tile sort, tile_sort.cu) also one RED per instance
+        // into its tile's counter, so that the tile ranges exist before anything is emitted
+        if (exact_binning) {
+          tiles_out = (uint32_t)((y1 - y0) * (x1 - x0));
+          if (tile_count != nullptr)
+            for (int ty = y0; ty < y1; ty++)
+              for (int x = x0; x < x1; x++) atomicAdd(tile_count + ty * gx + x, 1u);
+        } else {
+          uint32_t cnt = 0;
+          if (span.any)
+            for (int ty = y0; ty < y1; ty++) {
+              int cx0, cx1;
+              span.row(ty, cx0, cx1);
+              cnt += (uint32_t)(cx1 - cx0);
+              if (tile_count != nullptr)
+                for (int x = cx0; x < cx1; x++) atomicAdd(tile_count + ty * gx + x, 1u);
+            }
+          tiles_out = cnt;
+        }
+        // DA: z for the depth plane, the float the depth key is made from
+        out.q2 = make_float4(rgb[2], ext_x, ext_y, DA ? t.z : 0.f);
+        depth_out = t.z;
+      }
+    }
+  }
+  // stage-A sort input: the fp32 depth bit pattern (splats that emit nothing go last), value = splat id
+  const uint32_t dkey = tiles_out ? __float_as_uint(depth_out) : 0xffffffffu;
+  depth_keys[o] = dkey;
+  ids[o] = (uint32_t)o;
+  {
+    // key range of this frame (the caller's hint for the next one) and, with a hint, the bucket histogram + the
+    // splat's arrival rank in its bucket (binning.cu header)
+    const unsigned live = __activemask();
+    const uint32_t kmin = __reduce_min_sync(live, dkey);
+    const uint32_t kmax = __reduce_max_sync(live, tiles_out ? dkey : 0u);
+    const uint32_t warp_tiles = __reduce_add_sync(live, tiles_out);  // <= 32 x (tiles of the image): fits 32 bits
+    if ((threadIdx.x & 31) == (__ffs(live) - 1) && kmin != 0xffffffffu) {
+      atomicMax(bk.meta + 0, ~kmin);
+      atomicMax(bk.meta + 1, kmax);
+      // 64-bit instance total: the 32-bit emission offsets / tile ranges wrap silently beyond 2^32 - 1 instances,
+      // the host turns a non-zero high word into GAB200_ERR_OVERFLOW
+      atomicAdd(reinterpret_cast<unsigned long long*>(bk.meta + GAB_META_TOTAL64), (unsigned long long)warp_tiles);
+    }
+    if (bk.enabled && tiles_out) {
+      const uint32_t b = depth_bucket(dkey, bk);
+      bk.rank[o] = atomicAdd(bk.counts + b, 1u);
+      atomicAdd(bk.tiles + b, tiles_out);
+    }
+  }
+  rec[o] = out;
+  SplatAux ax;
+  ax.depth = depth_out; ax.radius = radius_out; ax.tiles = tiles_out; ax.pad = 0;
+  aux[o] = ax;
+  a.radii[o] = radius_out;
+  if (a.visibility != nullptr) a.visibility[o] = radius_out > 0 ? 1 : 0;
+  tiles_touched[o] = tiles_out;
+  if (clamped != nullptr) clamped[o] = clamp_bits;
 }
 
-// gab200_forward_depth_alpha: preprocess_kernel whose records also carry the view-space depth z in q2.w, read by the
-// depth plane of the blend (forward and backward)
-template <bool BOUND, bool DEVFOV>
-__global__ void __launch_bounds__(PRE_NT) preprocess_depth_kernel(gab200_forward_args a, SplatRec* __restrict__ rec,
-                                                                  SplatAux* __restrict__ aux,
-                                                                  uint32_t* __restrict__ tiles_touched,
-                                                                  uint8_t* __restrict__ clamped,
-                                                                  uint32_t* __restrict__ depth_keys,
-                                                                  uint32_t* __restrict__ ids, int exact_binning,
-                                                                  DepthBuckets bk, uint32_t* __restrict__ tile_count,
-                                                                  const float* __restrict__ tanfov) {
-  __shared__ Camera cam;
-  __shared__ float sh_s[PRE_NT * SH_SMEM_STRIDE_MAX];
-  pdl_wait();
-  pdl_trigger();
-  stage_camera(a, cam);
-#define GAB_PRE_OUT i
-#define GAB_PRE_REC_DEPTH
-#include "preprocess_splat.inc"
-#undef GAB_PRE_REC_DEPTH
-#undef GAB_PRE_OUT
+template <bool BOUND, int CAM>
+static decltype(&preprocess_kernel<BOUND, CAM, false>) preprocess_instance(bool da) {
+  return da ? preprocess_kernel<BOUND, CAM, true> : preprocess_kernel<BOUND, CAM, false>;
 }
 
-// gab200_forward_views: grid.y = view.  Camera row `view` of the table, its field of view read as DEVFOV reads it;
-// outputs at the virtual splat view * P + i, tile counts in the view's slice.
-template <bool BOUND>
-__global__ void __launch_bounds__(PRE_NT) preprocess_views_kernel(gab200_forward_args a,
-                                                                  const float* __restrict__ cameras,
-                                                                  SplatRec* __restrict__ rec, SplatAux* __restrict__ aux,
-                                                                  uint32_t* __restrict__ tiles_touched,
-                                                                  uint32_t* __restrict__ depth_keys,
-                                                                  uint32_t* __restrict__ ids, int exact_binning,
-                                                                  DepthBuckets bk, uint32_t* __restrict__ view_counts) {
-  constexpr bool DEVFOV = true;
-  __shared__ Camera cam;
-  __shared__ float sh_s[PRE_NT * SH_SMEM_STRIDE_MAX];
-  const int view = (int)blockIdx.y;
-  const float* row = cameras + (size_t)view * GAB200_CAMERA_FLOATS;
-  pdl_wait();
-  pdl_trigger();
-  stage_camera_row(row, cam);
-  const float* tanfov = row + 35;
-  uint8_t* const clamped = nullptr;
-  const int view_tiles = ((a.image_width + GAB_TILE - 1) / GAB_TILE) * ((a.image_height + GAB_TILE - 1) / GAB_TILE);
-  uint32_t* const tile_count = view_counts != nullptr ? view_counts + view * view_tiles : nullptr;
-#define GAB_PRE_OUT (view * a.P + i)
-#include "preprocess_splat.inc"
-#undef GAB_PRE_OUT
-}
-
-// gab200_forward_views_train: preprocess_views_kernel for BOUND_RAW inputs that also keeps the per-channel colour
-// clamp bits of every virtual splat, which the multi-view backward reads
-__global__ void __launch_bounds__(PRE_NT) preprocess_views_train_kernel(gab200_forward_args a,
-                                                                        const float* __restrict__ cameras,
-                                                                        SplatRec* __restrict__ rec,
-                                                                        SplatAux* __restrict__ aux,
-                                                                        uint32_t* __restrict__ tiles_touched,
-                                                                        uint8_t* __restrict__ clamped,
-                                                                        uint32_t* __restrict__ depth_keys,
-                                                                        uint32_t* __restrict__ ids, int exact_binning,
-                                                                        DepthBuckets bk,
-                                                                        uint32_t* __restrict__ view_counts) {
-  constexpr bool BOUND = true, DEVFOV = true;
-  __shared__ Camera cam;
-  __shared__ float sh_s[PRE_NT * SH_SMEM_STRIDE_MAX];
-  const int view = (int)blockIdx.y;
-  const float* row = cameras + (size_t)view * GAB200_CAMERA_FLOATS;
-  pdl_wait();
-  pdl_trigger();
-  stage_camera_row(row, cam);
-  const float* tanfov = row + 35;
-  const int view_tiles = ((a.image_width + GAB_TILE - 1) / GAB_TILE) * ((a.image_height + GAB_TILE - 1) / GAB_TILE);
-  uint32_t* const tile_count = view_counts != nullptr ? view_counts + view * view_tiles : nullptr;
-#define GAB_PRE_OUT (view * a.P + i)
-#include "preprocess_splat.inc"
-#undef GAB_PRE_OUT
-}
-
-// gab200_forward_views_depth_alpha / gab200_forward_views_train_depth_alpha: preprocess_views_kernel whose records also
-// carry the view-space depth z of virtual splat view * P + i in q2.w.  clamped != nullptr (the training form, BOUND_RAW
-// only): also the colour clamp bits, as preprocess_views_train_kernel keeps them.
-template <bool BOUND>
-__global__ void __launch_bounds__(PRE_NT) preprocess_views_depth_kernel(gab200_forward_args a,
-                                                                        const float* __restrict__ cameras,
-                                                                        SplatRec* __restrict__ rec,
-                                                                        SplatAux* __restrict__ aux,
-                                                                        uint32_t* __restrict__ tiles_touched,
-                                                                        uint8_t* __restrict__ clamped,
-                                                                        uint32_t* __restrict__ depth_keys,
-                                                                        uint32_t* __restrict__ ids, int exact_binning,
-                                                                        DepthBuckets bk,
-                                                                        uint32_t* __restrict__ view_counts) {
-  constexpr bool DEVFOV = true;
-  __shared__ Camera cam;
-  __shared__ float sh_s[PRE_NT * SH_SMEM_STRIDE_MAX];
-  const int view = (int)blockIdx.y;
-  const float* row = cameras + (size_t)view * GAB200_CAMERA_FLOATS;
-  pdl_wait();
-  pdl_trigger();
-  stage_camera_row(row, cam);
-  const float* tanfov = row + 35;
-  const int view_tiles = ((a.image_width + GAB_TILE - 1) / GAB_TILE) * ((a.image_height + GAB_TILE - 1) / GAB_TILE);
-  uint32_t* const tile_count = view_counts != nullptr ? view_counts + view * view_tiles : nullptr;
-#define GAB_PRE_OUT (view * a.P + i)
-#define GAB_PRE_REC_DEPTH
-#include "preprocess_splat.inc"
-#undef GAB_PRE_REC_DEPTH
-#undef GAB_PRE_OUT
-}
-
-void launch_preprocess(const gab200_forward_args& a, SplatRec* rec, SplatAux* aux, uint32_t* tiles_touched,
-                       uint8_t* clamped, uint32_t* depth_keys, uint32_t* ids, const DepthBuckets& buckets,
-                       uint32_t* tile_count, const float* tanfov, cudaStream_t stream, bool rec_depth) {
+void launch_preprocess(const gab200_forward_args& a, int views, const float* cameras, const float* tanfov,
+                       SplatRec* rec, SplatAux* aux, uint32_t* tiles_touched, uint8_t* clamped, uint32_t* depth_keys,
+                       uint32_t* ids, const DepthBuckets& buckets, uint32_t* tile_count, bool rec_depth,
+                       cudaStream_t stream) {
   const int threads = PRE_NT, blocks = (a.P + threads - 1) / threads;
   if (blocks == 0) return;
-  const bool bound = a.input_mode == GAB200_INPUT_BOUND_RAW;
-  auto kernel = bound ? (tanfov ? preprocess_kernel<true, true> : preprocess_kernel<true, false>)
-                      : (tanfov ? preprocess_kernel<false, true> : preprocess_kernel<false, false>);
-  if (rec_depth)
-    kernel = bound ? (tanfov ? preprocess_depth_kernel<true, true> : preprocess_depth_kernel<true, false>)
-                   : (tanfov ? preprocess_depth_kernel<false, true> : preprocess_depth_kernel<false, false>);
-  launch_pdl(kernel, blocks, threads, 0, stream, a, rec, aux, tiles_touched, clamped, depth_keys, ids, a.exact_binning,
-             buckets, tile_count, tanfov);
-}
-
-void launch_preprocess_views(const gab200_forward_args& a, int views, const float* cameras, SplatRec* rec, SplatAux* aux,
-                             uint32_t* tiles_touched, uint32_t* depth_keys, uint32_t* ids, const DepthBuckets& buckets,
-                             uint32_t* tile_count, uint8_t* clamped, cudaStream_t stream, bool rec_depth) {
-  const int threads = PRE_NT, blocks = (a.P + threads - 1) / threads;
-  if (blocks == 0) return;
-  if (rec_depth) {  // clamped != nullptr only for the training frame (BOUND_RAW, checked by the caller)
-    auto kernel = a.input_mode == GAB200_INPUT_BOUND_RAW ? preprocess_views_depth_kernel<true>
-                                                         : preprocess_views_depth_kernel<false>;
-    launch_pdl(kernel, dim3(blocks, views), threads, 0, stream, a, cameras, rec, aux, tiles_touched, clamped, depth_keys,
-               ids, a.exact_binning, buckets, tile_count);
-    return;
-  }
-  if (clamped != nullptr) {  // training frame (BOUND_RAW, checked by the caller)
-    launch_pdl(preprocess_views_train_kernel, dim3(blocks, views), threads, 0, stream, a, cameras, rec, aux,
-               tiles_touched, clamped, depth_keys, ids, a.exact_binning, buckets, tile_count);
-    return;
-  }
-  auto kernel = a.input_mode == GAB200_INPUT_BOUND_RAW ? preprocess_views_kernel<true> : preprocess_views_kernel<false>;
-  launch_pdl(kernel, dim3(blocks, views), threads, 0, stream, a, cameras, rec, aux, tiles_touched, depth_keys, ids,
-             a.exact_binning, buckets, tile_count);
+  const int cam = cameras != nullptr ? CAM_TABLE : tanfov != nullptr ? CAM_DEVFOV : CAM_ARGS;
+  auto kernel = a.input_mode == GAB200_INPUT_BOUND_RAW
+                    ? (cam == CAM_TABLE    ? preprocess_instance<true, CAM_TABLE>(rec_depth)
+                       : cam == CAM_DEVFOV ? preprocess_instance<true, CAM_DEVFOV>(rec_depth)
+                                           : preprocess_instance<true, CAM_ARGS>(rec_depth))
+                    : (cam == CAM_TABLE    ? preprocess_instance<false, CAM_TABLE>(rec_depth)
+                       : cam == CAM_DEVFOV ? preprocess_instance<false, CAM_DEVFOV>(rec_depth)
+                                           : preprocess_instance<false, CAM_ARGS>(rec_depth));
+  launch_pdl(kernel, dim3(blocks, cameras != nullptr ? views : 1), threads, 0, stream, a, cameras, tanfov, rec, aux,
+             tiles_touched, clamped, depth_keys, ids, a.exact_binning, buckets, tile_count);
 }
 
 // =====================================================================================================

@@ -194,7 +194,7 @@ class CaptureSlot:
         self.flag_host = torch.zeros(1, dtype=torch.int32).pin_memory()
         self.seq = 1
         self.info = {}
-        self.scratch = None   # a captured forward-only frame's own scratch (see _run_forward)
+        self.scratch = None   # a captured forward-only frame's own scratch (see _run_frame)
 
 
 _capture_slot = None
@@ -229,6 +229,46 @@ def check_rgb8(rgb8: Optional[torch.Tensor], rs: GaussianRasterizationSettings, 
     return rgb8
 
 
+def _run_frame(a: N.ForwardArgs, device, need_backward: bool, key, hints: FrameHints, name: str, enqueue, **extra):
+    """One forward through the library.  Inside a CUDA-graph capture (`_capture_slot`): the slot's fixed capacity and
+    counters, no host wait.  Otherwise the capacity and depth-range hints `hints` learnt from earlier frames of shape
+    `key`, updated with this frame's outcome.  enqueue(st, stream) calls the entry point; `extra` joins the info dict.
+    Returns (frame state, scratch holder, info)."""
+    slot = _capture_slot
+    # A forward-only frame captured into a graph must own its scratch: the pooled inference buffers are shared with
+    # every eager no_grad render and replaced when a larger frame comes along, so the graph's baked-in pointers would
+    # be overwritten or freed.  Allocated during the capture, the scratch lives in the graph's private pool.
+    cb, holder = N.begin_forward(device, need_backward or slot is not None)
+    if slot is not None and not need_backward:
+        slot.scratch = holder
+    a.alloc_geom = a.alloc_binning = a.alloc_image = cb
+    st = N.FrameState()
+    if slot is not None:      # graph capture: fixed capacity, no host wait; graph.py reads slot.counters after replays
+        a.sync_mode = N.SYNC_NONE
+        a.binning_hint = slot.capacity
+        a.depth_hint_lo, a.depth_hint_hi = slot.depth_range
+        a.frame_seq = slot.seq
+        a.counters_host = slot.counters.data_ptr()
+        a.overflow_flag = slot.flag.data_ptr()
+    else:
+        a.binning_hint, (a.depth_hint_lo, a.depth_hint_hi) = hints.get(key)
+        a.sync_mode = N.SYNC_LATE if (_SYNC_POLICY == "late" and a.binning_hint > 0) else N.SYNC_EXACT
+        hints.seq = (hints.seq + 1) & 0x7FFFFFFF
+        a.frame_seq = hints.seq
+    with torch.cuda.device(device):
+        n = enqueue(st, C.c_void_p(torch.cuda.current_stream(device).cuda_stream))
+    N.check(n, name)
+    info = dict(num_rendered=int(st.num_rendered), capacity=int(st.binning_capacity), sync_mode=int(a.sync_mode),
+                depth_sort_path=int(st.depth_sort_path), attempts=int(st.attempts), **extra)
+    if slot is not None:
+        slot.info = info
+    else:
+        hints.put(key, n, _widen_depth_range(st.depth_key_min, st.depth_key_max)
+                  if st.depth_key_min <= st.depth_key_max else (0, 0))
+        hints.last = info
+    return st, holder, info
+
+
 def _run_forward(a: N.ForwardArgs, device, need_backward: bool, hints: Optional[FrameHints] = None,
                  tanfov: Optional[torch.Tensor] = None, rgb8: Optional[torch.Tensor] = None, float_image: bool = True,
                  planes: Optional[tuple] = None):
@@ -244,50 +284,19 @@ def _run_forward(a: N.ForwardArgs, device, need_backward: bool, hints: Optional[
     visible = torch.empty((P,), dtype=torch.bool, device=device)   # radii > 0, written by the preprocess kernel
     a.out_color, a.radii, a.visibility = N.ptr(color), radii.data_ptr(), visible.data_ptr()
     _tls.visible = (radii.data_ptr(), visible)   # renderer.py hands it out as `visibility_filter`
-    slot = _capture_slot
-    # A forward-only frame captured into a graph must own its scratch: the pooled inference buffers are shared with
-    # every eager no_grad render and replaced when a larger frame comes along, so the graph's baked-in pointers would
-    # be overwritten or freed.  Allocated during the capture, the scratch lives in the graph's private pool.
-    cb, holder = N.begin_forward(device, need_backward or slot is not None)
-    if slot is not None and not need_backward:
-        slot.scratch = holder
-    a.alloc_geom = a.alloc_binning = a.alloc_image = cb
-    st = N.FrameState()
-    key = (device, W, H, P)
-    if slot is not None:      # graph capture: fixed capacity, no host wait; graph.py reads slot.counters after replays
-        a.sync_mode = N.SYNC_NONE
-        a.binning_hint = slot.capacity
-        a.depth_hint_lo, a.depth_hint_hi = slot.depth_range
-        a.frame_seq = slot.seq
-        a.counters_host = slot.counters.data_ptr()
-        a.overflow_flag = slot.flag.data_ptr()
+    hints = hints if hints is not None else _default_hints
+    if planes is not None:
+        enqueue = lambda st, stream: N.lib().gab200_forward_depth_alpha(  # noqa: E731
+            C.byref(a), N.ptr(tanfov), planes[0].data_ptr(), planes[1].data_ptr(), N.ptr(rgb8), C.byref(st), stream)
+    elif rgb8 is not None:
+        enqueue = lambda st, stream: N.lib().gab200_forward_display(  # noqa: E731
+            C.byref(a), N.ptr(tanfov), rgb8.data_ptr(), C.byref(st), stream)
+    elif tanfov is None:
+        enqueue = lambda st, stream: N.lib().gab200_forward(C.byref(a), C.byref(st), stream)  # noqa: E731
     else:
-        hints = hints if hints is not None else _default_hints
-        a.binning_hint, (a.depth_hint_lo, a.depth_hint_hi) = hints.get(key)
-        a.sync_mode = N.SYNC_LATE if (_SYNC_POLICY == "late" and a.binning_hint > 0) else N.SYNC_EXACT
-        hints.seq = (hints.seq + 1) & 0x7FFFFFFF
-        a.frame_seq = hints.seq
-    with torch.cuda.device(device):
-        stream = torch.cuda.current_stream(device).cuda_stream
-        if planes is not None:
-            n = N.lib().gab200_forward_depth_alpha(C.byref(a), N.ptr(tanfov), planes[0].data_ptr(),
-                                                   planes[1].data_ptr(), N.ptr(rgb8), C.byref(st), C.c_void_p(stream))
-        elif rgb8 is not None:
-            n = N.lib().gab200_forward_display(C.byref(a), N.ptr(tanfov), rgb8.data_ptr(), C.byref(st),
-                                               C.c_void_p(stream))
-        elif tanfov is None:
-            n = N.lib().gab200_forward(C.byref(a), C.byref(st), C.c_void_p(stream))
-        else:
-            n = N.lib().gab200_forward_device_fov(C.byref(a), tanfov.data_ptr(), C.byref(st), C.c_void_p(stream))
-    N.check(n, "gab200_forward")
-    info = dict(num_rendered=int(st.num_rendered), capacity=int(st.binning_capacity), sync_mode=int(a.sync_mode),
-                depth_sort_path=int(st.depth_sort_path), attempts=int(st.attempts))
-    if slot is not None:
-        slot.info = info
-    else:
-        hints.put(key, n, _widen_depth_range(st.depth_key_min, st.depth_key_max)
-                  if st.depth_key_min <= st.depth_key_max else (0, 0))
-        hints.last = info
+        enqueue = lambda st, stream: N.lib().gab200_forward_device_fov(  # noqa: E731
+            C.byref(a), tanfov.data_ptr(), C.byref(st), stream)
+    st, holder, info = _run_frame(a, device, need_backward, (device, W, H, P), hints, "gab200_forward", enqueue)
     _last_info = info
     if _KEEP_LAST:
         # pooled (inference) scratch stays valid until the next no_grad forward on this device
@@ -453,6 +462,53 @@ def _face_csr(binding: torch.Tensor, num_faces: int, chunk: int = 16):
     return b32, out
 
 
+def _fill_bound(a: N.ForwardArgs, device, _xyz, _rotation, _scaling, _opacity, f_dc, f_rest, colors_precomp, binding,
+                face_center, face_orien_mat, face_scaling):
+    """The BOUND_RAW inputs of `a` from the raw model tensors and the per-face frame.  Returns the tensors `a` points
+    at (keep them alive while the library may read them): (_xyz, _rotation, _scaling, _opacity, f_dc, f_rest,
+    colors_precomp, binding, face_center, face_orien_mat, face_scaling), binding int32 and the rest contiguous
+    float32, None where not given."""
+    a.input_mode = N.INPUT_BOUND_RAW
+    _xyz, _rotation = _f32c(_xyz, "_xyz", device), _f32c(_rotation, "_rotation", device)
+    _scaling, _opacity = _f32c(_scaling, "_scaling", device), _f32c(_opacity, "_opacity", device)
+    f_dc, f_rest = _f32c(f_dc, "_features_dc", device), _f32c(f_rest, "_features_rest", device)
+    colors_precomp = _f32c(colors_precomp, "colors_precomp", device)
+    a.sh_coeffs = 1 + (0 if f_rest is None else f_rest.shape[1])
+    a.means3D, a.rotations, a.scales, a.opacities = _xyz.data_ptr(), _rotation.data_ptr(), _scaling.data_ptr(), \
+        _opacity.data_ptr()
+    a.sh_dc, a.sh_rest, a.colors_precomp = N.ptr(f_dc), N.ptr(f_rest), N.ptr(colors_precomp)
+    if binding is not None:
+        if binding.dtype != torch.int32 or not binding.is_contiguous():
+            binding = _face_csr(binding, face_center.shape[0])[0]  # converted once per binding, not per frame
+        face_center = _f32c(face_center, "face_center", device)
+        face_orien_mat = _f32c(face_orien_mat, "face_orien_mat", device)
+        face_scaling = _f32c(face_scaling, "face_scaling", device)
+        a.binding, a.num_faces = binding.data_ptr(), face_center.shape[0]
+        a.face_center, a.face_orien_mat, a.face_scaling = face_center.data_ptr(), face_orien_mat.data_ptr(), \
+            face_scaling.data_ptr()
+    return (_xyz, _rotation, _scaling, _opacity, f_dc, f_rest, colors_precomp, binding, face_center, face_orien_mat,
+            face_scaling)
+
+
+def _grad_buffer(grad_sink, P: int, M: int, device, symm_ok: bool = True):
+    """One flat buffer for all per-splat parameter gradients (dist.py all-reduces it in ONE collective):
+    [_xyz 3 | _rotation 4 | _scaling 3 | _opacity 1 | f_dc 3 | f_rest 3(M-1)]  = 59 floats/splat at SH3.
+    It is grad_sink's symmetric gradient buffer when that is enabled, of this size and `symm_ok`, else a new tensor.
+    Returns (flat, the symmetric buffer used or None, (d_xyz, d_rot, d_scale, d_opac, d_dc, d_rest or None))."""
+    widths = (3, 4, 3, 1, 3, 3 * (M - 1))
+    symm = getattr(grad_sink, "symm_grad", None) if grad_sink is not None else None
+    if not (symm_ok and symm is not None and symm.enabled and symm.numel == P * sum(widths)):
+        symm = None
+    flat = symm.flat if symm is not None else torch.empty((P * sum(widths),), dtype=torch.float32, device=device)
+    views, off = [], 0
+    for w in widths:
+        views.append(flat[off:off + P * w])
+        off += P * w
+    grads = (views[0].view(P, 3), views[1].view(P, 4), views[2].view(P, 3), views[3].view(P, 1),
+             views[4].view(P, 1, 3), views[5].view(P, M - 1, 3) if M > 1 else None)
+    return flat, symm, grads
+
+
 class _RasterizeBound(torch.autograd.Function):
     @staticmethod
     def forward(ctx, _xyz, means2D, _rotation, _scaling, _opacity, f_dc, f_rest, face_center, face_orien_mat,
@@ -467,28 +523,11 @@ class _RasterizeBound(torch.autograd.Function):
         need_bw = any(ctx.needs_input_grad)
         a = N.ForwardArgs()
         cams = _fill_common(a, rs, device, P, need_bw)
-        a.input_mode = N.INPUT_BOUND_RAW
-        _xyz, _rotation = _f32c(_xyz, "_xyz", device), _f32c(_rotation, "_rotation", device)
-        _scaling, _opacity = _f32c(_scaling, "_scaling", device), _f32c(_opacity, "_opacity", device)
-        f_dc, f_rest = _f32c(f_dc, "_features_dc", device), _f32c(f_rest, "_features_rest", device)
-        colors_precomp = _f32c(colors_precomp, "colors_precomp", device)
-        M = 1 + (0 if f_rest is None else f_rest.shape[1])
-        a.sh_coeffs = M
-        a.means3D, a.rotations, a.scales, a.opacities = _xyz.data_ptr(), _rotation.data_ptr(), _scaling.data_ptr(), \
-            _opacity.data_ptr()
-        a.sh_dc, a.sh_rest, a.colors_precomp = N.ptr(f_dc), N.ptr(f_rest), N.ptr(colors_precomp)
-        F = 0
         binding_orig = binding
-        if binding is not None:
-            if binding.dtype != torch.int32 or not binding.is_contiguous():
-                binding = _face_csr(binding_orig, face_center.shape[0])[0]  # converted once per binding, not per frame
-            face_center = _f32c(face_center, "face_center", device)
-            face_orien_mat = _f32c(face_orien_mat, "face_orien_mat", device)
-            face_scaling = _f32c(face_scaling, "face_scaling", device)
-            F = face_center.shape[0]
-            a.binding, a.num_faces = binding.data_ptr(), F
-            a.face_center, a.face_orien_mat, a.face_scaling = face_center.data_ptr(), face_orien_mat.data_ptr(), \
-                face_scaling.data_ptr()
+        _xyz, _rotation, _scaling, _opacity, f_dc, f_rest, colors_precomp, binding, face_center, face_orien_mat, \
+            face_scaling = _fill_bound(a, device, _xyz, _rotation, _scaling, _opacity, f_dc, f_rest, colors_precomp,
+                                       binding, face_center, face_orien_mat, face_scaling)
+        M, F = a.sh_coeffs, a.num_faces
         tanfov = check_tanfov(tanfov, device)
         rgb8 = check_rgb8(rgb8, rs, device)
         if not float_image and (rgb8 is None or need_bw):
@@ -524,23 +563,13 @@ class _RasterizeBound(torch.autograd.Function):
         device = ctx.keep[1].device
         binding, colors_precomp = ctx.keep[10], ctx.keep[11]
         g = grad_out_color if grad_out_color.is_contiguous() else grad_out_color.contiguous()
-        # one flat buffer for all per-splat parameter gradients (dist.py all-reduces it in ONE collective):
-        # [_xyz 3 | _rotation 4 | _scaling 3 | _opacity 1 | f_dc 3 | f_rest 3(M-1)]  = 59 floats/splat at SH3
-        widths = (3, 4, 3, 1, 3, 3 * (M - 1))
         # frame-sharded data parallel with NVLS: the gradients are reduced INTO the symmetric buffer by the kernel
-        symm = getattr(ctx.grad_sink, "symm_grad", None) if ctx.grad_sink is not None else None
-        use_symm = symm is not None and symm.enabled and symm.numel == P * sum(widths) and colors_precomp is None
+        flat, symm, (d_xyz, d_rot, d_scale, d_opac, d_dc, d_rest) = _grad_buffer(ctx.grad_sink, P, M, device,
+                                                                                 colors_precomp is None)
+        use_symm = symm is not None
         # "push": the kernel reduces into every replica with multimem.red; "two_shot": plain stores into the local
         # replica, reduced afterwards by the NVLS all-reduce kernel (dist.SymmetricGradBuffer.end)
         use_mc = use_symm and getattr(symm, "mode", "push") == "push"
-        flat = symm.flat if use_symm else torch.empty((P * sum(widths),), dtype=torch.float32, device=device)
-        views, off = [], 0
-        for w in widths:
-            views.append(flat[off:off + P * w])
-            off += P * w
-        d_xyz, d_rot, d_scale, d_opac = views[0].view(P, 3), views[1].view(P, 4), views[2].view(P, 3), views[3].view(P, 1)
-        d_dc = views[4].view(P, 1, 3)
-        d_rest = views[5].view(P, M - 1, 3) if M > 1 else None
         d_means2D = torch.empty((P, 3), dtype=torch.float32, device=device)
         d_colors = torch.empty((P, 3), dtype=torch.float32, device=device) if colors_precomp is not None else None
         d_fc = d_fR = d_fs = None
@@ -641,6 +670,16 @@ def check_camera_table(cameras, device) -> torch.Tensor:
     return cameras
 
 
+def _views_args(rs: GaussianRasterizationSettings, P: int, need_backward: bool) -> N.ForwardArgs:
+    """The scalar fields of a K-view frame's arguments: what the views share (the cameras are in the table)."""
+    a = N.ForwardArgs()
+    a.abi_version, a.P = N.ABI_VERSION, P
+    a.sh_degree, a.image_width, a.image_height = int(rs.sh_degree), int(rs.image_width), int(rs.image_height)
+    a.scale_modifier, a.prefiltered, a.debug = float(rs.scale_modifier), int(bool(rs.prefiltered)), int(bool(rs.debug))
+    a.need_backward, a.exact_binning = int(need_backward), int(_EXACT_BINNING)
+    return a
+
+
 def rasterize_bound_views(raster_settings: GaussianRasterizationSettings, cameras: torch.Tensor, _xyz, _rotation,
                           _scaling, _opacity, features_dc, features_rest, binding=None, face_center=None,
                           face_orien_mat=None, face_scaling=None, colors_precomp=None, hints: Optional[FrameHints] = None,
@@ -669,31 +708,13 @@ def rasterize_bound_views(raster_settings: GaussianRasterizationSettings, camera
         raise RuntimeError("gaussianavatars_b200 has no CPU path: tensors must be CUDA tensors")
     cameras = check_camera_table(cameras, device)
     K, P, H, W = int(cameras.shape[0]), int(_xyz.shape[0]), int(rs.image_height), int(rs.image_width)
-    a = N.ForwardArgs()
-    a.abi_version, a.input_mode, a.P = N.ABI_VERSION, N.INPUT_BOUND_RAW, P
-    a.sh_degree, a.image_width, a.image_height = int(rs.sh_degree), W, H
-    a.scale_modifier, a.prefiltered, a.debug = float(rs.scale_modifier), int(bool(rs.prefiltered)), int(bool(rs.debug))
-    a.need_backward, a.exact_binning = 0, int(_EXACT_BINNING)
+    a = _views_args(rs, P, need_backward=False)
     bg = _cam(rs.bg, "bg", device)
     a.bg = bg.data_ptr()
     if _opacity.ndim == 1:
         _opacity = _opacity[:, None]
-    keep = [_f32c(t, n, device) for t, n in ((_xyz, "_xyz"), (_rotation, "_rotation"), (_scaling, "_scaling"),
-                                              (_opacity, "_opacity"), (features_dc, "_features_dc"),
-                                              (features_rest, "_features_rest"), (colors_precomp, "colors_precomp"))]
-    _xyz, _rotation, _scaling, _opacity, f_dc, f_rest, colors_precomp = keep
-    a.sh_coeffs = 1 + (0 if f_rest is None else f_rest.shape[1])
-    a.means3D, a.rotations, a.scales, a.opacities = _xyz.data_ptr(), _rotation.data_ptr(), _scaling.data_ptr(), \
-        _opacity.data_ptr()
-    a.sh_dc, a.sh_rest, a.colors_precomp = N.ptr(f_dc), N.ptr(f_rest), N.ptr(colors_precomp)
-    if binding is not None:
-        binding = _face_csr(binding, face_center.shape[0])[0] if (binding.dtype != torch.int32 or
-                                                                  not binding.is_contiguous()) else binding
-        face = [_f32c(t, n, device) for t, n in ((face_center, "face_center"), (face_orien_mat, "face_orien_mat"),
-                                                  (face_scaling, "face_scaling"))]
-        keep += face + [binding]
-        a.binding, a.num_faces = binding.data_ptr(), face[0].shape[0]
-        a.face_center, a.face_orien_mat, a.face_scaling = (t.data_ptr() for t in face)
+    keep = _fill_bound(a, device, _xyz, _rotation, _scaling, _opacity, features_dc, features_rest,  # noqa: F841
+                       colors_precomp, binding, face_center, face_orien_mat, face_scaling)
     color = torch.empty((K, 3, H, W), dtype=torch.float32, device=device) if float_image else None
     rgb8 = torch.empty((K, H, W, 3), dtype=torch.uint8, device=device) if display else None
     radii = torch.empty((K, P), dtype=torch.int32, device=device)
@@ -703,41 +724,14 @@ def rasterize_bound_views(raster_settings: GaussianRasterizationSettings, camera
     if depth_alpha:
         planes = (torch.empty((K, 1, H, W), dtype=torch.float32, device=device),
                   torch.empty((K, 1, H, W), dtype=torch.float32, device=device))
-    slot = _capture_slot
-    cb, holder = N.begin_forward(device, slot is not None)   # captured: the graph owns its scratch (see _run_forward)
-    if slot is not None:
-        slot.scratch = holder
-    a.alloc_geom = a.alloc_binning = a.alloc_image = cb
-    st = N.FrameState()
-    key = (device, W, H, P, K)
-    if slot is not None:
-        a.sync_mode, a.binning_hint = N.SYNC_NONE, slot.capacity
-        a.depth_hint_lo, a.depth_hint_hi = slot.depth_range
-        a.frame_seq, a.counters_host, a.overflow_flag = slot.seq, slot.counters.data_ptr(), slot.flag.data_ptr()
+        enqueue = lambda st, stream: N.lib().gab200_forward_views_depth_alpha(  # noqa: E731
+            C.byref(a), K, cameras.data_ptr(), planes[0].data_ptr(), planes[1].data_ptr(), N.ptr(rgb8), C.byref(st),
+            stream)
     else:
-        hints = hints if hints is not None else FrameHints()
-        a.binning_hint, (a.depth_hint_lo, a.depth_hint_hi) = hints.get(key)
-        a.sync_mode = N.SYNC_LATE if (_SYNC_POLICY == "late" and a.binning_hint > 0) else N.SYNC_EXACT
-        hints.seq = (hints.seq + 1) & 0x7FFFFFFF
-        a.frame_seq = hints.seq
-    with torch.cuda.device(device):
-        stream = torch.cuda.current_stream(device).cuda_stream
-        if planes is not None:
-            n = N.lib().gab200_forward_views_depth_alpha(C.byref(a), K, cameras.data_ptr(), planes[0].data_ptr(),
-                                                         planes[1].data_ptr(), N.ptr(rgb8), C.byref(st),
-                                                         C.c_void_p(stream))
-        else:
-            n = N.lib().gab200_forward_views(C.byref(a), K, cameras.data_ptr(), N.ptr(rgb8), C.byref(st),
-                                             C.c_void_p(stream))
-    N.check(n, "gab200_forward_views")
-    info = dict(num_rendered=int(st.num_rendered), capacity=int(st.binning_capacity), sync_mode=int(a.sync_mode),
-                depth_sort_path=int(st.depth_sort_path), attempts=int(st.attempts), views=K)
-    if slot is not None:
-        slot.info = info
-    else:
-        hints.put(key, n, _widen_depth_range(st.depth_key_min, st.depth_key_max)
-                  if st.depth_key_min <= st.depth_key_max else (0, 0))
-        hints.last = info
+        enqueue = lambda st, stream: N.lib().gab200_forward_views(  # noqa: E731
+            C.byref(a), K, cameras.data_ptr(), N.ptr(rgb8), C.byref(st), stream)
+    _run_frame(a, device, False, (device, W, H, P, K), hints if hints is not None else FrameHints(),
+               "gab200_forward_views", enqueue, views=K)
     if planes is not None:
         return color, rgb8, radii, visible, planes[0], planes[1]
     return color, rgb8, radii, visible
@@ -753,33 +747,14 @@ class _RasterizeBoundViews(torch.autograd.Function):
         ctx.grad_sink = grad_sink
         device = _xyz.device
         K, P, H, W = int(cameras.shape[0]), int(_xyz.shape[0]), int(rs.image_height), int(rs.image_width)
-        a = N.ForwardArgs()
-        a.abi_version, a.input_mode, a.P = N.ABI_VERSION, N.INPUT_BOUND_RAW, P
-        a.sh_degree, a.image_width, a.image_height = int(rs.sh_degree), W, H
-        a.scale_modifier, a.prefiltered, a.debug = float(rs.scale_modifier), int(bool(rs.prefiltered)), int(bool(rs.debug))
-        a.need_backward, a.exact_binning = 1, int(_EXACT_BINNING)
+        a = _views_args(rs, P, need_backward=True)
         bg = _cam(rs.bg, "bg", device)
         a.bg = bg.data_ptr()
-        _xyz, _rotation = _f32c(_xyz, "_xyz", device), _f32c(_rotation, "_rotation", device)
-        _scaling, _opacity = _f32c(_scaling, "_scaling", device), _f32c(_opacity, "_opacity", device)
-        f_dc, f_rest = _f32c(f_dc, "_features_dc", device), _f32c(f_rest, "_features_rest", device)
-        M = 1 + (0 if f_rest is None else f_rest.shape[1])
-        a.sh_coeffs = M
-        a.means3D, a.rotations, a.scales, a.opacities = _xyz.data_ptr(), _rotation.data_ptr(), _scaling.data_ptr(), \
-            _opacity.data_ptr()
-        a.sh_dc, a.sh_rest = N.ptr(f_dc), N.ptr(f_rest)
-        F = 0
         binding_orig = binding
-        if binding is not None:
-            if binding.dtype != torch.int32 or not binding.is_contiguous():
-                binding = _face_csr(binding_orig, face_center.shape[0])[0]
-            face_center = _f32c(face_center, "face_center", device)
-            face_orien_mat = _f32c(face_orien_mat, "face_orien_mat", device)
-            face_scaling = _f32c(face_scaling, "face_scaling", device)
-            F = face_center.shape[0]
-            a.binding, a.num_faces = binding.data_ptr(), F
-            a.face_center, a.face_orien_mat, a.face_scaling = face_center.data_ptr(), face_orien_mat.data_ptr(), \
-                face_scaling.data_ptr()
+        _xyz, _rotation, _scaling, _opacity, f_dc, f_rest, _, binding, face_center, face_orien_mat, face_scaling = \
+            _fill_bound(a, device, _xyz, _rotation, _scaling, _opacity, f_dc, f_rest, None, binding, face_center,
+                        face_orien_mat, face_scaling)
+        M, F = a.sh_coeffs, a.num_faces
         color = torch.empty((K, 3, H, W), dtype=torch.float32, device=device)
         radii = torch.empty((K, P), dtype=torch.int32, device=device)
         visible = torch.empty((K, P), dtype=torch.bool, device=device)
@@ -789,38 +764,13 @@ class _RasterizeBoundViews(torch.autograd.Function):
         if depth_alpha:
             planes = (torch.empty((K, 1, H, W), dtype=torch.float32, device=device),
                       torch.empty((K, 1, H, W), dtype=torch.float32, device=device))
-        slot = _capture_slot
-        cb, holder = N.begin_forward(device, True)
-        a.alloc_geom = a.alloc_binning = a.alloc_image = cb
-        st = N.FrameState()
-        key = (device, W, H, P, K)
-        if slot is not None:
-            a.sync_mode, a.binning_hint = N.SYNC_NONE, slot.capacity
-            a.depth_hint_lo, a.depth_hint_hi = slot.depth_range
-            a.frame_seq, a.counters_host, a.overflow_flag = slot.seq, slot.counters.data_ptr(), slot.flag.data_ptr()
+            enqueue = lambda st, stream: N.lib().gab200_forward_views_train_depth_alpha(  # noqa: E731
+                C.byref(a), K, cameras.data_ptr(), planes[0].data_ptr(), planes[1].data_ptr(), C.byref(st), stream)
         else:
-            a.binning_hint, (a.depth_hint_lo, a.depth_hint_hi) = hints.get(key)
-            a.sync_mode = N.SYNC_LATE if (_SYNC_POLICY == "late" and a.binning_hint > 0) else N.SYNC_EXACT
-            hints.seq = (hints.seq + 1) & 0x7FFFFFFF
-            a.frame_seq = hints.seq
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            if planes is not None:
-                n = N.lib().gab200_forward_views_train_depth_alpha(C.byref(a), K, cameras.data_ptr(),
-                                                                   planes[0].data_ptr(), planes[1].data_ptr(),
-                                                                   C.byref(st), C.c_void_p(stream))
-            else:
-                n = N.lib().gab200_forward_views_train(C.byref(a), K, cameras.data_ptr(), C.byref(st),
-                                                       C.c_void_p(stream))
-        N.check(n, "gab200_forward_views_train")
-        info = dict(num_rendered=int(st.num_rendered), capacity=int(st.binning_capacity), sync_mode=int(a.sync_mode),
-                    depth_sort_path=int(st.depth_sort_path), attempts=int(st.attempts), views=K)
-        if slot is not None:
-            slot.info = info
-        else:
-            hints.put(key, n, _widen_depth_range(st.depth_key_min, st.depth_key_max)
-                      if st.depth_key_min <= st.depth_key_max else (0, 0))
-            hints.last = info
+            enqueue = lambda st, stream: N.lib().gab200_forward_views_train(  # noqa: E731
+                C.byref(a), K, cameras.data_ptr(), C.byref(st), stream)
+        st, holder, _ = _run_frame(a, device, True, (device, W, H, P, K), hints, "gab200_forward_views_train",
+                                   enqueue, views=K)
         ctx.args, ctx.state, ctx.holder = a, st, holder
         ctx.keep = (bg, cameras, _xyz, _rotation, _scaling, _opacity, f_dc, f_rest, face_center, face_orien_mat,
                     face_scaling, binding)
@@ -841,19 +791,9 @@ class _RasterizeBoundViews(torch.autograd.Function):
         cameras = ctx.keep[1]
         device = cameras.device
         g = grad_out_color if grad_out_color.is_contiguous() else grad_out_color.contiguous()
-        # the flat per-splat gradient buffer of _RasterizeBound: [_xyz 3 | _rotation 4 | _scaling 3 | _opacity 1 |
-        # f_dc 3 | f_rest 3(M-1)], holding the sum over the K views
-        widths = (3, 4, 3, 1, 3, 3 * (M - 1))
-        symm = getattr(ctx.grad_sink, "symm_grad", None) if ctx.grad_sink is not None else None
-        use_symm = symm is not None and symm.enabled and symm.numel == P * sum(widths)
-        flat = symm.flat if use_symm else torch.empty((P * sum(widths),), dtype=torch.float32, device=device)
-        views, off = [], 0
-        for w in widths:
-            views.append(flat[off:off + P * w])
-            off += P * w
-        d_xyz, d_rot, d_scale, d_opac = views[0].view(P, 3), views[1].view(P, 4), views[2].view(P, 3), views[3].view(P, 1)
-        d_dc = views[4].view(P, 1, 3)
-        d_rest = views[5].view(P, M - 1, 3) if M > 1 else None
+        # the flat per-splat gradient buffer of _RasterizeBound, holding the sum over the K views
+        flat, symm, (d_xyz, d_rot, d_scale, d_opac, d_dc, d_rest) = _grad_buffer(ctx.grad_sink, P, M, device)
+        use_symm = symm is not None
         d_means2D = torch.empty((K, P, 3), dtype=torch.float32, device=device)
         d_fc = d_fR = d_fs = None
         if ctx.want_face:
