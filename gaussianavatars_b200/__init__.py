@@ -14,6 +14,7 @@ from .io import load_ply, save_ply, load_flame_param, save_flame_param
 from .densify import densify_and_prune, densify_arrays, add_densification_stats
 from .flame import FlameLBS, flame_pose, flame_param_groups
 from .mesh import mesh_overlay, MeshRenderer
+from .lpips import LpipsNet, lpips, launch_lpips, lpips_features
 
 __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gaussians", "rasterize_bound",
            "bind_activate", "set_exact_binning", "face_frame", "l1_loss_u8", "render", "render_bound", "render_display", "render_views",
@@ -21,4 +22,4 @@ __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gau
            "photometric_loss", "image_metrics", "Adam", "binding_regularizers", "load_ply", "save_ply", "load_flame_param", "save_flame_param", "densify_and_prune", "densify_arrays",
            "add_densification_stats", "expon_lr_schedule", "FlameLBS", "flame_pose", "flame_param_groups",
            "mesh_overlay", "MeshRenderer", "composite_rgba", "FrameStore",
-           "ViewSchedule", "epoch_order"]
+           "ViewSchedule", "epoch_order", "LpipsNet", "lpips", "launch_lpips", "lpips_features"]

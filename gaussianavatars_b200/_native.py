@@ -93,6 +93,19 @@ class MetricsArgs(C.Structure):
     ]
 
 
+LPIPS_ALEX, LPIPS_VGG16 = 0, 1
+
+
+class LpipsArgs(C.Structure):
+    """Mirror of gab200_lpips_args."""
+    _fields_ = [
+        ("abi_version", C.c_uint32), ("net", C.c_int32), ("height", C.c_int32), ("width", C.c_int32),
+        ("render_kind", C.c_int32), ("render", C.c_void_p), ("gt", C.c_void_p), ("weights", C.c_void_p),
+        ("row", C.c_void_p), ("table", C.c_void_p), ("table_rows", C.c_int32), ("skip_flag", C.c_void_p),
+        ("scratch", C.c_void_p), ("features", C.c_void_p),
+    ]
+
+
 MESH_POS_WORLD, MESH_POS_CLIP = 0, 1
 MESH_LIGHT_FRONT, MESH_LIGHT_CONSTANT = 0, 1
 MESH_BASE_NONE, MESH_BASE_FLOAT_CHW, MESH_BASE_U8_CHW = 0, 1, 2
@@ -219,7 +232,9 @@ EXPORTED_SYMBOLS = ("gab200_forward", "gab200_backward", "gab200_mark_visible", 
                     "gab200_forward_views_depth_alpha", "gab200_forward_views_train_depth_alpha",
                     "gab200_backward_views_depth_alpha", "gab200_composite_rgba",
                     "gab200_frame_encode_plan", "gab200_frame_encode", "gab200_frame_decode",
-                    "gab200_schedule_sample", "gab200_schedule_commit")
+                    "gab200_schedule_sample", "gab200_schedule_commit", "gab200_lpips_weights_bytes",
+                    "gab200_lpips_pack", "gab200_lpips_scratch_bytes", "gab200_lpips_features_bytes",
+                    "gab200_lpips")
 
 _lib = None
 _lock = threading.Lock()
@@ -334,6 +349,17 @@ def lib():
         L.gab200_image_metrics.argtypes = [C.POINTER(MetricsArgs), C.c_void_p]
         L.gab200_image_metrics_scratch_bytes.restype = C.c_size_t
         L.gab200_image_metrics_scratch_bytes.argtypes = [C.c_int32, C.c_int32]
+        L.gab200_lpips_weights_bytes.restype = C.c_size_t
+        L.gab200_lpips_weights_bytes.argtypes = [C.c_int32]
+        L.gab200_lpips_pack.restype = C.c_int32
+        L.gab200_lpips_pack.argtypes = [C.c_int32, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                        C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p]
+        L.gab200_lpips_scratch_bytes.restype = C.c_size_t
+        L.gab200_lpips_scratch_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
+        L.gab200_lpips_features_bytes.restype = C.c_size_t
+        L.gab200_lpips_features_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
+        L.gab200_lpips.restype = C.c_int32
+        L.gab200_lpips.argtypes = [C.POINTER(LpipsArgs), C.c_void_p]
         L.gab200_mesh_render.restype = C.c_int32
         L.gab200_mesh_render.argtypes = [C.POINTER(MeshArgs), C.c_void_p]
         L.gab200_mesh_scratch_bytes.restype = C.c_size_t

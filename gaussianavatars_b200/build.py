@@ -36,6 +36,7 @@ SOURCES = {
     "frames.cu": [],
     "schedule.cu": [],
     "metrics.cu": [],
+    "lpips.cu": [],
     "mesh.cu": ["--fmad=false"],
     "optim.cu": [],
 }

@@ -1048,6 +1048,42 @@ int32_t gab200_image_metrics(const gab200_metrics_args* a, void* stream_) {
   return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
 }
 
+size_t gab200_lpips_weights_bytes(int32_t net) { return lpips_weights_bytes(net); }
+
+int32_t gab200_lpips_pack(int32_t net, const float* const* conv_weight, const float* const* conv_bias,
+                          const float* const* lin_weight, void* packed, void* stream_) {
+  const int nconv = lpips_conv_count(net);
+  if (nconv == 0 || !conv_weight || !conv_bias || !lin_weight || !packed || ((uintptr_t)packed & 15) != 0)
+    return GAB200_ERR_INVALID_ARGUMENT;
+  for (int l = 0; l < nconv; l++)
+    if (!conv_weight[l] || !conv_bias[l]) return GAB200_ERR_INVALID_ARGUMENT;
+  for (int t = 0; t < 5; t++)
+    if (!lin_weight[t]) return GAB200_ERR_INVALID_ARGUMENT;
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  launch_lpips_pack(net, conv_weight, conv_bias, lin_weight, static_cast<float*>(packed), (cudaStream_t)stream_);
+  return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
+size_t gab200_lpips_scratch_bytes(int32_t net, int32_t height, int32_t width) {
+  return lpips_scratch_bytes(net, height, width);
+}
+
+size_t gab200_lpips_features_bytes(int32_t net, int32_t height, int32_t width) {
+  return lpips_features_bytes(net, height, width);
+}
+
+int32_t gab200_lpips(const gab200_lpips_args* a, void* stream_) {
+  if (a == nullptr || a->abi_version != GAB200_ABI_VERSION || a->table_rows < 1 || !a->render || !a->gt ||
+      !a->weights || !a->table || !a->scratch || ((uintptr_t)a->weights & 15) != 0 ||
+      ((uintptr_t)a->scratch & 15) != 0 || ((uintptr_t)a->features & 15) != 0 ||
+      (a->render_kind != GAB200_METRICS_FLOAT_CHW && a->render_kind != GAB200_METRICS_U8_HWC) ||
+      lpips_scratch_bytes(a->net, a->height, a->width) == 0)
+    return GAB200_ERR_INVALID_ARGUMENT;
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  launch_lpips(*a, (cudaStream_t)stream_);
+  return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
 static const int kMeshMaxSide = 16384;  // snapped coordinates (guard band + image) stay below 2^24 / 256 px
 
 size_t gab200_mesh_scratch_bytes(int32_t num_faces, int32_t width, int32_t height) {

@@ -256,6 +256,15 @@ size_t metrics_scratch_bytes(int H, int W);
 void launch_image_metrics(int H, int W, int kind, const void* render, const uint8_t* gt, const int32_t* row, int rows,
                           const int32_t* skip, float* table, void* scratch, cudaStream_t stream);
 
+// lpips.cu
+size_t lpips_weights_bytes(int net);
+size_t lpips_scratch_bytes(int net, int H, int W);
+size_t lpips_features_bytes(int net, int H, int W);
+int lpips_conv_count(int net);
+void launch_lpips_pack(int net, const float* const* conv_w, const float* const* conv_b, const float* const* lin,
+                       float* packed, cudaStream_t stream);
+void launch_lpips(const gab200_lpips_args& a, cudaStream_t stream);
+
 // mesh.cu
 size_t mesh_scratch_bytes(int F, int W, int H);
 cudaError_t launch_mesh_render(const gab200_mesh_args& a, cudaStream_t stream);

@@ -56,6 +56,7 @@ from .densify import add_densification_stats
 from .training import (METRIC_NAMES, Adam, binding_regularizers, launch_composite_rgba, launch_image_metrics,
                        metrics_scratch, photometric_loss)
 from .flame import check_timestep, flame_pose
+from .lpips import LpipsNet, launch_lpips, lpips_scratch
 
 _STATS = ("xyz_gradient_accum", "denom", "max_radii2D")
 _FLAME_KEYS = ("shape", "static_offset", "expr", "rotation", "neck_pose", "jaw_pose", "eyes_pose", "translation")
@@ -1199,12 +1200,15 @@ class GraphedEval(GraphedRender):
     next replay waits for.  What re-captures is exactly what re-captures a GraphedRender.  The capacity is sized and
     guarded as there; a replay that overflowed its capacity writes no row (the metrics launch reads the slot's sticky
     overflow flag), so a truncated render never produces a score: `scores()` then raises, naming the rows to redo
-    after `regrow()`.  `run(check=True)` re-captures and replays an overflowing view at once.  The rendered images
-    stay in `image` / `display` for what this graph does not compute (LPIPS)."""
+    after `regrow()`.  `run(check=True)` re-captures and replays an overflowing view at once.
+
+    lpips=net (an lpips.LpipsNet): the body also scores each view's LPIPS distance (gab200_lpips) into row `view` of
+    a (views,) device table, with the same rows and the same overflow flag as the metrics; scores() then adds
+    `lpips_per_view` and `lpips`.  training_report uses LpipsNet.from_hub_cache("alex"), metrics.py "vgg"."""
 
     def __init__(self, pc, width: int, height: int, bg: torch.Tensor, views: int, source: str = "float",
                  host_slots: int = 0, capacity: Optional[int] = None, headroom: float = 1.25, warm_cameras=None,
-                 warm_timesteps=None, views_per_replay: int = 1, schedule=None, frames=None):
+                 warm_timesteps=None, views_per_replay: int = 1, schedule=None, frames=None, lpips=None):
         """views_per_replay=K > 1: one replay renders K cameras of one timestep in one forward and scores them into
         rows view .. view + K - 1 (set_inputs(cameras=K cameras, gt_u8=(K,3,H,W), view=first row)); warm_cameras is a
         list of K-camera groups.  K is fixed per capture: a last group of fewer views is the business of a
@@ -1225,11 +1229,22 @@ class GraphedEval(GraphedRender):
             raise ValueError("views must be at least 1")
         if isinstance(views_per_replay, int) and views_per_replay > int(views):
             raise ValueError(f"views_per_replay={views_per_replay} exceeds the table's {int(views)} rows")
+        if lpips is not None:
+            if not isinstance(lpips, LpipsNet):
+                raise TypeError(f"lpips must be an LpipsNet, got {type(lpips).__name__}")
+            if min(int(width), int(height)) < lpips.min_side:
+                raise ValueError(f"LPIPS with {lpips.net} needs an image of at least {lpips.min_side}x"
+                                 f"{lpips.min_side} pixels, got {int(width)}x{int(height)}")
         super().__init__(pc, width, height, bg, outputs="float" if source == "float" else "u8", host_slots=host_slots,
                          capacity=capacity, headroom=headroom, warm_cameras=warm_cameras, warm_timesteps=warm_timesteps,
                          views_per_replay=views_per_replay)
         self.source, self.views = source, int(views)
         self.table = torch.empty((self.views, N.METRICS_FIELDS), dtype=torch.float32, device=self.device)
+        if lpips is not None and lpips.device != self.device:
+            raise ValueError(f"the LpipsNet is on {lpips.device}, the model on {self.device}")
+        self.lpips = lpips
+        self.lpips_table = torch.empty(self.views, dtype=torch.float32, device=self.device) \
+            if lpips is not None else None
         self.frames = frames
         self.frame_ids = None
         if (schedule is None) != (frames is None):
@@ -1253,8 +1268,10 @@ class GraphedEval(GraphedRender):
         self._metrics_scratch = None
 
     def reset(self):
-        """Every row of the table back to NaN (no score); with a schedule, the cursor back to its first record."""
+        """Every row of the tables back to NaN (no score); with a schedule, the cursor back to its first record."""
         self.table.fill_(float("nan"))
+        if self.lpips_table is not None:
+            self.lpips_table.fill_(float("nan"))
         if self.schedule is not None:
             self.set_cursor(0)
 
@@ -1309,18 +1326,27 @@ class GraphedEval(GraphedRender):
                 for k in range(self.K):
                     launch_image_metrics(rendered[k], self.gt[k], self.table, row=self.rows[k:k + 1],
                                          skip_flag=self.slot.flag, scratch=self._metrics_scratch)
+            if self.lpips is not None:   # after the metrics, into the same rows, under the same flag
+                for k in range(self.K):
+                    launch_lpips(rendered if self.K == 1 else rendered[k], self.gt if self.K == 1 else self.gt[k],
+                                 self.lpips, self.lpips_table, row=self.view if self.K == 1 else self.rows[k:k + 1],
+                                 skip_flag=self.slot.flag, scratch=self._lpips_scratch)
             if self.schedule is not None:
                 self._launch_commit()
 
     def _before_capture(self):
         super()._before_capture()
         self._metrics_scratch = metrics_scratch(self.H, self.W, self.device)
+        self._lpips_scratch = lpips_scratch(self.lpips, self.H, self.W) if self.lpips is not None else None
 
     def _state_key(self):
-        """Beyond a GraphedRender's key: with a frame store, the addresses of its arena and index."""
+        """Beyond a GraphedRender's key: with a frame store, the addresses of its arena and index; with LPIPS, the
+        address of the packed weights."""
         key = super()._state_key()
         if self.frames is not None:
             key.append(self.frames.pointers())
+        if self.lpips is not None:
+            key.append(self.lpips.weights.data_ptr())
         return key
 
     # ---- replay ----------------------------------------------------------------------------------------------------
@@ -1353,13 +1379,18 @@ class GraphedEval(GraphedRender):
         """Synchronises once and returns the first n rows (default: all): `per_view`, a (n, 4) float32 host tensor
         {l1, psnr, psnr_all, ssim}, and the mean of each column as training_report forms its means (the per-view floats
         summed in double, then divided by n: train.py:286-303).  `psnr` is train.py's PSNR, `psnr_all` metrics.py's.
+        With lpips=: `lpips_per_view`, a (n,) float32 host tensor, and `lpips`, its mean formed the same way.
         Raises if a requested row holds no score (NaN): its replay overflowed the capacity (run(check=False)), or the
         view was never run."""
         n = self.views if n is None else int(n)
         if not 1 <= n <= self.views:
             raise IndexError(f"n must lie in [1, {self.views}]")
         rows = self.table[:n].cpu()
-        missing = torch.isnan(rows).any(dim=1).nonzero().flatten().tolist()
+        nan = torch.isnan(rows).any(dim=1)
+        if self.lpips_table is not None:
+            lp = self.lpips_table[:n].cpu()
+            nan |= torch.isnan(lp)
+        missing = nan.nonzero().flatten().tolist()
         if missing:
             raise RuntimeError(f"GraphedEval: rows {missing} hold no score -- their replay overflowed the instance "
                                "capacity (run(check=False)) or never ran: call regrow() and run those views again")
@@ -1369,4 +1400,10 @@ class GraphedEval(GraphedRender):
             for v in rows[:, i].tolist():
                 total += v
             out[name] = total / n
+        if self.lpips_table is not None:
+            out["lpips_per_view"] = lp
+            total = 0.0
+            for v in lp.tolist():
+                total += v
+            out["lpips"] = total / n
         return out

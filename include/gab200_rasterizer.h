@@ -533,6 +533,64 @@ typedef struct gab200_metrics_args {
 size_t gab200_image_metrics_scratch_bytes(int32_t height, int32_t width);
 int32_t gab200_image_metrics(const gab200_metrics_args* args, void* stream);
 
+/* LPIPS distance (v0.1) of one rendered view against its ground truth, forward only, with no host wait (capturable).
+ * Replaces lpipsPyTorch's LPIPS as the reference calls it: AlexNet in training_report (train.py:290-302, per val / test
+ * view of the clamped render), VGG-16 in metrics.py:74 (the PNG bytes render.py wrote, read back as value/255).
+ *   Input: render and gt as gab200_image_metrics reads them (render_kind, clamp, value/255), each z-scored as
+ *     (x - (-.030, -.088, -.188)) / (.458, .448, .450) in float32 -- on [0, 1] inputs, as the reference does.
+ *   Network: torchvision's alexnet().features / vgg16().features up to the last target ReLU; the targets are the
+ *     ReLU before each pool and the last one (AlexNet relu1..relu5; VGG-16 relu1_2, relu2_2, relu3_3, relu4_3,
+ *     relu5_3).  Convolutions run on the tensor cores with TF32 operands rounded to nearest and FP32 accumulation,
+ *     the K loop in one fixed order; pools are exact.
+ *   Head: per target pixel f / (sqrt(sum_c f^2) + 1e-10) of both images, the squared difference, the lin layer's
+ *     dot product (FP32); per layer the mean over the pixels (sums in double, fixed order); the five means summed.
+ * The distance goes to table[*row] ((table_rows,) float32; row is a DEVICE int32, NULL = 0; a row outside
+ * [0, table_rows) writes nothing), unless *skip_flag (DEVICE int32 or NULL) is non-zero when the kernel runs.  No
+ * floating-point atomics: the same inputs and weights give bit-identical results on every call.
+ * weights: gab200_lpips_weights_bytes(net) bytes filled by gab200_lpips_pack, 16-byte aligned.
+ * scratch: gab200_lpips_scratch_bytes(net, height, width) bytes, 16-byte aligned: the per-CTA partial sums and two
+ *   activation buffers of both images (VGG-16 at 1920x1080: 2 x 1.06 GB).
+ * features: NULL, or a 16-byte aligned buffer of gab200_lpips_features_bytes(net, height, width) bytes that receives
+ *   every stage's output in float32, in order -- the
+ *   z-scored input (4 channels, the 4th 0), then each convolution's post-ReLU output and each pool's output -- each as
+ *   [2][H_s][W_s][C_s] (image 0 the render, image 1 the ground truth).  A test surface: the stages then write there
+ *   instead of the scratch buffers.
+ * gab200_lpips_scratch_bytes and gab200_lpips_features_bytes are 0 for an unknown net, and for an image the network
+ * cannot take: below 31 x 31 (AlexNet) or 16 x 16 (VGG-16) in either side.
+ * Invalid arguments (GAB200_ERR_INVALID_ARGUMENT): a NULL args, render, gt, weights, table or scratch, a misaligned
+ * weights, scratch or features, an unknown net or render_kind, a size gab200_lpips_scratch_bytes refuses,
+ * table_rows < 1, abi_version != GAB200_ABI_VERSION. */
+typedef enum gab200_lpips_net {
+  GAB200_LPIPS_ALEX = 0,
+  GAB200_LPIPS_VGG16 = 1
+} gab200_lpips_net;
+typedef struct gab200_lpips_args {
+  uint32_t abi_version;
+  int32_t net;              /* gab200_lpips_net */
+  int32_t height, width;
+  int32_t render_kind;      /* gab200_metrics_render_kind */
+  const void* render;       /* float [3,H,W] | uint8 [H,W,3] */
+  const uint8_t* gt;        /* [3,H,W] */
+  const void* weights;      /* gab200_lpips_pack's buffer */
+  const int32_t* row;       /* DEVICE int32 or NULL (= 0) */
+  float* table;             /* [table_rows] */
+  int32_t table_rows;
+  const int32_t* skip_flag; /* DEVICE int32 or NULL */
+  void* scratch;
+  float* features;          /* NULL, or every stage's output (see above) */
+} gab200_lpips_args;
+/* Bytes of the packed weights of a network (0 for an unknown net). */
+size_t gab200_lpips_weights_bytes(int32_t net);
+/* Packs a network's weights once: conv_weight[l] / conv_bias[l] are DEVICE pointers to torchvision's float32
+ * features.N.weight (OIHW, contiguous) and features.N.bias of the l-th convolution up to the last target (5 for AlexNet,
+ * 13 for VGG-16), lin_weight[t] the t-th lin layer's (C_t) float32 weights; the pointer arrays themselves are host
+ * memory.  packed: gab200_lpips_weights_bytes(net) bytes, 16-byte aligned.  Stream-ordered, no host wait. */
+int32_t gab200_lpips_pack(int32_t net, const float* const* conv_weight, const float* const* conv_bias,
+                          const float* const* lin_weight, void* packed, void* stream);
+size_t gab200_lpips_scratch_bytes(int32_t net, int32_t height, int32_t width);
+size_t gab200_lpips_features_bytes(int32_t net, int32_t height, int32_t width);
+int32_t gab200_lpips(const gab200_lpips_args* args, void* stream);
+
 /* The tracked mesh drawn over an image, forward only, in four launches with no host wait (capturable).  Replaces
  * what the reference's mesh renderer (mesh_renderer/__init__.py:183-274) asks of nvdiffrast -- dr.rasterize and
  * dr.antialias -- and, fused, render.py's mesh composite (render.py:75-81) and its uint8 quantisation.
