@@ -222,7 +222,7 @@ EXPORTED_SYMBOLS = ("gab200_forward", "gab200_backward", "gab200_mark_visible", 
                     "gab200_stage_timing_enable", "gab200_stage_times", "gab200_face_frame_forward",
                     "gab200_face_frame_backward", "gab200_host_times", "gab200_l1_loss_u8", "gab200_l1_loss_u8_backward",
                     "gab200_photometric_loss", "gab200_adam_step", "gab200_tune", "gab200_counters_ok",
-                    "gab200_regularize_forward", "gab200_regularize_backward", "gab200_nvls_allreduce", "gab200_densify_scratch_bytes", "gab200_densify_plan", "gab200_densify_apply",
+                    "gab200_regularize_forward", "gab200_regularize_backward", "gab200_nvls_allreduce", "gab200_densify_scratch_bytes", "gab200_densify_plan", "gab200_densify_plan_f64", "gab200_densify_apply",
                     "gab200_adam_step_device", "gab200_densify_stats", "gab200_flame_scratch_bytes",
                     "gab200_flame_prepare", "gab200_flame_forward", "gab200_flame_backward",
                     "gab200_forward_device_fov", "gab200_backward_device_fov", "gab200_forward_display",
@@ -319,6 +319,8 @@ def lib():
         L.gab200_densify_scratch_bytes.argtypes = [C.c_int32, C.c_int32]
         L.gab200_densify_plan.restype = C.c_int32
         L.gab200_densify_plan.argtypes = [C.POINTER(DensifyArgs), C.c_void_p]
+        L.gab200_densify_plan_f64.restype = C.c_int32
+        L.gab200_densify_plan_f64.argtypes = [C.POINTER(DensifyArgs), C.c_double, C.c_double, C.c_void_p]
         L.gab200_densify_apply.restype = C.c_int32
         L.gab200_densify_apply.argtypes = [C.POINTER(DensifyArgs), C.POINTER(DensifyOut), C.c_void_p]
         L.gab200_counters_ok.restype = C.c_int32

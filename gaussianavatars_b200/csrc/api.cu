@@ -1193,15 +1193,20 @@ static bool densify_args_ok(const gab200_densify_args* a) {
   return true;
 }
 
-int32_t gab200_densify_plan(const gab200_densify_args* a, void* stream_) {
+int32_t gab200_densify_plan_f64(const gab200_densify_args* a, double extent, double percent_dense, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   if (!densify_args_ok(a)) return GAB200_ERR_INVALID_ARGUMENT;
   if (check_arch() < 0) return GAB200_ERR_ARCH;
-  GAB_CUDA(launch_densify_plan(*a, stream));
+  GAB_CUDA(launch_densify_plan(*a, extent, percent_dense, stream));
   GAB_CUDA(cudaStreamSynchronize(stream));  // the caller sizes the outputs from totals_host
   const uint64_t rows = (uint64_t)a->totals_host[0] + a->totals_host[1] + 2ull * a->totals_host[2];
   if (rows > 0x7fffffffull) return GAB200_ERR_OVERFLOW;
   return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
+int32_t gab200_densify_plan(const gab200_densify_args* a, void* stream) {
+  if (a == nullptr) return GAB200_ERR_INVALID_ARGUMENT;
+  return gab200_densify_plan_f64(a, a->extent, a->percent_dense, stream);
 }
 
 int32_t gab200_densify_apply(const gab200_densify_args* a, const gab200_densify_out* o, void* stream_) {

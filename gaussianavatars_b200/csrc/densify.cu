@@ -28,17 +28,24 @@ namespace gab {
 
 enum : uint32_t { DF_CLONE = 1, DF_SPLIT = 2, DF_CRIT = 4, DF_CRIT_CHILD = 8 };
 
-__device__ __forceinline__ float world_scale_max(const gab200_densify_args& a, int i, float fs, float e[3]) {
-  float m = -1.f;
+// torch.max(dim=1) of a scale triple: a NaN component makes the maximum NaN (fmaxf would drop it), and a NaN maximum
+// compares false, so such a splat is never cloned, split or pruned for its size.
+__device__ __forceinline__ float max3_nan(const float v[3]) {
+  float m = v[0];
 #pragma unroll
-  for (int k = 0; k < 3; k++) {
-    e[k] = expf(a.scaling[3 * (size_t)i + k]) * fs;  // get_scaling (scene/gaussian_model.py:113-123)
-    m = fmaxf(m, e[k]);
-  }
+  for (int k = 1; k < 3; k++) m = (v[k] > m || isnan(v[k])) ? v[k] : m;
   return m;
 }
 
-__global__ void __launch_bounds__(256) densify_classify_kernel(gab200_densify_args a, uint32_t* __restrict__ flags,
+__device__ __forceinline__ float world_scale_max(const gab200_densify_args& a, int i, float fs, float e[3]) {
+#pragma unroll
+  for (int k = 0; k < 3; k++) e[k] = expf(a.scaling[3 * (size_t)i + k]) * fs;  // get_scaling (scene/gaussian_model.py:113-123)
+  return max3_nan(e);
+}
+
+// thr = f32(percent_dense * extent), big = f32(0.1 * extent), formed in double on the host: see launch_densify_plan.
+__global__ void __launch_bounds__(256) densify_classify_kernel(gab200_densify_args a, float thr, float big,
+                                                               uint32_t* __restrict__ flags,
                                                                int32_t* __restrict__ face_delta,
                                                                int32_t* __restrict__ face_cand) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -50,21 +57,19 @@ __global__ void __launch_bounds__(256) densify_classify_kernel(gab200_densify_ar
   const float fs = bound ? a.face_scaling[f] : 1.f;
   float e[3];
   const float smax = world_scale_max(a, i, fs, e);
-  const float thr = a.percent_dense * a.extent;
   const bool clone = fabsf(g) >= a.grad_threshold && smax <= thr;
   const bool split = g >= a.grad_threshold && smax > thr;
   const float op = 1.0f / (1.0f + expf(-a.opacity[i]));
   const bool ws = a.max_screen_size > 0.f;  // the radius criterion itself can never fire: see oracle/densify.py
-  const float big = 0.1f * a.extent;
   const bool crit = op < a.min_opacity || (ws && smax > big);
-  float cmax = -1.f;
+  float child[3];
 #pragma unroll
   for (int k = 0; k < 3; k++) {
     const float base = bound ? e[k] / fs : e[k];
     const float ns = logf(base / 1.6f);  // scaling_inverse_activation(... / (0.8 * N)), N = 2
-    cmax = fmaxf(cmax, expf(ns) * fs);
+    child[k] = expf(ns) * fs;
   }
-  const bool crit_child = op < a.min_opacity || (ws && cmax > big);
+  const bool crit_child = op < a.min_opacity || (ws && max3_nan(child) > big);
   flags[i] = (clone ? DF_CLONE : 0u) | (split ? DF_SPLIT : 0u) | (crit ? DF_CRIT : 0u) | (crit_child ? DF_CRIT_CHILD : 0u);
   if (bound) {
     if (clone || split) atomicAdd(face_delta + f, 1);  // + clone, or + 2 children - 1 parent
@@ -225,25 +230,31 @@ static DensifyScratch carve_densify(void* base, int P, int F) {
   return s;
 }
 
-cudaError_t launch_densify_plan(const gab200_densify_args& a, cudaStream_t stream) {
+cudaError_t launch_densify_plan(const gab200_densify_args& a, double extent, double percent_dense, cudaStream_t stream) {
   const int P = a.P, F = a.binding != nullptr ? a.num_faces : 0;
   DensifyScratch s = carve_densify(a.scratch, P, F);
   cudaError_t e;
   if (F > 0 && (e = cudaMemsetAsync(s.face, 0, sizeof(int32_t) * 2 * (size_t)F, stream)) != cudaSuccess) return e;
-  if (P == 0) return cudaMemsetAsync(s.totals, 0, sizeof(uint32_t) * 8, stream);
-  const int blocks = (P + 255) / 256;
-  densify_classify_kernel<<<blocks, 256, 0, stream>>>(a, s.flags, s.face, s.face + F);
-  count_launch();
-  densify_decide_kernel<<<blocks, 256, 0, stream>>>(a, s.flags, s.face, s.face + F, s.cnt);
-  count_launch();
-  for (int k = 0; k < 4; k++) {
-    size_t bytes = s.scan_bytes;
-    e = cub::DeviceScan::ExclusiveSum(s.scan_temp, bytes, s.cnt + (size_t)k * P, s.pos + (size_t)k * P, P, stream);
-    if (e != cudaSuccess) return e;
+  if (P == 0) {
+    if ((e = cudaMemsetAsync(s.totals, 0, sizeof(uint32_t) * 8, stream)) != cudaSuccess) return e;
+  } else {
+    // The reference compares float32 scales with Python products, formed in double and rounded once; a float product
+    // of the rounded factors differs from that by an ulp for about a third of all extents.
+    const float thr = (float)(percent_dense * extent), big = (float)(0.1 * extent);
+    const int blocks = (P + 255) / 256;
+    densify_classify_kernel<<<blocks, 256, 0, stream>>>(a, thr, big, s.flags, s.face, s.face + F);
+    count_launch();
+    densify_decide_kernel<<<blocks, 256, 0, stream>>>(a, s.flags, s.face, s.face + F, s.cnt);
+    count_launch();
+    for (int k = 0; k < 4; k++) {
+      size_t bytes = s.scan_bytes;
+      e = cub::DeviceScan::ExclusiveSum(s.scan_temp, bytes, s.cnt + (size_t)k * P, s.pos + (size_t)k * P, P, stream);
+      if (e != cudaSuccess) return e;
+      count_launch();
+    }
+    densify_totals_kernel<<<1, 32, 0, stream>>>(P, s.cnt, s.pos, s.totals);
     count_launch();
   }
-  densify_totals_kernel<<<1, 32, 0, stream>>>(P, s.cnt, s.pos, s.totals);
-  count_launch();
   return cudaMemcpyAsync(a.totals_host, s.totals, sizeof(uint32_t) * 4, cudaMemcpyDeviceToHost, stream);
 }
 
@@ -251,6 +262,12 @@ cudaError_t launch_densify_apply(const gab200_densify_args& a, const gab200_dens
   const int P = a.P, F = a.binding != nullptr ? a.num_faces : 0;
   DensifyScratch s = carve_densify(a.scratch, P, F);
   const int P_out = o.P_out;
+  // also when P_out = 0: the counters of a bound model without splats are all zero (its binding pointer may be NULL)
+  const int F_counter = (F > 0 || (P == 0 && a.num_faces > 0)) ? a.num_faces : 0;
+  if (F_counter > 0 && o.binding_counter != nullptr) {
+    cudaError_t e = cudaMemsetAsync(o.binding_counter, 0, sizeof(int32_t) * (size_t)F_counter, stream);
+    if (e != cudaSuccess) return e;
+  }
   if (P_out == 0 || P == 0) return cudaSuccess;
   const int blocks = (P + 255) / 256;
   densify_source_kernel<<<blocks, 256, 0, stream>>>(P, s.cnt, s.pos, s.totals, o.src_scratch, o.kind_scratch,
@@ -276,8 +293,6 @@ cudaError_t launch_densify_apply(const gab200_densify_args& a, const gab200_dens
     count_launch();
   }
   if (F > 0) {
-    cudaError_t e = cudaMemsetAsync(o.binding_counter, 0, sizeof(int32_t) * (size_t)F, stream);
-    if (e != cudaSuccess) return e;
     densify_binding_kernel<<<(P_out + 255) / 256, 256, 0, stream>>>(P_out, o.src_scratch, a.binding, o.binding,
                                                                      o.binding_counter);
     count_launch();

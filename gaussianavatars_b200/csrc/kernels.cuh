@@ -271,7 +271,8 @@ cudaError_t launch_mesh_render(const gab200_mesh_args& a, cudaStream_t stream);
 
 // densify.cu
 size_t densify_scratch_bytes(int P, int F);
-cudaError_t launch_densify_plan(const gab200_densify_args& a, cudaStream_t stream);
+cudaError_t launch_densify_plan(const gab200_densify_args& a, double extent, double percent_dense,
+                                cudaStream_t stream);
 cudaError_t launch_densify_apply(const gab200_densify_args& a, const gab200_densify_out& o, cudaStream_t stream);
 void launch_densify_stats(int P, const float* vgrad, const int32_t* radii, float* accum, float* denom, float* max_radii,
                           const int32_t* skip, cudaStream_t stream);

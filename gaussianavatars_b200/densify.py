@@ -87,7 +87,9 @@ def densify_arrays(params: Dict[str, torch.Tensor], state: Dict[str, Tuple[Optio
     a.totals_host = totals.data_ptr()
     with torch.cuda.device(device):
         stream = torch.cuda.current_stream(device).cuda_stream
-        N.check(N.lib().gab200_densify_plan(C.byref(a), C.c_void_p(stream)), "gab200_densify_plan")
+        # extent and percent_dense in double: the thresholds are rounded to float32 once, as the reference rounds them
+        N.check(N.lib().gab200_densify_plan_f64(C.byref(a), float(extent), float(percent_dense), C.c_void_p(stream)),
+                "gab200_densify_plan_f64")
         n_o, n_c, n_ch, S = (int(x) for x in totals.tolist())
         P2 = n_o + n_c + 2 * n_ch
         if noise is None:

@@ -762,12 +762,16 @@ int32_t gab200_nvls_allreduce(float* mc_ptr, int64_t n, int32_t rank, int32_t wo
  *                         [0, S) for the first child of the S split parents in index order, [S, 2S) for the second --
  *                         exactly what torch.normal(mean=0, std=...) draws), and rebuilds binding / binding_counter.
  * The densification statistics (xyz_gradient_accum, denom, max_radii2D) of the result are all zero in the reference
- * (densification_postfix :447-449): the caller allocates zeros of length P'. */
+ * (densification_postfix :447-449): the caller allocates zeros of length P'.
+ * A scale triple holding a NaN is never cloned, split or pruned for its size (torch.max propagates the NaN).  With
+ * P = 0 the plan still writes totals_host (all zero).  The apply zeroes out->binding_counter (when given) of a bound
+ * model even when P' = 0; a model without splats counts as bound when num_faces > 0, whatever its binding pointer
+ * (an empty tensor's data pointer may be NULL). */
 typedef struct gab200_densify_args {
   uint32_t abi_version;
   int32_t P, num_faces;
   int32_t sh_rest_width;   /* floats per splat of _features_rest: 3 * (M - 1) */
-  float grad_threshold, min_opacity, extent, percent_dense;
+  float grad_threshold, min_opacity, extent, percent_dense;   /* extent, percent_dense: see gab200_densify_plan_f64 */
   float max_screen_size;   /* <= 0: None */
   const float *xyz, *rotation, *scaling, *opacity, *f_dc, *f_rest;   /* raw parameters [P, 3|4|3|1|3|sh_rest_width] */
   const float* exp_avg[6];     /* Adam moments in the order xyz, rotation, scaling, opacity, f_dc, f_rest; NULL = none */
@@ -802,6 +806,13 @@ size_t gab200_densify_scratch_bytes(int32_t P, int32_t num_faces);
 int32_t gab200_densify_stats(int32_t P, const float* viewspace_grad, const int32_t* radii, float* xyz_gradient_accum,
                              float* denom, float* max_radii2D, const int32_t* skip_flag, void* stream);
 int32_t gab200_densify_plan(const gab200_densify_args* args, void* stream);
+/* gab200_densify_plan with extent and percent_dense as the caller holds them, in double; args->extent and
+ * args->percent_dense are not read.  The reference compares float32 scales with the Python products
+ * percent_dense * extent and 0.1 * extent: formed in double and rounded to float32 once.  This entry point forms both
+ * thresholds that way, so a splat sitting on a threshold is cloned, split or pruned as the reference decides.
+ * gab200_densify_plan forms them the same way from its float fields; after the rounding of the two factors the result
+ * is an ulp off the reference's for about a third of all extents. */
+int32_t gab200_densify_plan_f64(const gab200_densify_args* args, double extent, double percent_dense, void* stream);
 int32_t gab200_densify_apply(const gab200_densify_args* args, const gab200_densify_out* out, void* stream);
 
 /* FLAME head posing: blendshapes and linear blend skinning, forward and backward, for one timestep read from device

@@ -48,30 +48,33 @@ def build_rotation(r):
 
 
 def plan(params, stats, hyper, binding=None, binding_counter=None, face_scaling=None):
-    """Returns dict(clone, split, keep_orig, keep_clone, keep_child (bool [P]), child_scaling [P,3], std [P,3])."""
-    max_grad, min_opacity, extent, max_screen_size, percent_dense = (f32(h) for h in hyper)
+    """hyper: (max_grad, min_opacity, extent, max_screen_size or -1 for None, percent_dense) as the caller holds them
+    (Python floats).  Returns dict(clone, split, keep_orig, keep_clone, keep_child (bool [P]), child_scaling [P,3],
+    std [P,3])."""
+    max_grad, min_opacity = f32(hyper[0]), f32(hyper[1])
+    extent, max_screen_size, percent_dense = float(hyper[2]), float(hyper[3]), float(hyper[4])
     accum, denom = stats["xyz_gradient_accum"].reshape(-1).astype(f32), stats["denom"].reshape(-1).astype(f32)
-    with np.errstate(divide="ignore", invalid="ignore"):
+    with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
         g = accum / denom
-    g[np.isnan(g)] = 0
-    e = np.exp(params["scaling"].astype(f32))
-    if binding is not None:
-        fs = face_scaling.reshape(-1).astype(f32)[binding][:, None]
-        world = (e * fs).astype(f32)
-    else:
-        fs, world = None, e
-    smax = world.max(axis=1)
-    thr = f32(percent_dense * extent)
-    clone = (np.abs(g) >= max_grad) & (smax <= thr)
-    split = (g >= max_grad) & (smax > thr)
-    op = _sigmoid(params["opacity"].reshape(-1))
-    ws_on = max_screen_size > 0
-    big = f32(f32(0.1) * extent)
-    crit_orig = (op < min_opacity) | (ws_on & (smax > big))
-    base = (world / fs) if binding is not None else world
-    child_scaling = np.log((base / f32(0.8 * 2)).astype(f32)).astype(f32)
-    child_world = np.exp(child_scaling) * (fs if binding is not None else f32(1.0))
-    crit_child = (op < min_opacity) | (ws_on & (child_world.max(axis=1) > big))
+        g[np.isnan(g)] = 0
+        e = np.exp(params["scaling"].astype(f32))
+        if binding is not None:
+            fs = face_scaling.reshape(-1).astype(f32)[binding][:, None]
+            world = (e * fs).astype(f32)
+        else:
+            fs, world = None, e
+        smax = world.max(axis=1)   # a NaN component makes the maximum NaN, as torch.max does; NaN compares false
+        # the reference compares float32 with the Python products: formed in double, rounded to float32 once
+        thr, big = f32(percent_dense * extent), f32(0.1 * extent)
+        clone = (np.abs(g) >= max_grad) & (smax <= thr)
+        split = (g >= max_grad) & (smax > thr)
+        op = _sigmoid(params["opacity"].reshape(-1))
+        ws_on = max_screen_size > 0
+        crit_orig = (op < min_opacity) | (ws_on & (smax > big))
+        base = (world / fs) if binding is not None else world
+        child_scaling = np.log((base / f32(0.8 * 2)).astype(f32)).astype(f32)
+        child_world = np.exp(child_scaling) * (fs if binding is not None else f32(1.0))
+        crit_child = (op < min_opacity) | (ws_on & (child_world.max(axis=1) > big))
     if binding is not None:
         F = binding_counter.shape[0]
         delta = np.bincount(binding, weights=(clone | split).astype(np.int64), minlength=F).astype(np.int64)

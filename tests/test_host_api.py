@@ -60,6 +60,34 @@ def test_ctypes_structs_match_the_c_layout(tmp_path):
             assert int(got[f"{cname}.{fname}"]) == getattr(ct, fname).offset, f"{cname}.{fname}"
 
 
+def test_densify_entry_points_refuse_an_inconsistent_binding():
+    """Both plan entry points and the apply validate the same way, before any device work: the pointers below are
+    never dereferenced."""
+    from gaussianavatars_b200 import _native as N
+
+    def args(**kw):
+        a = N.DensifyArgs()
+        a.abi_version, a.P, a.sh_rest_width, a.num_faces = N.ABI_VERSION, 4, 0, 3
+        for f in ("xyz", "rotation", "scaling", "opacity", "f_dc", "xyz_gradient_accum", "denom", "scratch", "totals_host",
+                  "binding", "binding_counter", "face_scaling"):
+            setattr(a, f, 256)
+        for k, v in kw.items():
+            setattr(a, k, v)
+        return a
+
+    L = N.lib()
+    assert L.gab200_densify_plan(None, None) == -1 and L.gab200_densify_plan_f64(None, 1.0, 0.01, None) == -1
+    for bad in (dict(num_faces=0), dict(num_faces=-1), dict(binding_counter=None), dict(face_scaling=None),
+                dict(abi_version=N.ABI_VERSION + 1), dict(P=-1), dict(totals_host=None)):
+        assert L.gab200_densify_plan(C.byref(args(**bad)), None) == -1, bad
+        assert L.gab200_densify_plan_f64(C.byref(args(**bad)), 0.6044044044044043, 0.01, None) == -1, bad
+    o = N.DensifyOut()
+    o.P_out = 2
+    for f in ("xyz", "rotation", "scaling", "opacity", "f_dc", "src_scratch", "kind_scratch", "binding_counter"):
+        setattr(o, f, 256)
+    assert L.gab200_densify_apply(C.byref(args()), C.byref(o), None) == -1   # a bound result needs its binding
+
+
 def test_missing_library_fails_loudly(tmp_path, monkeypatch):
     from gaussianavatars_b200 import _native as N
 
