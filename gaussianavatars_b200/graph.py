@@ -50,7 +50,7 @@ from . import mesh as M
 from . import rasterizer as R
 from types import SimpleNamespace
 
-from .renderer import _forward_only, _views_forward, camera_table, render, render_views_train
+from .renderer import _forward_only, camera_table, render, render_views_train
 from .rasterizer import l1_loss_u8
 from .densify import add_densification_stats
 from .training import (METRIC_NAMES, Adam, binding_regularizers, launch_composite_rgba, launch_image_metrics,
@@ -198,6 +198,9 @@ class _Captured:
             raise ValueError(f"a {type(self).__name__} camera block with the field of view has {CAMERA_BLOCK_FOV} "
                              f"floats (camera_block(cam, fov=True)), got {blk.numel()}")
         return blk
+
+    def _gt_shape(self):
+        return (3, self.H, self.W) if self.K == 1 else (self.K, 3, self.H, self.W)
 
     def _set_pose_input(self, verts, timestep):
         """The checks of set_inputs' pose arguments; writes the timestep (a host int checked against the model's
@@ -609,9 +612,6 @@ class GraphedFrame(_Captured):
         self._uploads = bool(host_inputs)
         if schedule is not None:
             self._use_schedule(schedule, frames, log=True)
-
-    def _gt_shape(self):
-        return (3, self.H, self.W) if self.K == 1 else (self.K, 3, self.H, self.W)
 
     def _gt_input(self):
         """The device tensor the ground truth is written into: the RGBA frame(s) with rgba=True, else gt; None with a
@@ -1061,13 +1061,11 @@ class GraphedRender(_Captured):
         with torch.no_grad():
             if self.mesh_update:
                 self._pose()
-            if self.K > 1:   # the K cameras of the table in one forward
-                out = _views_forward(self.cam, self.W, self.H, self.pc, _Pipe, self.bg, self.scaling_modifier,
-                                     self.outputs != "float", self.outputs != "u8")
-            else:
-                out = _forward_only(self.camera, self.pc, _Pipe, self.bg, self.scaling_modifier,
-                                    self.outputs != "float" and not self.mesh, self.outputs != "u8" or self.mesh,
-                                    self.depth_alpha)
+            # K > 1: the K cameras of the table in one forward
+            out = _forward_only(self.camera if self.K == 1 else self.cam, self.pc, _Pipe, self.bg,
+                                self.scaling_modifier, self.outputs != "float" and not self.mesh,
+                                self.outputs != "u8" or self.mesh, self.depth_alpha,
+                                None if self.K == 1 else (self.W, self.H))
             if self.mesh:
                 out["display_u8"] = self._overlay(out["render"])
         self.image, self.display, self.radii = out["render"], out["display_u8"], out["radii"]
@@ -1262,10 +1260,6 @@ class GraphedEval(GraphedRender):
         # K > 1: the rows of the replay's views, view + k, one device int32 each
         self.rows = torch.arange(self.K, dtype=torch.int32, device=self.device) if self.K > 1 else None
         self.gt = torch.zeros(self._gt_shape(), dtype=torch.uint8, device=self.device)
-
-    def _gt_shape(self):
-        return (3, self.H, self.W) if self.K == 1 else (self.K, 3, self.H, self.W)
-        self._metrics_scratch = None
 
     def reset(self):
         """Every row of the tables back to NaN (no score); with a schedule, the cursor back to its first record."""

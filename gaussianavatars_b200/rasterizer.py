@@ -119,19 +119,26 @@ def hints_of(obj) -> "FrameHints":
     return h
 
 
-def _fill_common(a: N.ForwardArgs, rs: GaussianRasterizationSettings, device, P: int, need_backward: bool):
+def _fill_common(a: N.ForwardArgs, rs: GaussianRasterizationSettings, device, P: int, need_backward: bool,
+                 cameras: Optional[torch.Tensor] = None):
+    """The scalar fields and camera pointers of `a`; returns the tensors they point at.  With a (K, 37) camera table
+    the views' matrices, centres and fields of view are in the table: `a`'s stay unset."""
     a.abi_version = N.ABI_VERSION
     a.P = P
     a.sh_degree = int(rs.sh_degree)
     a.image_width = int(rs.image_width)
     a.image_height = int(rs.image_height)
-    a.tanfovx = float(rs.tanfovx)
-    a.tanfovy = float(rs.tanfovy)
     a.scale_modifier = float(rs.scale_modifier)
     a.prefiltered = int(bool(rs.prefiltered))
     a.debug = int(bool(rs.debug))
     a.need_backward = int(need_backward)
     a.exact_binning = int(_EXACT_BINNING)
+    if cameras is not None:
+        bg = _cam(rs.bg, "bg", device)
+        a.bg = bg.data_ptr()
+        return (bg,)
+    a.tanfovx = float(rs.tanfovx)
+    a.tanfovy = float(rs.tanfovy)
     cams = (_cam(rs.bg, "bg", device), _cam(rs.viewmatrix, "viewmatrix", device),
             _cam(rs.projmatrix, "projmatrix", device), _cam(rs.campos, "campos", device))
     a.bg, a.viewmatrix, a.projmatrix, a.campos = (t.data_ptr() for t in cams)
@@ -218,11 +225,11 @@ def check_tanfov(tanfov: Optional[torch.Tensor], device):
     return tanfov
 
 
-def check_rgb8(rgb8: Optional[torch.Tensor], rs: GaussianRasterizationSettings, device):
-    """A display-image destination: a contiguous (H,W,3) uint8 tensor on `device`, or None."""
+def check_rgb8(rgb8: Optional[torch.Tensor], rs: GaussianRasterizationSettings, device, lead: tuple = ()):
+    """A display-image destination: a contiguous lead + (H,W,3) uint8 tensor on `device`, or None."""
     if rgb8 is None:
         return None
-    shape = (int(rs.image_height), int(rs.image_width), 3)
+    shape = lead + (int(rs.image_height), int(rs.image_width), 3)
     if not isinstance(rgb8, torch.Tensor) or rgb8.device != device or rgb8.dtype != torch.uint8 or \
             tuple(rgb8.shape) != shape or not rgb8.is_contiguous():
         raise ValueError(f"rgb8 must be a contiguous {shape} uint8 tensor on {device}")
@@ -271,54 +278,82 @@ def _run_frame(a: N.ForwardArgs, device, need_backward: bool, key, hints: FrameH
 
 def _run_forward(a: N.ForwardArgs, device, need_backward: bool, hints: Optional[FrameHints] = None,
                  tanfov: Optional[torch.Tensor] = None, rgb8: Optional[torch.Tensor] = None, float_image: bool = True,
-                 planes: Optional[tuple] = None):
+                 planes: Optional[tuple] = None, cameras: Optional[torch.Tensor] = None):
     """tanfov: None (a.tanfovx / tanfovy) or the (2,) device tensor the kernels read instead
     (gab200_forward_device_fov); the backward must then be given the same tensor.
     rgb8: None, or a (H,W,3) uint8 tensor the blend writes the display image into (gab200_forward_display);
     float_image=False (with rgb8, no backward) skips the float image: the returned color is None.
-    planes: None, or (alpha, depth) (1,H,W) float32 tensors the blend also fills (gab200_forward_depth_alpha)."""
+    planes: None, or (alpha, depth) (1,H,W) float32 tensors the blend also fills (gab200_forward_depth_alpha).
+    cameras: None (one camera, from `a`), or a checked (K, 37) table of K views (gab200_forward_views[_train]
+    [_depth_alpha]; tanfov is not read): color, radii, rgb8 and planes then have a leading K, and the hints are those
+    of key (device, W, H, P, K).  Only single-view frames are recorded for last_frame_info / export_last_binning."""
     global _last, _last_info
     H, W, P = a.image_height, a.image_width, a.P
-    color = torch.empty((3, H, W), dtype=torch.float32, device=device) if float_image else None
-    radii = torch.empty((P,), dtype=torch.int32, device=device)
-    visible = torch.empty((P,), dtype=torch.bool, device=device)   # radii > 0, written by the preprocess kernel
+    lead = () if cameras is None else (int(cameras.shape[0]),)
+    color = torch.empty(lead + (3, H, W), dtype=torch.float32, device=device) if float_image else None
+    radii = torch.empty(lead + (P,), dtype=torch.int32, device=device)
+    visible = torch.empty(lead + (P,), dtype=torch.bool, device=device)   # radii > 0, written by the preprocess kernel
     a.out_color, a.radii, a.visibility = N.ptr(color), radii.data_ptr(), visible.data_ptr()
     _tls.visible = (radii.data_ptr(), visible)   # renderer.py hands it out as `visibility_filter`
     hints = hints if hints is not None else _default_hints
-    if planes is not None:
-        enqueue = lambda st, stream: N.lib().gab200_forward_depth_alpha(  # noqa: E731
-            C.byref(a), N.ptr(tanfov), planes[0].data_ptr(), planes[1].data_ptr(), N.ptr(rgb8), C.byref(st), stream)
-    elif rgb8 is not None:
-        enqueue = lambda st, stream: N.lib().gab200_forward_display(  # noqa: E731
-            C.byref(a), N.ptr(tanfov), rgb8.data_ptr(), C.byref(st), stream)
-    elif tanfov is None:
-        enqueue = lambda st, stream: N.lib().gab200_forward(C.byref(a), C.byref(st), stream)  # noqa: E731
+    alpha, depth = (None, None) if planes is None else (planes[0].data_ptr(), planes[1].data_ptr())
+
+    def enqueue(st, stream):
+        if cameras is not None:
+            K, table = lead[0], cameras.data_ptr()
+            if need_backward and planes is not None:
+                return N.lib().gab200_forward_views_train_depth_alpha(C.byref(a), K, table, alpha, depth, C.byref(st),
+                                                                      stream)
+            if need_backward:
+                return N.lib().gab200_forward_views_train(C.byref(a), K, table, C.byref(st), stream)
+            if planes is not None:
+                return N.lib().gab200_forward_views_depth_alpha(C.byref(a), K, table, alpha, depth, N.ptr(rgb8),
+                                                                C.byref(st), stream)
+            return N.lib().gab200_forward_views(C.byref(a), K, table, N.ptr(rgb8), C.byref(st), stream)
+        if planes is not None:
+            return N.lib().gab200_forward_depth_alpha(C.byref(a), N.ptr(tanfov), alpha, depth, N.ptr(rgb8),
+                                                      C.byref(st), stream)
+        if rgb8 is not None:
+            return N.lib().gab200_forward_display(C.byref(a), N.ptr(tanfov), rgb8.data_ptr(), C.byref(st), stream)
+        if tanfov is not None:
+            return N.lib().gab200_forward_device_fov(C.byref(a), tanfov.data_ptr(), C.byref(st), stream)
+        return N.lib().gab200_forward(C.byref(a), C.byref(st), stream)
+
+    if cameras is None:
+        st, holder, info = _run_frame(a, device, need_backward, (device, W, H, P), hints, "gab200_forward", enqueue)
+        _last_info = info
+        if _KEEP_LAST:
+            # pooled (inference) scratch stays valid until the next no_grad forward on this device
+            _last = (a, st, holder, device)
     else:
-        enqueue = lambda st, stream: N.lib().gab200_forward_device_fov(  # noqa: E731
-            C.byref(a), tanfov.data_ptr(), C.byref(st), stream)
-    st, holder, info = _run_frame(a, device, need_backward, (device, W, H, P), hints, "gab200_forward", enqueue)
-    _last_info = info
-    if _KEEP_LAST:
-        # pooled (inference) scratch stays valid until the next no_grad forward on this device
-        _last = (a, st, holder, device)
+        st, holder, _ = _run_frame(a, device, need_backward, (device, W, H, P) + lead, hints,
+                                   "gab200_forward_views_train" if need_backward else "gab200_forward_views", enqueue,
+                                   views=lead[0])
     return color, radii, st, holder
 
 
 def _run_backward(b: N.BackwardArgs, device, tanfov: Optional[torch.Tensor] = None,
-                  plane_grads: Optional[tuple] = None):
+                  plane_grads: Optional[tuple] = None, cameras: Optional[torch.Tensor] = None):
     """gab200_backward, or gab200_backward_device_fov with the tensor the forward read; plane_grads: (dL/dalpha,
-    dL/ddepth), each a contiguous (1,H,W) tensor or None, of a depth_alpha frame (gab200_backward_depth_alpha)."""
+    dL/ddepth), each a contiguous (1,H,W) tensor or None, of a depth_alpha frame (gab200_backward_depth_alpha).
+    cameras: the (K, 37) table of a K-view frame (gab200_backward_views[_depth_alpha]; plane gradients (K,1,H,W))."""
     with torch.cuda.device(device):
-        stream = torch.cuda.current_stream(device).cuda_stream
-        if plane_grads is not None:
-            N.check(N.lib().gab200_backward_depth_alpha(C.byref(b), N.ptr(tanfov), N.ptr(plane_grads[0]),
-                                                        N.ptr(plane_grads[1]), C.c_void_p(stream)),
+        stream = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+        ga, gd = (None, None) if plane_grads is None else (N.ptr(plane_grads[0]), N.ptr(plane_grads[1]))
+        if cameras is not None:
+            K, table = int(cameras.shape[0]), cameras.data_ptr()
+            if plane_grads is not None:
+                N.check(N.lib().gab200_backward_views_depth_alpha(C.byref(b), K, table, ga, gd, stream),
+                        "gab200_backward_views_depth_alpha")
+            else:
+                N.check(N.lib().gab200_backward_views(C.byref(b), K, table, stream), "gab200_backward_views")
+        elif plane_grads is not None:
+            N.check(N.lib().gab200_backward_depth_alpha(C.byref(b), N.ptr(tanfov), ga, gd, stream),
                     "gab200_backward_depth_alpha")
         elif tanfov is None:
-            N.check(N.lib().gab200_backward(C.byref(b), C.c_void_p(stream)), "gab200_backward")
+            N.check(N.lib().gab200_backward(C.byref(b), stream), "gab200_backward")
         else:
-            N.check(N.lib().gab200_backward_device_fov(C.byref(b), tanfov.data_ptr(), C.c_void_p(stream)),
-                    "gab200_backward")
+            N.check(N.lib().gab200_backward_device_fov(C.byref(b), tanfov.data_ptr(), stream), "gab200_backward")
 
 
 class _RasterizeGaussians(torch.autograd.Function):
@@ -510,36 +545,40 @@ def _grad_buffer(grad_sink, P: int, M: int, device, symm_ok: bool = True):
 
 
 class _RasterizeBound(torch.autograd.Function):
+    """The fused route's frame: one camera from raster_settings (and `tanfov`), or with `cameras`, a checked (K, 37)
+    table, the K views of one splat set, every image, radii and means2D with a leading K.  colors_precomp and the
+    multicast gradient buffer are single-view only (the K-view entry points refuse both)."""
+
     @staticmethod
     def forward(ctx, _xyz, means2D, _rotation, _scaling, _opacity, f_dc, f_rest, face_center, face_orien_mat,
                 face_scaling, binding, colors_precomp, raster_settings, grad_sink=None, tanfov=None, rgb8=None,
-                float_image=True, depth_alpha=False):
+                float_image=True, depth_alpha=False, hints=None, cameras=None):
         rs = raster_settings
         ctx.grad_sink = grad_sink
         device = _xyz.device
         if device.type != "cuda":
             raise RuntimeError("gaussianavatars_b200 has no CPU path: tensors must be CUDA tensors")
-        P = _xyz.shape[0]
+        P, H, W = _xyz.shape[0], int(rs.image_height), int(rs.image_width)
+        lead = () if cameras is None else (int(cameras.shape[0]),)
         need_bw = any(ctx.needs_input_grad)
         a = N.ForwardArgs()
-        cams = _fill_common(a, rs, device, P, need_bw)
+        cams = _fill_common(a, rs, device, P, need_bw, cameras)
         binding_orig = binding
         _xyz, _rotation, _scaling, _opacity, f_dc, f_rest, colors_precomp, binding, face_center, face_orien_mat, \
             face_scaling = _fill_bound(a, device, _xyz, _rotation, _scaling, _opacity, f_dc, f_rest, colors_precomp,
                                        binding, face_center, face_orien_mat, face_scaling)
         M, F = a.sh_coeffs, a.num_faces
         tanfov = check_tanfov(tanfov, device)
-        rgb8 = check_rgb8(rgb8, rs, device)
+        rgb8 = check_rgb8(rgb8, rs, device, lead)
         if not float_image and (rgb8 is None or need_bw):
             raise ValueError("float_image=False needs rgb8= and no gradient (the backward reads the float image's state)")
         planes = None
         if depth_alpha:
-            planes = (torch.empty((1, rs.image_height, rs.image_width), dtype=torch.float32, device=device),
-                      torch.empty((1, rs.image_height, rs.image_width), dtype=torch.float32, device=device))
-        color, radii, st, holder = _run_forward(a, device, need_bw,
-                                                hints_of(grad_sink) if grad_sink is not None else None, tanfov,
-                                                rgb8, float_image, planes)
-        ctx.tanfov = tanfov
+            planes = (torch.empty(lead + (1, H, W), dtype=torch.float32, device=device),
+                      torch.empty(lead + (1, H, W), dtype=torch.float32, device=device))
+        color, radii, st, holder = _run_forward(a, device, need_bw, hints, tanfov, rgb8, float_image, planes,
+                                                cameras=cameras)
+        ctx.tanfov, ctx.cameras = tanfov, cameras
         ctx.depth_alpha = bool(depth_alpha)
         if need_bw:
             ctx.args, ctx.state, ctx.holder = a, st, holder
@@ -570,7 +609,8 @@ class _RasterizeBound(torch.autograd.Function):
         # "push": the kernel reduces into every replica with multimem.red; "two_shot": plain stores into the local
         # replica, reduced afterwards by the NVLS all-reduce kernel (dist.SymmetricGradBuffer.end)
         use_mc = use_symm and getattr(symm, "mode", "push") == "push"
-        d_means2D = torch.empty((P, 3), dtype=torch.float32, device=device)
+        lead = () if ctx.cameras is None else (int(ctx.cameras.shape[0]),)
+        d_means2D = torch.empty(lead + (P, 3), dtype=torch.float32, device=device)
         d_colors = torch.empty((P, 3), dtype=torch.float32, device=device) if colors_precomp is not None else None
         d_fc = d_fR = d_fs = None
         if ctx.want_face:
@@ -600,13 +640,16 @@ class _RasterizeBound(torch.autograd.Function):
         plane_grads = None
         if ctx.depth_alpha:   # gradients of the alpha / depth planes (None: the loss does not read that plane)
             plane_grads = tuple(None if t is None else (t if t.is_contiguous() else t.contiguous()) for t in grad_planes)
-        _run_backward(b, device, ctx.tanfov, plane_grads)
+        if ctx.cameras is None:
+            _run_backward(b, device, ctx.tanfov, plane_grads)
+        else:   # the sum over the K views of every single-view gradient but d_means2D, one row per view
+            _run_backward(b, device, plane_grads=plane_grads, cameras=ctx.cameras)
         ctx.holder = None
         if ctx.grad_sink is not None:  # dist.py: ONE all-reduce over this buffer instead of six
             ctx.grad_sink.flat_grad = flat
             ctx.grad_sink._gab200_mc_used = bool(use_symm)  # SymmetricGradBuffer.end() only trusts the replica if set
         return (d_xyz, d_means2D, d_rot, d_scale, d_opac, d_dc, d_rest, d_fc, d_fR, d_fs, None, d_colors, None, None,
-                None, None, None, None)
+                None, None, None, None, None, None)
 
 
 def rasterize_bound(raster_settings: GaussianRasterizationSettings, _xyz, _rotation, _scaling, _opacity,
@@ -639,7 +682,8 @@ def rasterize_bound(raster_settings: GaussianRasterizationSettings, _xyz, _rotat
         _opacity = _opacity[:, None]
     return _RasterizeBound.apply(_xyz, means2D, _rotation, _scaling, _opacity, features_dc, features_rest,
                                  face_center, face_orien_mat, face_scaling, binding, colors_precomp, raster_settings,
-                                 grad_sink, tanfov, rgb8, bool(float_image), bool(depth_alpha))
+                                 grad_sink, tanfov, rgb8, bool(float_image), bool(depth_alpha),
+                                 hints_of(grad_sink) if grad_sink is not None else None)
 
 
 # ================================================================================================================
@@ -670,16 +714,6 @@ def check_camera_table(cameras, device) -> torch.Tensor:
     return cameras
 
 
-def _views_args(rs: GaussianRasterizationSettings, P: int, need_backward: bool) -> N.ForwardArgs:
-    """The scalar fields of a K-view frame's arguments: what the views share (the cameras are in the table)."""
-    a = N.ForwardArgs()
-    a.abi_version, a.P = N.ABI_VERSION, P
-    a.sh_degree, a.image_width, a.image_height = int(rs.sh_degree), int(rs.image_width), int(rs.image_height)
-    a.scale_modifier, a.prefiltered, a.debug = float(rs.scale_modifier), int(bool(rs.prefiltered)), int(bool(rs.debug))
-    a.need_backward, a.exact_binning = int(need_backward), int(_EXACT_BINNING)
-    return a
-
-
 def rasterize_bound_views(raster_settings: GaussianRasterizationSettings, cameras: torch.Tensor, _xyz, _rotation,
                           _scaling, _opacity, features_dc, features_rest, binding=None, face_center=None,
                           face_orien_mat=None, face_scaling=None, colors_precomp=None, hints: Optional[FrameHints] = None,
@@ -707,129 +741,17 @@ def rasterize_bound_views(raster_settings: GaussianRasterizationSettings, camera
     if device.type != "cuda":
         raise RuntimeError("gaussianavatars_b200 has no CPU path: tensors must be CUDA tensors")
     cameras = check_camera_table(cameras, device)
-    K, P, H, W = int(cameras.shape[0]), int(_xyz.shape[0]), int(rs.image_height), int(rs.image_width)
-    a = _views_args(rs, P, need_backward=False)
-    bg = _cam(rs.bg, "bg", device)
-    a.bg = bg.data_ptr()
+    K, H, W = int(cameras.shape[0]), int(rs.image_height), int(rs.image_width)
+    rgb8 = torch.empty((K, H, W, 3), dtype=torch.uint8, device=device) if display else None
     if _opacity.ndim == 1:
         _opacity = _opacity[:, None]
-    keep = _fill_bound(a, device, _xyz, _rotation, _scaling, _opacity, features_dc, features_rest,  # noqa: F841
-                       colors_precomp, binding, face_center, face_orien_mat, face_scaling)
-    color = torch.empty((K, 3, H, W), dtype=torch.float32, device=device) if float_image else None
-    rgb8 = torch.empty((K, H, W, 3), dtype=torch.uint8, device=device) if display else None
-    radii = torch.empty((K, P), dtype=torch.int32, device=device)
-    visible = torch.empty((K, P), dtype=torch.bool, device=device)
-    a.out_color, a.radii, a.visibility = N.ptr(color), radii.data_ptr(), visible.data_ptr()
-    planes = None
-    if depth_alpha:
-        planes = (torch.empty((K, 1, H, W), dtype=torch.float32, device=device),
-                  torch.empty((K, 1, H, W), dtype=torch.float32, device=device))
-        enqueue = lambda st, stream: N.lib().gab200_forward_views_depth_alpha(  # noqa: E731
-            C.byref(a), K, cameras.data_ptr(), planes[0].data_ptr(), planes[1].data_ptr(), N.ptr(rgb8), C.byref(st),
-            stream)
-    else:
-        enqueue = lambda st, stream: N.lib().gab200_forward_views(  # noqa: E731
-            C.byref(a), K, cameras.data_ptr(), N.ptr(rgb8), C.byref(st), stream)
-    _run_frame(a, device, False, (device, W, H, P, K), hints if hints is not None else FrameHints(),
-               "gab200_forward_views", enqueue, views=K)
-    if planes is not None:
-        return color, rgb8, radii, visible, planes[0], planes[1]
-    return color, rgb8, radii, visible
-
-
-class _RasterizeBoundViews(torch.autograd.Function):
-    """The K cameras of one timestep as one training frame (gab200_forward_views_train / gab200_backward_views)."""
-
-    @staticmethod
-    def forward(ctx, _xyz, means2D, _rotation, _scaling, _opacity, f_dc, f_rest, face_center, face_orien_mat,
-                face_scaling, binding, cameras, raster_settings, grad_sink, hints, depth_alpha=False):
-        rs = raster_settings
-        ctx.grad_sink = grad_sink
-        device = _xyz.device
-        K, P, H, W = int(cameras.shape[0]), int(_xyz.shape[0]), int(rs.image_height), int(rs.image_width)
-        a = _views_args(rs, P, need_backward=True)
-        bg = _cam(rs.bg, "bg", device)
-        a.bg = bg.data_ptr()
-        binding_orig = binding
-        _xyz, _rotation, _scaling, _opacity, f_dc, f_rest, _, binding, face_center, face_orien_mat, face_scaling = \
-            _fill_bound(a, device, _xyz, _rotation, _scaling, _opacity, f_dc, f_rest, None, binding, face_center,
-                        face_orien_mat, face_scaling)
-        M, F = a.sh_coeffs, a.num_faces
-        color = torch.empty((K, 3, H, W), dtype=torch.float32, device=device)
-        radii = torch.empty((K, P), dtype=torch.int32, device=device)
-        visible = torch.empty((K, P), dtype=torch.bool, device=device)
-        a.out_color, a.radii, a.visibility = color.data_ptr(), radii.data_ptr(), visible.data_ptr()
-        _tls.visible = (radii.data_ptr(), visible)
-        planes = None
-        if depth_alpha:
-            planes = (torch.empty((K, 1, H, W), dtype=torch.float32, device=device),
-                      torch.empty((K, 1, H, W), dtype=torch.float32, device=device))
-            enqueue = lambda st, stream: N.lib().gab200_forward_views_train_depth_alpha(  # noqa: E731
-                C.byref(a), K, cameras.data_ptr(), planes[0].data_ptr(), planes[1].data_ptr(), C.byref(st), stream)
-        else:
-            enqueue = lambda st, stream: N.lib().gab200_forward_views_train(  # noqa: E731
-                C.byref(a), K, cameras.data_ptr(), C.byref(st), stream)
-        st, holder, _ = _run_frame(a, device, True, (device, W, H, P, K), hints, "gab200_forward_views_train",
-                                   enqueue, views=K)
-        ctx.args, ctx.state, ctx.holder = a, st, holder
-        ctx.keep = (bg, cameras, _xyz, _rotation, _scaling, _opacity, f_dc, f_rest, face_center, face_orien_mat,
-                    face_scaling, binding)
-        ctx.dims = (K, P, M, F)
-        ctx.face_shapes = None if binding is None else (face_center.shape, face_orien_mat.shape, face_scaling.shape)
-        ctx.want_face = binding is not None and any(ctx.needs_input_grad[7:10])
-        ctx.csr = _face_csr(binding_orig, F)[1] if ctx.want_face else None
-        ctx.depth_alpha = planes is not None
-        ctx.mark_non_differentiable(radii)
-        if planes is not None:
-            return color, radii, planes[0], planes[1]
-        return color, radii
-
-    @staticmethod
-    def backward(ctx, grad_out_color, _grad_radii, *grad_planes):
-        a, st = ctx.args, ctx.state
-        K, P, M, F = ctx.dims
-        cameras = ctx.keep[1]
-        device = cameras.device
-        g = grad_out_color if grad_out_color.is_contiguous() else grad_out_color.contiguous()
-        # the flat per-splat gradient buffer of _RasterizeBound, holding the sum over the K views
-        flat, symm, (d_xyz, d_rot, d_scale, d_opac, d_dc, d_rest) = _grad_buffer(ctx.grad_sink, P, M, device)
-        use_symm = symm is not None
-        d_means2D = torch.empty((K, P, 3), dtype=torch.float32, device=device)
-        d_fc = d_fR = d_fs = None
-        if ctx.want_face:
-            fshape = ctx.face_shapes
-            d_fc = torch.empty(fshape[0], dtype=torch.float32, device=device)
-            d_fR = torch.empty(fshape[1], dtype=torch.float32, device=device)
-            d_fs = torch.empty(fshape[2], dtype=torch.float32, device=device)
-        b = N.BackwardArgs()
-        b.abi_version = N.ABI_VERSION
-        b.fwd, b.state = C.pointer(a), C.pointer(st)
-        b.dL_dout_color = g.data_ptr()
-        b.dL_dmeans3D, b.dL_dopacity, b.dL_dmeans2D = d_xyz.data_ptr(), d_opac.data_ptr(), d_means2D.data_ptr()
-        b.dL_dsh_dc, b.dL_dsh_rest = d_dc.data_ptr(), N.ptr(d_rest)
-        b.dL_dscales, b.dL_drotations = d_scale.data_ptr(), d_rot.data_ptr()
-        b.dL_dface_center, b.dL_dface_orien_mat, b.dL_dface_scaling = N.ptr(d_fc), N.ptr(d_fR), N.ptr(d_fs)
-        if ctx.csr is not None:
-            perm, c_face, c_start, c_end = ctx.csr
-            b.face_perm, b.face_chunk_face = perm.data_ptr(), c_face.data_ptr()
-            b.face_chunk_start, b.face_chunk_end = c_start.data_ptr(), c_end.data_ptr()
-            b.num_face_chunks = c_face.shape[0]
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            if ctx.depth_alpha:   # gradients of the (K,1,H,W) alpha / depth planes (None: the loss does not read one)
-                ga, gd = (None if t is None else (t if t.is_contiguous() else t.contiguous()) for t in grad_planes)
-                N.check(N.lib().gab200_backward_views_depth_alpha(C.byref(b), K, cameras.data_ptr(), N.ptr(ga),
-                                                                  N.ptr(gd), C.c_void_p(stream)),
-                        "gab200_backward_views_depth_alpha")
-            else:
-                N.check(N.lib().gab200_backward_views(C.byref(b), K, cameras.data_ptr(), C.c_void_p(stream)),
-                        "gab200_backward_views")
-        ctx.holder = None
-        if ctx.grad_sink is not None:  # dist.py all-reduces this buffer, as after a single-view backward
-            ctx.grad_sink.flat_grad = flat
-            ctx.grad_sink._gab200_mc_used = bool(use_symm)
-        return (d_xyz, d_means2D, d_rot, d_scale, d_opac, d_dc, d_rest, d_fc, d_fR, d_fs, None, None, None, None, None,
-                None)
+    d = lambda t: None if t is None else t.detach()  # noqa: E731  (no gradient: the forward keeps no backward state)
+    with torch.no_grad():
+        color, radii, *planes = _RasterizeBound.apply(
+            d(_xyz), None, d(_rotation), d(_scaling), d(_opacity), d(features_dc), d(features_rest), d(face_center),
+            d(face_orien_mat), d(face_scaling), binding, d(colors_precomp), rs, None, None, rgb8, bool(float_image),
+            bool(depth_alpha), hints if hints is not None else FrameHints(), cameras)
+    return (color, rgb8, radii, visible_of(radii), *planes)
 
 
 def rasterize_bound_views_train(raster_settings: GaussianRasterizationSettings, cameras: torch.Tensor, _xyz, _rotation,
@@ -868,9 +790,9 @@ def rasterize_bound_views_train(raster_settings: GaussianRasterizationSettings, 
         _opacity = _opacity[:, None]
     if hints is None:
         hints = view_hints_of(grad_sink) if grad_sink is not None else FrameHints()
-    return _RasterizeBoundViews.apply(_xyz, means2D, _rotation, _scaling, _opacity, features_dc, features_rest,
-                                      face_center, face_orien_mat, face_scaling, binding, cameras, raster_settings,
-                                      grad_sink, hints, bool(depth_alpha))
+    return _RasterizeBound.apply(_xyz, means2D, _rotation, _scaling, _opacity, features_dc, features_rest, face_center,
+                                 face_orien_mat, face_scaling, binding, None, raster_settings, grad_sink, None, None,
+                                 True, bool(depth_alpha), hints, cameras)
 
 
 def bind_activate(raster_settings_or_modifier, _xyz, _rotation, _scaling, _opacity, binding=None, face_center=None,

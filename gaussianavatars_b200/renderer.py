@@ -44,11 +44,17 @@ def _camera_block(cam, device):
     return blk
 
 
-def _settings(cam, pc, pipe, bg_color, scaling_modifier, device):
-    view, proj, center = _camera_block(cam, device)
+def _settings(cam, pc, pipe, bg_color, scaling_modifier, device, size=None):
+    """The settings of a frame of camera object `cam`, or of a (K, 37) camera table `cam` of image `size` (W, H): the
+    views' matrices, centres and fields of view are then in the table, and the settings carry none."""
+    if size is None:
+        W, H = int(cam.image_width), int(cam.image_height)
+        view, proj, center = _camera_block(cam, device)
+        tanfovx, tanfovy = math.tan(cam.FoVx * 0.5), math.tan(cam.FoVy * 0.5)
+    else:
+        (W, H), view, proj, center, tanfovx, tanfovy = size, None, None, None, 1.0, 1.0
     return GaussianRasterizationSettings(
-        image_height=int(cam.image_height), image_width=int(cam.image_width),
-        tanfovx=math.tan(cam.FoVx * 0.5), tanfovy=math.tan(cam.FoVy * 0.5), bg=bg_color,
+        image_height=H, image_width=W, tanfovx=tanfovx, tanfovy=tanfovy, bg=bg_color,
         scale_modifier=scaling_modifier, viewmatrix=view, projmatrix=proj, sh_degree=pc.active_sh_degree,
         campos=center, prefiltered=False, debug=bool(getattr(pipe, "debug", False)))
 
@@ -57,9 +63,10 @@ def _has_raw(pc):
     return all(hasattr(pc, n) for n in ("_xyz", "_rotation", "_scaling", "_opacity", "_features_dc", "_features_rest"))
 
 
-def _fused_frame(cam, pc, pipe, bg_color, scaling_modifier):
-    """The settings of a fused-route frame, the binding and the model's face frame (None without a binding)."""
-    rs = _settings(cam, pc, pipe, bg_color, scaling_modifier, pc._xyz.device)
+def _fused_frame(cam, pc, pipe, bg_color, scaling_modifier, size=None):
+    """The settings of a fused-route frame (of a camera, or of a camera table of image `size`), the binding and the
+    model's face frame (None without a binding)."""
+    rs = _settings(cam, pc, pipe, bg_color, scaling_modifier, pc._xyz.device, size)
     binding = getattr(pc, "binding", None)
     if binding is None:
         return rs, None, (None, None, None)
@@ -70,12 +77,23 @@ def _fused_frame(cam, pc, pipe, bg_color, scaling_modifier):
 
 def render_bound(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, override_color=None, depth_alpha=False):
     """Fused route (see module docstring).  depth_alpha=True adds the differentiable "alpha" and "depth" planes."""
-    rs, binding, (fc, fR, fs) = _fused_frame(viewpoint_camera, pc, pipe, bg_color, scaling_modifier)
-    screenspace_points = torch.zeros((pc._xyz.shape[0], 3), dtype=pc._xyz.dtype, device=pc._xyz.device,
+    return _train_frame(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, override_color, depth_alpha)
+
+
+def _train_frame(camera, pc, pipe, bg_color, scaling_modifier, override_color, depth_alpha, size=None):
+    """The differentiable fused-route frame of a camera object, or of the views of a (K, 37) device camera table of
+    image `size` (W, H) (render_views_train): then every output has a leading K."""
+    rs, binding, (fc, fR, fs) = _fused_frame(camera, pc, pipe, bg_color, scaling_modifier, size)
+    lead = () if size is None else (int(camera.shape[0]),)
+    screenspace_points = torch.zeros(lead + (pc._xyz.shape[0], 3), dtype=pc._xyz.dtype, device=pc._xyz.device,
                                      requires_grad=True)
-    out = rasterize_bound(rs, pc._xyz, pc._rotation, pc._scaling, pc._opacity, pc._features_dc, pc._features_rest,
-                          binding, fc, fR, fs, means2D=screenspace_points, colors_precomp=override_color, grad_sink=pc,
-                          tanfov=getattr(viewpoint_camera, "tanfov", None), depth_alpha=depth_alpha)
+    raw = (pc._xyz, pc._rotation, pc._scaling, pc._opacity, pc._features_dc, pc._features_rest, binding, fc, fR, fs)
+    if size is None:
+        out = rasterize_bound(rs, *raw, means2D=screenspace_points, colors_precomp=override_color, grad_sink=pc,
+                              tanfov=getattr(camera, "tanfov", None), depth_alpha=depth_alpha)
+    else:
+        out = rasterize_bound_views_train(rs, camera, *raw, means2D=screenspace_points, grad_sink=pc,
+                                          depth_alpha=depth_alpha)
     rendered_image, radii = out[0], out[1]
     res = {"render": rendered_image, "viewspace_points": screenspace_points, "visibility_filter": _visible(radii),
            "radii": radii}
@@ -84,26 +102,33 @@ def render_bound(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, ove
     return res
 
 
-def _forward_only(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, display: bool, float_image: bool,
-                  depth_alpha: bool = False):
+def _forward_only(camera, pc, pipe, bg_color, scaling_modifier, display: bool, float_image: bool,
+                  depth_alpha: bool = False, size=None):
     """Fused route, forward only (no autograd): the float image and/or the display image [and the alpha / depth
-    planes]."""
+    planes] of a camera object, or of the views of a (K, 37) device camera table of image `size` (W, H)
+    (render_views, GraphedRender): then every output has a leading K."""
     if not _has_raw(pc):
         raise ValueError("render_display needs the fused route: a model exposing the raw parameters "
                          "(_xyz, _rotation, _scaling, _opacity, _features_dc, _features_rest)")
     device = pc._xyz.device
     d = lambda t: None if t is None else t.detach()  # noqa: E731  (no gradient: the forward keeps no backward state)
     with torch.no_grad():
-        rs, binding, (fc, fR, fs) = _fused_frame(viewpoint_camera, pc, pipe, bg_color, scaling_modifier)
-        rgb8 = torch.empty((rs.image_height, rs.image_width, 3), dtype=torch.uint8, device=device) if display else None
-        out = rasterize_bound(rs, d(pc._xyz), d(pc._rotation), d(pc._scaling), d(pc._opacity), d(pc._features_dc),
-                              d(pc._features_rest), binding, d(fc), d(fR), d(fs), grad_sink=pc,
-                              tanfov=getattr(viewpoint_camera, "tanfov", None), rgb8=rgb8, float_image=float_image,
-                              depth_alpha=depth_alpha)
-    img, radii = out[0], out[1]
-    res = {"display_u8": rgb8, "render": img, "radii": radii, "visibility_filter": _visible(radii)}
+        rs, binding, (fc, fR, fs) = _fused_frame(camera, pc, pipe, bg_color, scaling_modifier, size)
+        raw = (d(pc._xyz), d(pc._rotation), d(pc._scaling), d(pc._opacity), d(pc._features_dc), d(pc._features_rest),
+               binding, d(fc), d(fR), d(fs))
+        if size is None:
+            rgb8 = torch.empty((rs.image_height, rs.image_width, 3), dtype=torch.uint8, device=device) \
+                if display else None
+            img, radii, *planes = rasterize_bound(rs, *raw, grad_sink=pc, tanfov=getattr(camera, "tanfov", None),
+                                                  rgb8=rgb8, float_image=float_image, depth_alpha=depth_alpha)
+            visible = _visible(radii)
+        else:
+            img, rgb8, radii, visible, *planes = rasterize_bound_views(
+                rs, camera, *raw, hints=view_hints_of(pc), display=display, float_image=float_image,
+                depth_alpha=depth_alpha)
+    res = {"display_u8": rgb8, "render": img, "radii": radii, "visibility_filter": visible}
     if depth_alpha:
-        res["alpha"], res["depth"] = out[2], out[3]
+        res["alpha"], res["depth"] = planes
     return res
 
 
@@ -141,7 +166,7 @@ def render_views(cameras, pc, pipe, bg_color, scaling_modifier=1.0, float_image=
     "visibility_filter": (K,P) bool}; view k equals render_display(cameras[k], ...) bit for bit.  depth_alpha=True adds
     "alpha" and "depth", (K,1,H,W) float32, view k's those of render_display(cameras[k], ..., depth_alpha=True)."""
     table, W, H = _views_table(cameras, pc, width, height, "render_views")
-    return _views_forward(table, W, H, pc, pipe, bg_color, scaling_modifier, True, float_image, depth_alpha)
+    return _forward_only(table, pc, pipe, bg_color, scaling_modifier, True, float_image, depth_alpha, (W, H))
 
 
 def _views_table(cameras, pc, width, height, what):
@@ -164,22 +189,6 @@ def _views_table(cameras, pc, width, height, what):
     return camera_table(cameras, device), W, H
 
 
-def _views_settings(W, H, pc, pipe, bg_color, scaling_modifier):
-    return GaussianRasterizationSettings(image_height=H, image_width=W, tanfovx=1.0, tanfovy=1.0, bg=bg_color,
-                                         scale_modifier=scaling_modifier, viewmatrix=None, projmatrix=None,
-                                         sh_degree=pc.active_sh_degree, campos=None, prefiltered=False,
-                                         debug=bool(getattr(pipe, "debug", False)))
-
-
-def _face_frame_of(pc):
-    binding = getattr(pc, "binding", None)
-    if binding is None:
-        return None, (None, None, None)
-    if getattr(pc, "face_center", None) is None:
-        pc.select_mesh_by_timestep(0)
-    return binding, (pc.face_center, pc.face_orien_mat, pc.face_scaling)
-
-
 def render_views_train(cameras, pc, pipe, bg_color, scaling_modifier=1.0, width=None, height=None, depth_alpha=False):
     """The training form of render_views: every camera of one timestep (the model's current face frame) in ONE
     differentiable forward (gab200_forward_views_train).  Returns render()'s dict with a leading K:
@@ -190,37 +199,7 @@ def render_views_train(cameras, pc, pipe, bg_color, scaling_modifier=1.0, width=
     planes, (K,1,H,W), view k's those of render(cameras[k], ..., depth_alpha=True): a mask or depth term of every view
     joins the same loss and the same backward."""
     table, W, H = _views_table(cameras, pc, width, height, "render_views_train")
-    rs = _views_settings(W, H, pc, pipe, bg_color, scaling_modifier)
-    binding, (fc, fR, fs) = _face_frame_of(pc)
-    K, P = int(table.shape[0]), int(pc._xyz.shape[0])
-    screenspace_points = torch.zeros((K, P, 3), dtype=pc._xyz.dtype, device=pc._xyz.device, requires_grad=True)
-    out = rasterize_bound_views_train(rs, table, pc._xyz, pc._rotation, pc._scaling, pc._opacity, pc._features_dc,
-                                      pc._features_rest, binding, fc, fR, fs, means2D=screenspace_points, grad_sink=pc,
-                                      depth_alpha=depth_alpha)
-    image, radii = out[0], out[1]
-    res = {"render": image, "viewspace_points": screenspace_points, "visibility_filter": _visible(radii),
-           "radii": radii}
-    if depth_alpha:
-        res["alpha"], res["depth"] = out[2], out[3]
-    return res
-
-
-def _views_forward(table, W, H, pc, pipe, bg_color, scaling_modifier, display: bool, float_image: bool,
-                   depth_alpha: bool = False):
-    """The fused route's K-view forward of a (K, 37) device camera table (render_views, GraphedRender)."""
-    d = lambda t: None if t is None else t.detach()  # noqa: E731
-    with torch.no_grad():
-        rs = _views_settings(W, H, pc, pipe, bg_color, scaling_modifier)
-        binding, (fc, fR, fs) = _face_frame_of(pc)
-        out = rasterize_bound_views(
-            rs, table, d(pc._xyz), d(pc._rotation), d(pc._scaling), d(pc._opacity), d(pc._features_dc),
-            d(pc._features_rest), binding, d(fc), d(fR), d(fs), hints=view_hints_of(pc), display=display,
-            float_image=float_image, depth_alpha=depth_alpha)
-    img, rgb8, radii, visible = out[:4]
-    res = {"display_u8": rgb8, "render": img, "radii": radii, "visibility_filter": visible}
-    if depth_alpha:
-        res["alpha"], res["depth"] = out[4], out[5]
-    return res
+    return _train_frame(table, pc, pipe, bg_color, scaling_modifier, None, depth_alpha, (W, H))
 
 
 def _visible(radii):
