@@ -50,7 +50,7 @@ def _nvcc():
 
 
 def _newest_header():
-    inc = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h", ".inc"))]
+    inc = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))]
     inc.append(os.path.join(HERE, "..", "include", "gab200_rasterizer.h"))
     return max(os.path.getmtime(p) for p in inc)
 

@@ -459,12 +459,8 @@ int enqueue_geometry(Frame& f, bool bucket, bool run_preprocess, uint32_t capaci
 // key emission of the frame's (virtual) splats in depth order
 void emit(const Frame& f, const uint32_t* offsets, uint32_t cap, uint32_t* cursor, const BinView& bv,
           const EmitClears& clr) {
-  if (f.cameras != nullptr)
-    launch_emit_keys_views(f.P, f.gx, f.gy, f.g.rec, f.g.aux, f.g.ids[f.selA], offsets, f.order_count, f.g.buckets.meta,
-                           cap, cursor, bv.keys[0], bv.vals[0], f.a->exact_binning, f.a->P, clr, f.stream);
-  else
-    launch_emit_keys(f.P, f.gx, f.gy, f.g.rec, f.g.aux, f.g.ids[f.selA], offsets, f.order_count, f.g.buckets.meta, cap,
-                     cursor, bv.keys[0], bv.vals[0], f.a->exact_binning, clr, f.stream);
+  launch_emit_keys(f.P, f.gx, f.gy, f.g.rec, f.g.aux, f.g.ids[f.selA], offsets, f.order_count, f.g.buckets.meta, cap,
+                   cursor, bv.keys[0], bv.vals[0], f.a->exact_binning, f.cameras != nullptr ? f.a->P : 0, clr, f.stream);
 }
 
 // emit -> per-instance tile sort -> ranges -> tile order -> blend, for a binning buffer of `cap` instances.
@@ -863,15 +859,10 @@ static int32_t run_backward(const gab200_backward_args* b, const float* tanfov, 
   GAB_STAGE_CHECK(dbg, stream);
   {
     StageScope sc(GAB200_STAGE_PREPROCESS_BWD, stream);
-    if (cameras != nullptr) {
-      gab200_backward_args bb = *b;
-      bb.fwd = &v;
-      launch_preprocess_backward_views(bb, views, cameras, g.aux, g.clamped, g.g2d, csr ? g.face_scratch : nullptr,
-                                       stream, da);
-    } else {
-      launch_preprocess_backward(*b, g.rec, g.aux, g.clamped, g.g2d, csr ? g.face_scratch : nullptr, tanfov, stream,
-                                 da);
-    }
+    gab200_backward_args bb = *b;
+    if (cameras != nullptr) bb.fwd = &v;  // the multi-view frame's arguments as its forward ran them
+    launch_preprocess_backward(bb, views, cameras, tanfov, g.aux, g.clamped, g.g2d, csr ? g.face_scratch : nullptr, da,
+                               stream);
   }
   GAB_STAGE_CHECK(dbg, stream);
   return GAB200_OK;

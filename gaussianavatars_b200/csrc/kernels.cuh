@@ -150,16 +150,12 @@ struct EmitClears {
 };
 // `capacity`: instances the key/value arrays hold -- anything beyond is dropped (the frame's counters say so);
 // counters[BUCKET_OVERFLOW] != 0 (depth order unusable) emits nothing.
+// view_splats > 0: the P virtual splats of a multi-view frame, view_splats per view -- instances of virtual splat v go
+// to the tiles (v / view_splats) * (gx * gy) + the tile in the view; 0: a single view
 void launch_emit_keys(int P, int gx, int gy, const SplatRec* rec, const SplatAux* aux, const uint32_t* order,
                       const uint32_t* offsets, const uint32_t* order_count, const uint32_t* counters, uint32_t capacity,
-                      uint32_t* cursor, uint32_t* keys, uint32_t* vals, int exact_binning, const EmitClears& clr,
-                      cudaStream_t stream);
-// the same over the P virtual splats of a multi-view frame, view_splats per view: instances of virtual splat v go to
-// the tiles (v / view_splats) * (gx * gy) + the tile in the view
-void launch_emit_keys_views(int P, int gx, int gy, const SplatRec* rec, const SplatAux* aux, const uint32_t* order,
-                            const uint32_t* offsets, const uint32_t* order_count, const uint32_t* counters, uint32_t cap,
-                            uint32_t* cursor, uint32_t* keys, uint32_t* vals, int exact_binning, int view_splats,
-                            const EmitClears& clr, cudaStream_t stream);
+                      uint32_t* cursor, uint32_t* keys, uint32_t* vals, int exact_binning, int view_splats,
+                      const EmitClears& clr, cudaStream_t stream);
 // keys[0..N) sorted; entries with key >= tiles are padding (sentinel) behind the last real instance
 void launch_tile_ranges(int64_t N, uint32_t tiles, const uint32_t* keys, uint2* ranges, cudaStream_t stream);
 void launch_expand_keys(int64_t N, const uint32_t* tile_keys, const uint32_t* ids, const SplatAux* aux, uint64_t* out,
@@ -202,19 +198,16 @@ void launch_blend_backward(int views, int W, int H, const uint2* ranges, const u
                            const uint8_t* strip_mask, float* g2d, bool da, const float* dL_dalpha,
                            const float* dL_ddepth, cudaStream_t stream);
 // preprocess_bwd.cu
-// depth: g2d slot 9 holds dL/dz (gab200_backward_depth_alpha), added to dL/dmean through the view matrix's third row;
-// no multicast
-void launch_preprocess_backward(const gab200_backward_args& b, const SplatRec* rec, const SplatAux* aux,
-                                const uint8_t* clamped, const float* g2d, float* face_scratch, const float* tanfov,
-                                cudaStream_t stream, bool depth = false);
-// gab200_backward_views (BOUND_RAW, no colors_precomp, no multicast): one thread per real splat sums the gradients of
-// its `views` virtual splats (camera row k of `cameras`; rec / aux / clamped / g2d rows k * P + i) and stores each
-// parameter gradient once; dL_dmeans2D [views,P,3]; face-frame gradients as launch_preprocess_backward's.
-// depth: g2d slot 9 holds each virtual splat's dL/dz (gab200_backward_views_depth_alpha), added through view k's own
-// view-matrix row
-void launch_preprocess_backward_views(const gab200_backward_args& b, int views, const float* cameras,
-                                      const SplatAux* aux, const uint8_t* clamped, const float* g2d,
-                                      float* face_scratch, cudaStream_t stream, bool depth = false);
+// cameras == NULL: one camera, its field of view from the device float[2] `tanfov` or, when that is NULL, from `b.fwd`;
+// either input mode, multicast gradients allowed (BOUND_RAW).  Otherwise (gab200_backward_views*: BOUND_RAW, no
+// colors_precomp, no multicast) `views` cameras: one thread per real splat sums the gradients of its `views` virtual
+// splats (camera row k of `cameras`; aux / clamped / g2d rows k * P + i) and stores each parameter gradient once;
+// dL_dmeans2D [views,P,3].  face_scratch != NULL (BOUND_RAW, CSR face route): per-splat face-frame gradients, summed
+// per face by face_grad_reduce_kernel.  da: g2d slot 9 holds each (virtual) splat's dL/dz of the depth plane, added
+// to dL/dmean through its view matrix's third row; no multicast
+void launch_preprocess_backward(const gab200_backward_args& b, int views, const float* cameras, const float* tanfov,
+                                const SplatAux* aux, const uint8_t* clamped, const float* g2d, float* face_scratch,
+                                bool da, cudaStream_t stream);
 #define GAB_FACE_GRAD_STRIDE 13  // per-splat face-frame gradient record: centre 3, orientation 9, scale 1
 
 // face_frame.cu

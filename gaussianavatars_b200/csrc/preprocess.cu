@@ -16,28 +16,13 @@ namespace gab {
 #define REC_SCALE_AC (-0.5f * 1.4426950408889634f)
 #define REC_SCALE_B (-1.4426950408889634f)
 
-// the camera of a block: viewmatrix (16) | projmatrix (16) | campos (3)
-__device__ __forceinline__ void stage_camera(const float* __restrict__ V, const float* __restrict__ Pm,
-                                             const float* __restrict__ campos, Camera& cam) {
-  int t = threadIdx.x;
-  if (t < 16) cam.V[t] = V[t];
-  else if (t < 32) cam.Pm[t - 16] = Pm[t - 16];
-  else if (t < 35) cam.campos[t - 32] = campos[t - 32];
-  __syncthreads();
-}
-
 // =====================================================================================================
 // K1: fused bind + activate + project + EWA + SH->RGB.  One thread per splat.
-// CAM: where the camera comes from.
-//   CAM_ARGS   : the by-value matrices and tanfovx / tanfovy of `a` (gab200_forward).
-//   CAM_DEVFOV : the same matrices, (tanfovx, tanfovy) from the device float[2] `tanfov` (gab200_forward_device_fov),
-//                so that a captured graph renders whatever field of view was written before the replay.
-//   CAM_TABLE  : row blockIdx.y of the device camera table (gab200_forward_views*), its field of view read as
-//                CAM_DEVFOV reads it; outputs at the virtual splat view * P + i, tile counts in the view's slice.
+// CAM (splat_math.cuh): CAM_TABLE renders row blockIdx.y of the camera table; outputs at the virtual splat
+// view * P + i, tile counts in the view's slice.
 // DA: the record also carries the view-space depth z in q2.w, read by the depth plane of the blend (forward and
 // backward).  clamped != nullptr: the per-channel colour clamp bits, which the backward reads.
 // =====================================================================================================
-enum { CAM_ARGS, CAM_DEVFOV, CAM_TABLE };
 template <bool BOUND, int CAM, bool DA>
 __global__ void __launch_bounds__(PRE_NT) preprocess_kernel(gab200_forward_args a, const float* __restrict__ cameras,
                                                             const float* __restrict__ tanfov, SplatRec* __restrict__ rec,
@@ -658,6 +643,7 @@ __device__ __forceinline__ void emit_keys(int P, int gx, int gy, const SplatRec*
   }
 }
 
+template <bool VIEWS>
 __global__ void __launch_bounds__(256) emit_keys_kernel(int P, int gx, int gy, const SplatRec* __restrict__ rec,
                                                         const SplatAux* __restrict__ aux,
                                                         const uint32_t* __restrict__ order,
@@ -666,33 +652,14 @@ __global__ void __launch_bounds__(256) emit_keys_kernel(int P, int gx, int gy, c
                                                         const uint32_t* __restrict__ counters, uint32_t cap,
                                                         uint32_t* __restrict__ cursor,
                                                         uint32_t* __restrict__ keys, uint32_t* __restrict__ vals,
-                                                        int exact_binning, bool sentinel, uint8_t* __restrict__ mask,
-                                                        uint32_t n_mask, uint2* __restrict__ ranges,
-                                                        uint32_t n_ranges) {
+                                                        int exact_binning, uint32_t view_splats, uint32_t view_tiles,
+                                                        bool sentinel, uint8_t* __restrict__ mask, uint32_t n_mask,
+                                                        uint2* __restrict__ ranges, uint32_t n_ranges) {
   pdl_wait();
   pdl_trigger();
   emit_clears(counters, order_count, cap, keys, sentinel, mask, n_mask, ranges, n_ranges);
-  emit_keys<false>(P, gx, gy, rec, aux, order, offsets, order_count, counters, cap, cursor, keys, vals, exact_binning, 1u,
-                   0u);
-}
-
-__global__ void __launch_bounds__(256) emit_keys_views_kernel(int P, int gx, int gy, const SplatRec* __restrict__ rec,
-                                                              const SplatAux* __restrict__ aux,
-                                                              const uint32_t* __restrict__ order,
-                                                              const uint32_t* __restrict__ offsets,
-                                                              const uint32_t* __restrict__ order_count,
-                                                              const uint32_t* __restrict__ counters, uint32_t cap,
-                                                              uint32_t* __restrict__ cursor,
-                                                              uint32_t* __restrict__ keys, uint32_t* __restrict__ vals,
-                                                              int exact_binning, uint32_t view_splats,
-                                                              uint32_t view_tiles, bool sentinel,
-                                                              uint8_t* __restrict__ mask, uint32_t n_mask,
-                                                              uint2* __restrict__ ranges, uint32_t n_ranges) {
-  pdl_wait();
-  pdl_trigger();
-  emit_clears(counters, order_count, cap, keys, sentinel, mask, n_mask, ranges, n_ranges);
-  emit_keys<true>(P, gx, gy, rec, aux, order, offsets, order_count, counters, cap, cursor, keys, vals, exact_binning,
-                  view_splats, view_tiles);
+  emit_keys<VIEWS>(P, gx, gy, rec, aux, order, offsets, order_count, counters, cap, cursor, keys, vals, exact_binning,
+                   view_splats, view_tiles);
 }
 
 __global__ void publish_counters_kernel(uint32_t* __restrict__ counters, const uint32_t* __restrict__ offsets, int P,
@@ -719,25 +686,14 @@ void launch_publish_counters(uint32_t* counters, const uint32_t* offsets, int P,
 
 void launch_emit_keys(int P, int gx, int gy, const SplatRec* rec, const SplatAux* aux, const uint32_t* order,
                       const uint32_t* offsets, const uint32_t* order_count, const uint32_t* counters, uint32_t cap,
-                      uint32_t* cursor, uint32_t* keys, uint32_t* vals, int exact_binning, const EmitClears& clr,
-                      cudaStream_t stream) {
+                      uint32_t* cursor, uint32_t* keys, uint32_t* vals, int exact_binning, int view_splats,
+                      const EmitClears& clr, cudaStream_t stream) {
   const int warps = (P + 31) / 32;
   const int threads = 256, blocks = (warps * 32 + threads - 1) / threads;
   if (blocks == 0) return;
-  launch_pdl(emit_keys_kernel, blocks, threads, 0, stream, P, gx, gy, rec, aux, order, offsets, order_count, counters,
-             cap, cursor, keys, vals, exact_binning, clr.sentinel, clr.mask, clr.n_mask, clr.ranges, clr.n_ranges);
-}
-
-void launch_emit_keys_views(int P, int gx, int gy, const SplatRec* rec, const SplatAux* aux, const uint32_t* order,
-                            const uint32_t* offsets, const uint32_t* order_count, const uint32_t* counters, uint32_t cap,
-                            uint32_t* cursor, uint32_t* keys, uint32_t* vals, int exact_binning, int view_splats,
-                            const EmitClears& clr, cudaStream_t stream) {
-  const int warps = (P + 31) / 32;
-  const int threads = 256, blocks = (warps * 32 + threads - 1) / threads;
-  if (blocks == 0) return;
-  launch_pdl(emit_keys_views_kernel, blocks, threads, 0, stream, P, gx, gy, rec, aux, order, offsets, order_count,
-             counters, cap, cursor, keys, vals, exact_binning, (uint32_t)view_splats, (uint32_t)(gx * gy),
-             clr.sentinel, clr.mask, clr.n_mask, clr.ranges, clr.n_ranges);
+  launch_pdl(view_splats > 0 ? emit_keys_kernel<true> : emit_keys_kernel<false>, blocks, threads, 0, stream, P, gx, gy,
+             rec, aux, order, offsets, order_count, counters, cap, cursor, keys, vals, exact_binning,
+             (uint32_t)view_splats, (uint32_t)(gx * gy), clr.sentinel, clr.mask, clr.n_mask, clr.ranges, clr.n_ranges);
 }
 
 // =====================================================================================================

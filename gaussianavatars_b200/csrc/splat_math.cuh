@@ -77,6 +77,25 @@ __device__ __forceinline__ void stage_rows_out(const float* smem, float* __restr
   }
 }
 
+// Where a per-splat kernel's camera comes from:
+//   CAM_ARGS   : the by-value matrices and tanfovx / tanfovy of `a` (gab200_forward, gab200_backward).
+//   CAM_DEVFOV : the same matrices, (tanfovx, tanfovy) from a device float[2] `tanfov` (gab200_forward_device_fov,
+//                gab200_backward_device_fov), so that a captured graph runs whatever field of view was written before
+//                the replay.
+//   CAM_TABLE  : rows of the device camera table (the *_views* forms), each row's field of view read as CAM_DEVFOV
+//                reads it.
+enum { CAM_ARGS, CAM_DEVFOV, CAM_TABLE };
+
+// the camera of a block: viewmatrix (16) | projmatrix (16) | campos (3)
+__device__ __forceinline__ void stage_camera(const float* __restrict__ V, const float* __restrict__ Pm,
+                                             const float* __restrict__ campos, Camera& cam) {
+  int t = threadIdx.x;
+  if (t < 16) cam.V[t] = V[t];
+  else if (t < 32) cam.Pm[t - 16] = Pm[t - 16];
+  else if (t < 35) cam.campos[t - 32] = campos[t - 32];
+  __syncthreads();
+}
+
 __device__ __forceinline__ float3 xform4x3(const float* M, float3 p) {
   float3 r;
   r.x = M[0] * p.x + M[4] * p.y + M[8] * p.z + M[12];
