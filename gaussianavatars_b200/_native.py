@@ -234,7 +234,8 @@ EXPORTED_SYMBOLS = ("gab200_forward", "gab200_backward", "gab200_mark_visible", 
                     "gab200_frame_encode_plan", "gab200_frame_encode", "gab200_frame_decode",
                     "gab200_schedule_sample", "gab200_schedule_commit", "gab200_lpips_weights_bytes",
                     "gab200_lpips_pack", "gab200_lpips_scratch_bytes", "gab200_lpips_features_bytes",
-                    "gab200_lpips")
+                    "gab200_lpips", "gab200_png_bound", "gab200_png_scratch_bytes", "gab200_png_encode",
+                    "gab200_png_copy")
 
 _lib = None
 _lock = threading.Lock()
@@ -341,6 +342,16 @@ def lib():
         L.gab200_frame_decode.restype = C.c_int32
         L.gab200_frame_decode.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gab200_png_bound.restype = C.c_int64
+        L.gab200_png_bound.argtypes = [C.c_int32, C.c_int32]
+        L.gab200_png_scratch_bytes.restype = C.c_size_t
+        L.gab200_png_scratch_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
+        L.gab200_png_encode.restype = C.c_int32
+        L.gab200_png_encode.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_int64, C.c_void_p, C.c_void_p]
+        L.gab200_png_copy.restype = C.c_int32
+        L.gab200_png_copy.argtypes = [C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_int64, C.c_void_p, C.c_void_p]
         L.gab200_schedule_sample.restype = C.c_int32
         L.gab200_schedule_sample.argtypes = [C.c_int32, C.c_int32, C.c_int32] + [C.c_void_p] * 11
         L.gab200_schedule_commit.restype = C.c_int32

@@ -34,6 +34,7 @@ SOURCES = {
     "loss.cu": [],
     "composite.cu": [],
     "frames.cu": [],
+    "png.cu": [],
     "schedule.cu": [],
     "metrics.cu": [],
     "lpips.cu": [],

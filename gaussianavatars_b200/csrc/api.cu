@@ -986,6 +986,38 @@ int32_t gab200_frame_decode(int32_t views, int32_t height, int32_t width, const 
   return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
 }
 
+int64_t gab200_png_bound(int32_t width, int32_t height) {
+  const int64_t b = png_bound(height, width);
+  return b < 0 ? GAB200_ERR_INVALID_ARGUMENT : b;
+}
+
+size_t gab200_png_scratch_bytes(int32_t views, int32_t height, int32_t width) {
+  return png_scratch_bytes(views, height, width);
+}
+
+int32_t gab200_png_encode(int32_t views, int32_t height, int32_t width, const uint8_t* rgb, void* scratch,
+                          uint8_t* out, int64_t out_stride, int64_t* out_len, void* stream_) {
+  if (views <= 0 || views > 65535 || height <= 0 || width <= 0) return GAB200_ERR_INVALID_ARGUMENT;
+  const int64_t bound = png_bound(height, width);
+  if (bound < 0 || out_stride < bound) return GAB200_ERR_INVALID_ARGUMENT;
+  if (!rgb || !scratch || !out || !out_len || ((uintptr_t)scratch & 255) != 0) return GAB200_ERR_INVALID_ARGUMENT;
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  launch_png_encode(views, height, width, rgb, scratch, out, out_stride, out_len, (cudaStream_t)stream_);
+  return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
+int32_t gab200_png_copy(int32_t views, const uint8_t* src, int64_t src_stride, const int64_t* src_len,
+                        const int32_t* flag, uint8_t* dst, int64_t dst_stride, int64_t* dst_len, void* stream_) {
+  if (views <= 0 || views > 65535 || src_stride <= 0 || dst_stride < src_stride || (src_stride & 15) != 0 ||
+      (dst_stride & 15) != 0)
+    return GAB200_ERR_INVALID_ARGUMENT;
+  if (!src || !src_len || !dst || !dst_len || ((uintptr_t)src & 15) != 0 || ((uintptr_t)dst & 15) != 0)
+    return GAB200_ERR_INVALID_ARGUMENT;
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  launch_png_copy(views, src, src_stride, src_len, flag, dst, dst_stride, dst_len, (cudaStream_t)stream_);
+  return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
 int32_t gab200_schedule_sample(int32_t records, int32_t views, int32_t length, const float* cams,
                                const int32_t* timesteps, const int32_t* frame_ids, const int32_t* order,
                                const int32_t* cursor, float* cam_out, int32_t* timestep_out, int32_t* ids_out,

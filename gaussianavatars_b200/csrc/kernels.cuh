@@ -236,6 +236,14 @@ void launch_frame_encode(int64_t frames, int H, int W, const uint8_t* gt, const 
 void launch_frame_decode(int views, int H, int W, const int32_t* ids, const uint8_t* arena, const int64_t* frame_base,
                          const uint32_t* tile_off, uint8_t* gt, uint8_t* mask, cudaStream_t stream);
 
+// png.cu
+int64_t png_bound(int H, int W);
+size_t png_scratch_bytes(int64_t views, int H, int W);
+void launch_png_encode(int views, int H, int W, const uint8_t* rgb, void* scratch, uint8_t* out, int64_t out_stride,
+                       int64_t* out_len, cudaStream_t stream);
+void launch_png_copy(int views, const uint8_t* src, int64_t src_stride, const int64_t* src_len, const int32_t* flag,
+                     uint8_t* dst, int64_t dst_stride, int64_t* dst_len, cudaStream_t stream);
+
 // schedule.cu
 void launch_schedule_sample(int records, int views, int length, const float* cams, const int32_t* timesteps,
                             const int32_t* frame_ids, const int32_t* order, const int32_t* cursor, float* cam_out,

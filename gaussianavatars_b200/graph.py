@@ -57,6 +57,7 @@ from .training import (METRIC_NAMES, Adam, binding_regularizers, launch_composit
                        metrics_scratch, photometric_loss)
 from .flame import check_timestep, flame_pose
 from .lpips import LpipsNet, launch_lpips, lpips_scratch
+from . import png as PNG
 
 _STATS = ("xyz_gradient_accum", "denom", "max_radii2D")
 _FLAME_KEYS = ("shape", "static_offset", "expr", "rotation", "neck_pose", "jaw_pose", "eyes_pose", "translation")
@@ -965,7 +966,8 @@ class GraphedRender(_Captured):
                  scaling_modifier: float = 1.0, mesh_update: bool = True, host_slots: int = 0,
                  capacity: Optional[int] = None, headroom: float = 1.25, warm_cameras=None, warm_timesteps=None,
                  mesh_opacity: Optional[float] = None, face_colors: Optional[torch.Tensor] = None,
-                 mesh_lighting: str = "front", views_per_replay: int = 1, depth_alpha: bool = False):
+                 mesh_lighting: str = "front", views_per_replay: int = 1, depth_alpha: bool = False,
+                 png: bool = False):
         """outputs: "u8" (the display image only: the float image is not written), "float" or "both".
         warm_cameras: camera objects or 37-float blocks rendered eagerly before the capture to size the capacity (and
         the depth-sort range); warm_timesteps: with a FLAME head, the timesteps each warm camera is rendered at
@@ -976,9 +978,15 @@ class GraphedRender(_Captured):
         dimension.  Not combinable with the mesh overlay.
         depth_alpha=True: every replay also refreshes `alpha` and `depth`, (1,H,W) float32 static tensors -- the
         splats' accumulated opacity and alpha-weighted view-space depth from the same blend (gab200_forward_depth_alpha;
-        with the mesh overlay they remain the splats').  Single-view replays only."""
+        with the mesh overlay they remain the splats').  Single-view replays only.
+        png=True: the captured body ends in the PNG encode of `display` (after the mesh overlay; png.encode_png's
+        kernels) into graph-owned scratch, `png_out` ((K, capacity) uint8) and `png_len` ((K,) int64).  With
+        host_slots the ring also receives the compressed files, and host_png(i) returns replay i's file (K files with
+        views_per_replay=K)."""
         if outputs not in ("u8", "float", "both"):
             raise ValueError("outputs must be 'u8', 'float' or 'both'")
+        if png and outputs == "float":
+            raise ValueError("png=True encodes the display image: it needs outputs 'u8' or 'both'")
         _check_views_per_replay(views_per_replay)
         if depth_alpha and views_per_replay > 1:
             raise ValueError("depth_alpha renders one camera per replay: it needs views_per_replay=1 (the K-view "
@@ -994,6 +1002,9 @@ class GraphedRender(_Captured):
                          warm_cameras, warm_timesteps)
         self.outputs, self.scaling_modifier, self.mesh_update = outputs, float(scaling_modifier), bool(mesh_update)
         self.host_slots = int(host_slots)
+        self.png = bool(png)
+        self.png_out = self.png_len = self._png_scratch = None
+        self.host_png_slots = self._png_staged = None
         self.host = self._copy_stream = None
         self._staged = self._host_events = self._stage_events = None
         self.image = self.display = self.radii = self.alpha = self.depth = None
@@ -1070,6 +1081,16 @@ class GraphedRender(_Captured):
                 out["display_u8"] = self._overlay(out["render"])
         self.image, self.display, self.radii = out["render"], out["display_u8"], out["radii"]
         self.alpha, self.depth = out.get("alpha"), out.get("depth")
+        if captured and self.png:   # the warm-up frames encode nothing
+            self._encode_png()
+
+    def _encode_png(self):
+        """The display frame(s) -> PNG files in buffers the capture allocates (the graph's own pool)."""
+        K, dev = self.K, self.device
+        self._png_scratch = PNG.scratch(K, self.H, self.W, dev)
+        self.png_out = torch.empty((K, PNG.slot_stride(self.W, self.H)), dtype=torch.uint8, device=dev)
+        self.png_len = torch.empty(K, dtype=torch.int64, device=dev)
+        PNG.launch_encode(self.display, self._png_scratch, self.png_out, self.png_len)
 
     def _overlay(self, image):
         """The mesh of the vertices the frame just posed (pc.verts) over the float splat image -> (H,W,3) uint8."""
@@ -1088,6 +1109,7 @@ class GraphedRender(_Captured):
     # ---- capture ---------------------------------------------------------------------------------------------------
     def _release(self):
         self.image = self.display = self.radii = self.alpha = self.depth = None
+        self.png_out = self.png_len = self._png_scratch = None
 
     def _before_capture(self):
         if self.camera is not None:
@@ -1122,6 +1144,14 @@ class GraphedRender(_Captured):
             torch.cuda.synchronize(self.device)
             self.host = [torch.empty(shape, dtype=torch.uint8).pin_memory() for _ in range(k)]
             self._staged = [torch.empty(shape, dtype=torch.uint8, device=self.device) for _ in range(2)]
+        if self.png:   # per slot: K int64 lengths (-1: the replay overflowed), then K files of png_out's stride
+            stride = int(self.png_out.shape[1])
+            rows = (8 * self.K + stride - 1) // stride + self.K
+            if self.host_png_slots is None or tuple(self.host_png_slots[0].shape) != (rows, stride):
+                torch.cuda.synchronize(self.device)
+                self.host_png_slots = [torch.empty((rows, stride), dtype=torch.uint8).pin_memory() for _ in range(k)]
+                self._png_staged = [torch.empty((rows, stride), dtype=torch.uint8, device=self.device)
+                                    for _ in range(2)]
         self._copy_stream = self._copy_stream or torch.cuda.Stream(device=self.device)
         self._host_events = [None] * k     # per host slot: the copy into it, and which replay it holds
         self._host_replay = [-1] * k
@@ -1137,15 +1167,51 @@ class GraphedRender(_Captured):
         if self._stage_events[s] is not None:
             cur.wait_event(self._stage_events[s])
         self._staged[s].copy_(self.display)
+        if self.png:   # the compressed bytes only, and -1 for a replay that overflowed (the slot's sticky flag)
+            self._png_copy(self.png_out, self.png_len, self._png_staged[s], self.slot.flag)
         ready = torch.cuda.Event()
         ready.record(cur)
         self._copy_stream.wait_event(ready)
         with torch.cuda.stream(self._copy_stream):
             self.host[h].copy_(self._staged[s], non_blocking=True)
+            if self.png:   # staged -> the pinned slot, written by a kernel through its mapped address
+                st = self._png_staged[s]
+                self._png_copy(self._png_rows(st), self._png_lengths(st), self.host_png_slots[h])
             done = torch.cuda.Event()
             done.record(self._copy_stream)
         self._stage_events[s] = self._host_events[h] = done
         self._host_replay[h] = i
+
+    def _png_lengths(self, slot):
+        """The (K,) int64 lengths at the head of a ring slot."""
+        return slot.reshape(-1)[:8 * self.K].view(torch.int64)
+
+    def _png_rows(self, slot):
+        """The K file rows at the tail of a ring slot."""
+        return slot[slot.shape[0] - self.K:]
+
+    def _png_copy(self, src, src_len, slot, flag=None):
+        PNG.launch_copy(src, src_len, self._png_rows(slot), self._png_lengths(slot), flag)
+
+    def host_png(self, replay: Optional[int] = None):
+        """Replay `replay`'s PNG file (default: the latest) as bytes -- K files with views_per_replay=K -- once its copy
+        has landed.  Raises when that replay overflowed its instance capacity: its frame is incomplete."""
+        if not self.png:
+            raise ValueError("host_png needs a frame built with png=True")
+        if not self.host_slots:
+            raise ValueError("host_png needs host_slots > 0")
+        i = self.replays - 1 if replay is None else int(replay)
+        h = i % self.host_slots
+        if self._host_replay[h] != i:
+            raise IndexError(f"replay {i} is not in the host ring (slot {h} holds replay {self._host_replay[h]})")
+        self._host_events[h].synchronize()
+        slot = self.host_png_slots[h]
+        lens, rows = self._png_lengths(slot).tolist(), self._png_rows(slot)
+        if min(lens) < 0:
+            raise RuntimeError(f"{type(self).__name__}: replay {i} overflowed its instance capacity, so its frame is "
+                               "incomplete and no PNG file is given for it: regrow() and run it again")
+        files = [rows[k, :lens[k]].numpy().tobytes() for k in range(self.K)]
+        return files[0] if self.K == 1 else files
 
     def host_frame(self, replay: Optional[int] = None) -> torch.Tensor:
         """The pinned (H,W,3) uint8 slot ((K,H,W,3) with views_per_replay=K) holding replay `replay` (default: the latest) once its copy has landed."""
@@ -1191,7 +1257,8 @@ class GraphedEval(GraphedRender):
     mean of the three per-channel PSNRs).  source="u8": it renders the display image only (render.py's bytes) and
     scores those as metrics.py reads them back (value/255); `psnr_all` is metrics.py's PSNR (one MSE over all
     values).  With host_slots (source="u8" only) each replay also ships its display frame to the pinned host ring, so
-    one replay yields both the PNG bytes render.py would write and the view's scores.
+    one replay yields both the PNG bytes render.py would write and the view's scores.  png=True (source="u8") also
+    encodes those bytes into a PNG file inside the replay, scores unchanged; host_png(i) returns it.
 
     camera, timestep, background, ground truth and view index are device buffers written by set_inputs: none of them
     re-captures.  A HOST ground truth (pinned, for an upload that overlaps the replays) travels on a copy stream the
@@ -1206,7 +1273,8 @@ class GraphedEval(GraphedRender):
 
     def __init__(self, pc, width: int, height: int, bg: torch.Tensor, views: int, source: str = "float",
                  host_slots: int = 0, capacity: Optional[int] = None, headroom: float = 1.25, warm_cameras=None,
-                 warm_timesteps=None, views_per_replay: int = 1, schedule=None, frames=None, lpips=None):
+                 warm_timesteps=None, views_per_replay: int = 1, schedule=None, frames=None, lpips=None,
+                 png: bool = False):
         """views_per_replay=K > 1: one replay renders K cameras of one timestep in one forward and scores them into
         rows view .. view + K - 1 (set_inputs(cameras=K cameras, gt_u8=(K,3,H,W), view=first row)); warm_cameras is a
         list of K-camera groups.  K is fixed per capture: a last group of fewer views is the business of a
@@ -1223,6 +1291,8 @@ class GraphedEval(GraphedRender):
                              "display bytes render.py writes, scored as metrics.py reads them)")
         if host_slots and source != "u8":
             raise ValueError("host_slots ships the display image: it needs source='u8'")
+        if png and source != "u8":
+            raise ValueError("png=True encodes the display image: it needs source='u8'")
         if int(views) < 1:
             raise ValueError("views must be at least 1")
         if isinstance(views_per_replay, int) and views_per_replay > int(views):
@@ -1235,7 +1305,7 @@ class GraphedEval(GraphedRender):
                                  f"{lpips.min_side} pixels, got {int(width)}x{int(height)}")
         super().__init__(pc, width, height, bg, outputs="float" if source == "float" else "u8", host_slots=host_slots,
                          capacity=capacity, headroom=headroom, warm_cameras=warm_cameras, warm_timesteps=warm_timesteps,
-                         views_per_replay=views_per_replay)
+                         views_per_replay=views_per_replay, png=png)
         self.source, self.views = source, int(views)
         self.table = torch.empty((self.views, N.METRICS_FIELDS), dtype=torch.float32, device=self.device)
         if lpips is not None and lpips.device != self.device:

@@ -448,6 +448,32 @@ int32_t gab200_frame_decode(int32_t views, int32_t height, int32_t width, const 
                             const int64_t* frame_base, const uint32_t* tile_off, uint8_t* gt_out, uint8_t* mask_out,
                             void* stream);
 
+/* PNG files written on the device (csrc/png.cu, gaussianavatars_b200.png): 8-bit RGB (colour type 2), not interlaced,
+ * chunks signature | IHDR | one IDAT | IEND, each with its CRC-32; the IDAT data is one zlib stream.  Each row gets
+ * the PNG filter with the least sum of its bytes read as signed magnitudes (v < 128 ? v : 256 - v; ties: the lowest
+ * filter id); the filtered stream is cut into 32 KiB segments, each one deflate block -- dynamic Huffman, fixed
+ * Huffman or stored, the smallest by exact bit count -- whose matches reach up to 32 KiB back into the same image.
+ * The same input always gives the same file.
+ *
+ * Bound: the largest file of a width x height image, 63 + n + 6 ceil(n / 32768) bytes for n = height (3 width + 1),
+ * or GAB200_ERR_INVALID_ARGUMENT for a size <= 0 or one whose IDAT would not fit its 31-bit length. */
+int64_t gab200_png_bound(int32_t width, int32_t height);
+/* Scratch bytes of an encode of `views` images (0 for sizes gab200_png_encode refuses). */
+size_t gab200_png_scratch_bytes(int32_t views, int32_t height, int32_t width);
+/* Encode rgb [views, height, width, 3] uint8 (contiguous, device): file k at out + k * out_stride (out_stride >=
+ * gab200_png_bound), its length to out_len[k] (int64, device).  scratch: gab200_png_scratch_bytes bytes, 256-byte
+ * aligned.  Reads nothing on the host: capturable.  Refused before any device work: a null pointer, a size <= 0, a
+ * size whose bound overflows, a stride below the bound, a misaligned scratch. */
+int32_t gab200_png_encode(int32_t views, int32_t height, int32_t width, const uint8_t* rgb, void* scratch,
+                          uint8_t* out, int64_t out_stride, int64_t* out_len, void* stream);
+/* Copy `views` files of an encode: src_len[k] bytes (rounded up to 16) of src + k * src_stride to dst + k *
+ * dst_stride and the length to dst_len[k] -- or, when flag is not NULL and *flag != 0 (a replay that overflowed its
+ * instance capacity), or src_len[k] < 0, no bytes and dst_len[k] = -1.  dst / dst_len may be mapped pinned host
+ * memory, so only the compressed bytes cross the bus.  Strides and src / dst: multiples of 16, dst_stride >=
+ * src_stride. */
+int32_t gab200_png_copy(int32_t views, const uint8_t* src, int64_t src_stride, const int64_t* src_len,
+                        const int32_t* flag, uint8_t* dst, int64_t dst_stride, int64_t* dst_len, void* stream);
+
 /* A device-resident view schedule (csrc/schedule.cu, gaussianavatars_b200.schedule.ViewSchedule): `records` records
  * of `views` cameras each -- cams [records, views, GAB200_CAMERA_FLOATS] float32, timesteps [records] int32 (may be
  * NULL), frame_ids [records, views] int32 (may be NULL) -- visited in the order order[0 .. length).  `cursor` is one
