@@ -7,12 +7,13 @@
 //                       (H rows of 1 + 3W bytes).  It also zeroes the view's deflate buffer.
 //   png_lz_kernel       one 1024-thread CTA per segment: PNG_SEG bytes of the filtered stream (the last one shorter),
 //                       staged in shared memory with the PNG_WIN bytes before it (matches reach back into earlier
-//                       segments of the same view, never into another view).  Per position the longest match of four
-//                       candidates -- distance 1, 3 (the previous pixel), 3W + 1 (the previous row, when <= 32768) and
-//                       the latest earlier position of the same 3-byte hash (a table refreshed every 1024 positions) --
-//                       ties to the earlier candidate in that order.  The greedy parse (next = p + max(1, len)) is
-//                       walked by pointer doubling: 15 rounds mark every position the parse from the segment's first
-//                       byte reaches.  Then the segment's dynamic Huffman codes (literal/length limited to 15 bits,
+//                       segments of the same view, never into another view).  Per position the longest match of five
+//                       candidates -- distance 1, 3 (the previous pixel), the nearest position of the same 3-byte hash
+//                       up to 256 back in the position's round of 1024, 3W + 1 (the previous row, when <= 32768) and
+//                       the latest position of the same hash before the round (a table refreshed every 1024
+//                       positions) -- ties to the earlier candidate in that order.  The greedy parse (next = p +
+//                       max(1, len)) is walked by pointer doubling: 15 rounds mark every position the parse from the
+//                       segment's first byte reaches.  Then the segment's dynamic Huffman codes (literal/length limited to 15 bits,
 //                       code-length codes to 7, the RLE codes 16/17/18 in the header; deterministic: leaves ordered by
 //                       (count, symbol)), the exact bit cost of the dynamic and the fixed block, and the smaller of the
 //                       two (ties: fixed) rendered at bit 0 of the segment's staging area, unless even a stored block

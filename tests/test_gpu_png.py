@@ -3,7 +3,14 @@ evaluation replays (GraphedRender / GraphedEval png=True, host_png).
 
 Every file is checked four ways -- PIL opens it as RGB of the right size with the input's pixels; zlib inflates the
 IDAT data to its end with nothing left over (the Adler-32); every chunk's CRC-32 is zlib.crc32 of its type and data;
-the chunk order and the IHDR fields -- and every row's filter byte is oracle/png.py's choice."""
+the chunk order and the IHDR fields -- every row's filter byte is oracle/png.py's choice, and, for every image of at
+most ORACLE_BYTES filtered bytes, the file is oracle/png.py's encode_png byte for byte.
+
+CORPUS holds natural images (flat, gradient, noise, mixed rows) and images built to force the encoder's rare paths: a
+literal tree and a code-length tree past their length limits, an all-literal segment that still compresses, matches at
+exactly 32768 and into the previous segment, both block-choice ties, and IDAT chunks that end on and one byte past a
+64 KiB CRC piece or span more than 1024 of them.  tests/test_oracle_png.py shows from the oracle's path report, on the
+CPU, that the corpus reaches every one of them."""
 import io
 import struct
 import zlib
@@ -39,7 +46,20 @@ def _chunks(data: bytes) -> list:
     return out
 
 
+# The largest image (filtered bytes) whose file is compared with the oracle's byte for byte: the oracle takes 1-2 s per
+# MB of filtered stream on one CPU core (0.4 s for the 400x300 noise image, 2.8 s for an 802x550 display frame), so the
+# 1080p display frame (6.2 MB) and noise_4800 (69 MB) get the other checks only.
+ORACLE_BYTES = 1 << 21
+
+
 def check_file(data: bytes, img: np.ndarray):
+    """check_stream, and the file is the oracle's when the image is at most ORACLE_BYTES filtered bytes."""
+    check_stream(data, img)
+    if opng.filtered_bytes(img.shape[1], img.shape[0]) <= ORACLE_BYTES:
+        assert data == opng.encode_png(img), "the file is not the oracle's, byte for byte"
+
+
+def check_stream(data: bytes, img: np.ndarray):
     """The four checks, the filters against the oracle, and the bound."""
     from PIL import Image
     from gaussianavatars_b200 import png_bound
@@ -81,6 +101,65 @@ def _mixed(H, W, seed):
     return img
 
 
+def _from_sub(f) -> np.ndarray:
+    """A one-row image whose Sub-filtered bytes are f (3W of them): each channel is the running sum of its bytes.  The
+    filter rule picks Sub when f is small signed bytes; the images below assert that it does."""
+    f = np.asarray(f, np.int64)
+    return (f.reshape(-1, 3).cumsum(0) & 255).astype(np.uint8)[None]
+
+
+def _de_bruijn(k: int, n: int) -> np.ndarray:
+    """The lexicographically least de Bruijn sequence B(k, n): every n-symbol word once, read cyclically."""
+    a, seq = [0] * (k * n), []
+
+    def db(t, p):
+        if t > n:
+            if n % p == 0:
+                seq.extend(a[1:p + 1])
+        else:
+            a[t] = a[t - p]
+            db(t + 1, p)
+            for j in range(a[t - p] + 1, k):
+                a[t] = j
+                db(t + 1, t)
+    db(1, 1)
+    return np.array(seq, np.int64)
+
+
+def _de_bruijn_row(W: int) -> np.ndarray:
+    """A 1 x W image whose filtered stream is B(32, 3) over the small signed bytes -16..15, cycled: the filter byte (1,
+    Sub) and the row make the first 32768 bytes, in which no 3 bytes repeat -- a segment of 32768 literals that still
+    compresses (5-bit codes), whose parse needs all 15 doubling rounds -- and every later byte repeats the one 32768
+    before it: matches at exactly the window's distance, 258 long, into the previous segment."""
+    v = _de_bruijn(32, 3)
+    v = np.where(v < 16, v, v + 224)
+    v = np.roll(v, -int(np.argmax(v == 1)))           # starts with the filter byte
+    return _from_sub(np.resize(np.roll(v, -1), 3 * W))
+
+
+def _fibonacci_bytes(n: int, seed: int) -> np.ndarray:
+    """n filtered bytes: 160 small signed values drawn uniformly and 12 more with counts 1, 2, 3, 5, ..., 233.  With the
+    end-of-block symbol's count of one the rare twelve form one chain, 17 deep under the body's 8, past the 15-bit
+    limit."""
+    rng = np.random.default_rng(seed)
+    fib = [1, 2]
+    while len(fib) < 12:
+        fib.append(fib[-1] + fib[-2])
+    body, chain = np.arange(-80, 80) & 255, np.arange(80, 92)
+    return rng.permutation(np.concatenate([np.repeat(chain, fib), rng.choice(body, n - sum(fib))]))
+
+
+def _hex(h: int, w: int, data: str) -> np.ndarray:
+    return np.frombuffer(bytes.fromhex(data), np.uint8).reshape(h, w, 3).copy()
+
+
+def _flat_tail(W: int, T: int, seed: int) -> np.ndarray:
+    """A noise row whose last T pixels are flat."""
+    img = np.random.default_rng(seed).integers(0, 256, (1, W, 3), dtype=np.uint8)
+    img[:, W - T:] = 7
+    return img
+
+
 _rng = np.random.default_rng(1)
 CORPUS = {
     "white": np.full((48, 64, 3), 255, np.uint8),
@@ -96,6 +175,24 @@ CORPUS = {
     "segment_minus_1": _mixed(1, 10922, 4),     # 32767
     "segment_plus_2": _mixed(1, 10923, 5),      # 32770
     **{f"mixed_{h}x{w}": _mixed(h, w, h * w) for h, w in ((97, 401), (128, 512), (211, 173), (300, 333), (64, 1030))},
+    # built for the rare paths (tests/test_oracle_png.py names the path each one reaches)
+    "de_bruijn": _de_bruijn_row(21846),
+    "fibonacci": _from_sub(_fibonacci_bytes(3 * 10922, 0)),
+    # found by a seeded search over tiny images: the fixed and dynamic costs tie (304 bits), and fixed wins over
+    # stored (336); a Huffman block of exactly the stored block's 480 bits; one of 818 bits, 2 over stored, rendered
+    # and then dropped
+    "tie_fixed_dynamic": _hex(1, 12, "349d34f07cf004073407bd347cbdbd9d047c04f0079d7c07bd04bdd9bd9d9df07cf0047c"),
+    "tie_stored_huffman": _hex(1, 18, "dad195a4f5cd87d9e4ce8d7ebae99ba4eeffda9cf3d2e1f67aa0cfe8d38a81e49cbf8cfdbafd8d"
+                                      "c3a9db7c94f1d4f4d1b3f0b5af88be"),
+    "stored_over_huffman": _hex(1, 32, "c426e5487322659f79b0a96af63a36f8ba697baa942ba38e4d91ffb0a7fc23effb4afe82d954bd"
+                                       "3421cb1ed55341c753943d2a214848b14ec89cf0b6f32bb34193f176181c82d516b3a853535fef"
+                                       "4fb5c761d83c302fab815a34fca77046c63e"),
+    # IDAT type + data: 65536 bytes (2 stored blocks: n + 5 S + 6 = 65532 data bytes) and 65537 bytes, one byte into
+    # a second png_assemble_kernel piece
+    "idat_65536": np.random.default_rng(3).integers(0, 256, (2, 10919, 3), dtype=np.uint8),
+    "idat_65537": _flat_tail(21845, 20, 3),
+    # 69 MB of stored blocks: 1055 pieces, so each png_finish_kernel thread combines a run of two
+    "noise_4800": np.random.default_rng(4).integers(0, 256, (4800, 4800, 3), dtype=np.uint8),
 }
 
 
@@ -105,6 +202,9 @@ def test_round_trip_filters_bound_and_determinism(name):
     data = _encode(img)
     check_file(data, img)
     assert _encode(img) == data, "two encodes of the same input differ"
+    if name == "noise_4800":   # png_finish_kernel's threads each combine a run of pieces
+        idat, = struct.unpack(">I", data[33:37])
+        assert -(-(4 + idat) // opng.PIECE) > 1024
 
 
 def test_noise_takes_stored_blocks():
@@ -122,6 +222,26 @@ def test_a_batch_of_16_different_images():
     files = encode_png(torch.from_numpy(imgs).to(DEV))
     assert isinstance(files, list) and len(files) == 16
     for k in range(16):
+        check_file(files[k], imgs[k])
+        assert files[k] == _encode(imgs[k]), f"view {k} of the batch differs from its own encode"
+
+
+def test_a_batch_whose_views_take_different_paths():
+    """One launch of four views of one shape, each its own mix of block kinds and segment paths: the de Bruijn row
+    (32768 literals, then matches at 32768), Fibonacci bytes (the literal tree past 15 bits), noise (stored) and a flat
+    image.  Each view's file is its own encode's and the oracle's."""
+    from gaussianavatars_b200 import encode_png
+    W = 21846
+    fib = _from_sub(np.concatenate([_fibonacci_bytes(3 * 10922, 0), _fibonacci_bytes(3 * W - 3 * 10922, 1)]))
+    imgs = np.stack([_de_bruijn_row(W), fib, np.random.default_rng(5).integers(0, 256, (1, W, 3), np.uint8),
+                     np.full((1, W, 3), 200, np.uint8)])
+    # per segment: block kind, literal tree past its limit, all literals, farthest match
+    paths = [tuple((r.kind, r.lit_depth[0] > 15, r.literals == r.symbols, r.farthest) for r in rep)
+             for rep in (opng.encode_png(img, report=True)[1] for img in imgs)]
+    assert len(set(paths)) == 4 and [p[0][0] for p in paths] == ["dynamic", "dynamic", "stored", "dynamic"], paths
+    assert paths[0][0][2] and paths[0][1][3] == 32768 and paths[1][0][1]
+    files = encode_png(torch.from_numpy(imgs).to(DEV))
+    for k in range(4):
         check_file(files[k], imgs[k])
         assert files[k] == _encode(imgs[k]), f"view {k} of the batch differs from its own encode"
 
