@@ -235,7 +235,8 @@ EXPORTED_SYMBOLS = ("gab200_forward", "gab200_backward", "gab200_mark_visible", 
                     "gab200_schedule_sample", "gab200_schedule_commit", "gab200_lpips_weights_bytes",
                     "gab200_lpips_pack", "gab200_lpips_scratch_bytes", "gab200_lpips_features_bytes",
                     "gab200_lpips", "gab200_png_bound", "gab200_png_scratch_bytes", "gab200_png_encode",
-                    "gab200_png_copy")
+                    "gab200_png_copy", "gab200_png_status_string", "gab200_png_decode_scratch_bytes",
+                    "gab200_png_decode")
 
 _lib = None
 _lock = threading.Lock()
@@ -352,6 +353,13 @@ def lib():
         L.gab200_png_copy.restype = C.c_int32
         L.gab200_png_copy.argtypes = [C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_int64, C.c_void_p, C.c_void_p]
+        L.gab200_png_status_string.restype = C.c_char_p
+        L.gab200_png_status_string.argtypes = [C.c_int32]
+        L.gab200_png_decode_scratch_bytes.restype = C.c_size_t
+        L.gab200_png_decode_scratch_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
+        L.gab200_png_decode.restype = C.c_int32
+        L.gab200_png_decode.argtypes = [C.c_int32, C.c_int32, C.c_int32] + [C.c_void_p] * 6 + [C.c_int32, C.c_void_p,
+                                                                                              C.c_void_p]
         L.gab200_schedule_sample.restype = C.c_int32
         L.gab200_schedule_sample.argtypes = [C.c_int32, C.c_int32, C.c_int32] + [C.c_void_p] * 11
         L.gab200_schedule_commit.restype = C.c_int32

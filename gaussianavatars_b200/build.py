@@ -35,6 +35,7 @@ SOURCES = {
     "composite.cu": [],
     "frames.cu": [],
     "png.cu": [],
+    "png_decode.cu": [],
     "schedule.cu": [],
     "metrics.cu": [],
     "lpips.cu": [],

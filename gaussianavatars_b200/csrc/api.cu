@@ -1018,6 +1018,41 @@ int32_t gab200_png_copy(int32_t views, const uint8_t* src, int64_t src_stride, c
   return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
 }
 
+const char* gab200_png_status_string(int32_t s) {
+  switch (s) {
+    case GAB200_PNG_OK: return "ok";
+    case GAB200_PNG_ZLIB_HEADER: return "invalid zlib header";
+    case GAB200_PNG_BLOCK_TYPE: return "invalid deflate block type";
+    case GAB200_PNG_STORED_LENGTH: return "invalid stored block length";
+    case GAB200_PNG_CODE_LENGTHS: return "invalid Huffman code lengths";
+    case GAB200_PNG_SYMBOL: return "invalid Huffman code";
+    case GAB200_PNG_DISTANCE: return "distance too far back";
+    case GAB200_PNG_TRUNCATED: return "truncated image data";
+    case GAB200_PNG_TOO_MUCH: return "image data inflates past the image";
+    case GAB200_PNG_TOO_LITTLE: return "image data inflates short of the image";
+    case GAB200_PNG_ADLER: return "Adler-32 mismatch";
+    case GAB200_PNG_FILTER: return "invalid row filter type";
+    default: return "unknown PNG status";
+  }
+}
+
+size_t gab200_png_decode_scratch_bytes(int32_t files, int32_t height, int32_t width) {
+  return png_decode_scratch_bytes(files, height, width);
+}
+
+int32_t gab200_png_decode(int32_t files, int32_t height, int32_t width, const uint8_t* zdata, const int64_t* zoff,
+                          const int64_t* zlen, const uint8_t* color_type, void* scratch, uint8_t* out,
+                          int32_t out_channels, int32_t* status, void* stream_) {
+  if (files <= 0 || png_decode_stride(height, width) < 0 || (out_channels != 3 && out_channels != 4))
+    return GAB200_ERR_INVALID_ARGUMENT;
+  if (!zdata || !zoff || !zlen || !color_type || !scratch || !out || !status) return GAB200_ERR_INVALID_ARGUMENT;
+  if (((uintptr_t)scratch & 255) != 0 || ((uintptr_t)out & 3) != 0) return GAB200_ERR_INVALID_ARGUMENT;
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  launch_png_decode(files, height, width, zdata, zoff, zlen, color_type, scratch, out, out_channels, status,
+                    (cudaStream_t)stream_);
+  return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
 int32_t gab200_schedule_sample(int32_t records, int32_t views, int32_t length, const float* cams,
                                const int32_t* timesteps, const int32_t* frame_ids, const int32_t* order,
                                const int32_t* cursor, float* cam_out, int32_t* timestep_out, int32_t* ids_out,

@@ -244,6 +244,13 @@ void launch_png_encode(int views, int H, int W, const uint8_t* rgb, void* scratc
 void launch_png_copy(int views, const uint8_t* src, int64_t src_stride, const int64_t* src_len, const int32_t* flag,
                      uint8_t* dst, int64_t dst_stride, int64_t* dst_len, cudaStream_t stream);
 
+// png_decode.cu
+int64_t png_decode_stride(int H, int W);
+size_t png_decode_scratch_bytes(int64_t files, int H, int W);
+void launch_png_decode(int files, int H, int W, const uint8_t* zdata, const int64_t* zoff, const int64_t* zlen,
+                       const uint8_t* color, void* scratch, uint8_t* out, int out_channels, int32_t* status,
+                       cudaStream_t stream);
+
 // schedule.cu
 void launch_schedule_sample(int records, int views, int length, const float* cams, const int32_t* timesteps,
                             const int32_t* frame_ids, const int32_t* order, const int32_t* cursor, float* cam_out,

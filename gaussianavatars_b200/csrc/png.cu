@@ -33,6 +33,7 @@
 // No file exceeds gab200_png_bound(W, H) = 63 + n + 6 S (n = H (3W + 1) filtered bytes, S = ceil(n / PNG_SEG)): every
 // block is at most its stored form, 42 bits of header and padding plus its bytes.
 #include "common.cuh"
+#include "deflate.cuh"
 #include "kernels.cuh"
 
 namespace gab {
@@ -114,22 +115,6 @@ __host__ __device__ inline Layout carve(void* scratch, int64_t views, int H, int
 }
 
 // ---- checksums ----------------------------------------------------------------------------------------------------
-constexpr uint32_t ADLER_BASE = 65521;
-
-// zlib's adler32_combine: the Adler-32 of A || B from those of A and B and B's length
-__device__ __forceinline__ uint32_t adler_combine(uint32_t a1, uint32_t a2, uint32_t len2) {
-  const uint32_t rem = len2 % ADLER_BASE;
-  uint32_t sum1 = a1 & 0xffff;
-  uint32_t sum2 = (uint32_t)(((uint64_t)rem * sum1) % ADLER_BASE);
-  sum1 += (a2 & 0xffff) + ADLER_BASE - 1;
-  sum2 += ((a1 >> 16) & 0xffff) + ((a2 >> 16) & 0xffff) + ADLER_BASE - rem;
-  if (sum1 >= ADLER_BASE) sum1 -= ADLER_BASE;
-  if (sum1 >= ADLER_BASE) sum1 -= ADLER_BASE;
-  if (sum2 >= (ADLER_BASE << 1)) sum2 -= (ADLER_BASE << 1);
-  if (sum2 >= ADLER_BASE) sum2 -= ADLER_BASE;
-  return sum1 | (sum2 << 16);
-}
-
 constexpr uint32_t CRC_POLY = 0xedb88320u;
 
 // a * b modulo the CRC-32 polynomial (reflected), as zlib's multmodp
@@ -335,8 +320,6 @@ __device__ __forceinline__ void put_bits(uint32_t* w, uint32_t off, uint64_t v, 
   if (s + nbits > 32) atomicOr(w + i + 1, (uint32_t)(lo >> 32));
   if (s + nbits > 64) atomicOr(w + i + 2, (uint32_t)(v >> (64 - s)));
 }
-
-__constant__ uint8_t CL_ORDER[CL_SYMS] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
 
 // The Huffman tables of one segment (shared memory, in the hash table's space once the matches are found)
 struct HuffSmem {

@@ -2,6 +2,7 @@
 
     store = FrameStore(width, height, bg, device)
     ids = store.add_rgba(rgba_u8)               # decoded capture frames (K,H,W,4): composite + encode, once
+    ids = store.add_png(paths)                  # or the capture's PNG files, decoded on the device
     gt, mask = store.decode(ids)                # eager: the bytes composite_rgba made, bit for bit
     frame = GraphedFrame(pc, width, height, fovx, fovy, bg, frames=store)
     frame.set_inputs(cameras=..., timestep=t, frames=ids)   # K ints: the replay decodes them on the device
@@ -25,10 +26,12 @@ from typing import Optional
 import torch
 
 from . import _native as N
+from .png import decode_png
 from .training import composite_rgba
 
 TILE = 16
 RECORD_MAX = 8 + 32 * 8 * 4   # bytes of one tile's record at width 8 in every plane
+PNG_BATCH = 256               # files per decode in add_png (the fastest of 16, 64, 256: profiles/h100/png_decode.jsonl)
 
 
 def _tiles(height: int, width: int) -> int:
@@ -134,6 +137,23 @@ class FrameStore:
             rgba_u8 = rgba_u8.to(self.device)
         gt, mask = composite_rgba(rgba_u8, self.bg)
         return self.add(gt, mask)
+
+    def add_png(self, files, batch: int = PNG_BATCH) -> list:
+        """The capture's PNG frames (paths or bytes; RGB or RGBA, the store's size) decoded on the device
+        (png.decode_png) `batch` files at a time, each batch then add_rgba'd; returns the new frames' ids.  The stored
+        frames are those of PIL's convert("RGBA") + add_rgba byte for byte.  `batch` bounds the decode's device memory:
+        about 2 H (4W + 1) bytes per file."""
+        if isinstance(batch, bool) or not isinstance(batch, int) or batch < 1:
+            raise ValueError(f"batch must be a positive int, got {batch!r}")
+        files = list(files)
+        ids = []
+        for i in range(0, len(files), batch):
+            rgba = decode_png(files[i:i + batch], 4, self.device)
+            if tuple(rgba.shape[1:3]) != (self.H, self.W):
+                raise ValueError(f"files {i}..{i + len(rgba) - 1} are {rgba.shape[2]}x{rgba.shape[1]}, the store holds "
+                                 f"{self.W}x{self.H} frames")
+            ids += self.add_rgba(rgba)
+        return ids
 
     # ---- reading frames --------------------------------------------------------------------------------------------
     def check_ids(self, ids) -> list:

@@ -474,6 +474,42 @@ int32_t gab200_png_encode(int32_t views, int32_t height, int32_t width, const ui
 int32_t gab200_png_copy(int32_t views, const uint8_t* src, int64_t src_stride, const int64_t* src_len,
                         const int32_t* flag, uint8_t* dst, int64_t dst_stride, int64_t* dst_len, void* stream);
 
+/* PNG files read on the device (csrc/png_decode.cu, gaussianavatars_b200.png.decode_png): the IDAT data of `files`
+ * files of one size, 8-bit RGB (colour type 2) or RGBA (6), not interlaced.  Each file's data is a zlib stream of any
+ * deflate blocks and window size that stock zlib accepts; it must inflate to exactly height (1 + width c) bytes (c = 3
+ * or 4), each row one filter byte (0..4) and its filtered pixels, and end with their Adler-32.  Nothing after the
+ * Adler-32 is read.  One warp per file inflates it into the scratch, then the row filters are undone as a wavefront
+ * of 32 rows.  The per-file status is the first error in stream order: */
+enum gab200_png_status {
+  GAB200_PNG_OK = 0,
+  GAB200_PNG_ZLIB_HEADER = 1,    /* CM != 8, CINFO > 7, FCHECK fails or FDICT set                             */
+  GAB200_PNG_BLOCK_TYPE = 2,     /* BTYPE 3                                                                    */
+  GAB200_PNG_STORED_LENGTH = 3,  /* a stored block's LEN != ~NLEN                                              */
+  GAB200_PNG_CODE_LENGTHS = 4,   /* HLIT > 286, HDIST > 30, a bad code-length code, repeat or code, no code 256 */
+  GAB200_PNG_SYMBOL = 5,         /* an unused code, literal/length 286 / 287, distance 30 / 31                  */
+  GAB200_PNG_DISTANCE = 6,       /* a distance before the first byte                                           */
+  GAB200_PNG_TRUNCATED = 7,      /* the data ends inside the stream or its Adler-32                            */
+  GAB200_PNG_TOO_MUCH = 8,       /* the stream inflates to more than height (1 + width c) bytes                */
+  GAB200_PNG_TOO_LITTLE = 9,     /* ... or to fewer                                                            */
+  GAB200_PNG_ADLER = 10,         /* the Adler-32 does not match                                                */
+  GAB200_PNG_FILTER = 11         /* a row's filter byte > 4 (reported only for an otherwise valid stream)      */
+};
+/* A short description of a gab200_png_status value ("unknown PNG status" for any other value). */
+const char* gab200_png_status_string(int32_t status);
+/* Scratch bytes of a decode of `files` files (0 for sizes gab200_png_decode refuses). */
+size_t gab200_png_decode_scratch_bytes(int32_t files, int32_t height, int32_t width);
+/* Decode: file f's stream is zdata[zoff[f] .. zoff[f] + zlen[f]) (zoff, zlen: int64, device; each range inside the
+ * zdata allocation; a negative zlen reads as 0), its colour type color_type[f] (uint8, device: 6 is RGBA, any other
+ * value decodes as 2, RGB).  Writes status[f] (int32, device) and, for a file whose status is GAB200_PNG_OK, out[f]
+ * [height, width, out_channels] uint8 (RGB files get alpha 255; out_channels 3 drops alpha); the image of a failed
+ * file is undefined.  A file never reads or writes another file's data.  scratch: gab200_png_decode_scratch_bytes
+ * bytes, 256-byte aligned; out: 4-byte aligned.  Reads nothing on the host.  Refused before any device work: files,
+ * height or width <= 0, height (1 + 4 width) > 2^31 - 1, out_channels other than 3 or 4, a null pointer, a
+ * misaligned scratch or out. */
+int32_t gab200_png_decode(int32_t files, int32_t height, int32_t width, const uint8_t* zdata, const int64_t* zoff,
+                          const int64_t* zlen, const uint8_t* color_type, void* scratch, uint8_t* out,
+                          int32_t out_channels, int32_t* status, void* stream);
+
 /* A device-resident view schedule (csrc/schedule.cu, gaussianavatars_b200.schedule.ViewSchedule): `records` records
  * of `views` cameras each -- cams [records, views, GAB200_CAMERA_FLOATS] float32, timesteps [records] int32 (may be
  * NULL), frame_ids [records, views] int32 (may be NULL) -- visited in the order order[0 .. length).  `cursor` is one
