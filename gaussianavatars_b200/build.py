@@ -36,6 +36,7 @@ SOURCES = {
     "frames.cu": [],
     "png.cu": [],
     "png_decode.cu": [],
+    "resize.cu": [],
     "schedule.cu": [],
     "metrics.cu": [],
     "lpips.cu": [],

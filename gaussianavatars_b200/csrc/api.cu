@@ -1053,6 +1053,20 @@ int32_t gab200_png_decode(int32_t files, int32_t height, int32_t width, const ui
   return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
 }
 
+size_t gab200_resize_scratch_bytes(int64_t planes, int32_t in_height, int32_t in_width, int32_t out_height,
+                                   int32_t out_width) {
+  return resize_scratch_bytes(planes, in_height, in_width, out_height, out_width);
+}
+
+int32_t gab200_resize_u8(int64_t planes, int32_t in_height, int32_t in_width, int32_t out_height, int32_t out_width,
+                         const uint8_t* src, uint8_t* dst, void* scratch, void* stream_) {
+  if (resize_scratch_bytes(planes, in_height, in_width, out_height, out_width) == 0) return GAB200_ERR_INVALID_ARGUMENT;
+  if (!src || !dst || !scratch || ((uintptr_t)scratch & 255) != 0) return GAB200_ERR_INVALID_ARGUMENT;
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  launch_resize_u8(planes, in_height, in_width, out_height, out_width, src, dst, scratch, (cudaStream_t)stream_);
+  return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
 int32_t gab200_schedule_sample(int32_t records, int32_t views, int32_t length, const float* cams,
                                const int32_t* timesteps, const int32_t* frame_ids, const int32_t* order,
                                const int32_t* cursor, float* cam_out, int32_t* timestep_out, int32_t* ids_out,

@@ -251,6 +251,11 @@ void launch_png_decode(int files, int H, int W, const uint8_t* zdata, const int6
                        const uint8_t* color, void* scratch, uint8_t* out, int out_channels, int32_t* status,
                        cudaStream_t stream);
 
+// resize.cu
+size_t resize_scratch_bytes(int64_t planes, int in_h, int in_w, int out_h, int out_w);
+void launch_resize_u8(int64_t planes, int in_h, int in_w, int out_h, int out_w, const uint8_t* src, uint8_t* dst,
+                      void* scratch, cudaStream_t stream);
+
 // schedule.cu
 void launch_schedule_sample(int records, int views, int length, const float* cams, const int32_t* timesteps,
                             const int32_t* frame_ids, const int32_t* order, const int32_t* cursor, float* cam_out,

@@ -3,6 +3,7 @@
     store = FrameStore(width, height, bg, device)
     ids = store.add_rgba(rgba_u8)               # decoded capture frames (K,H,W,4): composite + encode, once
     ids = store.add_png(paths)                  # or the capture's PNG files, decoded on the device
+    ids = store.add_png(paths, resize=True)     # ... of another size: composited, then resized as the loader does
     gt, mask = store.decode(ids)                # eager: the bytes composite_rgba made, bit for bit
     frame = GraphedFrame(pc, width, height, fovx, fovy, bg, frames=store)
     frame.set_inputs(cameras=..., timestep=t, frames=ids)   # K ints: the replay decodes them on the device
@@ -130,29 +131,35 @@ class FrameStore:
         self._used += total
         return ids
 
-    def add_rgba(self, rgba_u8: torch.Tensor) -> list:
+    def add_rgba(self, rgba_u8: torch.Tensor, resize: bool = False) -> list:
         """Decoded capture frames ((H,W,4) or (F,H,W,4) uint8) -> training.composite_rgba onto the store's background,
-        then add(gt, mask).  A CPU batch is uploaded first."""
+        then add(gt, mask).  A CPU batch is uploaded first.  resize: frames of another size are composited at their
+        own size, then resized to the store's (composite_rgba(size=): the reference loader's bicubic resize, and the
+        alpha bytes resized as an "L" image); without it they must have the store's size."""
         if isinstance(rgba_u8, torch.Tensor) and rgba_u8.device.type == "cpu":
             rgba_u8 = rgba_u8.to(self.device)
-        gt, mask = composite_rgba(rgba_u8, self.bg)
+        gt, mask = composite_rgba(rgba_u8, self.bg, size=(self.W, self.H) if resize else None)
         return self.add(gt, mask)
 
-    def add_png(self, files, batch: int = PNG_BATCH) -> list:
+    def add_png(self, files, batch: int = PNG_BATCH, resize: bool = False) -> list:
         """The capture's PNG frames (paths or bytes; RGB or RGBA, the store's size) decoded on the device
         (png.decode_png) `batch` files at a time, each batch then add_rgba'd; returns the new frames' ids.  The stored
         frames are those of PIL's convert("RGBA") + add_rgba byte for byte.  `batch` bounds the decode's device memory:
-        about 2 H (4W + 1) bytes per file."""
+        about 2 H (4W + 1) bytes per file.
+
+        resize: the files may have another size than the store's (one size per batch): each batch is decoded,
+        composited at its own size and resized to the store's -- what the reference's loader makes of a capture
+        larger than its camera (resize.loader_size), byte for byte.  Without it a file of another size raises."""
         if isinstance(batch, bool) or not isinstance(batch, int) or batch < 1:
             raise ValueError(f"batch must be a positive int, got {batch!r}")
         files = list(files)
         ids = []
         for i in range(0, len(files), batch):
             rgba = decode_png(files[i:i + batch], 4, self.device)
-            if tuple(rgba.shape[1:3]) != (self.H, self.W):
+            if not resize and tuple(rgba.shape[1:3]) != (self.H, self.W):
                 raise ValueError(f"files {i}..{i + len(rgba) - 1} are {rgba.shape[2]}x{rgba.shape[1]}, the store holds "
-                                 f"{self.W}x{self.H} frames")
-            ids += self.add_rgba(rgba)
+                                 f"{self.W}x{self.H} frames (resize=True resizes them)")
+            ids += self.add_rgba(rgba, resize)
         return ids
 
     # ---- reading frames --------------------------------------------------------------------------------------------

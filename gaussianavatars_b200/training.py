@@ -3,8 +3,9 @@ CUDA launches behind the same C ABI:
 
   photometric_loss(image, gt, lambda_dssim)   <- l1_loss * (1 - lambda) + (1 - ssim) * lambda
                                                  (utils/loss_utils.py:17-18,36-63, train.py:131-132)
-  composite_rgba(rgba_u8, bg)                 <- the loader's RGBA composite onto the background, and the alpha
-                                                 mask it drops (scene/__init__.py:48-51)
+  composite_rgba(rgba_u8, bg, size=None)      <- the loader's RGBA composite onto the background, and the alpha
+                                                 mask it drops (scene/__init__.py:48-51); with `size`, then its
+                                                 resize to the camera's size (PILtoTorch, resize.py)
   image_metrics(render, gt_u8)                <- clamp + l1_loss, psnr, ssim of one val / test view (train.py:277-288)
                                                  and metrics.py:71-74 (evaluation, forward only)
   Adam(param_groups, lr, betas, eps)          <- torch.optim.Adam(l, lr=0.0, eps=1e-15).step()
@@ -23,6 +24,7 @@ from typing import Optional
 import torch
 
 from . import _native as N
+from .resize import check_size, resize_u8
 
 
 # ================================================================================================================
@@ -116,7 +118,7 @@ def launch_composite_rgba(rgba_u8: torch.Tensor, bg: torch.Tensor, gt_out: torch
 
 
 @torch.no_grad()
-def composite_rgba(rgba_u8: torch.Tensor, bg) -> tuple:
+def composite_rgba(rgba_u8: torch.Tensor, bg, size=None) -> tuple:
     """(gt_u8, mask_u8) of decoded RGBA capture frames, computed on the device: what the reference's loader
     (CameraDataset.__getitem__, scene/__init__.py:48-51) makes of `np.array(Image.open(p).convert("RGBA"))` on the
     host, bit for bit, plus the alpha channel it throws away.
@@ -124,7 +126,18 @@ def composite_rgba(rgba_u8: torch.Tensor, bg) -> tuple:
     rgba_u8: a CUDA uint8 (H, W, 4) frame or (K, H, W, 4) frames.  bg: the camera's background (3 values, 0 or 1 per
     channel in the reference; other colours go through the same formula).  Returns the uint8 ground truth (3, H, W) /
     (K, 3, H, W) -- trunc((c/255 * a/255 + bg * (1 - a/255)) * 255) in float64, the loader's bytes -- and the alpha
-    bytes (1, H, W) / (K, 1, H, W), the foreground mask (value/255) of a mask loss."""
+    bytes (1, H, W) / (K, 1, H, W), the foreground mask (value/255) of a mask loss.
+
+    size (width, height): the frames are composited at their own size, then resized to it as the loader's PILtoTorch
+    resizes them (resize.resize_u8: PIL's bicubic resize of the "RGB" image, bit for bit) -- the ground truth of a
+    camera whose size differs from its files' (resize.loader_size).  The mask is resized as PIL resizes an "L" image
+    of the alpha bytes; the reference drops alpha, so that resized mask is this project's definition.  Capturable."""
+    if size is not None:
+        width, height = check_size(size)
+        gt, mask = composite_rgba(rgba_u8, bg)
+        if (width, height) == (int(gt.shape[-1]), int(gt.shape[-2])):
+            return gt, mask   # PIL's resize to the image's own size is a copy
+        return resize_u8(gt, width, height), resize_u8(mask, width, height)
     views = check_rgba(rgba_u8)
     device = rgba_u8.device
     H, W = int(rgba_u8.shape[-3]), int(rgba_u8.shape[-2])

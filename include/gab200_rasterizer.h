@@ -510,6 +510,27 @@ int32_t gab200_png_decode(int32_t files, int32_t height, int32_t width, const ui
                           const int64_t* zlen, const uint8_t* color_type, void* scratch, uint8_t* out,
                           int32_t out_channels, int32_t* status, void* stream);
 
+/* Pillow's bicubic resize of 8-bit planes (csrc/resize.cu, gaussianavatars_b200.resize.resize_u8): what
+ * `Image.resize((out_width, out_height))` makes of an "L" image, or of each channel of an "RGB" one, bit for bit --
+ * the reference loader's resize of a composited frame to its camera's size (PILtoTorch, utils/general_utils.py:22).
+ * Per axis, output index i reads inputs first .. first + taps - 1 with scale = in / out, filterscale = max(scale, 1),
+ * center = (i + 0.5) scale, first = max(int(center - 2 filterscale + 0.5), 0), first + taps = min(int(center +
+ * 2 filterscale + 0.5), in), weighted by the Keys cubic (a = -0.5) at (j + first - center + 0.5) / filterscale,
+ * normalised by the weights' double sum and rounded half away from zero to 22 fractional bits; each output byte is
+ * clamp((2^21 + sum of pixel * weight) >> 22, 0, 255) in int32.  The width is resampled first into a uint8
+ * intermediate, then the height; an axis whose size does not change is not resampled (oracle/resize.py restates it).
+ *
+ * Scratch bytes of a resize of `planes` planes (0 for sizes gab200_resize_u8 refuses). */
+size_t gab200_resize_scratch_bytes(int64_t planes, int32_t in_height, int32_t in_width, int32_t out_height,
+                                   int32_t out_width);
+/* Resize src [planes, in_height, in_width] uint8 (contiguous, device; e.g. F frames x 3 colour planes) -> dst [planes,
+ * out_height, out_width].  scratch: gab200_resize_scratch_bytes bytes, 256-byte aligned.  The weights are made on the
+ * device from the sizes: nothing is read on the host or allocated, so the call is capturable.  Refused before any
+ * device work: a size or plane count <= 0, planes * in_height or planes * out_height > 2^31 - 1, a null pointer, a
+ * misaligned scratch. */
+int32_t gab200_resize_u8(int64_t planes, int32_t in_height, int32_t in_width, int32_t out_height, int32_t out_width,
+                         const uint8_t* src, uint8_t* dst, void* scratch, void* stream);
+
 /* A device-resident view schedule (csrc/schedule.cu, gaussianavatars_b200.schedule.ViewSchedule): `records` records
  * of `views` cameras each -- cams [records, views, GAB200_CAMERA_FLOATS] float32, timesteps [records] int32 (may be
  * NULL), frame_ids [records, views] int32 (may be NULL) -- visited in the order order[0 .. length).  `cursor` is one
