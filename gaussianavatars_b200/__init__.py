@@ -17,6 +17,7 @@ from .mesh import mesh_overlay, MeshRenderer
 from .lpips import LpipsNet, lpips, launch_lpips, lpips_features
 from .png import decode_png, encode_png, png_bound
 from .resize import loader_size, resize_u8
+from .video import VideoWriter, encode_video
 
 __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gaussians", "rasterize_bound",
            "bind_activate", "set_exact_binning", "face_frame", "l1_loss_u8", "render", "render_bound", "render_display", "render_views",
@@ -25,4 +26,4 @@ __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gau
            "add_densification_stats", "expon_lr_schedule", "FlameLBS", "flame_pose", "flame_param_groups",
            "mesh_overlay", "MeshRenderer", "composite_rgba", "FrameStore",
            "ViewSchedule", "epoch_order", "LpipsNet", "lpips", "launch_lpips", "lpips_features",
-           "decode_png", "encode_png", "png_bound", "loader_size", "resize_u8"]
+           "decode_png", "encode_png", "png_bound", "loader_size", "resize_u8", "VideoWriter", "encode_video"]

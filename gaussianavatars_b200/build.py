@@ -37,6 +37,7 @@ SOURCES = {
     "png.cu": [],
     "png_decode.cu": [],
     "resize.cu": [],
+    "h264.cu": [],
     "schedule.cu": [],
     "metrics.cu": [],
     "lpips.cu": [],

@@ -1053,6 +1053,27 @@ int32_t gab200_png_decode(int32_t files, int32_t height, int32_t width, const ui
   return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
 }
 
+int64_t gab200_h264_bound(int32_t width, int32_t height) { return h264_bound(width, height); }
+
+size_t gab200_h264_scratch_bytes(int32_t frames, int32_t height, int32_t width) {
+  return h264_scratch_bytes(frames, height, width);
+}
+
+int32_t gab200_h264_encode(int32_t frames, int32_t height, int32_t width, int32_t qp, const uint8_t* rgb, void* scratch,
+                           uint8_t* out, int64_t out_stride, int64_t* out_len, void* stream_) {
+  if (h264_scratch_bytes(frames, height, width) == 0 || qp < 0 || qp > 51) return GAB200_ERR_INVALID_ARGUMENT;
+  if (out_stride < h264_bound(width, height)) return GAB200_ERR_INVALID_ARGUMENT;
+  if (!rgb || !scratch || !out || !out_len || ((uintptr_t)scratch & 255) != 0) return GAB200_ERR_INVALID_ARGUMENT;
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  launch_h264_encode(frames, height, width, qp, rgb, scratch, out, out_stride, out_len, (cudaStream_t)stream_);
+  return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
+int32_t gab200_h264_parameter_sets(int32_t width, int32_t height, int32_t qp, int32_t fps_num, int32_t fps_den,
+                                   uint8_t* out, int64_t cap) {
+  return h264_parameter_sets(width, height, qp, fps_num, fps_den, out, cap);
+}
+
 size_t gab200_resize_scratch_bytes(int64_t planes, int32_t in_height, int32_t in_width, int32_t out_height,
                                    int32_t out_width) {
   return resize_scratch_bytes(planes, in_height, in_width, out_height, out_width);

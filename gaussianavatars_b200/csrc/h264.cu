@@ -1,0 +1,978 @@
+// h264.cu -- H.264 video frames encoded on the device (gab200_h264_bound / gab200_h264_scratch_bytes /
+// gab200_h264_encode / gab200_h264_parameter_sets): Constrained Baseline, every picture one IDR slice, CAVLC,
+// deblocking off, one fixed QP; each macroblock I_16x16 (luma and chroma modes of least SATD) or I_PCM.
+// oracle/h264.py restates every step, and the tests compare its bytes with these.
+//
+// Per batch of frames the encode runs these kernels, each named for a trace:
+//   h264_convert_kernel  RGB -> BT.601 limited-range Y, Cb, Cr planes padded to whole macroblocks by edge replication.
+//   h264_mb_kernel       one launch per anti-diagonal d = mbx + mby (W/16 + H/16 - 1 launches), one 128-thread CTA per
+//                        (macroblock on d, frame): prediction from the reconstructed left / top / top-left samples of
+//                        earlier diagonals, mode decision by SATD, transform, quantisation, reconstruction into the
+//                        recon planes, per-4x4 TotalCoeff, the macroblock's CAVLC bit count and the I_PCM fallback;
+//                        the levels are kept for the writer.  The per-diagonal launch is the wavefront's only
+//                        synchronisation: no CTA ever waits on another.
+//   h264_scan_kernel     one CTA per frame: the macroblocks' bit offsets in raster order, an exclusive scan of the maps
+//                        x -> x + L (I_16x16) and x -> ceil8(x + 9) + 3072 (I_PCM, whose samples start byte-aligned),
+//                        a family closed under composition; zeroes the slice's words and writes the slice header and
+//                        the stop bit.
+//   h264_write_kernel    one warp per macroblock: its bits at its offset, one lane per residual block, OR-ed into the
+//                        slice's words with atomics (neighbours share the first and last word).
+//   h264_ep_count_kernel one thread per 256-byte piece of the slice: for each zero-run state the piece can start in
+//                        (0, 1, >= 2 zero bytes), the state it ends in and the emulation-prevention bytes it inserts.
+//   h264_ep_plan_kernel  one warp per frame: the pieces' start states and output offsets in order, the sample's length
+//                        and its 4-byte length prefix and NAL header.
+//   h264_ep_emit_kernel  one thread per piece: its bytes, with 0x03 inserted, into the frame's output slot.
+#include <algorithm>
+#include <vector>
+
+#include "common.cuh"
+#include "kernels.cuh"
+
+namespace gab {
+
+namespace {
+
+constexpr int PCM_BITS = 9 + 384 * 8;        // ue(25) + the samples, before pcm_alignment_zero_bits
+constexpr int MAX_LEVEL = 2063;              // what level_prefix <= 15 codes at every suffixLength
+constexpr int HEADER_BITS = 22;              // the slice header (idr_pic_id 1)
+constexpr int EP_PIECE = 256;                // bytes of the slice per emulation-prevention piece
+constexpr int MAX_MBS = 36864;               // level 5.2's MaxFS
+constexpr int BLOCKS = 27;                   // residual blocks of a macroblock, in bitstream order (see h264_mb_kernel)
+
+__constant__ int8_t c_zigzag[16] = {0, 1, 4, 8, 5, 2, 3, 6, 9, 12, 13, 10, 7, 11, 14, 15};
+__constant__ int8_t c_chroma_qp[52] = {0,  1,  2,  3,  4,  5,  6,  7,  8,  9,  10, 11, 12, 13, 14, 15, 16, 17,
+                                       18, 19, 20, 21, 22, 23, 24, 25, 26, 27, 28, 29, 29, 30, 31, 32, 32, 33,
+                                       34, 34, 35, 35, 36, 36, 37, 37, 37, 38, 38, 38, 39, 39, 39, 39};
+__constant__ int c_mf[6][3] = {{13107, 5243, 8066}, {11916, 4660, 7490}, {10082, 4194, 6554},
+                               {9362, 3647, 5825},  {8192, 3355, 5243},  {7282, 2893, 4559}};
+__constant__ int c_v[6][3] = {{10, 16, 13}, {11, 18, 14}, {13, 20, 16}, {14, 23, 18}, {16, 25, 20}, {18, 29, 23}};
+// luma4x4BlkIdx -> (x, y) of the 4x4 block in the macroblock, in blocks
+__constant__ int8_t c_blk_x[16] = {0, 1, 0, 1, 2, 3, 2, 3, 0, 1, 0, 1, 2, 3, 2, 3};
+__constant__ int8_t c_blk_y[16] = {0, 0, 1, 1, 0, 0, 1, 1, 2, 2, 3, 3, 2, 2, 3, 3};
+
+// Table 9-5, [TrailingOnes + 4 TotalCoeff]
+__constant__ uint8_t c_ct_len[4][68] = {
+    {1,  0,  0,  0,  6,  2,  0,  0,  8,  6,  3,  0,  9,  8,  7,  5,  10, 9,  8,  6,  11, 10, 9,
+     7,  13, 11, 10, 8,  13, 13, 11, 9,  13, 13, 13, 10, 14, 14, 13, 11, 14, 14, 14, 13, 15, 15,
+     14, 14, 15, 15, 15, 14, 16, 15, 15, 15, 16, 16, 16, 15, 16, 16, 16, 16, 16, 16, 16, 16},
+    {2,  0,  0,  0,  6,  2,  0,  0,  6,  5,  3,  0,  7,  6,  6,  4,  8,  6,  6,  4,  8,  7,  7,
+     5,  9,  8,  8,  6,  11, 9,  9,  6,  11, 11, 11, 7,  12, 11, 11, 9,  12, 12, 12, 11, 12, 12,
+     12, 11, 13, 13, 13, 12, 13, 13, 13, 13, 13, 14, 13, 13, 14, 14, 14, 13, 14, 14, 14, 14},
+    {4, 0, 0, 0, 6, 4, 0, 0, 6, 5, 4, 0, 6, 5, 5, 4,  7,  5,  5,  4,  7,  5,  5,  4,  7,  6,  6,  4,  7,  6,  6,  4,  8,  7,
+     7, 5, 8, 8, 7, 6, 9, 8, 8, 7, 9, 9, 8, 8, 9, 9, 9, 8, 10, 9, 9, 9, 10, 10, 10, 10, 10, 10, 10, 10, 10, 10, 10, 10},
+    {6, 0, 0, 0, 6, 6, 0, 0, 6, 6, 6, 0, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6,
+     6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6}};
+__constant__ uint8_t c_ct_code[4][68] = {
+    {1,  0,  0, 0,  5, 1, 0, 0,  7,  4,  1, 0,  7,  6,  5,  3,  7,  6,  5,  3, 7, 6, 5,
+     4,  15, 6, 5,  4, 11, 14, 5, 4, 8, 10, 13, 4, 15, 14, 9, 4, 11, 10, 13, 12, 15, 14,
+     9,  12, 11, 10, 13, 8, 15, 1, 9, 12, 11, 14, 13, 8, 7, 10, 9, 12, 4, 6, 5, 8},
+    {3,  0,  0,  0,  11, 2,  0,  0,  7,  7,  3,  0,  7,  10, 9,  5,  7,  6, 5, 4, 4, 6, 5,
+     6,  7,  6,  5,  8,  15, 6,  5,  4,  11, 14, 13, 4,  15, 10, 9,  4,  11, 14, 13, 12, 8, 10,
+     9,  8,  15, 14, 13, 12, 11, 10, 9,  12, 7,  11, 6,  8,  9,  8,  10, 1,  7,  6,  5,  4},
+    {15, 0,  0,  0,  15, 14, 0,  0,  11, 15, 13, 0,  8,  12, 14, 12, 15, 10, 11, 11, 11, 8, 9,
+     10, 9,  14, 13, 9,  8,  10, 9,  8,  15, 14, 13, 13, 11, 14, 10, 12, 15, 10, 13, 12, 11, 14,
+     9,  12, 8,  10, 13, 8,  13, 7,  9,  12, 9,  12, 11, 10, 5,  8,  7,  6,  1,  4,  3,  2},
+    {3,  0,  0,  0,  0,  1,  0,  0,  4,  5,  6,  0,  8,  9,  10, 11, 12, 13, 14, 15, 16, 17, 18,
+     19, 20, 21, 22, 23, 24, 25, 26, 27, 28, 29, 30, 31, 32, 33, 34, 35, 36, 37, 38, 39, 40, 41,
+     42, 43, 44, 45, 46, 47, 48, 49, 50, 51, 52, 53, 54, 55, 56, 57, 58, 59, 60, 61, 62, 63}};
+__constant__ uint8_t c_cdc_len[20] = {2, 0, 0, 0, 6, 1, 0, 0, 6, 6, 3, 0, 6, 7, 7, 6, 6, 8, 8, 7};
+__constant__ uint8_t c_cdc_code[20] = {1, 0, 0, 0, 7, 1, 0, 0, 4, 6, 1, 0, 3, 3, 2, 5, 2, 3, 2, 0};
+// Tables 9-7 / 9-8, [TotalCoeff - 1][total_zeros]
+__constant__ uint8_t c_tz_len[15][16] = {
+    {1, 3, 3, 4, 4, 5, 5, 6, 6, 7, 7, 8, 8, 9, 9, 9}, {3, 3, 3, 3, 3, 4, 4, 4, 4, 5, 5, 6, 6, 6, 6},
+    {4, 3, 3, 3, 4, 4, 3, 3, 4, 5, 5, 6, 5, 6},       {5, 3, 4, 4, 3, 3, 3, 4, 3, 4, 5, 5, 5},
+    {4, 4, 4, 3, 3, 3, 3, 3, 4, 5, 4, 5},             {6, 5, 3, 3, 3, 3, 3, 3, 4, 3, 6},
+    {6, 5, 3, 3, 3, 2, 3, 4, 3, 6},                   {6, 4, 5, 3, 2, 2, 3, 3, 6},
+    {6, 6, 4, 2, 2, 3, 2, 5},                         {5, 5, 3, 2, 2, 2, 4},
+    {4, 4, 3, 3, 1, 3},                               {4, 4, 2, 1, 3},
+    {3, 3, 1, 2},                                     {2, 2, 1},
+    {1, 1}};
+__constant__ uint8_t c_tz_code[15][16] = {
+    {1, 3, 2, 3, 2, 3, 2, 3, 2, 3, 2, 3, 2, 3, 2, 1}, {7, 6, 5, 4, 3, 5, 4, 3, 2, 3, 2, 3, 2, 1, 0},
+    {5, 7, 6, 5, 4, 3, 4, 3, 2, 3, 2, 1, 1, 0},       {3, 7, 5, 4, 6, 5, 4, 3, 3, 2, 2, 1, 0},
+    {5, 4, 3, 7, 6, 5, 4, 3, 2, 1, 1, 0},             {1, 1, 7, 6, 5, 4, 3, 2, 1, 1, 0},
+    {1, 1, 5, 4, 3, 3, 2, 1, 1, 0},                   {1, 1, 1, 3, 3, 2, 2, 1, 0},
+    {1, 0, 1, 3, 2, 1, 1, 1},                         {1, 0, 1, 3, 2, 1, 1},
+    {0, 1, 1, 2, 1, 3},                               {0, 1, 1, 1, 1},
+    {0, 1, 1, 1},                                     {0, 1, 1},
+    {0, 1}};
+__constant__ uint8_t c_ctz_len[3][4] = {{1, 2, 3, 3}, {1, 2, 2}, {1, 1}};
+__constant__ uint8_t c_ctz_code[3][4] = {{1, 1, 1, 0}, {1, 1, 0}, {1, 0}};
+// Table 9-10, [min(zerosLeft, 7) - 1][run_before]
+__constant__ uint8_t c_rb_len[7][15] = {{1, 1},          {1, 2, 2},          {2, 2, 2, 2},         {2, 2, 2, 3, 3},
+                                        {2, 2, 3, 3, 3, 3}, {2, 3, 3, 3, 3, 3, 3}, {3, 3, 3, 3, 3, 3, 3, 4, 5, 6, 7, 8, 9, 10, 11}};
+__constant__ uint8_t c_rb_code[7][15] = {{1, 0},          {1, 1, 0},          {3, 2, 1, 0},         {3, 2, 1, 1, 0},
+                                         {3, 2, 3, 2, 1, 0}, {3, 0, 1, 3, 2, 5, 4}, {7, 6, 5, 4, 3, 2, 1, 1, 1, 1, 1, 1, 1, 1, 1}};
+
+// The per-frame scratch: offsets from the frame's base (each 256-byte aligned), and the frame stride.
+struct Layout {
+  int W, H, wm, hm, nmb, pieces;
+  int64_t src, rec, tot, lev, info, bits, off, raw, ep, meta, stride;
+};
+
+int64_t align256(int64_t x) { return (x + 255) / 256 * 256; }
+
+int64_t raw_bytes_bound(int nmb) { return (HEADER_BITS + (int64_t)nmb * (PCM_BITS + 7) + 1 + 7) / 8; }
+
+Layout layout(int H, int W) {
+  Layout l;
+  l.W = W;
+  l.H = H;
+  l.wm = (W + 15) / 16;
+  l.hm = (H + 15) / 16;
+  l.nmb = l.wm * l.hm;
+  const int64_t raw = raw_bytes_bound(l.nmb);
+  l.pieces = (int)((raw + EP_PIECE - 1) / EP_PIECE);
+  const int64_t plane = (int64_t)l.nmb * 384;   // Y, Cb, Cr of every macroblock
+  int64_t o = 0;
+  l.src = o;  o = align256(o + plane);
+  l.rec = o;  o = align256(o + plane);
+  l.tot = o;  o = align256(o + (int64_t)l.nmb * 24);                 // TotalCoeff: 16 luma, 4 Cb, 4 Cr per macroblock
+  l.lev = o;  o = align256(o + (int64_t)l.nmb * BLOCKS * 16 * 2);    // int16 levels in scan order
+  l.info = o; o = align256(o + (int64_t)l.nmb * 4);
+  l.bits = o; o = align256(o + (int64_t)l.nmb * 4);
+  l.off = o;  o = align256(o + (int64_t)l.nmb * 4);
+  l.raw = o;  o = align256(o + (raw + 7) / 4 * 4 + 4);                // the slice's words, one spare
+  l.ep = o;   o = align256(o + (int64_t)l.pieces * 16);               // per piece: 3 counts + end states | start state
+  l.meta = o; o = align256(o + 16);                                   // raw byte count
+  l.stride = o;
+  return l;
+}
+
+__device__ __forceinline__ int clip255(int v) { return min(max(v, 0), 255); }
+
+// Plane layout: luma rows of 16 wm bytes, then Cb and Cr rows of 8 wm bytes.
+struct Planes {
+  uint8_t* y;
+  uint8_t* cb;
+  uint8_t* cr;
+  int ys, cs;   // row strides
+  __device__ Planes(uint8_t* base, const Layout& l) {
+    ys = 16 * l.wm;
+    cs = 8 * l.wm;
+    y = base;
+    cb = base + (int64_t)ys * 16 * l.hm;
+    cr = cb + (int64_t)cs * 8 * l.hm;
+  }
+  __device__ uint8_t* chroma(int p) const { return p ? cr : cb; }
+};
+
+// ---- colour conversion -----------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) h264_convert_kernel(const uint8_t* __restrict__ rgb, uint8_t* scratch,
+                                                            Layout l) {
+  const int f = blockIdx.y;
+  const int cw = 8 * l.wm, chh = 8 * l.hm;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= cw * chh) return;
+  const int cx = i % cw, cy = i / cw;
+  const uint8_t* img = rgb + (int64_t)f * l.H * l.W * 3;
+  Planes p(scratch + (int64_t)f * l.stride + l.src, l);
+  for (int dy = 0; dy < 2; dy++)
+    for (int dx = 0; dx < 2; dx++) {
+      const int x = min(2 * cx + dx, l.W - 1), y = min(2 * cy + dy, l.H - 1);
+      const uint8_t* px = img + ((int64_t)y * l.W + x) * 3;
+      p.y[(2 * cy + dy) * p.ys + 2 * cx + dx] = (uint8_t)(((66 * px[0] + 129 * px[1] + 25 * px[2] + 128) >> 8) + 16);
+    }
+  const int sx = 2 * min(cx, l.W / 2 - 1), sy = 2 * min(cy, l.H / 2 - 1);
+  int r4 = 0, g4 = 0, b4 = 0;
+  for (int dy = 0; dy < 2; dy++)
+    for (int dx = 0; dx < 2; dx++) {
+      const uint8_t* px = img + ((int64_t)(sy + dy) * l.W + sx + dx) * 3;
+      r4 += px[0];
+      g4 += px[1];
+      b4 += px[2];
+    }
+  p.cb[cy * p.cs + cx] = (uint8_t)(((-38 * r4 - 74 * g4 + 112 * b4 + 512) >> 10) + 128);
+  p.cr[cy * p.cs + cx] = (uint8_t)(((112 * r4 - 94 * g4 - 18 * b4 + 512) >> 10) + 128);
+}
+
+// ---- bits ------------------------------------------------------------------------------------------------------
+// OR `len` (<= 32) bits of `code` into the big-endian bit string held in little-endian words, at bit `pos`.
+__device__ __forceinline__ void put_bits(uint32_t* buf, uint32_t pos, uint32_t code, int len) {
+  if (len <= 0) return;
+  const uint64_t v = (uint64_t)code << (64 - len - (int)(pos & 31));
+  const uint32_t hi = (uint32_t)(v >> 32), lo = (uint32_t)v;
+  if (hi) atomicOr(buf + (pos >> 5), __byte_perm(hi, 0, 0x0123));
+  if (lo) atomicOr(buf + (pos >> 5) + 1, __byte_perm(lo, 0, 0x0123));
+}
+
+__device__ __forceinline__ int ue_bits(int v) { return 2 * (32 - __clz(v + 1)) - 1; }
+
+struct BitSink {
+  uint32_t* buf;
+  uint32_t pos;
+  int n;
+  __device__ void u(uint32_t code, int len) {
+    if (buf) put_bits(buf, pos + n, code, len);
+    n += len;
+  }
+};
+
+// One residual_block_cavlc (9.2) of coefficients c[0 .. maxn) in scan order, context nc (-1: chroma DC); returns bits.
+__device__ int cavlc_block(const int* c, int maxn, int nc, BitSink& s) {
+  const int n0 = s.n;
+  int total = 0, last = -1;
+  for (int i = 0; i < maxn; i++)
+    if (c[i]) {
+      total++;
+      last = i;
+    }
+  int t1 = 0;
+  for (int i = last; i >= 0 && t1 < 3; i--) {
+    if (!c[i]) continue;
+    if (c[i] == 1 || c[i] == -1) t1++;
+    else break;
+  }
+  if (nc < 0) {
+    s.u(c_cdc_code[4 * total + t1], c_cdc_len[4 * total + t1]);
+  } else {
+    const int tab = nc < 2 ? 0 : nc < 4 ? 1 : nc < 8 ? 2 : 3;
+    s.u(c_ct_code[tab][4 * total + t1], c_ct_len[tab][4 * total + t1]);
+  }
+  if (total == 0) return s.n - n0;
+  int sl = (total > 10 && t1 < 3) ? 1 : 0;
+  int k = 0;   // nonzero coefficients seen, highest frequency first
+  for (int i = last; i >= 0; i--) {
+    const int v = c[i];
+    if (!v) continue;
+    if (k < t1) {
+      s.u(v < 0, 1);
+    } else {
+      int code = v > 0 ? 2 * v - 2 : -2 * v - 1;
+      if (k == t1 && t1 < 3) code -= 2;
+      int prefix, suffix, slen;
+      if (sl == 0) {
+        if (code < 14) { prefix = code; suffix = 0; slen = 0; }
+        else if (code < 30) { prefix = 14; suffix = code - 14; slen = 4; }
+        else { prefix = 15; suffix = code - 30; slen = 12; }
+      } else if (code < (15 << sl)) {
+        prefix = code >> sl; suffix = code & ((1 << sl) - 1); slen = sl;
+      } else {
+        prefix = 15; suffix = code - (15 << sl); slen = 12;
+      }
+      s.u(1, prefix + 1);
+      s.u((uint32_t)suffix, slen);
+      if (sl == 0) sl = 1;
+      if (abs(v) > (3 << (sl - 1)) && sl < 6) sl++;
+    }
+    k++;
+  }
+  const int zeros = last + 1 - total;
+  if (total < maxn) {
+    if (nc < 0) s.u(c_ctz_code[total - 1][zeros], c_ctz_len[total - 1][zeros]);
+    else s.u(c_tz_code[total - 1][zeros], c_tz_len[total - 1][zeros]);
+  }
+  int left = zeros, prev = last;
+  for (int i = last - 1; i >= 0 && left > 0; i--) {
+    if (!c[i]) continue;
+    const int run = prev - i - 1, t = min(left, 7) - 1;
+    s.u(c_rb_code[t][run], c_rb_len[t][run]);
+    left -= run;
+    prev = i;
+  }
+  return s.n - n0;
+}
+
+// TotalCoeff grid of a frame: per macroblock 16 luma (luma4x4BlkIdx raster: [by * 4 + bx]), 4 Cb, 4 Cr.
+__device__ __forceinline__ int tot_at(const uint8_t* tot, const Layout& l, int plane, int x, int y) {
+  const int per = plane == 0 ? 4 : 2;
+  const int mb = (y / per) * l.wm + x / per;
+  const int bx = x % per, by = y % per;
+  return tot[(int64_t)mb * 24 + (plane == 0 ? by * 4 + bx : 16 + 4 * (plane - 1) + by * 2 + bx)];
+}
+
+__device__ int nc_of(const uint8_t* tot, const Layout& l, int plane, int x, int y) {
+  const int a = x > 0 ? tot_at(tot, l, plane, x - 1, y) : -1;
+  const int b = y > 0 ? tot_at(tot, l, plane, x, y - 1) : -1;
+  if (a >= 0 && b >= 0) return (a + b + 1) >> 1;
+  return a >= 0 ? a : b >= 0 ? b : 0;
+}
+
+// Block id (0 .. 26, bitstream order) -> (plane, x, y of its 4x4 block in the plane's grid, max coefficients).
+__device__ void block_geom(int id, int mx, int my, int& plane, int& x, int& y, int& maxn) {
+  if (id == 0) { plane = 0; x = 4 * mx; y = 4 * my; maxn = 16; }
+  else if (id <= 16) { plane = 0; x = 4 * mx + c_blk_x[id - 1]; y = 4 * my + c_blk_y[id - 1]; maxn = 15; }
+  else if (id <= 18) { plane = -1; x = y = 0; maxn = 4; }
+  else { const int b = (id - 19) & 3; plane = 1 + (id - 19) / 4; x = 2 * mx + (b & 1); y = 2 * my + (b >> 1); maxn = 15; }
+}
+
+__device__ __forceinline__ bool block_present(int id, int cbpl, int cbpc) {
+  return id == 0 || (id <= 16 && cbpl) || (id > 16 && id <= 18 && cbpc >= 1) || (id > 18 && cbpc == 2);
+}
+
+__device__ __forceinline__ int mb_header_bits(int lmode, int cmode, int cbpl, int cbpc) {
+  return ue_bits(1 + lmode + 4 * cbpc + (cbpl ? 12 : 0)) + ue_bits(cmode) + 1;
+}
+
+// ---- the macroblock kernel ---------------------------------------------------------------------------------------
+__device__ __forceinline__ int quant(int c, int mf, int qbits, int f) {
+  const int q = (abs(c) * mf + f) >> qbits;
+  return c < 0 ? -q : q;
+}
+
+__device__ __forceinline__ int pos_class(int i) {   // raster index in a 4x4 block -> 0 (even, even), 1 (odd, odd), 2
+  const int r = i >> 2, c = i & 3;
+  return (!(r & 1) && !(c & 1)) ? 0 : ((r & 1) && (c & 1)) ? 1 : 2;
+}
+
+// 8.5.12.2 on a 4x4 block d (raster, row-major), in place -> residual (h + 32) >> 6
+__device__ void idct4(int* d) {
+  for (int i = 0; i < 4; i++) {
+    int* r = d + 4 * i;
+    const int e0 = r[0] + r[2], e1 = r[0] - r[2], e2 = (r[1] >> 1) - r[3], e3 = r[1] + (r[3] >> 1);
+    r[0] = e0 + e3; r[1] = e1 + e2; r[2] = e1 - e2; r[3] = e0 - e3;
+  }
+  for (int j = 0; j < 4; j++) {
+    const int f0 = d[j], f1 = d[4 + j], f2 = d[8 + j], f3 = d[12 + j];
+    const int g0 = f0 + f2, g1 = f0 - f2, g2 = (f1 >> 1) - f3, g3 = f1 + (f3 >> 1);
+    d[j] = (g0 + g3 + 32) >> 6; d[4 + j] = (g1 + g2 + 32) >> 6; d[8 + j] = (g1 - g2 + 32) >> 6;
+    d[12 + j] = (g0 - g3 + 32) >> 6;
+  }
+}
+
+struct MbShared {
+  int src[384];          // Y (16x16), Cb (8x8), Cr (8x8)
+  int pred[384];         // the chosen modes' predictions
+  int top[32], left[32]; // luma 0..15, Cb 16..23, Cr 24..31
+  int tl[3];
+  int par[3][8];         // per plane: DC value(s) and the plane parameters a, b, c
+  int cost[8];           // SATD of luma modes 0..3, chroma modes 0..3
+  int w[24][16];         // transform coefficients, then dequantised coefficients
+  int lev[24][16];       // quantised AC levels (raster; [0] unused)
+  int dc[16], cdc[2][4]; // quantised DC levels (luma [by * 4 + bx], chroma raster)
+  int dcr[16], cdcr[2][4];
+  int tot[24];
+  int maxlev, bits, lmode, cmode, cbpl, cbpc, pcm;
+};
+
+__device__ int predict(const MbShared& s, int plane, int mode, int x, int y) {
+  if (plane == 0) {
+    switch (mode) {
+      case 0: return s.top[x];
+      case 1: return s.left[y];
+      case 2: return s.par[0][0];
+      default: return clip255((s.par[0][1] + s.par[0][2] * (x - 7) + s.par[0][3] * (y - 7) + 16) >> 5);
+    }
+  }
+  const int o = 16 + 8 * (plane - 1);
+  switch (mode) {
+    case 0: return s.par[plane][(y >> 2) * 2 + (x >> 2)];
+    case 1: return s.left[o + y];
+    case 2: return s.top[o + x];
+    default: return clip255((s.par[plane][4] + s.par[plane][5] * (x - 3) + s.par[plane][6] * (y - 3) + 16) >> 5);
+  }
+}
+
+__global__ void __launch_bounds__(128) h264_mb_kernel(int d, int qp, uint8_t* scratch, Layout l) {
+  __shared__ MbShared s;
+  const int f = blockIdx.y, t = threadIdx.x;
+  const int mx = max(0, d - l.hm + 1) + blockIdx.x, my = d - mx;
+  const int mb = my * l.wm + mx;
+  const bool has_l = mx > 0, has_t = my > 0;
+  uint8_t* base = scratch + (int64_t)f * l.stride;
+  const Planes src(base + l.src, l), rec(base + l.rec, l);
+  uint8_t* tot = base + l.tot;
+  const int qpc = c_chroma_qp[qp];
+
+  for (int i = t; i < 384; i += 128) {
+    if (i < 256) s.src[i] = src.y[(16 * my + i / 16) * src.ys + 16 * mx + i % 16];
+    else {
+      const int p = (i - 256) / 64, j = (i - 256) % 64;
+      s.src[i] = src.chroma(p)[(8 * my + j / 8) * src.cs + 8 * mx + j % 8];
+    }
+  }
+  if (t < 32) {
+    const int p = t < 16 ? 0 : 1 + (t - 16) / 8, j = t < 16 ? t : (t - 16) % 8;
+    const uint8_t* pl = p == 0 ? rec.y : rec.chroma(p - 1);
+    const int st = p == 0 ? rec.ys : rec.cs, n = p == 0 ? 16 : 8;
+    s.top[t] = has_t ? pl[(n * my - 1) * st + n * mx + j] : 0;
+    s.left[t] = has_l ? pl[(n * my + j) * st + n * mx - 1] : 0;
+  }
+  if (t >= 32 && t < 35) {
+    const int p = t - 32;
+    const uint8_t* pl = p == 0 ? rec.y : rec.chroma(p - 1);
+    const int st = p == 0 ? rec.ys : rec.cs, n = p == 0 ? 16 : 8;
+    s.tl[p] = has_t && has_l ? pl[(n * my - 1) * st + n * mx - 1] : 0;
+  }
+  if (t < 8) s.cost[t] = 0;
+  if (t == 0) { s.maxlev = 0; s.bits = 0; }
+  __syncthreads();
+
+  // prediction parameters: DC values and the plane mode's a, b, c (8.3.3.3-4, 8.3.4.1-4)
+  if (t == 0) {
+    int st = 0, sl = 0, H = 0, V = 0;
+    for (int i = 0; i < 16; i++) { st += s.top[i]; sl += s.left[i]; }
+    s.par[0][0] = has_t && has_l ? (st + sl + 16) >> 5 : has_t ? (st + 8) >> 4 : has_l ? (sl + 8) >> 4 : 128;
+    for (int x = 0; x < 8; x++) {
+      H += (x + 1) * (s.top[8 + x] - (6 - x >= 0 ? s.top[6 - x] : s.tl[0]));
+      V += (x + 1) * (s.left[8 + x] - (6 - x >= 0 ? s.left[6 - x] : s.tl[0]));
+    }
+    s.par[0][1] = 16 * (s.left[15] + s.top[15]);
+    s.par[0][2] = (5 * H + 32) >> 6;
+    s.par[0][3] = (5 * V + 32) >> 6;
+  } else if (t == 32 || t == 64) {
+    const int p = t / 32, o = 16 + 8 * (p - 1);
+    const int* top = s.top + o;
+    const int* left = s.left + o;
+    for (int b = 0; b < 4; b++) {
+      const int bx = b & 1, by = b >> 1;
+      int st = 0, sl = 0;
+      for (int i = 0; i < 4; i++) { st += top[4 * bx + i]; sl += left[4 * by + i]; }
+      const int ts = (st + 2) >> 2, ls = (sl + 2) >> 2;
+      int v;
+      if (bx == by) v = has_t && has_l ? (st + sl + 4) >> 3 : has_t ? ts : has_l ? ls : 128;
+      else if (bx == 1) v = has_t ? ts : has_l ? ls : 128;
+      else v = has_l ? ls : has_t ? ts : 128;
+      s.par[p][b] = v;
+    }
+    int H = 0, V = 0;
+    for (int x = 0; x < 4; x++) {
+      H += (x + 1) * (top[4 + x] - (2 - x >= 0 ? top[2 - x] : s.tl[p]));
+      V += (x + 1) * (left[4 + x] - (2 - x >= 0 ? left[2 - x] : s.tl[p]));
+    }
+    s.par[p][4] = 16 * (left[7] + top[7]);
+    s.par[p][5] = (34 * H + 32) >> 6;
+    s.par[p][6] = (34 * V + 32) >> 6;
+  }
+  __syncthreads();
+
+  // SATD of every mode: 64 luma (mode, block) tasks, 32 chroma (mode, plane, block) tasks
+  if (t < 96) {
+    int plane, mode, bx, by, so;
+    if (t < 64) { plane = 0; mode = t / 16; bx = t & 3; by = (t >> 2) & 3; so = 0; }
+    else { const int u = t - 64; mode = u / 8; plane = 1 + (u / 4) % 2; bx = u & 1; by = (u >> 1) & 1; so = 256 + 64 * (plane - 1); }
+    const int n = plane == 0 ? 16 : 8;
+    int r[16];
+    for (int i = 0; i < 16; i++) {
+      const int x = 4 * bx + (i & 3), y = 4 * by + (i >> 2);
+      r[i] = s.src[so + y * n + x] - predict(s, plane, mode, x, y);
+    }
+    for (int i = 0; i < 4; i++) {   // rows
+      int* q = r + 4 * i;
+      const int a0 = q[0] + q[1], a1 = q[0] - q[1], a2 = q[2] + q[3], a3 = q[2] - q[3];
+      q[0] = a0 + a2; q[1] = a1 + a3; q[2] = a0 - a2; q[3] = a1 - a3;
+    }
+    int sum = 0;
+    for (int j = 0; j < 4; j++) {   // columns
+      const int a0 = r[j] + r[4 + j], a1 = r[j] - r[4 + j], a2 = r[8 + j] + r[12 + j], a3 = r[8 + j] - r[12 + j];
+      sum += abs(a0 + a2) + abs(a1 + a3) + abs(a0 - a2) + abs(a1 - a3);
+    }
+    atomicAdd(&s.cost[plane == 0 ? mode : 4 + mode], sum);
+  }
+  __syncthreads();
+  if (t == 0) {
+    const bool lav[4] = {has_t, has_l, true, has_t && has_l};
+    const bool cav[4] = {true, has_l, has_t, has_t && has_l};
+    int lm = 2, cm = 0;
+    for (int m = 0; m < 4; m++) {
+      if (lav[m] && (s.cost[m] < s.cost[lm] || (s.cost[m] == s.cost[lm] && m < lm))) lm = m;
+      if (cav[m] && (s.cost[4 + m] < s.cost[4 + cm] || (s.cost[4 + m] == s.cost[4 + cm] && m < cm))) cm = m;
+    }
+    s.lmode = lm;
+    s.cmode = cm;
+  }
+  __syncthreads();
+  for (int i = t; i < 384; i += 128) {
+    if (i < 256) s.pred[i] = predict(s, 0, s.lmode, i & 15, i >> 4);
+    else { const int p = 1 + (i - 256) / 64, j = (i - 256) % 64; s.pred[i] = predict(s, p, s.cmode, j & 7, j >> 3); }
+  }
+  __syncthreads();
+
+  // forward transform and AC quantisation: one thread per 4x4 block (16 luma raster, 4 Cb, 4 Cr)
+  if (t < 24) {
+    const bool luma = t < 16;
+    const int bx = luma ? (t & 3) : (t & 1), by = luma ? (t >> 2) : ((t >> 1) & 1);
+    const int n = luma ? 16 : 8, so = luma ? 0 : 256 + 64 * ((t - 16) / 4);
+    const int q = luma ? qp : qpc;
+    int x[16], m[16];
+    for (int i = 0; i < 16; i++) {
+      const int o = so + (4 * by + (i >> 2)) * n + 4 * bx + (i & 3);
+      x[i] = s.src[o] - s.pred[o];
+    }
+    for (int i = 0; i < 4; i++)      // m = CF x (columns)
+      for (int j = 0; j < 4; j++) {
+        const int a = x[j], b = x[4 + j], c = x[8 + j], e = x[12 + j];
+        m[i * 4 + j] = i == 0 ? a + b + c + e : i == 1 ? 2 * a + b - c - 2 * e : i == 2 ? a - b - c + e : a - 2 * b + 2 * c - e;
+      }
+    const int qbits = 15 + q / 6, fq = (1 << qbits) / 3;
+    int nz = 0, mx_ = 0;
+    for (int i = 0; i < 4; i++) {    // w = m CF^T (rows)
+      const int a = m[4 * i], b = m[4 * i + 1], c = m[4 * i + 2], e = m[4 * i + 3];
+      const int w4[4] = {a + b + c + e, 2 * a + b - c - 2 * e, a - b - c + e, a - 2 * b + 2 * c - e};
+      for (int j = 0; j < 4; j++) {
+        const int k = 4 * i + j;
+        s.w[t][k] = w4[j];
+        const int lv = k == 0 ? 0 : quant(w4[j], c_mf[q % 6][pos_class(k)], qbits, fq);
+        s.lev[t][k] = lv;
+        nz += lv != 0;
+        mx_ = max(mx_, abs(lv));
+      }
+    }
+    s.tot[t] = nz;
+    atomicMax(&s.maxlev, mx_);
+  }
+  __syncthreads();
+
+  // DC transforms, quantisation and their dequantisation (8.5.10, 8.5.11)
+  if (t == 0) {
+    int a[16], b[16];
+    for (int i = 0; i < 16; i++) a[i] = s.w[i][0];   // [by * 4 + bx]
+    // b = HD a HD, >> 1
+    for (int j = 0; j < 4; j++) {
+      const int p0 = a[j], p1 = a[4 + j], p2 = a[8 + j], p3 = a[12 + j];
+      b[j] = p0 + p1 + p2 + p3; b[4 + j] = p0 + p1 - p2 - p3; b[8 + j] = p0 - p1 - p2 + p3; b[12 + j] = p0 - p1 + p2 - p3;
+    }
+    const int qbits = 15 + qp / 6, fq = (1 << qbits) / 3;
+    int mx_ = 0;
+    for (int i = 0; i < 4; i++) {
+      const int p0 = b[4 * i], p1 = b[4 * i + 1], p2 = b[4 * i + 2], p3 = b[4 * i + 3];
+      const int r4[4] = {p0 + p1 + p2 + p3, p0 + p1 - p2 - p3, p0 - p1 - p2 + p3, p0 - p1 + p2 - p3};
+      for (int j = 0; j < 4; j++) {
+        const int lv = quant(r4[j] >> 1, c_mf[qp % 6][0], qbits + 1, 2 * fq);
+        s.dc[4 * i + j] = lv;
+        mx_ = max(mx_, abs(lv));
+      }
+    }
+    atomicMax(&s.maxlev, mx_);
+    // inverse: f = HD c HD, then scaled
+    for (int j = 0; j < 4; j++) {
+      const int p0 = s.dc[j], p1 = s.dc[4 + j], p2 = s.dc[8 + j], p3 = s.dc[12 + j];
+      b[j] = p0 + p1 + p2 + p3; b[4 + j] = p0 + p1 - p2 - p3; b[8 + j] = p0 - p1 - p2 + p3; b[12 + j] = p0 - p1 + p2 - p3;
+    }
+    const int ls = 16 * c_v[qp % 6][0];
+    for (int i = 0; i < 4; i++) {
+      const int p0 = b[4 * i], p1 = b[4 * i + 1], p2 = b[4 * i + 2], p3 = b[4 * i + 3];
+      const int r4[4] = {p0 + p1 + p2 + p3, p0 + p1 - p2 - p3, p0 - p1 - p2 + p3, p0 - p1 + p2 - p3};
+      for (int j = 0; j < 4; j++)
+        s.dcr[4 * i + j] = qp >= 36 ? (r4[j] * ls) << (qp / 6 - 6) : (r4[j] * ls + (1 << (5 - qp / 6))) >> (6 - qp / 6);
+    }
+  } else if (t == 32 || t == 64) {
+    const int p = t / 64, o = 16 + 4 * p;
+    const int a0 = s.w[o][0], a1 = s.w[o + 1][0], a2 = s.w[o + 2][0], a3 = s.w[o + 3][0];
+    const int c4[4] = {a0 + a1 + a2 + a3, a0 - a1 + a2 - a3, a0 + a1 - a2 - a3, a0 - a1 - a2 + a3};
+    const int qbits = 15 + qpc / 6, fq = (1 << qbits) / 3;
+    int mx_ = 0;
+    for (int i = 0; i < 4; i++) {
+      s.cdc[p][i] = quant(c4[i], c_mf[qpc % 6][0], qbits + 1, 2 * fq);
+      mx_ = max(mx_, abs(s.cdc[p][i]));
+    }
+    atomicMax(&s.maxlev, mx_);
+    const int l0 = s.cdc[p][0], l1 = s.cdc[p][1], l2 = s.cdc[p][2], l3 = s.cdc[p][3];
+    const int f4[4] = {l0 + l1 + l2 + l3, l0 - l1 + l2 - l3, l0 + l1 - l2 - l3, l0 - l1 - l2 + l3};
+    const int ls = 16 * c_v[qpc % 6][0];
+    for (int i = 0; i < 4; i++) s.cdcr[p][i] = ((f4[i] * ls) << (qpc / 6)) >> 5;
+  }
+  __syncthreads();
+
+  // reconstruction: dequantise, inverse transform, add the prediction
+  if (t < 24) {
+    const bool luma = t < 16;
+    const int q = luma ? qp : qpc;
+    int dq[16];
+    for (int k = 1; k < 16; k++) {
+      const int ls = 16 * c_v[q % 6][pos_class(k)], c = s.lev[t][k];
+      dq[k] = q >= 24 ? (c * ls) << (q / 6 - 4) : (c * ls + (1 << (3 - q / 6))) >> (4 - q / 6);
+    }
+    dq[0] = luma ? s.dcr[t] : s.cdcr[(t - 16) / 4][(t - 16) & 3];
+    idct4(dq);
+    for (int k = 0; k < 16; k++) s.w[t][k] = dq[k];   // the residual
+  }
+  __syncthreads();
+  if (t == 0) {
+    int al = 0, ac = 0, dcc = 0;
+    for (int i = 0; i < 16; i++) al += s.tot[i];
+    for (int i = 16; i < 24; i++) ac += s.tot[i];
+    for (int i = 0; i < 8; i++) dcc |= s.cdc[i / 4][i % 4];
+    s.cbpl = al ? 15 : 0;
+    s.cbpc = ac ? 2 : dcc ? 1 : 0;
+  }
+  __syncthreads();
+  // TotalCoeff of this macroblock's blocks (nC of its own later blocks reads them): luma by luma4x4 raster position
+  if (t < 24) tot[(int64_t)mb * 24 + t] = (uint8_t)s.tot[t];
+  __syncthreads();
+
+  // CAVLC bit count, one thread per residual block: 0 luma DC, 1..16 luma AC (luma4x4BlkIdx order), 17/18 Cb/Cr
+  // DC, 19..22 Cb AC, 23..26 Cr AC; the levels in scan order go to the writer
+  if (t < BLOCKS) {
+    int c[16], plane, x, y, maxn;
+    block_geom(t, mx, my, plane, x, y, maxn);
+    if (t == 0) for (int k = 0; k < 16; k++) c[k] = s.dc[c_zigzag[k]];
+    else if (t <= 16) { const int b = c_blk_y[t - 1] * 4 + c_blk_x[t - 1]; for (int k = 0; k < 15; k++) c[k] = s.lev[b][c_zigzag[k + 1]]; }
+    else if (t <= 18) for (int k = 0; k < 4; k++) c[k] = s.cdc[t - 17][k];
+    else { const int b = 16 + (t - 19); for (int k = 0; k < 15; k++) c[k] = s.lev[b][c_zigzag[k + 1]]; }
+    int16_t* out = reinterpret_cast<int16_t*>(base + l.lev) + ((int64_t)mb * BLOCKS + t) * 16;
+    for (int k = 0; k < maxn; k++) out[k] = (int16_t)max(-32768, min(32767, c[k]));
+    if (s.maxlev <= MAX_LEVEL && block_present(t, s.cbpl, s.cbpc)) {
+      BitSink sink{nullptr, 0, 0};
+      const int nc = plane < 0 ? -1 : nc_of(tot, l, plane, x, y);
+      atomicAdd(&s.bits, cavlc_block(c, maxn, nc, sink));
+    }
+  }
+  __syncthreads();
+  if (t == 0) {
+    const int bits = s.bits + mb_header_bits(s.lmode, s.cmode, s.cbpl, s.cbpc);
+    s.pcm = s.maxlev > MAX_LEVEL || bits > PCM_BITS;
+    reinterpret_cast<int*>(base + l.info)[mb] = s.lmode | s.cmode << 2 | s.cbpc << 4 | (s.cbpl ? 1 : 0) << 6 | s.pcm << 7;
+    reinterpret_cast<int*>(base + l.bits)[mb] = s.pcm ? 0 : bits;
+  }
+  __syncthreads();
+  if (s.pcm && t < 24) tot[(int64_t)mb * 24 + t] = 16;
+  for (int i = t; i < 384; i += 128) {
+    int v;
+    if (s.pcm) v = s.src[i];
+    else if (i < 256) v = clip255(s.pred[i] + s.w[((i >> 4) >> 2) * 4 + ((i & 15) >> 2)][((i >> 4) & 3) * 4 + (i & 3)]);
+    else {
+      const int p = (i - 256) / 64, j = (i - 256) % 64, x = j & 7, y = j >> 3;
+      v = clip255(s.pred[i] + s.w[16 + 4 * p + (y >> 2) * 2 + (x >> 2)][(y & 3) * 4 + (x & 3)]);
+    }
+    if (i < 256) rec.y[(16 * my + (i >> 4)) * rec.ys + 16 * mx + (i & 15)] = (uint8_t)v;
+    else {
+      const int p = (i - 256) / 64, j = (i - 256) % 64;
+      rec.chroma(p)[(8 * my + (j >> 3)) * rec.cs + 8 * mx + (j & 7)] = (uint8_t)v;
+    }
+  }
+}
+
+// ---- bit offsets -------------------------------------------------------------------------------------------------
+// x -> x + a (ceil == 0) or ceil8(x + a) + b (ceil == 1)
+struct Map {
+  int a, b, ceil;
+};
+
+__device__ __forceinline__ Map compose(Map f, Map g) {   // g after f
+  if (!g.ceil) return f.ceil ? Map{f.a, f.b + g.a, 1} : Map{f.a + g.a, 0, 0};
+  if (!f.ceil) return Map{f.a + g.a, g.b, 1};
+  return Map{f.a, ((f.b + g.a + 7) & ~7) + g.b, 1};
+}
+
+__device__ __forceinline__ int apply(Map m, int x) { return m.ceil ? ((x + m.a + 7) & ~7) + m.b : x + m.a; }
+
+__global__ void __launch_bounds__(1024) h264_scan_kernel(uint8_t* scratch, Layout l) {
+  __shared__ Map part[1024];
+  __shared__ int s_total;
+  const int f = blockIdx.x, t = threadIdx.x;
+  uint8_t* base = scratch + (int64_t)f * l.stride;
+  const int* info = reinterpret_cast<const int*>(base + l.info);
+  const int* bits = reinterpret_cast<const int*>(base + l.bits);
+  int* off = reinterpret_cast<int*>(base + l.off);
+  const int per = (l.nmb + 1023) / 1024, lo = min(t * per, l.nmb), hi = min(lo + per, l.nmb);
+  Map m{0, 0, 0};
+  for (int i = lo; i < hi; i++) m = compose(m, (info[i] >> 7) & 1 ? Map{9, PCM_BITS - 9, 1} : Map{bits[i], 0, 0});
+  part[t] = m;
+  __syncthreads();
+  for (int s = 1; s < 1024; s <<= 1) {   // inclusive Hillis-Steele scan
+    const Map prev = t >= s ? part[t - s] : Map{0, 0, 0};
+    __syncthreads();
+    if (t >= s) part[t] = compose(prev, part[t]);
+    __syncthreads();
+  }
+  int x = t == 0 ? HEADER_BITS : apply(part[t - 1], HEADER_BITS);
+  for (int i = lo; i < hi; i++) {
+    off[i] = x;
+    x = (info[i] >> 7) & 1 ? ((x + 9 + 7) & ~7) + PCM_BITS - 9 : x + bits[i];
+  }
+  if (t == 1023) s_total = apply(part[1023], HEADER_BITS);
+  __syncthreads();
+  const int total = s_total;                       // bits before the stop bit
+  const int nbytes = (total + 1 + 7) / 8;
+  uint32_t* raw = reinterpret_cast<uint32_t*>(base + l.raw);
+  for (int i = t; i < (nbytes + 3) / 4 + 1; i += 1024) raw[i] = 0;
+  __syncthreads();
+  if (t == 0) {
+    // first_mb_in_slice 0, slice_type 7, pps 0, frame_num 0000, idr_pic_id 1, two flags, slice_qp_delta 0,
+    // disable_deblocking_filter_idc 1
+    put_bits(raw, 0, 0x22208Au, HEADER_BITS);    // 1 0001000 1 0000 010 0 0 1 010
+    put_bits(raw, total, 1, 1);                  // rbsp_stop_one_bit
+    reinterpret_cast<int*>(base + l.meta)[0] = nbytes;
+  }
+}
+
+// ---- bit writing -------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(128) h264_write_kernel(uint8_t* scratch, Layout l) {
+  const int f = blockIdx.y, lane = threadIdx.x & 31;
+  const int mb = blockIdx.x * 4 + (threadIdx.x >> 5);
+  if (mb >= l.nmb) return;
+  uint8_t* base = scratch + (int64_t)f * l.stride;
+  uint32_t* raw = reinterpret_cast<uint32_t*>(base + l.raw);
+  const int info = reinterpret_cast<const int*>(base + l.info)[mb];
+  const uint32_t pos = (uint32_t)reinterpret_cast<const int*>(base + l.off)[mb];
+  const int mx = mb % l.wm, my = mb / l.wm;
+  if ((info >> 7) & 1) {   // I_PCM: ue(25), alignment, 256 Y + 64 Cb + 64 Cr samples
+    if (lane == 0) put_bits(raw, pos, 26, 9);
+    const uint32_t p0 = (pos + 9 + 7) & ~7u;
+    const Planes rec(base + l.rec, l);
+    for (int i = lane; i < 384; i += 32) {
+      int v;
+      if (i < 256) v = rec.y[(16 * my + (i >> 4)) * rec.ys + 16 * mx + (i & 15)];
+      else {
+        const int p = (i - 256) / 64, j = (i - 256) % 64;
+        v = rec.chroma(p)[(8 * my + (j >> 3)) * rec.cs + 8 * mx + (j & 7)];
+      }
+      put_bits(raw, p0 + 8 * i, (uint32_t)v, 8);
+    }
+    return;
+  }
+  const int lmode = info & 3, cmode = (info >> 2) & 3, cbpc = (info >> 4) & 3, cbpl = (info >> 6) & 1;
+  const uint8_t* tot = base + l.tot;
+  int c[16], plane = 0, x = 0, y = 0, maxn = 0, nc = 0, n = 0;
+  const bool present = lane < BLOCKS && block_present(lane, cbpl, cbpc);
+  if (present) {
+    block_geom(lane, mx, my, plane, x, y, maxn);
+    const int16_t* lev = reinterpret_cast<const int16_t*>(base + l.lev) + ((int64_t)mb * BLOCKS + lane) * 16;
+    for (int k = 0; k < 16; k++) c[k] = k < maxn ? lev[k] : 0;
+    nc = plane < 0 ? -1 : nc_of(tot, l, plane, x, y);
+    BitSink sink{nullptr, 0, 0};
+    n = cavlc_block(c, maxn, nc, sink);
+  }
+  int incl = n;
+  for (int s = 1; s < 32; s <<= 1) {
+    const int v = __shfl_up_sync(0xffffffffu, incl, s);
+    if (lane >= s) incl += v;
+  }
+  const int mbt = 1 + lmode + 4 * cbpc + (cbpl ? 12 : 0);
+  const int hb = mb_header_bits(lmode, cmode, cbpl, cbpc);
+  if (lane == 0) {
+    BitSink h{raw, pos, 0};
+    h.u(mbt + 1, ue_bits(mbt));
+    h.u(cmode + 1, ue_bits(cmode));
+    h.u(1, 1);                                   // mb_qp_delta 0
+  }
+  if (present) {
+    BitSink sink{raw, pos + hb + incl - n, 0};
+    cavlc_block(c, maxn, nc, sink);
+  }
+}
+
+// ---- emulation prevention and packing ----------------------------------------------------------------------------
+// Per piece and start state z (0, 1, >= 2 zero bytes before it): ep[j] = {count(z=0), count(1), count(2),
+// end states (2 bits each) | start state << 8 (written by the plan)}; the plan then overwrites count(0) with the
+// piece's output offset.
+__global__ void __launch_bounds__(128) h264_ep_count_kernel(uint8_t* scratch, Layout l) {
+  const int f = blockIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
+  uint8_t* base = scratch + (int64_t)f * l.stride;
+  const int nbytes = reinterpret_cast<const int*>(base + l.meta)[0];
+  const int lo = j * EP_PIECE;
+  if (lo >= nbytes) return;
+  const int hi = min(lo + EP_PIECE, nbytes);
+  const uint8_t* raw = base + l.raw;
+  int z[3] = {0, 1, 2}, cnt[3] = {0, 0, 0};
+  for (int i = lo; i < hi; i++) {
+    const int b = raw[i];
+    for (int s = 0; s < 3; s++) {
+      if (z[s] >= 2 && b <= 3) { cnt[s]++; z[s] = 0; }
+      z[s] = b == 0 ? min(z[s] + 1, 2) : 0;
+    }
+  }
+  int4* ep = reinterpret_cast<int4*>(base + l.ep);
+  ep[j] = make_int4(cnt[0], cnt[1], cnt[2], z[0] | z[1] << 2 | z[2] << 4);
+}
+
+__global__ void __launch_bounds__(32) h264_ep_plan_kernel(uint8_t* scratch, Layout l, uint8_t* out, int64_t out_stride,
+                                                          int64_t* out_len) {
+  const int f = blockIdx.x, lane = threadIdx.x;
+  uint8_t* base = scratch + (int64_t)f * l.stride;
+  const int nbytes = reinterpret_cast<const int*>(base + l.meta)[0];
+  const int np = (nbytes + EP_PIECE - 1) / EP_PIECE;
+  int4* ep = reinterpret_cast<int4*>(base + l.ep);
+  int state = 0, added = 0;                      // the NAL header byte 0x65 is not zero
+  for (int j0 = 0; j0 < np; j0 += 32) {
+    const int j = j0 + lane;
+    const int4 e = j < np ? ep[j] : make_int4(0, 0, 0, 0);
+    for (int k = 0; k < 32 && j0 + k < np; k++) {
+      const int c0 = __shfl_sync(0xffffffffu, e.x, k), c1 = __shfl_sync(0xffffffffu, e.y, k);
+      const int c2 = __shfl_sync(0xffffffffu, e.z, k), st = __shfl_sync(0xffffffffu, e.w, k);
+      if (lane == k) ep[j] = make_int4((j0 + k) * EP_PIECE + added, 0, 0, state);
+      added += state == 0 ? c0 : state == 1 ? c1 : c2;
+      state = (st >> (2 * state)) & 3;
+    }
+  }
+  if (lane == 0) {
+    const int64_t body = 1 + (int64_t)nbytes + added;
+    uint8_t* o = out + (int64_t)f * out_stride;
+    o[0] = (uint8_t)(body >> 24); o[1] = (uint8_t)(body >> 16); o[2] = (uint8_t)(body >> 8); o[3] = (uint8_t)body;
+    o[4] = 0x65;                                 // nal_ref_idc 3, nal_unit_type 5 (IDR slice)
+    out_len[f] = 4 + body;
+  }
+}
+
+__global__ void __launch_bounds__(128) h264_ep_emit_kernel(uint8_t* scratch, Layout l, uint8_t* out,
+                                                           int64_t out_stride) {
+  const int f = blockIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
+  uint8_t* base = scratch + (int64_t)f * l.stride;
+  const int nbytes = reinterpret_cast<const int*>(base + l.meta)[0];
+  const int lo = j * EP_PIECE;
+  if (lo >= nbytes) return;
+  const int hi = min(lo + EP_PIECE, nbytes);
+  const int4 e = reinterpret_cast<const int4*>(base + l.ep)[j];
+  const uint8_t* raw = base + l.raw;
+  uint8_t* o = out + (int64_t)f * out_stride + 5 + e.x;
+  int z = e.w;
+  for (int i = lo; i < hi; i++) {
+    const int b = raw[i];
+    if (z >= 2 && b <= 3) { *o++ = 3; z = 0; }
+    *o++ = (uint8_t)b;
+    z = b == 0 ? min(z + 1, 2) : 0;
+  }
+}
+
+// ---- host: level, parameter sets ---------------------------------------------------------------------------------
+struct LevelRow {
+  int idc, mbps, fs;
+};
+const LevelRow kLevels[] = {{10, 1485, 99},      {11, 3000, 396},     {12, 6000, 396},     {13, 11880, 396},
+                            {20, 11880, 396},    {21, 19800, 792},    {22, 20250, 1620},   {30, 40500, 1620},
+                            {31, 108000, 3600},  {32, 216000, 5120},  {40, 245760, 8192},  {41, 245760, 8192},
+                            {42, 522240, 8704},  {50, 589824, 22080}, {51, 983040, 36864}, {52, 2073600, 36864}};
+
+bool fits(int wm, int hm, int fs) { return (int64_t)wm * hm <= fs && (int64_t)wm * wm <= 8 * fs && (int64_t)hm * hm <= 8 * fs; }
+
+struct HostBits {
+  std::vector<uint8_t> bytes;
+  int n = 0;
+  void u(uint64_t v, int len) {
+    for (int i = len - 1; i >= 0; i--) {
+      if (n % 8 == 0) bytes.push_back(0);
+      if ((v >> i) & 1) bytes.back() |= (uint8_t)(0x80 >> (n % 8));
+      n++;
+    }
+  }
+  void ue(uint32_t v) {
+    const uint64_t x = (uint64_t)v + 1;
+    int L = 0;
+    while ((x >> L) > 1) L++;
+    u(x, 2 * L + 1);
+  }
+  void se(int v) { ue(v > 0 ? 2 * v - 1 : -2 * v); }
+  std::vector<uint8_t> nal(int type) {   // trailing bits, emulation prevention, the header byte
+    u(1, 1);
+    while (n % 8) u(0, 1);
+    std::vector<uint8_t> o{(uint8_t)(0x60 | type)};
+    int zeros = 0;
+    for (uint8_t b : bytes) {
+      if (zeros >= 2 && b <= 3) { o.push_back(3); zeros = 0; }
+      o.push_back(b);
+      zeros = b == 0 ? zeros + 1 : 0;
+    }
+    return o;
+  }
+};
+
+}  // namespace
+
+int h264_level_idc(int W, int H, int fps_num, int fps_den) {
+  const int wm = (W + 15) / 16, hm = (H + 15) / 16;
+  for (const LevelRow& r : kLevels)
+    if (fits(wm, hm, r.fs) && (int64_t)wm * hm * fps_num <= (int64_t)r.mbps * fps_den) return r.idc;
+  return fits(wm, hm, MAX_MBS) ? 52 : -1;
+}
+
+int64_t h264_bound(int W, int H) {
+  if (W <= 0 || H <= 0 || (W & 1) || (H & 1) || W > 65536 || H > 65536) return -1;
+  if (h264_level_idc(W, H, 0, 1) < 0) return -1;
+  const int64_t n = raw_bytes_bound(((W + 15) / 16) * ((H + 15) / 16));
+  return 5 + n + (n + 1) / 2;
+}
+
+size_t h264_scratch_bytes(int64_t frames, int H, int W) {
+  if (frames <= 0 || frames > 65535 || h264_bound(W, H) < 0) return 0;
+  return (size_t)(frames * layout(H, W).stride);
+}
+
+int32_t h264_parameter_sets(int W, int H, int qp, int fps_num, int fps_den, uint8_t* out, int64_t cap) {
+  if (h264_bound(W, H) < 0 || qp < 0 || qp > 51 || fps_num <= 0 || fps_den <= 0 || fps_num > (INT32_MAX / 2)) return -1;
+  const int wc = (W + 15) / 16 * 16, hc = (H + 15) / 16 * 16;
+  HostBits s;
+  s.u(66, 8);                    // profile_idc: Baseline
+  s.u(0xC0, 8);                  // constraint_set0_flag, constraint_set1_flag: Constrained Baseline
+  s.u(h264_level_idc(W, H, fps_num, fps_den), 8);
+  s.ue(0);                       // seq_parameter_set_id
+  s.ue(0);                       // log2_max_frame_num_minus4
+  s.ue(2);                       // pic_order_cnt_type
+  s.ue(0);                       // max_num_ref_frames
+  s.u(0, 1);                     // gaps_in_frame_num_value_allowed_flag
+  s.ue(wc / 16 - 1);
+  s.ue(hc / 16 - 1);
+  s.u(1, 1);                     // frame_mbs_only_flag
+  s.u(1, 1);                     // direct_8x8_inference_flag
+  const bool crop = wc != W || hc != H;
+  s.u(crop, 1);
+  if (crop) {
+    s.ue(0);
+    s.ue((wc - W) / 2);
+    s.ue(0);
+    s.ue((hc - H) / 2);
+  }
+  s.u(1, 1);                     // vui_parameters_present_flag
+  s.u(0, 1);                     // aspect_ratio_info_present_flag
+  s.u(0, 1);                     // overscan_info_present_flag
+  s.u(1, 1);                     // video_signal_type_present_flag
+  s.u(5, 3);                     // video_format: unspecified
+  s.u(0, 1);                     // video_full_range_flag: limited range
+  s.u(1, 1);                     // colour_description_present_flag
+  s.u(2, 8);                     // colour_primaries: unspecified
+  s.u(2, 8);                     // transfer_characteristics: unspecified
+  s.u(6, 8);                     // matrix_coefficients: BT.601
+  s.u(0, 1);                     // chroma_loc_info_present_flag
+  s.u(1, 1);                     // timing_info_present_flag
+  s.u((uint32_t)fps_den, 32);    // num_units_in_tick
+  s.u(2 * (uint32_t)fps_num, 32);// time_scale
+  s.u(1, 1);                     // fixed_frame_rate_flag
+  s.u(0, 1);                     // nal_hrd_parameters_present_flag
+  s.u(0, 1);                     // vcl_hrd_parameters_present_flag
+  s.u(0, 1);                     // pic_struct_present_flag
+  s.u(0, 1);                     // bitstream_restriction_flag
+  const std::vector<uint8_t> sps = s.nal(7);
+  HostBits p;
+  p.ue(0);                       // pic_parameter_set_id
+  p.ue(0);                       // seq_parameter_set_id
+  p.u(0, 1);                     // entropy_coding_mode_flag: CAVLC
+  p.u(0, 1);                     // bottom_field_pic_order_in_frame_present_flag
+  p.ue(0);                       // num_slice_groups_minus1
+  p.ue(0);
+  p.ue(0);                       // num_ref_idx_l0/l1_default_active_minus1
+  p.u(0, 1);                     // weighted_pred_flag
+  p.u(0, 2);                     // weighted_bipred_idc
+  p.se(qp - 26);                 // pic_init_qp_minus26
+  p.se(0);                       // pic_init_qs_minus26
+  p.se(0);                       // chroma_qp_index_offset
+  p.u(1, 1);                     // deblocking_filter_control_present_flag
+  p.u(0, 1);                     // constrained_intra_pred_flag
+  p.u(0, 1);                     // redundant_pic_cnt_present_flag
+  const std::vector<uint8_t> pps = p.nal(8);
+  const int64_t need = 4 + (int64_t)sps.size() + (int64_t)pps.size();
+  if (out == nullptr || cap < need) return -1;
+  int64_t o = 0;
+  for (const std::vector<uint8_t>* v : {&sps, &pps}) {
+    out[o++] = (uint8_t)(v->size() >> 8);
+    out[o++] = (uint8_t)v->size();
+    for (uint8_t b : *v) out[o++] = b;
+  }
+  return (int32_t)need;
+}
+
+void launch_h264_encode(int frames, int H, int W, int qp, const uint8_t* rgb, void* scratch, uint8_t* out,
+                        int64_t out_stride, int64_t* out_len, cudaStream_t stream) {
+  const Layout l = layout(H, W);
+  uint8_t* s = static_cast<uint8_t*>(scratch);
+  const unsigned F = (unsigned)frames;
+  h264_convert_kernel<<<dim3((unsigned)((64 * l.nmb + 255) / 256), F), 256, 0, stream>>>(rgb, s, l);
+  count_launch();
+  for (int d = 0; d < l.wm + l.hm - 1; d++) {
+    const int n = std::min(d, l.wm - 1) - std::max(0, d - l.hm + 1) + 1;
+    h264_mb_kernel<<<dim3((unsigned)n, F), 128, 0, stream>>>(d, qp, s, l);
+    count_launch();
+  }
+  h264_scan_kernel<<<F, 1024, 0, stream>>>(s, l);
+  count_launch();
+  h264_write_kernel<<<dim3((unsigned)((l.nmb + 3) / 4), F), 128, 0, stream>>>(s, l);
+  count_launch();
+  const unsigned pb = (unsigned)((l.pieces + 127) / 128);
+  h264_ep_count_kernel<<<dim3(pb, F), 128, 0, stream>>>(s, l);
+  count_launch();
+  h264_ep_plan_kernel<<<F, 32, 0, stream>>>(s, l, out, out_stride, out_len);
+  count_launch();
+  h264_ep_emit_kernel<<<dim3(pb, F), 128, 0, stream>>>(s, l, out, out_stride);
+  count_launch();
+}
+
+}  // namespace gab

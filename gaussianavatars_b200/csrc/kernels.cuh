@@ -244,6 +244,14 @@ void launch_png_encode(int views, int H, int W, const uint8_t* rgb, void* scratc
 void launch_png_copy(int views, const uint8_t* src, int64_t src_stride, const int64_t* src_len, const int32_t* flag,
                      uint8_t* dst, int64_t dst_stride, int64_t* dst_len, cudaStream_t stream);
 
+// h264.cu
+int64_t h264_bound(int W, int H);
+int h264_level_idc(int W, int H, int fps_num, int fps_den);
+size_t h264_scratch_bytes(int64_t frames, int H, int W);
+int32_t h264_parameter_sets(int W, int H, int qp, int fps_num, int fps_den, uint8_t* out, int64_t cap);
+void launch_h264_encode(int frames, int H, int W, int qp, const uint8_t* rgb, void* scratch, uint8_t* out,
+                        int64_t out_stride, int64_t* out_len, cudaStream_t stream);
+
 // png_decode.cu
 int64_t png_decode_stride(int H, int W);
 size_t png_decode_scratch_bytes(int64_t files, int H, int W);

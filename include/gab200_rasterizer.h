@@ -531,6 +531,49 @@ size_t gab200_resize_scratch_bytes(int64_t planes, int32_t in_height, int32_t in
 int32_t gab200_resize_u8(int64_t planes, int32_t in_height, int32_t in_width, int32_t out_height, int32_t out_width,
                          const uint8_t* src, uint8_t* dst, void* scratch, void* stream);
 
+/* H.264 video frames encoded on the device (csrc/h264.cu, gaussianavatars_b200.video): Constrained Baseline
+ * (profile_idc 66, constraint_set0/1), 8-bit 4:2:0, CAVLC.  Every picture is one IDR slice (pic_order_cnt_type 2,
+ * max_num_ref_frames 0), so every frame is a seek point and the frames of a batch are independent.  Deblocking is off
+ * (disable_deblocking_filter_idc 1): a conforming decoder outputs exactly the encoder's reconstruction.  One QP per
+ * stream; the chroma QP from Table 8-15 with chroma_qp_index_offset 0.
+ *
+ * RGB -> BT.601 limited range in integers: Y = ((66 R + 129 G + 25 B + 128) >> 8) + 16; with R4, G4, B4 the sums of a
+ * 2x2 block, Cb = ((-38 R4 - 74 G4 + 112 B4 + 512) >> 10) + 128, Cr = ((112 R4 - 94 G4 - 18 B4 + 512) >> 10) + 128
+ * (the VUI says matrix_coefficients 6, video_full_range_flag 0).  Width and height must be even; a size that is not a
+ * multiple of 16 is padded by edge replication and cropped by the SPS's frame_cropping.
+ *
+ * Each macroblock is I_16x16: the luma mode (V, H, DC, Plane) and the chroma mode (DC, H, V, Plane) of least SATD
+ * (sum of |4x4 Hadamard| of the residual) among those available, ties to the lowest mode number; forward quantisation
+ * (|c| MF + f) >> qbits with f = 2^qbits / 3, doubled with qbits + 1 for the DC transforms.  It becomes I_PCM when a
+ * level falls outside +-2063 (what Baseline's level_prefix <= 15 codes) or its CAVLC bits exceed 9 + 3072.
+ * oracle/h264.py restates the encode bit for bit.
+ *
+ * Each sample carries idr_pic_id 1.  Consecutive IDR pictures need different ids, so a muxer sets idr_pic_id 2 on
+ * every other sample by setting bit 0 of byte 6 of the sample (0x82 -> 0x83: ue(1) and ue(2) have one length).
+ * There is no rate control: the bit rate is not held to the level's MaxBR.
+ *
+ * Bound: the largest sample of a width x height frame, 5 + n + ceil(n / 2) for the n bytes of a slice of I_PCM
+ * macroblocks; -1 for a size <= 0, an odd size, or a frame above level 5.2 (36864 macroblocks, or a side above
+ * sqrt(8 * 36864) macroblocks). */
+int64_t gab200_h264_bound(int32_t width, int32_t height);
+/* Scratch bytes of an encode of `frames` frames (0 for a size or count gab200_h264_encode refuses). */
+size_t gab200_h264_scratch_bytes(int32_t frames, int32_t height, int32_t width);
+/* Encode rgb [frames, height, width, 3] uint8 (contiguous, device): frame k's access unit, one MP4 sample (a 4-byte
+ * big-endian length and the IDR slice NAL unit, emulation-prevented), at out + k * out_stride (out_stride >= the
+ * bound), its length to out_len[k] (int64, device).  scratch: gab200_h264_scratch_bytes bytes, 256-byte aligned.
+ * The macroblocks run as a wavefront, one launch per anti-diagonal (width / 16 + height / 16 - 1 launches).  Reads
+ * nothing on the host: capturable.  Refused before any device work: frames outside 1..65535, a refused size, qp
+ * outside 0..51, a stride below the bound, a null pointer, a misaligned scratch. */
+int32_t gab200_h264_encode(int32_t frames, int32_t height, int32_t width, int32_t qp, const uint8_t* rgb, void* scratch,
+                           uint8_t* out, int64_t out_stride, int64_t* out_len, void* stream);
+/* The stream's SPS and PPS NAL units (header byte included, emulation-prevented) on the host, as an avcC box lists
+ * them: a 2-byte big-endian length and the SPS, then a 2-byte length and the PPS.  level_idc is the smallest level of
+ * Table A-1 whose MaxFS, frame-side limit and MaxMBPS at fps_num / fps_den cover the size (5.2 when only the rate
+ * exceeds them); the VUI's timing is num_units_in_tick = fps_den, time_scale = 2 fps_num.  Returns the bytes written,
+ * or -1 for a refused size, qp or rate, or a capacity too small. */
+int32_t gab200_h264_parameter_sets(int32_t width, int32_t height, int32_t qp, int32_t fps_num, int32_t fps_den,
+                                   uint8_t* out, int64_t cap);
+
 /* A device-resident view schedule (csrc/schedule.cu, gaussianavatars_b200.schedule.ViewSchedule): `records` records
  * of `views` cameras each -- cams [records, views, GAB200_CAMERA_FLOATS] float32, timesteps [records] int32 (may be
  * NULL), frame_ids [records, views] int32 (may be NULL) -- visited in the order order[0 .. length).  `cursor` is one
