@@ -25,8 +25,8 @@
 //     in which the bands' dependency chains interleave (ILP); otherwise the live bands run under warp-uniform
 //     branches and dead bands cost nothing.  Lanes whose pixel did not contribute carry alpha = G = 0 through the
 //     same instructions (no divergence).  Per-lane partial sums over the K pixels collapse to three moments
-//     (S0,S1,S2) because dx is shared, and the nine per-splat gradient components leave through a three-stage
-//     pipelined shared-memory row reduction that ends in one 9-lane RED.ADD.F32 per (warp, splat).
+//     (S0,S1,S2) because dx is shared, and the nine per-splat gradient components of three consecutive visits leave
+//     together through a shared-memory row reduction that ends in one 27-lane RED.ADD.F32 per three visits.
 // Tensor cores are not used: there is no dense contraction on this path (north_star).
 #include <type_traits>
 
@@ -566,12 +566,15 @@ struct BandLoop<K, K, DA> {
 };
 
 // Shared memory of one backward warp task: NR gradient components per splat (9; 10 with the depth plane's dL/dz).
+// rows holds one batch of three visits, row slot * NR + component, one float per lane.  The stride of 36 floats puts
+// the rows that eight consecutive lanes read with LDS.128 on eight different 4-bank groups (36 = 4 mod 32), so the
+// lane-per-row loads are conflict-free; the stores (one row, 32 consecutive floats) are too.  One batch, not two: two
+// padded batches (7.8 KB per warp, 8.6 KB with DA) would not let five 4-warp CTAs fit in the SM's 228 KB.
 #define ROWS_STRIDE 36
 template <int NR>
 struct __align__(16) WarpSmemT {
   SplatRec rec[2][32];
-  float rows[2][NR * ROWS_STRIDE];  // [visit parity][component][lane], row stride 36 floats
-  float part[2][32];                // [visit parity][component * 2 + half]  (2 NR used)
+  float rows[3 * NR][ROWS_STRIDE];  // [visit slot * NR + component][lane]
   uint32_t ids[ID_RING][32 + 4];
   uint8_t masks[ID_RING][32 + 16];
   uint64_t mbar[ID_RING];
@@ -583,11 +586,12 @@ struct __align__(16) WarpSmemT {
 //     apart freely, and each walks only up to ITS pixels' largest n_contrib.
 //   * A visit whose K bands are all live is one straight-line block, so the compiler interleaves the bands'
 //     dependency chains; otherwise each band runs under a warp-uniform branch and dead bands cost nothing (BandLoop).
-//   * The nine gradient components leave through a SOFTWARE-PIPELINED reduction: visit j stores its nine per-lane
-//     values as rows of a shared-memory tile; during visit j+1 eighteen lanes each add half a row (4 LDS.128) and
-//     store 18 partials; during visit j+2 nine lanes add the two halves and issue the RED.  No shuffle, no exposed
-//     shared-memory or shuffle latency: the loads of rounds 1 and 2 are issued at the top of a visit and consumed
-//     after its band math.
+//   * The NR gradient components of three consecutive visits leave together through one BATCHED reduction: each
+//     visit stores its NR per-lane values as rows slot * NR .. slot * NR + NR-1 of a shared-memory tile; after the
+//     third, lane l < 3 NR loads row l (8 LDS.128), adds it with the same tree the single-visit reduction used (each
+//     per-(warp, splat) sum is the same float) and issues the batch's one RED (27 lanes; 30 with DA); the walk's end
+//     sends a partial batch.  The loads are not held across the next visit's band math: 32 more live floats there
+//     spill at the 96-register bound of 5 CTAs per SM, so their latency is left to the SM's other warps.
 // DA (gab200_backward_depth_alpha): records from the preprocess with DA (z in q2.w); dL_dalpha / dL_ddepth [H,W] or
 // NULL (zero); a tenth component, dL/dz, leaves for g2d slot 9.
 template <int K, bool DA>
@@ -693,22 +697,26 @@ __device__ __forceinline__ void backward_task(int tile, int tl, WarpSmemT<DA ? 1
   uint32_t id_c, mine_c, id_n = 0xffffffffu, mine_n = 0u;
   stage_chunk(0, id_c, mine_c);
 
-  // reduction pipeline state: ids of the two visits whose sums are still on their way out
-  uint32_t id1 = 0xffffffffu, id2 = 0xffffffffu;  // visit j-1 (rows written), visit j-2 (partials written)
-  uint32_t par = 0;                                // parity of the current visit
-  // round 1 (lane < 2 NR): component c1 = lane / 2, half h1 = lane & 1: sum of rows[c1][16 h1 .. 16 h1 + 15]
-  const int c1 = min(lane >> 1, NR - 1), h1 = lane & 1;
-  // round 2 (lane < NR): component lane: part[2 lane] + part[2 lane + 1]
-  auto reduce_step = [&](uint32_t id_rows, uint32_t id_part) {
-    // partials of the visit before last -> global
-    const float2 pp = *reinterpret_cast<const float2*>(&sm.part[par][2 * min(lane, NR - 1)]);
-    // rows of the last visit -> partials
-    const float4* r4 = reinterpret_cast<const float4*>(&sm.rows[par ^ 1][c1 * ROWS_STRIDE + h1 * 16]);
-    const float4 a = r4[0], b = r4[1], c = r4[2], d = r4[3];
-    if (id_part != 0xffffffffu && lane < NR) atomicAdd(g2d + (size_t)id_part * GAB_G2D_STRIDE + lane, pp.x + pp.y);
-    const float s = (((a.x + a.y) + (a.z + a.w)) + ((b.x + b.y) + (b.z + b.w))) +
-                    (((c.x + c.y) + (c.z + c.w)) + ((d.x + d.y) + (d.z + d.w)));
-    if (id_rows != 0xffffffffu && lane < 2 * NR) sm.part[par ^ 1][lane] = s;
+  // batch reduction state: `fill` visits (0..3, warp-uniform) have their rows in sm.rows; lane l < 3 NR owns row l,
+  // component l % NR of the batch's visit l / NR, whose splat id is my_id.  Lanes >= 3 NR have my_slot = 3 and never
+  // send anything.
+  int fill = 0;
+  const int my_slot = lane / NR;
+  uint32_t my_id = 0xffffffffu;
+  const float4* my_row = reinterpret_cast<const float4*>(sm.rows[min(lane, 3 * NR - 1)]);
+  float* my_g2d = g2d + lane % NR;
+  // the batch's rows -> g2d: lane l < 3 NR sums row l (8 LDS.128, the tree of the two 16-float halves, then their
+  // sum) and sends it if a visit of this batch filled its slot
+  auto send_batch = [&]() {
+    __syncwarp();  // the rows of the batch's last visit are complete
+    float h[2];
+#pragma unroll
+    for (int k = 0; k < 2; k++) {
+      const float4 a = my_row[4 * k], b = my_row[4 * k + 1], c = my_row[4 * k + 2], d = my_row[4 * k + 3];
+      h[k] = (((a.x + a.y) + (a.z + a.w)) + ((b.x + b.y) + (b.z + b.w))) +
+             (((c.x + c.y) + (c.z + c.w)) + ((d.x + d.y) + (d.z + d.w)));
+    }
+    if (my_slot < fill) atomicAdd(my_g2d + (size_t)my_id * GAB_G2D_STRIDE, h[0] + h[1]);
   };
 
   for (int c = 0; c < nchunks; c++) {
@@ -726,12 +734,11 @@ __device__ __forceinline__ void backward_task(int tile, int tl, WarpSmemT<DA ? 1
       const uint32_t m = __shfl_sync(FULLMASK, mine_c, jj);
       const uint32_t id0 = __shfl_sync(FULLMASK, id_c, jj);
       const int pos = n - 1 - (c * 32 + jj);
-      __syncwarp();  // rows/partials of the previous visit are complete; this visit's buffers are free
+      __syncwarp();  // a batch sent after the previous visit has been read; its slot 0 is free
       const float4 q0 = cur[jj].q0;
       const float4 q1 = cur[jj].q1;
       const float cbl = cur[jj].q2.x;
       const float czl = DA ? cur[jj].q2.w : 0.f;
-      reduce_step(id1, id2);
       const float dx = q0.x - fx;
       const float tA = q0.z * dx;
       SplatSumsT<DA> s;
@@ -742,7 +749,7 @@ __device__ __forceinline__ void backward_task(int tile, int tl, WarpSmemT<DA ? 1
       else BandLoop<K, 0, DA>::run(m, p, pos, q0.y, tA, dx, q0.w, q1.x, q1.y, q1.z, q1.w, cbl, s, czl);
       const float A = q0.z * CONIC_UNSCALE_AC, B = q0.w * CONIC_UNSCALE_B, C = q1.x * CONIC_UNSCALE_AC;
       const float dxS0 = dx * s.S0;
-      float* row = &sm.rows[par][lane];
+      float* row = &sm.rows[fill * NR][lane];
       row[0 * ROWS_STRIDE] = (-A * dxS0 - B * s.S1) * half_W;  // dL/dmean2D.x (NDC units)
       row[1 * ROWS_STRIDE] = (-C * s.S1 - B * dxS0) * half_H;  // dL/dmean2D.y
       row[2 * ROWS_STRIDE] = -0.5f * dx * dxS0;                // dL/dconic.xx
@@ -753,23 +760,18 @@ __device__ __forceinline__ void backward_task(int tile, int tl, WarpSmemT<DA ? 1
       row[7 * ROWS_STRIDE] = s.gg;
       row[8 * ROWS_STRIDE] = s.gb;
       if constexpr (DA) row[9 * ROWS_STRIDE] = s.gz;         // dL/dz (view-space depth)
-      id2 = id1;
-      id1 = id0;
-      par ^= 1;
+      if (my_slot == fill) my_id = id0;
+      if (++fill == 3) {  // the batch is full
+        send_batch();
+        fill = 0;
+      }
     }
     id_c = id_n;
     mine_c = mine_n;
   }
   cp_async_wait<0>();
-  // drain the reduction pipeline: two more steps
-#pragma unroll
-  for (int k = 0; k < 2; k++) {
-    __syncwarp();
-    reduce_step(id1, id2);
-    id2 = id1;
-    id1 = 0xffffffffu;
-    par ^= 1;
-  }
+  // the last, partial batch (a lane whose slot no visit of it filled sends nothing)
+  if (fill > 0) send_batch();
 }
 
 // CTA = 128 threads: CTAs [0, n_heavy) take one heavy tile on four warps, K = 2; the rest take two light tiles each,
