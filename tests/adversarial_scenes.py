@@ -335,6 +335,120 @@ def pair_table(st):
 ALPHA_MIN = F32(1.0) / F32(255.0)
 
 
+# Error bound of the blend's float32 decisions against the oracle's (the margins of `knife_edges`).  The blend takes
+#   pw = fma(C' dy, dy, fma(B', dy, A' dx) dx)   with (A', B', C') = (-A/2, -B, -C/2) log2(e) from its own preprocess,
+#   G  = ex2.approx(pw),   alpha = min(.99, o G),
+# where the oracle takes power = -(A dx^2 + C dy^2)/2 - B dx dy and G = expf(power).  Per pair, with
+#   Q = |A| dx^2/2 + |B dx dy| + |C| dy^2/2   (the terms of the quadratic form, before they cancel):
+#   |pw / log2(e) - power| <= KNIFE_CONIC_REL Q        a conic off by up to ~60 ulp per component (the preprocess
+#                                                      need not match the oracle's bit for bit), plus the few
+#                                                      roundings of either evaluation and of the log2(e) scale.
+#                                                      The 60 ulp are an assumed bound, not a measured one: no test
+#                                                      compares the device conic with the oracle's.  A device conic
+#                                                      further off shows as unexplained entries, not as a pass;
+#   |G'/G - 1| <= that + KNIFE_EXP_REL                 ex2.approx.ftz.f32 is within 2^-22 relative (PTX ISA), expf
+#                                                      within one ulp, and o G rounds once.
+# At a splat's exact centre (dx = dy = 0) both sides evaluate power = 0 and G = 1 exactly, so alpha = o bit for bit.
+KNIFE_CONIC_REL = 2.0 ** -17
+KNIFE_EXP_REL = 2.0 ** -20
+# A second class, not a decision: a splat whose 3D covariance has condition number kappa carries float32 rounding
+# amplified by about kappa through the covariance and conic chain (forward and backward), so the kernel's and the
+# oracle's gradients of it may differ by ~kappa 2^-24 relative.  Beyond KNIFE_COND that reaches a tenth of the
+# gradient gate's rtol: a needle with axis ratio 1e3 (kappa 1e6) moved one dL/dmeans3D entry by 1.3 % on the H100.
+KNIFE_COND = 1e-4 * 2.0 ** 24
+T_STOP = F32(0.0001)
+
+
+def knife_edges(st, conic_rel=KNIFE_CONIC_REL, exp_rel=KNIFE_EXP_REL, xy_abs=0.0):
+    """Where a blend whose decisions are within the error bound above of the oracle's may decide otherwise.
+
+    From the float32 oracle state, per (instance, pixel) pair of every tile:
+      * knife pairs: `power` within the bound of 0, or `alpha` within it of 1/255 (accepted on one side, skipped on
+        the other);
+      * the walk under the oracle's decisions: T after each accepted pair (float32, the blend's order) with a relative
+        error bound that sums, over the accepted pairs in front, alpha/(1-alpha) times their alpha's error (zero where
+        o G clears the 0.99 clamp by the bound) plus one rounding, and alpha/(1-alpha) in full for every knife pair (a
+        flip multiplies T by 1-alpha or its inverse).  A pair is REACHED unless an accepted pair in front ends the
+        walk (T < 1e-4) by more than that bound;
+      * knife pixels: a reached knife pair, or a reached accepted pair whose T is within its bound of 1e-4.
+    A flip in a knife pixel moves T for the splats behind it and the colour composited behind the splats in front of
+    it, so every splat with a reached accepted or knife pair in a knife pixel is affected.
+
+    `xy_abs` bounds the error of the pixel-space centre (0 when both sides share the preprocess's float32 centre;
+    float64 models pass their own).  Returns a dict: `pixels` (H, W) and `splats` (P,) boolean masks, `pairs` (number
+    of knife pairs; `ill`, the splats of the KNIFE_COND class, which `affected` adds for the covariance chain's
+    gradients only), and the oracle's own `n_contrib` and `final_T` restated from the walk (a check of the restatement).
+    """
+    W, H = st.W, st.H
+    gx = (W + 15) // 16
+    pixels = np.zeros(H * W, bool)
+    splats = np.zeros(st.P, bool)
+    n_contrib = np.zeros(H * W, np.int64)
+    final_T = np.ones(H * W, F32)
+    n_pairs = 0
+    ly, lx = np.meshgrid(np.arange(16), np.arange(16), indexing="ij")
+    for tile in range(st.ranges.shape[0]):
+        r0, r1 = int(st.ranges[tile, 0]), int(st.ranges[tile, 1])
+        if r1 <= r0:
+            continue
+        xs, ys = (tile % gx) * 16 + lx.reshape(-1), (tile // gx) * 16 + ly.reshape(-1)
+        inside = (xs < W) & (ys < H)
+        xs, ys = xs[inside], ys[inside]
+        pix = ys * W + xs
+        ids = st.vals_sorted[r0:r1].astype(np.int64)
+        co = st.conic_opacity[ids]
+        dx = st.xy[ids, 0][:, None] - xs[None, :].astype(F32)
+        dy = st.xy[ids, 1][:, None] - ys[None, :].astype(F32)
+        power = F32(-0.5) * (co[:, 0:1] * dx * dx + co[:, 2:3] * dy * dy) - co[:, 1:2] * dx * dy
+        og = co[:, 3:4] * np.exp(np.minimum(power, F32(0)).astype(np.float64)).astype(F32)   # expf, correctly rounded
+        alpha = np.minimum(F32(0.99), og)
+        acc = (power <= 0) & (alpha >= ALPHA_MIN)
+        A, B, C = (co[:, k:k + 1].astype(np.float64) for k in range(3))
+        dx64, dy64 = dx.astype(np.float64), dy.astype(np.float64)
+        Q = 0.5 * np.abs(A) * dx64 ** 2 + np.abs(B * dx64 * dy64) + 0.5 * np.abs(C) * dy64 ** 2
+        dpow = conic_rel * Q + xy_abs * (np.abs(A * dx64 + B * dy64) + np.abs(B * dx64 + C * dy64))
+        rel = np.where(Q == 0, 0.0, dpow + exp_rel)          # relative error bound of G, hence of o G
+        a64 = alpha.astype(np.float64)
+        knife = ((Q > 0) & (np.abs(power) <= dpow)) | ((power <= dpow) & (np.abs(a64 - float(ALPHA_MIN)) < a64 * rel))
+        odds = a64 / (1.0 - a64)
+        firm = og.astype(np.float64) * (1.0 - rel) >= 0.99   # on the clamp on both sides
+        d = np.where(acc, np.where(firm, 0.0, odds * rel) + 2.0 ** -23, 0.0) + np.where(knife, odds, 0.0)
+        T = np.cumprod(np.where(acc, F32(1) - alpha, F32(1)), axis=0, dtype=F32)   # T after each pair
+        margin = T.astype(np.float64) * np.expm1(np.cumsum(d, axis=0))
+        ends = acc & (T.astype(np.float64) + margin < float(T_STOP))
+        reached = np.cumsum(ends, axis=0) - ends == 0        # no accepted pair in front ends the walk for sure
+        near_stop = acc & reached & (np.abs(T.astype(np.float64) - float(T_STOP)) <= margin)
+        kpix = (knife & reached).any(0) | near_stop.any(0)
+        pixels[pix] |= kpix
+        hit = ((acc | knife) & reached)[:, kpix].any(1)
+        splats[ids[hit]] = True
+        n_pairs += int((knife & reached).sum())
+        # the oracle's walk itself: it stops at the first accepted pair that takes T below 1e-4
+        stop = acc & (T < T_STOP)
+        live = np.cumsum(stop, axis=0) == 0
+        took = acc & live
+        last = np.where(took.any(0), took.shape[0] - np.argmax(took[::-1], axis=0), 0)
+        n_contrib[pix] = last
+        final_T[pix] = np.where(took.any(0), T[np.maximum(last - 1, 0), np.arange(pix.size)], F32(1))
+    c = st.cov3D.astype(np.float64)
+    S = np.stack([c[:, [0, 1, 2]], c[:, [1, 3, 4]], c[:, [2, 4, 5]]], 1)
+    ev = np.abs(np.linalg.eigvalsh(S))
+    ill = (st.radii > 0) & (ev[:, 2] > KNIFE_COND * ev[:, 0])
+    return dict(pixels=pixels.reshape(H, W), splats=splats, ill=ill, pairs=n_pairs,
+                n_contrib=n_contrib.reshape(H, W), final_T=final_T.reshape(H, W))
+
+
+# the gradients that pass through the covariance and conic chain of the preprocess (activated and bound names)
+COV_CHAIN = {"means3D", "scales", "rotations", "cov3D_precomp", "_xyz", "_scaling", "_rotation"}
+
+
+def affected(ke, name):
+    """The splats knife_edges explains for the gradient `name`: the knife splats, and for the tensors of the
+    covariance chain also the ill-conditioned ones (the blend's own outputs -- means2D, opacity, colour -- do not
+    pass through that chain, so no condition number explains an error in them)."""
+    return ke["splats"] | ke["ill"] if name in COV_CHAIN else ke["splats"]
+
+
 def accepted_instances(st):
     """Stream positions j the oracle's blend took into some pixel (power <= 0, alpha >= 1/255, before n_contrib)."""
     t = pair_table(st)

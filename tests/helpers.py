@@ -75,6 +75,68 @@ def assert_grad_tight(g_cuda, g_ref, what="", rtol=GRAD_RTOL, atol_frac=GRAD_ATO
     return s
 
 
+# Explained gates: the outliers the gates above let through by count must each sit where a threshold decision can
+# flip (tests/adversarial_scenes.py::knife_edges).  Every entry outside that set is within the tolerance, without
+# exception; the entries inside it keep the cap.
+def _affected(mask, shape):
+    mask = np.asarray(mask, bool)
+    return np.broadcast_to(mask.reshape(mask.shape + (1,) * (len(shape) - mask.ndim)), shape)
+
+
+def assert_grad_explained(g_cuda, g_ref, affected, what="", rtol=GRAD_RTOL, atol_frac=GRAD_ATOL_FRAC, cap=GRAD_CAP,
+                          knife_allowed=None):
+    """`affected`: boolean mask of the entries a knife edge explains, of the tensor's shape or of its leading
+    dimensions (the (P,) splat mask of knife_edges).  The affected entries keep assert_grad_tight's allowance: at
+    most `knife_allowed` (default max(8, GRAD_OUTLIER_FRAC n)) beyond the tolerance, none beyond `cap` max|ref|."""
+    g_ref = np.asarray(g_ref, np.float64)
+    g_cuda = np.asarray(g_cuda, np.float64).reshape(g_ref.shape)
+    aff = _affected(affected, g_ref.shape)
+    scale = float(np.abs(g_ref).max()) + 1e-300 if g_ref.size else 1.0
+    d = np.abs(g_cuda - g_ref)
+    ratio = d / (atol_frac * scale + rtol * np.abs(g_ref))
+    free = ratio[~aff]
+    worst_free = float(free.max()) if free.size else 0.0
+    worst_knife = float(d[aff].max() / scale) if aff.any() else 0.0
+    n_bad = int((free > 1.0).sum())
+    print(f"[grad] {what:<28s} n={d.size:>9d} max|ref|={scale:.3e} knife={int(aff.sum())} "
+          f"tol-ratio worst={worst_free:.2e} outside the knife set, knife worst|d|/max|ref|={worst_knife:.2e} "
+          f"unexplained={n_bad}")
+    assert np.isfinite(g_cuda).all(), f"{what}: non-finite gradient"
+    if n_bad:
+        at = np.unravel_index(int(np.argmax(np.where(aff, -1.0, ratio))), ratio.shape)
+        raise AssertionError(f"{what}: {n_bad}/{d.size} entries outside the knife set beyond atol+rtol|ref| (rtol {rtol}, "
+                             f"atol {atol_frac} max|ref|); worst ratio {worst_free:.3e} at {tuple(map(int, at))}: "
+                             f"{g_cuda[at]:.6e} vs {g_ref[at]:.6e}")
+    assert worst_knife <= cap, f"{what}: a knife entry off by {worst_knife:.3e} of max|ref| (cap {cap})"
+    allowed = max(8, int(GRAD_OUTLIER_FRAC * d.size)) if knife_allowed is None else knife_allowed
+    n_knife = int((ratio[aff] > 1.0).sum())
+    assert n_knife <= allowed, f"{what}: {n_knife} knife entries beyond atol+rtol|ref| (allowed {allowed})"
+    return dict(n=int(d.size), knife=int(aff.sum()), worst=worst_free, knife_worst=worst_knife)
+
+
+def assert_image_explained(img_cuda, img_ref, knife_pixels, what="", tol=IMG_TOL, cap=KNIFE_ABS, frac=KNIFE_FRAC):
+    """Every value of a pixel outside `knife_pixels` ((H, W), broadcast over leading channels) within `tol`; the knife
+    pixels keep assert_image_close's allowance: at most max(2, frac n) values beyond `tol`, none beyond `cap`."""
+    img_ref = np.asarray(img_ref, np.float64)
+    d = np.abs(np.asarray(img_cuda, np.float64).reshape(img_ref.shape) - img_ref)
+    kp = np.asarray(knife_pixels, bool)
+    aff = np.broadcast_to(kp.reshape((1,) * (d.ndim - kp.ndim) + kp.shape), d.shape)
+    free = d[~aff]
+    worst_free = float(free.max()) if free.size else 0.0
+    worst_knife = float(d[aff].max()) if aff.any() else 0.0
+    n_bad = int((free > tol).sum())
+    print(f"[image] {what:<28s} n={d.size:>9d} knife pixels={int(kp.sum())} max|d| outside={worst_free:.3e} "
+          f"knife max|d|={worst_knife:.3e} unexplained={n_bad}")
+    if n_bad:
+        at = np.unravel_index(int(np.argmax(np.where(aff, -1.0, d))), d.shape)
+        raise AssertionError(f"{what}: {n_bad}/{d.size} values outside the knife pixels differ by more than {tol}; "
+                             f"worst {worst_free:.3e} at {tuple(map(int, at))}")
+    assert worst_knife <= cap, f"{what}: a knife pixel off by {worst_knife:.3e} (cap {cap})"
+    n_knife = int((d[aff] > tol).sum())
+    assert n_knife <= max(2, frac * d.size), f"{what}: {n_knife} knife-pixel values differ by more than {tol}"
+    return worst_free, worst_knife
+
+
 def image_stats(img_cuda: np.ndarray, img_ref: np.ndarray):
     d = np.abs(img_cuda.astype(np.float64) - img_ref.astype(np.float64))
     return dict(max_abs=float(d.max()), n_over_1e4=int((d > IMG_TOL).sum()), n=int(d.size))

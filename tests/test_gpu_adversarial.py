@@ -9,8 +9,9 @@ Schedule matrix (full cross product, 24 schedules; every test of this file runs 
                             on every tile of 32 or more entries)
 Per scene and schedule: radii bit-exact; the sorted stream bit-exact (exact binning) or an order-preserving
 subsequence keeping every instance the oracle's blend accepted (culled); image and final_T within the parity budget
-and the image bit-identical across all schedules; every input gradient within the tight gate of the oracle's and of
-the first schedule's, exactly zero for splats without an instance and for clamped colour channels; on the ragged sizes
+and the image bit-identical across all schedules; every input gradient within the explained gate
+(helpers.assert_grad_explained: no entry beyond the tolerance outside adversarial_scenes.knife_edges) of the oracle's
+and of the first schedule's, exactly zero for splats without an instance and for clamped colour channels; on the ragged sizes
 the display bytes equal render.py's quantisation, and (first schedule) image and gradients equal float64 autograd of
 the dense model."""
 import numpy as np
@@ -80,7 +81,10 @@ def _reference(case):
         st = h.oracle_forward(sc)
         gout = torch.randn(3, sc["H"], sc["W"], generator=torch.Generator().manual_seed(7))
         g = h.oracle_backward(sc, st, gout.numpy())
-        _REF[case] = dict(sc=sc, st=st, gout=gout, g=g, accepted=A.accepted_instances(st))
+        ke = A.knife_edges(st)
+        print(f"[knife] {_cid(case)}: {ke['pairs']} pairs, {int(ke['pixels'].sum())} pixels, "
+              f"{int(ke['splats'].sum())}/{st.P} splats")
+        _REF[case] = dict(sc=sc, st=st, gout=gout, g=g, accepted=A.accepted_instances(st), ke=ke)
     return _REF[case]
 
 
@@ -157,7 +161,7 @@ def _quant(img):
 @pytest.mark.parametrize("case", CASES, ids=_cid)
 def test_adversarial_scene(case, schedule):
     ref = _reference(case)
-    sc, st, g_ref = ref["sc"], ref["st"], ref["g"]
+    sc, st, g_ref, ke = ref["sc"], ref["st"], ref["g"], ref["ke"]
     what = f"{_cid(case)} [{_sid(schedule)}]"
     out = _run(sc, schedule, ref["gout"])
 
@@ -184,12 +188,12 @@ def test_adversarial_scene(case, schedule):
     img = out["img"].cpu().numpy()
     s = h.image_stats(img, st.out_color)
     print(f"[image] {what:<60s} max|d|={s['max_abs']:.3e} >1e-4: {s['n_over_1e4']}/{s['n']}")
-    h.assert_image_close(img, st.out_color, f"{what}: image")
+    h.assert_image_explained(img, st.out_color, ke["pixels"], f"{what}: image")
     # 4. final_T
-    h.assert_image_close(out["T"], np.broadcast_to(st.final_T, out["T"].shape), f"{what}: final_T")
+    h.assert_image_explained(out["T"], np.broadcast_to(st.final_T, out["T"].shape), ke["pixels"], f"{what}: final_T")
     # 5. gradients
     for k, g in out["grads"].items():
-        h.assert_grad_tight(g, g_ref[k], f"{_cid(case)} dL/d{k}")
+        h.assert_grad_explained(g, g_ref[k], A.affected(ke, k), f"{_cid(case)} dL/d{k}")
     invis = st.radii == 0
     for k, g in out["grads"].items():
         assert not np.any(g[invis]), f"{what}: dL/d{k} nonzero for a splat without an instance"
@@ -202,7 +206,7 @@ def test_adversarial_scene(case, schedule):
     first = _FIRST.setdefault(case, (schedule, out["img"], out["grads"]))
     assert torch.equal(out["img"], first[1]), f"{what}: image differs from schedule [{_sid(first[0])}]"
     for k, g in out["grads"].items():
-        h.assert_grad_tight(g, first[2][k], f"{_cid(case)} dL/d{k} vs first schedule")
+        h.assert_grad_explained(g, first[2][k], A.affected(ke, k), f"{_cid(case)} dL/d{k} vs first schedule")
     if case[1] is None:
         return
     # 6. display bytes (ragged sizes)
@@ -214,6 +218,6 @@ def test_adversarial_scene(case, schedule):
         from tests.test_oracle_adversarial import dense_image_and_grads
 
         img64, g64 = dense_image_and_grads(sc, st, seed=7)
-        h.assert_image_close(img, img64, f"{what}: image vs float64")
+        h.assert_image_explained(img, img64, ke["pixels"], f"{what}: image vs float64")
         for k, g in out["grads"].items():
-            h.assert_grad_tight(g, g64[k], f"{_cid(case)} dL/d{k} vs float64")
+            h.assert_grad_explained(g, g64[k], A.affected(ke, k), f"{_cid(case)} dL/d{k} vs float64")

@@ -291,10 +291,17 @@ def test_plain_backward_on_a_depth_alpha_state_is_the_colour_backward(monkeypatc
 def test_planes_and_gradients_against_the_oracle_and_float64_at_ragged_sizes(name, W, H):
     """Plain GaussianModel inputs (binding=None): the planes against the C-oracle composition (tests/planes64.py),
     dL/d_xyz and dL/dmeans2D of <alpha, ga> + <depth, gd> against float64 autograd of the dense model."""
+    from tests import adversarial_scenes as A
+    planes_against_the_oracle_and_float64(A.build(name, W, H), f"{name} {W}x{H}")
+
+
+def planes_against_the_oracle_and_float64(sc, what):
+    """The check of the test above on the activated scene `sc`, under the explained gates of tests/helpers.py (the
+    knife set of adversarial_scenes.knife_edges on the oracle's state)."""
     from gaussianavatars_b200.rasterizer import bind_activate, rasterize_bound
     from tests import adversarial_scenes as A
     from tests import planes64 as P64
-    sc = A.build(name, W, H)
+    W, H = sc["W"], sc["H"]
     P = sc["means3D"].shape[0]
     shs = sc["shs"].to(DEV)
     leaves = [sc["means3D"].to(DEV).clone().requires_grad_(True), sc["rotations"].to(DEV),
@@ -313,9 +320,13 @@ def test_planes_and_gradients_against_the_oracle_and_float64_at_ragged_sizes(nam
     act = dict(means3D=m.cpu(), opacities=op.cpu(), scales=s.cpu(), rotations=rot.contiguous())
     a_o, d_o, st = P64.oracle_planes(act["means3D"].numpy(), act["opacities"].numpy(), sc["cam"], W, H,
                                      scales=act["scales"].numpy(), rotations=act["rotations"].numpy())
-    h.assert_image_close(alpha.detach().cpu().numpy(), a_o, f"{name} {W}x{H}: alpha vs oracle")
+    ke = A.knife_edges(st)
+    print(f"[knife] {what}: {ke['pairs']} pairs, {int(ke['pixels'].sum())} pixels, {int(ke['splats'].sum())}/{P} "
+          f"splats, {int(ke['ill'].sum())} ill-conditioned")
+    h.assert_image_explained(alpha.detach().cpu().numpy(), a_o, ke["pixels"], f"{what}: alpha vs oracle")
     dscale = max(1.0, float(abs(d_o).max()))
-    h.assert_image_close(depth.detach().cpu().numpy() / dscale, d_o / dscale, f"{name} {W}x{H}: depth vs oracle")
+    h.assert_image_explained(depth.detach().cpu().numpy() / dscale, d_o / dscale, ke["pixels"],
+                             f"{what}: depth vs oracle")
     cam = sc["cam"]
     t64 = {k: v.double().clone().requires_grad_(k == "means3D") for k, v in act.items()}
     m64 = torch.zeros((P, 3), dtype=torch.float64, requires_grad=True)
@@ -326,8 +337,10 @@ def test_planes_and_gradients_against_the_oracle_and_float64_at_ragged_sizes(nam
                                 radii=torch.from_numpy(st.radii).long(), rect_xy=torch.from_numpy(st.xy),
                                 depths=torch.from_numpy(st.depths))
     ((a64 * ga.double()).sum() + (d64 * gd.double()).sum()).backward()
-    h.assert_grad_tight(leaves[0].grad.double().cpu().numpy(), t64["means3D"].grad.numpy(), f"{name} {W}x{H}: _xyz")
-    h.assert_grad_tight(m2.grad.double().cpu().numpy(), m64.grad.numpy(), f"{name} {W}x{H}: means2D")
+    h.assert_grad_explained(leaves[0].grad.double().cpu().numpy(), t64["means3D"].grad.numpy(),
+                            A.affected(ke, "_xyz"), f"{what}: _xyz")
+    h.assert_grad_explained(m2.grad.double().cpu().numpy(), m64.grad.numpy(), A.affected(ke, "means2D"),
+                            f"{what}: means2D")
 
 
 def test_depth_and_alpha_gradients_reach_the_flame_parameters():

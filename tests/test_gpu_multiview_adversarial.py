@@ -29,6 +29,7 @@ from tests import adversarial_scenes as A
 from tests import bound_rigs as B
 from tests import helpers as h
 from tests import train_step_oracle as T
+from tests import walk_scenes as WS
 from tests.test_oracle_multiview_adversarial import MAIN, scene
 
 pytestmark = pytest.mark.gpu
@@ -291,8 +292,9 @@ def _dense_sum(case, K):
     return out
 
 
-def _gate_all(what, got, raw, verts, m2d_rows, K, slack):
-    """Summed raw gradients and each valid view's dL/dmeans2D row under assert_grad_tight, dL/dverts under
+def _gate_all(what, got, raw, verts, m2d_rows, K, slack, kes):
+    """Summed raw gradients and each valid view's dL/dmeans2D row under assert_grad_explained (the knife set of a raw
+    gradient is the union of the valid views' knife_edges; of a view's row, that view's), dL/dverts under
     train_step_oracle.gate_vertex.  An array the fixed gate rejects passes only if its largest error stays within
     `slack` of it: twice the error of the reference's own float32 chain (_reference32) against the float64 one, the
     rule of test_gpu_train_step.  A needle's covariance has a condition number near 1e6, and any float32 route from
@@ -302,9 +304,13 @@ def _gate_all(what, got, raw, verts, m2d_rows, K, slack):
         e_c = float(np.abs(np.asarray(a, np.float64) - ref).max())
         print(f"[grad] {what} {name} beyond the fixed gate: max|d| {e_c:.3e}, 2 x float32 reference {slack[name]:.3e}")
         assert e_c <= slack[name], f"{what}: {name} beyond the gate and beyond twice the float32 reference's error"
+    live = [ke for ke in kes if ke is not None]
     for k in B.RAW:
+        aff = np.zeros(got["grads"][k].shape[0], bool)
+        for ke in live:
+            aff |= A.affected(ke, k)
         try:
-            h.assert_grad_tight(got["grads"][k], raw[k], f"{what} d{k}")
+            h.assert_grad_explained(got["grads"][k], raw[k], aff, f"{what} d{k}")
         except AssertionError:
             fallback(k, got["grads"][k], raw[k])
     rec = T.gate_vertex(f"{what} dverts", got["verts"], verts)
@@ -314,7 +320,8 @@ def _gate_all(what, got, raw, verts, m2d_rows, K, slack):
         fallback("verts", got["verts"], verts)
     for k in range(K):
         if m2d_rows[k] is not None:
-            h.assert_grad_tight(got["m2d"][k], m2d_rows[k], f"{what} dmeans2D view {k}")
+            aff = np.zeros(m2d_rows[k].shape[0], bool) if kes[k] is None else A.affected(kes[k], "means2D")
+            h.assert_grad_explained(got["m2d"][k], m2d_rows[k], aff, f"{what} dmeans2D view {k}")
 
 
 def _check(case, K, sched):
@@ -324,6 +331,9 @@ def _check(case, K, sched):
     out = _views(case, K, sched)
     singles = [_single(case, k) for k in range(K)]
     P = bound["params"]["_xyz"].shape[0]
+    kes = [None if st is None else A.knife_edges(st) for st in c["sts"][:K]]
+    print(f"[knife] {what}: " + ", ".join("-" if ke is None else f"{int(ke['pixels'].sum())} px/{int(ke['splats'].sum())} "
+                                          f"splats" for ke in kes))
     if sched[1] == 0 and any(s is not None and (s.radii > 0).any() for s in c["sts"][:K]):
         assert out["path"] != 0, f"{what}: the hinted frame did not take the bucket depth sort"
 
@@ -341,7 +351,8 @@ def _check(case, K, sched):
             assert torch.equal(out["img"][k], bg), f"{what}: the invalid-FoV view is not the background"
             continue
         assert np.array_equal(radii, st.radii), f"{what}: view {k} radii differ from the C oracle"
-        h.assert_image_close(out["img"][k].cpu().numpy(), st.out_color, f"{what}: view {k} image vs oracle")
+        h.assert_image_explained(out["img"][k].cpu().numpy(), st.out_color, kes[k]["pixels"],
+                                 f"{what}: view {k} image vs oracle")
     first = _FIRST.setdefault((case, K), (sched, out["img"]))
     assert torch.equal(out["img"], first[1]), f"{what}: images differ from schedule [{_sid(first[0])}]"
 
@@ -354,17 +365,17 @@ def _check(case, K, sched):
     # 2. against K single-view steps, summed
     raw = {k: sum(s["grads"][k] for s in singles) for k in B.RAW}
     _gate_all(f"{_cid(case)} K={K} vs singles", out, raw, sum(s["verts"] for s in singles),
-              [s["m2d"] for s in singles], K, slack)
+              [s["m2d"] for s in singles], K, slack, kes)
 
     # 3. against the C oracle per view, pulled back in float64
     _gate_all(f"{_cid(case)} K={K} vs oracle", out, raw_o, verts_o,
-              [None if g is None else g["means2D"] for g in c["gs"][:K]], K, slack)
+              [None if g is None else g["means2D"] for g in c["gs"][:K]], K, slack, kes)
 
     # 4. against float64 (ragged sizes, first schedule)
     if case[1] is not None and sched == FIRST:
         raw_d, verts_d, m2d_d = _dense_sum(case, K)
         _gate_all(f"{_cid(case)} K={K} vs float64", out, raw_d, verts_d,
-                  [None if c["sts"][k] is None else m2d_d[k] for k in range(K)], K, slack)
+                  [None if c["sts"][k] is None else m2d_d[k] for k in range(K)], K, slack, kes)
 
     # 5. exact zeros
     radii = out["radii"].cpu().numpy()                                        # (K, P)
@@ -410,4 +421,12 @@ def test_main_cases_other_view_counts(case, K, schedule):
 @pytest.mark.parametrize("schedule", [FIRST, RAGGED_SECOND], ids=_sid, indirect=True)
 @pytest.mark.parametrize("case", RAGGED, ids=_cid)
 def test_ragged_sizes_six_views(case, schedule):
+    _check(case, 6, schedule)
+
+
+@pytest.mark.parametrize("schedule", [FIRST, (0, 1, True, "bwd32")], ids=_sid, indirect=True)
+@pytest.mark.parametrize("case", [("walk:" + n, None, None) for n in WS.WALK], ids=_cid)
+def test_walk_scenes_six_views(case, schedule):
+    """The walk scenes bound to a rig: a K-view backward whose global tile order interleaves the views
+    (tests/test_oracle_walk.py), light-only and with K = 2 on every tile of 32 or more entries."""
     _check(case, 6, schedule)

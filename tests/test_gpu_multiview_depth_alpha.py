@@ -21,6 +21,7 @@ import numpy as np
 import pytest
 import torch
 
+from tests import adversarial_scenes as A
 from tests import bound_rigs as B
 from tests import helpers as h
 from tests import train_step_oracle as T
@@ -395,7 +396,8 @@ def test_planes_and_summed_gradients_against_float64_at_ragged_sizes(name, W, H)
     raw = {k: z(t, lv[k]) for k, t in zip(B.RAW, g64[:6])}
     rows = [None if c["sts"][k] is None else z(g64[7 + k], m2ds[k]) for k in range(K)]
     slack = {k: 0.0 for k in list(B.RAW) + ["verts"]}   # no fallback: the fixed gates only
-    _gate_all(f"{name}-{W}x{H} K={K} planes vs float64", got, raw, z(g64[6], vv), rows, K, slack)
+    kes = [None if st is None else A.knife_edges(st) for st in c["sts"][:K]]
+    _gate_all(f"{name}-{W}x{H} K={K} planes vs float64", got, raw, z(g64[6], vv), rows, K, slack, kes)
 
 
 # ---- 5. FLAME -------------------------------------------------------------------------------------------------------

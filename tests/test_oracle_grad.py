@@ -6,6 +6,7 @@ import torch
 
 from oracle import dense64
 from oracle import rasterizer as orc
+from tests import adversarial_scenes as A
 from tests import helpers as h
 
 
@@ -36,7 +37,8 @@ def test_oracle_backward_equals_float64_autograd(deg, seed, mod):
     t64 = _leaf64(scene, ("means3D", "opacities", "scales", "rotations", "shs"))
     m2 = torch.zeros(P, 3, dtype=torch.float64, requires_grad=True)
     img, _ = _dense(scene, t64, m2, torch.from_numpy(st.radii).long(), scale_modifier=mod)
-    assert np.abs(img.detach().float().numpy() - st.out_color).max() < 5e-6
+    ke = A.knife_edges(st)
+    h.assert_image_explained(st.out_color, img.detach().numpy(), ke["pixels"], "oracle image vs float64", tol=5e-6, cap=5e-6)
     gout = torch.randn(3, H, W, generator=torch.Generator().manual_seed(1))
     img.backward(gout.double())
     g = orc.backward(st, gout.numpy(), scene["means3D"].numpy(), cam.world_view_transform.numpy(),
@@ -44,7 +46,7 @@ def test_oracle_backward_equals_float64_autograd(deg, seed, mod):
                      scene["bg"].numpy(), **kw)
     for name, ref in [("means3D", t64["means3D"].grad), ("means2D", m2.grad), ("opacities", t64["opacities"].grad),
                       ("scales", t64["scales"].grad), ("rotations", t64["rotations"].grad), ("shs", t64["shs"].grad)]:
-        h.assert_grad_close(g[name], ref.numpy(), f"oracle dL/d{name}", rtol=2e-5, frac=0.0)
+        h.assert_grad_explained(g[name], ref.numpy(), A.affected(ke, name), f"oracle dL/d{name}", rtol=0.0, atol_frac=2e-5, knife_allowed=3)
 
 
 def test_oracle_backward_precomputed_routes():
@@ -68,9 +70,10 @@ def test_oracle_backward_precomputed_routes():
     gout = torch.randn(3, H, W, generator=torch.Generator().manual_seed(3))
     img.backward(gout.double())
     g = orc.backward(st, gout.numpy(), scene["means3D"].numpy(), *args, cam.tanfovx, cam.tanfovy, scene["bg"].numpy())
-    h.assert_grad_close(g["colors_precomp"], c64.grad.numpy(), "dL/dcolors", rtol=2e-5, frac=0.0)
-    h.assert_grad_close(g["cov3D_precomp"], v64.grad.numpy(), "dL/dcov3D", rtol=5e-5, frac=0.0)
-    h.assert_grad_close(g["means3D"], t64["means3D"].grad.numpy(), "dL/dmeans3D", rtol=5e-5, frac=0.0)
+    ke = A.knife_edges(st)
+    h.assert_grad_explained(g["colors_precomp"], c64.grad.numpy(), A.affected(ke, "colors_precomp"), "dL/dcolors", rtol=0.0, atol_frac=2e-5, knife_allowed=3)
+    h.assert_grad_explained(g["cov3D_precomp"], v64.grad.numpy(), A.affected(ke, "cov3D_precomp"), "dL/dcov3D", rtol=0.0, atol_frac=5e-5, knife_allowed=3)
+    h.assert_grad_explained(g["means3D"], t64["means3D"].grad.numpy(), A.affected(ke, "means3D"), "dL/dmeans3D", rtol=0.0, atol_frac=5e-5, knife_allowed=3)
 
 
 def test_oracle_gradient_against_float64_finite_differences():

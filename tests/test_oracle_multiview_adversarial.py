@@ -28,6 +28,9 @@ def scene(case):
     """The activated scene of a case: the builders of tests/adversarial_scenes.py; the main saturating stack also
     holds a 2100-splat stack (beyond the 1984 / 2048 blend thresholds)."""
     name, W, H = case
+    if name.startswith("walk:"):      # the walk scenes of tests/walk_scenes.py
+        from tests import walk_scenes as WS
+        return WS.build(name[5:])
     if name == "saturating_stack" and W is None:
         sc = A.saturating_stack(stacks=(20, 400, 2100))
         sc["name"] = name
