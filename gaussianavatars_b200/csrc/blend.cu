@@ -470,22 +470,25 @@ void launch_blend_forward(int views, int W, int H, const uint2* ranges, const ui
 // Backward
 // =====================================================================================================
 // Per-pixel state of the reverse walk (K pixels per lane, one per band).
+// U is the dL/dpixel-weighted sum of everything behind the splat being visited, T_j included:
+//   U_i = sum_{j>i} (c_j . d) alpha_j T_j + T_final (bg . d)        (d = dL/dpixel)
+// so the reference's T_i ((c_i - colour behind) . d) - T_final (bg . d) / (1 - alpha_i) is T_i (c_i . d) - U_i / (1 -
+// alpha_i), and one scalar per pixel replaces the three composited channels.
 template <int K>
 struct PixState {
   float fy[K];                // pixel row as float
   float T[K];                 // transmittance in front of the splat being visited (starts at final_T)
-  float ar[K], ag[K], ab[K];  // colour composited behind the splat being visited
+  float U[K];                 // sum behind the splat being visited (starts at final_T * (bg . dL/dpixel))
   float dr[K], dg[K], db[K];  // dL/dpixel
-  float bgT[K];               // final_T * (bg . dL/dpixel)  (DA: final_T * (bg . dL/dpixel - dL/dalpha))
   int nc[K];                  // n_contrib: only list positions below it contributed to the pixel
 };
-struct SplatSums {  // per-lane sums over the lane's pixels for one splat
-  float S0, S1, S2, go, gr, gg, gb;
+struct SplatSums {  // per-lane sums over the lane's pixels for one splat; go = sum t, S1 = sum t dy, S2 = sum t dy^2
+  float S1, S2, go, gr, gg, gb;  // with t = G dL/dalpha (dL/dG = opacity t: the opacity is applied once per visit)
 };
-// DA (depth plane): a fourth channel with colour z and background 0, and dL/dalpha folded into bgT
+// DA (depth plane): a fourth channel with colour z and background 0, z dL/ddepth in c . d, and alpha = 1 - T_final
+// puts -T_final dL/dalpha into U's start
 template <int K>
 struct PixStateDA : PixState<K> {
-  float az[K];  // depth composited behind the splat being visited
   float dD[K];  // dL/ddepth
 };
 struct SplatSumsDA : SplatSums {
@@ -500,13 +503,15 @@ using SplatSumsT = std::conditional_t<DA, SplatSumsDA, SplatSums>;
 // dependency chains are independent and interleave.  A lane whose pixel did not receive this splat in the forward
 // (beyond its n_contrib, outside the footprint, alpha < 1/255) runs the same instructions with alpha = G = 0 and
 // T multiplied by exactly 1: every one of its contributions is an exact zero.
-template <int K, int M, bool DA = false>
+// FRESH: s holds nothing yet and the lowest band of M sets each sum instead of adding to it (no add of a zero).
+template <int K, int M, bool DA = false, bool FRESH = false>
 __device__ __forceinline__ void visit_bands(PixStateT<K, DA>& p, int pos, float py, float tA, float dx, float Bp,
                                             float Cp, float op, float cr, float cg, float cb, SplatSumsT<DA>& s,
                                             float cz = 0.f) {
 #pragma unroll
   for (int i = 0; i < K; i++) {
     if (!((M >> i) & 1)) continue;
+    const bool set = FRESH && (1 << i) == (M & -M);
     const float dy = py - p.fy[i];
     const float pw = fmaf(Cp * dy, dy, fmaf(Bp, dy, tA) * dx);  // the forward's expression, bit for bit
     const float G = ex2_approx(pw);
@@ -518,33 +523,24 @@ __device__ __forceinline__ void visit_bands(PixStateT<K, DA>& p, int pos, float 
     const float Tn = p.T[i] * ra;  // transmittance in FRONT of this splat
     p.T[i] = Tn;
     const float w = al * Tn;
-    s.gr = fmaf(w, p.dr[i], s.gr);
-    s.gg = fmaf(w, p.dg[i], s.gg);
-    s.gb = fmaf(w, p.db[i], s.gb);
-    // dL/dalpha = T * sum_ch (c - colour behind) dpix  -  T_final/(1-alpha) * (bg . dpix)
-    const float er = cr - p.ar[i], eg = cg - p.ag[i], eb = cb - p.ab[i];
-    float dLda = er * p.dr[i];
-    dLda = fmaf(eg, p.dg[i], dLda);
-    dLda = fmaf(eb, p.db[i], dLda);
-    float ez = 0.f;
+    s.gr = set ? w * p.dr[i] : fmaf(w, p.dr[i], s.gr);
+    s.gg = set ? w * p.dg[i] : fmaf(w, p.dg[i], s.gg);
+    s.gb = set ? w * p.db[i] : fmaf(w, p.db[i], s.gb);
+    // dL/dalpha = T (c . dpix) - U / (1 - alpha)
+    float cd = cr * p.dr[i];
+    cd = fmaf(cg, p.dg[i], cd);
+    cd = fmaf(cb, p.db[i], cd);
     if constexpr (DA) {
-      ez = cz - p.az[i];
-      dLda = fmaf(ez, p.dD[i], dLda);
-      s.gz = fmaf(w, p.dD[i], s.gz);
+      cd = fmaf(cz, p.dD[i], cd);
+      s.gz = set ? w * p.dD[i] : fmaf(w, p.dD[i], s.gz);
     }
-    dLda = fmaf(dLda, Tn, -p.bgT[i] * ra);
-    // colour behind the NEXT (nearer) splat: this one composited over what was behind it
-    p.ar[i] = fmaf(al, er, p.ar[i]);
-    p.ag[i] = fmaf(al, eg, p.ag[i]);
-    p.ab[i] = fmaf(al, eb, p.ab[i]);
-    if constexpr (DA) p.az[i] = fmaf(al, ez, p.az[i]);
+    const float dLda = fmaf(Tn, cd, -p.U[i] * ra);
+    p.U[i] = fmaf(w, cd, p.U[i]);  // the sum behind the NEXT (nearer) splat
     const float t = Gv * dLda;  // G dL/dalpha
-    s.go += t;
-    const float s_ = op * t;    // G dL/dG
-    const float sd = s_ * dy;
-    s.S0 += s_;
-    s.S1 += sd;
-    s.S2 = fmaf(sd, dy, s.S2);
+    const float sd = t * dy;
+    s.go = set ? t : s.go + t;
+    s.S1 = set ? sd : s.S1 + sd;
+    s.S2 = set ? sd * dy : fmaf(sd, dy, s.S2);
   }
 }
 
@@ -622,7 +618,6 @@ __device__ __forceinline__ void backward_task(int tile, int tl, WarpSmemT<DA ? 1
   for (int i = 0; i < K; i++) {
     const int y = pixy0 + 4 * i;
     p.fy[i] = (float)y;
-    p.ar[i] = p.ag[i] = p.ab[i] = 0.f;
     float T0 = 0.f, dr = 0.f, dg = 0.f, db = 0.f, dA = 0.f, dZ = 0.f;
     p.nc[i] = 0;
     if (pixx < W && y < H) {
@@ -642,11 +637,10 @@ __device__ __forceinline__ void backward_task(int tile, int tl, WarpSmemT<DA ? 1
     p.dg[i] = dg;
     p.db[i] = db;
     if constexpr (DA) {  // alpha = 1 - T_final: dL/dT_final gains -dL/dalpha, which joins the background term
-      p.bgT[i] = T0 * ((bg0 * dr + bg1 * dg + bg2 * db) - dA);
-      p.az[i] = 0.f;
+      p.U[i] = T0 * ((bg0 * dr + bg1 * dg + bg2 * db) - dA);
       p.dD[i] = dZ;
     } else {
-      p.bgT[i] = T0 * (bg0 * dr + bg1 * dg + bg2 * db);
+      p.U[i] = T0 * (bg0 * dr + bg1 * dg + bg2 * db);
     }
     n = max(n, p.nc[i]);
   }
@@ -742,19 +736,23 @@ __device__ __forceinline__ void backward_task(int tile, int tl, WarpSmemT<DA ? 1
       const float dx = q0.x - fx;
       const float tA = q0.z * dx;
       SplatSumsT<DA> s;
-      s.S0 = s.S1 = s.S2 = s.go = s.gr = s.gg = s.gb = 0.f;
-      if constexpr (DA) s.gz = 0.f;
-      if (m == (1u << K) - 1u)
-        visit_bands<K, (1 << K) - 1, DA>(p, pos, q0.y, tA, dx, q0.w, q1.x, q1.y, q1.z, q1.w, cbl, s, czl);
-      else BandLoop<K, 0, DA>::run(m, p, pos, q0.y, tA, dx, q0.w, q1.x, q1.y, q1.z, q1.w, cbl, s, czl);
+      if (m == (1u << K) - 1u) {
+        visit_bands<K, (1 << K) - 1, DA, true>(p, pos, q0.y, tA, dx, q0.w, q1.x, q1.y, q1.z, q1.w, cbl, s, czl);
+      } else {
+        s.S1 = s.S2 = s.go = s.gr = s.gg = s.gb = 0.f;
+        if constexpr (DA) s.gz = 0.f;
+        BandLoop<K, 0, DA>::run(m, p, pos, q0.y, tA, dx, q0.w, q1.x, q1.y, q1.z, q1.w, cbl, s, czl);
+      }
       const float A = q0.z * CONIC_UNSCALE_AC, B = q0.w * CONIC_UNSCALE_B, C = q1.x * CONIC_UNSCALE_AC;
-      const float dxS0 = dx * s.S0;
+      // sums of G dL/dG = opacity t
+      const float S0 = q1.y * s.go, S1 = q1.y * s.S1, S2 = q1.y * s.S2;
+      const float dxS0 = dx * S0;
       float* row = &sm.rows[fill * NR][lane];
-      row[0 * ROWS_STRIDE] = (-A * dxS0 - B * s.S1) * half_W;  // dL/dmean2D.x (NDC units)
-      row[1 * ROWS_STRIDE] = (-C * s.S1 - B * dxS0) * half_H;  // dL/dmean2D.y
-      row[2 * ROWS_STRIDE] = -0.5f * dx * dxS0;                // dL/dconic.xx
-      row[3 * ROWS_STRIDE] = -0.5f * dx * s.S1;                // dL/dconic.xy (stored once)
-      row[4 * ROWS_STRIDE] = -0.5f * s.S2;                     // dL/dconic.yy
+      row[0 * ROWS_STRIDE] = (-A * dxS0 - B * S1) * half_W;  // dL/dmean2D.x (NDC units)
+      row[1 * ROWS_STRIDE] = (-C * S1 - B * dxS0) * half_H;  // dL/dmean2D.y
+      row[2 * ROWS_STRIDE] = -0.5f * dx * dxS0;              // dL/dconic.xx
+      row[3 * ROWS_STRIDE] = -0.5f * dx * S1;                // dL/dconic.xy (stored once)
+      row[4 * ROWS_STRIDE] = -0.5f * S2;                     // dL/dconic.yy
       row[5 * ROWS_STRIDE] = s.go;                             // dL/dopacity
       row[6 * ROWS_STRIDE] = s.gr;
       row[7 * ROWS_STRIDE] = s.gg;
