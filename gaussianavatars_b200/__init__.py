@@ -13,7 +13,7 @@ from .schedule import ViewSchedule, epoch_order
 from .io import load_ply, save_ply, load_flame_param, save_flame_param
 from .densify import densify_and_prune, densify_arrays, add_densification_stats
 from .flame import FlameLBS, flame_pose, flame_param_groups
-from .mesh import mesh_overlay, MeshRenderer
+from .mesh import mesh_overlay, mesh_overlay_views, MeshRenderer
 from .lpips import LpipsNet, lpips, launch_lpips, lpips_features
 from .png import decode_png, encode_png, png_bound
 from .resize import loader_size, resize_u8
@@ -24,6 +24,6 @@ __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gau
            "render_views_train",
            "photometric_loss", "image_metrics", "Adam", "binding_regularizers", "load_ply", "save_ply", "load_flame_param", "save_flame_param", "densify_and_prune", "densify_arrays",
            "add_densification_stats", "expon_lr_schedule", "FlameLBS", "flame_pose", "flame_param_groups",
-           "mesh_overlay", "MeshRenderer", "composite_rgba", "FrameStore",
+           "mesh_overlay", "mesh_overlay_views", "MeshRenderer", "composite_rgba", "FrameStore",
            "ViewSchedule", "epoch_order", "LpipsNet", "lpips", "launch_lpips", "lpips_features",
            "decode_png", "encode_png", "png_bound", "loader_size", "resize_u8", "VideoWriter", "encode_video"]

@@ -238,7 +238,7 @@ EXPORTED_SYMBOLS = ("gab200_forward", "gab200_backward", "gab200_mark_visible", 
                     "gab200_png_copy", "gab200_png_status_string", "gab200_png_decode_scratch_bytes",
                     "gab200_png_decode", "gab200_resize_scratch_bytes", "gab200_resize_u8",
                     "gab200_h264_bound", "gab200_h264_scratch_bytes", "gab200_h264_encode",
-                    "gab200_h264_parameter_sets")
+                    "gab200_h264_parameter_sets", "gab200_mesh_views_scratch_bytes", "gab200_mesh_render_views")
 
 _lib = None
 _lock = threading.Lock()
@@ -399,6 +399,10 @@ def lib():
         L.gab200_mesh_render.argtypes = [C.POINTER(MeshArgs), C.c_void_p]
         L.gab200_mesh_scratch_bytes.restype = C.c_size_t
         L.gab200_mesh_scratch_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
+        L.gab200_mesh_render_views.restype = C.c_int32
+        L.gab200_mesh_render_views.argtypes = [C.POINTER(MeshArgs), C.c_int32, C.c_void_p]
+        L.gab200_mesh_views_scratch_bytes.restype = C.c_size_t
+        L.gab200_mesh_views_scratch_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32]
         L.gab200_adam_step.restype = C.c_int32
         L.gab200_adam_step.argtypes = [C.c_int32, C.POINTER(AdamSegment), C.c_int64, C.c_double, C.c_double,
                                        C.c_double, C.c_void_p]

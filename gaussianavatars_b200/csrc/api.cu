@@ -1181,7 +1181,17 @@ static const int kMeshMaxSide = 16384;  // snapped coordinates (guard band + ima
 
 size_t gab200_mesh_scratch_bytes(int32_t num_faces, int32_t width, int32_t height) {
   if (num_faces < 1 || width < 1 || height < 1 || width > kMeshMaxSide || height > kMeshMaxSide) return 0;
-  return mesh_scratch_bytes(num_faces, width, height);
+  return mesh_scratch_bytes(1, num_faces, width, height);
+}
+
+// views outside [1, 65535] (the resolve's grid z), or K * F face records beyond int32
+static bool mesh_views_ok(int32_t views, int32_t num_faces) {
+  return views >= 1 && views <= 65535 && (int64_t)views * num_faces <= INT32_MAX;
+}
+
+size_t gab200_mesh_views_scratch_bytes(int32_t views, int32_t num_faces, int32_t width, int32_t height) {
+  if (gab200_mesh_scratch_bytes(num_faces, width, height) == 0 || !mesh_views_ok(views, num_faces)) return 0;
+  return mesh_scratch_bytes(views, num_faces, width, height);
 }
 
 static bool mesh_args_ok(const gab200_mesh_args* a) {
@@ -1206,7 +1216,17 @@ static bool mesh_args_ok(const gab200_mesh_args* a) {
 int32_t gab200_mesh_render(const gab200_mesh_args* a, void* stream_) {
   if (!mesh_args_ok(a)) return GAB200_ERR_INVALID_ARGUMENT;
   if (check_arch() < 0) return GAB200_ERR_ARCH;
-  return launch_mesh_render(*a, (cudaStream_t)stream_) == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+  return launch_mesh_render(*a, 1, (cudaStream_t)stream_) == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
+int32_t gab200_mesh_render_views(const gab200_mesh_args* a, int32_t views, void* stream_) {
+  if (!mesh_args_ok(a) || !mesh_views_ok(views, a->F)) return GAB200_ERR_INVALID_ARGUMENT;
+  // what the K-view callers use: a world-space mesh composited into uint8 frames, nothing else
+  if (a->pos_kind != GAB200_MESH_POS_WORLD || !a->out_u8 || a->out_rgba || a->out_float || a->out_rast ||
+      a->in_rast || a->in_color || a->out_color)
+    return GAB200_ERR_INVALID_ARGUMENT;
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  return launch_mesh_render(*a, views, (cudaStream_t)stream_) == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
 }
 
 int32_t gab200_adam_step(int32_t num_segments, const gab200_adam_segment* segs, int64_t step, double beta1,

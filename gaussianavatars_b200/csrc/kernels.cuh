@@ -287,8 +287,8 @@ void launch_lpips_pack(int net, const float* const* conv_w, const float* const* 
 void launch_lpips(const gab200_lpips_args& a, cudaStream_t stream);
 
 // mesh.cu
-size_t mesh_scratch_bytes(int F, int W, int H);
-cudaError_t launch_mesh_render(const gab200_mesh_args& a, cudaStream_t stream);
+size_t mesh_scratch_bytes(int K, int F, int W, int H);   // K views (1: gab200_mesh_render)
+cudaError_t launch_mesh_render(const gab200_mesh_args& a, int K, cudaStream_t stream);
 
 // densify.cu
 size_t densify_scratch_bytes(int P, int F);

@@ -5,16 +5,22 @@
 // Compiled with --fmad=false: every float below is rounded op by op in the order written, so the numpy restatement in
 // tests/mesh_oracle.py reproduces the snapped vertices, the depth keys and therefore the winner map bit for bit.
 //
+// Every launch carries a view index: one call draws one vertex set under K cameras (gab200_mesh_render_views), each
+// (view, face) projected through row k of a [K,37] camera table into its own face records and its own winner map, and
+// view k's pixels read base plane k and write output plane k.  The single-view call is K = 1 of the same kernels, and
+// view k of a K-view call is bit for bit the single-view call with camera k and base k: no value crosses views, and
+// the only shared step -- the persistent raster warps' division of the work items -- ends in an order-free atomicMin.
+//
 // Launches (all stream-ordered, no host wait, capturable):
-//   mesh_setup_kernel    one thread per face: clip coordinates ([v,1] . full_proj, or given), clip against the
+//   mesh_setup_kernel    one thread per (view, face): clip coordinates ([v,1] . full_proj, or given), clip against the
 //                        clip volume -w <= z <= w and a guard band of 2^15 px, snap to 1/256 px, flat colour, pixel
 //                        bounding box and its number of 8x4 pixel tiles
-//   cub InclusiveSum     tiles per face -> offsets (u64)
-//   mesh_silhouette_kernel  (antialias only) one thread per face: which of its edges are screen-space silhouettes
-//   mesh_raster_kernel   persistent warps, each an equal share of the (face, 8x4 tile) work items, one item at a time
+//   cub InclusiveSum     tiles per (view, face) -> offsets (u64)
+//   mesh_silhouette_kernel  (antialias only) one thread per (view, face): which of its edges are screen-space silhouettes
+//   mesh_raster_kernel   persistent warps, each an equal share of the (view, face, 8x4 tile) work items of all views
 //                        (a face covering 1e5 px is spread over many warps): int64 edge functions with a
 //                        top-left rule, z/w at the pixel centre, 64-bit atomicMin of (depth key << 32 | face id)
-//   mesh_resolve_kernel  one thread per pixel: shading, silhouette antialiasing from the winners of the pixel and its
+//   mesh_resolve_kernel  one thread per (view, pixel): shading, silhouette antialiasing from the winners of the pixel and its
 //                        4 neighbours, then the requested outputs
 // Pixel convention: column c / row r has its centre at (c + 1/2, r + 1/2) with X = (x/w + 1) W/2, Y = (y/w + 1) H/2,
 // so row 0 is clip y = -1: the top row of the splat image for a camera's own full_proj_transform, and nvdiffrast's
@@ -47,10 +53,11 @@ struct __align__(16) FaceEdges {        // the unclipped triangle, for the silho
 
 struct MeshParams {
   int V, F, W, H, pos_kind;
+  int K;                                // views: the records of view k are [k F, k F + F), its winners [k H W, ...)
   const float* verts;
   const int32_t* faces;
   const int32_t* adj;
-  const float* cam;
+  const float* cam;                     // camera block of view 0; view k's at cam + k * GAB200_CAMERA_FLOATS
   float gx, gy;                         // guard band in NDC units: 2^16 / W, 2^16 / H
 };
 
@@ -68,14 +75,14 @@ __device__ __forceinline__ float plane_dist(const PV& v, int k, float gx, float 
 }
 
 // clip coordinates of vertex i: [v,1] . M (row-vector layout of full_proj_transform), summed left to right
-__device__ __forceinline__ PV clip_vertex(const MeshParams& p, int i) {
+__device__ __forceinline__ PV clip_vertex(const MeshParams& p, const float* cam, int i) {
   PV o;
   if (p.pos_kind == GAB200_MESH_POS_CLIP) {
     const float* v = p.verts + 4 * (int64_t)i;
     o.x = v[0]; o.y = v[1]; o.z = v[2]; o.w = v[3];
   } else {
     const float* v = p.verts + 3 * (int64_t)i;
-    const float* M = p.cam + 16;
+    const float* M = cam + 16;
     float c[4];
 #pragma unroll
     for (int j = 0; j < 4; j++)
@@ -157,8 +164,10 @@ struct SubTri {
 __global__ void __launch_bounds__(128) mesh_setup_kernel(MeshParams p, const float* face_colors, float3 bg,
                                                          int lighting, FacePoly* polys, FaceEdges* edges,
                                                          float4* colors, uint64_t* tiles, int32_t* error_flag) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  if (f >= p.F) return;
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;   // record of (view, face): K F <= INT32_MAX
+  if (t >= p.K * p.F) return;
+  const int view = t / p.F, f = t - view * p.F;
+  const float* cam = p.cam + (int64_t)view * GAB200_CAMERA_FLOATS;
   FacePoly P;
   P.n = 0;
   FaceEdges E;
@@ -172,7 +181,7 @@ __global__ void __launch_bounds__(128) mesh_setup_kernel(MeshParams p, const flo
   } else {
     PV a[MAXP], b[MAXP];
     for (int k = 0; k < 3; k++) {
-      a[k] = clip_vertex(p, idx[k]);
+      a[k] = clip_vertex(p, cam, idx[k]);
       a[k].b0 = k == 0 ? 1.f : 0.f;
       a[k].b1 = k == 1 ? 1.f : 0.f;
       if (inside_all(a[k], p.gx, p.gy)) {
@@ -233,7 +242,7 @@ __global__ void __launch_bounds__(128) mesh_setup_kernel(MeshParams p, const flo
     }
     if (p.pos_kind == GAB200_MESH_POS_WORLD) {
       // face normal in the OpenGL camera frame (rows 1, 2 of the view transform negated), 'front' light on +z
-      const float* Wv = p.cam;
+      const float* Wv = cam;
       float c[3][3];
       for (int k = 0; k < 3; k++) {
         const float* v = p.verts + 3 * (int64_t)idx[k];
@@ -263,38 +272,47 @@ __global__ void __launch_bounds__(128) mesh_setup_kernel(MeshParams p, const flo
   uint64_t nt = 0;
   if (P.n > 0 && P.c1 >= P.c0 && P.r1 >= P.r0)
     nt = (uint64_t)((P.c1 - P.c0) / 8 + 1) * (uint64_t)((P.r1 - P.r0) / 4 + 1);
-  polys[f] = P;
-  edges[f] = E;
-  colors[f] = col;
-  tiles[f] = nt;
+  polys[t] = P;
+  edges[t] = E;
+  colors[t] = col;
+  tiles[t] = nt;
 }
 
-// Persistent warps over the (face, 8x4 tile) work items: warp k takes the k-th equal share of the items in order, finds
-// the face of its first item by one binary search (the first f with offsets[f] > w) and walks the faces forward.
-__global__ void __launch_bounds__(256) mesh_raster_kernel(int F, int W, const FacePoly* __restrict__ polys,
+// Persistent warps over the (view, face, 8x4 tile) work items: warp k takes the k-th equal share of the items in order,
+// finds the record of its first item by one binary search (the first t with offsets[t] > w) and walks the records
+// forward.  Record t is face t mod F of view t / F; its key carries the face index and lands in that view's map.
+__global__ void __launch_bounds__(256) mesh_raster_kernel(int F, int KF, int W, int64_t HW,
+                                                          const FacePoly* __restrict__ polys,
                                                           const uint64_t* __restrict__ offsets,
                                                           unsigned long long* __restrict__ winner) {
   const int lane = threadIdx.x & 31;
-  const uint64_t total = offsets[F - 1];
+  const uint64_t total = offsets[KF - 1];
   const uint64_t nwarps = (uint64_t)gridDim.x * (blockDim.x >> 5);
   const uint64_t per = (total + nwarps - 1) / nwarps;
   uint64_t w = ((uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * per;
   const uint64_t wend = min(total, w + per);
   if (w >= wend) return;
-  int lo = 0, hi = F - 1;
+  int lo = 0, hi = KF - 1;
   while (lo < hi) {
     const int mid = (lo + hi) >> 1;
     if (offsets[mid] > w) hi = mid; else lo = mid + 1;
   }
-  int f = lo;
-  uint64_t base = f > 0 ? offsets[f - 1] : 0ull, end = offsets[f];
+  int t = lo;
+  int view = t / F, f = t - view * F;
+  unsigned long long* map = winner + view * HW;
+  uint64_t base = t > 0 ? offsets[t - 1] : 0ull, end = offsets[t];
   for (; w < wend; w++) {
-    while (w >= end) {
-      base = end;
-      end = offsets[++f];
+    if (w >= end) {
+      do {
+        base = end;
+        end = offsets[++t];
+      } while (w >= end);
+      view = t / F;
+      f = t - view * F;
+      map = winner + view * HW;
     }
     const uint64_t local = w - base;
-    const FacePoly& P = polys[f];
+    const FacePoly& P = polys[t];
     const int c0 = P.c0, r0 = P.r0;
     const uint64_t ntx = (uint64_t)((P.c1 - c0) / 8 + 1);
     const int c = c0 + (int)(local % ntx) * 8 + (lane & 7);
@@ -310,7 +328,7 @@ __global__ void __launch_bounds__(256) mesh_raster_kernel(int F, int W, const Fa
       const uint64_t key = ((uint64_t)depth_key(T.depth(P, e0, e1, e2)) << 32) | (uint32_t)f;
       best = key < best ? key : best;
     }
-    if (best != EMPTY) atomicMin(winner + (int64_t)r * W + c, (unsigned long long)best);
+    if (best != EMPTY) atomicMin(map + (int64_t)r * W + c, (unsigned long long)best);
   }
 }
 
@@ -324,13 +342,15 @@ __global__ void mesh_keys_from_rast_kernel(int n, int F, const float* __restrict
   winner[i] = k;
 }
 
-// One thread per face: which of its edges are screen-space silhouettes -- a mesh boundary, or the face across it lies
+// One thread per (view, face): which of its edges are screen-space silhouettes -- a mesh boundary, or the face across it lies
 // on the face's side of the edge's projected line (the opposite vertex of the neighbour read from its own record:
 // the same snapped position a projection here would give).  Edges with a vertex outside the clip volume, and every
 // edge of a face with such a vertex (orient 0), never are.
-__global__ void __launch_bounds__(128) mesh_silhouette_kernel(MeshParams p, FaceEdges* edges) {
-  const int T = blockIdx.x * blockDim.x + threadIdx.x;
-  if (T >= p.F) return;
+__global__ void __launch_bounds__(128) mesh_silhouette_kernel(MeshParams p, FaceEdges* all_edges) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= p.K * p.F) return;
+  const int view = t / p.F, T = t - view * p.F;
+  FaceEdges* edges = all_edges + (int64_t)view * p.F;   // this view's records
   const FaceEdges E = edges[T];
   int a[3], n[3];
   if (E.orient == 0 || !face_ok(p, T, a[0], a[1], a[2])) return;
@@ -406,14 +426,21 @@ struct ResolveOut {
   float* out_color;
 };
 
+// One thread per (view, pixel), view = blockIdx.z.  Only base and out_u8 have a view dimension: the other outputs
+// exist for single-view calls only.
 __global__ void __launch_bounds__(256) mesh_resolve_kernel(MeshParams p, ResolveOut o,
-                                                           const FacePoly* __restrict__ polys,
-                                                           const FaceEdges* __restrict__ edges,
-                                                           const float4* __restrict__ colors,
-                                                           const uint64_t* __restrict__ winner) {
+                                                           const FacePoly* __restrict__ all_polys,
+                                                           const FaceEdges* __restrict__ all_edges,
+                                                           const float4* __restrict__ all_colors,
+                                                           const uint64_t* __restrict__ all_winner) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x, r = blockIdx.y;
   if (c >= p.W) return;
   const int64_t pix = (int64_t)r * p.W + c, HW = (int64_t)p.W * p.H;
+  const int64_t view = blockIdx.z;
+  const FacePoly* __restrict__ polys = all_polys + view * p.F;
+  const FaceEdges* __restrict__ edges = all_edges + view * p.F;
+  const float4* __restrict__ colors = all_colors + view * p.F;
+  const uint64_t* __restrict__ winner = all_winner + view * HW;
   const uint64_t kq = winner[pix];
   // neighbours in the fixed order left, right, up, down
   float wgt[4] = {0.f, 0.f, 0.f, 0.f};
@@ -489,17 +516,18 @@ __global__ void __launch_bounds__(256) mesh_resolve_kernel(MeshParams p, Resolve
   for (int ch = 0; ch < 3; ch++) {
     float b;
     if (o.base_kind == GAB200_MESH_BASE_U8_CHW)
-      b = __fdiv_rn((float)static_cast<const uint8_t*>(o.base)[ch * HW + pix], 255.f);
+      b = __fdiv_rn((float)static_cast<const uint8_t*>(o.base)[(3 * view + ch) * HW + pix], 255.f);
     else
-      b = static_cast<const float*>(o.base)[ch * HW + pix];
+      b = static_cast<const float*>(o.base)[(3 * view + ch) * HW + pix];
     const float v = __fadd_rn(__fmul_rn(__fmul_rn(rgb[ch], a), op), __fmul_rn(b, keep));
     if (o.out_float) o.out_float[ch * HW + pix] = v;
     q[ch] = quantize_u8(v);
   }
   if (o.out_u8) {
-    o.out_u8[3 * pix] = (uint8_t)q[0];
-    o.out_u8[3 * pix + 1] = (uint8_t)q[1];
-    o.out_u8[3 * pix + 2] = (uint8_t)q[2];
+    uint8_t* out = o.out_u8 + 3 * (view * HW + pix);
+    out[0] = (uint8_t)q[0];
+    out[1] = (uint8_t)q[1];
+    out[2] = (uint8_t)q[2];
   }
 }
 
@@ -520,60 +548,64 @@ size_t scan_temp_bytes_u64(int F) {
   return bytes;
 }
 
-MeshScratch carve_mesh(void* base, int F, int W, int H) {
+// K views: K F face records (K = 1: the single-view layout) and K winner maps
+MeshScratch carve_mesh(void* base, int K, int F, int W, int H) {
+  const int KF = K * F;
   Carver cv(base);
   MeshScratch s;
-  s.polys = cv.take<FacePoly>(F);
-  s.edges = cv.take<FaceEdges>(F);
-  s.colors = cv.take<float4>(F);
-  s.tiles = cv.take<uint64_t>(F);
-  s.offsets = cv.take<uint64_t>(F);
-  s.winner = cv.take<uint64_t>((size_t)W * H);
-  s.scan_bytes = scan_temp_bytes_u64(F);
+  s.polys = cv.take<FacePoly>(KF);
+  s.edges = cv.take<FaceEdges>(KF);
+  s.colors = cv.take<float4>(KF);
+  s.tiles = cv.take<uint64_t>(KF);
+  s.offsets = cv.take<uint64_t>(KF);
+  s.winner = cv.take<uint64_t>((size_t)K * W * H);
+  s.scan_bytes = scan_temp_bytes_u64(KF);
   s.scan_temp = cv.take<char>(s.scan_bytes);
   return s;
 }
 
 }  // namespace
 
-size_t mesh_scratch_bytes(int F, int W, int H) {
+size_t mesh_scratch_bytes(int K, int F, int W, int H) {
   Carver cv(nullptr);
-  cv.take<FacePoly>(F);
-  cv.take<FaceEdges>(F);
-  cv.take<float4>(F);
-  cv.take<uint64_t>(F);
-  cv.take<uint64_t>(F);
-  cv.take<uint64_t>((size_t)W * H);
-  cv.take<char>(scan_temp_bytes_u64(F));
+  const int KF = K * F;
+  cv.take<FacePoly>(KF);
+  cv.take<FaceEdges>(KF);
+  cv.take<float4>(KF);
+  cv.take<uint64_t>(KF);
+  cv.take<uint64_t>(KF);
+  cv.take<uint64_t>((size_t)K * W * H);
+  cv.take<char>(scan_temp_bytes_u64(KF));
   return cv.bytes();
 }
 
-cudaError_t launch_mesh_render(const gab200_mesh_args& a, cudaStream_t stream) {
-  MeshScratch s = carve_mesh(a.scratch, a.F, a.width, a.height);
+cudaError_t launch_mesh_render(const gab200_mesh_args& a, int K, cudaStream_t stream) {
+  MeshScratch s = carve_mesh(a.scratch, K, a.F, a.width, a.height);
   MeshParams p;
-  p.V = a.V; p.F = a.F; p.W = a.width; p.H = a.height; p.pos_kind = a.pos_kind;
+  p.V = a.V; p.F = a.F; p.W = a.width; p.H = a.height; p.pos_kind = a.pos_kind; p.K = K;
   p.verts = a.verts; p.faces = a.faces; p.adj = a.adjacency; p.cam = a.camera;
   p.gx = 65536.f / (float)a.width;  // IEEE division on the host, as the oracle's float32 division
   p.gy = 65536.f / (float)a.height;
   const float3 bg = make_float3(a.background[0], a.background[1], a.background[2]);
-  mesh_setup_kernel<<<(a.F + 127) / 128, 128, 0, stream>>>(p, a.face_colors, bg, a.lighting, s.polys, s.edges,
-                                                            s.colors, s.tiles, a.error_flag);
+  const int KF = K * a.F;
+  mesh_setup_kernel<<<(KF + 127) / 128, 128, 0, stream>>>(p, a.face_colors, bg, a.lighting, s.polys, s.edges,
+                                                          s.colors, s.tiles, a.error_flag);
   count_launch();
   if (a.antialias) {
-    mesh_silhouette_kernel<<<(a.F + 127) / 128, 128, 0, stream>>>(p, s.edges);
+    mesh_silhouette_kernel<<<(KF + 127) / 128, 128, 0, stream>>>(p, s.edges);
     count_launch();
   }
   const int64_t HW = (int64_t)a.width * a.height;
-  if (a.in_rast) {
+  if (a.in_rast) {   // single-view calls only
     mesh_keys_from_rast_kernel<<<(unsigned)((HW + 255) / 256), 256, 0, stream>>>((int)HW, a.F, a.in_rast, s.winner);
     count_launch();
   } else {
-    cudaError_t e = cudaMemsetAsync(s.winner, 0xff, HW * sizeof(uint64_t), stream);
+    cudaError_t e = cudaMemsetAsync(s.winner, 0xff, K * HW * sizeof(uint64_t), stream);
     if (e != cudaSuccess) return e;
-    e = cub::DeviceScan::InclusiveSum(s.scan_temp, s.scan_bytes, s.tiles, s.offsets, a.F, stream);
+    e = cub::DeviceScan::InclusiveSum(s.scan_temp, s.scan_bytes, s.tiles, s.offsets, KF, stream);
     if (e != cudaSuccess) return e;
     count_launch();
-    mesh_raster_kernel<<<GAB_NUM_SMS * 8, 256, 0, stream>>>(a.F, a.width, s.polys, s.offsets,
+    mesh_raster_kernel<<<GAB_NUM_SMS * 8, 256, 0, stream>>>(a.F, KF, a.width, HW, s.polys, s.offsets,
                                                             reinterpret_cast<unsigned long long*>(s.winner));
     count_launch();
   }
@@ -582,8 +614,8 @@ cudaError_t launch_mesh_render(const gab200_mesh_args& a, cudaStream_t stream) {
   o.bg = bg; o.base = a.base; o.opacity = a.opacity; o.in_color = a.in_color;
   o.out_u8 = a.out_u8; o.out_float = a.out_float; o.out_rgba = a.out_rgba; o.out_rast = a.out_rast;
   o.out_color = a.out_color;
-  mesh_resolve_kernel<<<dim3((a.width + 255) / 256, a.height), 256, 0, stream>>>(p, o, s.polys, s.edges, s.colors,
-                                                                                 s.winner);
+  mesh_resolve_kernel<<<dim3((a.width + 255) / 256, a.height, K), 256, 0, stream>>>(p, o, s.polys, s.edges, s.colors,
+                                                                                    s.winner);
   count_launch();
   return cudaPeekAtLastError();
 }

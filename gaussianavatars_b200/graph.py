@@ -960,7 +960,11 @@ class GraphedRender(_Captured):
     (mesh.mesh_overlay) composite the mesh of the vertices the graph just posed at opacity o and write `display`.
     Pixels the mesh does not reach get the bytes the display epilogue would have written.  Opacity and face_colors
     ((F,3), e.g. the viewer's splats-per-face colouring) are device buffers written by set_inputs: a slider or a colour
-    picker never re-captures.  `mesh_error` is a device int32 set to 1 when a face index is out of range."""
+    picker never re-captures.  `mesh_error` is a device int32 set to 1 when a face index is out of range.  With
+    views_per_replay=K the mesh is drawn under all K cameras in one launch sequence (mesh.mesh_overlay_views), each
+    view bit for bit its single-camera overlay."""
+
+    _MESH_OVER_GT = False   # the mesh is drawn over the splat image into `display` (GraphedEval: over `gt`)
 
     def __init__(self, pc, width: int, height: int, bg: torch.Tensor, outputs: str = "u8",
                  scaling_modifier: float = 1.0, mesh_update: bool = True, host_slots: int = 0,
@@ -975,7 +979,7 @@ class GraphedRender(_Captured):
         views_per_replay=K > 1: every replay renders K cameras of one timestep in one forward
         (gab200_forward_views): the head is posed once, set_inputs(cameras=...) takes K cameras (or a (K, 37) table),
         warm_cameras is a list of such camera groups, and display / image / radii / the host slots carry a leading K
-        dimension.  Not combinable with the mesh overlay.
+        dimension; with mesh_opacity the mesh is drawn over each of the K float images into `display` (K,H,W,3).
         depth_alpha=True: every replay also refreshes `alpha` and `depth`, (1,H,W) float32 static tensors -- the
         splats' accumulated opacity and alpha-weighted view-space depth from the same blend (gab200_forward_depth_alpha;
         with the mesh overlay they remain the splats').  Single-view replays only.
@@ -991,8 +995,6 @@ class GraphedRender(_Captured):
         if depth_alpha and views_per_replay > 1:
             raise ValueError("depth_alpha renders one camera per replay: it needs views_per_replay=1 (the K-view "
                              "forward has no alpha / depth planes)")
-        if views_per_replay > 1 and mesh_opacity is not None:
-            raise ValueError("the mesh overlay draws one camera per replay: it needs views_per_replay=1")
         self.K = int(views_per_replay)
         if host_slots < 0 or (host_slots > 0 and outputs == "float"):
             raise ValueError("host_slots copies the display image: it needs outputs 'u8' or 'both'")
@@ -1010,11 +1012,16 @@ class GraphedRender(_Captured):
         self.image = self.display = self.radii = self.alpha = self.depth = None
         self.depth_alpha = bool(depth_alpha)
         self.mesh = mesh_opacity is not None
+        self.mesh_display = self.mesh_png_out = self.mesh_png_len = None
+        self.host_mesh_png_slots = self._mesh_png_staged = None
         if self.mesh:
-            if outputs == "float":
+            if outputs == "float" and not self._MESH_OVER_GT:
                 raise ValueError("the mesh overlay writes the display image: it needs outputs 'u8' or 'both'")
             if getattr(pc, "faces", None) is None:
                 raise ValueError("mesh_opacity needs a model with a mesh (pc.faces)")
+            if pc.faces.dtype not in (torch.int32, torch.int64):
+                raise ValueError(f"the mesh overlay draws integer faces: pc.faces is {pc.faces.dtype}, not int32 / "
+                                 "int64")
             if mesh_lighting not in M.LIGHTING:
                 raise ValueError(f"mesh_lighting must be one of {sorted(M.LIGHTING)}, got {mesh_lighting!r}")
             self.mesh_lighting = mesh_lighting
@@ -1073,11 +1080,12 @@ class GraphedRender(_Captured):
             if self.mesh_update:
                 self._pose()
             # K > 1: the K cameras of the table in one forward
+            over = self.mesh and not self._MESH_OVER_GT   # the mesh over the float splat image(s)
             out = _forward_only(self.camera if self.K == 1 else self.cam, self.pc, _Pipe, self.bg,
-                                self.scaling_modifier, self.outputs != "float" and not self.mesh,
-                                self.outputs != "u8" or self.mesh, self.depth_alpha,
+                                self.scaling_modifier, self.outputs != "float" and not over,
+                                self.outputs != "u8" or over, self.depth_alpha,
                                 None if self.K == 1 else (self.W, self.H))
-            if self.mesh:
+            if over:
                 out["display_u8"] = self._overlay(out["render"])
         self.image, self.display, self.radii = out["render"], out["display_u8"], out["radii"]
         self.alpha, self.depth = out.get("alpha"), out.get("depth")
@@ -1086,34 +1094,45 @@ class GraphedRender(_Captured):
 
     def _encode_png(self):
         """The display frame(s) -> PNG files in buffers the capture allocates (the graph's own pool)."""
-        K, dev = self.K, self.device
-        self._png_scratch = PNG.scratch(K, self.H, self.W, dev)
-        self.png_out = torch.empty((K, PNG.slot_stride(self.W, self.H)), dtype=torch.uint8, device=dev)
-        self.png_len = torch.empty(K, dtype=torch.int64, device=dev)
-        PNG.launch_encode(self.display, self._png_scratch, self.png_out, self.png_len)
+        self._png_scratch = PNG.scratch(self.K, self.H, self.W, self.device)
+        self.png_out, self.png_len = self._encode(self.display)
 
-    def _overlay(self, image):
-        """The mesh of the vertices the frame just posed (pc.verts) over the float splat image -> (H,W,3) uint8."""
+    def _encode(self, u8):
+        """u8 (H,W,3) | (K,H,W,3) -> (files (K, stride) uint8, lengths (K,) int64), through the frame's PNG scratch."""
+        K, dev = self.K, self.device
+        out = torch.empty((K, PNG.slot_stride(self.W, self.H)), dtype=torch.uint8, device=dev)
+        length = torch.empty(K, dtype=torch.int64, device=dev)
+        PNG.launch_encode(u8, self._png_scratch, out, length)
+        return out, length
+
+    def _overlay(self, base):
+        """The mesh of the vertices the frame just posed (pc.verts) over `base` -- the float splat image(s), or the
+        uint8 ground truth -- at the frame's camera(s) -> (H,W,3) uint8, or (K,H,W,3) in one K-view call."""
         pc = self.pc
         if pc.verts is None:
             raise ValueError("the mesh overlay draws the posed vertices (pc.verts): pose the model first")
         faces = getattr(pc, "faces_i32", None)
         faces = pc.faces.to(torch.int32).contiguous() if faces is None else faces
-        display = torch.empty(self.H, self.W, 3, dtype=torch.uint8, device=self.device)
+        shape = (self.H, self.W, 3) if self.K == 1 else (self.K, self.H, self.W, 3)
+        display = torch.empty(shape, dtype=torch.uint8, device=self.device)
         M.launch_mesh(verts=pc.verts.detach().reshape(-1, 3), faces=faces, width=self.W, height=self.H,
                       camera=self.cam, adjacency=self._adjacency.get(pc.faces).to(self.device),
-                      face_colors=self.face_colors, lighting=self.mesh_lighting, antialias=True, base=image,
-                      opacity=self._opacity, out_u8=display, error_flag=self.mesh_error)
+                      face_colors=self.face_colors, lighting=self.mesh_lighting, antialias=True, base=base.contiguous(),
+                      opacity=self._opacity, out_u8=display, error_flag=self.mesh_error,
+                      views=None if self.K == 1 else self.K)
         return display
 
     # ---- capture ---------------------------------------------------------------------------------------------------
     def _release(self):
         self.image = self.display = self.radii = self.alpha = self.depth = None
         self.png_out = self.png_len = self._png_scratch = None
+        self.mesh_display = self.mesh_png_out = self.mesh_png_len = None
 
     def _before_capture(self):
         if self.camera is not None:
             self.camera.image_width, self.camera.image_height = self.W, self.H
+        if self.mesh:   # the adjacency's build reads sizes on the host: never inside the capture
+            self._adjacency.get(self.pc.faces)
 
     def _after_capture(self):
         # the mesh tensors the replay writes (the model's attributes are replaced by any eager frame)
@@ -1152,6 +1171,14 @@ class GraphedRender(_Captured):
                 self.host_png_slots = [torch.empty((rows, stride), dtype=torch.uint8).pin_memory() for _ in range(k)]
                 self._png_staged = [torch.empty((rows, stride), dtype=torch.uint8, device=self.device)
                                     for _ in range(2)]
+            if self.mesh_png_out is not None and (self.host_mesh_png_slots is None or
+                                                  tuple(self.host_mesh_png_slots[0].shape) != (rows, stride)):
+                # GraphedEval's mesh files travel beside the render's, in the same layout
+                torch.cuda.synchronize(self.device)
+                self.host_mesh_png_slots = [torch.empty((rows, stride), dtype=torch.uint8).pin_memory()
+                                            for _ in range(k)]
+                self._mesh_png_staged = [torch.empty((rows, stride), dtype=torch.uint8, device=self.device)
+                                         for _ in range(2)]
         self._copy_stream = self._copy_stream or torch.cuda.Stream(device=self.device)
         self._host_events = [None] * k     # per host slot: the copy into it, and which replay it holds
         self._host_replay = [-1] * k
@@ -1169,6 +1196,8 @@ class GraphedRender(_Captured):
         self._staged[s].copy_(self.display)
         if self.png:   # the compressed bytes only, and -1 for a replay that overflowed (the slot's sticky flag)
             self._png_copy(self.png_out, self.png_len, self._png_staged[s], self.slot.flag)
+        if self.mesh_png_out is not None:   # the mesh over the ground truth does not depend on the splats: no flag
+            self._png_copy(self.mesh_png_out, self.mesh_png_len, self._mesh_png_staged[s])
         ready = torch.cuda.Event()
         ready.record(cur)
         self._copy_stream.wait_event(ready)
@@ -1177,6 +1206,9 @@ class GraphedRender(_Captured):
             if self.png:   # staged -> the pinned slot, written by a kernel through its mapped address
                 st = self._png_staged[s]
                 self._png_copy(self._png_rows(st), self._png_lengths(st), self.host_png_slots[h])
+            if self.mesh_png_out is not None:
+                st = self._mesh_png_staged[s]
+                self._png_copy(self._png_rows(st), self._png_lengths(st), self.host_mesh_png_slots[h])
             done = torch.cuda.Event()
             done.record(self._copy_stream)
         self._stage_events[s] = self._host_events[h] = done
@@ -1198,14 +1230,18 @@ class GraphedRender(_Captured):
         has landed.  Raises when that replay overflowed its instance capacity: its frame is incomplete."""
         if not self.png:
             raise ValueError("host_png needs a frame built with png=True")
+        return self._host_files(self.host_png_slots, replay, "host_png")
+
+    def _host_files(self, slots, replay, name):
+        """Replay `replay`'s files from a ring of PNG slots (one file, or a list of K)."""
         if not self.host_slots:
-            raise ValueError("host_png needs host_slots > 0")
+            raise ValueError(f"{name} needs host_slots > 0")
         i = self.replays - 1 if replay is None else int(replay)
         h = i % self.host_slots
         if self._host_replay[h] != i:
             raise IndexError(f"replay {i} is not in the host ring (slot {h} holds replay {self._host_replay[h]})")
         self._host_events[h].synchronize()
-        slot = self.host_png_slots[h]
+        slot = slots[h]
         lens, rows = self._png_lengths(slot).tolist(), self._png_rows(slot)
         if min(lens) < 0:
             raise RuntimeError(f"{type(self).__name__}: replay {i} overflowed its instance capacity, so its frame is "
@@ -1269,12 +1305,22 @@ class GraphedEval(GraphedRender):
 
     lpips=net (an lpips.LpipsNet): the body also scores each view's LPIPS distance (gab200_lpips) into row `view` of
     a (views,) device table, with the same rows and the same overflow flag as the metrics; scores() then adds
-    `lpips_per_view` and `lpips`.  training_report uses LpipsNet.from_hub_cache("alex"), metrics.py "vgg"."""
+    `lpips_per_view` and `lpips`.  training_report uses LpipsNet.from_hub_cache("alex"), metrics.py "vgg".
+
+    mesh_opacity=o (source="u8"): render.py's renders_mesh.  After the view is rendered and scored, the body draws the
+    mesh of the vertices it posed over the uint8 ground truth `gt` at opacity o (render.py:75-81) into `mesh_display`
+    ((H,W,3), or (K,H,W,3) in one K-view call); scores and `display` are those of the frame without it.  With png=True
+    it is also encoded into `mesh_png_out` / `mesh_png_len`, and with host_slots those files travel in the ring beside
+    the render's: host_mesh_png(i).  The mesh frame does not depend on the splats, so a replay that overflowed its
+    capacity still draws (and ships) it.  face_colors and mesh_lighting mean what they mean for a GraphedRender."""
+
+    _MESH_OVER_GT = True
 
     def __init__(self, pc, width: int, height: int, bg: torch.Tensor, views: int, source: str = "float",
                  host_slots: int = 0, capacity: Optional[int] = None, headroom: float = 1.25, warm_cameras=None,
                  warm_timesteps=None, views_per_replay: int = 1, schedule=None, frames=None, lpips=None,
-                 png: bool = False):
+                 png: bool = False, mesh_opacity: Optional[float] = None, face_colors: Optional[torch.Tensor] = None,
+                 mesh_lighting: str = "front"):
         """views_per_replay=K > 1: one replay renders K cameras of one timestep in one forward and scores them into
         rows view .. view + K - 1 (set_inputs(cameras=K cameras, gt_u8=(K,3,H,W), view=first row)); warm_cameras is a
         list of K-camera groups.  K is fixed per capture: a last group of fewer views is the business of a
@@ -1293,6 +1339,9 @@ class GraphedEval(GraphedRender):
             raise ValueError("host_slots ships the display image: it needs source='u8'")
         if png and source != "u8":
             raise ValueError("png=True encodes the display image: it needs source='u8'")
+        if mesh_opacity is not None and source != "u8":
+            raise ValueError("mesh_opacity draws render.py's renders_mesh over the uint8 ground truth: it needs "
+                             "source='u8'")
         if int(views) < 1:
             raise ValueError("views must be at least 1")
         if isinstance(views_per_replay, int) and views_per_replay > int(views):
@@ -1305,7 +1354,8 @@ class GraphedEval(GraphedRender):
                                  f"{lpips.min_side} pixels, got {int(width)}x{int(height)}")
         super().__init__(pc, width, height, bg, outputs="float" if source == "float" else "u8", host_slots=host_slots,
                          capacity=capacity, headroom=headroom, warm_cameras=warm_cameras, warm_timesteps=warm_timesteps,
-                         views_per_replay=views_per_replay, png=png)
+                         views_per_replay=views_per_replay, png=png, mesh_opacity=mesh_opacity,
+                         face_colors=face_colors, mesh_lighting=mesh_lighting)
         self.source, self.views = source, int(views)
         self.table = torch.empty((self.views, N.METRICS_FIELDS), dtype=torch.float32, device=self.device)
         if lpips is not None and lpips.device != self.device:
@@ -1340,7 +1390,8 @@ class GraphedEval(GraphedRender):
             self.set_cursor(0)
 
     # ---- inputs ------------------------------------------------------------------------------------------------
-    def set_inputs(self, camera=None, timestep=None, gt_u8=None, view=None, verts=None, bg=None, cameras=None):
+    def set_inputs(self, camera=None, timestep=None, gt_u8=None, view=None, verts=None, bg=None, cameras=None,
+                   mesh_opacity=None, face_colors=None):
         """As GraphedRender.set_inputs, plus the view's ground truth (uint8 (3,H,W), a device tensor or a pinned host
         tensor) and its row in the table (a host int in [0, views)).  None of them re-captures.  views_per_replay=K >
         1: `cameras` (K), gt_u8 (K,3,H,W), and `view` is the first of the K rows (view + K <= views)."""
@@ -1358,7 +1409,8 @@ class GraphedEval(GraphedRender):
         want = (3, *size) if self.K == 1 else (self.K, 3, *size)
         if gt_u8 is not None and (gt_u8.dtype != torch.uint8 or tuple(gt_u8.shape) != want):
             raise ValueError(f"gt_u8 must be a uint8 {want} tensor, got {gt_u8.dtype} {tuple(gt_u8.shape)}")
-        super().set_inputs(camera=camera, timestep=timestep, verts=verts, bg=bg, cameras=cameras)
+        super().set_inputs(camera=camera, timestep=timestep, verts=verts, bg=bg, cameras=cameras,
+                           mesh_opacity=mesh_opacity, face_colors=face_colors)
         if tuple(self.gt.shape) != self._gt_shape():   # a camera of another size (the next run() re-captures)
             self._await_upload()
             self.gt = torch.zeros(self._gt_shape(), dtype=torch.uint8, device=self.device)
@@ -1395,6 +1447,11 @@ class GraphedEval(GraphedRender):
                     launch_lpips(rendered if self.K == 1 else rendered[k], self.gt if self.K == 1 else self.gt[k],
                                  self.lpips, self.lpips_table, row=self.view if self.K == 1 else self.rows[k:k + 1],
                                  skip_flag=self.slot.flag, scratch=self._lpips_scratch)
+            if self.mesh:   # render.py's renders_mesh: over the ground truth, whatever the splats did
+                with torch.no_grad():
+                    self.mesh_display = self._overlay(self.gt)
+                if self.png:
+                    self.mesh_png_out, self.mesh_png_len = self._encode(self.mesh_display)
             if self.schedule is not None:
                 self._launch_commit()
 
@@ -1429,6 +1486,14 @@ class GraphedEval(GraphedRender):
         self.replays += 1
         if self.host_slots:
             self._ship()
+
+    def host_mesh_png(self, replay: Optional[int] = None):
+        """Replay `replay`'s mesh PNG file (default: the latest) as bytes -- K files with views_per_replay=K -- once its
+        copy has landed: render.py's renders_mesh/*.png.  Given for an overflowed replay too (the mesh frame does not
+        depend on the splats)."""
+        if not (self.mesh and self.png):
+            raise ValueError("host_mesh_png needs a GraphedEval built with mesh_opacity= and png=True")
+        return self._host_files(self.host_mesh_png_slots, replay, "host_mesh_png")
 
     def run_all(self, check: bool = True) -> Optional[int]:
         """schedule=: scores every record of the order not scored yet, as back-to-back replays with no host input (R

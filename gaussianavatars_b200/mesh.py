@@ -2,6 +2,7 @@
 (mesh_renderer/__init__.py) asks of nvdiffrast, and render.py's mesh composite (render.py:75-81), fused.
 
     frame = mesh_overlay(pc.verts, pc.faces, view, gt_u8)       # render.py --render_mesh: (H,W,3) uint8 bytes
+    frames = mesh_overlay_views(pc.verts, pc.faces, cams, gts)  # K cameras of one timestep: (K,H,W,3), one call
 
 `mesh_overlay` renders at the camera's (H,W), as the reference's `use_opengl=True` path does.  Its default CUDA context
 renders at (H//8*8, W//8*8) -- or 2048x2048 when a side exceeds 2048 -- and resizes bilinearly; the two agree whenever W
@@ -89,8 +90,9 @@ def _camera_floats(camera, device) -> torch.Tensor:
 def launch_mesh(*, verts, faces, width, height, pos_kind=N.MESH_POS_WORLD, camera=None, adjacency=None,
                 face_colors=None, background=(1.0, 1.0, 1.0), lighting="front", antialias=True, base=None,
                 opacity=None, out_u8=None, out_float=None, out_rgba=None, out_rast=None, in_rast=None, in_color=None,
-                out_color=None, error_flag=None, stream=None):
-    """One gab200_mesh_render call on device tensors (no checks beyond the library's own); returns nothing."""
+                out_color=None, error_flag=None, stream=None, views=None):
+    """One gab200_mesh_render call on device tensors (no checks beyond the library's own); returns nothing.
+    views=K: one gab200_mesh_render_views call instead -- camera a (K,37) table, base (K,3,H,W), out_u8 (K,H,W,3)."""
     dev = verts.device
     F = faces.shape[0]
     _check_size(width, height)
@@ -113,11 +115,16 @@ def launch_mesh(*, verts, faces, width, height, pos_kind=N.MESH_POS_WORLD, camer
     a.channels = 0 if in_color is None else in_color.shape[-1]
     a.error_flag = N.ptr(error_flag)
     L = N.lib()
-    nbytes = L.gab200_mesh_scratch_bytes(F, width, height)
+    nbytes = L.gab200_mesh_scratch_bytes(F, width, height) if views is None else \
+        L.gab200_mesh_views_scratch_bytes(int(views), F, width, height)
     scratch = torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=dev)
     a.scratch = scratch.data_ptr()
     s = torch.cuda.current_stream(dev) if stream is None else stream
-    N.check(L.gab200_mesh_render(C.byref(a), C.c_void_p(s.cuda_stream)), "gab200_mesh_render")
+    if views is None:
+        N.check(L.gab200_mesh_render(C.byref(a), C.c_void_p(s.cuda_stream)), "gab200_mesh_render")
+    else:
+        N.check(L.gab200_mesh_render_views(C.byref(a), int(views), C.c_void_p(s.cuda_stream)),
+                "gab200_mesh_render_views")
 
 
 def opacity_pair(mesh_opacity: float, device) -> torch.Tensor:
@@ -182,6 +189,56 @@ def mesh_overlay(verts: torch.Tensor, faces: torch.Tensor, camera, base: torch.T
                 antialias=antialias, base=base.detach().to(dev).contiguous(), opacity=opacity_pair(mesh_opacity, dev),
                 out_u8=result if out == "u8" else None, out_float=result if out == "float" else None,
                 error_flag=error_flag)
+    return result
+
+
+def _check_cameras(cameras, K: int, W: int, H: int):
+    """K camera objects of the base's size, or a (K,37) float32 table; returns the objects' list, or the table."""
+    if isinstance(cameras, torch.Tensor):
+        if tuple(cameras.shape) != (K, N.CAMERA_FLOATS) or cameras.dtype != torch.float32:
+            raise ValueError(f"the camera table of {K} views is ({K},{N.CAMERA_FLOATS}) float32 "
+                             f"(renderer.camera_table), got {tuple(cameras.shape)} {cameras.dtype}")
+        return cameras.detach()
+    cams = list(cameras)
+    if len(cams) != K:
+        raise ValueError(f"{len(cams)} cameras for {K} base planes")
+    for c in cams:
+        if (int(c.image_width), int(c.image_height)) != (W, H):
+            raise ValueError(f"a camera is {c.image_width}x{c.image_height}, base is {W}x{H}")
+    return cams
+
+
+def mesh_overlay_views(verts: torch.Tensor, faces: torch.Tensor, cameras, base: torch.Tensor,
+                       mesh_opacity: float = 0.5, face_colors: Optional[torch.Tensor] = None,
+                       background: Sequence[float] = (1.0, 1.0, 1.0), lighting: str = "front", antialias: bool = True,
+                       error_flag: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """mesh_overlay under K cameras of one vertex set in one call (gab200_mesh_render_views): frame k is bit for bit
+    mesh_overlay(verts, faces, cameras[k], base[k], ...) with out="u8".
+    cameras: K camera objects of the base's size, or a (K,37) float32 table (renderer.camera_table); base (K,3,H,W)
+    float32, or uint8 read as value/255.  Returns (K,H,W,3) uint8.  The scratch holds K winner maps: K * 8 * H * W
+    bytes and more (~265 MB for K = 16 at 1080p)."""
+    if base.dim() != 4 or base.shape[1] != 3 or base.dtype not in (torch.float32, torch.uint8):
+        raise ValueError(f"base must be (K,3,H,W) float32 or uint8, got {tuple(base.shape)} {base.dtype}")
+    K, H, W = int(base.shape[0]), int(base.shape[2]), int(base.shape[3])
+    if not 1 <= K <= N.MAX_VIEWS:
+        raise ValueError(f"base holds 1 .. {N.MAX_VIEWS} views, got {K}")
+    _check_size(W, H)
+    cams = _check_cameras(cameras, K, W, H)
+    v = _verts_v3(verts)
+    dev = v.device
+    if isinstance(cams, torch.Tensor):
+        table = cams.to(dev).contiguous()
+    else:
+        from .renderer import camera_table
+
+        table = camera_table(cams, dev)
+    f = _faces_i32(faces, dev)
+    adj = _overlay_adjacency.get(faces).to(dev) if antialias else None
+    result = torch.empty(K, H, W, 3, dtype=torch.uint8, device=dev)
+    launch_mesh(verts=v, faces=f, width=W, height=H, camera=table, adjacency=adj,
+                face_colors=_face_colors(face_colors, f.shape[0], dev), background=background, lighting=lighting,
+                antialias=antialias, base=base.detach().to(dev).contiguous(), opacity=opacity_pair(mesh_opacity, dev),
+                out_u8=result, error_flag=error_flag, views=K)
     return result
 
 

@@ -803,6 +803,26 @@ typedef struct gab200_mesh_args {
 size_t gab200_mesh_scratch_bytes(int32_t num_faces, int32_t width, int32_t height);
 int32_t gab200_mesh_render(const gab200_mesh_args* args, void* stream);
 
+/* The tracked mesh over every camera of a rig in one call: one vertex set drawn under `views` cameras, in the same
+ * four launches as gab200_mesh_render (each (view, face) and each (view, pixel) one thread; the raster work items of
+ * all views shared by the same persistent warps).  View k of the call is bit for bit gab200_mesh_render with camera
+ * row k, base plane k and the same other arguments -- out_u8 plane k and error_flag; views == 1 is that call.
+ *   args->camera: DEVICE float[views][GAB200_CAMERA_FLOATS], row k view k's 37-float block (as gab200_forward_views)
+ *   args->base:   [views,3,H,W] float (GAB200_MESH_BASE_FLOAT_CHW) or uint8 (GAB200_MESH_BASE_U8_CHW), plane k view k's
+ *   args->out_u8: [views,H,W,3] uint8, plane k view k's composite
+ * Everything else (verts, faces, adjacency, face_colors, background, lighting, antialias, opacity, error_flag) is
+ * shared by the views and means what it means for gab200_mesh_render.
+ * scratch: gab200_mesh_views_scratch_bytes(views, F, width, height) bytes, 256-byte aligned: `views` times one view's
+ * face records (304 bytes per face) and winner map (8 bytes per pixel) plus the prefix sum's temporary space -- about
+ * views * (8 W H + 304 F) bytes, so 16 views of a 9,996-face head at 1920x1080 take ~314 MB; 0 for a refused size.
+ * views == 1 is gab200_mesh_scratch_bytes.
+ * Invalid arguments (GAB200_ERR_INVALID_ARGUMENT, before any device work): every error of gab200_mesh_render, views
+ * outside [1, 65535], views * F > INT32_MAX, pos_kind GAB200_MESH_POS_CLIP, a NULL out_u8 (and
+ * so a missing base or opacity), and any of out_rgba, out_float, out_rast, in_rast, in_color, out_color: the K-view
+ * call composites uint8 frames only. */
+size_t gab200_mesh_views_scratch_bytes(int32_t views, int32_t num_faces, int32_t width, int32_t height);
+int32_t gab200_mesh_render_views(const gab200_mesh_args* args, int32_t views, void* stream);
+
 /* Adam over several parameter arrays in one launch (SURVEY.md 8f rank 3).  Replaces `gaussians.optimizer.step()` for
  * the splat parameter groups (scene/gaussian_model.py:213-232 builds `torch.optim.Adam(l, lr=0.0, eps=1e-15)` with one
  * group -- and one learning rate -- per array; train.py:207-209): amsgrad off, no weight decay, bias-corrected, `step`
