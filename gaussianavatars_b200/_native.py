@@ -238,7 +238,9 @@ EXPORTED_SYMBOLS = ("gab200_forward", "gab200_backward", "gab200_mark_visible", 
                     "gab200_png_copy", "gab200_png_status_string", "gab200_png_decode_scratch_bytes",
                     "gab200_png_decode", "gab200_resize_scratch_bytes", "gab200_resize_u8",
                     "gab200_h264_bound", "gab200_h264_scratch_bytes", "gab200_h264_encode",
-                    "gab200_h264_parameter_sets", "gab200_mesh_views_scratch_bytes", "gab200_mesh_render_views")
+                    "gab200_h264_parameter_sets", "gab200_mesh_views_scratch_bytes", "gab200_mesh_render_views",
+                    "gab200_h264_p_bound", "gab200_h264_state_bytes", "gab200_h264_stream_scratch_bytes",
+                    "gab200_h264_encode_stream", "gab200_h264_stream_parameter_sets")
 
 _lib = None
 _lock = threading.Lock()
@@ -374,6 +376,16 @@ def lib():
         L.gab200_h264_encode.argtypes = [C.c_int32] * 4 + [C.c_void_p] * 3 + [C.c_int64, C.c_void_p, C.c_void_p]
         L.gab200_h264_parameter_sets.restype = C.c_int32
         L.gab200_h264_parameter_sets.argtypes = [C.c_int32] * 5 + [C.c_void_p, C.c_int64]
+        L.gab200_h264_p_bound.restype = C.c_int64
+        L.gab200_h264_p_bound.argtypes = [C.c_int32, C.c_int32]
+        L.gab200_h264_state_bytes.restype = C.c_size_t
+        L.gab200_h264_state_bytes.argtypes = [C.c_int32, C.c_int32]
+        L.gab200_h264_stream_scratch_bytes.restype = C.c_size_t
+        L.gab200_h264_stream_scratch_bytes.argtypes = [C.c_int32] * 4
+        L.gab200_h264_encode_stream.restype = C.c_int32
+        L.gab200_h264_encode_stream.argtypes = [C.c_int32] * 5 + [C.c_void_p] * 4 + [C.c_int64, C.c_void_p, C.c_void_p]
+        L.gab200_h264_stream_parameter_sets.restype = C.c_int32
+        L.gab200_h264_stream_parameter_sets.argtypes = [C.c_int32] * 6 + [C.c_void_p, C.c_int64]
         L.gab200_schedule_sample.restype = C.c_int32
         L.gab200_schedule_sample.argtypes = [C.c_int32, C.c_int32, C.c_int32] + [C.c_void_p] * 11
         L.gab200_schedule_commit.restype = C.c_int32

@@ -1065,13 +1065,42 @@ int32_t gab200_h264_encode(int32_t frames, int32_t height, int32_t width, int32_
   if (out_stride < h264_bound(width, height)) return GAB200_ERR_INVALID_ARGUMENT;
   if (!rgb || !scratch || !out || !out_len || ((uintptr_t)scratch & 255) != 0) return GAB200_ERR_INVALID_ARGUMENT;
   if (check_arch() < 0) return GAB200_ERR_ARCH;
-  launch_h264_encode(frames, height, width, qp, rgb, scratch, out, out_stride, out_len, (cudaStream_t)stream_);
+  launch_h264_encode(frames, height, width, qp, 1, rgb, nullptr, scratch, out, out_stride, out_len,
+                     (cudaStream_t)stream_);
   return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
 }
 
 int32_t gab200_h264_parameter_sets(int32_t width, int32_t height, int32_t qp, int32_t fps_num, int32_t fps_den,
                                    uint8_t* out, int64_t cap) {
-  return h264_parameter_sets(width, height, qp, fps_num, fps_den, out, cap);
+  return h264_parameter_sets(width, height, qp, fps_num, fps_den, 1, out, cap);
+}
+
+int64_t gab200_h264_p_bound(int32_t width, int32_t height) { return h264_p_bound(width, height); }
+
+size_t gab200_h264_state_bytes(int32_t height, int32_t width) { return h264_state_bytes(height, width); }
+
+size_t gab200_h264_stream_scratch_bytes(int32_t frames, int32_t height, int32_t width, int32_t gop) {
+  if (gop < 1 || gop > 65535) return 0;
+  return h264_scratch_bytes(frames, height, width);
+}
+
+int32_t gab200_h264_encode_stream(int32_t frames, int32_t height, int32_t width, int32_t qp, int32_t gop,
+                                  const uint8_t* rgb, void* state, void* scratch, uint8_t* out, int64_t out_stride,
+                                  int64_t* out_len, void* stream_) {
+  if (h264_scratch_bytes(frames, height, width) == 0 || qp < 0 || qp > 51 || gop < 1 || gop > 65535)
+    return GAB200_ERR_INVALID_ARGUMENT;
+  if (out_stride < (gop > 1 ? h264_p_bound(width, height) : h264_bound(width, height))) return GAB200_ERR_INVALID_ARGUMENT;
+  if (!rgb || !state || !scratch || !out || !out_len) return GAB200_ERR_INVALID_ARGUMENT;
+  if (((uintptr_t)scratch & 255) != 0 || ((uintptr_t)state & 255) != 0) return GAB200_ERR_INVALID_ARGUMENT;
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  launch_h264_encode(frames, height, width, qp, gop, rgb, static_cast<uint8_t*>(state), scratch, out, out_stride,
+                     out_len, (cudaStream_t)stream_);
+  return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
+int32_t gab200_h264_stream_parameter_sets(int32_t width, int32_t height, int32_t qp, int32_t fps_num, int32_t fps_den,
+                                          int32_t gop, uint8_t* out, int64_t cap) {
+  return h264_parameter_sets(width, height, qp, fps_num, fps_den, gop, out, cap);
 }
 
 size_t gab200_resize_scratch_bytes(int64_t planes, int32_t in_height, int32_t in_width, int32_t out_height,

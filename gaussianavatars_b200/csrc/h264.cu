@@ -1,20 +1,28 @@
 // h264.cu -- H.264 video frames encoded on the device (gab200_h264_bound / gab200_h264_scratch_bytes /
-// gab200_h264_encode / gab200_h264_parameter_sets): Constrained Baseline, every picture one IDR slice, CAVLC,
-// deblocking off, one fixed QP; each macroblock I_16x16 (luma and chroma modes of least SATD) or I_PCM.
-// oracle/h264.py restates every step, and the tests compare its bytes with these.
+// gab200_h264_encode / gab200_h264_parameter_sets, and for streams with P pictures gab200_h264_p_bound /
+// gab200_h264_state_bytes / gab200_h264_encode_stream / gab200_h264_stream_parameter_sets): Constrained Baseline,
+// CAVLC, deblocking off, one fixed QP.  An IDR picture's macroblocks are I_16x16 (luma and chroma modes of least SATD)
+// or I_PCM; a P picture's are P_Skip, P_L0_16x16 (one quarter-sample vector), I_16x16 or I_PCM.  oracle/h264.py and
+// tests/h264_stream_oracle.py restate every step, and the tests compare their bytes with these.
 //
 // Per batch of frames the encode runs these kernels, each named for a trace:
 //   h264_convert_kernel  RGB -> BT.601 limited-range Y, Cb, Cr planes padded to whole macroblocks by edge replication.
-//   h264_mb_kernel       one launch per anti-diagonal d = mbx + mby (W/16 + H/16 - 1 launches), one 128-thread CTA per
-//                        (macroblock on d, frame): prediction from the reconstructed left / top / top-left samples of
-//                        earlier diagonals, mode decision by SATD, transform, quantisation, reconstruction into the
-//                        recon planes, per-4x4 TotalCoeff, the macroblock's CAVLC bit count and the I_PCM fallback;
-//                        the levels are kept for the writer.  The per-diagonal launch is the wavefront's only
-//                        synchronisation: no CTA ever waits on another.
+//   h264_frame_kernel    each frame's picture type and frame_num from the stream position in the state.
+//   h264_mb_kernel       one launch per step of a wavefront over (frame, anti-diagonal d = mbx + mby): frame f runs
+//                        diagonal step - lag f, lag 0 when every frame is an IDR picture (W/16 + H/16 - 1 launches)
+//                        and LAG when a frame refers to the one before (LAG more launches per frame).  One 128-thread
+//                        CTA per (macroblock on d, frame): in a P picture the motion search in the previous picture;
+//                        prediction from the reconstructed left / top / top-left samples of earlier diagonals, mode
+//                        decision by SATD, transform, quantisation, reconstruction into the recon planes, per-4x4
+//                        TotalCoeff, the macroblock's CAVLC bit count and the I_PCM fallback; the levels are kept for
+//                        the writer.  The launch boundary is the wavefront's only synchronisation: no CTA ever waits
+//                        on another.
+//   h264_mvp_kernel      P pictures, one thread per macroblock: the vector predictors, P_Skip and the mvd bits.
+//   h264_run_kernel      P pictures, one thread per macroblock: the skip runs and their bits.
 //   h264_scan_kernel     one CTA per frame: the macroblocks' bit offsets in raster order, an exclusive scan of the maps
-//                        x -> x + L (I_16x16) and x -> ceil8(x + 9) + 3072 (I_PCM, whose samples start byte-aligned),
-//                        a family closed under composition; zeroes the slice's words and writes the slice header and
-//                        the stop bit.
+//                        x -> x + L and x -> ceil8(x + r + 9) + 3072 (I_PCM behind a skip run of r bits, its samples
+//                        byte-aligned), a family closed under composition; zeroes the slice's words and writes the
+//                        slice header and the stop bit.
 //   h264_write_kernel    one warp per macroblock: its bits at its offset, one lane per residual block, OR-ed into the
 //                        slice's words with atomics (neighbours share the first and last word).
 //   h264_ep_count_kernel one thread per 256-byte piece of the slice: for each zero-run state the piece can start in
@@ -22,7 +30,9 @@
 //   h264_ep_plan_kernel  one warp per frame: the pieces' start states and output offsets in order, the sample's length
 //                        and its 4-byte length prefix and NAL header.
 //   h264_ep_emit_kernel  one thread per piece: its bytes, with 0x03 inserted, into the frame's output slot.
+//   h264_state_kernel    the last frame's reconstruction and the advanced position into the stream's state.
 #include <algorithm>
+#include <climits>
 #include <vector>
 
 #include "common.cuh"
@@ -38,6 +48,21 @@ constexpr int HEADER_BITS = 22;              // the slice header (idr_pic_id 1)
 constexpr int EP_PIECE = 256;                // bytes of the slice per emulation-prevention piece
 constexpr int MAX_MBS = 36864;               // level 5.2's MaxFS
 constexpr int BLOCKS = 27;                   // residual blocks of a macroblock, in bitstream order (see h264_mb_kernel)
+constexpr int P_HEADER_BITS = 18;            // the P slice header
+constexpr int SEARCH = 16;                   // integer motion search range, samples
+constexpr int MVD_BITS = 2 * 17;             // se(v) of the largest |mvd|, 2 * (4 SEARCH + 3) quarter samples, twice
+constexpr int INTRA_BIAS = 24;               // intra's SATD handicap against inter, in units of lambda
+// A vector reaches 4 SEARCH + 3 quarter samples, and the 6-tap filter 2 samples before and 3 after: the window of a
+// macroblock's reference samples spans REACH samples on each side, WIN samples in all.
+constexpr int REACH = (4 * SEARCH + 3) / 4 + 3;
+constexpr int WIN_OFF = REACH + 1;
+constexpr int WIN = 16 + 2 * WIN_OFF;
+// Frame f + 1 runs diagonal d in the launch where frame f runs d + LAG: its window reaches REACH_MB macroblocks right
+// and down, so frame f must have finished diagonal d + 2 REACH_MB in an earlier launch.
+constexpr int REACH_MB = (REACH + 15) / 16;
+constexpr int LAG = 2 * REACH_MB + 1;
+static_assert(LAG == 5, "the stream's frame lag");
+static_assert(16 * REACH_MB >= REACH, "the reference window stays within REACH_MB macroblocks");
 
 __constant__ int8_t c_zigzag[16] = {0, 1, 4, 8, 5, 2, 3, 6, 9, 12, 13, 10, 7, 11, 14, 15};
 __constant__ int8_t c_chroma_qp[52] = {0,  1,  2,  3,  4,  5,  6,  7,  8,  9,  10, 11, 12, 13, 14, 15, 16, 17,
@@ -46,6 +71,10 @@ __constant__ int8_t c_chroma_qp[52] = {0,  1,  2,  3,  4,  5,  6,  7,  8,  9,  1
 __constant__ int c_mf[6][3] = {{13107, 5243, 8066}, {11916, 4660, 7490}, {10082, 4194, 6554},
                                {9362, 3647, 5825},  {8192, 3355, 5243},  {7282, 2893, 4559}};
 __constant__ int c_v[6][3] = {{10, 16, 13}, {11, 18, 14}, {13, 20, 16}, {14, 23, 18}, {16, 25, 20}, {18, 29, 23}};
+// Table 9-4, inter column: coded_block_pattern -> codeNum
+__constant__ uint8_t c_inter_cbp[48] = {0,  2,  3,  7,  4,  8,  17, 13, 5,  18, 9,  14, 10, 15, 16, 11,
+                                        1,  32, 33, 36, 34, 37, 44, 40, 35, 45, 38, 41, 39, 42, 43, 19,
+                                        6,  24, 25, 20, 26, 21, 46, 28, 27, 47, 22, 29, 23, 30, 31, 12};
 // luma4x4BlkIdx -> (x, y) of the 4x4 block in the macroblock, in blocks
 __constant__ int8_t c_blk_x[16] = {0, 1, 0, 1, 2, 3, 2, 3, 0, 1, 0, 1, 2, 3, 2, 3};
 __constant__ int8_t c_blk_y[16] = {0, 0, 1, 1, 0, 0, 1, 1, 2, 2, 3, 3, 2, 2, 3, 3};
@@ -107,12 +136,16 @@ __constant__ uint8_t c_rb_code[7][15] = {{1, 0},          {1, 1, 0},          {3
 // The per-frame scratch: offsets from the frame's base (each 256-byte aligned), and the frame stride.
 struct Layout {
   int W, H, wm, hm, nmb, pieces;
-  int64_t src, rec, tot, lev, info, bits, off, raw, ep, meta, stride;
+  int64_t src, rec, tot, lev, info, bits, off, mv, mvd, run, raw, ep, meta, stride;
 };
 
 int64_t align256(int64_t x) { return (x + 255) / 256 * 256; }
 
 int64_t raw_bytes_bound(int nmb) { return (HEADER_BITS + (int64_t)nmb * (PCM_BITS + 7) + 1 + 7) / 8; }
+// A P slice: a skip run of at most 3 bits per macroblock it closes, the mvd and I_PCM at its worst alignment.
+int64_t raw_bytes_bound_p(int nmb) {
+  return (P_HEADER_BITS + (int64_t)nmb * (3 + MVD_BITS + PCM_BITS + 7) + 1 + 7) / 8;
+}
 
 Layout layout(int H, int W) {
   Layout l;
@@ -121,7 +154,7 @@ Layout layout(int H, int W) {
   l.wm = (W + 15) / 16;
   l.hm = (H + 15) / 16;
   l.nmb = l.wm * l.hm;
-  const int64_t raw = raw_bytes_bound(l.nmb);
+  const int64_t raw = std::max(raw_bytes_bound(l.nmb), raw_bytes_bound_p(l.nmb));
   l.pieces = (int)((raw + EP_PIECE - 1) / EP_PIECE);
   const int64_t plane = (int64_t)l.nmb * 384;   // Y, Cb, Cr of every macroblock
   int64_t o = 0;
@@ -132,9 +165,12 @@ Layout layout(int H, int W) {
   l.info = o; o = align256(o + (int64_t)l.nmb * 4);
   l.bits = o; o = align256(o + (int64_t)l.nmb * 4);
   l.off = o;  o = align256(o + (int64_t)l.nmb * 4);
+  l.mv = o;   o = align256(o + (int64_t)l.nmb * 4);                   // P: x | y << 16, quarter samples
+  l.mvd = o;  o = align256(o + (int64_t)l.nmb * 4);
+  l.run = o;  o = align256(o + (int64_t)l.nmb * 4);                   // P: the skip run coded before the macroblock
   l.raw = o;  o = align256(o + (raw + 7) / 4 * 4 + 4);                // the slice's words, one spare
   l.ep = o;   o = align256(o + (int64_t)l.pieces * 16);               // per piece: 3 counts + end states | start state
-  l.meta = o; o = align256(o + 16);                                   // raw byte count
+  l.meta = o; o = align256(o + 16);                                   // raw byte count, P picture, frame_num
   l.stride = o;
   return l;
 }
@@ -209,7 +245,7 @@ struct BitSink {
 };
 
 // One residual_block_cavlc (9.2) of coefficients c[0 .. maxn) in scan order, context nc (-1: chroma DC); returns bits.
-__device__ int cavlc_block(const int* c, int maxn, int nc, BitSink& s) {
+__device__ __forceinline__ int cavlc_block(const int* c, int maxn, int nc, BitSink& s) {
   const int n0 = s.n;
   int total = 0, last = -1;
   for (int i = 0; i < maxn; i++)
@@ -296,12 +332,26 @@ __device__ void block_geom(int id, int mx, int my, int& plane, int& x, int& y, i
   else { const int b = (id - 19) & 3; plane = 1 + (id - 19) / 4; x = 2 * mx + (b & 1); y = 2 * my + (b >> 1); maxn = 15; }
 }
 
-__device__ __forceinline__ bool block_present(int id, int cbpl, int cbpc) {
-  return id == 0 || (id <= 16 && cbpl) || (id > 16 && id <= 18 && cbpc >= 1) || (id > 18 && cbpc == 2);
+// A macroblock's info word: luma mode (bits 0-1), chroma mode (2-3), CodedBlockPatternChroma (4-5), I_16x16 AC
+// coded (6), I_PCM (7), P_L0_16x16 (8), its CodedBlockPatternLuma (9-12), P_Skip (13).
+__device__ __forceinline__ bool block_present(int id, int info) {
+  const bool inter = (info >> 8) & 1;
+  const int cbpc = (info >> 4) & 3;
+  if (id == 0) return !inter;
+  if (id <= 16) return inter ? (info >> (9 + ((id - 1) >> 2))) & 1 : (info >> 6) & 1;
+  return id <= 18 ? cbpc >= 1 : cbpc == 2;
 }
 
-__device__ __forceinline__ int mb_header_bits(int lmode, int cmode, int cbpl, int cbpc) {
-  return ue_bits(1 + lmode + 4 * cbpc + (cbpl ? 12 : 0)) + ue_bits(cmode) + 1;
+__device__ __forceinline__ int i16_mb_type(int info, bool is_p) {
+  return 1 + (info & 3) + 4 * ((info >> 4) & 3) + ((info >> 6) & 1 ? 12 : 0) + (is_p ? 5 : 0);
+}
+
+__device__ __forceinline__ int inter_cbp(int info) { return ((info >> 9) & 15) | ((info >> 4) & 3) << 4; }
+
+// mb_type through mb_qp_delta: I_16x16 (mb_type + 5 in a P slice), or P_L0_16x16 without its mvd
+__device__ __forceinline__ int mb_header_bits(int info, bool is_p) {
+  if ((info >> 8) & 1) return 1 + ue_bits(c_inter_cbp[inter_cbp(info)]) + (inter_cbp(info) ? 1 : 0);
+  return ue_bits(i16_mb_type(info, is_p)) + ue_bits((info >> 2) & 3) + 1;
 }
 
 // ---- the macroblock kernel ---------------------------------------------------------------------------------------
@@ -333,16 +383,19 @@ __device__ void idct4(int* d) {
 struct MbShared {
   int src[384];          // Y (16x16), Cb (8x8), Cr (8x8)
   int pred[384];         // the chosen modes' predictions
+  int ipred[384];        // P: the inter prediction at the chosen vector
   int top[32], left[32]; // luma 0..15, Cb 16..23, Cr 24..31
   int tl[3];
   int par[3][8];         // per plane: DC value(s) and the plane parameters a, b, c
   int cost[8];           // SATD of luma modes 0..3, chroma modes 0..3
   int w[24][16];         // transform coefficients, then dequantised coefficients
-  int lev[24][16];       // quantised AC levels (raster; [0] unused)
+  int lev[24][16];       // quantised levels (raster; [0] unused in intra blocks)
   int dc[16], cdc[2][4]; // quantised DC levels (luma [by * 4 + bx], chroma raster)
   int dcr[16], cdcr[2][4];
   int tot[24];
-  int maxlev, bits, lmode, cmode, cbpl, cbpc, pcm;
+  int c9[9];             // P: the costs of a refinement's candidates
+  uint8_t win[WIN * WIN];// P: the reference samples around the macroblock, coordinates clamped to the picture
+  int maxlev, bits, lmode, cmode, cbpl, cbpc, pcm, inter, key, mvx, mvy, icost;
 };
 
 __device__ int predict(const MbShared& s, int plane, int mode, int x, int y) {
@@ -363,16 +416,156 @@ __device__ int predict(const MbShared& s, int plane, int mode, int x, int y) {
   }
 }
 
-__global__ void __launch_bounds__(128) h264_mb_kernel(int d, int qp, uint8_t* scratch, Layout l) {
+__device__ __forceinline__ int se_bits(int v) { return ue_bits(v > 0 ? 2 * v - 1 : -2 * v); }
+__device__ __forceinline__ int lambda_of(int qp) { return 1 << max(0, (qp - 12) / 6); }
+
+__device__ __forceinline__ int tap6(const uint8_t* p, int step) {
+  return p[-2 * step] - 5 * p[-step] + 20 * p[0] + 20 * p[step] - 5 * p[2 * step] + p[3 * step];
+}
+
+// 8.4.2.2.1: the luma sample at (x, y) of the macroblock displaced by (mvx, mvy) quarter samples, from the window.
+__device__ __forceinline__ int luma_at(const uint8_t* win, int x, int y, int mvx, int mvy) {
+  const int xf = mvx & 3, yf = mvy & 3;
+  const uint8_t* g = win + (WIN_OFF + y + (mvy >> 2)) * WIN + WIN_OFF + x + (mvx >> 2);
+  if (!xf && !yf) return g[0];
+  const int b = clip255((tap6(g, 1) + 16) >> 5), h = clip255((tap6(g, WIN) + 16) >> 5);
+  const int s = clip255((tap6(g + WIN, 1) + 16) >> 5), m = clip255((tap6(g + 1, WIN) + 16) >> 5);
+  int j = 0;
+  if ((xf == 2 && yf) || (yf == 2 && xf)) {
+    int v[6];
+    for (int k = 0; k < 6; k++) v[k] = tap6(g + k - 2, WIN);
+    j = clip255((v[0] - 5 * v[1] + 20 * v[2] + 20 * v[3] - 5 * v[4] + v[5] + 512) >> 10);
+  }
+  auto avg = [](int p, int q) { return (p + q + 1) >> 1; };
+  switch (yf * 4 + xf) {
+    case 1: return avg(g[0], b);
+    case 2: return b;
+    case 3: return avg(g[1], b);
+    case 4: return avg(g[0], h);
+    case 5: return avg(b, h);
+    case 6: return avg(b, j);
+    case 7: return avg(b, m);
+    case 8: return h;
+    case 9: return avg(h, j);
+    case 10: return j;
+    case 11: return avg(j, m);
+    case 12: return avg(g[WIN], h);
+    case 13: return avg(h, s);
+    case 14: return avg(j, s);
+    default: return avg(m, s);
+  }
+}
+
+// 8.4.2.2.2: the chroma sample at (x, y) of plane p's coded picture displaced by (mvx, mvy) eighth samples.
+__device__ __forceinline__ int chroma_at(const Planes& ref, const Layout& l, int p, int x, int y, int mvx, int mvy) {
+  const int xi = x + (mvx >> 3), yi = y + (mvy >> 3), xf = mvx & 7, yf = mvy & 7;
+  const int w1 = 8 * l.wm - 1, h1 = 8 * l.hm - 1;
+  const uint8_t* pl = ref.chroma(p);
+  const int x0 = min(max(xi, 0), w1), x1 = min(max(xi + 1, 0), w1);
+  const int y0 = min(max(yi, 0), h1) * ref.cs, y1 = min(max(yi + 1, 0), h1) * ref.cs;
+  return ((8 - xf) * (8 - yf) * pl[y0 + x0] + xf * (8 - yf) * pl[y0 + x1] + (8 - xf) * yf * pl[y1 + x0] +
+          xf * yf * pl[y1 + x1] + 32) >> 6;
+}
+
+__device__ __forceinline__ int satd4(const int* r) {   // r: 16 residuals, raster; sum of |4x4 Hadamard|
+  int q[16];
+  for (int i = 0; i < 4; i++) {
+    const int a0 = r[4 * i] + r[4 * i + 1], a1 = r[4 * i] - r[4 * i + 1];
+    const int a2 = r[4 * i + 2] + r[4 * i + 3], a3 = r[4 * i + 2] - r[4 * i + 3];
+    q[4 * i] = a0 + a2; q[4 * i + 1] = a1 + a3; q[4 * i + 2] = a0 - a2; q[4 * i + 3] = a1 - a3;
+  }
+  int sum = 0;
+  for (int j = 0; j < 4; j++) {
+    const int a0 = q[j] + q[4 + j], a1 = q[j] - q[4 + j], a2 = q[8 + j] + q[12 + j], a3 = q[8 + j] - q[12 + j];
+    sum += abs(a0 + a2) + abs(a1 + a3) + abs(a0 - a2) + abs(a1 - a3);
+  }
+  return sum;
+}
+
+__constant__ int8_t c_nb[8][2] = {{-1, -1}, {0, -1}, {1, -1}, {-1, 0}, {1, 0}, {-1, 1}, {0, 1}, {1, 1}};  // (dx, dy)
+
+// The motion search of a P macroblock (128 threads): an integer full search over +-SEARCH samples by SAD, then a
+// half- and a quarter-sample refinement over the 8 neighbours by SATD, each cost + lambda * the vector's se(v) bits;
+// every minimum keeps the first candidate (raster order, then the centre before its neighbours).  Leaves the vector in
+// s.mvx / s.mvy, its cost in s.icost and its luma and chroma prediction in s.ipred.
+__device__ __forceinline__ void motion_search(MbShared& s, const Planes& ref, const Layout& l, int mx, int my, int qp) {
+  const int t = threadIdx.x, L = lambda_of(qp);
+  const int x0 = 16 * mx - WIN_OFF, y0 = 16 * my - WIN_OFF, wc = 16 * l.wm, hc = 16 * l.hm;
+  for (int i = t; i < WIN * WIN; i += 128) {
+    const int x = min(max(x0 + i % WIN, 0), wc - 1), y = min(max(y0 + i / WIN, 0), hc - 1);
+    s.win[i] = ref.y[(int64_t)y * ref.ys + x];
+  }
+  if (t == 0) s.key = INT_MAX;
+  __syncthreads();
+  constexpr int SIDE = 2 * SEARCH + 1;
+  int best = INT_MAX;
+  for (int c = t; c < SIDE * SIDE; c += 128) {
+    const int dx = c % SIDE - SEARCH, dy = c / SIDE - SEARCH;
+    int sad = 0;
+    for (int y = 0; y < 16; y++) {
+      const uint8_t* row = s.win + (WIN_OFF + y + dy) * WIN + WIN_OFF + dx;
+      for (int x = 0; x < 16; x++) sad += abs(s.src[16 * y + x] - (int)row[x]);
+    }
+    best = min(best, (sad + L * (se_bits(4 * dx) + se_bits(4 * dy))) << 11 | c);
+  }
+  atomicMin(&s.key, best);
+  __syncthreads();
+  int mvx = 4 * ((s.key & 2047) % SIDE - SEARCH), mvy = 4 * ((s.key & 2047) / SIDE - SEARCH);
+  for (int step = 2; step >= 1; step--) {
+    if (t < 9) {
+      const int vx = mvx + (t ? c_nb[t - 1][0] * step : 0), vy = mvy + (t ? c_nb[t - 1][1] * step : 0);
+      s.c9[t] = L * (se_bits(vx) + se_bits(vy));
+    }
+    __syncthreads();
+    for (int task = t; task < 9 * 16; task += 128) {
+      const int k = task / 16, bx = task & 3, by = (task >> 2) & 3;
+      const int vx = mvx + (k ? c_nb[k - 1][0] * step : 0), vy = mvy + (k ? c_nb[k - 1][1] * step : 0);
+      int r[16];
+      for (int i = 0; i < 16; i++) {
+        const int x = 4 * bx + (i & 3), y = 4 * by + (i >> 2);
+        r[i] = s.src[16 * y + x] - luma_at(s.win, x, y, vx, vy);
+      }
+      atomicAdd(&s.c9[k], satd4(r));
+    }
+    __syncthreads();
+    int k = 0;
+    for (int i = 1; i < 9; i++)
+      if (s.c9[i] < s.c9[k]) k = i;
+    if (k) { mvx += c_nb[k - 1][0] * step; mvy += c_nb[k - 1][1] * step; }
+    if (step == 1 && t == 0) { s.mvx = mvx; s.mvy = mvy; s.icost = s.c9[k]; }
+    __syncthreads();
+  }
+  for (int i = t; i < 384; i += 128) {
+    if (i < 256) s.ipred[i] = luma_at(s.win, i & 15, i >> 4, mvx, mvy);
+    else {
+      const int p = (i - 256) / 64, j = (i - 256) % 64;
+      s.ipred[i] = chroma_at(ref, l, p, 8 * mx + (j & 7), 8 * my + (j >> 3), mvx, mvy);
+    }
+  }
+}
+
+// Frame f's P picture flag and frame_num from the stream position.
+__device__ __forceinline__ const int* frame_meta(const uint8_t* scratch, const Layout& l, int f) {
+  return reinterpret_cast<const int*>(scratch + (int64_t)f * l.stride + l.meta);
+}
+
+// One launch per step of the wavefront over (frame, anti-diagonal): frame f runs diagonal step - lag f (lag 0 when
+// every frame is an IDR picture; LAG when a frame refers to the one before it).
+__global__ void __maxnreg__(80) h264_mb_kernel(int step, int lag, int f_lo, int qp, uint8_t* scratch,
+                                                      const uint8_t* state, Layout l) {
   __shared__ MbShared s;
-  const int f = blockIdx.y, t = threadIdx.x;
+  const int f = f_lo + blockIdx.y, t = threadIdx.x;
+  const int d = step - lag * f;
+  if (d < 0 || d >= l.wm + l.hm - 1) return;
   const int mx = max(0, d - l.hm + 1) + blockIdx.x, my = d - mx;
+  if (mx > min(d, l.wm - 1)) return;
   const int mb = my * l.wm + mx;
   const bool has_l = mx > 0, has_t = my > 0;
   uint8_t* base = scratch + (int64_t)f * l.stride;
   const Planes src(base + l.src, l), rec(base + l.rec, l);
   uint8_t* tot = base + l.tot;
   const int qpc = c_chroma_qp[qp];
+  const bool is_p = frame_meta(scratch, l, f)[1] != 0;
 
   for (int i = t; i < 384; i += 128) {
     if (i < 256) s.src[i] = src.y[(16 * my + i / 16) * src.ys + 16 * mx + i % 16];
@@ -395,8 +588,12 @@ __global__ void __launch_bounds__(128) h264_mb_kernel(int d, int qp, uint8_t* sc
     s.tl[p] = has_t && has_l ? pl[(n * my - 1) * st + n * mx - 1] : 0;
   }
   if (t < 8) s.cost[t] = 0;
-  if (t == 0) { s.maxlev = 0; s.bits = 0; }
+  if (t == 0) { s.maxlev = 0; s.bits = 0; s.inter = 0; }
   __syncthreads();
+  if (is_p) {   // the reference: the previous frame of the batch, or the stream state's picture
+    const Planes ref(f > 0 ? scratch + (int64_t)(f - 1) * l.stride + l.rec : const_cast<uint8_t*>(state) + 256, l);
+    motion_search(s, ref, l, mx, my, qp);
+  }
 
   // prediction parameters: DC values and the plane mode's a, b, c (8.3.3.3-4, 8.3.4.1-4)
   if (t == 0) {
@@ -447,17 +644,7 @@ __global__ void __launch_bounds__(128) h264_mb_kernel(int d, int qp, uint8_t* sc
       const int x = 4 * bx + (i & 3), y = 4 * by + (i >> 2);
       r[i] = s.src[so + y * n + x] - predict(s, plane, mode, x, y);
     }
-    for (int i = 0; i < 4; i++) {   // rows
-      int* q = r + 4 * i;
-      const int a0 = q[0] + q[1], a1 = q[0] - q[1], a2 = q[2] + q[3], a3 = q[2] - q[3];
-      q[0] = a0 + a2; q[1] = a1 + a3; q[2] = a0 - a2; q[3] = a1 - a3;
-    }
-    int sum = 0;
-    for (int j = 0; j < 4; j++) {   // columns
-      const int a0 = r[j] + r[4 + j], a1 = r[j] - r[4 + j], a2 = r[8 + j] + r[12 + j], a3 = r[8 + j] - r[12 + j];
-      sum += abs(a0 + a2) + abs(a1 + a3) + abs(a0 - a2) + abs(a1 - a3);
-    }
-    atomicAdd(&s.cost[plane == 0 ? mode : 4 + mode], sum);
+    atomicAdd(&s.cost[plane == 0 ? mode : 4 + mode], satd4(r));
   }
   __syncthreads();
   if (t == 0) {
@@ -470,15 +657,19 @@ __global__ void __launch_bounds__(128) h264_mb_kernel(int d, int qp, uint8_t* sc
     }
     s.lmode = lm;
     s.cmode = cm;
+    s.inter = is_p && !(s.cost[lm] + INTRA_BIAS * lambda_of(qp) < s.icost);
   }
   __syncthreads();
+  const bool inter = s.inter;
   for (int i = t; i < 384; i += 128) {
-    if (i < 256) s.pred[i] = predict(s, 0, s.lmode, i & 15, i >> 4);
+    if (inter) s.pred[i] = s.ipred[i];
+    else if (i < 256) s.pred[i] = predict(s, 0, s.lmode, i & 15, i >> 4);
     else { const int p = 1 + (i - 256) / 64, j = (i - 256) % 64; s.pred[i] = predict(s, p, s.cmode, j & 7, j >> 3); }
   }
   __syncthreads();
 
-  // forward transform and AC quantisation: one thread per 4x4 block (16 luma raster, 4 Cb, 4 Cr)
+  // forward transform and quantisation: one thread per 4x4 block (16 luma raster, 4 Cb, 4 Cr); the dead zone is
+  // f = 2^qbits / 3 for intra, 2^qbits / 6 for inter; an inter luma block keeps its DC coefficient
   if (t < 24) {
     const bool luma = t < 16;
     const int bx = luma ? (t & 3) : (t & 1), by = luma ? (t >> 2) : ((t >> 1) & 1);
@@ -494,7 +685,8 @@ __global__ void __launch_bounds__(128) h264_mb_kernel(int d, int qp, uint8_t* sc
         const int a = x[j], b = x[4 + j], c = x[8 + j], e = x[12 + j];
         m[i * 4 + j] = i == 0 ? a + b + c + e : i == 1 ? 2 * a + b - c - 2 * e : i == 2 ? a - b - c + e : a - 2 * b + 2 * c - e;
       }
-    const int qbits = 15 + q / 6, fq = (1 << qbits) / 3;
+    const int qbits = 15 + q / 6, fq = (1 << qbits) / (inter ? 6 : 3);
+    const int k0 = inter && luma ? 0 : 1;
     int nz = 0, mx_ = 0;
     for (int i = 0; i < 4; i++) {    // w = m CF^T (rows)
       const int a = m[4 * i], b = m[4 * i + 1], c = m[4 * i + 2], e = m[4 * i + 3];
@@ -502,7 +694,7 @@ __global__ void __launch_bounds__(128) h264_mb_kernel(int d, int qp, uint8_t* sc
       for (int j = 0; j < 4; j++) {
         const int k = 4 * i + j;
         s.w[t][k] = w4[j];
-        const int lv = k == 0 ? 0 : quant(w4[j], c_mf[q % 6][pos_class(k)], qbits, fq);
+        const int lv = k < k0 ? 0 : quant(w4[j], c_mf[q % 6][pos_class(k)], qbits, fq);
         s.lev[t][k] = lv;
         nz += lv != 0;
         mx_ = max(mx_, abs(lv));
@@ -514,7 +706,7 @@ __global__ void __launch_bounds__(128) h264_mb_kernel(int d, int qp, uint8_t* sc
   __syncthreads();
 
   // DC transforms, quantisation and their dequantisation (8.5.10, 8.5.11)
-  if (t == 0) {
+  if (t == 0 && !inter) {
     int a[16], b[16];
     for (int i = 0; i < 16; i++) a[i] = s.w[i][0];   // [by * 4 + bx]
     // b = HD a HD, >> 1
@@ -550,7 +742,7 @@ __global__ void __launch_bounds__(128) h264_mb_kernel(int d, int qp, uint8_t* sc
     const int p = t / 64, o = 16 + 4 * p;
     const int a0 = s.w[o][0], a1 = s.w[o + 1][0], a2 = s.w[o + 2][0], a3 = s.w[o + 3][0];
     const int c4[4] = {a0 + a1 + a2 + a3, a0 - a1 + a2 - a3, a0 + a1 - a2 - a3, a0 - a1 - a2 + a3};
-    const int qbits = 15 + qpc / 6, fq = (1 << qbits) / 3;
+    const int qbits = 15 + qpc / 6, fq = (1 << qbits) / (inter ? 6 : 3);
     int mx_ = 0;
     for (int i = 0; i < 4; i++) {
       s.cdc[p][i] = quant(c4[i], c_mf[qpc % 6][0], qbits + 1, 2 * fq);
@@ -569,21 +761,24 @@ __global__ void __launch_bounds__(128) h264_mb_kernel(int d, int qp, uint8_t* sc
     const bool luma = t < 16;
     const int q = luma ? qp : qpc;
     int dq[16];
-    for (int k = 1; k < 16; k++) {
+    for (int k = 0; k < 16; k++) {
       const int ls = 16 * c_v[q % 6][pos_class(k)], c = s.lev[t][k];
       dq[k] = q >= 24 ? (c * ls) << (q / 6 - 4) : (c * ls + (1 << (3 - q / 6))) >> (4 - q / 6);
     }
-    dq[0] = luma ? s.dcr[t] : s.cdcr[(t - 16) / 4][(t - 16) & 3];
+    if (!(inter && luma)) dq[0] = luma ? s.dcr[t] : s.cdcr[(t - 16) / 4][(t - 16) & 3];
     idct4(dq);
     for (int k = 0; k < 16; k++) s.w[t][k] = dq[k];   // the residual
   }
   __syncthreads();
   if (t == 0) {
-    int al = 0, ac = 0, dcc = 0;
-    for (int i = 0; i < 16; i++) al += s.tot[i];
+    int al = 0, ac = 0, dcc = 0, m8 = 0;
+    for (int i = 0; i < 16; i++) {
+      al += s.tot[i];
+      if (s.tot[i]) m8 |= 1 << (((i >> 3) << 1) | ((i & 3) >> 1));   // the block's 8x8 quadrant
+    }
     for (int i = 16; i < 24; i++) ac += s.tot[i];
     for (int i = 0; i < 8; i++) dcc |= s.cdc[i / 4][i % 4];
-    s.cbpl = al ? 15 : 0;
+    s.cbpl = inter ? m8 : al ? 15 : 0;
     s.cbpc = ac ? 2 : dcc ? 1 : 0;
   }
   __syncthreads();
@@ -591,18 +786,24 @@ __global__ void __launch_bounds__(128) h264_mb_kernel(int d, int qp, uint8_t* sc
   if (t < 24) tot[(int64_t)mb * 24 + t] = (uint8_t)s.tot[t];
   __syncthreads();
 
-  // CAVLC bit count, one thread per residual block: 0 luma DC, 1..16 luma AC (luma4x4BlkIdx order), 17/18 Cb/Cr
-  // DC, 19..22 Cb AC, 23..26 Cr AC; the levels in scan order go to the writer
+  // CAVLC bit count, one thread per residual block: 0 luma DC, 1..16 luma AC (luma4x4BlkIdx order; an inter block's
+  // 16 coefficients), 17/18 Cb/Cr DC, 19..26 Cb AC, 23..26 Cr AC; the levels in scan order go to the writer
+  const int info = s.lmode | s.cmode << 2 | s.cbpc << 4 | (!inter && s.cbpl ? 1 : 0) << 6 | inter << 8 |
+                   (inter ? s.cbpl : 0) << 9;
   if (t < BLOCKS) {
     int c[16], plane, x, y, maxn;
     block_geom(t, mx, my, plane, x, y, maxn);
     if (t == 0) for (int k = 0; k < 16; k++) c[k] = s.dc[c_zigzag[k]];
-    else if (t <= 16) { const int b = c_blk_y[t - 1] * 4 + c_blk_x[t - 1]; for (int k = 0; k < 15; k++) c[k] = s.lev[b][c_zigzag[k + 1]]; }
+    else if (t <= 16) {
+      const int b = c_blk_y[t - 1] * 4 + c_blk_x[t - 1];
+      if (inter) maxn = 16;
+      for (int k = 0; k < maxn; k++) c[k] = s.lev[b][c_zigzag[k + 16 - maxn]];
+    }
     else if (t <= 18) for (int k = 0; k < 4; k++) c[k] = s.cdc[t - 17][k];
     else { const int b = 16 + (t - 19); for (int k = 0; k < 15; k++) c[k] = s.lev[b][c_zigzag[k + 1]]; }
     int16_t* out = reinterpret_cast<int16_t*>(base + l.lev) + ((int64_t)mb * BLOCKS + t) * 16;
     for (int k = 0; k < maxn; k++) out[k] = (int16_t)max(-32768, min(32767, c[k]));
-    if (s.maxlev <= MAX_LEVEL && block_present(t, s.cbpl, s.cbpc)) {
+    if (s.maxlev <= MAX_LEVEL && block_present(t, info)) {
       BitSink sink{nullptr, 0, 0};
       const int nc = plane < 0 ? -1 : nc_of(tot, l, plane, x, y);
       atomicAdd(&s.bits, cavlc_block(c, maxn, nc, sink));
@@ -610,10 +811,11 @@ __global__ void __launch_bounds__(128) h264_mb_kernel(int d, int qp, uint8_t* sc
   }
   __syncthreads();
   if (t == 0) {
-    const int bits = s.bits + mb_header_bits(s.lmode, s.cmode, s.cbpl, s.cbpc);
+    const int bits = s.bits + mb_header_bits(info, is_p);
     s.pcm = s.maxlev > MAX_LEVEL || bits > PCM_BITS;
-    reinterpret_cast<int*>(base + l.info)[mb] = s.lmode | s.cmode << 2 | s.cbpc << 4 | (s.cbpl ? 1 : 0) << 6 | s.pcm << 7;
+    reinterpret_cast<int*>(base + l.info)[mb] = s.pcm ? (1 << 7) : info;
     reinterpret_cast<int*>(base + l.bits)[mb] = s.pcm ? 0 : bits;
+    reinterpret_cast<int*>(base + l.mv)[mb] = inter && !s.pcm ? (s.mvx & 0xffff) | (int)((unsigned)s.mvy << 16) : 0;
   }
   __syncthreads();
   if (s.pcm && t < 24) tot[(int64_t)mb * 24 + t] = 16;
@@ -631,6 +833,77 @@ __global__ void __launch_bounds__(128) h264_mb_kernel(int d, int qp, uint8_t* sc
       rec.chroma(p)[(8 * my + (j >> 3)) * rec.cs + 8 * mx + (j & 7)] = (uint8_t)v;
     }
   }
+}
+
+// ---- P slices: vector prediction and skip runs, after every decision is made -------------------------------------
+struct Neighbour {
+  bool avail;
+  int ref, x, y;   // ref 0 for an inter macroblock, -1 for an intra one or none
+};
+
+__device__ Neighbour neighbour(const int* info, const int* mv, const Layout& l, int x, int y) {
+  if (x < 0 || y < 0 || x >= l.wm) return {false, -1, 0, 0};
+  const int mb = y * l.wm + x;
+  if (!((info[mb] >> 8) & 1)) return {true, -1, 0, 0};
+  const int v = mv[mb];
+  return {true, 0, (int)(int16_t)(v & 0xffff), v >> 16};
+}
+
+__device__ __forceinline__ int median3(int a, int b, int c) { return max(min(a, b), min(max(a, b), c)); }
+
+// 8.4.1.3 (mvp of a 16x16 partition with refIdx 0) and 8.4.1.1 (P_Skip); one thread per macroblock.  A P_L0_16x16
+// macroblock with no coded coefficient whose vector equals its mvpSkip becomes P_Skip; the others get their mvd bits.
+__global__ void __launch_bounds__(128) h264_mvp_kernel(uint8_t* scratch, Layout l) {
+  const int f = blockIdx.y, mb = blockIdx.x * blockDim.x + threadIdx.x;
+  if (mb >= l.nmb || !frame_meta(scratch, l, f)[1]) return;
+  uint8_t* base = scratch + (int64_t)f * l.stride;
+  int* info = reinterpret_cast<int*>(base + l.info);
+  const int* mv = reinterpret_cast<const int*>(base + l.mv);
+  const int me = info[mb];
+  if (!((me >> 8) & 1)) return;
+  const int x = mb % l.wm, y = mb / l.wm;
+  const Neighbour A = neighbour(info, mv, l, x - 1, y);
+  Neighbour B = neighbour(info, mv, l, x, y - 1);
+  Neighbour C = neighbour(info, mv, l, x + 1, y - 1);
+  if (!C.avail) C = neighbour(info, mv, l, x - 1, y - 1);
+  const bool skip0 = !A.avail || !B.avail || (A.ref == 0 && A.x == 0 && A.y == 0) || (B.ref == 0 && B.x == 0 && B.y == 0);
+  if (!B.avail && !C.avail && A.avail) B = C = A;
+  int px, py;
+  const int n = (A.ref == 0) + (B.ref == 0) + (C.ref == 0);
+  if (n == 1) {
+    const Neighbour& o = A.ref == 0 ? A : B.ref == 0 ? B : C;
+    px = o.x; py = o.y;
+  } else {
+    px = median3(A.x, B.x, C.x);
+    py = median3(A.y, B.y, C.y);
+  }
+  const int vx = (int)(int16_t)(mv[mb] & 0xffff), vy = mv[mb] >> 16;
+  const int sx = skip0 ? 0 : px, sy = skip0 ? 0 : py;
+  int* bits = reinterpret_cast<int*>(base + l.bits);
+  if (inter_cbp(me) == 0 && vx == sx && vy == sy) {
+    info[mb] = me | 1 << 13;
+    bits[mb] = 0;
+    return;
+  }
+  const int dx = vx - px, dy = vy - py;
+  reinterpret_cast<int*>(base + l.mvd)[mb] = (dx & 0xffff) | (int)((unsigned)dy << 16);
+  bits[mb] += se_bits(dx) + se_bits(dy);
+}
+
+// Each coded macroblock's mb_skip_run (the P_Skip macroblocks just before it) and the slice's trailing run, which the
+// last macroblock carries when it is skipped; one thread per macroblock.
+__global__ void __launch_bounds__(128) h264_run_kernel(uint8_t* scratch, Layout l) {
+  const int f = blockIdx.y, mb = blockIdx.x * blockDim.x + threadIdx.x;
+  if (mb >= l.nmb || !frame_meta(scratch, l, f)[1]) return;
+  uint8_t* base = scratch + (int64_t)f * l.stride;
+  const int* info = reinterpret_cast<const int*>(base + l.info);
+  const bool skipped = (info[mb] >> 13) & 1;
+  if (skipped && mb != l.nmb - 1) return;
+  int r = 0;
+  while (r < mb && ((info[mb - 1 - r] >> 13) & 1)) r++;
+  if (skipped) r++;
+  reinterpret_cast<int*>(base + l.run)[mb] = r;
+  if (!((info[mb] >> 7) & 1)) reinterpret_cast<int*>(base + l.bits)[mb] += ue_bits(r);
 }
 
 // ---- bit offsets -------------------------------------------------------------------------------------------------
@@ -654,10 +927,18 @@ __global__ void __launch_bounds__(1024) h264_scan_kernel(uint8_t* scratch, Layou
   uint8_t* base = scratch + (int64_t)f * l.stride;
   const int* info = reinterpret_cast<const int*>(base + l.info);
   const int* bits = reinterpret_cast<const int*>(base + l.bits);
+  const int* run = reinterpret_cast<const int*>(base + l.run);
   int* off = reinterpret_cast<int*>(base + l.off);
+  const int* meta = frame_meta(scratch, l, f);
+  const bool is_p = meta[1] != 0;
+  const int header = is_p ? P_HEADER_BITS : HEADER_BITS;
+  // an I_PCM macroblock: its skip run, ue(mb_type), then its samples byte-aligned
+  auto map = [&](int i) {
+    return (info[i] >> 7) & 1 ? Map{(is_p ? ue_bits(run[i]) : 0) + 9, PCM_BITS - 9, 1} : Map{bits[i], 0, 0};
+  };
   const int per = (l.nmb + 1023) / 1024, lo = min(t * per, l.nmb), hi = min(lo + per, l.nmb);
   Map m{0, 0, 0};
-  for (int i = lo; i < hi; i++) m = compose(m, (info[i] >> 7) & 1 ? Map{9, PCM_BITS - 9, 1} : Map{bits[i], 0, 0});
+  for (int i = lo; i < hi; i++) m = compose(m, map(i));
   part[t] = m;
   __syncthreads();
   for (int s = 1; s < 1024; s <<= 1) {   // inclusive Hillis-Steele scan
@@ -666,12 +947,12 @@ __global__ void __launch_bounds__(1024) h264_scan_kernel(uint8_t* scratch, Layou
     if (t >= s) part[t] = compose(prev, part[t]);
     __syncthreads();
   }
-  int x = t == 0 ? HEADER_BITS : apply(part[t - 1], HEADER_BITS);
+  int x = t == 0 ? header : apply(part[t - 1], header);
   for (int i = lo; i < hi; i++) {
     off[i] = x;
-    x = (info[i] >> 7) & 1 ? ((x + 9 + 7) & ~7) + PCM_BITS - 9 : x + bits[i];
+    x = apply(map(i), x);
   }
-  if (t == 1023) s_total = apply(part[1023], HEADER_BITS);
+  if (t == 1023) s_total = apply(part[1023], header);
   __syncthreads();
   const int total = s_total;                       // bits before the stop bit
   const int nbytes = (total + 1 + 7) / 8;
@@ -681,7 +962,10 @@ __global__ void __launch_bounds__(1024) h264_scan_kernel(uint8_t* scratch, Layou
   if (t == 0) {
     // first_mb_in_slice 0, slice_type 7, pps 0, frame_num 0000, idr_pic_id 1, two flags, slice_qp_delta 0,
     // disable_deblocking_filter_idc 1
-    put_bits(raw, 0, 0x22208Au, HEADER_BITS);    // 1 0001000 1 0000 010 0 0 1 010
+    if (is_p)   // first_mb_in_slice 0, slice_type 5, pps 0, frame_num, three flags 0, slice_qp_delta 0, idc 1
+      put_bits(raw, 0, 0x4Du << 11 | (uint32_t)meta[2] << 7 | 0x0Au, P_HEADER_BITS);   // 1 00110 1 ffff 0 0 0 1 010
+    else
+      put_bits(raw, 0, 0x22208Au, HEADER_BITS);  // 1 0001000 1 0000 010 0 0 1 010
     put_bits(raw, total, 1, 1);                  // rbsp_stop_one_bit
     reinterpret_cast<int*>(base + l.meta)[0] = nbytes;
   }
@@ -695,10 +979,19 @@ __global__ void __launch_bounds__(128) h264_write_kernel(uint8_t* scratch, Layou
   uint8_t* base = scratch + (int64_t)f * l.stride;
   uint32_t* raw = reinterpret_cast<uint32_t*>(base + l.raw);
   const int info = reinterpret_cast<const int*>(base + l.info)[mb];
-  const uint32_t pos = (uint32_t)reinterpret_cast<const int*>(base + l.off)[mb];
+  const bool is_p = frame_meta(scratch, l, f)[1] != 0;
+  uint32_t pos = (uint32_t)reinterpret_cast<const int*>(base + l.off)[mb];
   const int mx = mb % l.wm, my = mb / l.wm;
-  if ((info >> 7) & 1) {   // I_PCM: ue(25), alignment, 256 Y + 64 Cb + 64 Cr samples
-    if (lane == 0) put_bits(raw, pos, 26, 9);
+  if (is_p) {   // mb_skip_run before a coded macroblock; the trailing run on a skipped last one
+    const int skipped = (info >> 13) & 1;
+    if (skipped && mb != l.nmb - 1) return;
+    const int r = reinterpret_cast<const int*>(base + l.run)[mb];
+    if (lane == 0) put_bits(raw, pos, r + 1, ue_bits(r));
+    if (skipped) return;
+    pos += ue_bits(r);
+  }
+  if ((info >> 7) & 1) {   // I_PCM: ue(25) (ue(30) in a P slice), alignment, 256 Y + 64 Cb + 64 Cr samples
+    if (lane == 0) put_bits(raw, pos, is_p ? 31 : 26, 9);
     const uint32_t p0 = (pos + 9 + 7) & ~7u;
     const Planes rec(base + l.rec, l);
     for (int i = lane; i < 384; i += 32) {
@@ -712,12 +1005,13 @@ __global__ void __launch_bounds__(128) h264_write_kernel(uint8_t* scratch, Layou
     }
     return;
   }
-  const int lmode = info & 3, cmode = (info >> 2) & 3, cbpc = (info >> 4) & 3, cbpl = (info >> 6) & 1;
+  const bool inter = (info >> 8) & 1;
   const uint8_t* tot = base + l.tot;
   int c[16], plane = 0, x = 0, y = 0, maxn = 0, nc = 0, n = 0;
-  const bool present = lane < BLOCKS && block_present(lane, cbpl, cbpc);
+  const bool present = lane < BLOCKS && block_present(lane, info);
   if (present) {
     block_geom(lane, mx, my, plane, x, y, maxn);
+    if (inter && lane >= 1 && lane <= 16) maxn = 16;
     const int16_t* lev = reinterpret_cast<const int16_t*>(base + l.lev) + ((int64_t)mb * BLOCKS + lane) * 16;
     for (int k = 0; k < 16; k++) c[k] = k < maxn ? lev[k] : 0;
     nc = plane < 0 ? -1 : nc_of(tot, l, plane, x, y);
@@ -729,9 +1023,22 @@ __global__ void __launch_bounds__(128) h264_write_kernel(uint8_t* scratch, Layou
     const int v = __shfl_up_sync(0xffffffffu, incl, s);
     if (lane >= s) incl += v;
   }
-  const int mbt = 1 + lmode + 4 * cbpc + (cbpl ? 12 : 0);
-  const int hb = mb_header_bits(lmode, cmode, cbpl, cbpc);
-  if (lane == 0) {
+  int hb = mb_header_bits(info, is_p);
+  if (inter) {
+    const int v = reinterpret_cast<const int*>(base + l.mvd)[mb];
+    const int dx = (int16_t)(v & 0xffff), dy = v >> 16;
+    const int cbp = inter_cbp(info), code = c_inter_cbp[cbp];
+    hb += se_bits(dx) + se_bits(dy);
+    if (lane == 0) {
+      BitSink h{raw, pos, 0};
+      h.u(1, 1);                                 // mb_type P_L0_16x16
+      h.u(dx > 0 ? 2 * dx : -2 * dx + 1, se_bits(dx));
+      h.u(dy > 0 ? 2 * dy : -2 * dy + 1, se_bits(dy));
+      h.u(code + 1, ue_bits(code));
+      if (cbp) h.u(1, 1);                        // mb_qp_delta 0
+    }
+  } else if (lane == 0) {
+    const int mbt = i16_mb_type(info, is_p), cmode = (info >> 2) & 3;
     BitSink h{raw, pos, 0};
     h.u(mbt + 1, ue_bits(mbt));
     h.u(cmode + 1, ue_bits(cmode));
@@ -790,7 +1097,7 @@ __global__ void __launch_bounds__(32) h264_ep_plan_kernel(uint8_t* scratch, Layo
     const int64_t body = 1 + (int64_t)nbytes + added;
     uint8_t* o = out + (int64_t)f * out_stride;
     o[0] = (uint8_t)(body >> 24); o[1] = (uint8_t)(body >> 16); o[2] = (uint8_t)(body >> 8); o[3] = (uint8_t)body;
-    o[4] = 0x65;                                 // nal_ref_idc 3, nal_unit_type 5 (IDR slice)
+    o[4] = frame_meta(scratch, l, f)[1] ? 0x61 : 0x65;   // nal_ref_idc 3, nal_unit_type 1 (P) or 5 (IDR slice)
     out_len[f] = 4 + body;
   }
 }
@@ -813,6 +1120,31 @@ __global__ void __launch_bounds__(128) h264_ep_emit_kernel(uint8_t* scratch, Lay
     *o++ = (uint8_t)b;
     z = b == 0 ? min(z + 1, 2) : 0;
   }
+}
+
+// ---- stream state -------------------------------------------------------------------------------------------------
+// State: the stream position (int64) at byte 0, the previous picture's padded reconstruction (the Planes layout) from
+// byte 256.  Frame f of a batch is stream position pos + f: an IDR picture when that is a multiple of gop, else a P
+// picture with frame_num (position - last IDR) mod 16.
+__global__ void __launch_bounds__(256) h264_frame_kernel(uint8_t* scratch, Layout l, const uint8_t* state, int gop,
+                                                         int frames) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= frames) return;
+  const int64_t n = (state ? *reinterpret_cast<const int64_t*>(state) : 0) + f;
+  int* meta = reinterpret_cast<int*>(scratch + (int64_t)f * l.stride + l.meta);
+  meta[1] = gop > 1 && n % gop != 0;
+  meta[2] = (int)((n % gop) % 16);
+}
+
+// The last frame's reconstruction becomes the state's picture, and the position advances by the batch.
+__global__ void __launch_bounds__(256) h264_state_kernel(const uint8_t* scratch, Layout l, uint8_t* state,
+                                                         int frames) {
+  const uint4* src = reinterpret_cast<const uint4*>(scratch + (int64_t)(frames - 1) * l.stride + l.rec);
+  uint4* dst = reinterpret_cast<uint4*>(state + 256);
+  const int64_t n = (int64_t)l.nmb * 384 / 16;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    dst[i] = src[i];
+  if (blockIdx.x == 0 && threadIdx.x == 0) *reinterpret_cast<int64_t*>(state) += frames;
 }
 
 // ---- host: level, parameter sets ---------------------------------------------------------------------------------
@@ -873,13 +1205,25 @@ int64_t h264_bound(int W, int H) {
   return 5 + n + (n + 1) / 2;
 }
 
+int64_t h264_p_bound(int W, int H) {
+  if (h264_bound(W, H) < 0) return -1;
+  const int64_t n = raw_bytes_bound_p(((W + 15) / 16) * ((H + 15) / 16));
+  return 5 + n + (n + 1) / 2;
+}
+
+size_t h264_state_bytes(int H, int W) {
+  if (h264_bound(W, H) < 0) return 0;
+  return (size_t)(256 + align256((int64_t)((W + 15) / 16) * ((H + 15) / 16) * 384));
+}
+
 size_t h264_scratch_bytes(int64_t frames, int H, int W) {
   if (frames <= 0 || frames > 65535 || h264_bound(W, H) < 0) return 0;
   return (size_t)(frames * layout(H, W).stride);
 }
 
-int32_t h264_parameter_sets(int W, int H, int qp, int fps_num, int fps_den, uint8_t* out, int64_t cap) {
+int32_t h264_parameter_sets(int W, int H, int qp, int fps_num, int fps_den, int gop, uint8_t* out, int64_t cap) {
   if (h264_bound(W, H) < 0 || qp < 0 || qp > 51 || fps_num <= 0 || fps_den <= 0 || fps_num > (INT32_MAX / 2)) return -1;
+  if (gop < 1 || gop > 65535) return -1;
   const int wc = (W + 15) / 16 * 16, hc = (H + 15) / 16 * 16;
   HostBits s;
   s.u(66, 8);                    // profile_idc: Baseline
@@ -888,7 +1232,7 @@ int32_t h264_parameter_sets(int W, int H, int qp, int fps_num, int fps_den, uint
   s.ue(0);                       // seq_parameter_set_id
   s.ue(0);                       // log2_max_frame_num_minus4
   s.ue(2);                       // pic_order_cnt_type
-  s.ue(0);                       // max_num_ref_frames
+  s.ue(gop > 1 ? 1 : 0);         // max_num_ref_frames: a P picture refers to the previous picture
   s.u(0, 1);                     // gaps_in_frame_num_value_allowed_flag
   s.ue(wc / 16 - 1);
   s.ue(hc / 16 - 1);
@@ -950,16 +1294,32 @@ int32_t h264_parameter_sets(int W, int H, int qp, int fps_num, int fps_den, uint
   return (int32_t)need;
 }
 
-void launch_h264_encode(int frames, int H, int W, int qp, const uint8_t* rgb, void* scratch, uint8_t* out,
-                        int64_t out_stride, int64_t* out_len, cudaStream_t stream) {
+void launch_h264_encode(int frames, int H, int W, int qp, int gop, const uint8_t* rgb, uint8_t* state, void* scratch,
+                        uint8_t* out, int64_t out_stride, int64_t* out_len, cudaStream_t stream) {
   const Layout l = layout(H, W);
   uint8_t* s = static_cast<uint8_t*>(scratch);
   const unsigned F = (unsigned)frames;
   h264_convert_kernel<<<dim3((unsigned)((64 * l.nmb + 255) / 256), F), 256, 0, stream>>>(rgb, s, l);
   count_launch();
-  for (int d = 0; d < l.wm + l.hm - 1; d++) {
-    const int n = std::min(d, l.wm - 1) - std::max(0, d - l.hm + 1) + 1;
-    h264_mb_kernel<<<dim3((unsigned)n, F), 128, 0, stream>>>(d, qp, s, l);
+  h264_frame_kernel<<<(F + 255) / 256, 256, 0, stream>>>(s, l, state, gop, frames);
+  count_launch();
+  // The wavefront over (frame, anti-diagonal): step k runs diagonal k - lag f of every frame f that has one.
+  const int D = l.wm + l.hm - 1, lag = gop > 1 ? LAG : 0;
+  auto diag_len = [&](int d) { return std::min(d, l.wm - 1) - std::max(0, d - l.hm + 1) + 1; };
+  for (int k = 0; k < D + (frames - 1) * lag; k++) {
+    const int f_lo = lag ? std::max(0, (k - (D - 1) + lag - 1) / lag) : 0;
+    const int f_hi = lag ? std::min(frames - 1, k / lag) : frames - 1;
+    int n = 0;   // 0 when lag > D leaves a step between two frames' wavefronts
+    for (int f = f_lo; f <= f_hi && n < std::min(l.wm, l.hm); f++) n = std::max(n, diag_len(k - lag * f));
+    if (n == 0) continue;
+    h264_mb_kernel<<<dim3((unsigned)n, (unsigned)(f_hi - f_lo + 1)), 128, 0, stream>>>(k, lag, f_lo, qp, s, state, l);
+    count_launch();
+  }
+  const unsigned mbb = (unsigned)((l.nmb + 127) / 128);
+  if (gop > 1) {
+    h264_mvp_kernel<<<dim3(mbb, F), 128, 0, stream>>>(s, l);
+    count_launch();
+    h264_run_kernel<<<dim3(mbb, F), 128, 0, stream>>>(s, l);
     count_launch();
   }
   h264_scan_kernel<<<F, 1024, 0, stream>>>(s, l);
@@ -973,6 +1333,10 @@ void launch_h264_encode(int frames, int H, int W, int qp, const uint8_t* rgb, vo
   count_launch();
   h264_ep_emit_kernel<<<dim3(pb, F), 128, 0, stream>>>(s, l, out, out_stride);
   count_launch();
+  if (state) {
+    h264_state_kernel<<<std::min(1024u, (unsigned)((l.nmb * 24 + 255) / 256)), 256, 0, stream>>>(s, l, state, frames);
+    count_launch();
+  }
 }
 
 }  // namespace gab

@@ -1,16 +1,18 @@
 """MP4 videos written from device frames: what render.py's `ffmpeg -framerate 25 -i '<dir>/*.png' -pix_fmt yuv420p
 renders.mp4` makes of the PNG files it wrote, without the PNG files.
 
-    with VideoWriter(path, W, H, fps=25, qp=20) as vw:    # render.py's renders.mp4 / gt.mp4 / renders_mesh.mp4
+    with VideoWriter(path, W, H, fps=25, qp=20, gop=25) as vw:   # render.py's renders.mp4 / gt.mp4 / renders_mesh.mp4
         for t in timesteps:
             player.run(...)
             vw.add(player.display)                        # CUDA (H,W,3) or (K,H,W,3) uint8
-    data = encode_video(frames, fps=25, qp=20)            # a whole MP4 in memory
+    data = encode_video(frames, fps=25, qp=20, gop=1)     # a whole MP4 in memory
 
-The frames are encoded on the device (csrc/h264.cu, include/gab200_rasterizer.h gab200_h264_encode): H.264
-Constrained Baseline, every frame an IDR picture, one fixed QP, BT.601 limited-range 4:2:0.  Only the compressed
-samples cross to the host, through a ring of pinned slots; the file is ftyp | mdat | moov, muxed here.  The bytes are
-deterministic and differ from libx264's.
+The frames are encoded on the device (csrc/h264.cu, include/gab200_rasterizer.h gab200_h264_encode and
+gab200_h264_encode_stream): H.264 Constrained Baseline, one fixed QP, BT.601 limited-range 4:2:0.  With gop=1 (the
+default) every frame is an IDR picture; with gop=N every N-th frame is, and the others are P pictures that refer to
+the frame before them, which is far smaller when successive frames look alike (a fixed camera).  Only the compressed
+samples cross to the host, through a ring of pinned slots; the file is ftyp | mdat | moov, muxed here, with an stss
+box listing the IDR frames when gop > 1.  The bytes are deterministic and differ from libx264's.
 """
 from __future__ import annotations
 
@@ -38,9 +40,19 @@ def video_bound(width: int, height: int) -> int:
     return b
 
 
-def slot_stride(width: int, height: int) -> int:
-    """Bytes per sample in an output buffer: the bound rounded up to 16 (gab200_png_copy moves 16-byte words)."""
-    return (video_bound(width, height) + 15) // 16 * 16
+def slot_stride(width: int, height: int, gop: int = 1) -> int:
+    """Bytes per sample in an output buffer: the bound (of a P sample when gop > 1) rounded up to 16 (gab200_png_copy
+    moves 16-byte words)."""
+    b = video_bound(width, height)
+    if gop > 1:
+        b = int(N.lib().gab200_h264_p_bound(int(width), int(height)))
+    return (b + 15) // 16 * 16
+
+
+def _check_gop(gop) -> int:
+    if isinstance(gop, bool) or not isinstance(gop, int) or not 1 <= gop <= 65535:
+        raise ValueError(f"gop must be an int in 1..65535, got {gop!r}")
+    return gop
 
 
 def _check_qp(qp) -> int:
@@ -78,10 +90,11 @@ def check_frames(frames, name: str = "frames") -> tuple:
     return K, H, W
 
 
-def parameter_sets(width: int, height: int, qp: int, fps: Fraction) -> tuple:
-    """(SPS, PPS) NAL units of the stream (gab200_h264_parameter_sets)."""
+def parameter_sets(width: int, height: int, qp: int, fps: Fraction, gop: int = 1) -> tuple:
+    """(SPS, PPS) NAL units of the stream (gab200_h264_stream_parameter_sets)."""
     buf = (C.c_uint8 * 256)()
-    n = int(N.lib().gab200_h264_parameter_sets(width, height, qp, fps.numerator, fps.denominator, buf, len(buf)))
+    n = int(N.lib().gab200_h264_stream_parameter_sets(width, height, qp, fps.numerator, fps.denominator, gop, buf,
+                                                      len(buf)))
     if n < 0:
         raise ValueError(f"no parameter sets for {width}x{height} at qp {qp}, {fps} frames/s")
     data = bytes(buf[:n])
@@ -98,6 +111,25 @@ def launch_encode(frames: torch.Tensor, qp: int, scratch_buf: torch.Tensor, out:
     stream = C.c_void_p(torch.cuda.current_stream(frames.device).cuda_stream)
     N.check(N.lib().gab200_h264_encode(K, H, W, qp, frames.data_ptr(), scratch_buf.data_ptr(), out.data_ptr(),
                                        out.stride(0), out_len.data_ptr(), stream), "gab200_h264_encode")
+
+
+def launch_encode_stream(frames: torch.Tensor, qp: int, gop: int, state: torch.Tensor, scratch_buf: torch.Tensor,
+                         out: torch.Tensor, out_len: torch.Tensor):
+    """Enqueues gab200_h264_encode_stream on the current stream: frames (K,H,W,3) are the next K frames of the stream
+    whose state (state_buffer) the encode reads and advances on the device.  Reads nothing on the host: capturable."""
+    K, H, W = check_frames(frames)
+    stream = C.c_void_p(torch.cuda.current_stream(frames.device).cuda_stream)
+    N.check(N.lib().gab200_h264_encode_stream(K, H, W, qp, gop, frames.data_ptr(), state.data_ptr(),
+                                              scratch_buf.data_ptr(), out.data_ptr(), out.stride(0),
+                                              out_len.data_ptr(), stream), "gab200_h264_encode_stream")
+
+
+def state_buffer(H: int, W: int, device) -> torch.Tensor:
+    """A zeroed stream state: its next frame is an IDR picture."""
+    n = int(N.lib().gab200_h264_state_bytes(H, W))
+    if n == 0:
+        raise ValueError(f"no H.264 stream of {W}x{H}")
+    return torch.zeros(n, dtype=torch.uint8, device=device)
 
 
 def scratch(K: int, H: int, W: int, device) -> torch.Tensor:
@@ -122,10 +154,11 @@ FTYP = _box(b"ftyp", b"isom", struct.pack(">I", 512), b"isomiso2avc1mp41")
 MDAT_HEADER = 16          # size 1, 'mdat', 64-bit largesize
 
 
-def moov_box(sizes, first_offset: int, width: int, height: int, sps: bytes, pps: bytes, fps: Fraction) -> bytes:
+def moov_box(sizes, first_offset: int, width: int, height: int, sps: bytes, pps: bytes, fps: Fraction,
+             sync=None) -> bytes:
     """The movie box of one video track whose samples of `sizes` bytes lie back to back from file offset
-    `first_offset`, one chunk per sample (stco, or co64 once an offset passes 2^32); every sample is a sync sample,
-    so there is no stss."""
+    `first_offset`, one chunk per sample (stco, or co64 once an offset passes 2^32).  sync: None when every sample is
+    a sync sample (no stss), else the 1-based numbers of the sync samples, listed in an stss box."""
     n = len(sizes)
     dur = n * fps.denominator
     avcc = _box(b"avcC", bytes([1, sps[1], sps[2], sps[3], 0xFF, 0xE1]), struct.pack(">H", len(sps)), sps, bytes([1]),
@@ -144,7 +177,9 @@ def moov_box(sizes, first_offset: int, width: int, height: int, sps: bytes, pps:
     stts = struct.pack(">III", 1, n, fps.denominator) if n else struct.pack(">I", 0)
     stbl = _box(b"stbl", _full(b"stsd", 0, 0, struct.pack(">I", 1), avc1), _full(b"stts", 0, 0, stts),
                 _full(b"stsc", 0, 0, struct.pack(">IIII", 1, 1, 1, 1)),
-                _full(b"stsz", 0, 0, struct.pack(">II", 0, n), struct.pack(">%dI" % n, *sizes)), co)
+                _full(b"stsz", 0, 0, struct.pack(">II", 0, n), struct.pack(">%dI" % n, *sizes)),
+                b"" if sync is None else _full(b"stss", 0, 0, struct.pack(">I", len(sync)),
+                                               struct.pack(">%dI" % len(sync), *sync)), co)
     minf = _box(b"minf", _full(b"vmhd", 0, 1, bytes(8)),
                 _box(b"dinf", _full(b"dref", 0, 0, struct.pack(">I", 1), _full(b"url ", 0, 1))), stbl)
     mdia = _box(b"mdia", _full(b"mdhd", 0, 0, struct.pack(">IIIIHH", 0, 0, fps.numerator, dur, 0x55C4, 0)),
@@ -162,18 +197,21 @@ class VideoWriter:
     waits on the GPU only when the ring is full; close() encodes the partial last batch and writes the moov box.
 
     path: a file name, or a seekable binary file object (left open).  fps: an int or a fractions.Fraction (the
-    track's timescale is its numerator, each sample lasts its denominator)."""
+    track's timescale is its numerator, each sample lasts its denominator).  gop: every gop-th frame, the first
+    included, is an IDR picture and the others P pictures (1: every frame an IDR picture); the writer owns the
+    stream's state on the device, so a batch may start anywhere in a GOP."""
 
     RING = 3
 
-    def __init__(self, path, width: int, height: int, fps=25, qp: int = 20, batch: int = 16, device=None):
+    def __init__(self, path, width: int, height: int, fps=25, qp: int = 20, batch: int = 16, device=None, gop: int = 1):
         self.fps = _check_fps(fps)
         self.qp = _check_qp(qp)
+        self.gop = _check_gop(gop)
         if isinstance(batch, bool) or not isinstance(batch, int) or not 1 <= batch <= 65535:
             raise ValueError(f"batch must be an int in 1..65535, got {batch!r}")
         self.W, self.H = int(width), int(height)
-        self.stride = slot_stride(self.W, self.H)
-        self.sps, self.pps = parameter_sets(self.W, self.H, self.qp, self.fps)
+        self.stride = slot_stride(self.W, self.H, self.gop)
+        self.sps, self.pps = parameter_sets(self.W, self.H, self.qp, self.fps, self.gop)
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         if self.device.type != "cuda":
             raise ValueError(f"VideoWriter encodes on a CUDA device, got {self.device}")
@@ -183,12 +221,14 @@ class VideoWriter:
             self._scratch = scratch(batch, self.H, self.W, self.device)
             self._out = torch.empty((batch, self.stride), dtype=torch.uint8, device=self.device)
             self._out_len = torch.empty(batch, dtype=torch.int64, device=self.device)
+            self._state = state_buffer(self.H, self.W, self.device) if self.gop > 1 else None
             self._ring = [(torch.empty((batch, self.stride), dtype=torch.uint8, pin_memory=True),
                            torch.empty(batch, dtype=torch.int64, pin_memory=True)) for _ in range(self.RING)]
         self._pending = deque()        # (ring slot, event, frame count), oldest first
         self._next_slot = 0
         self._fill = 0
         self._sizes = []
+        self._sync = []                # 1-based numbers of the IDR samples
         self._own = isinstance(path, (str, os.PathLike))
         self._f = open(path, "wb") if self._own else path
         self._start = self._f.tell()
@@ -229,7 +269,11 @@ class VideoWriter:
         self._next_slot = (slot + 1) % self.RING
         if len(self._pending) == self.RING:
             self._drain(1)
-        launch_encode(self._frames[:n], self.qp, self._scratch, self._out, self._out_len)
+        if self._state is None:
+            launch_encode(self._frames[:n], self.qp, self._scratch, self._out, self._out_len)
+        else:
+            launch_encode_stream(self._frames[:n], self.qp, self.gop, self._state, self._scratch, self._out,
+                                 self._out_len)
         host, host_len = self._ring[slot]
         launch_copy(self._out[:n], self._out_len[:n], host, host_len)
         ev = torch.cuda.Event()
@@ -245,8 +289,10 @@ class VideoWriter:
             hv = host.numpy()
             for k in range(n):
                 s = bytearray(hv[k, :lens[k]].tobytes())
-                if len(self._sizes) % 2:
-                    s[6] |= 1                      # idr_pic_id 2 on odd samples (include/gab200_rasterizer.h)
+                if s[4] == 0x65:                   # an IDR picture
+                    if len(self._sync) % 2:
+                        s[6] |= 1                  # idr_pic_id 2 on odd IDR pictures (include/gab200_rasterizer.h)
+                    self._sync.append(len(self._sizes) + 1)
                 self._f.write(s)
                 self._sizes.append(lens[k])
 
@@ -258,7 +304,8 @@ class VideoWriter:
                 self._encode()
             self._drain(len(self._pending))
         end = self._f.tell()
-        self._f.write(moov_box(self._sizes, self._mdat + MDAT_HEADER, self.W, self.H, self.sps, self.pps, self.fps))
+        self._f.write(moov_box(self._sizes, self._mdat + MDAT_HEADER, self.W, self.H, self.sps, self.pps, self.fps,
+                               self._sync if self.gop > 1 else None))
         after = self._f.tell()
         self._f.seek(self._mdat + 8)
         self._f.write(struct.pack(">Q", end - self._mdat))
@@ -273,10 +320,10 @@ class VideoWriter:
 
 
 @torch.no_grad()
-def encode_video(frames: torch.Tensor, fps=25, qp: int = 20) -> bytes:
+def encode_video(frames: torch.Tensor, fps=25, qp: int = 20, gop: int = 1) -> bytes:
     """A whole MP4 of a CUDA uint8 (H,W,3) frame or (K,H,W,3) clip, in memory."""
     K, H, W = check_frames(frames)
     buf = io.BytesIO()
-    with VideoWriter(buf, W, H, fps=fps, qp=qp, batch=min(K, 16), device=frames.device) as vw:
+    with VideoWriter(buf, W, H, fps=fps, qp=qp, batch=min(K, 16), device=frames.device, gop=gop) as vw:
         vw.add(frames)
     return buf.getvalue()

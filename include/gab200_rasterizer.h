@@ -574,6 +574,44 @@ int32_t gab200_h264_encode(int32_t frames, int32_t height, int32_t width, int32_
 int32_t gab200_h264_parameter_sets(int32_t width, int32_t height, int32_t qp, int32_t fps_num, int32_t fps_den,
                                    uint8_t* out, int64_t cap);
 
+/* A stream with P pictures (gaussianavatars_b200.video VideoWriter(gop=N)).  Stream position n is an IDR picture when
+ * n % gop == 0, byte for byte the sample gab200_h264_encode makes of that frame alone; every other picture is one P
+ * slice (nal_ref_idc 3, nal_unit_type 1) that refers to the previous picture, with frame_num (n - last IDR) mod 16,
+ * no reordering, no reference count override and no adaptive marking.  The SPS differs from the intra stream's in
+ * max_num_ref_frames (1 when gop > 1); with gop 1 the stream is gab200_h264_encode's.
+ *
+ * A P macroblock is P_Skip, P_L0_16x16 (one quarter-sample vector), I_16x16 (mb_type + 5) or I_PCM (30), decided from
+ * pixels alone: an integer full search over +-16 samples by 16x16 luma SAD + lambda * (the se(v) bits of the vector's
+ * two components), lambda = 2^max(0, (qp - 12) / 6), then a half- and a quarter-sample refinement over the 8
+ * neighbours by SATD + the same term, every minimum the first in a fixed order; intra when its least luma SATD + 24
+ * lambda is below that cost; inter residuals quantised with f = 2^qbits / 6; I_PCM when a level leaves +-2063 or the
+ * macroblock's bits, the mvd and skip run aside, exceed 9 + 3072.  The motion vector predictors (8.4.1.3) and the
+ * skip runs follow from those decisions: a P_L0_16x16 macroblock without coded coefficients whose vector equals its
+ * mvpSkip (8.4.1.1) is P_Skip.  The reference is the previous picture's padded reconstruction, read at coordinates
+ * clamped to the coded picture.  tests/h264_stream_oracle.py restates the encode bit for bit. */
+/* The largest P sample of a width x height frame: 5 + n + ceil(n / 2) for the n bytes of a slice of I_PCM macroblocks
+ * each behind a 3-bit skip run and a 34-bit mvd allowance; -1 where gab200_h264_bound is -1. */
+int64_t gab200_h264_p_bound(int32_t width, int32_t height);
+/* Bytes of a stream's state: the stream position (int64) at byte 0 and the previous picture's padded reconstruction
+ * from byte 256.  A zeroed state starts a stream: its next frame is an IDR picture.  0 for a refused size. */
+size_t gab200_h264_state_bytes(int32_t height, int32_t width);
+/* Scratch bytes of gab200_h264_encode_stream (0 for a size, count or gop it refuses). */
+size_t gab200_h264_stream_scratch_bytes(int32_t frames, int32_t height, int32_t width, int32_t gop);
+/* Encode rgb [frames, height, width, 3] as the next frames of the stream whose state (gab200_h264_state_bytes bytes,
+ * device, 256-byte aligned) the call reads and advances on the device; samples as gab200_h264_encode writes them,
+ * out_stride >= gab200_h264_p_bound when gop > 1.  The macroblocks run as one wavefront over (frame, anti-diagonal):
+ * frame f + 1 runs diagonal d in the launch where frame f runs diagonal d + 5, since a macroblock's reference window
+ * reaches 19 samples, two macroblocks, right and down (width / 16 + height / 16 - 1 + 5 (frames - 1) launches).
+ * Reads nothing on the host: capturable, and a replay continues the stream.  Refused before any device work: what
+ * gab200_h264_encode refuses, gop outside 1..65535, a null or misaligned state. */
+int32_t gab200_h264_encode_stream(int32_t frames, int32_t height, int32_t width, int32_t qp, int32_t gop,
+                                  const uint8_t* rgb, void* state, void* scratch, uint8_t* out, int64_t out_stride,
+                                  int64_t* out_len, void* stream);
+/* gab200_h264_parameter_sets of a stream with this gop (max_num_ref_frames 1 when gop > 1); -1 also for a gop outside
+ * 1..65535. */
+int32_t gab200_h264_stream_parameter_sets(int32_t width, int32_t height, int32_t qp, int32_t fps_num, int32_t fps_den,
+                                          int32_t gop, uint8_t* out, int64_t cap);
+
 /* A device-resident view schedule (csrc/schedule.cu, gaussianavatars_b200.schedule.ViewSchedule): `records` records
  * of `views` cameras each -- cams [records, views, GAB200_CAMERA_FLOATS] float32, timesteps [records] int32 (may be
  * NULL), frame_ids [records, views] int32 (may be NULL) -- visited in the order order[0 .. length).  `cursor` is one
