@@ -18,6 +18,7 @@ from .lpips import LpipsNet, lpips, launch_lpips, lpips_features
 from .png import decode_png, encode_png, png_bound
 from .resize import loader_size, resize_u8
 from .video import VideoWriter, encode_video
+from .trajectory import CameraPath, keyframe, export_trajectory
 
 __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gaussians", "rasterize_bound",
            "bind_activate", "set_exact_binning", "face_frame", "l1_loss_u8", "render", "render_bound", "render_display", "render_views",
@@ -26,4 +27,5 @@ __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gau
            "add_densification_stats", "expon_lr_schedule", "FlameLBS", "flame_pose", "flame_param_groups",
            "mesh_overlay", "mesh_overlay_views", "MeshRenderer", "composite_rgba", "FrameStore",
            "ViewSchedule", "epoch_order", "LpipsNet", "lpips", "launch_lpips", "lpips_features",
-           "decode_png", "encode_png", "png_bound", "loader_size", "resize_u8", "VideoWriter", "encode_video"]
+           "decode_png", "encode_png", "png_bound", "loader_size", "resize_u8", "VideoWriter", "encode_video",
+           "CameraPath", "keyframe", "export_trajectory"]

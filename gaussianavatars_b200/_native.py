@@ -32,7 +32,8 @@ class ForwardArgs(C.Structure):
         ("tanfovx", C.c_float), ("tanfovy", C.c_float), ("scale_modifier", C.c_float),
         ("prefiltered", C.c_int32), ("debug", C.c_int32), ("need_backward", C.c_int32), ("binning_hint", C.c_int32),
         ("exact_binning", C.c_int32), ("depth_hint_lo", C.c_uint32), ("depth_hint_hi", C.c_uint32),
-        ("sync_mode", C.c_int32), ("frame_seq", C.c_uint32), ("counters_host", C.c_void_p),
+        ("sync_mode", C.c_int32), ("frame_seq", C.c_uint32), ("display_quantize", C.c_int32),
+        ("counters_host", C.c_void_p),
         ("overflow_flag", C.c_void_p),
         ("bg", C.c_void_p), ("viewmatrix", C.c_void_p), ("projmatrix", C.c_void_p), ("campos", C.c_void_p),
         ("means3D", C.c_void_p), ("opacities", C.c_void_p), ("scales", C.c_void_p), ("rotations", C.c_void_p),
@@ -106,6 +107,19 @@ class LpipsArgs(C.Structure):
     ]
 
 
+QUANTIZE_RENDER, QUANTIZE_VIEWER = 0, 1
+QUANTIZE = {"render": QUANTIZE_RENDER, "viewer": QUANTIZE_VIEWER}   # gab200_display_quantize
+
+
+def quantize_mode(quantize: str) -> int:
+    """The gab200_display_quantize of a display image: "render" (render.py's bytes) or "viewer" (the local viewer's
+    export)."""
+    if quantize not in QUANTIZE:
+        raise ValueError(f"quantize must be 'render' (render.py's bytes) or 'viewer' (the local viewer's export), got "
+                         f"{quantize!r}")
+    return QUANTIZE[quantize]
+
+
 MESH_POS_WORLD, MESH_POS_CLIP = 0, 1
 MESH_LIGHT_FRONT, MESH_LIGHT_CONSTANT = 0, 1
 MESH_BASE_NONE, MESH_BASE_FLOAT_CHW, MESH_BASE_U8_CHW = 0, 1, 2
@@ -121,7 +135,7 @@ class MeshArgs(C.Structure):
         ("antialias", C.c_int32), ("base_kind", C.c_int32), ("base", C.c_void_p), ("opacity", C.c_void_p),
         ("out_u8", C.c_void_p), ("out_float", C.c_void_p), ("out_rgba", C.c_void_p), ("out_rast", C.c_void_p),
         ("in_rast", C.c_void_p), ("in_color", C.c_void_p), ("out_color", C.c_void_p), ("channels", C.c_int32),
-        ("error_flag", C.c_void_p), ("scratch", C.c_void_p),
+        ("quantize", C.c_int32), ("error_flag", C.c_void_p), ("scratch", C.c_void_p),
     ]
 
 

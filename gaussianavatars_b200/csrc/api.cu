@@ -3,6 +3,7 @@
 // instance count N (gab200_sync_mode: a wait in the middle, a wait at the end that normally finds its answer ready,
 // or no wait at all under CUDA-graph capture).  No torch types, no exceptions; process-wide state is limited to
 // atomics (launch counter, profiling timers, tuning knobs).
+#include <cstddef>
 #include <atomic>
 #include <chrono>
 #include <cstdio>
@@ -258,6 +259,7 @@ int tune_get(int knob) {
 // display_only: gab200_forward_display with a uint8 image and no backward, the one case out_color may be NULL
 static bool validate(const gab200_forward_args* a, bool display_only = false) {
   if (a == nullptr || a->abi_version != GAB200_ABI_VERSION) return false;
+  if (a->display_quantize != GAB200_QUANTIZE_RENDER && a->display_quantize != GAB200_QUANTIZE_VIEWER) return false;
   if (a->P < 0 || a->image_width <= 0 || a->image_height <= 0) return false;
   if ((a->out_color == nullptr && !display_only) || (a->P > 0 && a->radii == nullptr)) return false;
   if (!a->bg || !a->viewmatrix || !a->projmatrix || !a->campos) return false;
@@ -536,7 +538,7 @@ int enqueue_binning_blend(Frame& f, void* bin, int64_t cap, int64_t n_known, siz
     StageScope sc(GAB200_STAGE_BLEND_FWD, stream);
     launch_blend_forward(f.views, f.W, f.H, f.iv.ranges, f.iv.order, f.iv.order_info, bv.vals[selector], f.g.rec, a->bg,
                          a->out_color, f.iv.final_T, f.iv.n_contrib, bv.strip_mask, f.out_rgb8, f.out_alpha,
-                         f.out_depth, stream);
+                         f.out_depth, a->display_quantize, stream);
   }
   GAB_STAGE_CHECK(f.dbg, stream);
   return GAB200_OK;
@@ -561,6 +563,8 @@ static int64_t run_forward(const gab200_forward_args* a, const float* tanfov, ui
   cudaStream_t stream = (cudaStream_t)stream_;
   if (!validate(a, out_rgb8 != nullptr && a != nullptr && a->need_backward == 0) || st == nullptr)
     return GAB200_ERR_INVALID_ARGUMENT;
+  // the viewer's display bytes come from the forward-only forms without the planes
+  if (a->display_quantize == GAB200_QUANTIZE_VIEWER && (a->need_backward != 0 || da)) return GAB200_ERR_INVALID_ARGUMENT;
   if (check_arch() < 0) return GAB200_ERR_ARCH;
   memset(st, 0, sizeof(*st));
   Frame f;
@@ -1223,6 +1227,14 @@ size_t gab200_mesh_views_scratch_bytes(int32_t views, int32_t num_faces, int32_t
   return mesh_scratch_bytes(views, num_faces, width, height);
 }
 
+// The quantisation modes sit in the structs' alignment holes: their sizes and every other offset stay those of earlier
+// releases of ABI version 3.
+static_assert(offsetof(gab200_forward_args, display_quantize) == 76 && offsetof(gab200_forward_args, counters_host) == 80,
+              "gab200_forward_args layout");
+static_assert(offsetof(gab200_mesh_args, quantize) == 164 && offsetof(gab200_mesh_args, error_flag) == 168 &&
+                  sizeof(gab200_mesh_args) == 184,
+              "gab200_mesh_args layout");
+
 static bool mesh_args_ok(const gab200_mesh_args* a) {
   if (a == nullptr || a->abi_version != GAB200_ABI_VERSION || a->V < 1 || a->F < 1 || a->width < 1 || a->height < 1 ||
       a->width > kMeshMaxSide || a->height > kMeshMaxSide || !a->verts || !a->faces || !a->scratch ||
@@ -1232,6 +1244,7 @@ static bool mesh_args_ok(const gab200_mesh_args* a) {
   if (a->lighting != GAB200_MESH_LIGHT_FRONT && a->lighting != GAB200_MESH_LIGHT_CONSTANT) return false;
   if (a->base_kind < GAB200_MESH_BASE_NONE || a->base_kind > GAB200_MESH_BASE_U8_CHW) return false;
   if (a->antialias != 0 && a->antialias != 1) return false;
+  if (a->quantize != GAB200_QUANTIZE_RENDER && a->quantize != GAB200_QUANTIZE_VIEWER) return false;
   if (a->antialias && !a->adjacency) return false;
   if (a->pos_kind == GAB200_MESH_POS_WORLD && !a->camera) return false;
   const bool composite = a->out_u8 || a->out_float;

@@ -135,6 +135,7 @@ struct BandGeom {
 #define BLEND_OUT_FLOAT 1  // [3,H,W] float32
 #define BLEND_OUT_U8 2     // [H,W,3] uint8
 #define BLEND_OUT_TRAIN 4  // final_T and n_contrib [H,W] and the block masks, which the backward reads
+#define BLEND_OUT_VIEWER 8 // with BLEND_OUT_U8: the display bytes quantised as the local viewer's export does
 __device__ __forceinline__ uint32_t quantize_u8(float c) {
   return __float2uint_rz(fminf(fmaxf(__fadd_rn(__fmul_rn(c, 255.f), 0.5f), 0.f), 255.f));
 }
@@ -142,9 +143,12 @@ __device__ __forceinline__ uint32_t quantize_u8(float c) {
 // (row, j < 6) writes word j, bytes 4j .. 4j+3, which lie in pixels p0 = 4j/3 and p0 + 1 from byte 4j - 3 p0 of p0:
 // two shuffles per band, and the warp stores whole aligned 32-bit words instead of 96 scattered bytes.  A row whose
 // start is not word-aligned (W % 4 != 0) or that the image's right edge cuts stores bytes.  All 32 lanes call this.
+// VIEWER: quantize_u8_viewer in place of quantize_u8 (GAB200_QUANTIZE_VIEWER).
+template <bool VIEWER>
 __device__ __forceinline__ void store_display(uint8_t* __restrict__ out, int W, int H, int pixx, int y, int lane,
                                               float r, float g, float b) {
-  const uint32_t px = quantize_u8(r) | (quantize_u8(g) << 8) | (quantize_u8(b) << 16);
+  const uint32_t px = VIEWER ? quantize_u8_viewer(r) | (quantize_u8_viewer(g) << 8) | (quantize_u8_viewer(b) << 16)
+                             : quantize_u8(r) | (quantize_u8(g) << 8) | (quantize_u8(b) << 16);
   const int j = lane & 7, x0 = pixx - j;
   const int p0 = min((4 * j) / 3, 6);
   const uint32_t lo = __shfl_sync(FULLMASK, px, (lane & ~7) | p0);
@@ -394,8 +398,8 @@ __device__ __forceinline__ void forward_tile(int tile, int tl, GroupBarrier<256 
   if (OUT & BLEND_OUT_U8) {
 #pragma unroll
     for (int i = 0; i < K; i++)
-      store_display(out_rgb8, W, H, pixx, pixy0 + 4 * i, lane, fmaf(T[i], bg0, Cr[i]), fmaf(T[i], bg1, Cg[i]),
-                    fmaf(T[i], bg2, Cb[i]));
+      store_display<(OUT & BLEND_OUT_VIEWER) != 0>(out_rgb8, W, H, pixx, pixy0 + 4 * i, lane, fmaf(T[i], bg0, Cr[i]),
+                                                   fmaf(T[i], bg1, Cg[i]), fmaf(T[i], bg2, Cb[i]));
   }
 }
 
@@ -438,10 +442,13 @@ __global__ void __launch_bounds__(256, DA                                 ? GAB_
 
 template <bool DA, bool VIEWS>
 static decltype(&blend_forward_kernel<BLEND_OUT_FLOAT, DA, VIEWS>) blend_forward_instance(int out) {
-  constexpr int F = BLEND_OUT_FLOAT, U = BLEND_OUT_U8, T = BLEND_OUT_TRAIN;
+  constexpr int F = BLEND_OUT_FLOAT, U = BLEND_OUT_U8, T = BLEND_OUT_TRAIN, V = BLEND_OUT_VIEWER;
   if constexpr (!DA) {  // the plane forms keep the training outputs at run time whatever OUT says
     if (out == (F | T)) return blend_forward_kernel<F | T, DA, VIEWS>;
     if (out == (F | U | T)) return blend_forward_kernel<F | U | T, DA, VIEWS>;
+    // the viewer's quantisation: forward-only display forms without the planes (the entry points refuse the rest)
+    if (out == (U | V)) return blend_forward_kernel<U | V, DA, VIEWS>;
+    if (out == (F | U | V)) return blend_forward_kernel<F | U | V, DA, VIEWS>;
   }
   out &= F | U;
   return out == F ? blend_forward_kernel<F, DA, VIEWS>
@@ -452,12 +459,13 @@ static decltype(&blend_forward_kernel<BLEND_OUT_FLOAT, DA, VIEWS>) blend_forward
 void launch_blend_forward(int views, int W, int H, const uint2* ranges, const uint32_t* order,
                           const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec, const float* bg,
                           float* out_color, float* final_T, uint32_t* n_contrib, uint8_t* strip_mask, uint8_t* out_rgb8,
-                          float* out_alpha, float* out_depth, cudaStream_t stream) {
+                          float* out_alpha, float* out_depth, int quantize, cudaStream_t stream) {
   const int gx = (W + GAB_TILE - 1) / GAB_TILE, gy = (H + GAB_TILE - 1) / GAB_TILE;
   const int view_tiles = gx * gy, tiles = views * view_tiles;
   if (tiles == 0) return;
   const int out = (out_color != nullptr ? BLEND_OUT_FLOAT : 0) | (out_rgb8 != nullptr ? BLEND_OUT_U8 : 0) |
-                  (final_T != nullptr ? BLEND_OUT_TRAIN : 0);
+                  (final_T != nullptr ? BLEND_OUT_TRAIN : 0) |
+                  (out_rgb8 != nullptr && quantize == GAB200_QUANTIZE_VIEWER ? BLEND_OUT_VIEWER : 0);
   const bool da = out_alpha != nullptr || out_depth != nullptr;
   auto kernel = da ? (views > 1 ? blend_forward_instance<true, true>(out) : blend_forward_instance<true, false>(out))
                    : (views > 1 ? blend_forward_instance<false, true>(out) : blend_forward_instance<false, false>(out));

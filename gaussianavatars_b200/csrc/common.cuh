@@ -37,6 +37,12 @@ struct __align__(16) SplatAux {
 //    dL/dz (depth plane only; else pad), pad*2)
 #define GAB_G2D_STRIDE 12
 
+// The local viewer's export quantisation (GAB200_QUANTIZE_VIEWER): numpy's (np.clip(c, 0, 1) * 255).astype(np.uint8)
+// on a float32 pixel, one rounded multiply and truncation.  fmaxf first: a NaN channel gives 0.
+__device__ __forceinline__ uint32_t quantize_u8_viewer(float c) {
+  return __float2uint_rz(__fmul_rn(fminf(fmaxf(c, 0.f), 1.f), 255.f));
+}
+
 struct Camera {  // staged once per block in shared memory
   float V[16];
   float Pm[16];

@@ -186,10 +186,11 @@ cudaError_t run_sort(void* temp, size_t temp_bytes, uint32_t* keys_a, uint32_t* 
 // out_color [views,3,H,W] / out_rgb8 [views,H,W,3]: either may be NULL.  final_T != NULL (the training forms): also
 // final_T / n_contrib [views,H,W] and the per-instance block masks, kept for launch_blend_backward.
 // out_alpha / out_depth [views,H,W]: the accumulated alpha and depth planes (either may be NULL; records with z in q2.w)
+// quantize: gab200_display_quantize of out_rgb8; GAB200_QUANTIZE_VIEWER only without final_T and the planes
 void launch_blend_forward(int views, int W, int H, const uint2* ranges, const uint32_t* order,
                           const uint32_t* order_info, const uint32_t* point_list, const SplatRec* rec, const float* bg,
                           float* out_color, float* final_T, uint32_t* n_contrib, uint8_t* strip_mask, uint8_t* out_rgb8,
-                          float* out_alpha, float* out_depth, cudaStream_t stream);
+                          float* out_alpha, float* out_depth, int quantize, cudaStream_t stream);
 // the same tiles: dL_dpix [views,3,H,W]; g2d rows of the views * P virtual splats.  da: also the plane gradients
 // dL_dalpha / dL_ddepth [views,H,W] (NULL: zero); dL/dz -> g2d slot 9 of each virtual splat's row
 void launch_blend_backward(int views, int W, int H, const uint2* ranges, const uint32_t* order,

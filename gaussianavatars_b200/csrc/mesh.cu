@@ -427,7 +427,8 @@ struct ResolveOut {
 };
 
 // One thread per (view, pixel), view = blockIdx.z.  Only base and out_u8 have a view dimension: the other outputs
-// exist for single-view calls only.
+// exist for single-view calls only.  VIEWER: out_u8 quantised as the local viewer's export (GAB200_QUANTIZE_VIEWER).
+template <bool VIEWER>
 __global__ void __launch_bounds__(256) mesh_resolve_kernel(MeshParams p, ResolveOut o,
                                                            const FacePoly* __restrict__ all_polys,
                                                            const FaceEdges* __restrict__ all_edges,
@@ -521,7 +522,7 @@ __global__ void __launch_bounds__(256) mesh_resolve_kernel(MeshParams p, Resolve
       b = static_cast<const float*>(o.base)[(3 * view + ch) * HW + pix];
     const float v = __fadd_rn(__fmul_rn(__fmul_rn(rgb[ch], a), op), __fmul_rn(b, keep));
     if (o.out_float) o.out_float[ch * HW + pix] = v;
-    q[ch] = quantize_u8(v);
+    q[ch] = VIEWER ? quantize_u8_viewer(v) : quantize_u8(v);
   }
   if (o.out_u8) {
     uint8_t* out = o.out_u8 + 3 * (view * HW + pix);
@@ -614,8 +615,11 @@ cudaError_t launch_mesh_render(const gab200_mesh_args& a, int K, cudaStream_t st
   o.bg = bg; o.base = a.base; o.opacity = a.opacity; o.in_color = a.in_color;
   o.out_u8 = a.out_u8; o.out_float = a.out_float; o.out_rgba = a.out_rgba; o.out_rast = a.out_rast;
   o.out_color = a.out_color;
-  mesh_resolve_kernel<<<dim3((a.width + 255) / 256, a.height, K), 256, 0, stream>>>(p, o, s.polys, s.edges, s.colors,
-                                                                                    s.winner);
+  const dim3 grid((a.width + 255) / 256, a.height, K);
+  if (a.quantize == GAB200_QUANTIZE_VIEWER)
+    mesh_resolve_kernel<true><<<grid, 256, 0, stream>>>(p, o, s.polys, s.edges, s.colors, s.winner);
+  else
+    mesh_resolve_kernel<false><<<grid, 256, 0, stream>>>(p, o, s.polys, s.edges, s.colors, s.winner);
   count_launch();
   return cudaPeekAtLastError();
 }

@@ -428,7 +428,7 @@ class _Captured:
                 raise RuntimeError(f"{type(self).__name__}: iteration {c} still overflows its instance capacity after "
                                    "re-capture")
             grown_at = c
-            self.regrow()   # an overflowed replay and the ones behind it committed nothing: redo them from c
+            self.regrow(c)   # an overflowed replay and the ones behind it committed nothing: redo them from c
             for _ in range(want - c):
                 self._replay_scheduled()
         self._cursor_host, self._pending = want, 0
@@ -452,9 +452,16 @@ class _Captured:
         return dict(num_rendered=int(c[R.N.CTR_NUM_RENDERED]) & 0xFFFFFFFF, capacity=int(c[R.N.CTR_CAPACITY]) & 0xFFFFFFFF,
                     bucket_overflow=int(c[R.N.CTR_BUCKET_OVERFLOW]), listed=int(c[R.N.CTR_NUM_LISTED]) & 0xFFFFFFFF)
 
-    def regrow(self):
-        """Re-capture with the capacity the overflowing frame asked for (x headroom) and a fresh depth range."""
+    def regrow(self, iteration: Optional[int] = None):
+        """Re-capture with the capacity the overflowing frame asked for (x headroom) and a fresh depth range.
+        iteration: with a schedule whose records size the warm-up (no warm cameras), the iteration whose replay
+        overflowed: its record joins the warm-up frames, so that the new depth range and capacity cover it too (a
+        record at a timestep no warm-up frame posed can reach depths outside their range)."""
         torch.cuda.synchronize(self.device)
+        if iteration is not None and self.schedule is not None and self._warm_pairs is not None:
+            s, r = self.schedule, self.schedule.record(int(iteration))
+            self._warm_pairs.append((s.cams[r] if self.K > 1 else s.cams[r, 0],
+                                     None if s.timesteps_host is None else s.timesteps_host[r]))
         need = self.counters()["num_rendered"]
         self.capture(capacity=max(self._room_for(need), int(self.slot.capacity * 1.5)))
 
@@ -962,7 +969,19 @@ class GraphedRender(_Captured):
     ((F,3), e.g. the viewer's splats-per-face colouring) are device buffers written by set_inputs: a slider or a colour
     picker never re-captures.  `mesh_error` is a device int32 set to 1 when a face index is out of range.  With
     views_per_replay=K the mesh is drawn under all K cameras in one launch sequence (mesh.mesh_overlay_views), each
-    view bit for bit its single-camera overlay."""
+    view bit for bit its single-camera overlay.
+
+    quantize="viewer": `display` holds the bytes the reference's local viewer exports (local_viewer.py's
+    (np.clip(rgb, 0, 1) * 255).astype(np.uint8): a float32 multiply and truncation, no +0.5) instead of render.py's,
+    written by the same blend epilogue -- or, with mesh_opacity, by the same mesh resolve -- with no extra pass.
+
+    schedule=s (a schedule.ViewSchedule, e.g. trajectory.CameraPath.schedule()): every captured replay plays the next
+    record of the schedule by itself.  A sampler kernel at its head copies record order[cursor] -- the camera row and
+    the timestep -- into the frame's inputs, and a commit kernel at its end advances the device `cursor` unless the
+    replay overflowed its capacity (csrc/schedule.cu, as GraphedFrame and GraphedEval use them).  run_all() plays the
+    rest of the order, run_iterations(n) the next n records, set_cursor(i) moves the cursor; set_inputs(camera=,
+    cameras=, timestep=) is refused.  With check=True one synchronisation ends the run; a replay that overflowed, and
+    every replay behind it, committed nothing, so the frame regrows and replays from the record that overflowed."""
 
     _MESH_OVER_GT = False   # the mesh is drawn over the splat image into `display` (GraphedEval: over `gt`)
 
@@ -971,7 +990,7 @@ class GraphedRender(_Captured):
                  capacity: Optional[int] = None, headroom: float = 1.25, warm_cameras=None, warm_timesteps=None,
                  mesh_opacity: Optional[float] = None, face_colors: Optional[torch.Tensor] = None,
                  mesh_lighting: str = "front", views_per_replay: int = 1, depth_alpha: bool = False,
-                 png: bool = False):
+                 png: bool = False, quantize: str = "render", schedule=None):
         """outputs: "u8" (the display image only: the float image is not written), "float" or "both".
         warm_cameras: camera objects or 37-float blocks rendered eagerly before the capture to size the capacity (and
         the depth-sort range); warm_timesteps: with a FLAME head, the timesteps each warm camera is rendered at
@@ -986,9 +1005,16 @@ class GraphedRender(_Captured):
         png=True: the captured body ends in the PNG encode of `display` (after the mesh overlay; png.encode_png's
         kernels) into graph-owned scratch, `png_out` ((K, capacity) uint8) and `png_len` ((K,) int64).  With
         host_slots the ring also receives the compressed files, and host_png(i) returns replay i's file (K files with
-        views_per_replay=K)."""
+        views_per_replay=K).
+        quantize: the bytes of `display`, "render" (render.py's, the default) or "viewer" (the local viewer's export);
+        "viewer" needs outputs 'u8' or 'both' and is not combinable with depth_alpha.
+        schedule: a ViewSchedule the replays follow on the device (see the class documentation)."""
         if outputs not in ("u8", "float", "both"):
             raise ValueError("outputs must be 'u8', 'float' or 'both'")
+        N.quantize_mode(quantize)
+        if quantize != "render" and (outputs == "float" or depth_alpha):
+            raise ValueError("quantize='viewer' quantises the display image of a frame without the alpha / depth "
+                             "planes: it needs outputs 'u8' or 'both' and depth_alpha=False")
         if png and outputs == "float":
             raise ValueError("png=True encodes the display image: it needs outputs 'u8' or 'both'")
         _check_views_per_replay(views_per_replay)
@@ -1031,6 +1057,9 @@ class GraphedRender(_Captured):
                 self._set_face_colors(face_colors)
             self.mesh_error = torch.zeros(1, dtype=torch.int32, device=self.device)
             self._adjacency = M._AdjacencyCache()
+        self.quantize = quantize
+        if schedule is not None:
+            self._use_schedule(schedule, None, log=False)
 
     def _set_face_colors(self, face_colors):
         fc = face_colors.detach().reshape(-1, 3)
@@ -1047,6 +1076,9 @@ class GraphedRender(_Captured):
         """Copies new inputs into the graph's device buffers; none of them re-captures.  A camera OBJECT of another
         image size changes the frame's size (the next run() re-captures).  views_per_replay=K > 1: `cameras` (K
         camera objects of one size, or a (K, 37) table) instead of `camera`."""
+        if self.schedule is not None and any(x is not None for x in (camera, cameras, timestep)):
+            raise ValueError("this frame samples its camera and timestep from its schedule on the device: "
+                             "set_inputs(camera=, cameras=, timestep=) is refused (set_cursor moves it)")
         if (camera is not None and self.K > 1) or (cameras is not None and self.K == 1):
             raise ValueError("a frame with views_per_replay > 1 takes cameras=, one with a single view camera=")
         if cameras is not None:
@@ -1076,6 +1108,15 @@ class GraphedRender(_Captured):
 
     # ---- the frame body (run eagerly for warm-up, then captured) -------------------------------------------------
     def _body(self, captured: bool = False):
+        scheduled = captured and self.schedule is not None
+        if scheduled:   # this replay's record: camera row and timestep
+            self._launch_sample()
+        self._frame(captured)
+        if scheduled:   # advance the cursor, unless this replay overflowed
+            self._launch_commit()
+
+    def _frame(self, captured: bool):
+        """The playback frame: pose, forward, mesh overlay, PNG encode."""
         with torch.no_grad():
             if self.mesh_update:
                 self._pose()
@@ -1084,7 +1125,8 @@ class GraphedRender(_Captured):
             out = _forward_only(self.camera if self.K == 1 else self.cam, self.pc, _Pipe, self.bg,
                                 self.scaling_modifier, self.outputs != "float" and not over,
                                 self.outputs != "u8" or over, self.depth_alpha,
-                                None if self.K == 1 else (self.W, self.H))
+                                None if self.K == 1 else (self.W, self.H),
+                                "render" if over else self.quantize)   # with the mesh, its resolve quantises
             if over:
                 out["display_u8"] = self._overlay(out["render"])
         self.image, self.display, self.radii = out["render"], out["display_u8"], out["radii"]
@@ -1119,7 +1161,7 @@ class GraphedRender(_Captured):
                       camera=self.cam, adjacency=self._adjacency.get(pc.faces).to(self.device),
                       face_colors=self.face_colors, lighting=self.mesh_lighting, antialias=True, base=base.contiguous(),
                       opacity=self._opacity, out_u8=display, error_flag=self.mesh_error,
-                      views=None if self.K == 1 else self.K)
+                      views=None if self.K == 1 else self.K, quantize=self.quantize)
         return display
 
     # ---- capture ---------------------------------------------------------------------------------------------------
@@ -1262,6 +1304,9 @@ class GraphedRender(_Captured):
 
     # ---- replay ----------------------------------------------------------------------------------------------------
     def run(self, check: bool = False):
+        if self.schedule is not None:   # the schedule's next record
+            self._run_scheduled(1, check)
+            return self
         if self._stale():
             self.capture()
         self.graph.replay()
@@ -1274,6 +1319,25 @@ class GraphedRender(_Captured):
         if self.host_slots:
             self._ship()
         return self
+
+    def _replay_scheduled(self):
+        self.graph.replay()
+        self.replays += 1
+        if self.host_slots:
+            self._ship()
+
+    def run_iterations(self, n: int, check: bool = True) -> Optional[int]:
+        """schedule=: the next n records of the order as n back-to-back replays with no host input (re-capturing first
+        if the model changed).  Refused on the host, before anything runs, when they could pass the end of the order.
+        check=True synchronises once and regrows after an overflow (see the class documentation).  Returns the number
+        of records played (check=True), else None."""
+        return self._run_scheduled(n, check)
+
+    def run_all(self, check: bool = True) -> Optional[int]:
+        """schedule=: every record of the order not played yet (L replays after set_cursor(0)), as run_iterations."""
+        if self.schedule is None:
+            raise ValueError("run_all needs a frame built with schedule=")
+        return self._run_scheduled(self.schedule.L - self._cursor_host - self._pending, check)
 
 
 class GraphedEval(GraphedRender):
@@ -1432,7 +1496,7 @@ class GraphedEval(GraphedRender):
         if captured and self.schedule is not None:   # this replay's record, its rows, and its ground truth
             self._launch_sample(ids=self.frame_ids, rows=self.view if self.K == 1 else self.rows)
             self.frames.launch_decode(self.frame_ids, self.gt, None)
-        super()._body(captured)
+        self._frame(captured)
         if captured:   # the warm-up frames score nothing: they would write the current view's row
             rendered = self.image if self.source == "float" else self.display
             if self.K == 1:
@@ -1480,12 +1544,6 @@ class GraphedEval(GraphedRender):
         if self._side is not None:
             self._mark_read()
         return self
-
-    def _replay_scheduled(self):
-        self.graph.replay()
-        self.replays += 1
-        if self.host_slots:
-            self._ship()
 
     def host_mesh_png(self, replay: Optional[int] = None):
         """Replay `replay`'s mesh PNG file (default: the latest) as bytes -- K files with views_per_replay=K -- once its

@@ -90,9 +90,10 @@ def _camera_floats(camera, device) -> torch.Tensor:
 def launch_mesh(*, verts, faces, width, height, pos_kind=N.MESH_POS_WORLD, camera=None, adjacency=None,
                 face_colors=None, background=(1.0, 1.0, 1.0), lighting="front", antialias=True, base=None,
                 opacity=None, out_u8=None, out_float=None, out_rgba=None, out_rast=None, in_rast=None, in_color=None,
-                out_color=None, error_flag=None, stream=None, views=None):
+                out_color=None, error_flag=None, stream=None, views=None, quantize="render"):
     """One gab200_mesh_render call on device tensors (no checks beyond the library's own); returns nothing.
-    views=K: one gab200_mesh_render_views call instead -- camera a (K,37) table, base (K,3,H,W), out_u8 (K,H,W,3)."""
+    views=K: one gab200_mesh_render_views call instead -- camera a (K,37) table, base (K,3,H,W), out_u8 (K,H,W,3).
+    quantize: how out_u8 is quantised, "render" (render.py's bytes) or "viewer" (the local viewer's export)."""
     dev = verts.device
     F = faces.shape[0]
     _check_size(width, height)
@@ -113,6 +114,7 @@ def launch_mesh(*, verts, faces, width, height, pos_kind=N.MESH_POS_WORLD, camer
     a.out_u8, a.out_float, a.out_rgba, a.out_rast = N.ptr(out_u8), N.ptr(out_float), N.ptr(out_rgba), N.ptr(out_rast)
     a.in_rast, a.in_color, a.out_color = N.ptr(in_rast), N.ptr(in_color), N.ptr(out_color)
     a.channels = 0 if in_color is None else in_color.shape[-1]
+    a.quantize = N.quantize_mode(quantize)
     a.error_flag = N.ptr(error_flag)
     L = N.lib()
     nbytes = L.gab200_mesh_scratch_bytes(F, width, height) if views is None else \

@@ -552,7 +552,7 @@ class _RasterizeBound(torch.autograd.Function):
     @staticmethod
     def forward(ctx, _xyz, means2D, _rotation, _scaling, _opacity, f_dc, f_rest, face_center, face_orien_mat,
                 face_scaling, binding, colors_precomp, raster_settings, grad_sink=None, tanfov=None, rgb8=None,
-                float_image=True, depth_alpha=False, hints=None, cameras=None):
+                float_image=True, depth_alpha=False, hints=None, cameras=None, quantize=N.QUANTIZE_RENDER):
         rs = raster_settings
         ctx.grad_sink = grad_sink
         device = _xyz.device
@@ -563,6 +563,10 @@ class _RasterizeBound(torch.autograd.Function):
         need_bw = any(ctx.needs_input_grad)
         a = N.ForwardArgs()
         cams = _fill_common(a, rs, device, P, need_bw, cameras)
+        a.display_quantize = quantize
+        if quantize != N.QUANTIZE_RENDER and (rgb8 is None or need_bw or depth_alpha):
+            raise ValueError("the viewer's quantisation writes the display image of a forward-only frame without the "
+                             "alpha / depth planes: it needs rgb8=, no gradient and depth_alpha=False")
         binding_orig = binding
         _xyz, _rotation, _scaling, _opacity, f_dc, f_rest, colors_precomp, binding, face_center, face_orien_mat, \
             face_scaling = _fill_bound(a, device, _xyz, _rotation, _scaling, _opacity, f_dc, f_rest, colors_precomp,
@@ -649,13 +653,13 @@ class _RasterizeBound(torch.autograd.Function):
             ctx.grad_sink.flat_grad = flat
             ctx.grad_sink._gab200_mc_used = bool(use_symm)  # SymmetricGradBuffer.end() only trusts the replica if set
         return (d_xyz, d_means2D, d_rot, d_scale, d_opac, d_dc, d_rest, d_fc, d_fR, d_fs, None, d_colors, None, None,
-                None, None, None, None, None, None)
+                None, None, None, None, None, None, None)
 
 
 def rasterize_bound(raster_settings: GaussianRasterizationSettings, _xyz, _rotation, _scaling, _opacity,
                     features_dc, features_rest, binding=None, face_center=None, face_orien_mat=None,
                     face_scaling=None, means2D=None, colors_precomp=None, grad_sink=None, tanfov=None, rgb8=None,
-                    float_image=True, depth_alpha=False):
+                    float_image=True, depth_alpha=False, quantize: str = "render"):
     """Fused binding + rasterization.  Returns (color (3,H,W), radii (P,) int32); with depth_alpha=True
     (color, radii, alpha (1,H,W), depth (1,H,W)).
 
@@ -667,6 +671,8 @@ def rasterize_bound(raster_settings: GaussianRasterizationSettings, _xyz, _rotat
     `rgb8`: optional contiguous (H,W,3) uint8 CUDA tensor that the forward blend also fills with the display image,
     bit for bit torch's color.mul(255).add_(0.5).clamp_(0, 255).permute(1, 2, 0).to(torch.uint8)
     (gab200_forward_display).  float_image=False (rgb8 given, no gradient) skips the float image: color is None.
+    quantize="viewer" (rgb8 given, no gradient, no planes): the display bytes are the local viewer's export instead,
+    (np.clip(color, 0, 1) * 255).astype(np.uint8) on the float32 image -- no +0.5 (GAB200_QUANTIZE_VIEWER).
     depth_alpha=True (gab200_forward_depth_alpha): also the accumulated alpha 1 - T_final and the alpha-weighted
     view-space depth sum_i w_i z_i (not normalised: depth / alpha is a viewer's depth) of the same blend, both
     differentiable; the colour image, radii and display bytes are those of depth_alpha=False bit for bit.  The gradients
@@ -683,7 +689,8 @@ def rasterize_bound(raster_settings: GaussianRasterizationSettings, _xyz, _rotat
     return _RasterizeBound.apply(_xyz, means2D, _rotation, _scaling, _opacity, features_dc, features_rest,
                                  face_center, face_orien_mat, face_scaling, binding, colors_precomp, raster_settings,
                                  grad_sink, tanfov, rgb8, bool(float_image), bool(depth_alpha),
-                                 hints_of(grad_sink) if grad_sink is not None else None)
+                                 hints_of(grad_sink) if grad_sink is not None else None, None,
+                                 N.quantize_mode(quantize))
 
 
 # ================================================================================================================
@@ -717,7 +724,8 @@ def check_camera_table(cameras, device) -> torch.Tensor:
 def rasterize_bound_views(raster_settings: GaussianRasterizationSettings, cameras: torch.Tensor, _xyz, _rotation,
                           _scaling, _opacity, features_dc, features_rest, binding=None, face_center=None,
                           face_orien_mat=None, face_scaling=None, colors_precomp=None, hints: Optional[FrameHints] = None,
-                          display: bool = True, float_image: bool = False, depth_alpha: bool = False):
+                          display: bool = True, float_image: bool = False, depth_alpha: bool = False,
+                          quantize: str = "render"):
     """Fused binding + rasterization of K cameras in ONE forward (gab200_forward_views), forward only.
 
     `cameras`: (K, 37) float32 device table, row k = camera_block(cam_k, fov=True); each view uses its own matrices,
@@ -729,7 +737,7 @@ def rasterize_bound_views(raster_settings: GaussianRasterizationSettings, camera
     gradient while grad mode is on is refused.
     depth_alpha=True (gab200_forward_views_depth_alpha): also returns alpha and depth, (K,1,H,W) float32 each, the planes
     of rasterize_bound(..., depth_alpha=True) for every view; the other outputs are those of depth_alpha=False bit for
-    bit."""
+    bit.  quantize: as rasterize_bound's."""
     tensors = [t for t in (_xyz, _rotation, _scaling, _opacity, features_dc, features_rest, face_center,
                            face_orien_mat, face_scaling, colors_precomp) if t is not None]
     if torch.is_grad_enabled() and any(t.requires_grad for t in tensors):
@@ -750,7 +758,7 @@ def rasterize_bound_views(raster_settings: GaussianRasterizationSettings, camera
         color, radii, *planes = _RasterizeBound.apply(
             d(_xyz), None, d(_rotation), d(_scaling), d(_opacity), d(features_dc), d(features_rest), d(face_center),
             d(face_orien_mat), d(face_scaling), binding, d(colors_precomp), rs, None, None, rgb8, bool(float_image),
-            bool(depth_alpha), hints if hints is not None else FrameHints(), cameras)
+            bool(depth_alpha), hints if hints is not None else FrameHints(), cameras, N.quantize_mode(quantize))
     return (color, rgb8, radii, visible_of(radii), *planes)
 
 

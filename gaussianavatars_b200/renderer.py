@@ -103,10 +103,11 @@ def _train_frame(camera, pc, pipe, bg_color, scaling_modifier, override_color, d
 
 
 def _forward_only(camera, pc, pipe, bg_color, scaling_modifier, display: bool, float_image: bool,
-                  depth_alpha: bool = False, size=None):
+                  depth_alpha: bool = False, size=None, quantize: str = "render"):
     """Fused route, forward only (no autograd): the float image and/or the display image [and the alpha / depth
     planes] of a camera object, or of the views of a (K, 37) device camera table of image `size` (W, H)
-    (render_views, GraphedRender): then every output has a leading K."""
+    (render_views, GraphedRender): then every output has a leading K.  quantize: the display image's bytes,
+    "render" or "viewer" (rasterizer.rasterize_bound)."""
     if not _has_raw(pc):
         raise ValueError("render_display needs the fused route: a model exposing the raw parameters "
                          "(_xyz, _rotation, _scaling, _opacity, _features_dc, _features_rest)")
@@ -120,27 +121,33 @@ def _forward_only(camera, pc, pipe, bg_color, scaling_modifier, display: bool, f
             rgb8 = torch.empty((rs.image_height, rs.image_width, 3), dtype=torch.uint8, device=device) \
                 if display else None
             img, radii, *planes = rasterize_bound(rs, *raw, grad_sink=pc, tanfov=getattr(camera, "tanfov", None),
-                                                  rgb8=rgb8, float_image=float_image, depth_alpha=depth_alpha)
+                                                  rgb8=rgb8, float_image=float_image, depth_alpha=depth_alpha,
+                                                  quantize=quantize)
             visible = _visible(radii)
         else:
             img, rgb8, radii, visible, *planes = rasterize_bound_views(
                 rs, camera, *raw, hints=view_hints_of(pc), display=display, float_image=float_image,
-                depth_alpha=depth_alpha)
+                depth_alpha=depth_alpha, quantize=quantize)
     res = {"display_u8": rgb8, "render": img, "radii": radii, "visibility_filter": visible}
     if depth_alpha:
         res["alpha"], res["depth"] = planes
     return res
 
 
-def render_display(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, float_image=False, depth_alpha=False):
+def render_display(viewpoint_camera, pc, pipe, bg_color, scaling_modifier=1.0, float_image=False, depth_alpha=False,
+                   quantize="render"):
     """One playback frame: the fused route's forward only, no autograd, with the image as the reference's render.py
     and viewers consume it -- `display_u8`, a (H,W,3) uint8 tensor equal bit for bit to
     render(...)["render"].mul(255).add_(0.5).clamp_(0, 255).permute(1, 2, 0).to(torch.uint8), written by the forward
     blend itself (3 bytes per pixel instead of 12, no eager quantisation chain).  float_image=True also returns the
     float (3,H,W) image as "render" (else None).  Returns {"display_u8", "render", "radii", "visibility_filter"};
     depth_alpha=True adds "alpha" and "depth" (1,H,W) float32, from the same blend (the viewers' opacity / depth modes;
-    a normalised depth is depth / alpha)."""
-    return _forward_only(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, True, float_image, depth_alpha)
+    a normalised depth is depth / alpha).
+    quantize="viewer": `display_u8` holds the bytes the reference's local viewer exports instead,
+    (np.clip(render, 0, 1) * 255).astype(np.uint8) -- a float32 multiply and truncation, no +0.5 -- from the same blend
+    epilogue (not combinable with depth_alpha)."""
+    return _forward_only(viewpoint_camera, pc, pipe, bg_color, scaling_modifier, True, float_image, depth_alpha,
+                         quantize=quantize)
 
 
 def camera_table(cameras, device) -> torch.Tensor:

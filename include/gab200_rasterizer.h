@@ -93,6 +93,18 @@ typedef void* (*gab200_alloc_fn)(void* user, size_t bytes);
 
 /* Everything one frame's forward needs.  Replaces the argument list of
  * diff_gaussian_rasterization._C.rasterize_gaussians (SURVEY.md 3.3 / Appendix B.6). */
+/* How a display image (uint8 [H,W,3]) is quantised from the float pixel c of each channel.
+ *   GAB200_QUANTIZE_RENDER: render.py's  (uint8) clamp(c * 255 + 0.5, 0, 255), the multiply and the add rounded
+ *                           separately, truncation on the cast -- torch's mul(255).add_(0.5).clamp_(0, 255).to(uint8).
+ *   GAB200_QUANTIZE_VIEWER: the local viewer's export  (uint8) (clamp(c, 0, 1) * 255), one rounded float32 multiply and
+ *                           truncation, no +0.5 -- numpy's (np.clip(rgb, 0, 1) * 255).astype(np.uint8) on float32.
+ *                           A NaN channel gives 0.
+ * The mode is a compile-time parameter of the kernels: the RENDER kernels are unchanged by the VIEWER ones. */
+typedef enum gab200_display_quantize {
+  GAB200_QUANTIZE_RENDER = 0,
+  GAB200_QUANTIZE_VIEWER = 1
+} gab200_display_quantize;
+
 typedef struct gab200_forward_args {
   uint32_t abi_version;    /* = GAB200_ABI_VERSION */
   int32_t input_mode;      /* gab200_input_mode */
@@ -120,6 +132,10 @@ typedef struct gab200_forward_args {
   uint32_t depth_hint_hi;
   int32_t sync_mode;       /* gab200_sync_mode */
   uint32_t frame_seq;      /* any value; echoed in counters[GAB200_CTR_SEQ] */
+  int32_t display_quantize; /* gab200_display_quantize: how the display image (out_rgb8) is quantised.  It fills the
+                              alignment hole before counters_host, so the struct's size and offsets are those of
+                              earlier releases: zero-initialise the struct (a stale value other than 0 or 1 is
+                              refused) */
   uint32_t* counters_host; /* HOST pointer (pinned memory), GAB200_NUM_COUNTERS words, or NULL: where the frame counters
                               are copied.  Required for GAB200_SYNC_NONE; the other modes fall back to a slot the
                               library keeps per host thread. */
@@ -267,6 +283,9 @@ int32_t gab200_backward_device_fov(const gab200_backward_args* args, const float
  * separately and truncation on the cast, i.e. torch's mul(255).add_(0.5).clamp_(0, 255).permute(1, 2, 0).to(uint8)
  * of out_color, bit for bit.  It is written by the forward blend itself: 3 bytes per pixel instead of 12, no extra
  * pass, and a D2H copy of the frame is a quarter of the float image's.
+ * args->display_quantize = GAB200_QUANTIZE_VIEWER writes the local viewer's bytes instead (gab200_display_quantize);
+ * it is valid with need_backward == 0 only, and not with gab200_forward_depth_alpha / gab200_forward_views_depth_alpha
+ * (GAB200_ERR_INVALID_ARGUMENT).
  * args->out_color may be NULL only when out_rgb8 is not NULL and args->need_backward == 0 (the float image is then
  * not written at all); any other NULL output is GAB200_ERR_INVALID_ARGUMENT.  tanfov: as gab200_forward_device_fov
  * (NULL: args->tanfovx / tanfovy).  out_rgb8 == NULL: exactly gab200_forward_device_fov.  Every sync mode is
@@ -789,7 +808,8 @@ int32_t gab200_lpips(const gab200_lpips_args* args, void* stream);
  *   out_u8    [H,W,3] uint8 / out_float [3,H,W] float: the composite
  *               rgb * a * o + base * (a * (1 - o) + (1 - a))
  *             in torch's evaluation order, every op rounded (render.py's expression), out_u8 quantised as render.py
- *             does (mul(255).add_(0.5).clamp_(0, 255), truncation).  base: float [3,H,W] (GAB200_MESH_BASE_FLOAT_CHW)
+ *             does (mul(255).add_(0.5).clamp_(0, 255), truncation), or with quantize = GAB200_QUANTIZE_VIEWER as the
+ *             local viewer's export does (clip to [0, 1], * 255, truncation).  base: float [3,H,W] (GAB200_MESH_BASE_FLOAT_CHW)
  *             or uint8 [3,H,W] read as value/255 correctly rounded (GAB200_MESH_BASE_U8_CHW).  opacity: DEVICE
  *             float[2] = {o, 1 - o}, both rounded from the caller's double, as torch rounds its Python scalars;
  *             read when the kernel runs (a replayed graph picks up a new opacity)                  POS_WORLD
@@ -802,7 +822,7 @@ int32_t gab200_lpips(const gab200_lpips_args* args, void* stream);
  *   drawn and nothing is read out of bounds.
  * scratch: gab200_mesh_scratch_bytes(F, width, height) bytes of device memory, 256-byte aligned.
  * Invalid arguments (GAB200_ERR_INVALID_ARGUMENT): abi_version, V < 1, F < 1, width / height outside [1, 16384], a
- * NULL verts / faces / scratch, an unknown pos_kind / lighting / base_kind, POS_WORLD without camera, antialias
+ * NULL verts / faces / scratch, an unknown pos_kind / lighting / base_kind / quantize, POS_WORLD without camera, antialias
  * without adjacency, no output, out_rgba / out_u8 / out_float with POS_CLIP, out_u8 / out_float without base or
  * opacity, out_color without in_color or a channel count outside [1, 64]. */
 typedef enum gab200_mesh_pos_kind { GAB200_MESH_POS_WORLD = 0, GAB200_MESH_POS_CLIP = 1 } gab200_mesh_pos_kind;
@@ -835,6 +855,8 @@ typedef struct gab200_mesh_args {
   const float* in_color;       /* [H,W,channels] or NULL */
   float* out_color;            /* [H,W,channels] */
   int32_t channels;
+  int32_t quantize;            /* gab200_display_quantize of out_u8 (0: render.py's); fills the alignment hole before
+                                  error_flag, so the struct's size and offsets are unchanged */
   int32_t* error_flag;         /* DEVICE int32 or NULL */
   void* scratch;
 } gab200_mesh_args;
