@@ -48,17 +48,29 @@ def quat_to_R(q):
         2 * (x * z - r * y), 2 * (y * z + r * x), 1 - 2 * (x * x + y * y)], dim=1).reshape(-1, 3, 3)
 
 
-def render(means3D, means2D, opacities, viewmatrix, projmatrix, campos, W, H, tanfovx, tanfovy, bg, *, shs=None,
-           sh_degree=0, colors_precomp=None, scales=None, rotations=None, cov3D_precomp=None, scale_modifier=1.0,
-           radii=None, rect_xy=None, depths=None):
-    """All tensor arguments float64.  `radii` (int, from the fp32 oracle) fixes the discrete tile rectangles so the
-    comparison is not at the mercy of ceil() knife edges.  `rect_xy` ((P,2) float32 pixel centres, from the fp32
-    oracle) also takes the rectangles' centres from there, evaluated in float32 as the oracle does: a centre that
-    float32 puts exactly on a truncation edge (an integer pixel centre with (py + r + 15) / 16 integral, say) lands a
-    hair below it in float64 and would drop a whole tile row.  `depths` ((P,) float32 view-space depths, from the fp32
-    oracle) decides the blend order in place of this model's own depths rounded to float32: two splats a rounding
-    apart in depth composite in the oracle's order.  Returns (image (3,H,W), aux dict); aux also holds the discrete
-    decisions (`keep`, `alpha_clamped`, `colour_clamped`, `guard_clamped`) a caller can hold fixed."""
+# Wrong variants of the chain (`project(..., variant=...)`), each a mistake a per-splat backward could make; the
+# per-splat gradient gate of tests/test_oracle_preprocess.py must reject every one of them.
+VARIANTS = ("guard_grad", "no_dilation_bwd", "sh3_sign", "colour_clamp_ignored", "normalised_quat", "scale_grad_unmod")
+
+
+def _value_of(value, grad_path):
+    """`value` forward, the derivative of `grad_path` backward."""
+    return grad_path + (value - grad_path).detach()
+
+
+def project(means3D, viewmatrix, projmatrix, campos, W, H, tanfovx, tanfovy, *, shs=None, sh_degree=0,
+            colors_precomp=None, scales=None, rotations=None, cov3D_precomp=None, scale_modifier=1.0,
+            guard_clamped=None, colour_clamped=None, keep=None, conic_dropped=None, variant=None):
+    """The per-splat part of the forward in float64, differentiable: view-space t (P,3), ndc (P,2), pixel centre `pix`
+    (P,2), the dilated 2-D covariance `cov2d` (a, b, c) and its determinant, the conic (A, B, C) (P,3), the clamped
+    colour `rgb` (P,3) and the depth t.z (P,).
+
+    The float32 side's discrete decisions can be held fixed, as render() does with the tile rectangles:
+    `guard_clamped` ((P,2) bool: the guard band clamped t.x / t.y), `colour_clamped` ((P,3) bool: the channel's SH
+    sum was below 0) and `keep` ((P,) bool: the splat is rendered; every output of another splat is detached).  Left
+    None, each is this model's own.  `conic_dropped` ((P,) bool): the float32 backward's 1 / (det^2 + 1e-7) rounded
+    to 0 (det^2 overflows), so no gradient leaves through the conic of those splats (the reference module's guard).
+    `variant`: one of VARIANTS (a deliberately wrong backward), or None."""
     dt = torch.float64
     P = means3D.shape[0]
     V = viewmatrix.reshape(16).to(dt)
@@ -73,24 +85,33 @@ def render(means3D, means2D, opacities, viewmatrix, projmatrix, campos, W, H, ta
     hw = Pm[3] * x + Pm[7] * y + Pm[11] * z + Pm[15]
     p_w = 1.0 / (hw + 0.0000001)
     ndc_x, ndc_y = hx * p_w, hy * p_w
-    in_front = tz > 0.2
 
     if cov3D_precomp is not None:
         c3 = cov3D_precomp
         Sigma = torch.stack([c3[:, 0], c3[:, 1], c3[:, 2], c3[:, 1], c3[:, 3], c3[:, 4], c3[:, 2], c3[:, 4], c3[:, 5]],
                             dim=1).reshape(P, 3, 3)
     else:
-        R = quat_to_R(rotations)
+        q = rotations
+        if variant == "normalised_quat":
+            q = q / q.norm(dim=1, keepdim=True)
+        R = quat_to_R(q)
         # gradient w.r.t. s=mod*scale reported as dL/dscale: value mod*scale, derivative 1
-        s = scales + ((scale_modifier - 1.0) * scales).detach()
+        s = scales * scale_modifier if variant == "scale_grad_unmod" else scales + ((scale_modifier - 1.0) * scales).detach()
         Sigma = R @ torch.diag_embed(s * s) @ R.transpose(1, 2)
 
     limx, limy = 1.3 * tanfovx, 1.3 * tanfovy
     txtz, tytz = tx / tz, ty / tz
-    cx = (txtz < -limx) | (txtz > limx)
-    cy = (tytz < -limy) | (tytz > limy)
-    txc = torch.where(cx, (txtz.clamp(-limx, limx) * tz).detach(), tx)
-    tyc = torch.where(cy, (tytz.clamp(-limy, limy) * tz).detach(), ty)
+    if guard_clamped is None:
+        cx = (txtz < -limx) | (txtz > limx)
+        cy = (tytz < -limy) | (tytz > limy)
+    else:
+        cx, cy = guard_clamped[:, 0], guard_clamped[:, 1]
+    if variant == "guard_grad":   # the clamped value, but d/dt.x as if unclamped
+        txc = torch.where(cx, _value_of(txtz.clamp(-limx, limx) * tz, tx), tx)
+        tyc = torch.where(cy, _value_of(tytz.clamp(-limy, limy) * tz, ty), ty)
+    else:
+        txc = torch.where(cx, (txtz.clamp(-limx, limx) * tz).detach(), tx)
+        tyc = torch.where(cy, (tytz.clamp(-limy, limy) * tz).detach(), ty)
     zero = torch.zeros_like(tz)
     J = torch.stack([fx / tz, zero, -(fx * txc) / (tz * tz), zero, fy / tz, -(fy * tyc) / (tz * tz)], dim=1).reshape(P, 2, 3)
     Wv = torch.stack([V[0], V[4], V[8], V[1], V[5], V[9], V[2], V[6], V[10]]).reshape(3, 3)
@@ -100,21 +121,65 @@ def render(means3D, means2D, opacities, viewmatrix, projmatrix, campos, W, H, ta
     det = a * c - b * b
     # conic with the 1/(det^2+1e-7)-style guard irrelevant at fp64 tolerance
     conA, conB, conC = c / det, -b / det, a / det
+    if variant == "no_dilation_bwd":   # the conic's derivatives taken at the undilated covariance
+        a0, c0 = cov[:, 0, 0], cov[:, 1, 1]
+        det0 = a0 * c0 - b * b
+        conA, conB, conC = _value_of(conA, c0 / det0), _value_of(conB, -b / det0), _value_of(conC, a0 / det0)
 
-    px = ((ndc_x + 1.0) * W - 1.0) * 0.5 + means2D[:, 0] * (0.5 * W)
-    py = ((ndc_y + 1.0) * H - 1.0) * 0.5 + means2D[:, 1] * (0.5 * H)
+    if conic_dropped is not None:
+        conA, conB, conC = (torch.where(conic_dropped, v.detach(), v) for v in (conA, conB, conC))
 
     if colors_precomp is not None:
         rgb = colors_precomp
-        colour_clamped = torch.zeros_like(rgb, dtype=torch.bool)
+        if colour_clamped is None:
+            colour_clamped = torch.zeros_like(rgb, dtype=torch.bool)
     else:
         d = means3D - campos.reshape(1, 3)
         d = d / d.norm(dim=1, keepdim=True)
         B = sh_basis(sh_degree, d)
+        if variant == "sh3_sign" and sh_degree > 2:
+            B = torch.cat((B[:, :12], -B[:, 12:13], B[:, 13:]), dim=1)
         nb = B.shape[1]
         rgb = (B[:, :, None] * shs[:, :nb, :]).sum(dim=1) + 0.5
-        colour_clamped = rgb.detach() < 0
-        rgb = torch.clamp_min(rgb, 0.0)
+        if colour_clamped is None:
+            colour_clamped = rgb.detach() < 0
+        if variant == "colour_clamp_ignored":
+            rgb = _value_of(torch.clamp_min(rgb, 0.0), rgb)
+        else:
+            rgb = torch.where(colour_clamped, torch.zeros_like(rgb), rgb)
+
+    out = dict(t=torch.stack((tx, ty, tz), 1), ndc=torch.stack((ndc_x, ndc_y), 1),
+               pix=torch.stack((((ndc_x + 1.0) * W - 1.0) * 0.5, ((ndc_y + 1.0) * H - 1.0) * 0.5), 1),
+               cov2d=torch.stack((a, b, c), 1), det=det, conic=torch.stack((conA, conB, conC), 1), rgb=rgb, depth=tz)
+    if keep is not None:
+        out = {k: torch.where(keep.reshape((-1,) + (1,) * (v.ndim - 1)), v, v.detach()) for k, v in out.items()}
+    out.update(guard_clamped=torch.stack((cx, cy), dim=1), colour_clamped=colour_clamped)
+    return out
+
+
+def render(means3D, means2D, opacities, viewmatrix, projmatrix, campos, W, H, tanfovx, tanfovy, bg, *, shs=None,
+           sh_degree=0, colors_precomp=None, scales=None, rotations=None, cov3D_precomp=None, scale_modifier=1.0,
+           radii=None, rect_xy=None, depths=None):
+    """All tensor arguments float64.  `radii` (int, from the fp32 oracle) fixes the discrete tile rectangles so the
+    comparison is not at the mercy of ceil() knife edges.  `rect_xy` ((P,2) float32 pixel centres, from the fp32
+    oracle) also takes the rectangles' centres from there, evaluated in float32 as the oracle does: a centre that
+    float32 puts exactly on a truncation edge (an integer pixel centre with (py + r + 15) / 16 integral, say) lands a
+    hair below it in float64 and would drop a whole tile row.  `depths` ((P,) float32 view-space depths, from the fp32
+    oracle) decides the blend order in place of this model's own depths rounded to float32: two splats a rounding
+    apart in depth composite in the oracle's order.  Returns (image (3,H,W), aux dict); aux also holds the discrete
+    decisions (`keep`, `alpha_clamped`, `colour_clamped`, `guard_clamped`) a caller can hold fixed."""
+    dt = torch.float64
+    pr = project(means3D, viewmatrix, projmatrix, campos, W, H, tanfovx, tanfovy, shs=shs, sh_degree=sh_degree,
+                 colors_precomp=colors_precomp, scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp,
+                 scale_modifier=scale_modifier)
+    tz = pr["depth"]
+    in_front = tz > 0.2
+    a, c, det = pr["cov2d"][:, 0], pr["cov2d"][:, 2], pr["det"]
+    conA, conB, conC = pr["conic"].unbind(1)
+    px = pr["pix"][:, 0] + means2D[:, 0] * (0.5 * W)
+    py = pr["pix"][:, 1] + means2D[:, 1] * (0.5 * H)
+    rgb, colour_clamped = pr["rgb"], pr["colour_clamped"]
+    cx, cy = pr["guard_clamped"].unbind(1)
 
     # discrete tile rectangles
     gx, gy = (W + 15) // 16, (H + 15) // 16

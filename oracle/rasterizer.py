@@ -157,20 +157,41 @@ def backward(st: OracleState, dL_dpix, means3D, viewmatrix, projmatrix, campos, 
     lib.oracle_blend_backward(C.c_int(P), C.c_int(W), C.c_int(H), _p(st.ranges), _p(vs), _p(st.xy),
                               _p(st.conic_opacity), _p(st.rgb), _p(bg), _p(st.final_T), _p(st.n_contrib),
                               _p(dL_dpix), _p(g_mean2D), _p(g_conic), _p(g_opac), _p(g_color))
+    g = preprocess_backward(st, g_mean2D, g_conic, g_color, means3D, viewmatrix, projmatrix, campos, tanfovx, tanfovy,
+                            shs=shs, sh_degree=sh_degree, scales=scales, rotations=rotations,
+                            scale_modifier=scale_modifier)
+    g_means2D = np.zeros((P, 3), np.float32)
+    g_means2D[:, :2] = g_mean2D
+    return dict(g, means2D=g_means2D, colors_precomp=g_color, opacities=g_opac, conic=g_conic)
+
+
+def preprocess_backward(st: OracleState, dL_dmean2D, dL_dconic, dL_dcolor, means3D, viewmatrix, projmatrix, campos,
+                        tanfovx, tanfovy, *, shs=None, sh_degree=0, scales=None, rotations=None, scale_modifier=1.0,
+                        radii=None, clamped=None):
+    """Stage 5 alone: the per-splat upstream dL/dmean2D (P,2, NDC units), dL/dconic (P,3, the off-diagonal entry
+    stored once) and dL/dcolor (P,3) -> dict of means3D, cov3D_precomp, shs, scales and rotations gradients (numpy
+    float32; None where the input is absent).  `radii` / `clamped` replace the state's visibility and colour clamp
+    bits (another forward's decisions)."""
+    lib = load()
+    P, W, H = st.P, st.W, st.H
+    means3D = _f32(means3D)
+    shs, scales, rotations = _f32(shs), _f32(scales), _f32(rotations)
+    V, Pm, cam = _f32(viewmatrix).reshape(16), _f32(projmatrix).reshape(16), _f32(campos).reshape(3)
+    radii = st.radii if radii is None else np.ascontiguousarray(radii, np.int32)
+    clamped = st.clamped if clamped is None else np.ascontiguousarray(clamped, np.uint8)
+    g_mean2D, g_conic, g_color = _f32(dL_dmean2D), _f32(dL_dconic), _f32(dL_dcolor)
+    M = 0 if shs is None else shs.shape[1]
     g_means3D = np.zeros((P, 3), np.float32)
     g_cov3D = np.zeros((P, 6), np.float32)
     g_sh = np.zeros((P, M, 3), np.float32) if shs is not None else None
     g_scales = np.zeros((P, 3), np.float32) if scales is not None else None
     g_rots = np.zeros((P, 4), np.float32) if scales is not None else None
-    lib.oracle_preprocess_backward(C.c_int(P), C.c_int(sh_degree), C.c_int(M), _p(means3D), _p(st.radii), _p(shs),
-                                   _p(st.clamped), _p(scales), _p(rotations), C.c_float(scale_modifier),
+    lib.oracle_preprocess_backward(C.c_int(P), C.c_int(sh_degree), C.c_int(M), _p(means3D), _p(radii), _p(shs),
+                                   _p(clamped), _p(scales), _p(rotations), C.c_float(scale_modifier),
                                    _p(st.cov3D), _p(V), _p(Pm), _p(cam), C.c_int(W), C.c_int(H), C.c_float(tanfovx),
                                    C.c_float(tanfovy), _p(g_mean2D), _p(g_conic), _p(g_color), _p(g_means3D),
                                    _p(g_cov3D), _p(g_sh), _p(g_scales), _p(g_rots))
-    g_means2D = np.zeros((P, 3), np.float32)
-    g_means2D[:, :2] = g_mean2D
-    return dict(means3D=g_means3D, means2D=g_means2D, shs=g_sh, colors_precomp=g_color, opacities=g_opac,
-                scales=g_scales, rotations=g_rots, cov3D_precomp=g_cov3D, conic=g_conic)
+    return dict(means3D=g_means3D, shs=g_sh, scales=g_scales, rotations=g_rots, cov3D_precomp=g_cov3D)
 
 
 def mark_visible(means3D, viewmatrix):

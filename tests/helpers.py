@@ -142,6 +142,21 @@ def image_stats(img_cuda: np.ndarray, img_ref: np.ndarray):
     return dict(max_abs=float(d.max()), n_over_1e4=int((d > IMG_TOL).sum()), n=int(d.size))
 
 
+def carve(sizes):
+    """Byte offsets of consecutive Carver::take calls (256-B aligned), as csrc/common.cuh lays the buffers out."""
+    off, out = 0, []
+    for s in sizes:
+        off = (off + 255) & ~255
+        out.append(off)
+        off += s
+    return out
+
+
+def buffer(holder, ptr):
+    """The tensor of a frame's scratch holder that starts at device address `ptr`."""
+    return next(t for t in holder if t.data_ptr() == ptr)
+
+
 def random_scene(P=10_000, W=256, H=256, sh_degree=0, seed=0, fov=60.0, scale_shift=0.0, max_sh_degree=None):
     """Config-1 style scene: activated (reference-surface) inputs as CPU float32 tensors."""
     sp = syn.random_splats(P, seed=seed, sh_degree=sh_degree, max_sh_degree=max_sh_degree)

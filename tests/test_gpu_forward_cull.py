@@ -34,20 +34,6 @@ ALPHA_MIN = float(F32(1.0) / F32(255.0))
 LOG2E = F32(1.4426950408889634)
 
 
-def _carve(sizes):
-    """Byte offsets of consecutive Carver::take calls (256-B aligned), as csrc/common.cuh lays the buffers out."""
-    off, out = 0, []
-    for s in sizes:
-        off = (off + 255) & ~255
-        out.append(off)
-        off += s
-    return out
-
-
-def _buffer(holder, ptr):
-    return next(t for t in holder if t.data_ptr() == ptr)
-
-
 def _read_frame(P, W, H):
     """The last forward's records, sorted ids, ranges, block masks, final_T and n_contrib (needs a training forward:
     keep_last_state(True) and inputs that require grad)."""
@@ -58,13 +44,13 @@ def _read_frame(P, W, H):
     assert holder is not None, "the frame was not a training forward"
     gx, gy = (W + 15) // 16, (H + 15) // 16
     tiles = gx * gy
-    geom = _buffer(holder, st.geom_buffer)
+    geom = h.buffer(holder, st.geom_buffer)
     rec = geom[: P * 48].view(torch.float32).reshape(P, 12).cpu().numpy()
     nb = max(int(st.binning_capacity), 1) + 320
-    off = _carve([4 * nb] * 4 + [nb])[4]
-    strip = _buffer(holder, st.binning_buffer)[off: off + n].cpu().numpy()
-    offs = _carve([(tiles + 1) * 8, tiles * 4, 16, tiles * 4, tiles * 4, W * H * 4, W * H * 4])
-    img = _buffer(holder, st.image_buffer)
+    off = h.carve([4 * nb] * 4 + [nb])[4]
+    strip = h.buffer(holder, st.binning_buffer)[off: off + n].cpu().numpy()
+    offs = h.carve([(tiles + 1) * 8, tiles * 4, 16, tiles * 4, tiles * 4, W * H * 4, W * H * 4])
+    img = h.buffer(holder, st.image_buffer)
     final_T = img[offs[5]: offs[5] + 4 * W * H].view(torch.float32).reshape(H, W).cpu().numpy()
     n_contrib = img[offs[6]: offs[6] + 4 * W * H].view(torch.int32).reshape(H, W).cpu().numpy()
     return dict(rec=rec, vals=vals.cpu().numpy().view(np.uint32), ranges=ranges.cpu().numpy().view(np.uint32),
