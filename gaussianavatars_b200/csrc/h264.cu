@@ -1,22 +1,29 @@
 // h264.cu -- H.264 video frames encoded on the device (gab200_h264_bound / gab200_h264_scratch_bytes /
 // gab200_h264_encode / gab200_h264_parameter_sets, and for streams with P pictures gab200_h264_p_bound /
-// gab200_h264_state_bytes / gab200_h264_encode_stream / gab200_h264_stream_parameter_sets): Constrained Baseline,
-// CAVLC, deblocking off, one fixed QP.  An IDR picture's macroblocks are I_16x16 (luma and chroma modes of least SATD)
-// or I_PCM; a P picture's are P_Skip, P_L0_16x16 (one quarter-sample vector), I_16x16 or I_PCM.  oracle/h264.py and
-// tests/h264_stream_oracle.py restate every step, and the tests compare their bytes with these.
+// gab200_h264_state_bytes / gab200_h264_encode_stream / gab200_h264_stream_parameter_sets, and for deblocked streams
+// gab200_h264_deblocked_scratch_bytes / gab200_h264_encode_deblocked): Constrained Baseline, CAVLC, one fixed QP,
+// deblocking off (disable_deblocking_filter_idc 1) unless the stream is deblocked (idc 0, offsets 0).  An IDR
+// picture's macroblocks are I_16x16 (luma and chroma modes of least SATD) or I_PCM; a P picture's are P_Skip,
+// P_L0_16x16 (one quarter-sample vector), I_16x16 or I_PCM.  oracle/h264.py, tests/h264_stream_oracle.py and
+// tests/h264_deblock_oracle.py restate every step, and the tests compare their bytes with these.
 //
 // Per batch of frames the encode runs these kernels, each named for a trace:
 //   h264_convert_kernel  RGB -> BT.601 limited-range Y, Cb, Cr planes padded to whole macroblocks by edge replication.
 //   h264_frame_kernel    each frame's picture type and frame_num from the stream position in the state.
 //   h264_mb_kernel       one launch per step of a wavefront over (frame, anti-diagonal d = mbx + mby): frame f runs
 //                        diagonal step - lag f, lag 0 when every frame is an IDR picture (W/16 + H/16 - 1 launches)
-//                        and LAG when a frame refers to the one before (LAG more launches per frame).  One 128-thread
+//                        and LAG when a frame refers to the one before (LAG more launches per frame); a deblocked P
+//                        stream runs lines d = mbx + 2 mby instead, lag LAG_DB (see LAG_DB).  One 128-thread
 //                        CTA per (macroblock on d, frame): in a P picture the motion search in the previous picture;
 //                        prediction from the reconstructed left / top / top-left samples of earlier diagonals, mode
 //                        decision by SATD, transform, quantisation, reconstruction into the recon planes, per-4x4
 //                        TotalCoeff, the macroblock's CAVLC bit count and the I_PCM fallback; the levels are kept for
 //                        the writer.  The launch boundary is the wavefront's only synchronisation: no CTA ever waits
 //                        on another.
+//   h264_deblock_kernel  deblocked streams, launched after h264_mb_kernel in each step: one warp per macroblock on
+//                        line mbx + 2 mby = step - lag f - DB_LAG of frame f; bS from the macroblocks' info, TotalCoeff
+//                        and vectors, then the filter (8.7) of its edges from the unfiltered recon planes into the
+//                        filtered planes flt, which P pictures refer to (W/16 + 2 H/16 - 2 steps per frame).
 //   h264_mvp_kernel      P pictures, one thread per macroblock: the vector predictors, P_Skip and the mvd bits.
 //   h264_run_kernel      P pictures, one thread per macroblock: the skip runs and their bits.
 //   h264_scan_kernel     one CTA per frame: the macroblocks' bit offsets in raster order, an exclusive scan of the maps
@@ -30,7 +37,8 @@
 //   h264_ep_plan_kernel  one warp per frame: the pieces' start states and output offsets in order, the sample's length
 //                        and its 4-byte length prefix and NAL header.
 //   h264_ep_emit_kernel  one thread per piece: its bytes, with 0x03 inserted, into the frame's output slot.
-//   h264_state_kernel    the last frame's reconstruction and the advanced position into the stream's state.
+//   h264_state_kernel    the last frame's reconstruction (filtered when the stream is deblocked) and the advanced
+//                        position into the stream's state.
 #include <algorithm>
 #include <climits>
 #include <vector>
@@ -63,6 +71,17 @@ constexpr int REACH_MB = (REACH + 15) / 16;
 constexpr int LAG = 2 * REACH_MB + 1;
 static_assert(LAG == 5, "the stream's frame lag");
 static_assert(16 * REACH_MB >= REACH, "the reference window stays within REACH_MB macroblocks");
+// The deblocked stream.  Filtering macroblock (x, y) changes up to 3 samples into (x - 1, y) and (x, y - 1), which
+// (x + 1, y - 1)'s left edge changed before it, so the filter runs on lines x + 2 y: line t is filtered in the launch
+// after the encode's own launch of the step where the encode has finished every macroblock of line t, DB_LAG steps
+// behind the frame's encode line (the encode of a P stream runs on the same lines x + 2 y; an IDR-only stream keeps
+// its anti-diagonals, and x + y <= x + 2 y).  Macroblock (x, y)'s filtered samples are final once (x + 1, y) and
+// (x, y + 1) are filtered, line x + 2 y + 2.  Frame f + 1's window at (x, y) reaches the filtered macroblocks up to
+// (x + REACH_MB, y + REACH_MB), final after line x + 2 y + 3 REACH_MB + 2 of frame f: that line must be filtered in an
+// earlier step, LAG_DB > 3 REACH_MB + 2 + DB_LAG.
+constexpr int DB_LAG = 0;
+constexpr int LAG_DB = 3 * REACH_MB + 3 + DB_LAG;
+static_assert(DB_LAG == 0 && LAG_DB == 9, "the deblocked stream's filter and frame lags");
 
 __constant__ int8_t c_zigzag[16] = {0, 1, 4, 8, 5, 2, 3, 6, 9, 12, 13, 10, 7, 11, 14, 15};
 __constant__ int8_t c_chroma_qp[52] = {0,  1,  2,  3,  4,  5,  6,  7,  8,  9,  10, 11, 12, 13, 14, 15, 16, 17,
@@ -135,8 +154,9 @@ __constant__ uint8_t c_rb_code[7][15] = {{1, 0},          {1, 1, 0},          {3
 
 // The per-frame scratch: offsets from the frame's base (each 256-byte aligned), and the frame stride.
 struct Layout {
-  int W, H, wm, hm, nmb, pieces;
-  int64_t src, rec, tot, lev, info, bits, off, mv, mvd, run, raw, ep, meta, stride;
+  int W, H, wm, hm, nmb, pieces, deblock;
+  // flt: the picture a P picture refers to and the state keeps -- the deblocked copy of rec, or rec itself
+  int64_t src, rec, tot, lev, info, bits, off, mv, mvd, run, raw, ep, meta, flt, stride;
 };
 
 int64_t align256(int64_t x) { return (x + 255) / 256 * 256; }
@@ -147,8 +167,9 @@ int64_t raw_bytes_bound_p(int nmb) {
   return (P_HEADER_BITS + (int64_t)nmb * (3 + MVD_BITS + PCM_BITS + 7) + 1 + 7) / 8;
 }
 
-Layout layout(int H, int W) {
+Layout layout(int H, int W, bool deblock = false) {
   Layout l;
+  l.deblock = deblock;
   l.W = W;
   l.H = H;
   l.wm = (W + 15) / 16;
@@ -171,6 +192,8 @@ Layout layout(int H, int W) {
   l.raw = o;  o = align256(o + (raw + 7) / 4 * 4 + 4);                // the slice's words, one spare
   l.ep = o;   o = align256(o + (int64_t)l.pieces * 16);               // per piece: 3 counts + end states | start state
   l.meta = o; o = align256(o + 16);                                   // raw byte count, P picture, frame_num
+  l.flt = l.rec;
+  if (deblock) { l.flt = o; o = align256(o + plane); }                 // the deblocked picture
   l.stride = o;
   return l;
 }
@@ -549,16 +572,28 @@ __device__ __forceinline__ const int* frame_meta(const uint8_t* scratch, const L
   return reinterpret_cast<const int*>(scratch + (int64_t)f * l.stride + l.meta);
 }
 
-// One launch per step of the wavefront over (frame, anti-diagonal): frame f runs diagonal step - lag f (lag 0 when
-// every frame is an IDR picture; LAG when a frame refers to the one before it).
-__global__ void __maxnreg__(80) h264_mb_kernel(int step, int lag, int f_lo, int qp, uint8_t* scratch,
+// The macroblocks of wavefront line d: mbx + mby = d (slope 1) or mbx + 2 mby = d (slope 2); the k-th of them.
+__device__ __forceinline__ bool line_mb(int d, int slope, int k, int wm, int hm, int& mx, int& my) {
+  if (slope == 1) {
+    if (d < 0 || d >= wm + hm - 1) return false;
+    mx = max(0, d - hm + 1) + k;
+    my = d - mx;
+    return mx <= min(d, wm - 1);
+  }
+  if (d < 0 || d >= wm + 2 * hm - 2) return false;
+  my = max(0, (d - wm + 2) / 2) + k;
+  mx = d - 2 * my;
+  return my <= min(d / 2, hm - 1);
+}
+
+// One launch per step of the wavefront over (frame, line): frame f runs line step - lag f (lag 0 when every frame is
+// an IDR picture; LAG when a frame refers to the one before it, LAG_DB when it refers to the deblocked one).
+__global__ void __maxnreg__(80) h264_mb_kernel(int step, int lag, int slope, int f_lo, int qp, uint8_t* scratch,
                                                       const uint8_t* state, Layout l) {
   __shared__ MbShared s;
   const int f = f_lo + blockIdx.y, t = threadIdx.x;
-  const int d = step - lag * f;
-  if (d < 0 || d >= l.wm + l.hm - 1) return;
-  const int mx = max(0, d - l.hm + 1) + blockIdx.x, my = d - mx;
-  if (mx > min(d, l.wm - 1)) return;
+  int mx, my;
+  if (!line_mb(step - lag * f, slope, blockIdx.x, l.wm, l.hm, mx, my)) return;
   const int mb = my * l.wm + mx;
   const bool has_l = mx > 0, has_t = my > 0;
   uint8_t* base = scratch + (int64_t)f * l.stride;
@@ -590,8 +625,8 @@ __global__ void __maxnreg__(80) h264_mb_kernel(int step, int lag, int f_lo, int 
   if (t < 8) s.cost[t] = 0;
   if (t == 0) { s.maxlev = 0; s.bits = 0; s.inter = 0; }
   __syncthreads();
-  if (is_p) {   // the reference: the previous frame of the batch, or the stream state's picture
-    const Planes ref(f > 0 ? scratch + (int64_t)(f - 1) * l.stride + l.rec : const_cast<uint8_t*>(state) + 256, l);
+  if (is_p) {   // the reference: the previous frame of the batch (deblocked when the stream is), or the state's
+    const Planes ref(f > 0 ? scratch + (int64_t)(f - 1) * l.stride + l.flt : const_cast<uint8_t*>(state) + 256, l);
     motion_search(s, ref, l, mx, my, qp);
   }
 
@@ -835,6 +870,155 @@ __global__ void __maxnreg__(80) h264_mb_kernel(int step, int lag, int f_lo, int 
   }
 }
 
+// ---- the deblocking filter (8.7) ---------------------------------------------------------------------------------
+// Tables 8-16 (alpha', beta') and 8-17 (tC0 at bS 1, 2, 3), indexed by indexA = indexB = qPav (offsets 0).
+__constant__ uint8_t c_alpha[52] = {0,  0,  0,  0,  0,  0,  0,  0,  0,  0,  0,   0,   0,   0,   0,   0,   4,   4,
+                                    5,  6,  7,  8,  9,  10, 12, 13, 15, 17, 20,  22,  25,  28,  32,  36,  40,  45,
+                                    50, 56, 63, 71, 80, 90, 101, 113, 127, 144, 162, 182, 203, 226, 255, 255};
+__constant__ uint8_t c_beta[52] = {0, 0, 0, 0, 0, 0, 0, 0, 0,  0,  0,  0,  0,  0,  0,  0,  2,  2,  2,  3,  3,  3,  3,  4,  4,  4,
+                                   6, 6, 7, 7, 8, 8, 9, 9, 10, 10, 11, 11, 12, 12, 13, 13, 14, 14, 15, 15, 16, 16, 17, 17, 18, 18};
+__constant__ uint8_t c_tc0[52][3] = {
+    {0, 0, 0}, {0, 0, 0}, {0, 0, 0},   {0, 0, 0},   {0, 0, 0},    {0, 0, 0},    {0, 0, 0},    {0, 0, 0},
+    {0, 0, 0}, {0, 0, 0}, {0, 0, 0},   {0, 0, 0},   {0, 0, 0},    {0, 0, 0},    {0, 0, 0},    {0, 0, 0},
+    {0, 0, 0}, {0, 0, 1}, {0, 0, 1},   {0, 0, 1},   {0, 0, 1},    {0, 1, 1},    {0, 1, 1},    {1, 1, 1},
+    {1, 1, 1}, {1, 1, 1}, {1, 1, 1},   {1, 1, 2},   {1, 1, 2},    {1, 1, 2},    {1, 1, 2},    {1, 2, 3},
+    {1, 2, 3}, {2, 2, 3}, {2, 2, 4},   {2, 3, 4},   {2, 3, 4},    {3, 3, 5},    {3, 4, 6},    {3, 4, 6},
+    {4, 5, 7}, {4, 5, 8}, {4, 6, 9},   {5, 7, 10},  {6, 8, 11},   {6, 8, 13},   {7, 10, 14},  {8, 11, 16},
+    {9, 12, 18}, {10, 13, 20}, {11, 15, 23}, {13, 17, 25}};
+
+// One line of samples across an edge: q points at q0, p_i = q[-(i + 1) step], q_i = q[i step] (8.7.2.3, 8.7.2.4).
+__device__ __forceinline__ void filter_line(uint8_t* q, int step, bool chroma, int bS, int qpav) {
+  const int alpha = c_alpha[qpav], beta = c_beta[qpav];
+  const int p0 = q[-step], p1 = q[-2 * step], q0 = q[0], q1 = q[step];
+  if (!(abs(p0 - q0) < alpha && abs(p1 - p0) < beta && abs(q1 - q0) < beta)) return;
+  if (chroma) {
+    if (bS < 4) {
+      const int tc = c_tc0[qpav][bS - 1] + 1;
+      const int delta = min(max((((q0 - p0) << 2) + (p1 - q1) + 4) >> 3, -tc), tc);
+      q[-step] = (uint8_t)clip255(p0 + delta);
+      q[0] = (uint8_t)clip255(q0 - delta);
+    } else {
+      q[-step] = (uint8_t)((2 * p1 + p0 + q1 + 2) >> 2);
+      q[0] = (uint8_t)((2 * q1 + q0 + p1 + 2) >> 2);
+    }
+    return;
+  }
+  const int p2 = q[-3 * step], q2 = q[2 * step];
+  const bool ap = abs(p2 - p0) < beta, aq = abs(q2 - q0) < beta;
+  if (bS < 4) {
+    const int tc0 = c_tc0[qpav][bS - 1], tc = tc0 + ap + aq;
+    const int delta = min(max((((q0 - p0) << 2) + (p1 - q1) + 4) >> 3, -tc), tc);
+    q[-step] = (uint8_t)clip255(p0 + delta);
+    q[0] = (uint8_t)clip255(q0 - delta);
+    if (ap) q[-2 * step] = (uint8_t)(p1 + min(max((p2 + ((p0 + q0 + 1) >> 1) - (p1 << 1)) >> 1, -tc0), tc0));
+    if (aq) q[step] = (uint8_t)(q1 + min(max((q2 + ((p0 + q0 + 1) >> 1) - (q1 << 1)) >> 1, -tc0), tc0));
+    return;
+  }
+  const bool strong = abs(p0 - q0) < ((alpha >> 2) + 2);
+  if (ap && strong) {
+    const int p3 = q[-4 * step];
+    q[-step] = (uint8_t)((p2 + 2 * p1 + 2 * p0 + 2 * q0 + q1 + 4) >> 3);
+    q[-2 * step] = (uint8_t)((p2 + p1 + p0 + q0 + 2) >> 2);
+    q[-3 * step] = (uint8_t)((2 * p3 + 3 * p2 + p1 + p0 + q0 + 4) >> 3);
+  } else {
+    q[-step] = (uint8_t)((2 * p1 + p0 + q1 + 2) >> 2);
+  }
+  if (aq && strong) {
+    const int q3 = q[3 * step];
+    q[0] = (uint8_t)((p1 + 2 * p0 + 2 * q0 + 2 * q1 + q2 + 4) >> 3);
+    q[step] = (uint8_t)((p0 + q0 + q1 + q2 + 2) >> 2);
+    q[2 * step] = (uint8_t)((2 * q3 + 3 * q2 + q1 + q0 + p0 + 4) >> 3);
+  } else {
+    q[0] = (uint8_t)((2 * q1 + q0 + p1 + 2) >> 2);
+  }
+}
+
+// One warp per macroblock (x, y) on line x + 2 y = step - lag f - DB_LAG of frame f: the macroblock's samples from
+// rec (no filtering has reached them yet), the 4 columns left of it and the 4 rows above it from flt (their
+// macroblocks' filtering is done); bS of every 4-sample edge segment, then the vertical edges left to right (one lane
+// per row: 16 luma, 8 Cb, 8 Cr), then the horizontal edges top to bottom (one lane per column); the samples the
+// filter may have changed go back to flt.
+__global__ void __launch_bounds__(32) h264_deblock_kernel(int step, int lag, int f_lo, int qp, uint8_t* scratch,
+                                                          Layout l) {
+  __shared__ uint8_t sy[20][20];        // luma rows and columns -4 .. 15
+  __shared__ uint8_t sc[2][10][10];     // chroma rows and columns -2 .. 7
+  __shared__ uint8_t sbs[2][4][4];      // [vertical, horizontal][edge][segment]
+  const int f = f_lo + blockIdx.y, t = threadIdx.x;
+  int mx, my;
+  if (!line_mb(step - lag * f - DB_LAG, 2, blockIdx.x, l.wm, l.hm, mx, my)) return;
+  uint8_t* base = scratch + (int64_t)f * l.stride;
+  const uint8_t* rec = base + l.rec;
+  uint8_t* flt = base + l.flt;
+  const int ys = 16 * l.wm, cs = 8 * l.wm;
+  const int64_t c0 = (int64_t)ys * 16 * l.hm, cpl = (int64_t)cs * 8 * l.hm;   // Cb's offset, a chroma plane's bytes
+  const bool has_l = mx > 0, has_t = my > 0;
+  for (int i = t; i < 400; i += 32) {
+    const int r = i / 20 - 4, c = i % 20 - 4;
+    if ((r < 0 && (c < 0 || !has_t)) || (c < 0 && !has_l)) continue;
+    sy[r + 4][c + 4] = (r < 0 || c < 0 ? flt : rec)[(int64_t)(16 * my + r) * ys + 16 * mx + c];
+  }
+  for (int i = t; i < 200; i += 32) {
+    const int p = i / 100, r = i % 100 / 10 - 2, c = i % 10 - 2;
+    if ((r < 0 && (c < 0 || !has_t)) || (c < 0 && !has_l)) continue;
+    sc[p][r + 2][c + 2] = (r < 0 || c < 0 ? flt : rec)[c0 + p * cpl + (int64_t)(8 * my + r) * cs + 8 * mx + c];
+  }
+  // bS (8.7.2.1): one lane per (direction, edge, segment)
+  const int* info = reinterpret_cast<const int*>(base + l.info);
+  const int* mv = reinterpret_cast<const int*>(base + l.mv);
+  const uint8_t* tot = base + l.tot;
+  const int mb = my * l.wm + mx, mb_l = mb - 1, mb_t = mb - l.wm;
+  {
+    const int dir = t >> 4, e = (t >> 2) & 3, seg = t & 3;
+    const int qbx = dir ? seg : e, qby = dir ? e : seg;
+    const int nb = e ? mb : dir ? mb_t : mb_l;
+    const int pbx = dir ? seg : (e ? e - 1 : 3), pby = dir ? (e ? e - 1 : 3) : seg;
+    int bS = 0;
+    if (e || (dir ? has_t : has_l)) {
+      const bool intra = !((info[mb] >> 8) & 1) || !((info[nb] >> 8) & 1);
+      if (intra) bS = e ? 3 : 4;
+      else if (tot[(int64_t)mb * 24 + qby * 4 + qbx] || tot[(int64_t)nb * 24 + pby * 4 + pbx]) bS = 2;
+      else {
+        const int a = mv[mb], b = mv[nb];
+        bS = abs((int16_t)(a & 0xffff) - (int16_t)(b & 0xffff)) >= 4 || abs((a >> 16) - (b >> 16)) >= 4;
+      }
+    }
+    sbs[dir][e][seg] = (uint8_t)bS;
+  }
+  // qP: the stream QP, 0 on an I_PCM side; chroma averages each side's QPc
+  const int qp_q = (info[mb] >> 7) & 1 ? 0 : qp;
+  const int qp_l = has_l && !((info[mb_l] >> 7) & 1) ? qp : 0, qp_t = has_t && !((info[mb_t] >> 7) & 1) ? qp : 0;
+  __syncwarp();
+  for (int dir = 0; dir < 2; dir++) {
+    const int qp_p = dir ? qp_t : qp_l;
+    if (t < 16) {
+      for (int e = 0; e < 4; e++) {
+        const int bS = sbs[dir][e][t >> 2];
+        if (bS) filter_line(dir ? &sy[4 * e + 4][t + 4] : &sy[t + 4][4 * e + 4], dir ? 20 : 1, false, bS,
+                            e ? qp_q : (qp_p + qp_q + 1) >> 1);
+      }
+    } else {
+      const int p = (t - 16) >> 3, k = t & 7;
+      for (int e = 0; e < 2; e++) {
+        const int bS = sbs[dir][2 * e][k >> 1];
+        const int qc = c_chroma_qp[qp_q];
+        if (bS) filter_line(dir ? &sc[p][4 * e + 2][k + 2] : &sc[p][k + 2][4 * e + 2], dir ? 10 : 1, true, bS,
+                            e ? qc : (c_chroma_qp[qp_p] + qc + 1) >> 1);
+      }
+    }
+    __syncwarp();
+  }
+  for (int i = t; i < 361; i += 32) {   // rows and columns -3 .. 15, the corner excepted
+    const int r = i / 19 - 3, c = i % 19 - 3;
+    if ((r < 0 && (c < 0 || !has_t)) || (c < 0 && !has_l)) continue;
+    flt[(int64_t)(16 * my + r) * ys + 16 * mx + c] = sy[r + 4][c + 4];
+  }
+  for (int i = t; i < 162; i += 32) {   // rows and columns -1 .. 7
+    const int p = i / 81, r = i % 81 / 9 - 1, c = i % 9 - 1;
+    if ((r < 0 && (c < 0 || !has_t)) || (c < 0 && !has_l)) continue;
+    flt[c0 + p * cpl + (int64_t)(8 * my + r) * cs + 8 * mx + c] = sc[p][r + 2][c + 2];
+  }
+}
+
 // ---- P slices: vector prediction and skip runs, after every decision is made -------------------------------------
 struct Neighbour {
   bool avail;
@@ -961,11 +1145,12 @@ __global__ void __launch_bounds__(1024) h264_scan_kernel(uint8_t* scratch, Layou
   __syncthreads();
   if (t == 0) {
     // first_mb_in_slice 0, slice_type 7, pps 0, frame_num 0000, idr_pic_id 1, two flags, slice_qp_delta 0,
-    // disable_deblocking_filter_idc 1
-    if (is_p)   // first_mb_in_slice 0, slice_type 5, pps 0, frame_num, three flags 0, slice_qp_delta 0, idc 1
-      put_bits(raw, 0, 0x4Du << 11 | (uint32_t)meta[2] << 7 | 0x0Au, P_HEADER_BITS);   // 1 00110 1 ffff 0 0 0 1 010
+    // disable_deblocking_filter_idc 1 (010); deblocked: idc 0 and both offsets se(0) (1 1 1), as many bits
+    const uint32_t idc = l.deblock ? 7u : 2u;
+    if (is_p)   // first_mb_in_slice 0, slice_type 5, pps 0, frame_num, three flags 0, slice_qp_delta 0, idc
+      put_bits(raw, 0, 0x4Du << 11 | (uint32_t)meta[2] << 7 | 0x08u | idc, P_HEADER_BITS);   // 1 00110 1 ffff 0 0 0 1 010
     else
-      put_bits(raw, 0, 0x22208Au, HEADER_BITS);  // 1 0001000 1 0000 010 0 0 1 010
+      put_bits(raw, 0, 0x222088u | idc, HEADER_BITS);  // 1 0001000 1 0000 010 0 0 1 010
     put_bits(raw, total, 1, 1);                  // rbsp_stop_one_bit
     reinterpret_cast<int*>(base + l.meta)[0] = nbytes;
   }
@@ -1136,10 +1321,10 @@ __global__ void __launch_bounds__(256) h264_frame_kernel(uint8_t* scratch, Layou
   meta[2] = (int)((n % gop) % 16);
 }
 
-// The last frame's reconstruction becomes the state's picture, and the position advances by the batch.
+// The last frame's reconstruction (deblocked when the stream is) becomes the state's picture, and the position advances by the batch.
 __global__ void __launch_bounds__(256) h264_state_kernel(const uint8_t* scratch, Layout l, uint8_t* state,
                                                          int frames) {
-  const uint4* src = reinterpret_cast<const uint4*>(scratch + (int64_t)(frames - 1) * l.stride + l.rec);
+  const uint4* src = reinterpret_cast<const uint4*>(scratch + (int64_t)(frames - 1) * l.stride + l.flt);
   uint4* dst = reinterpret_cast<uint4*>(state + 256);
   const int64_t n = (int64_t)l.nmb * 384 / 16;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
@@ -1216,9 +1401,9 @@ size_t h264_state_bytes(int H, int W) {
   return (size_t)(256 + align256((int64_t)((W + 15) / 16) * ((H + 15) / 16) * 384));
 }
 
-size_t h264_scratch_bytes(int64_t frames, int H, int W) {
+size_t h264_scratch_bytes(int64_t frames, int H, int W, bool deblock) {
   if (frames <= 0 || frames > 65535 || h264_bound(W, H) < 0) return 0;
-  return (size_t)(frames * layout(H, W).stride);
+  return (size_t)(frames * layout(H, W, deblock).stride);
 }
 
 int32_t h264_parameter_sets(int W, int H, int qp, int fps_num, int fps_den, int gop, uint8_t* out, int64_t cap) {
@@ -1294,26 +1479,47 @@ int32_t h264_parameter_sets(int W, int H, int qp, int fps_num, int fps_den, int 
   return (int32_t)need;
 }
 
-void launch_h264_encode(int frames, int H, int W, int qp, int gop, const uint8_t* rgb, uint8_t* state, void* scratch,
-                        uint8_t* out, int64_t out_stride, int64_t* out_len, cudaStream_t stream) {
-  const Layout l = layout(H, W);
+void launch_h264_encode(int frames, int H, int W, int qp, int gop, bool deblock, const uint8_t* rgb, uint8_t* state,
+                        void* scratch, uint8_t* out, int64_t out_stride, int64_t* out_len, cudaStream_t stream) {
+  const Layout l = layout(H, W, deblock);
   uint8_t* s = static_cast<uint8_t*>(scratch);
   const unsigned F = (unsigned)frames;
   h264_convert_kernel<<<dim3((unsigned)((64 * l.nmb + 255) / 256), F), 256, 0, stream>>>(rgb, s, l);
   count_launch();
   h264_frame_kernel<<<(F + 255) / 256, 256, 0, stream>>>(s, l, state, gop, frames);
   count_launch();
-  // The wavefront over (frame, anti-diagonal): step k runs diagonal k - lag f of every frame f that has one.
-  const int D = l.wm + l.hm - 1, lag = gop > 1 ? LAG : 0;
-  auto diag_len = [&](int d) { return std::min(d, l.wm - 1) - std::max(0, d - l.hm + 1) + 1; };
-  for (int k = 0; k < D + (frames - 1) * lag; k++) {
-    const int f_lo = lag ? std::max(0, (k - (D - 1) + lag - 1) / lag) : 0;
-    const int f_hi = lag ? std::min(frames - 1, k / lag) : frames - 1;
-    int n = 0;   // 0 when lag > D leaves a step between two frames' wavefronts
-    for (int f = f_lo; f <= f_hi && n < std::min(l.wm, l.hm); f++) n = std::max(n, diag_len(k - lag * f));
-    if (n == 0) continue;
-    h264_mb_kernel<<<dim3((unsigned)n, (unsigned)(f_hi - f_lo + 1)), 128, 0, stream>>>(k, lag, f_lo, qp, s, state, l);
-    count_launch();
+  // The wavefront over (frame, line): step k encodes line k - lag f of every frame f that has one (anti-diagonals
+  // mbx + mby, or lines mbx + 2 mby in a deblocked P stream) and then filters line k - lag f - DB_LAG.
+  const int slope = deblock && gop > 1 ? 2 : 1, D = l.wm + slope * (l.hm - 1), DB = l.wm + 2 * (l.hm - 1);
+  const int lag = gop > 1 ? (deblock ? LAG_DB : LAG) : 0;
+  auto line_len = [&](int d, int sl) {
+    if (d < 0 || d >= l.wm + sl * (l.hm - 1)) return 0;
+    return sl == 1 ? std::min(d, l.wm - 1) - std::max(0, d - l.hm + 1) + 1
+                   : std::min(d / 2, l.hm - 1) - std::max(0, (d - l.wm + 2) / 2) + 1;
+  };
+  // the frames with a line at step k of a wavefront `off` steps behind, `lines` lines long, and its longest line
+  auto frames_at = [&](int k, int off, int lines, int sl, int& f_lo, int& f_hi) {
+    f_lo = lag ? std::max(0, (k - off - (lines - 1) + lag - 1) / lag) : 0;
+    f_hi = lag ? std::min(frames - 1, (k - off) / lag) : frames - 1;
+    int n = 0;   // 0 when lag > lines leaves a step between two frames' wavefronts
+    for (int f = f_lo; f <= f_hi && n < std::min(l.wm, l.hm); f++) n = std::max(n, line_len(k - off - lag * f, sl));
+    return n;
+  };
+  const int steps = std::max(D, deblock ? DB + DB_LAG : 0) + (frames - 1) * lag;
+  for (int k = 0; k < steps; k++) {
+    int f_lo, f_hi;
+    int n = frames_at(k, 0, D, slope, f_lo, f_hi);
+    if (n > 0) {
+      h264_mb_kernel<<<dim3((unsigned)n, (unsigned)(f_hi - f_lo + 1)), 128, 0, stream>>>(k, lag, slope, f_lo, qp, s,
+                                                                                       state, l);
+      count_launch();
+    }
+    if (!deblock) continue;
+    n = frames_at(k, DB_LAG, DB, 2, f_lo, f_hi);
+    if (n > 0) {
+      h264_deblock_kernel<<<dim3((unsigned)n, (unsigned)(f_hi - f_lo + 1)), 32, 0, stream>>>(k, lag, f_lo, qp, s, l);
+      count_launch();
+    }
   }
   const unsigned mbb = (unsigned)((l.nmb + 127) / 128);
   if (gop > 1) {

@@ -5,14 +5,17 @@ renders.mp4` makes of the PNG files it wrote, without the PNG files.
         for t in timesteps:
             player.run(...)
             vw.add(player.display)                        # CUDA (H,W,3) or (K,H,W,3) uint8
-    data = encode_video(frames, fps=25, qp=20, gop=1)     # a whole MP4 in memory
+    data = encode_video(frames, fps=25, qp=20, gop=1, deblock=False)   # a whole MP4 in memory
 
 The frames are encoded on the device (csrc/h264.cu, include/gab200_rasterizer.h gab200_h264_encode and
 gab200_h264_encode_stream): H.264 Constrained Baseline, one fixed QP, BT.601 limited-range 4:2:0.  With gop=1 (the
 default) every frame is an IDR picture; with gop=N every N-th frame is, and the others are P pictures that refer to
-the frame before them, which is far smaller when successive frames look alike (a fixed camera).  Only the compressed
-samples cross to the host, through a ring of pinned slots; the file is ftyp | mdat | moov, muxed here, with an stss
-box listing the IDR frames when gop > 1.  The bytes are deterministic and differ from libx264's.
+the frame before them, which is far smaller when successive frames look alike (a fixed camera).  Deblocking is off by
+default, so a decoder outputs the encoder's reconstruction as it is; with deblock=True every slice turns the in-loop
+deblocking filter on, and the encoder filters each picture as a decoder does (gab200_h264_encode_deblocked), the P
+pictures predicting from the filtered one.  Only the compressed samples cross to the host, through a ring of pinned
+slots; the file is ftyp | mdat | moov, muxed here, with an stss box listing the IDR frames when gop > 1.  The bytes are
+deterministic and differ from libx264's.
 """
 from __future__ import annotations
 
@@ -53,6 +56,12 @@ def _check_gop(gop) -> int:
     if isinstance(gop, bool) or not isinstance(gop, int) or not 1 <= gop <= 65535:
         raise ValueError(f"gop must be an int in 1..65535, got {gop!r}")
     return gop
+
+
+def _check_deblock(deblock) -> bool:
+    if not isinstance(deblock, bool):
+        raise ValueError(f"deblock must be a bool, got {deblock!r}")
+    return deblock
 
 
 def _check_qp(qp) -> int:
@@ -124,6 +133,19 @@ def launch_encode_stream(frames: torch.Tensor, qp: int, gop: int, state: torch.T
                                               out_len.data_ptr(), stream), "gab200_h264_encode_stream")
 
 
+def launch_encode_deblocked(frames: torch.Tensor, qp: int, gop: int, state, scratch_buf: torch.Tensor,
+                            out: torch.Tensor, out_len: torch.Tensor):
+    """Enqueues gab200_h264_encode_deblocked on the current stream: launch_encode_stream's samples with the deblocking
+    filter on, scratch from deblocked_scratch.  state may be None when gop is 1.  Reads nothing on the host:
+    capturable."""
+    K, H, W = check_frames(frames)
+    stream = C.c_void_p(torch.cuda.current_stream(frames.device).cuda_stream)
+    N.check(N.lib().gab200_h264_encode_deblocked(K, H, W, qp, gop, frames.data_ptr(),
+                                                 None if state is None else state.data_ptr(), scratch_buf.data_ptr(),
+                                                 out.data_ptr(), out.stride(0), out_len.data_ptr(), stream),
+            "gab200_h264_encode_deblocked")
+
+
 def state_buffer(H: int, W: int, device) -> torch.Tensor:
     """A zeroed stream state: its next frame is an IDR picture."""
     n = int(N.lib().gab200_h264_state_bytes(H, W))
@@ -136,6 +158,13 @@ def scratch(K: int, H: int, W: int, device) -> torch.Tensor:
     n = int(N.lib().gab200_h264_scratch_bytes(K, H, W))
     if n == 0:
         raise ValueError(f"no H.264 encode of {K} frames of {W}x{H}")
+    return torch.empty(n, dtype=torch.uint8, device=device)
+
+
+def deblocked_scratch(K: int, H: int, W: int, gop: int, device) -> torch.Tensor:
+    n = int(N.lib().gab200_h264_deblocked_scratch_bytes(K, H, W, gop))
+    if n == 0:
+        raise ValueError(f"no deblocked H.264 encode of {K} frames of {W}x{H} with gop {gop}")
     return torch.empty(n, dtype=torch.uint8, device=device)
 
 
@@ -199,14 +228,17 @@ class VideoWriter:
     path: a file name, or a seekable binary file object (left open).  fps: an int or a fractions.Fraction (the
     track's timescale is its numerator, each sample lasts its denominator).  gop: every gop-th frame, the first
     included, is an IDR picture and the others P pictures (1: every frame an IDR picture); the writer owns the
-    stream's state on the device, so a batch may start anywhere in a GOP."""
+    stream's state on the device, so a batch may start anywhere in a GOP.  deblock: the in-loop deblocking filter on
+    in every slice of the stream (a bool; the writer keeps one mode for its whole stream)."""
 
     RING = 3
 
-    def __init__(self, path, width: int, height: int, fps=25, qp: int = 20, batch: int = 16, device=None, gop: int = 1):
+    def __init__(self, path, width: int, height: int, fps=25, qp: int = 20, batch: int = 16, device=None, gop: int = 1,
+                 deblock: bool = False):
         self.fps = _check_fps(fps)
         self.qp = _check_qp(qp)
         self.gop = _check_gop(gop)
+        self.deblock = _check_deblock(deblock)
         if isinstance(batch, bool) or not isinstance(batch, int) or not 1 <= batch <= 65535:
             raise ValueError(f"batch must be an int in 1..65535, got {batch!r}")
         self.W, self.H = int(width), int(height)
@@ -218,7 +250,8 @@ class VideoWriter:
         self.batch = batch
         with torch.cuda.device(self.device):
             self._frames = torch.empty((batch, self.H, self.W, 3), dtype=torch.uint8, device=self.device)
-            self._scratch = scratch(batch, self.H, self.W, self.device)
+            self._scratch = deblocked_scratch(batch, self.H, self.W, self.gop, self.device) if self.deblock else \
+                scratch(batch, self.H, self.W, self.device)
             self._out = torch.empty((batch, self.stride), dtype=torch.uint8, device=self.device)
             self._out_len = torch.empty(batch, dtype=torch.int64, device=self.device)
             self._state = state_buffer(self.H, self.W, self.device) if self.gop > 1 else None
@@ -269,7 +302,10 @@ class VideoWriter:
         self._next_slot = (slot + 1) % self.RING
         if len(self._pending) == self.RING:
             self._drain(1)
-        if self._state is None:
+        if self.deblock:
+            launch_encode_deblocked(self._frames[:n], self.qp, self.gop, self._state, self._scratch, self._out,
+                                    self._out_len)
+        elif self._state is None:
             launch_encode(self._frames[:n], self.qp, self._scratch, self._out, self._out_len)
         else:
             launch_encode_stream(self._frames[:n], self.qp, self.gop, self._state, self._scratch, self._out,
@@ -320,10 +356,11 @@ class VideoWriter:
 
 
 @torch.no_grad()
-def encode_video(frames: torch.Tensor, fps=25, qp: int = 20, gop: int = 1) -> bytes:
+def encode_video(frames: torch.Tensor, fps=25, qp: int = 20, gop: int = 1, deblock: bool = False) -> bytes:
     """A whole MP4 of a CUDA uint8 (H,W,3) frame or (K,H,W,3) clip, in memory."""
     K, H, W = check_frames(frames)
     buf = io.BytesIO()
-    with VideoWriter(buf, W, H, fps=fps, qp=qp, batch=min(K, 16), device=frames.device, gop=gop) as vw:
+    with VideoWriter(buf, W, H, fps=fps, qp=qp, batch=min(K, 16), device=frames.device, gop=gop,
+                     deblock=deblock) as vw:
         vw.add(frames)
     return buf.getvalue()

@@ -553,7 +553,8 @@ int32_t gab200_resize_u8(int64_t planes, int32_t in_height, int32_t in_width, in
 /* H.264 video frames encoded on the device (csrc/h264.cu, gaussianavatars_b200.video): Constrained Baseline
  * (profile_idc 66, constraint_set0/1), 8-bit 4:2:0, CAVLC.  Every picture is one IDR slice (pic_order_cnt_type 2,
  * max_num_ref_frames 0), so every frame is a seek point and the frames of a batch are independent.  Deblocking is off
- * (disable_deblocking_filter_idc 1): a conforming decoder outputs exactly the encoder's reconstruction.  One QP per
+ * (disable_deblocking_filter_idc 1) except in gab200_h264_encode_deblocked's streams: a conforming decoder outputs
+ * exactly the encoder's reconstruction (its filtered copy when the stream is deblocked).  One QP per
  * stream; the chroma QP from Table 8-15 with chroma_qp_index_offset 0.
  *
  * RGB -> BT.601 limited range in integers: Y = ((66 R + 129 G + 25 B + 128) >> 8) + 16; with R4, G4, B4 the sums of a
@@ -630,6 +631,27 @@ int32_t gab200_h264_encode_stream(int32_t frames, int32_t height, int32_t width,
  * 1..65535. */
 int32_t gab200_h264_stream_parameter_sets(int32_t width, int32_t height, int32_t qp, int32_t fps_num, int32_t fps_den,
                                           int32_t gop, uint8_t* out, int64_t cap);
+
+/* A deblocked stream (gaussianavatars_b200.video VideoWriter(deblock=True)): gab200_h264_encode_stream's stream
+ * (gop 1: gab200_h264_encode's) with every slice's disable_deblocking_filter_idc 0 and slice_alpha_c0_offset_div2 =
+ * slice_beta_offset_div2 = 0, which keeps the slice headers' lengths; the SPS and PPS are
+ * gab200_h264_stream_parameter_sets'.  The encoder applies the in-loop filter (8.7) to every picture: intra
+ * prediction reads the unfiltered samples of its picture, and a P picture's motion search and inter prediction read
+ * the previous picture filtered, as a decoder does.  bS 4 on a macroblock edge with an intra side, 3 on an intra
+ * macroblock's inner edges, 2 where a 4x4 luma block has coefficients, 1 where the two vectors differ by 4 quarter
+ * samples or more; qP the stream QP, 0 on an I_PCM side.  The filter runs on lines mbx + 2 mby inside the encode's
+ * wavefront; a P stream's encode runs on those lines too, frame f + 1 nine lines behind frame f (its window reaches
+ * two macroblocks right and down into the filtered picture).  tests/h264_deblock_oracle.py restates the filter. */
+/* Scratch bytes of gab200_h264_encode_deblocked: the plain scratch and the filtered planes (0 for a size, count or gop
+ * it refuses). */
+size_t gab200_h264_deblocked_scratch_bytes(int32_t frames, int32_t height, int32_t width, int32_t gop);
+/* Encode rgb [frames, height, width, 3] as the next frames of a deblocked stream; arguments, bounds and samples as
+ * gab200_h264_encode_stream's, except that state may be NULL when gop is 1 (the frames are then independent).  With a
+ * state its picture is the last frame's filtered picture.  Refused before any device work: what
+ * gab200_h264_encode_stream refuses, a NULL state only when gop > 1. */
+int32_t gab200_h264_encode_deblocked(int32_t frames, int32_t height, int32_t width, int32_t qp, int32_t gop,
+                                     const uint8_t* rgb, void* state, void* scratch, uint8_t* out, int64_t out_stride,
+                                     int64_t* out_len, void* stream);
 
 /* A device-resident view schedule (csrc/schedule.cu, gaussianavatars_b200.schedule.ViewSchedule): `records` records
  * of `views` cameras each -- cams [records, views, GAB200_CAMERA_FLOATS] float32, timesteps [records] int32 (may be
