@@ -255,7 +255,8 @@ EXPORTED_SYMBOLS = ("gab200_forward", "gab200_backward", "gab200_mark_visible", 
                     "gab200_h264_parameter_sets", "gab200_mesh_views_scratch_bytes", "gab200_mesh_render_views",
                     "gab200_h264_p_bound", "gab200_h264_state_bytes", "gab200_h264_stream_scratch_bytes",
                     "gab200_h264_encode_stream", "gab200_h264_stream_parameter_sets",
-                    "gab200_h264_deblocked_scratch_bytes", "gab200_h264_encode_deblocked")
+                    "gab200_h264_deblocked_scratch_bytes", "gab200_h264_encode_deblocked",
+                    "gab200_h264_flags_scratch_bytes", "gab200_h264_encode_flags")
 
 _lib = None
 _lock = threading.Lock()
@@ -405,6 +406,11 @@ def lib():
         L.gab200_h264_deblocked_scratch_bytes.argtypes = [C.c_int32] * 4
         L.gab200_h264_encode_deblocked.restype = C.c_int32
         L.gab200_h264_encode_deblocked.argtypes = [C.c_int32] * 5 + [C.c_void_p] * 4 + [C.c_int64, C.c_void_p, C.c_void_p]
+        L.gab200_h264_flags_scratch_bytes.restype = C.c_size_t
+        L.gab200_h264_flags_scratch_bytes.argtypes = [C.c_int32] * 4 + [C.c_uint32]
+        L.gab200_h264_encode_flags.restype = C.c_int32
+        L.gab200_h264_encode_flags.argtypes = [C.c_int32] * 5 + [C.c_uint32] + [C.c_void_p] * 4 + [C.c_int64, C.c_void_p,
+                                                                                                  C.c_void_p]
         L.gab200_schedule_sample.restype = C.c_int32
         L.gab200_schedule_sample.argtypes = [C.c_int32, C.c_int32, C.c_int32] + [C.c_void_p] * 11
         L.gab200_schedule_commit.restype = C.c_int32

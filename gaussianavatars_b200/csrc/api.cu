@@ -1069,7 +1069,7 @@ int32_t gab200_h264_encode(int32_t frames, int32_t height, int32_t width, int32_
   if (out_stride < h264_bound(width, height)) return GAB200_ERR_INVALID_ARGUMENT;
   if (!rgb || !scratch || !out || !out_len || ((uintptr_t)scratch & 255) != 0) return GAB200_ERR_INVALID_ARGUMENT;
   if (check_arch() < 0) return GAB200_ERR_ARCH;
-  launch_h264_encode(frames, height, width, qp, 1, false, rgb, nullptr, scratch, out, out_stride, out_len,
+  launch_h264_encode(frames, height, width, qp, 1, false, false, rgb, nullptr, scratch, out, out_stride, out_len,
                      (cudaStream_t)stream_);
   return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
 }
@@ -1097,7 +1097,7 @@ int32_t gab200_h264_encode_stream(int32_t frames, int32_t height, int32_t width,
   if (!rgb || !state || !scratch || !out || !out_len) return GAB200_ERR_INVALID_ARGUMENT;
   if (((uintptr_t)scratch & 255) != 0 || ((uintptr_t)state & 255) != 0) return GAB200_ERR_INVALID_ARGUMENT;
   if (check_arch() < 0) return GAB200_ERR_ARCH;
-  launch_h264_encode(frames, height, width, qp, gop, false, rgb, static_cast<uint8_t*>(state), scratch, out,
+  launch_h264_encode(frames, height, width, qp, gop, false, false, rgb, static_cast<uint8_t*>(state), scratch, out,
                      out_stride, out_len, (cudaStream_t)stream_);
   return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
 }
@@ -1116,8 +1116,27 @@ int32_t gab200_h264_encode_deblocked(int32_t frames, int32_t height, int32_t wid
   if (!rgb || (!state && gop > 1) || !scratch || !out || !out_len) return GAB200_ERR_INVALID_ARGUMENT;
   if (((uintptr_t)scratch & 255) != 0 || ((uintptr_t)state & 255) != 0) return GAB200_ERR_INVALID_ARGUMENT;
   if (check_arch() < 0) return GAB200_ERR_ARCH;
-  launch_h264_encode(frames, height, width, qp, gop, true, rgb, static_cast<uint8_t*>(state), scratch, out,
+  launch_h264_encode(frames, height, width, qp, gop, true, false, rgb, static_cast<uint8_t*>(state), scratch, out,
                      out_stride, out_len, (cudaStream_t)stream_);
+  return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
+}
+
+size_t gab200_h264_flags_scratch_bytes(int32_t frames, int32_t height, int32_t width, int32_t gop, uint32_t flags) {
+  if (gop < 1 || gop > 65535 || (flags & ~(uint32_t)(GAB200_H264_DEBLOCK | GAB200_H264_INTRA4X4))) return 0;
+  return h264_scratch_bytes(frames, height, width, flags & GAB200_H264_DEBLOCK, flags & GAB200_H264_INTRA4X4);
+}
+
+int32_t gab200_h264_encode_flags(int32_t frames, int32_t height, int32_t width, int32_t qp, int32_t gop, uint32_t flags,
+                                 const uint8_t* rgb, void* state, void* scratch, uint8_t* out, int64_t out_stride,
+                                 int64_t* out_len, void* stream_) {
+  if (gab200_h264_flags_scratch_bytes(frames, height, width, gop, flags) == 0 || qp < 0 || qp > 51)
+    return GAB200_ERR_INVALID_ARGUMENT;
+  if (out_stride < (gop > 1 ? h264_p_bound(width, height) : h264_bound(width, height))) return GAB200_ERR_INVALID_ARGUMENT;
+  if (!rgb || (!state && gop > 1) || !scratch || !out || !out_len) return GAB200_ERR_INVALID_ARGUMENT;
+  if (((uintptr_t)scratch & 255) != 0 || ((uintptr_t)state & 255) != 0) return GAB200_ERR_INVALID_ARGUMENT;
+  if (check_arch() < 0) return GAB200_ERR_ARCH;
+  launch_h264_encode(frames, height, width, qp, gop, flags & GAB200_H264_DEBLOCK, flags & GAB200_H264_INTRA4X4, rgb,
+                     static_cast<uint8_t*>(state), scratch, out, out_stride, out_len, (cudaStream_t)stream_);
   return cudaPeekAtLastError() == cudaSuccess ? GAB200_OK : GAB200_ERR_CUDA;
 }
 

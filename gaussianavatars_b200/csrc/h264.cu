@@ -1,11 +1,14 @@
 // h264.cu -- H.264 video frames encoded on the device (gab200_h264_bound / gab200_h264_scratch_bytes /
 // gab200_h264_encode / gab200_h264_parameter_sets, and for streams with P pictures gab200_h264_p_bound /
 // gab200_h264_state_bytes / gab200_h264_encode_stream / gab200_h264_stream_parameter_sets, and for deblocked streams
-// gab200_h264_deblocked_scratch_bytes / gab200_h264_encode_deblocked): Constrained Baseline, CAVLC, one fixed QP,
+// gab200_h264_deblocked_scratch_bytes / gab200_h264_encode_deblocked, and for every option through one flags word
+// gab200_h264_flags_scratch_bytes / gab200_h264_encode_flags): Constrained Baseline, CAVLC, one fixed QP,
 // deblocking off (disable_deblocking_filter_idc 1) unless the stream is deblocked (idc 0, offsets 0).  An IDR
-// picture's macroblocks are I_16x16 (luma and chroma modes of least SATD) or I_PCM; a P picture's are P_Skip,
-// P_L0_16x16 (one quarter-sample vector), I_16x16 or I_PCM.  oracle/h264.py, tests/h264_stream_oracle.py and
-// tests/h264_deblock_oracle.py restate every step, and the tests compare their bytes with these.
+// picture's macroblocks are I_16x16 (luma and chroma modes of least SATD), I_NxN when the stream has the intra 4x4
+// option (Intra_4x4 modes per 4x4 block, see h264_mb_kernel) or I_PCM; a P picture's are P_Skip, P_L0_16x16 (one
+// quarter-sample vector), I_16x16, I_NxN or I_PCM.  oracle/h264.py, tests/h264_stream_oracle.py,
+// tests/h264_deblock_oracle.py and tests/h264_intra4x4_oracle.py restate every step, and the tests compare their
+// bytes with these.
 //
 // Per batch of frames the encode runs these kernels, each named for a trace:
 //   h264_convert_kernel  RGB -> BT.601 limited-range Y, Cb, Cr planes padded to whole macroblocks by edge replication.
@@ -15,11 +18,12 @@
 //                        and LAG when a frame refers to the one before (LAG more launches per frame); a deblocked P
 //                        stream runs lines d = mbx + 2 mby instead, lag LAG_DB (see LAG_DB).  One 128-thread
 //                        CTA per (macroblock on d, frame): in a P picture the motion search in the previous picture;
-//                        prediction from the reconstructed left / top / top-left samples of earlier diagonals, mode
-//                        decision by SATD, transform, quantisation, reconstruction into the recon planes, per-4x4
-//                        TotalCoeff, the macroblock's CAVLC bit count and the I_PCM fallback; the levels are kept for
-//                        the writer.  The launch boundary is the wavefront's only synchronisation: no CTA ever waits
-//                        on another.
+//                        prediction from the reconstructed left / top / top-left samples of earlier diagonals (with
+//                        the intra 4x4 option, <true>, also the I_NxN candidate's 16 blocks as a wavefront inside the
+//                        CTA), mode decision by SATD, transform, quantisation, reconstruction into the recon planes,
+//                        per-4x4 TotalCoeff, the macroblock's CAVLC bit count and the I_PCM fallback; the levels are
+//                        kept for the writer.  The launch boundary is the wavefront's only synchronisation: no CTA
+//                        ever waits on another.
 //   h264_deblock_kernel  deblocked streams, launched after h264_mb_kernel in each step: one warp per macroblock on
 //                        line mbx + 2 mby = step - lag f - DB_LAG of frame f; bS from the macroblocks' info, TotalCoeff
 //                        and vectors, then the filter (8.7) of its edges from the unfiltered recon planes into the
@@ -60,6 +64,10 @@ constexpr int P_HEADER_BITS = 18;            // the P slice header
 constexpr int SEARCH = 16;                   // integer motion search range, samples
 constexpr int MVD_BITS = 2 * 17;             // se(v) of the largest |mvd|, 2 * (4 SEARCH + 3) quarter samples, twice
 constexpr int INTRA_BIAS = 24;               // intra's SATD handicap against inter, in units of lambda
+// I_NxN's handicap against I_16x16, in units of lambda, on top of its blocks' mode bits (see h264_mb_kernel): of the
+// candidates -8, 0, 8 and 16 (scripts/video_intra4x4_sweep.py --bias), 8 gave the fewest bytes or the best Y-PSNR
+// at qp 26 to 38, and at qp 20 bytes within 1.5 % of the fewest with a higher Y-PSNR than 16's.
+constexpr int I4_BIAS = 8;
 // A vector reaches 4 SEARCH + 3 quarter samples, and the 6-tap filter 2 samples before and 3 after: the window of a
 // macroblock's reference samples spans REACH samples on each side, WIN samples in all.
 constexpr int REACH = (4 * SEARCH + 3) / 4 + 3;
@@ -94,6 +102,10 @@ __constant__ int c_v[6][3] = {{10, 16, 13}, {11, 18, 14}, {13, 20, 16}, {14, 23,
 __constant__ uint8_t c_inter_cbp[48] = {0,  2,  3,  7,  4,  8,  17, 13, 5,  18, 9,  14, 10, 15, 16, 11,
                                         1,  32, 33, 36, 34, 37, 44, 40, 35, 45, 38, 41, 39, 42, 43, 19,
                                         6,  24, 25, 20, 26, 21, 46, 28, 27, 47, 22, 29, 23, 30, 31, 12};
+// Table 9-4, intra column: coded_block_pattern -> codeNum
+__constant__ uint8_t c_intra_cbp[48] = {3,  29, 30, 17, 31, 18, 37, 8,  32, 38, 19, 9,  20, 10, 11, 2,
+                                        16, 33, 34, 21, 35, 22, 39, 4,  36, 40, 23, 5,  24, 6,  7,  1,
+                                        41, 42, 43, 25, 44, 26, 46, 12, 45, 47, 27, 13, 28, 14, 15, 0};
 // luma4x4BlkIdx -> (x, y) of the 4x4 block in the macroblock, in blocks
 __constant__ int8_t c_blk_x[16] = {0, 1, 0, 1, 2, 3, 2, 3, 0, 1, 0, 1, 2, 3, 2, 3};
 __constant__ int8_t c_blk_y[16] = {0, 0, 1, 1, 0, 0, 1, 1, 2, 2, 3, 3, 2, 2, 3, 3};
@@ -155,8 +167,9 @@ __constant__ uint8_t c_rb_code[7][15] = {{1, 0},          {1, 1, 0},          {3
 // The per-frame scratch: offsets from the frame's base (each 256-byte aligned), and the frame stride.
 struct Layout {
   int W, H, wm, hm, nmb, pieces, deblock;
-  // flt: the picture a P picture refers to and the state keeps -- the deblocked copy of rec, or rec itself
-  int64_t src, rec, tot, lev, info, bits, off, mv, mvd, run, raw, ep, meta, flt, stride;
+  // flt: the picture a P picture refers to and the state keeps -- the deblocked copy of rec, or rec itself;
+  // modes: the I_NxN streams' Intra4x4PredMode per 4x4 block, 8 bytes per macroblock
+  int64_t src, rec, tot, lev, info, bits, off, mv, mvd, run, raw, ep, meta, flt, modes, stride;
 };
 
 int64_t align256(int64_t x) { return (x + 255) / 256 * 256; }
@@ -167,7 +180,7 @@ int64_t raw_bytes_bound_p(int nmb) {
   return (P_HEADER_BITS + (int64_t)nmb * (3 + MVD_BITS + PCM_BITS + 7) + 1 + 7) / 8;
 }
 
-Layout layout(int H, int W, bool deblock = false) {
+Layout layout(int H, int W, bool deblock = false, bool intra4x4 = false) {
   Layout l;
   l.deblock = deblock;
   l.W = W;
@@ -194,6 +207,8 @@ Layout layout(int H, int W, bool deblock = false) {
   l.meta = o; o = align256(o + 16);                                   // raw byte count, P picture, frame_num
   l.flt = l.rec;
   if (deblock) { l.flt = o; o = align256(o + plane); }                 // the deblocked picture
+  l.modes = 0;
+  if (intra4x4) { l.modes = o; o = align256(o + (int64_t)l.nmb * 8); } // raster 4x4 block k in bits 4k .. 4k + 3
   l.stride = o;
   return l;
 }
@@ -356,9 +371,10 @@ __device__ void block_geom(int id, int mx, int my, int& plane, int& x, int& y, i
 }
 
 // A macroblock's info word: luma mode (bits 0-1), chroma mode (2-3), CodedBlockPatternChroma (4-5), I_16x16 AC
-// coded (6), I_PCM (7), P_L0_16x16 (8), its CodedBlockPatternLuma (9-12), P_Skip (13).
+// coded (6), I_PCM (7), P_L0_16x16 (8), its CodedBlockPatternLuma (9-12), P_Skip (13), I_NxN (14, with its
+// CodedBlockPatternLuma in 9-12 and its luma blocks coded as an inter macroblock's: 16 coefficients, no DC block).
 __device__ __forceinline__ bool block_present(int id, int info) {
-  const bool inter = (info >> 8) & 1;
+  const bool inter = info & (1 << 8 | 1 << 14);
   const int cbpc = (info >> 4) & 3;
   if (id == 0) return !inter;
   if (id <= 16) return inter ? (info >> (9 + ((id - 1) >> 2))) & 1 : (info >> 6) & 1;
@@ -375,6 +391,88 @@ __device__ __forceinline__ int inter_cbp(int info) { return ((info >> 9) & 15) |
 __device__ __forceinline__ int mb_header_bits(int info, bool is_p) {
   if ((info >> 8) & 1) return 1 + ue_bits(c_inter_cbp[inter_cbp(info)]) + (inter_cbp(info) ? 1 : 0);
   return ue_bits(i16_mb_type(info, is_p)) + ue_bits((info >> 2) & 3) + 1;
+}
+
+// ---- Intra_4x4 (8.3.1) -------------------------------------------------------------------------------------------
+// luma4x4BlkIdx of the 4x4 block at (bx, by) of a macroblock
+__device__ __forceinline__ int blk_idx(int bx, int by) { return 8 * (by >> 1) + 4 * (bx >> 1) + 2 * (by & 1) + (bx & 1); }
+
+__device__ __forceinline__ int mode_at(uint64_t modes, int bx, int by) { return (int)(modes >> (4 * (4 * by + bx))) & 15; }
+
+// 8.3.1.1: predIntra4x4PredMode of block (bx, by) of macroblock (mx, my), whose own modes are `own`; a neighbouring
+// macroblock that is unavailable gives 2, one that is not I_NxN gives mode 2 for its blocks.
+__device__ __forceinline__ int i4_pred_mode(uint64_t own, const int* info, const uint64_t* modes, int wm, int mx,
+                                            int my, int bx, int by) {
+  int a, b;
+  if (bx > 0) a = mode_at(own, bx - 1, by);
+  else if (mx == 0) return 2;
+  else a = (info[my * wm + mx - 1] >> 14) & 1 ? mode_at(modes[my * wm + mx - 1], 3, by) : 2;
+  if (by > 0) b = mode_at(own, bx, by - 1);
+  else if (my == 0) return 2;
+  else b = (info[(my - 1) * wm + mx] >> 14) & 1 ? mode_at(modes[(my - 1) * wm + mx], bx, 3) : 2;
+  return min(a, b);
+}
+
+// An I_NxN macroblock's mb_type through mb_qp_delta: ue(0) (ue(5) in a P slice), per block in luma4x4BlkIdx order
+// prev_intra4x4_pred_mode_flag or 0 and rem_intra4x4_pred_mode u(3), intra_chroma_pred_mode, coded_block_pattern
+// (intra column), mb_qp_delta; returns its bits, writes them when s has a buffer.
+__device__ int i4_header(const int* info, const uint64_t* modes, int wm, int mx, int my, bool is_p, BitSink& s) {
+  const int n0 = s.n, me = info[my * wm + mx];
+  const uint64_t own = modes[my * wm + mx];
+  s.u(is_p ? 6 : 1, is_p ? 5 : 1);
+  for (int k = 0; k < 16; k++) {
+    const int bx = c_blk_x[k], by = c_blk_y[k];
+    const int m = mode_at(own, bx, by), pm = i4_pred_mode(own, info, modes, wm, mx, my, bx, by);
+    if (m == pm) s.u(1, 1);
+    else s.u(m < pm ? m : m - 1, 4);
+  }
+  const int cmode = (me >> 2) & 3, cbp = ((me >> 9) & 15) | ((me >> 4) & 3) << 4, code = c_intra_cbp[cbp];
+  s.u(cmode + 1, ue_bits(cmode));
+  s.u(code + 1, ue_bits(code));
+  if (cbp) s.u(1, 1);                            // mb_qp_delta 0
+  return s.n - n0;
+}
+
+// 8.3.1.2: the prediction of Intra4x4PredMode `mode` at (x, y) of a 4x4 block from its edge e: e[3 - j] = p[-1, j],
+// e[4] = p[-1, -1], e[5 + i] = p[i, -1] (i = 0 .. 7, p[4..7, -1] already substituted when unavailable); dc is mode 2's.
+__device__ __forceinline__ int pred4(const int* e, int mode, int dc, int x, int y) {
+  auto P = [&](int i, int j) { return j < 0 ? e[5 + i] : e[3 - j]; };   // p[i, j], i = -1 or j = -1
+  auto f3 = [](int a, int b, int c) { return (a + 2 * b + c + 2) >> 2; };
+  auto f2 = [](int a, int b) { return (a + b + 1) >> 1; };
+  switch (mode) {
+    case 0: return P(x, -1);
+    case 1: return P(-1, y);
+    case 2: return dc;
+    case 3: return x == 3 && y == 3 ? (P(6, -1) + 3 * P(7, -1) + 2) >> 2 : f3(P(x + y, -1), P(x + y + 1, -1), P(x + y + 2, -1));
+    case 4:
+      if (x > y) return f3(P(x - y - 2, -1), P(x - y - 1, -1), P(x - y, -1));
+      if (x < y) return f3(P(-1, y - x - 2), P(-1, y - x - 1), P(-1, y - x));
+      return f3(P(0, -1), P(-1, -1), P(-1, 0));
+    case 5: {
+      const int z = 2 * x - y;
+      if (z >= 0 && !(z & 1)) return f2(P(x - (y >> 1) - 1, -1), P(x - (y >> 1), -1));
+      if (z > 0) return f3(P(x - (y >> 1) - 2, -1), P(x - (y >> 1) - 1, -1), P(x - (y >> 1), -1));
+      if (z == -1) return f3(P(-1, 0), P(-1, -1), P(0, -1));
+      return f3(P(-1, y - 1), P(-1, y - 2), P(-1, y - 3));
+    }
+    case 6: {
+      const int z = 2 * y - x;
+      if (z >= 0 && !(z & 1)) return f2(P(-1, y - (x >> 1) - 1), P(-1, y - (x >> 1)));
+      if (z > 0) return f3(P(-1, y - (x >> 1) - 2), P(-1, y - (x >> 1) - 1), P(-1, y - (x >> 1)));
+      if (z == -1) return f3(P(-1, 0), P(-1, -1), P(0, -1));
+      return f3(P(x - 1, -1), P(x - 2, -1), P(x - 3, -1));
+    }
+    case 7:
+      if (!(y & 1)) return f2(P(x + (y >> 1), -1), P(x + (y >> 1) + 1, -1));
+      return f3(P(x + (y >> 1), -1), P(x + (y >> 1) + 1, -1), P(x + (y >> 1) + 2, -1));
+    default: {
+      const int z = x + 2 * y;
+      if (z > 5) return P(-1, 3);
+      if (z == 5) return (P(-1, 2) + 3 * P(-1, 3) + 2) >> 2;
+      if (!(z & 1)) return f2(P(-1, y + (x >> 1)), P(-1, y + (x >> 1) + 1));
+      return f3(P(-1, y + (x >> 1)), P(-1, y + (x >> 1) + 1), P(-1, y + (x >> 1) + 2));
+    }
+  }
 }
 
 // ---- the macroblock kernel ---------------------------------------------------------------------------------------
@@ -419,6 +517,14 @@ struct MbShared {
   int c9[9];             // P: the costs of a refinement's candidates
   uint8_t win[WIN * WIN];// P: the reference samples around the macroblock, coordinates clamped to the picture
   int maxlev, bits, lmode, cmode, cbpl, cbpc, pcm, inter, key, mvx, mvy, icost;
+};
+
+// The I_NxN candidate's part (h264_mb_kernel<true> only); its levels and TotalCoeff go to lev[0..15] / tot[0..15].
+struct MbSharedI4 : MbShared {
+  int r4[256];           // the reconstruction, raster
+  int c4[2][9];          // SATD of the current step's (block, mode) pairs
+  uint64_t own;          // the chosen modes, raster block k in bits 4k .. 4k + 3
+  int sum4, mbits4, max4, nxn;   // sum of the blocks' costs, their mode bits, the largest |level|, I_NxN chosen
 };
 
 __device__ int predict(const MbShared& s, int plane, int mode, int x, int y) {
@@ -588,9 +694,22 @@ __device__ __forceinline__ bool line_mb(int d, int slope, int k, int wm, int hm,
 
 // One launch per step of the wavefront over (frame, line): frame f runs line step - lag f (lag 0 when every frame is
 // an IDR picture; LAG when a frame refers to the one before it, LAG_DB when it refers to the deblocked one).
+//
+// I4: the I_NxN candidate (Intra_4x4, 8.3.1) beside I_16x16.  Its 16 blocks run in decode order as a wavefront over
+// bx + 2 by (10 steps, at most 2 blocks a step; a block's left, top, top-left and top-right lie on earlier steps):
+// one thread per (block, mode) gives every available mode SATD(src - pred); one thread per block adds lambda * its
+// mode bits (1 for predIntra4x4PredMode, else 4), takes the least cost (ties: the lower mode), and transforms,
+// quantises (intra dead zone, all 16 coefficients) and reconstructs the block before the next step predicts from
+// it.  Block 5 never takes modes 3 or 7, the only ones that read macroblock C (above right): C lies on the current
+// macroblock's own anti-diagonal, so without them the wavefronts, lags and launches are those of the I_16x16 streams.
+// I_NxN replaces I_16x16 when the sum of its block costs + I4_BIAS * lambda is below I_16x16's least luma SATD; in
+// a P picture the cheaper intra candidate meets the inter one through INTRA_BIAS as I_16x16 alone did.  I_NxN falls
+// back to I_PCM on MAX_LEVEL and PCM_BITS as I_16x16 does: its bits, like every coded macroblock's, never exceed
+// PCM_BITS, so gab200_h264_bound / gab200_h264_p_bound and the slot strides hold for these streams as they are.
+template <bool I4>
 __global__ void __maxnreg__(80) h264_mb_kernel(int step, int lag, int slope, int f_lo, int qp, uint8_t* scratch,
                                                       const uint8_t* state, Layout l) {
-  __shared__ MbShared s;
+  __shared__ std::conditional_t<I4, MbSharedI4, MbShared> s;
   const int f = f_lo + blockIdx.y, t = threadIdx.x;
   int mx, my;
   if (!line_mb(step - lag * f, slope, blockIdx.x, l.wm, l.hm, mx, my)) return;
@@ -681,6 +800,104 @@ __global__ void __maxnreg__(80) h264_mb_kernel(int step, int lag, int slope, int
     }
     atomicAdd(&s.cost[plane == 0 ? mode : 4 + mode], satd4(r));
   }
+  if constexpr (I4) {
+    if (t == 0) { s.own = 0; s.sum4 = 0; s.mbits4 = 0; s.max4 = 0; }
+    const int* info = reinterpret_cast<const int*>(base + l.info);
+    const uint64_t* modes = reinterpret_cast<const uint64_t*>(base + l.modes);
+    const int L = lambda_of(qp);
+    // the 4x4 block's edge (see pred4) and which of its samples exist, in the order left, top, top-right
+    auto edge = [&](int bx, int by, int* e, bool& al, bool& at) {
+      al = bx > 0 || has_l;
+      at = by > 0 || has_t;
+      const bool atr = bx < 3 && (by == 0 ? has_t : blk_idx(bx + 1, by - 1) < blk_idx(bx, by));
+      const int x0 = 4 * bx, y0 = 4 * by;
+      auto p = [&](int x, int y) {   // the reconstructed sample at (x, y) of the macroblock, x, y >= -1
+        return y < 0 ? (x < 0 ? s.tl[0] : s.top[x]) : x < 0 ? s.left[y] : s.r4[16 * y + x];
+      };
+      for (int j = 0; j < 4; j++) e[3 - j] = al ? p(x0 - 1, y0 + j) : 0;
+      e[4] = al && at ? p(x0 - 1, y0 - 1) : 0;
+      for (int i = 0; i < 8; i++) e[5 + i] = at ? p(i < 4 || atr ? x0 + i : x0 + 3, y0 - 1) : 0;
+    };
+    auto dc4 = [](const int* e, bool al, bool at) {
+      const int sl = e[0] + e[1] + e[2] + e[3], st = e[5] + e[6] + e[7] + e[8];
+      return al && at ? (sl + st + 4) >> 3 : at ? (st + 2) >> 2 : al ? (sl + 2) >> 2 : 128;
+    };
+    for (int st = 0; st < 10; st++) {
+      const int by_lo = max(0, (st - 2) / 2);   // blocks (st - 2 by, by) with 0 <= st - 2 by <= 3
+      __syncthreads();
+      if (t < 18) {
+        const int by = by_lo + t / 9, bx = st - 2 * by, m = t % 9;
+        if (by <= 3 && bx >= 0) {
+          int e[13];
+          bool al, at;
+          edge(bx, by, e, al, at);
+          // 8.3.1.2's availability; block 5 never takes modes 3 and 7 (macroblock C)
+          const bool ok = m == 2 || (m == 1 || m == 8 ? al
+                                     : m == 0 ? at
+                                     : m == 3 || m == 7 ? at && !(bx == 3 && by == 0)
+                                     : al && at);
+          int cost = INT_MAX;
+          if (ok) {
+            const int dc = dc4(e, al, at);
+            int r[16];
+            for (int i = 0; i < 16; i++)
+              r[i] = s.src[16 * (4 * by + (i >> 2)) + 4 * bx + (i & 3)] - pred4(e, m, dc, i & 3, i >> 2);
+            cost = satd4(r);
+          }
+          s.c4[t / 9][m] = cost;
+        }
+      }
+      __syncthreads();
+      if (t < 2) {
+        const int by = by_lo + t, bx = st - 2 * by;
+        if (by <= 3 && bx >= 0) {
+          const int pm = i4_pred_mode(s.own, info, modes, l.wm, mx, my, bx, by);
+          int m = 0, best = INT_MAX;
+          for (int k = 0; k < 9; k++) {
+            if (s.c4[t][k] == INT_MAX) continue;
+            const int c = s.c4[t][k] + L * (k == pm ? 1 : 4);
+            if (c < best) { best = c; m = k; }
+          }
+          int e[13];
+          bool al, at;
+          edge(bx, by, e, al, at);
+          const int dc = dc4(e, al, at), b = 4 * by + bx;
+          int pr[16], x[16], w[16];
+          for (int i = 0; i < 16; i++) {
+            pr[i] = pred4(e, m, dc, i & 3, i >> 2);
+            x[i] = s.src[16 * (4 * by + (i >> 2)) + 4 * bx + (i & 3)] - pr[i];
+          }
+          for (int i = 0; i < 4; i++)      // CF x CF^T
+            for (int j = 0; j < 4; j++) {
+              const int a = x[j], b1 = x[4 + j], c = x[8 + j], d = x[12 + j];
+              w[i * 4 + j] = i == 0 ? a + b1 + c + d : i == 1 ? 2 * a + b1 - c - 2 * d
+                             : i == 2 ? a - b1 - c + d : a - 2 * b1 + 2 * c - d;
+            }
+          const int qbits = 15 + qp / 6, fq = (1 << qbits) / 3;
+          int nz = 0, mx_ = 0, dq[16];
+          for (int i = 0; i < 4; i++) {
+            const int a = w[4 * i], b1 = w[4 * i + 1], c = w[4 * i + 2], d = w[4 * i + 3];
+            const int w4[4] = {a + b1 + c + d, 2 * a + b1 - c - 2 * d, a - b1 - c + d, a - 2 * b1 + 2 * c - d};
+            for (int j = 0; j < 4; j++) {
+              const int k = 4 * i + j, lv = quant(w4[j], c_mf[qp % 6][pos_class(k)], qbits, fq);
+              const int ls = 16 * c_v[qp % 6][pos_class(k)];
+              s.lev[b][k] = lv;
+              nz += lv != 0;
+              mx_ = max(mx_, abs(lv));
+              dq[k] = qp >= 24 ? (lv * ls) << (qp / 6 - 4) : (lv * ls + (1 << (3 - qp / 6))) >> (4 - qp / 6);
+            }
+          }
+          idct4(dq);
+          for (int i = 0; i < 16; i++) s.r4[16 * (4 * by + (i >> 2)) + 4 * bx + (i & 3)] = clip255(pr[i] + dq[i]);
+          s.tot[b] = nz;
+          atomicMax(&s.max4, mx_);
+          atomicAdd(&s.sum4, best);
+          atomicAdd(&s.mbits4, m == pm ? 1 : 4);
+          atomicOr(reinterpret_cast<unsigned long long*>(&s.own), (unsigned long long)m << (4 * b));
+        }
+      }
+    }
+  }
   __syncthreads();
   if (t == 0) {
     const bool lav[4] = {has_t, has_l, true, has_t && has_l};
@@ -692,10 +909,21 @@ __global__ void __maxnreg__(80) h264_mb_kernel(int step, int lag, int slope, int
     }
     s.lmode = lm;
     s.cmode = cm;
-    s.inter = is_p && !(s.cost[lm] + INTRA_BIAS * lambda_of(qp) < s.icost);
+    int intra = s.cost[lm];
+    if constexpr (I4) {
+      s.nxn = s.sum4 + I4_BIAS * lambda_of(qp) < intra;
+      if (s.nxn) intra = s.sum4 + I4_BIAS * lambda_of(qp);
+    }
+    s.inter = is_p && !(intra + INTRA_BIAS * lambda_of(qp) < s.icost);
+    if constexpr (I4) {
+      s.nxn = s.nxn && !s.inter;
+      if (s.nxn) s.maxlev = s.max4;
+    }
   }
   __syncthreads();
   const bool inter = s.inter;
+  bool nxn = false;
+  if constexpr (I4) nxn = s.nxn;
   for (int i = t; i < 384; i += 128) {
     if (inter) s.pred[i] = s.ipred[i];
     else if (i < 256) s.pred[i] = predict(s, 0, s.lmode, i & 15, i >> 4);
@@ -704,8 +932,9 @@ __global__ void __maxnreg__(80) h264_mb_kernel(int step, int lag, int slope, int
   __syncthreads();
 
   // forward transform and quantisation: one thread per 4x4 block (16 luma raster, 4 Cb, 4 Cr); the dead zone is
-  // f = 2^qbits / 3 for intra, 2^qbits / 6 for inter; an inter luma block keeps its DC coefficient
-  if (t < 24) {
+  // f = 2^qbits / 3 for intra, 2^qbits / 6 for inter; an inter luma block keeps its DC coefficient (an I_NxN
+  // macroblock's luma blocks are already coded)
+  if (t < 24 && !(nxn && t < 16)) {
     const bool luma = t < 16;
     const int bx = luma ? (t & 3) : (t & 1), by = luma ? (t >> 2) : ((t >> 1) & 1);
     const int n = luma ? 16 : 8, so = luma ? 0 : 256 + 64 * ((t - 16) / 4);
@@ -741,7 +970,7 @@ __global__ void __maxnreg__(80) h264_mb_kernel(int step, int lag, int slope, int
   __syncthreads();
 
   // DC transforms, quantisation and their dequantisation (8.5.10, 8.5.11)
-  if (t == 0 && !inter) {
+  if (t == 0 && !inter && !nxn) {
     int a[16], b[16];
     for (int i = 0; i < 16; i++) a[i] = s.w[i][0];   // [by * 4 + bx]
     // b = HD a HD, >> 1
@@ -792,7 +1021,7 @@ __global__ void __maxnreg__(80) h264_mb_kernel(int step, int lag, int slope, int
   __syncthreads();
 
   // reconstruction: dequantise, inverse transform, add the prediction
-  if (t < 24) {
+  if (t < 24 && !(nxn && t < 16)) {
     const bool luma = t < 16;
     const int q = luma ? qp : qpc;
     int dq[16];
@@ -813,7 +1042,7 @@ __global__ void __maxnreg__(80) h264_mb_kernel(int step, int lag, int slope, int
     }
     for (int i = 16; i < 24; i++) ac += s.tot[i];
     for (int i = 0; i < 8; i++) dcc |= s.cdc[i / 4][i % 4];
-    s.cbpl = inter ? m8 : al ? 15 : 0;
+    s.cbpl = inter || nxn ? m8 : al ? 15 : 0;
     s.cbpc = ac ? 2 : dcc ? 1 : 0;
   }
   __syncthreads();
@@ -823,15 +1052,15 @@ __global__ void __maxnreg__(80) h264_mb_kernel(int step, int lag, int slope, int
 
   // CAVLC bit count, one thread per residual block: 0 luma DC, 1..16 luma AC (luma4x4BlkIdx order; an inter block's
   // 16 coefficients), 17/18 Cb/Cr DC, 19..26 Cb AC, 23..26 Cr AC; the levels in scan order go to the writer
-  const int info = s.lmode | s.cmode << 2 | s.cbpc << 4 | (!inter && s.cbpl ? 1 : 0) << 6 | inter << 8 |
-                   (inter ? s.cbpl : 0) << 9;
+  const int info = s.lmode | s.cmode << 2 | s.cbpc << 4 | (!inter && !nxn && s.cbpl ? 1 : 0) << 6 | inter << 8 |
+                   (inter || nxn ? s.cbpl : 0) << 9 | nxn << 14;
   if (t < BLOCKS) {
     int c[16], plane, x, y, maxn;
     block_geom(t, mx, my, plane, x, y, maxn);
     if (t == 0) for (int k = 0; k < 16; k++) c[k] = s.dc[c_zigzag[k]];
     else if (t <= 16) {
       const int b = c_blk_y[t - 1] * 4 + c_blk_x[t - 1];
-      if (inter) maxn = 16;
+      if (inter || nxn) maxn = 16;
       for (int k = 0; k < maxn; k++) c[k] = s.lev[b][c_zigzag[k + 16 - maxn]];
     }
     else if (t <= 18) for (int k = 0; k < 4; k++) c[k] = s.cdc[t - 17][k];
@@ -846,7 +1075,13 @@ __global__ void __maxnreg__(80) h264_mb_kernel(int step, int lag, int slope, int
   }
   __syncthreads();
   if (t == 0) {
-    const int bits = s.bits + mb_header_bits(info, is_p);
+    int hb = mb_header_bits(info, is_p);
+    if constexpr (I4) {
+      reinterpret_cast<uint64_t*>(base + l.modes)[mb] = s.own;
+      const int cbp = s.cbpl | s.cbpc << 4;
+      if (nxn) hb = (is_p ? 5 : 1) + s.mbits4 + ue_bits(s.cmode) + ue_bits(c_intra_cbp[cbp]) + (cbp ? 1 : 0);
+    }
+    const int bits = s.bits + hb;
     s.pcm = s.maxlev > MAX_LEVEL || bits > PCM_BITS;
     reinterpret_cast<int*>(base + l.info)[mb] = s.pcm ? (1 << 7) : info;
     reinterpret_cast<int*>(base + l.bits)[mb] = s.pcm ? 0 : bits;
@@ -857,7 +1092,9 @@ __global__ void __maxnreg__(80) h264_mb_kernel(int step, int lag, int slope, int
   for (int i = t; i < 384; i += 128) {
     int v;
     if (s.pcm) v = s.src[i];
-    else if (i < 256) v = clip255(s.pred[i] + s.w[((i >> 4) >> 2) * 4 + ((i & 15) >> 2)][((i >> 4) & 3) * 4 + (i & 3)]);
+    else if (nxn && i < 256) {
+      if constexpr (I4) v = s.r4[i];
+    } else if (i < 256) v = clip255(s.pred[i] + s.w[((i >> 4) >> 2) * 4 + ((i & 15) >> 2)][((i >> 4) & 3) * 4 + (i & 3)]);
     else {
       const int p = (i - 256) / 64, j = (i - 256) % 64, x = j & 7, y = j >> 3;
       v = clip255(s.pred[i] + s.w[16 + 4 * p + (y >> 2) * 2 + (x >> 2)][(y & 3) * 4 + (x & 3)]);
@@ -1190,13 +1427,13 @@ __global__ void __launch_bounds__(128) h264_write_kernel(uint8_t* scratch, Layou
     }
     return;
   }
-  const bool inter = (info >> 8) & 1;
+  const bool inter = (info >> 8) & 1, nxn = (info >> 14) & 1;
   const uint8_t* tot = base + l.tot;
   int c[16], plane = 0, x = 0, y = 0, maxn = 0, nc = 0, n = 0;
   const bool present = lane < BLOCKS && block_present(lane, info);
   if (present) {
     block_geom(lane, mx, my, plane, x, y, maxn);
-    if (inter && lane >= 1 && lane <= 16) maxn = 16;
+    if ((inter || nxn) && lane >= 1 && lane <= 16) maxn = 16;
     const int16_t* lev = reinterpret_cast<const int16_t*>(base + l.lev) + ((int64_t)mb * BLOCKS + lane) * 16;
     for (int k = 0; k < 16; k++) c[k] = k < maxn ? lev[k] : 0;
     nc = plane < 0 ? -1 : nc_of(tot, l, plane, x, y);
@@ -1222,6 +1459,11 @@ __global__ void __launch_bounds__(128) h264_write_kernel(uint8_t* scratch, Layou
       h.u(code + 1, ue_bits(code));
       if (cbp) h.u(1, 1);                        // mb_qp_delta 0
     }
+  } else if (nxn) {
+    const int* infos = reinterpret_cast<const int*>(base + l.info);
+    const uint64_t* modes = reinterpret_cast<const uint64_t*>(base + l.modes);
+    BitSink h{lane == 0 ? raw : nullptr, pos, 0};
+    hb = i4_header(infos, modes, l.wm, mx, my, is_p, h);
   } else if (lane == 0) {
     const int mbt = i16_mb_type(info, is_p), cmode = (info >> 2) & 3;
     BitSink h{raw, pos, 0};
@@ -1401,9 +1643,9 @@ size_t h264_state_bytes(int H, int W) {
   return (size_t)(256 + align256((int64_t)((W + 15) / 16) * ((H + 15) / 16) * 384));
 }
 
-size_t h264_scratch_bytes(int64_t frames, int H, int W, bool deblock) {
+size_t h264_scratch_bytes(int64_t frames, int H, int W, bool deblock, bool intra4x4) {
   if (frames <= 0 || frames > 65535 || h264_bound(W, H) < 0) return 0;
-  return (size_t)(frames * layout(H, W, deblock).stride);
+  return (size_t)(frames * layout(H, W, deblock, intra4x4).stride);
 }
 
 int32_t h264_parameter_sets(int W, int H, int qp, int fps_num, int fps_den, int gop, uint8_t* out, int64_t cap) {
@@ -1479,9 +1721,10 @@ int32_t h264_parameter_sets(int W, int H, int qp, int fps_num, int fps_den, int 
   return (int32_t)need;
 }
 
-void launch_h264_encode(int frames, int H, int W, int qp, int gop, bool deblock, const uint8_t* rgb, uint8_t* state,
-                        void* scratch, uint8_t* out, int64_t out_stride, int64_t* out_len, cudaStream_t stream) {
-  const Layout l = layout(H, W, deblock);
+void launch_h264_encode(int frames, int H, int W, int qp, int gop, bool deblock, bool intra4x4, const uint8_t* rgb,
+                        uint8_t* state, void* scratch, uint8_t* out, int64_t out_stride, int64_t* out_len,
+                        cudaStream_t stream) {
+  const Layout l = layout(H, W, deblock, intra4x4);
   uint8_t* s = static_cast<uint8_t*>(scratch);
   const unsigned F = (unsigned)frames;
   h264_convert_kernel<<<dim3((unsigned)((64 * l.nmb + 255) / 256), F), 256, 0, stream>>>(rgb, s, l);
@@ -1510,8 +1753,9 @@ void launch_h264_encode(int frames, int H, int W, int qp, int gop, bool deblock,
     int f_lo, f_hi;
     int n = frames_at(k, 0, D, slope, f_lo, f_hi);
     if (n > 0) {
-      h264_mb_kernel<<<dim3((unsigned)n, (unsigned)(f_hi - f_lo + 1)), 128, 0, stream>>>(k, lag, slope, f_lo, qp, s,
-                                                                                       state, l);
+      const dim3 grid((unsigned)n, (unsigned)(f_hi - f_lo + 1));
+      if (intra4x4) h264_mb_kernel<true><<<grid, 128, 0, stream>>>(k, lag, slope, f_lo, qp, s, state, l);
+      else h264_mb_kernel<false><<<grid, 128, 0, stream>>>(k, lag, slope, f_lo, qp, s, state, l);
       count_launch();
     }
     if (!deblock) continue;

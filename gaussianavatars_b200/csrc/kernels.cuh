@@ -249,11 +249,12 @@ void launch_png_copy(int views, const uint8_t* src, int64_t src_stride, const in
 int64_t h264_bound(int W, int H);
 int64_t h264_p_bound(int W, int H);
 int h264_level_idc(int W, int H, int fps_num, int fps_den);
-size_t h264_scratch_bytes(int64_t frames, int H, int W, bool deblock = false);
+size_t h264_scratch_bytes(int64_t frames, int H, int W, bool deblock = false, bool intra4x4 = false);
 size_t h264_state_bytes(int H, int W);
 int32_t h264_parameter_sets(int W, int H, int qp, int fps_num, int fps_den, int gop, uint8_t* out, int64_t cap);
-void launch_h264_encode(int frames, int H, int W, int qp, int gop, bool deblock, const uint8_t* rgb, uint8_t* state,
-                        void* scratch, uint8_t* out, int64_t out_stride, int64_t* out_len, cudaStream_t stream);
+void launch_h264_encode(int frames, int H, int W, int qp, int gop, bool deblock, bool intra4x4, const uint8_t* rgb,
+                        uint8_t* state, void* scratch, uint8_t* out, int64_t out_stride, int64_t* out_len,
+                        cudaStream_t stream);
 
 // png_decode.cu
 int64_t png_decode_stride(int H, int W);

@@ -270,12 +270,13 @@ class CameraPath:
 def export_trajectory(pc, path: CameraPath, out_dir, *, bg: torch.Tensor, mesh_opacity: Optional[float] = None,
                       face_colors: Optional[torch.Tensor] = None, scaling_modifier: float = 1.0, video=None,
                       gop: int = 25, fps: int = 25, qp: int = 20, batch: int = 16, ref_json=None,
-                      capacity: Optional[int] = None, deblock: bool = False) -> dict:
+                      capacity: Optional[int] = None, deblock: bool = False, intra4x4: bool = False) -> dict:
     """What the viewer's "export traj" button writes, rendered on the device: out_dir/00000.png ... (one PNG per frame
     of the path, the viewer's bytes: GraphedRender(quantize="viewer", png=True)) and out_dir/trajectory.json
     (path.trajectory_json(ref_json)).  mesh_opacity: the viewer's "show mesh" at that opacity (its default colour
     alpha is 0.5), face_colors its face colours; scaling_modifier its "Scale modifier" slider.  video: a file name or
-    binary file object, also written as an MP4 of the same frames (video.VideoWriter at fps, qp, gop and deblock).
+    binary file object, also written as an MP4 of the same frames (video.VideoWriter at fps, qp, gop, deblock and
+    intra4x4).
 
     The frames are played by one scheduled GraphedRender, `batch` replays at a time with no host input; each batch
     ends in one synchronisation, after which its PNG files are written from the pinned ring and its frames join the
@@ -288,6 +289,8 @@ def export_trajectory(pc, path: CameraPath, out_dir, *, bg: torch.Tensor, mesh_o
         raise ValueError(f"batch must be a positive int, got {batch!r}")
     if not isinstance(deblock, bool):
         raise ValueError(f"deblock must be a bool, got {deblock!r}")
+    if not isinstance(intra4x4, bool):
+        raise ValueError(f"intra4x4 must be a bool, got {intra4x4!r}")
     num_timesteps = int(pc.flame_param["expr"].shape[0]) if getattr(pc, "flame", None) is not None else None
     if (path.num_timesteps is None) != (num_timesteps is None):
         raise ValueError("the path carries FLAME timesteps exactly when the model has a FLAME head: build it with "
@@ -303,8 +306,8 @@ def export_trajectory(pc, path: CameraPath, out_dir, *, bg: torch.Tensor, mesh_o
     view = GraphedRender(pc, path.W, path.H, bg, outputs="u8", scaling_modifier=scaling_modifier, host_slots=B,
                          capacity=capacity, mesh_opacity=mesh_opacity, face_colors=face_colors, png=True,
                          quantize="viewer", schedule=sched)
-    writer = VideoWriter(video, path.W, path.H, fps=fps, qp=qp, batch=B, device=device, gop=gop, deblock=deblock) \
-        if video is not None else None
+    writer = VideoWriter(video, path.W, path.H, fps=fps, qp=qp, batch=B, device=device, gop=gop, deblock=deblock,
+                         intra4x4=intra4x4) if video is not None else None
     frames = torch.empty((B, path.H, path.W, 3), dtype=torch.uint8, device=device) if writer is not None else None
     try:
         view.capture()

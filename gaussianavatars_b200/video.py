@@ -5,7 +5,7 @@ renders.mp4` makes of the PNG files it wrote, without the PNG files.
         for t in timesteps:
             player.run(...)
             vw.add(player.display)                        # CUDA (H,W,3) or (K,H,W,3) uint8
-    data = encode_video(frames, fps=25, qp=20, gop=1, deblock=False)   # a whole MP4 in memory
+    data = encode_video(frames, fps=25, qp=20, gop=1, deblock=False, intra4x4=False)   # a whole MP4 in memory
 
 The frames are encoded on the device (csrc/h264.cu, include/gab200_rasterizer.h gab200_h264_encode and
 gab200_h264_encode_stream): H.264 Constrained Baseline, one fixed QP, BT.601 limited-range 4:2:0.  With gop=1 (the
@@ -13,7 +13,9 @@ default) every frame is an IDR picture; with gop=N every N-th frame is, and the 
 the frame before them, which is far smaller when successive frames look alike (a fixed camera).  Deblocking is off by
 default, so a decoder outputs the encoder's reconstruction as it is; with deblock=True every slice turns the in-loop
 deblocking filter on, and the encoder filters each picture as a decoder does (gab200_h264_encode_deblocked), the P
-pictures predicting from the filtered one.  Only the compressed samples cross to the host, through a ring of pinned
+pictures predicting from the filtered one.  With intra4x4=True an intra macroblock may also be I_NxN, nine
+directional predictions per 4x4 block in place of one per 16x16 block (gab200_h264_encode_flags); the parameter sets
+are the same, so every decoder that plays the other files plays these.  Only the compressed samples cross to the host, through a ring of pinned
 slots; the file is ftyp | mdat | moov, muxed here, with an stss box listing the IDR frames when gop > 1.  The bytes are
 deterministic and differ from libx264's.
 """
@@ -32,6 +34,8 @@ from . import _native as N
 from .png import launch_copy
 
 MAX_QP = 51
+H264_DEBLOCK = 1          # include/gab200_rasterizer.h GAB200_H264_DEBLOCK
+H264_INTRA4X4 = 2         # GAB200_H264_INTRA4X4
 
 
 def video_bound(width: int, height: int) -> int:
@@ -62,6 +66,12 @@ def _check_deblock(deblock) -> bool:
     if not isinstance(deblock, bool):
         raise ValueError(f"deblock must be a bool, got {deblock!r}")
     return deblock
+
+
+def _check_intra4x4(intra4x4) -> bool:
+    if not isinstance(intra4x4, bool):
+        raise ValueError(f"intra4x4 must be a bool, got {intra4x4!r}")
+    return intra4x4
 
 
 def _check_qp(qp) -> int:
@@ -146,6 +156,23 @@ def launch_encode_deblocked(frames: torch.Tensor, qp: int, gop: int, state, scra
             "gab200_h264_encode_deblocked")
 
 
+def launch_encode_flags(frames: torch.Tensor, qp: int, gop: int, deblock: bool, intra4x4: bool, state, scratch_buf,
+                        out: torch.Tensor, out_len: torch.Tensor):
+    """Enqueues gab200_h264_encode_flags on the current stream: launch_encode_deblocked's samples (the filter only
+    when deblock) with I_NxN macroblocks when intra4x4, scratch from flags_scratch.  state may be None when gop is 1.
+    Reads nothing on the host: capturable."""
+    K, H, W = check_frames(frames)
+    stream = C.c_void_p(torch.cuda.current_stream(frames.device).cuda_stream)
+    N.check(N.lib().gab200_h264_encode_flags(K, H, W, qp, gop, _flags(deblock, intra4x4), frames.data_ptr(),
+                                             None if state is None else state.data_ptr(), scratch_buf.data_ptr(),
+                                             out.data_ptr(), out.stride(0), out_len.data_ptr(), stream),
+            "gab200_h264_encode_flags")
+
+
+def _flags(deblock: bool, intra4x4: bool) -> int:
+    return (H264_DEBLOCK if deblock else 0) | (H264_INTRA4X4 if intra4x4 else 0)
+
+
 def state_buffer(H: int, W: int, device) -> torch.Tensor:
     """A zeroed stream state: its next frame is an IDR picture."""
     n = int(N.lib().gab200_h264_state_bytes(H, W))
@@ -165,6 +192,13 @@ def deblocked_scratch(K: int, H: int, W: int, gop: int, device) -> torch.Tensor:
     n = int(N.lib().gab200_h264_deblocked_scratch_bytes(K, H, W, gop))
     if n == 0:
         raise ValueError(f"no deblocked H.264 encode of {K} frames of {W}x{H} with gop {gop}")
+    return torch.empty(n, dtype=torch.uint8, device=device)
+
+
+def flags_scratch(K: int, H: int, W: int, gop: int, deblock: bool, intra4x4: bool, device) -> torch.Tensor:
+    n = int(N.lib().gab200_h264_flags_scratch_bytes(K, H, W, gop, _flags(deblock, intra4x4)))
+    if n == 0:
+        raise ValueError(f"no H.264 encode of {K} frames of {W}x{H} with gop {gop}")
     return torch.empty(n, dtype=torch.uint8, device=device)
 
 
@@ -229,16 +263,18 @@ class VideoWriter:
     track's timescale is its numerator, each sample lasts its denominator).  gop: every gop-th frame, the first
     included, is an IDR picture and the others P pictures (1: every frame an IDR picture); the writer owns the
     stream's state on the device, so a batch may start anywhere in a GOP.  deblock: the in-loop deblocking filter on
-    in every slice of the stream (a bool; the writer keeps one mode for its whole stream)."""
+    in every slice of the stream (a bool; the writer keeps one mode for its whole stream).  intra4x4: intra
+    macroblocks may also be I_NxN, each 4x4 block predicted on its own (a bool, for the whole stream)."""
 
     RING = 3
 
     def __init__(self, path, width: int, height: int, fps=25, qp: int = 20, batch: int = 16, device=None, gop: int = 1,
-                 deblock: bool = False):
+                 deblock: bool = False, intra4x4: bool = False):
         self.fps = _check_fps(fps)
         self.qp = _check_qp(qp)
         self.gop = _check_gop(gop)
         self.deblock = _check_deblock(deblock)
+        self.intra4x4 = _check_intra4x4(intra4x4)
         if isinstance(batch, bool) or not isinstance(batch, int) or not 1 <= batch <= 65535:
             raise ValueError(f"batch must be an int in 1..65535, got {batch!r}")
         self.W, self.H = int(width), int(height)
@@ -250,8 +286,12 @@ class VideoWriter:
         self.batch = batch
         with torch.cuda.device(self.device):
             self._frames = torch.empty((batch, self.H, self.W, 3), dtype=torch.uint8, device=self.device)
-            self._scratch = deblocked_scratch(batch, self.H, self.W, self.gop, self.device) if self.deblock else \
-                scratch(batch, self.H, self.W, self.device)
+            if self.intra4x4:
+                self._scratch = flags_scratch(batch, self.H, self.W, self.gop, self.deblock, True, self.device)
+            elif self.deblock:
+                self._scratch = deblocked_scratch(batch, self.H, self.W, self.gop, self.device)
+            else:
+                self._scratch = scratch(batch, self.H, self.W, self.device)
             self._out = torch.empty((batch, self.stride), dtype=torch.uint8, device=self.device)
             self._out_len = torch.empty(batch, dtype=torch.int64, device=self.device)
             self._state = state_buffer(self.H, self.W, self.device) if self.gop > 1 else None
@@ -302,7 +342,10 @@ class VideoWriter:
         self._next_slot = (slot + 1) % self.RING
         if len(self._pending) == self.RING:
             self._drain(1)
-        if self.deblock:
+        if self.intra4x4:
+            launch_encode_flags(self._frames[:n], self.qp, self.gop, self.deblock, True, self._state, self._scratch,
+                                self._out, self._out_len)
+        elif self.deblock:
             launch_encode_deblocked(self._frames[:n], self.qp, self.gop, self._state, self._scratch, self._out,
                                     self._out_len)
         elif self._state is None:
@@ -356,11 +399,13 @@ class VideoWriter:
 
 
 @torch.no_grad()
-def encode_video(frames: torch.Tensor, fps=25, qp: int = 20, gop: int = 1, deblock: bool = False) -> bytes:
+def encode_video(frames: torch.Tensor, fps=25, qp: int = 20, gop: int = 1, deblock: bool = False,
+                 intra4x4: bool = False) -> bytes:
     """A whole MP4 of a CUDA uint8 (H,W,3) frame or (K,H,W,3) clip, in memory."""
+    _check_intra4x4(intra4x4)
     K, H, W = check_frames(frames)
     buf = io.BytesIO()
     with VideoWriter(buf, W, H, fps=fps, qp=qp, batch=min(K, 16), device=frames.device, gop=gop,
-                     deblock=deblock) as vw:
+                     deblock=deblock, intra4x4=intra4x4) as vw:
         vw.add(frames)
     return buf.getvalue()

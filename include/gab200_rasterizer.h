@@ -653,6 +653,25 @@ int32_t gab200_h264_encode_deblocked(int32_t frames, int32_t height, int32_t wid
                                      const uint8_t* rgb, void* state, void* scratch, uint8_t* out, int64_t out_stride,
                                      int64_t* out_len, void* stream);
 
+/* The coding options of gab200_h264_encode_flags, OR-ed into its flags word. */
+#define GAB200_H264_DEBLOCK 1u   /* gab200_h264_encode_deblocked's in-loop filter */
+#define GAB200_H264_INTRA4X4 2u  /* I_NxN (Intra_4x4) macroblocks beside I_16x16 */
+/* One entry for every option (gaussianavatars_b200.video VideoWriter(deblock=, intra4x4=)).  Without
+ * GAB200_H264_INTRA4X4 the samples are byte for byte gab200_h264_encode's (gop 1, no state, no other flag),
+ * gab200_h264_encode_stream's (a state) or gab200_h264_encode_deblocked's (GAB200_H264_DEBLOCK).  With it an intra
+ * macroblock may also be I_NxN (mb_type ue(0), ue(5) in a P slice), legal in Constrained Baseline, so the SPS and PPS
+ * are unchanged: each 4x4 block takes the Intra_4x4 mode (8.3.1.2, the nine of them) of least SATD + lambda * its mode
+ * bits (1 when it is predIntra4x4PredMode, else 4), its 16 coefficients quantised with the intra dead zone; block 5
+ * never takes modes 3 or 7, which read the macroblock above right, so the wavefronts and launch counts are the
+ * option's without I_NxN.  I_NxN replaces I_16x16 when its block costs sum below I_16x16's least luma SATD, and in a P
+ * picture the cheaper of the two meets the inter cost as I_16x16 did; I_PCM replaces it as it replaces I_16x16, so
+ * the bounds hold.  state may be NULL when gop is 1.  tests/h264_intra4x4_oracle.py restates the encode bit for bit.
+ * Refused before any device work: unknown flag bits, and what gab200_h264_encode_deblocked refuses. */
+size_t gab200_h264_flags_scratch_bytes(int32_t frames, int32_t height, int32_t width, int32_t gop, uint32_t flags);
+int32_t gab200_h264_encode_flags(int32_t frames, int32_t height, int32_t width, int32_t qp, int32_t gop, uint32_t flags,
+                                 const uint8_t* rgb, void* state, void* scratch, uint8_t* out, int64_t out_stride,
+                                 int64_t* out_len, void* stream);
+
 /* A device-resident view schedule (csrc/schedule.cu, gaussianavatars_b200.schedule.ViewSchedule): `records` records
  * of `views` cameras each -- cams [records, views, GAB200_CAMERA_FLOATS] float32, timesteps [records] int32 (may be
  * NULL), frame_ids [records, views] int32 (may be NULL) -- visited in the order order[0 .. length).  `cursor` is one
